@@ -37,14 +37,20 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
     std::unique_ptr<Distributed_Sparse> d_ops(hnh_make_algorithm(algorithm_name, spmat, R, c, &local_ops));
     std::unique_ptr<Distributed_ALS> d_als;
     std::unique_ptr<GAT> gnn;
-    if (app == "gat") {
+    DenseMatrix gat_output_grad;
+    if (app == "gat" || app == "gat_train") {
         // the three layers of the reference's GAT benchmark: (input width, width per head, heads)
         vector<GATLayer> layers{GATLayer(256, 256, 4), GATLayer(1024, 256, 4), GATLayer(1024, 256, 6)};
         gnn.reset(new GAT(layers, d_ops.get()));
+        // gat_train: forwardPass() then backwardPass(dL/d output = ones) per call
+        if (app == "gat_train") {
+            gnn->check_backward_supported();
+            gat_output_grad = DenseMatrix::Constant(gnn->buffers.back().rows(), gnn->buffers.back().cols(), 1.0);
+        }
     } else if (app == "als") {
         d_als.reset(new Distributed_ALS(d_ops.get(), true));
     } else if (app != "vanilla") {
-        throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\" or \"gat\"");
+        throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\", \"gat\" or \"gat_train\"");
     }
 
     DenseMatrix A = d_ops->like_A_matrix(0.001);
@@ -64,6 +70,9 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
             }
         } else if (app == "gat") {
             gnn->forwardPass();
+        } else if (app == "gat_train") {
+            gnn->forwardPass();
+            gnn->backwardPass(gat_output_grad);
         } else {
             d_als->application_communication_time = 0.0;
             d_als->run_cg(1);

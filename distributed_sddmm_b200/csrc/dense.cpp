@@ -244,6 +244,33 @@ void DenseMatrix::setMiddleColsRelu(int64_t start, const DenseMatrix &m) {
     require(m.rows() == rows_ && start >= 0 && start + m.cols() <= cols_, "middleCols assignment: shape mismatch");
     abi_check(hnh_relu_cols_f64(data(), cols_, start, m.data(), m.rows(), m.cols(), cs()), "relu_cols");
 }
+void VectorXd::leakyReluGrad(double alpha) {
+    abi_check(hnh_leaky_relu_grad_f64(data(), data(), n_, alpha, cs()), "leaky_relu_grad");
+}
+void DenseMatrix::setTransposeTimes(const DenseMatrix &a, const DenseMatrix &b) {
+    require(a.rows() == b.rows(), "transposed product: row counts differ");
+    require(buf_.owns() || (rows_ == a.cols() && cols_ == b.cols()), "transposed product: shape mismatch on a view");
+    resize(a.cols(), b.cols());
+    const int64_t ws = hnh_dgemm_tn_workspace_bytes(a.cols(), b.cols(), a.rows());
+    if (ws < 0) abi_check((int)ws, "dgemm_tn");
+    hnh::DeviceBuffer<char> workspace((size_t)ws);  // from the caching allocator, released stream-ordered
+    abi_check(hnh_dgemm_tn_f64(data(), a.data(), b.data(), a.cols(), b.cols(), a.rows(), workspace.data(), (size_t)ws, cs()),
+              "dgemm_tn");
+}
+void DenseMatrix::setTimesTranspose(const DenseMatrix &a, const DenseMatrix &b, bool accumulate) {
+    require(a.cols() == b.cols(), "product with a transpose: inner dimensions differ");
+    if (accumulate || !buf_.owns())
+        require(rows_ == a.rows() && cols_ == b.rows(), "product with a transpose: shape mismatch");
+    resize(a.rows(), b.rows());
+    abi_check(hnh_dgemm_nt_f64(data(), a.data(), b.data(), a.rows(), b.rows(), a.cols(), accumulate ? 1 : 0, cs()), "dgemm_nt");
+}
+void DenseMatrix::setMiddleColsReluGrad(const DenseMatrix &grad, const DenseMatrix &out, int64_t start) {
+    require(grad.rows() == out.rows() && grad.cols() == out.cols() && rows_ == out.rows() && start >= 0 &&
+                start + cols_ <= out.cols(),
+            "middleCols ReLU gradient: shape mismatch");
+    abi_check(hnh_relu_cols_backward_f64(data(), grad.data(), out.data(), out.cols(), start, rows_, cols_, cs()),
+              "relu_cols_backward");
+}
 
 VectorXd batch_dot_product(const DenseMatrix &A, const DenseMatrix &B) {
     require(A.rows() == B.rows() && A.cols() == B.cols(), "batch_dot_product: shape mismatch");

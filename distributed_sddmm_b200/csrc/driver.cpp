@@ -435,6 +435,7 @@ int hnhd_gat_set_weight(hnhd_gat_t *g, int layer, int head, const double *host) 
     return guarded([&] {
         if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
         gat_weight(g, layer, head).copy_from_host(host);
+        g->g->activations_current = false;
     });
 }
 int hnhd_gat_buffer_shape(hnhd_gat_t *g, int buffer, int64_t *rows, int64_t *cols) {
@@ -448,6 +449,7 @@ int hnhd_gat_set_input(hnhd_gat_t *g, const double *host) {
     return guarded([&] {
         if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
         gat_buffer(g, 0).copy_from_host(host);
+        g->g->activations_current = false;
     });
 }
 int hnhd_gat_get_buffer(hnhd_gat_t *g, int buffer, double *host) {
@@ -460,6 +462,32 @@ int hnhd_gat_forward(hnhd_gat_t *g) {
     return guarded([&] {
         if (!g) throw hnh::Error(HNH_E_INVALID, "null gat");
         g->g->forwardPass();
+    });
+}
+int hnhd_gat_backward(hnhd_gat_t *g, const double *host_output_grad) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null gat");
+        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const DenseMatrix &out = g->g->buffers.back();
+        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
+        g->g->backwardPass(grad);
+    });
+}
+int hnhd_gat_get_weight_grad(hnhd_gat_t *g, int layer, int head, double *host) {
+    return guarded([&] {
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_weight(g, layer, head);  // validates layer and head
+        const GATLayer &l = g->g->layers[(size_t)layer];
+        if (l.wGrads.size() != l.wMats.size()) throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
+        l.wGrads[(size_t)head].copy_to_host(host);
+    });
+}
+int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null gat");
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
+        g->g->input_grad.copy_to_host(host);
     });
 }
 void hnhd_gat_destroy(hnhd_gat_t *g) { delete g; }

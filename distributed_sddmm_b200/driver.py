@@ -338,7 +338,7 @@ def benchmark_algorithm(S: SpmatLocal, name: str, R: int, c: int, fused=True, ap
 
 
 class GAT:
-    """Multi-head graph attention forward pass (include/hnh/gat.hpp).  layers: [(input_features,
+    """Multi-head graph attention: forward pass and weight / input gradients (include/hnh/gat.hpp).  layers: [(input_features,
     features_per_head, num_heads), ...].  The algorithm object must outlive this one."""
 
     def __init__(self, alg: Algorithm, layers, leaky_relu_alpha: float = 0.2):
@@ -375,6 +375,26 @@ class GAT:
 
     def forward(self):
         check(lib().hnhd_gat_forward(self.h), "gat_forward")
+
+    def backward(self, grad_out):
+        """Backward pass (collective): grad_out = dL/d(network output), this rank's rows.  Needs a forward pass
+        since the last set_weight / set_input; the gradients are then read with weight_grad / input_grad."""
+        g = np.ascontiguousarray(grad_out, dtype=np.float64)
+        last = len(self.layers)
+        assert g.shape == self.buffer_shape(last), (g.shape, self.buffer_shape(last))
+        check(lib().hnhd_gat_backward(self.h, g.ctypes.data), "gat_backward")
+
+    def weight_grad(self, layer: int, head: int):
+        """dL/d weight (layer, head), summed over all ranks."""
+        out = np.empty(self.weight_shape(layer, head), dtype=np.float64)
+        check(lib().hnhd_gat_get_weight_grad(self.h, layer, head, out.ctypes.data), "gat_get_weight_grad")
+        return out
+
+    def input_grad(self):
+        """dL/d(network input), this rank's rows."""
+        out = np.empty(self.buffer_shape(0), dtype=np.float64)
+        check(lib().hnhd_gat_get_input_grad(self.h, out.ctypes.data), "gat_get_input_grad")
+        return out
 
     def __del__(self):
         try:

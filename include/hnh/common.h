@@ -79,6 +79,8 @@ public:
     // this[i] = max(this[i], 0) + alpha * min(this[i], 0)
     // (`v = v.array().max(0) + v.array().min(0) * alpha` of gat.hpp:98)
     void leakyRelu(double alpha);
+    // this[i] = this[i] > 0 ? 1 : alpha: the derivative of leakyRelu at the values it was applied to
+    void leakyReluGrad(double alpha);
 
     // host interop (not in Eigen; the data lives in HBM)
     static VectorXd from_host(const double *h, int64_t n);
@@ -165,6 +167,14 @@ public:
     DenseMatrix operator*(const DenseMatrix &o) const;
     // this.middleCols(start, m.cols()) = m.array().max(0)   (gat.hpp:104)
     void setMiddleColsRelu(int64_t start, const DenseMatrix &m);
+    // the GAT backward products (GAT::backwardPass), on this library's DMMA GEMMs:
+    //   this = a^T * b                        (hnh_dgemm_tn_f64; a and b have the same row count)
+    //   this = a * b^T, or this += a * b^T    (hnh_dgemm_nt_f64; a and b have the same column count)
+    void setTransposeTimes(const DenseMatrix &a, const DenseMatrix &b);
+    void setTimesTranspose(const DenseMatrix &a, const DenseMatrix &b, bool accumulate);
+    // this = grad.middleCols(start, w) where out.middleCols(start, w) > 0, else 0; w = cols() (the ReLU gradient of
+    // setMiddleColsRelu: grad and out are the gradient and the value of the matrix the ReLU wrote into)
+    void setMiddleColsReluGrad(const DenseMatrix &grad, const DenseMatrix &out, int64_t start);
 
     // this = c + alpha * diag(s) * m  (row-scaled axpy; s empty == all ones). In place allowed.
     void setRowAxpy(const DenseMatrix &c, double alpha, const VectorXd *s, const DenseMatrix &m);

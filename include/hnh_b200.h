@@ -157,6 +157,26 @@ int hnh_relu_cols_f64(double *dst, int64_t ld_dst, int64_t col0, const double *s
 int hnh_dgemm_f64(double *C, const double *A, const double *B, int64_t m, int64_t n, int64_t k,
                   void *stream);
 
+/* ---- GAT backward pass helpers (include/hnh/gat.hpp, GAT::backwardPass) ----------------------
+ * dst[i] = src[i] > 0 ? 1 : alpha   (derivative of hnh_leaky_relu_f64; alpha at 0; dst may alias src) */
+int hnh_leaky_relu_grad_f64(double *dst, const double *src, int64_t n, double alpha, void *stream);
+/* dst[i, j] = out[i, col0 + j] > 0 ? grad[i, col0 + j] : 0 for a rows x cols contiguous dst; grad and out
+ * have ld columns (the gradient through hnh_relu_cols_f64; 0 at 0) */
+int hnh_relu_cols_backward_f64(double *dst, const double *grad, const double *out, int64_t ld, int64_t col0,
+                               int64_t rows, int64_t cols, void *stream);
+/* C (m x n) = A^T * B with A k x m and B k x n, all row-major and contiguous (the weight gradient X^T dP).
+ * fp64 tensor-core MMA; k is split over the CTAs and the partial tiles go to `workspace`, which must hold
+ * hnh_dgemm_tn_workspace_bytes(m, n, k) bytes (0: none needed); a second pass adds them in a fixed order, so
+ * repeated calls give bit-identical results.  m, n <= 2^20.  The workspace size depends on the shape only;
+ * it is negative (HNH_E_INVALID) for a bad shape. */
+int64_t hnh_dgemm_tn_workspace_bytes(int64_t m, int64_t n, int64_t k);
+int hnh_dgemm_tn_f64(double *C, const double *A, const double *B, int64_t m, int64_t n, int64_t k,
+                     void *workspace, size_t workspace_bytes, void *stream);
+/* C (m x n) = A * B^T (accumulate == 0) or C += A * B^T (accumulate != 0), with A m x k and B n x k, all
+ * row-major and contiguous (the input gradient dP W^T).  fp64 tensor-core MMA, the tiling of hnh_dgemm_f64. */
+int hnh_dgemm_nt_f64(double *C, const double *A, const double *B, int64_t m, int64_t n, int64_t k,
+                     int accumulate, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

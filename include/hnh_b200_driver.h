@@ -191,6 +191,15 @@ int hnhd_gat_buffer_shape(hnhd_gat_t *g, int buffer, int64_t *rows, int64_t *col
 int hnhd_gat_set_input(hnhd_gat_t *g, const double *host);          /* buffer 0 */
 int hnhd_gat_get_buffer(hnhd_gat_t *g, int buffer, double *host);   /* synchronises */
 int hnhd_gat_forward(hnhd_gat_t *g);                                /* forwardPass(); stream-ordered */
+/* GAT backward pass (GAT::backwardPass): host_output_grad = dL/d(last buffer), this rank's rows, in the
+ * shape hnhd_gat_buffer_shape reports for the last buffer.  Collective.  HNH_E_INVALID on every rank where the
+ * layout has no backward pass (R-split layouts at p > 1; 1.5D dense shift with local kernel fusion at c > 1),
+ * and when no forward pass has run since the last set_weight / set_input.  The gradients are then read with: */
+int hnhd_gat_backward(hnhd_gat_t *g, const double *host_output_grad);
+/* dL/d weight (layer, head), summed over all ranks (identical on every rank); hnhd_gat_weight_shape's shape */
+int hnhd_gat_get_weight_grad(hnhd_gat_t *g, int layer, int head, double *host);
+/* dL/d buffer 0 (this rank's rows); hnhd_gat_buffer_shape(0)'s shape */
+int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host);
 void hnhd_gat_destroy(hnhd_gat_t *g);
 
 #ifdef __cplusplus

@@ -1,8 +1,10 @@
 #!/usr/bin/env python
 """benchmark_algorithm (the reference's benchmark entry point, benchmark_dist.cpp:26-167) for the applications it
 knows -- vanilla FusedMM, one ALS-CG round (run_cg(1): 2 x 10 batched CG iterations around fusedSpMM), the GAT
-forward pass -- at the launched world size (torchrun).  One JSON record per (application, algorithm) on rank 0.
-Environment: LOGM, NPR, R, C, ALGS, APPS, TRIALS, WARMUP."""
+forward pass ("gat"), and one GAT training step ("gat_train": forward pass, then the backward pass for an all-ones
+output gradient; the weights stay as "gat" leaves them) -- at the launched world size (torchrun).  One JSON record
+per (application, algorithm) on rank 0.  Environment: LOGM, NPR, R, C, ALGS, APPS (e.g. APPS=gat,gat_train),
+TRIALS, WARMUP."""
 import json
 import os
 import sys
@@ -35,8 +37,12 @@ for app in apps:
         if rank == 0:
             keep = {k: rec.get(k) for k in ("elapsed", "overall_throughput", "num_trials", "warmup", "application_communication_time",
                                             "perf_stats", "error") if k in rec}
+            # device memory in use after the run (cudaMemGetInfo): the library's caching allocator keeps what it
+            # allocated, so this is close to the run's peak
+            free_b, total_b = torch.cuda.mem_get_info()
             keep.update(app=app, alg=alg, logM=logM, nnz_per_row=npr, R=R, c=c, p=world,
-                        ms_per_call=(rec["elapsed"] / rec["num_trials"] * 1e3) if "elapsed" in rec else None)
+                        ms_per_call=(rec["elapsed"] / rec["num_trials"] * 1e3) if "elapsed" in rec else None,
+                        device_used_gib=round((total_b - free_b) / 2**30, 1))
             print(json.dumps(keep), flush=True)
 del S
 D.world_finalize()
