@@ -47,6 +47,14 @@ ABI = {
     "hnh_dgemm_tn_workspace_bytes": (C.c_int64, [_I64, _I64, _I64]),
     "hnh_dgemm_tn_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _I64, _P, C.c_size_t, _P]),
     "hnh_dgemm_nt_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _I64, C.c_int, _P]),
+    "hnh_edge_keys_from_index": (C.c_int, [_P, _P, _I64, _I64, _P]),
+    "hnh_edge_softmax_piece_bound": (C.c_int64, [_I64, _I64]),
+    "hnh_edge_softmax_plan": (C.c_int, [_P, _I64, _I64, _P, _P, _P, _P, _I64, C.POINTER(C.c_int64), _P]),
+    "hnh_edge_softmax_stats_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I64, _P, _P, _P, _P, _P]),
+    "hnh_edge_softmax_rescale_f64": (C.c_int, [_P, _P, _P, _I64, _P]),
+    "hnh_edge_softmax_apply_f64": (C.c_int, [_P, _P, _P, _I64, _P, _P, _P]),
+    "hnh_edge_softmax_dot_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _P, _P, _P]),
+    "hnh_edge_softmax_backward_f64": (C.c_int, [_P, _P, _P, _P, _I64, _P, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -190,6 +198,9 @@ ABI.update({
     "hnhd_gat_backward": (C.c_int, [_P, _P]),
     "hnhd_gat_get_weight_grad": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "hnhd_gat_get_input_grad": (C.c_int, [_P, _P]),
+    "hnhd_gat_set_attention": (C.c_int, [_P, C.c_char_p]),
+    "hnhd_alg_edge_softmax": (C.c_int, [_P, _P, C.c_int]),
+    "hnhd_alg_edge_softmax_backward": (C.c_int, [_P, _P, _P, C.c_int]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),

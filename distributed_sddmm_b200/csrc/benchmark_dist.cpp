@@ -38,19 +38,27 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
     std::unique_ptr<Distributed_ALS> d_als;
     std::unique_ptr<GAT> gnn;
     DenseMatrix gat_output_grad;
-    if (app == "gat" || app == "gat_train") {
+    const bool gat_app = app == "gat" || app == "gat_train" || app == "gat_softmax" || app == "gat_softmax_train";
+    const bool gat_train = app == "gat_train" || app == "gat_softmax_train";
+    if (gat_app) {
         // the three layers of the reference's GAT benchmark: (input width, width per head, heads)
         vector<GATLayer> layers{GATLayer(256, 256, 4), GATLayer(1024, 256, 4), GATLayer(1024, 256, 6)};
         gnn.reset(new GAT(layers, d_ops.get()));
-        // gat_train: forwardPass() then backwardPass(dL/d output = ones) per call
-        if (app == "gat_train") {
+        // gat_softmax*: softmax attention (the edge softmax of the scores) instead of the reference's
+        if (app == "gat_softmax" || app == "gat_softmax_train") {
+            d_ops->check_full_rows("GAT softmax attention");
+            gnn->set_attention("softmax");
+        }
+        // gat_train / gat_softmax_train: forwardPass() then backwardPass(dL/d output = ones) per call
+        if (gat_train) {
             gnn->check_backward_supported();
             gat_output_grad = DenseMatrix::Constant(gnn->buffers.back().rows(), gnn->buffers.back().cols(), 1.0);
         }
     } else if (app == "als") {
         d_als.reset(new Distributed_ALS(d_ops.get(), true));
     } else if (app != "vanilla") {
-        throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\", \"gat\" or \"gat_train\"");
+        throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\", \"gat\", \"gat_train\", \"gat_softmax\" or "
+                                        "\"gat_softmax_train\"");
     }
 
     DenseMatrix A = d_ops->like_A_matrix(0.001);
@@ -68,11 +76,9 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
                 d_ops->sddmmA(A, B, Sv, sddmm_result);
                 d_ops->spmmA(A, B, Sv);
             }
-        } else if (app == "gat") {
+        } else if (gat_app) {
             gnn->forwardPass();
-        } else if (app == "gat_train") {
-            gnn->forwardPass();
-            gnn->backwardPass(gat_output_grad);
+            if (gat_train) gnn->backwardPass(gat_output_grad);
         } else {
             d_als->application_communication_time = 0.0;
             d_als->run_cg(1);

@@ -22,6 +22,7 @@ public:
     virtual void allgather(int rank, int size, const void *send, void *recv, size_t bytes_each, cudaStream_t s) = 0;
     virtual void reduce_scatter(int rank, int size, const double *send, double *recv, size_t count_each, cudaStream_t s) = 0;
     virtual void allreduce(double *buf, size_t count, cudaStream_t s) = 0;
+    virtual void allreduce_max(int size, double *buf, size_t count, cudaStream_t s) = 0;
     // default: through host memory with the transport's host all-to-all
     virtual void alltoallv(int rank, int size, const void *send, const size_t *sb, const size_t *sd, void *recv, const size_t *rb,
                            const size_t *rd, cudaStream_t s) {
@@ -70,6 +71,7 @@ public:
         copy_d2d(recv, send, c * sizeof(double), s);
     }
     void allreduce(double *, size_t, cudaStream_t) override {}
+    void allreduce_max(int, double *, size_t, cudaStream_t) override {}
     void alltoallv(int, int, const void *send, const size_t *sb, const size_t *sd, void *recv, const size_t *rb, const size_t *rd,
                    cudaStream_t s) override {
         if (sb[0] != rb[0]) throw Error(HNH_E_COMM, "self alltoallv: size mismatch");
@@ -131,6 +133,9 @@ public:
     }
     void allreduce(double *buf, size_t count, cudaStream_t s) override {
         nccl_check(ncclAllReduce(buf, buf, count, ncclDouble, ncclSum, comm_, s), "ncclAllReduce");
+    }
+    void allreduce_max(int, double *buf, size_t count, cudaStream_t s) override {
+        nccl_check(ncclAllReduce(buf, buf, count, ncclDouble, ncclMax, comm_, s), "ncclAllReduce");
     }
 
     void alltoallv(int rank, int size, const void *send, const size_t *sb, const size_t *sd, void *recv, const size_t *rb,
@@ -255,6 +260,22 @@ public:
         call(cb_.allreduce_f64(cb_.ctx, id_, (double *)hs, count), "allreduce");
         h2d(buf, hs, count * sizeof(double), s);
     }
+    // the callback table has no max reduction: every rank gathers all contributions and takes the maximum of
+    // each element in rank order (the same result everywhere)
+    void allreduce_max(int size, double *buf, size_t count, cudaStream_t s) override {
+        const size_t b = count * sizeof(double);
+        char *hs = pinned_a(b), *hr = pinned_b(b * size);
+        d2h(hs, buf, b, s);
+        call(cb_.allgather(cb_.ctx, id_, hs, hr, b), "allgather");
+        double *out = (double *)hs;
+        const double *all = (const double *)hr;
+        for (size_t i = 0; i < count; i++) {
+            double m = all[i];
+            for (int q = 1; q < size; q++) m = std::max(m, all[(size_t)q * count + i]);
+            out[i] = m;
+        }
+        h2d(buf, hs, b, s);
+    }
     void host_sendrecv(int, const void *send, size_t sb, int dst, void *recv, size_t rb, int src) override {
         call(cb_.sendrecv(cb_.ctx, id_, send, sb, dst, recv, rb, src), "sendrecv");
     }
@@ -345,6 +366,10 @@ void Comm::alltoallv(const void *send, const size_t *sb, const size_t *sd, void 
 void Comm::allreduce_sum_f64(double *buf, size_t count, cudaStream_t s) {
     if (size_ > 1) bytes_sent_ += 2 * count * sizeof(double) * (size_ - 1) / size_;
     t_->allreduce(buf, count, s);
+}
+void Comm::allreduce_max_f64(double *buf, size_t count, cudaStream_t s) {
+    if (size_ > 1) bytes_sent_ += 2 * count * sizeof(double) * (size_ - 1) / size_;
+    t_->allreduce_max(size_, buf, count, s);
 }
 void Comm::host_sendrecv(const void *send, size_t sb, int dst, void *recv, size_t rb, int src) {
     t_->host_sendrecv(rank_, send, sb, dst, recv, rb, src);

@@ -2,8 +2,12 @@
 #include "hnh/distributed_sparse.h"
 
 #include <algorithm>
+#include <array>
 #include <iostream>
+#include <mutex>
 
+#include "hnh/15D_dense_shift.hpp"
+#include "hnh/25D_cannon_dense.hpp"
 #include "hnh_b200.h"
 
 using hnh::Runtime;
@@ -199,6 +203,158 @@ void Distributed_Sparse::hadamard_values(VectorXd &result, VectorXd &SValues, Sp
         else
             hnh::cuda_check(cudaMemsetAsync(result.data() + off, 0, sizeof(double) * (size_t)n, compute()), "memset");
     }
+}
+
+// ---- edge softmax ------------------------------------------------------------------------------------------
+void Distributed_Sparse::check_full_rows(const string &operation) const {
+    if (p == 1) return;
+    const string where = algorithm_name + " at p = " + std::to_string(p) + ", c = " + std::to_string(c);
+    if (r_split) throw hnh::Error(HNH_E_INVALID, operation + ": not defined for " + where + ": the layout splits the dense operands along R");
+    const Sparse15D_Dense_Shift *dense_shift = dynamic_cast<const Sparse15D_Dense_Shift *>(this);
+    if (dense_shift == nullptr) throw hnh::Error(HNH_E_INVALID, operation + ": not defined for " + where);
+    if (dense_shift->fusionApproach == 2 && c > 1)
+        throw hnh::Error(HNH_E_INVALID, operation + ": not defined for " + where +
+                                            " with local kernel fusion (fusion 2): the forward SpMM accumulates onto the "
+                                            "gathered projection when c > 1");
+}
+
+namespace {
+
+// The row grouping of one value order (edgeSoftmax), built on first use.  Kept in a table keyed by the algorithm
+// object rather than in the object, so that the layout of Distributed_Sparse and of its subclasses is unchanged.
+struct EdgeRows {
+    hnh::DeviceBuffer<int32_t> keys, perm, row_start, piece_first, piece_row;
+    int64_t n = 0, pieces = 0;
+};
+std::mutex edge_rows_mutex;
+using EdgeRowsTable = std::map<const Distributed_Sparse *, std::array<std::unique_ptr<EdgeRows>, 2>>;
+// never destroyed: an object still alive at exit must not free device memory after the runtime has gone
+EdgeRowsTable &edge_rows_table() {
+    static EdgeRowsTable *t = new EdgeRowsTable;
+    return *t;
+}
+
+// The SpmatLocal whose CSR blocks, concatenated in blockStarts order, hold the entries of a value vector of `order`
+// (the one algorithm() works on for that mode), and the global S-row of local index 0 in block b of it: S keeps
+// the S-rows as its local rows, ST as its local columns.  Exact wherever check_full_rows passes.
+SpmatLocal *values_matrix(const Distributed_Sparse &d, KernelMode order) {
+    bool in_ST = order == k_sddmmB;
+    if (const Sparse15D_Dense_Shift *ds = dynamic_cast<const Sparse15D_Dense_Shift *>(&d))
+        in_ST = (ds->fusionApproach == 1) == (order == k_sddmmA);  // fusion 1 keeps A-order values in ST's blocks
+    else if (dynamic_cast<const Sparse25D_Cannon_Dense *>(&d))
+        in_ST = order == k_sddmmA;  // blocks stored transposed: A-order values in ST's block
+    return in_ST ? d.ST.get() : d.S.get();
+}
+int64_t values_row_offset(const Distributed_Sparse &d, const SpmatLocal &m, int block) {
+    // p = 1: one block starting at row 0.  1.5D dense shift: S holds block row grid->i (height localArows * c), block b
+    // of ST holds S-rows [b * localArows, (b + 1) * localArows)
+    if (d.p == 1) return 0;
+    return &m == d.ST.get() ? (int64_t)block * d.localArows : (int64_t)d.grid->i * d.localArows * d.c;
+}
+
+EdgeRows &edge_rows(Distributed_Sparse &d, KernelMode order, int64_t n) {
+    if (order != k_sddmmA && order != k_sddmmB)
+        throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: the value order must be k_sddmmA or k_sddmmB");
+    const int64_t want = order == k_sddmmA ? d.num_S_values() : d.num_ST_values();
+    if (n != want)
+        throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: the value vector has " + to_string(n) + " entries, this order " + to_string(want));
+    std::unique_ptr<EdgeRows> *slot;
+    {
+        std::lock_guard<std::mutex> lock(edge_rows_mutex);
+        slot = &edge_rows_table()[&d][order == k_sddmmA ? 0 : 1];
+    }
+    if (*slot) return **slot;
+    const int64_t M = d.M;
+    if (M >= INT32_MAX) throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: S has " + to_string(M) + " rows; at most 2^31 - 2");
+    SpmatLocal &m = *values_matrix(d, order);
+    const bool is_ST = &m == d.ST.get();
+    if ((int64_t)m.blockStarts.back() != n)
+        throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: the value vector does not cover the local blocks");
+    cudaStream_t s = Runtime::get().compute_stream();
+    std::unique_ptr<EdgeRows> e(new EdgeRows);
+    e->n = n;
+    e->keys.resize((size_t)n);
+    e->perm.resize((size_t)n);
+    e->row_start.resize((size_t)M + 1);
+    e->piece_first.resize((size_t)M + 1);
+    const int64_t bound = hnh_edge_softmax_piece_bound(n, M);
+    if (bound < 0) hnh::abi_check((int)bound, "edge_softmax_piece_bound");
+    e->piece_row.resize((size_t)std::max<int64_t>(bound, 1));
+    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
+        const int64_t off = (int64_t)m.blockStarts[b], nb = (int64_t)m.blockStarts[b + 1] - off;
+        if (nb == 0) continue;
+        CSRLocal *blk = m.csr_blocks[b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: block " + to_string(b) + " does not match its value range");
+        // S stores its rows as rows, ST as columns; a transposed block swaps the two
+        const bool stored_row = is_ST == blk->transpose;
+        const int64_t *idx = stored_row ? blk->row_idx_device() : blk->getActive()->col_idx.data();
+        hnh::abi_check(hnh_edge_keys_from_index(e->keys.data() + off, idx, nb, values_row_offset(d, m, (int)b), s),
+                       "edge_keys_from_index");
+    }
+    int64_t pieces = 0;
+    hnh::abi_check(hnh_edge_softmax_plan(e->keys.data(), n, M, e->perm.data(), e->row_start.data(), e->piece_first.data(),
+                                         e->piece_row.data(), (int64_t)e->piece_row.size(), &pieces, s),
+                   "edge_softmax_plan");
+    e->pieces = pieces;
+    *slot = std::move(e);
+    return **slot;
+}
+
+}  // namespace
+
+void Distributed_Sparse::release_edge_softmax() {
+    std::lock_guard<std::mutex> lock(edge_rows_mutex);
+    edge_rows_table().erase(this);
+}
+
+namespace {
+// dst op= over the world (sum or max), ordered on the compute stream
+void allreduce_rows(double *d, int64_t n, bool max) {
+    std::shared_ptr<hnh::Comm> world = hnh::Comm::world();
+    if (world->size() == 1) return;
+    Runtime &rt = Runtime::get();
+    rt.chain(rt.compute_stream(), rt.comm_stream());
+    if (max) world->allreduce_max_f64(d, (size_t)n, rt.comm_stream());
+    else world->allreduce_sum_f64(d, (size_t)n, rt.comm_stream());
+    rt.chain(rt.comm_stream(), rt.compute_stream());
+}
+}  // namespace
+
+void Distributed_Sparse::edgeSoftmax(VectorXd &values, KernelMode order) {
+    check_full_rows("edgeSoftmax");
+    EdgeRows &e = edge_rows(*this, order, values.size());
+    VectorXd piece_max(e.pieces), piece_sum(e.pieces), row_max(M), row_sum(M);
+    hnh::abi_check(hnh_edge_softmax_stats_f64(values.data(), e.perm.data(), e.row_start.data(), e.piece_first.data(),
+                                              e.piece_row.data(), M, e.pieces, piece_max.data(), piece_sum.data(),
+                                              row_max.data(), row_sum.data(), compute()),
+                   "edge_softmax_stats");
+    if (p > 1) {
+        VectorXd local_max = row_max;
+        allreduce_rows(row_max.data(), M, true);
+        hnh::abi_check(hnh_edge_softmax_rescale_f64(row_sum.data(), local_max.data(), row_max.data(), M, compute()),
+                       "edge_softmax_rescale");
+        allreduce_rows(row_sum.data(), M, false);
+    }
+    hnh::abi_check(hnh_edge_softmax_apply_f64(values.data(), values.data(), e.keys.data(), e.n, row_max.data(), row_sum.data(),
+                                              compute()),
+                   "edge_softmax_apply");
+}
+
+void Distributed_Sparse::edgeSoftmaxBackward(const VectorXd &alpha, VectorXd &grad, KernelMode order) {
+    check_full_rows("edgeSoftmaxBackward");
+    if (alpha.size() != grad.size())
+        throw hnh::Error(HNH_E_INVALID, "edgeSoftmaxBackward: alpha has " + to_string(alpha.size()) + " entries, grad " +
+                                            to_string(grad.size()));
+    EdgeRows &e = edge_rows(*this, order, grad.size());
+    VectorXd piece_dot(e.pieces), row_dot(M);
+    hnh::abi_check(hnh_edge_softmax_dot_f64(alpha.data(), grad.data(), e.perm.data(), e.row_start.data(), e.piece_first.data(),
+                                            e.piece_row.data(), M, e.pieces, piece_dot.data(), row_dot.data(), compute()),
+                   "edge_softmax_dot");
+    allreduce_rows(row_dot.data(), M, false);
+    hnh::abi_check(hnh_edge_softmax_backward_f64(grad.data(), alpha.data(), grad.data(), e.keys.data(), e.n, row_dot.data(),
+                                                 compute()),
+                   "edge_softmax_backward");
 }
 
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {

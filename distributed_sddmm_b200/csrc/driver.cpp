@@ -318,6 +318,23 @@ int hnhd_alg_fused_host(hnhd_alg_t *a, hnhd_dense_t *A, hnhd_dense_t *B, hnhd_ve
     });
 }
 
+static KernelMode value_order(int mode) {
+    if (mode != 0 && mode != 1) throw hnh::Error(HNH_E_INVALID, "edge softmax: mode must be 0 (A order) or 1 (B order)");
+    return mode == 0 ? k_sddmmA : k_sddmmB;
+}
+int hnhd_alg_edge_softmax(hnhd_alg_t *a, hnhd_vec_t *vec, int mode) {
+    return guarded([&] {
+        if (!a || !vec) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_edge_softmax: null argument");
+        a->alg->edgeSoftmax(vec->v, value_order(mode));
+    });
+}
+int hnhd_alg_edge_softmax_backward(hnhd_alg_t *a, const hnhd_vec_t *alpha, hnhd_vec_t *grad, int mode) {
+    return guarded([&] {
+        if (!a || !alpha || !grad) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_edge_softmax_backward: null argument");
+        a->alg->edgeSoftmaxBackward(alpha->v, grad->v, value_order(mode));
+    });
+}
+
 int hnhd_timer_start(void) {
     return guarded([] {
         if (!g_t0) {
@@ -488,6 +505,12 @@ int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host) {
         if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
         if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
         g->g->input_grad.copy_to_host(host);
+    });
+}
+int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind) {
+    return guarded([&] {
+        if (!g || !kind) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_set_attention: null argument");
+        g->g->set_attention(kind);
     });
 }
 void hnhd_gat_destroy(hnhd_gat_t *g) { delete g; }

@@ -181,6 +181,12 @@ class Vec:
             pass
 
 
+def _value_order(mode: str) -> int:
+    if mode not in ("A", "B"):
+        raise ValueError(f'mode must be "A" or "B", not {mode!r}')
+    return 0 if mode == "A" else 1
+
+
 class Algorithm:
     """A Distributed_Sparse subclass instance with the library's StandardKernel plugged in."""
 
@@ -248,6 +254,16 @@ class Algorithm:
         ptr = lambda t: t.data_ptr() if hasattr(t, "data_ptr") else t.ctypes.data  # noqa: E731
         check(lib().hnhd_alg_fused_host(self.h, A.h, B.h, S.h, R.h, ptr(hostA), ptr(hostB), ptr(hostOut),
                                         0 if mode == "A" else 1, chunk_rows), "hnhd_alg_fused_host")
+
+    def edge_softmax(self, values: Vec, mode: str = "A"):
+        """In place, collective: values (like_S_values for mode "A", like_ST_values for "B") become their softmax
+        over the stored entries of each row of S, on all ranks (Distributed_Sparse::edgeSoftmax)."""
+        check(lib().hnhd_alg_edge_softmax(self.h, values.h, _value_order(mode)), "edge_softmax")
+
+    def edge_softmax_backward(self, alpha: Vec, grad: Vec, mode: str = "A"):
+        """In place on grad, collective: grad = dL/d alpha becomes dL/d(scores) = alpha * (grad - t), with t the
+        row sums of alpha * grad (Distributed_Sparse::edgeSoftmaxBackward)."""
+        check(lib().hnhd_alg_edge_softmax_backward(self.h, alpha.h, grad.h, _value_order(mode)), "edge_softmax_backward")
 
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
@@ -339,14 +355,23 @@ def benchmark_algorithm(S: SpmatLocal, name: str, R: int, c: int, fused=True, ap
 
 class GAT:
     """Multi-head graph attention: forward pass and weight / input gradients (include/hnh/gat.hpp).  layers: [(input_features,
-    features_per_head, num_heads), ...].  The algorithm object must outlive this one."""
+    features_per_head, num_heads), ...].  attention: "leaky" (LeakyReLU of the scores, the reference's formula) or
+    "softmax" (their softmax over each node's neighbours).  The algorithm object must outlive this one."""
 
-    def __init__(self, alg: Algorithm, layers, leaky_relu_alpha: float = 0.2):
+    def __init__(self, alg: Algorithm, layers, leaky_relu_alpha: float = 0.2, attention: str = "leaky"):
+        if attention not in ("leaky", "softmax"):
+            raise ValueError(f'attention must be "leaky" or "softmax", not {attention!r}')
         self.alg = alg
         self.layers = [tuple(int(x) for x in l) for l in layers]
         flat = (C.c_int * (3 * len(self.layers)))(*[x for l in self.layers for x in l])
         self.h = C.c_void_p()
         check(lib().hnhd_gat_create(alg.h, len(self.layers), flat, float(leaky_relu_alpha), C.byref(self.h)), "gat_create")
+        self.set_attention(attention)
+
+    def set_attention(self, kind: str):
+        """"leaky" or "softmax"; the next backward pass needs a forward pass first."""
+        check(lib().hnhd_gat_set_attention(self.h, kind.encode()), "gat_set_attention")
+        self.attention = kind
 
     def weight_shape(self, layer: int, head: int):
         r, c = C.c_int64(), C.c_int64()

@@ -50,6 +50,7 @@ public:
     // send holds size()*count_each doubles; rank i receives the sum of everyone's i-th chunk
     void reduce_scatter_sum_f64(const double *send, double *recv, size_t count_each, cudaStream_t s);
     void allreduce_sum_f64(double *buf, size_t count, cudaStream_t s);
+    void allreduce_max_f64(double *buf, size_t count, cudaStream_t s);  // element-wise maximum over the ranks
     // MPI_Alltoallv on device buffers (byte counts / displacements per rank)
     void alltoallv(const void *send, const size_t *send_bytes, const size_t *send_displs, void *recv,
                    const size_t *recv_bytes, const size_t *recv_displs, cudaStream_t s);

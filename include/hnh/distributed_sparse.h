@@ -67,7 +67,7 @@ public:
     bool overlap;
 
     explicit Distributed_Sparse(KernelImplementation *k);
-    virtual ~Distributed_Sparse() {}
+    virtual ~Distributed_Sparse() { release_edge_softmax(); }
 
     virtual void setRValue(int R) = 0;
     void check_initialized();
@@ -142,6 +142,32 @@ public:
     // world-summed squared norms of a local matrix / vector ("fingerprints", scratch.cpp:26-76)
     double fingerprint(const DenseMatrix &m);
     double fingerprint(const VectorXd &v);
+
+    // ---- edge softmax: a softmax over the stored entries of each row of S ----------------------------------
+    // edgeSoftmax: values (a value vector of `order`: k_sddmmA for like_S_values, k_sddmmB for like_ST_values)
+    // becomes alpha_uv = exp(x_uv - m_u) / s_u, with m_u the maximum and s_u the sum of exp(x_uv - m_u) over the
+    // stored entries of row u of S on all ranks -- the normalisation of graph attention between an SDDMM and an
+    // SpMM.  edgeSoftmaxBackward: grad (dL/d alpha, the same order) becomes dL/dx = alpha o (grad - t), with
+    // t_u = sum over row u of alpha o grad.  Collective, in place, stream-ordered.  Each call builds its row
+    // statistics from the vector it is given, which holds every stored entry of S exactly once over all ranks;
+    // row statistics are M-long vectors reduced over the world (forward: one max and one sum all-reduce,
+    // backward: one sum all-reduce; none at p = 1).  The A and B orders sum in different orders, so a softmax
+    // of the same scores in the two orders may differ in the last bits.  The first call per order builds the
+    // entries' row keys and a stable grouping by row on the device and keeps them until this object is destroyed
+    // (in a table beside the object: the class layout and its virtual table stay those of earlier releases, so
+    // programs compiled against earlier headers keep working with this library).
+    // Defined where every rank holds full-width rows (check_full_rows); HNH_E_INVALID on every rank elsewhere.
+    void edgeSoftmax(VectorXd &values, KernelMode order);
+    void edgeSoftmaxBackward(const VectorXd &alpha, VectorXd &grad, KernelMode order);
+
+    // Throws HNH_E_INVALID ("<operation>: not defined for <algorithm> at p = .., c = ..") unless every rank holds
+    // full-width rows of the dense operands and the A and B layouts coincide: p = 1 (any algorithm), and 1.5D
+    // dense shift with replication reuse (fusion 1) at any c or with local kernel fusion (fusion 2) at c = 1.
+    // GAT's backward pass and softmax attention and edgeSoftmax need this.  Decided from global quantities
+    // only, so every rank throws together and no collective is left waiting.
+    void check_full_rows(const string &operation) const;
+    // frees what edgeSoftmax keeps for this object (the destructor calls it)
+    void release_edge_softmax();
 
 protected:
     hnh::EventTimers timers_;

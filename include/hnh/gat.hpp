@@ -24,9 +24,20 @@
 // orders, so the B-mode vectors come from B-mode SDDMMs of the same operands, never from a permutation.  Per head:
 // 4 SDDMM passes (e and de in both orders), 3 SpMM passes and 3 GEMMs (P, dW, dX).
 //
+// Softmax attention (set_attention("softmax"); the default "leaky" is the reference's formula above) normalises
+// the scores over each node's neighbours: alpha_u. = softmax over the stored entries of row u of LeakyReLU(e_u.)
+// (Distributed_Sparse::edgeSoftmax, on the A-order scores), and Z = S_alpha H.  Its backward, with
+// a = LeakyReLU(e):
+//     dalpha = S o (dZ P^T)                              SDDMM with SValues = 1, both orders
+//     de     = LeakyReLU'(e) o alpha o (dalpha - t)      t_u = sum_v alpha_uv dalpha_uv (edgeSoftmaxBackward)
+//     dP     = S_de P + S_alpha^T dZ + S_de^T P          the leaky formula with a_B replaced by alpha_B
+// alpha is recomputed in both orders.  Per head this adds one O(nnz) softmax to the forward pass, and four O(nnz)
+// softmax calls (and, at p > 1, six M-long all-reduces) to the backward pass; the sparse pass count is unchanged.
+//
 // The forward pass is the GAT formula only where every rank holds full-width rows and the A and B layouts coincide:
 // p = 1 (any algorithm), 1.5D dense shift with replication reuse (fusion 1) at any c, and with local kernel fusion
-// (fusion 2) at c = 1.  Only there is the backward defined; elsewhere backwardPass throws HNH_E_INVALID on every rank.
+// (fusion 2) at c = 1 (Distributed_Sparse::check_full_rows).  Only there are the backward pass and softmax attention
+// defined; elsewhere they throw HNH_E_INVALID on every rank.
 #pragma once
 #include <string>
 #include <vector>
@@ -94,6 +105,7 @@ public:
         VectorXd scores = d_ops->like_S_values(1.0);
         d_ops->algorithm(projected, neighbours, pattern, &scores, k_sddmmA, true);
         scores.leakyRelu(leaky_relu_alpha);
+        if (softmax_) d_ops->edgeSoftmax(scores, k_sddmmA);
 
         projected.setZero();  // becomes the SpMM accumulator
         d_ops->algorithm(projected, neighbours, scores, nullptr, k_spmmA, false);
@@ -101,6 +113,7 @@ public:
     }
 
     void forwardPass() {
+        if (softmax_) d_ops->check_full_rows("GAT softmax attention");
         for (size_t i = 0; i < layers.size(); i++)
             for (int j = 0; j < layers[i].num_heads; j++) computeSelfAttentionHead((int)i, j);
         activations_current = true;
@@ -114,20 +127,17 @@ public:
 
     // Throws HNH_E_INVALID unless the backward pass is defined on this algorithm object (see the top of this
     // file).  Decided from global quantities only, so every rank throws together and no collective is left waiting.
-    void check_backward_supported() const {
-        const string where = d_ops->algorithm_name + " at p = " + std::to_string(d_ops->p) + ", c = " +
-                             std::to_string(d_ops->c);
-        if (d_ops->p == 1) return;
-        if (d_ops->r_split)
-            throw hnh::Error(HNH_E_INVALID, "GAT::backwardPass: not defined for " + where +
-                                                ": the layout splits the dense operands along R");
-        const Sparse15D_Dense_Shift *dense_shift = dynamic_cast<const Sparse15D_Dense_Shift *>(d_ops);
-        if (dense_shift == nullptr)
-            throw hnh::Error(HNH_E_INVALID, "GAT::backwardPass: not defined for " + where);
-        if (dense_shift->fusionApproach == 2 && d_ops->c > 1)
-            throw hnh::Error(HNH_E_INVALID, "GAT::backwardPass: not defined for " + where +
-                                                " with local kernel fusion (fusion 2): the forward SpMM accumulates "
-                                                "onto the gathered projection when c > 1");
+    void check_backward_supported() const { d_ops->check_full_rows("GAT::backwardPass"); }
+
+    // "leaky" (the reference's attention, the default) or "softmax" (see the top of this file).  Changing it makes
+    // the activations stale.
+    const string &attention() const { return attention_; }
+    void set_attention(const string &kind) {
+        if (kind != "leaky" && kind != "softmax")
+            throw hnh::Error(HNH_E_INVALID, "GAT: attention must be \"leaky\" or \"softmax\", not \"" + kind + "\"");
+        if (kind != attention_) activations_current = false;
+        attention_ = kind;
+        softmax_ = kind == "softmax";
     }
 
     // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d wMats in layers[i].wGrads (summed over all
@@ -170,23 +180,40 @@ public:
         // so P serves as both of them.
         DenseMatrix P = input * W;
 
-        // attention scores in both value orders; g = LeakyReLU'(e) (A order, B order), a = LeakyReLU(e) (B order)
+        // attention scores in both value orders; g = LeakyReLU'(e) (A order, B order), a = LeakyReLU(e) (B order; with
+        // softmax attention alpha = edge softmax of LeakyReLU(e), both orders)
         VectorXd ones_A = d_ops->like_S_values(1.0), ones_B = d_ops->like_ST_values(1.0);
         VectorXd g_A = d_ops->like_S_values(0.0), g_B = d_ops->like_ST_values(0.0);
         d_ops->sddmmA(P, P, ones_A, g_A);
         d_ops->sddmmB(P, P, ones_B, g_B);
-        VectorXd a_B = g_B;
+        VectorXd a_A, a_B = g_B;
         a_B.leakyRelu(leaky_relu_alpha);
+        if (softmax_) {
+            a_A = g_A;
+            a_A.leakyRelu(leaky_relu_alpha);
+            d_ops->edgeSoftmax(a_A, k_sddmmA);
+            d_ops->edgeSoftmax(a_B, k_sddmmB);
+        }
         g_A.leakyReluGrad(leaky_relu_alpha);
         g_B.leakyReluGrad(leaky_relu_alpha);
 
         // dZ, then de = g o S o (dZ P^T) in both orders: the SDDMM multiplies its dots by SValues = g.  (Not
-        // fusedSpMM: the fusion-2 one ignores SValues.)
+        // fusedSpMM: the fusion-2 one ignores SValues.)  Softmax attention: dalpha = S o (dZ P^T) in both orders,
+        // then de = g o edgeSoftmaxBackward(alpha, dalpha).
         DenseMatrix dZ(P.rows(), P.cols());
         dZ.setMiddleColsReluGrad(G, output, (int64_t)j * layer.features_per_head);
         VectorXd de_A = d_ops->like_S_values(0.0), de_B = d_ops->like_ST_values(0.0);
-        d_ops->sddmmA(dZ, P, g_A, de_A);
-        d_ops->sddmmB(dZ, P, g_B, de_B);
+        if (softmax_) {
+            d_ops->sddmmA(dZ, P, ones_A, de_A);
+            d_ops->sddmmB(dZ, P, ones_B, de_B);
+            d_ops->edgeSoftmaxBackward(a_A, de_A, k_sddmmA);
+            d_ops->edgeSoftmaxBackward(a_B, de_B, k_sddmmB);
+            scale_in_place(de_A, g_A);
+            scale_in_place(de_B, g_B);
+        } else {
+            d_ops->sddmmA(dZ, P, g_A, de_A);
+            d_ops->sddmmB(dZ, P, g_B, de_B);
+        }
 
         // dP = S_de P + S_a^T dZ + S_de^T P (A- and B-shaped rows coincide in every supported layout)
         DenseMatrix dP = d_ops->like_A_matrix(0.0), part = d_ops->like_B_matrix(0.0);
@@ -204,6 +231,14 @@ public:
     }
 
 private:
+    string attention_ = "leaky";
+    bool softmax_ = false;
+
+    // v[i] *= s[i]
+    static void scale_in_place(VectorXd &v, const VectorXd &s) {
+        hnh::abi_check(hnh_hadamard_f64(v.data(), v.data(), s.data(), v.size(), hnh::Runtime::get().compute_stream()), "hadamard");
+    }
+
     static void allreduce_world(DenseMatrix &m) {
         std::shared_ptr<hnh::Comm> world = hnh::Comm::world();
         if (world->size() == 1) return;

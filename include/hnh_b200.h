@@ -177,6 +177,47 @@ int hnh_dgemm_tn_f64(double *C, const double *A, const double *B, int64_t m, int
 int hnh_dgemm_nt_f64(double *C, const double *A, const double *B, int64_t m, int64_t n, int64_t k,
                      int accumulate, void *stream);
 
+/* ---- edge softmax: a softmax over the entries of each row (Distributed_Sparse::edgeSoftmax) ----------
+ * x is a value vector of n entries; keys[i] in [0, num_rows) is the row of entry i.  A plan groups the
+ * entries by row: perm (n) lists them by ascending key, stably; row u's entries are
+ * perm[row_start[u] .. row_start[u + 1]); each row is cut into pieces of at most 1024 entries, the pieces of
+ * row u are piece_first[u] .. piece_first[u + 1] - 1 and piece_row[q] is the row of piece q.  Reductions
+ * run one warp per piece, then one warp per row, in an order fixed by the plan: no floating-point atomics,
+ * repeated calls give bit-identical results.  Empty input is a no-op.
+ *
+ * keys[i] = (int32) (idx[i] + offset): the global row of the entries of one CSR block from its stored row or
+ * column index */
+int hnh_edge_keys_from_index(int32_t *keys, const int64_t *idx, int64_t n, int64_t offset, void *stream);
+/* room for piece_row that any plan of n entries over num_rows rows fits in (negative: bad size) */
+int64_t hnh_edge_softmax_piece_bound(int64_t n, int64_t num_rows);
+/* Builds the plan of `keys` (synchronises): perm (n), row_start and piece_first (num_rows + 1 each),
+ * piece_row (piece_capacity); *num_pieces receives the piece count.  n and num_rows below 2^31 - 1;
+ * HNH_E_INVALID when a key lies outside [0, num_rows). */
+int hnh_edge_softmax_plan(const int32_t *keys, int64_t n, int64_t num_rows, int32_t *perm, int32_t *row_start,
+                          int32_t *piece_first, int32_t *piece_row, int64_t piece_capacity, int64_t *num_pieces,
+                          void *stream);
+/* row_max[u] = max of x over row u, row_sum[u] = sum of exp(x - row_max[u]) over row u, for every row
+ * (-inf and 0 for a row without entries).  piece_max / piece_sum: num_pieces doubles of workspace. */
+int hnh_edge_softmax_stats_f64(const double *x, const int32_t *perm, const int32_t *row_start,
+                               const int32_t *piece_first, const int32_t *piece_row, int64_t num_rows,
+                               int64_t num_pieces, double *piece_max, double *piece_sum, double *row_max,
+                               double *row_sum, void *stream);
+/* row_sum[u] *= exp(local_max[u] - global_max[u]) (0 where local_max[u] = -inf): a sum made relative to
+ * this rank's row maximum, made relative to the maximum over all ranks */
+int hnh_edge_softmax_rescale_f64(double *row_sum, const double *local_max, const double *global_max,
+                                 int64_t num_rows, void *stream);
+/* alpha[i] = exp(x[i] - row_max[keys[i]]) / row_sum[keys[i]]   (alpha may alias x) */
+int hnh_edge_softmax_apply_f64(double *alpha, const double *x, const int32_t *keys, int64_t n,
+                               const double *row_max, const double *row_sum, void *stream);
+/* row_dot[u] = sum over row u of alpha[i] * grad[i] (0 for a row without entries); piece_dot: num_pieces
+ * doubles of workspace */
+int hnh_edge_softmax_dot_f64(const double *alpha, const double *grad, const int32_t *perm, const int32_t *row_start,
+                             const int32_t *piece_first, const int32_t *piece_row, int64_t num_rows,
+                             int64_t num_pieces, double *piece_dot, double *row_dot, void *stream);
+/* dx[i] = alpha[i] * (grad[i] - row_dot[keys[i]])   (dx may alias grad) */
+int hnh_edge_softmax_backward_f64(double *dx, const double *alpha, const double *grad, const int32_t *keys,
+                                  int64_t n, const double *row_dot, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

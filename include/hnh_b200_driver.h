@@ -152,6 +152,14 @@ int hnhd_alg_op(hnhd_alg_t *alg, int op, hnhd_dense_t *A, hnhd_dense_t *B, hnhd_
 int hnhd_alg_fused_host(hnhd_alg_t *alg, hnhd_dense_t *A, hnhd_dense_t *B, hnhd_vec_t *svals, hnhd_vec_t *result,
                         const double *hostA, const double *hostB, double *hostOut, int mode, int64_t chunk_rows);
 
+/* Edge softmax (Distributed_Sparse::edgeSoftmax): vec becomes, in place, the softmax of its entries over each
+ * row of S; mode 0 = A order (hnhd_vec_like(.., 0, ..): sddmmA / spmmA values), 1 = B order (ST values).
+ * Backward (edgeSoftmaxBackward): grad = dL/d alpha becomes dL/d(scores) = alpha o (grad - t), with t the row
+ * sums of alpha o grad.  Collective, stream-ordered.  HNH_E_INVALID on every rank where a rank does not hold
+ * full-width rows (R-split layouts at p > 1; 1.5D dense shift with local kernel fusion at c > 1). */
+int hnhd_alg_edge_softmax(hnhd_alg_t *alg, hnhd_vec_t *vec, int mode);
+int hnhd_alg_edge_softmax_backward(hnhd_alg_t *alg, const hnhd_vec_t *alpha, hnhd_vec_t *grad, int mode);
+
 /* CUDA-event timing on the library's compute stream: start, ..., stop -> milliseconds. */
 int hnhd_timer_start(void);
 int hnhd_timer_stop(double *ms_out);
@@ -200,6 +208,11 @@ int hnhd_gat_backward(hnhd_gat_t *g, const double *host_output_grad);
 int hnhd_gat_get_weight_grad(hnhd_gat_t *g, int layer, int head, double *host);
 /* dL/d buffer 0 (this rank's rows); hnhd_gat_buffer_shape(0)'s shape */
 int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host);
+/* attention of every head (GAT::set_attention): "leaky" (the default: LeakyReLU of the scores, the
+ * reference's formula) or "softmax" (their edge softmax over each row of S).  Makes the activations stale.
+ * With "softmax" the forward pass raises HNH_E_INVALID on every rank, before any launch, where the layout has
+ * no edge softmax (as hnhd_alg_edge_softmax). */
+int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind);
 void hnhd_gat_destroy(hnhd_gat_t *g);
 
 #ifdef __cplusplus
