@@ -55,6 +55,10 @@ ABI = {
     "hnh_edge_softmax_apply_f64": (C.c_int, [_P, _P, _P, _I64, _P, _P, _P]),
     "hnh_edge_softmax_dot_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _P, _P, _P]),
     "hnh_edge_softmax_backward_f64": (C.c_int, [_P, _P, _P, _P, _I64, _P, _P]),
+    "hnh_edge_sum_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I64, _P, _P, _P]),
+    "hnh_gat_node_scalars_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I64, _P]),
+    "hnh_gat_edge_scores_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, C.c_double, C.c_int, _P]),
+    "hnh_gat_rank2_update_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -199,8 +203,12 @@ ABI.update({
     "hnhd_gat_get_weight_grad": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "hnhd_gat_get_input_grad": (C.c_int, [_P, _P]),
     "hnhd_gat_set_attention": (C.c_int, [_P, C.c_char_p]),
+    "hnhd_gat_set_attention_vectors": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
+    "hnhd_gat_get_attention_grads": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
     "hnhd_alg_edge_softmax": (C.c_int, [_P, _P, C.c_int]),
     "hnhd_alg_edge_softmax_backward": (C.c_int, [_P, _P, _P, C.c_int]),
+    "hnhd_alg_additive_scores": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_double, C.c_int]),
+    "hnhd_alg_edge_sums": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),

@@ -222,9 +222,14 @@ namespace {
 
 // The row grouping of one value order (edgeSoftmax), built on first use.  Kept in a table keyed by the algorithm
 // object rather than in the object, so that the layout of Distributed_Sparse and of its subclasses is unchanged.
+// Additive attention adds, also on first use, the entries' global S-columns (`cols`: additiveScores) and, for the A
+// order, their grouping by column (`col_perm` .. `col_pieces`: edgeSums).
 struct EdgeRows {
     hnh::DeviceBuffer<int32_t> keys, perm, row_start, piece_first, piece_row;
     int64_t n = 0, pieces = 0;
+    hnh::DeviceBuffer<int32_t> cols, col_perm, col_start, col_piece_first, col_piece_row;
+    bool has_cols = false;
+    int64_t col_pieces = -1;  // -1: no column grouping yet
 };
 std::mutex edge_rows_mutex;
 using EdgeRowsTable = std::map<const Distributed_Sparse *, std::array<std::unique_ptr<EdgeRows>, 2>>;
@@ -251,6 +256,33 @@ int64_t values_row_offset(const Distributed_Sparse &d, const SpmatLocal &m, int 
     if (d.p == 1) return 0;
     return &m == d.ST.get() ? (int64_t)block * d.localArows : (int64_t)d.grid->i * d.localArows * d.c;
 }
+// The same for S-columns (additive attention), with the A and B roles swapped: block b of S holds S-columns
+// [b * localBrows, (b + 1) * localBrows), ST holds block row grid->i (height localBrows * c) of S^T.
+int64_t values_col_offset(const Distributed_Sparse &d, const SpmatLocal &m, int block) {
+    if (d.p == 1) return 0;
+    return &m == d.ST.get() ? (int64_t)d.grid->i * d.localBrows * d.c : (int64_t)block * d.localBrows;
+}
+
+// keys[i] = the global S-row (columns == false) or S-column (columns == true) of entry i of a value vector of `order`
+// with n entries, from the CSR blocks that hold that order
+void entry_keys(Distributed_Sparse &d, KernelMode order, int64_t n, int32_t *keys, bool columns, cudaStream_t s) {
+    SpmatLocal &m = *values_matrix(d, order);
+    const bool is_ST = &m == d.ST.get();
+    if ((int64_t)m.blockStarts.back() != n)
+        throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: the value vector does not cover the local blocks");
+    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
+        const int64_t off = (int64_t)m.blockStarts[b], nb = (int64_t)m.blockStarts[b + 1] - off;
+        if (nb == 0) continue;
+        CSRLocal *blk = m.csr_blocks[b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: block " + to_string(b) + " does not match its value range");
+        // S stores its rows as rows, ST as columns; a transposed block swaps the two
+        const bool stored_row = (is_ST == blk->transpose) != columns;
+        const int64_t *idx = stored_row ? blk->row_idx_device() : blk->getActive()->col_idx.data();
+        const int64_t offset = columns ? values_col_offset(d, m, (int)b) : values_row_offset(d, m, (int)b);
+        hnh::abi_check(hnh_edge_keys_from_index(keys + off, idx, nb, offset, s), "edge_keys_from_index");
+    }
+}
 
 EdgeRows &edge_rows(Distributed_Sparse &d, KernelMode order, int64_t n) {
     if (order != k_sddmmA && order != k_sddmmB)
@@ -266,10 +298,6 @@ EdgeRows &edge_rows(Distributed_Sparse &d, KernelMode order, int64_t n) {
     if (*slot) return **slot;
     const int64_t M = d.M;
     if (M >= INT32_MAX) throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: S has " + to_string(M) + " rows; at most 2^31 - 2");
-    SpmatLocal &m = *values_matrix(d, order);
-    const bool is_ST = &m == d.ST.get();
-    if ((int64_t)m.blockStarts.back() != n)
-        throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: the value vector does not cover the local blocks");
     cudaStream_t s = Runtime::get().compute_stream();
     std::unique_ptr<EdgeRows> e(new EdgeRows);
     e->n = n;
@@ -280,18 +308,7 @@ EdgeRows &edge_rows(Distributed_Sparse &d, KernelMode order, int64_t n) {
     const int64_t bound = hnh_edge_softmax_piece_bound(n, M);
     if (bound < 0) hnh::abi_check((int)bound, "edge_softmax_piece_bound");
     e->piece_row.resize((size_t)std::max<int64_t>(bound, 1));
-    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
-        const int64_t off = (int64_t)m.blockStarts[b], nb = (int64_t)m.blockStarts[b + 1] - off;
-        if (nb == 0) continue;
-        CSRLocal *blk = m.csr_blocks[b];
-        if (blk == nullptr || blk->num_coords != nb)
-            throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: block " + to_string(b) + " does not match its value range");
-        // S stores its rows as rows, ST as columns; a transposed block swaps the two
-        const bool stored_row = is_ST == blk->transpose;
-        const int64_t *idx = stored_row ? blk->row_idx_device() : blk->getActive()->col_idx.data();
-        hnh::abi_check(hnh_edge_keys_from_index(e->keys.data() + off, idx, nb, values_row_offset(d, m, (int)b), s),
-                       "edge_keys_from_index");
-    }
+    entry_keys(d, order, n, e->keys.data(), false, s);
     int64_t pieces = 0;
     hnh::abi_check(hnh_edge_softmax_plan(e->keys.data(), n, M, e->perm.data(), e->row_start.data(), e->piece_first.data(),
                                          e->piece_row.data(), (int64_t)e->piece_row.size(), &pieces, s),
@@ -299,6 +316,37 @@ EdgeRows &edge_rows(Distributed_Sparse &d, KernelMode order, int64_t n) {
     e->pieces = pieces;
     *slot = std::move(e);
     return **slot;
+}
+
+// edge_rows with the entries' S-columns (additive attention)
+EdgeRows &edge_cols(Distributed_Sparse &d, KernelMode order, int64_t n) {
+    EdgeRows &e = edge_rows(d, order, n);
+    if (e.has_cols) return e;
+    if (d.N >= INT32_MAX) throw hnh::Error(HNH_E_INVALID, "additive attention: S has " + to_string(d.N) + " columns; at most 2^31 - 2");
+    e.cols.resize((size_t)n);
+    entry_keys(d, order, n, e.cols.data(), true, Runtime::get().compute_stream());
+    e.has_cols = true;
+    return e;
+}
+
+// edge_cols of the A order with the entries grouped by S-column, as edge_rows groups them by S-row
+EdgeRows &edge_col_plan(Distributed_Sparse &d, int64_t n) {
+    EdgeRows &e = edge_cols(d, k_sddmmA, n);
+    if (e.col_pieces >= 0) return e;
+    const int64_t N = d.N;
+    e.col_perm.resize((size_t)n);
+    e.col_start.resize((size_t)N + 1);
+    e.col_piece_first.resize((size_t)N + 1);
+    const int64_t bound = hnh_edge_softmax_piece_bound(n, N);
+    if (bound < 0) hnh::abi_check((int)bound, "edge_softmax_piece_bound");
+    e.col_piece_row.resize((size_t)std::max<int64_t>(bound, 1));
+    int64_t pieces = 0;
+    hnh::abi_check(hnh_edge_softmax_plan(e.cols.data(), n, N, e.col_perm.data(), e.col_start.data(), e.col_piece_first.data(),
+                                         e.col_piece_row.data(), (int64_t)e.col_piece_row.size(), &pieces,
+                                         Runtime::get().compute_stream()),
+                   "edge_softmax_plan");
+    e.col_pieces = pieces;
+    return e;
 }
 
 }  // namespace
@@ -355,6 +403,39 @@ void Distributed_Sparse::edgeSoftmaxBackward(const VectorXd &alpha, VectorXd &gr
     hnh::abi_check(hnh_edge_softmax_backward_f64(grad.data(), alpha.data(), grad.data(), e.keys.data(), e.n, row_dot.data(),
                                                  compute()),
                    "edge_softmax_backward");
+}
+
+// ---- additive attention --------------------------------------------------------------------------------------
+void Distributed_Sparse::additiveScores(const VectorXd &s, const VectorXd &t, VectorXd &out, KernelMode order, double alpha,
+                                        bool derivative) {
+    check_full_rows("additiveScores");
+    if (s.size() < M || t.size() < N)
+        throw hnh::Error(HNH_E_INVALID, "additiveScores: s has " + to_string(s.size()) + " entries and t " + to_string(t.size()) +
+                                            "; S is " + to_string(M) + " x " + to_string(N));
+    EdgeRows &e = edge_cols(*this, order, out.size());
+    hnh::abi_check(hnh_gat_edge_scores_f64(out.data(), s.data(), t.data(), e.keys.data(), e.cols.data(), e.n, alpha,
+                                           derivative ? 1 : 0, compute()),
+                   "gat_edge_scores");
+}
+
+void Distributed_Sparse::edgeSums(const VectorXd &values, VectorXd &row_sums, VectorXd &col_sums) {
+    check_full_rows("edgeSums");
+    if (row_sums.size() < M || col_sums.size() < N)
+        throw hnh::Error(HNH_E_INVALID, "edgeSums: room for " + to_string(row_sums.size()) + " row sums and " +
+                                            to_string(col_sums.size()) + " column sums; S is " + to_string(M) + " x " +
+                                            to_string(N));
+    EdgeRows &e = edge_col_plan(*this, values.size());
+    VectorXd piece(std::max<int64_t>({e.pieces, e.col_pieces, 1}));
+    row_sums.setZero();  // the entries past M / N stay 0
+    col_sums.setZero();
+    hnh::abi_check(hnh_edge_sum_f64(values.data(), e.perm.data(), e.row_start.data(), e.piece_first.data(), e.piece_row.data(), M,
+                                    e.pieces, piece.data(), row_sums.data(), compute()),
+                   "edge_sum rows");
+    hnh::abi_check(hnh_edge_sum_f64(values.data(), e.col_perm.data(), e.col_start.data(), e.col_piece_first.data(),
+                                    e.col_piece_row.data(), N, e.col_pieces, piece.data(), col_sums.data(), compute()),
+                   "edge_sum columns");
+    allreduce_rows(row_sums.data(), M, false);
+    allreduce_rows(col_sums.data(), N, false);
 }
 
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {

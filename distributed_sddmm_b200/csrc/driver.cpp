@@ -335,6 +335,20 @@ int hnhd_alg_edge_softmax_backward(hnhd_alg_t *a, const hnhd_vec_t *alpha, hnhd_
     });
 }
 
+int hnhd_alg_additive_scores(hnhd_alg_t *a, const hnhd_vec_t *s, const hnhd_vec_t *t, hnhd_vec_t *out, int mode, double alpha,
+                              int derivative) {
+    return guarded([&] {
+        if (!a || !s || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_additive_scores: null argument");
+        a->alg->additiveScores(s->v, t->v, out->v, value_order(mode), alpha, derivative != 0);
+    });
+}
+int hnhd_alg_edge_sums(hnhd_alg_t *a, const hnhd_vec_t *values, hnhd_vec_t *row_sums, hnhd_vec_t *col_sums) {
+    return guarded([&] {
+        if (!a || !values || !row_sums || !col_sums) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_edge_sums: null argument");
+        a->alg->edgeSums(values->v, row_sums->v, col_sums->v);
+    });
+}
+
 int hnhd_timer_start(void) {
     return guarded([] {
         if (!g_t0) {
@@ -511,6 +525,35 @@ int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind) {
     return guarded([&] {
         if (!g || !kind) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_set_attention: null argument");
         g->g->set_attention(kind);
+    });
+}
+// copy n doubles between host and device on the compute stream and wait for the copy
+static void gat_copy(double *dst, const double *src, int64_t n, cudaMemcpyKind kind) {
+    cudaStream_t s = hnh::Runtime::get().compute_stream();
+    hnh::cuda_check(cudaMemcpyAsync(dst, src, sizeof(double) * (size_t)n, kind, s), "gat attention vector copy");
+    hnh::cuda_check(cudaStreamSynchronize(s), "gat attention vector copy");
+}
+int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const double *a1, const double *a2) {
+    return guarded([&] {
+        if (!a1 || !a2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_weight(g, layer, head);  // validates layer and head
+        GATLayer &l = g->g->layers[(size_t)layer];
+        const int64_t off = (int64_t)head * l.features_per_head;
+        gat_copy(l.a1.data() + off, a1, l.features_per_head, cudaMemcpyHostToDevice);
+        gat_copy(l.a2.data() + off, a2, l.features_per_head, cudaMemcpyHostToDevice);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2) {
+    return guarded([&] {
+        if (!da1 || !da2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_weight(g, layer, head);  // validates layer and head
+        const GATLayer &l = g->g->layers[(size_t)layer];
+        if (l.a1Grads.size() != l.a1.size() || l.a2Grads.size() != l.a2.size())
+            throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
+        const int64_t off = (int64_t)head * l.features_per_head;
+        gat_copy(da1, l.a1Grads.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
+        gat_copy(da2, l.a2Grads.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
     });
 }
 void hnhd_gat_destroy(hnhd_gat_t *g) { delete g; }

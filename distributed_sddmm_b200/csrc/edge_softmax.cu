@@ -192,6 +192,22 @@ __global__ void piece_dot_kernel(const double *__restrict__ a, const double *__r
     }
 }
 
+// piece_dot_kernel's order with one operand: the sum of x over each piece
+__global__ void piece_sum_kernel(const double *__restrict__ x, const int32_t *__restrict__ perm, const int32_t *__restrict__ row_start,
+                                 const int32_t *__restrict__ piece_first, const int32_t *__restrict__ piece_row, int64_t num_pieces,
+                                 double *__restrict__ piece_val) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t q = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; q < num_pieces; q += warps) {
+        int64_t lo, hi;
+        piece_range(q, row_start, piece_first, piece_row, &lo, &hi);
+        double t = 0.0;
+        for (int64_t p = lo + lane; p < hi; p += 32) t += x[perm[p]];
+        t = sum_warp_reduce(t);
+        if (lane == 0) piece_val[q] = t;
+    }
+}
+
 __global__ void row_sum_kernel(const int32_t *__restrict__ piece_first, int64_t num_rows, const double *__restrict__ piece_val,
                                double *__restrict__ row_val) {
     const int lane = threadIdx.x & 31;
@@ -369,6 +385,24 @@ int hnh_edge_softmax_dot_f64(const double *alpha, const double *grad, const int3
     row_sum_kernel<<<grid_for(num_rows, kThreads / 32), kThreads, 0, st>>>(piece_first, num_rows, piece_dot, row_dot);
     count_launch(1);
     return check_cuda(cudaGetLastError(), "edge softmax dot kernels launch");
+}
+
+int hnh_edge_sum_f64(const double *x, const int32_t *perm, const int32_t *row_start, const int32_t *piece_first,
+                     const int32_t *piece_row, int64_t num_rows, int64_t num_pieces, double *piece_sum, double *row_sum,
+                     void *stream) {
+    int rc = check_plan("hnh_edge_sum_f64", perm, row_start, piece_first, piece_row, num_rows, num_pieces);
+    if (rc) return rc;
+    if (num_rows == 0) return HNH_OK;
+    if (!row_sum || (num_pieces > 0 && (!x || !piece_sum))) return set_error(HNH_E_INVALID, "hnh_edge_sum_f64: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (num_pieces > 0) {
+        piece_sum_kernel<<<grid_for(num_pieces, kThreads / 32), kThreads, 0, st>>>(x, perm, row_start, piece_first, piece_row,
+                                                                                    num_pieces, piece_sum);
+        count_launch(1);
+    }
+    row_sum_kernel<<<grid_for(num_rows, kThreads / 32), kThreads, 0, st>>>(piece_first, num_rows, piece_sum, row_sum);
+    count_launch(1);
+    return check_cuda(cudaGetLastError(), "edge sum kernels launch");
 }
 
 int hnh_edge_softmax_backward_f64(double *dx, const double *alpha, const double *grad, const int32_t *keys, int64_t n,

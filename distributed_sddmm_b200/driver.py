@@ -265,6 +265,16 @@ class Algorithm:
         row sums of alpha * grad (Distributed_Sparse::edgeSoftmaxBackward)."""
         check(lib().hnhd_alg_edge_softmax_backward(self.h, alpha.h, grad.h, _value_order(mode)), "edge_softmax_backward")
 
+    def additive_scores(self, s: Vec, t: Vec, out: Vec, mode: str = "A", alpha: float = 0.2, derivative: bool = False):
+        """out (a value vector of `mode`) = LeakyReLU(s[row] + t[col]) per stored entry of S, or its derivative; s and
+        t are whole node vectors (Distributed_Sparse::additiveScores)."""
+        check(lib().hnhd_alg_additive_scores(self.h, s.h, t.h, out.h, _value_order(mode), float(alpha), int(derivative)),
+              "additive_scores")
+
+    def edge_sums(self, values: Vec, row_sums: Vec, col_sums: Vec):
+        """Collective: the row and column sums of an A-order value vector over all ranks (Distributed_Sparse::edgeSums)."""
+        check(lib().hnhd_alg_edge_sums(self.h, values.h, row_sums.h, col_sums.h), "edge_sums")
+
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
 
@@ -355,12 +365,16 @@ def benchmark_algorithm(S: SpmatLocal, name: str, R: int, c: int, fused=True, ap
 
 class GAT:
     """Multi-head graph attention: forward pass and weight / input gradients (include/hnh/gat.hpp).  layers: [(input_features,
-    features_per_head, num_heads), ...].  attention: "leaky" (LeakyReLU of the scores, the reference's formula) or
-    "softmax" (their softmax over each node's neighbours).  The algorithm object must outlive this one."""
+    features_per_head, num_heads), ...].  attention: "leaky" (LeakyReLU of the scores, the reference's formula),
+    "softmax" (their softmax over each node's neighbours) or "additive" (the softmax of LeakyReLU(a1 . h_u + a2 . h_v),
+    Velickovic et al. 2018; a1 and a2 per head through set_attention_vectors, zero by default).  The algorithm object
+    must outlive this one."""
+
+    ATTENTIONS = ("leaky", "softmax", "additive")
 
     def __init__(self, alg: Algorithm, layers, leaky_relu_alpha: float = 0.2, attention: str = "leaky"):
-        if attention not in ("leaky", "softmax"):
-            raise ValueError(f'attention must be "leaky" or "softmax", not {attention!r}')
+        if attention not in self.ATTENTIONS:
+            raise ValueError(f'attention must be "leaky", "softmax" or "additive", not {attention!r}')
         self.alg = alg
         self.layers = [tuple(int(x) for x in l) for l in layers]
         flat = (C.c_int * (3 * len(self.layers)))(*[x for l in self.layers for x in l])
@@ -369,7 +383,7 @@ class GAT:
         self.set_attention(attention)
 
     def set_attention(self, kind: str):
-        """"leaky" or "softmax"; the next backward pass needs a forward pass first."""
+        """"leaky", "softmax" or "additive"; the next backward pass needs a forward pass first."""
         check(lib().hnhd_gat_set_attention(self.h, kind.encode()), "gat_set_attention")
         self.attention = kind
 
@@ -408,6 +422,24 @@ class GAT:
         last = len(self.layers)
         assert g.shape == self.buffer_shape(last), (g.shape, self.buffer_shape(last))
         check(lib().hnhd_gat_backward(self.h, g.ctypes.data), "gat_backward")
+
+    def set_attention_vectors(self, layer: int, head: int, a1, a2):
+        """The additive attention vectors of (layer, head), features_per_head long each; the next backward pass needs
+        a forward pass first."""
+        fph = self.layers[layer][1]
+        a1, a2 = (np.ascontiguousarray(a, dtype=np.float64) for a in (a1, a2))
+        assert a1.shape == (fph,) and a2.shape == (fph,), (a1.shape, a2.shape, fph)
+        check(lib().hnhd_gat_set_attention_vectors(self.h, layer, head, a1.ctypes.data, a2.ctypes.data),
+              "gat_set_attention_vectors")
+
+    def attention_grads(self, layer: int, head: int):
+        """(dL/d a1, dL/d a2) of (layer, head) after a backward pass, summed over all ranks (zero unless the
+        attention is additive)."""
+        fph = self.layers[layer][1]
+        da1, da2 = np.empty(fph), np.empty(fph)
+        check(lib().hnhd_gat_get_attention_grads(self.h, layer, head, da1.ctypes.data, da2.ctypes.data),
+              "gat_get_attention_grads")
+        return da1, da2
 
     def weight_grad(self, layer: int, head: int):
         """dL/d weight (layer, head), summed over all ranks."""

@@ -166,6 +166,18 @@ public:
     // GAT's backward pass and softmax attention and edgeSoftmax need this.  Decided from global quantities
     // only, so every rank throws together and no collective is left waiting.
     void check_full_rows(const string &operation) const;
+
+    // ---- additive graph attention (GAT::set_attention("additive")) ------------------------------------------
+    // additiveScores: out (a value vector of `order`) becomes LeakyReLU(s[u] + t[v]) for every stored entry (u, v)
+    // of S -- or, with `derivative`, its derivative: 1 where s[u] + t[v] > 0, alpha elsewhere.  s is indexed by
+    // global S-row (at least M entries), t by global S-column (at least N): node vectors every rank holds whole.
+    // Elementwise, no communication.  edgeSums: row_sums[u] / col_sums[v] become the sums of `values` (an A-order
+    // vector) over the stored entries of row u / column v of S on all ranks, in a fixed order (bit-identical
+    // repeats); entries past M / N are set to 0.  Two sum all-reduces at p > 1.  The first call per order builds
+    // the entries' column keys, and edgeSums the grouping of the A order by column; they are kept with
+    // edgeSoftmax's row grouping.  Defined where check_full_rows passes; HNH_E_INVALID on every rank elsewhere.
+    void additiveScores(const VectorXd &s, const VectorXd &t, VectorXd &out, KernelMode order, double alpha, bool derivative);
+    void edgeSums(const VectorXd &values, VectorXd &row_sums, VectorXd &col_sums);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

@@ -34,10 +34,26 @@
 // alpha is recomputed in both orders.  Per head this adds one O(nnz) softmax to the forward pass, and four O(nnz)
 // softmax calls (and, at p > 1, six M-long all-reduces) to the backward pass; the sparse pass count is unchanged.
 //
+// Additive attention (set_attention("additive"), the attention of Velickovic et al. 2018) scores an edge from two
+// node scalars instead of an r-wide dot product.  With a1, a2 the head's slices [j * fph, (j + 1) * fph) of
+// layer.a1 / layer.a2 (zero after construction: uniform attention, i.e. mean aggregation):
+//     s = P a1, t = P a2                   over this rank's rows, gathered into whole node vectors  (hnh_gat_node_scalars_f64)
+//     alpha = edge softmax of x_uv = LeakyReLU(s_u + t_v)                  (Distributed_Sparse::additiveScores, edgeSoftmax)
+//     Z = S_alpha P, X_out[:, head window] = ReLU(Z)
+// Backward, with x' = LeakyReLU'(s_u + t_v):
+//     dalpha = S o (dZ P^T)                                  SDDMM with SValues = 1, A order only
+//     de     = x' o edgeSoftmaxBackward(alpha, dalpha)       A order
+//     ds_u = sum_v de_uv, dt_v = sum_u de_uv                 world row and column sums (Distributed_Sparse::edgeSums)
+//     dP     = S_alpha^T dZ + ds a1^T + dt a2^T              one B-order SpMM (alpha recomputed in the B order from s and
+//                                                            t), then a rank-2 row update (hnh_gat_rank2_update_f64)
+//     da1 = P^T ds, da2 = P^T dt over this rank's rows, summed over all ranks (layer.a1Grads / a2Grads); dW, dX as above
+// Per head: forward 1 SpMM pass, backward 1 SDDMM and 1 SpMM pass, against 1 + 1 and 4 + 3 for the dot-product
+// attention.  The forward stores nothing extra: P, s, t and alpha are recomputed.
+//
 // The forward pass is the GAT formula only where every rank holds full-width rows and the A and B layouts coincide:
 // p = 1 (any algorithm), 1.5D dense shift with replication reuse (fusion 1) at any c, and with local kernel fusion
-// (fusion 2) at c = 1 (Distributed_Sparse::check_full_rows).  Only there are the backward pass and softmax attention
-// defined; elsewhere they throw HNH_E_INVALID on every rank.
+// (fusion 2) at c = 1 (Distributed_Sparse::check_full_rows).  Only there are the backward pass and softmax and additive
+// attention defined; elsewhere they throw HNH_E_INVALID on every rank.
 #pragma once
 #include <string>
 #include <vector>
@@ -54,8 +70,13 @@ public:
 
     vector<DenseMatrix> wMats;  // one input_width x head_width projection per head
     vector<DenseMatrix> wGrads; // dL/d wMats[j] after GAT::backwardPass (empty before the first one); same on every rank
-    VectorXd a1;                // attention vectors: declared by the reference, unused by its forward pass
+    // attention vectors (declared by the reference, unused by its forward pass): num_heads * features_per_head
+    // doubles each, head j's at [j * features_per_head, (j + 1) * features_per_head).  GAT allocates them as zeros;
+    // only additive attention reads them.
+    VectorXd a1;
     VectorXd a2;
+    VectorXd a1Grads;  // dL/d a1, dL/d a2 after GAT::backwardPass (empty before the first one; zero unless the
+    VectorXd a2Grads;  // attention is additive); same on every rank
 
     GATLayer(int in_width, int head_width, int heads)
         : input_features(in_width), features_per_head(head_width), num_heads(heads) {}
@@ -88,6 +109,8 @@ public:
             layer.wMats.clear();
             for (int h = 0; h < layer.num_heads; h++)
                 layer.wMats.push_back(DenseMatrix::Constant(in_cols, d_ops->localAcols, 0.0));
+            layer.a1 = VectorXd::Constant((int64_t)layer.num_heads * layer.features_per_head, 0.0);
+            layer.a2 = VectorXd::Constant((int64_t)layer.num_heads * layer.features_per_head, 0.0);
         }
     }
 
@@ -101,19 +124,29 @@ public:
         DenseMatrix neighbours = projected;  // the same projection in the role of the other SDDMM operand
         d_ops->de_shift(&neighbours, nullptr, k_spmmA);
 
-        VectorXd pattern = d_ops->like_S_values(1.0);
         VectorXd scores = d_ops->like_S_values(1.0);
-        d_ops->algorithm(projected, neighbours, pattern, &scores, k_sddmmA, true);
-        scores.leakyRelu(leaky_relu_alpha);
-        if (softmax_) d_ops->edgeSoftmax(scores, k_sddmmA);
+        if (additive_) {
+            VectorXd s, t;
+            node_scalars(layer, j, projected, s, t);
+            d_ops->additiveScores(s, t, scores, k_sddmmA, leaky_relu_alpha, false);
+            d_ops->edgeSoftmax(scores, k_sddmmA);
+        } else {
+            VectorXd pattern = d_ops->like_S_values(1.0);
+            d_ops->algorithm(projected, neighbours, pattern, &scores, k_sddmmA, true);
+            scores.leakyRelu(leaky_relu_alpha);
+            if (softmax_) d_ops->edgeSoftmax(scores, k_sddmmA);
+        }
 
         projected.setZero();  // becomes the SpMM accumulator
-        d_ops->algorithm(projected, neighbours, scores, nullptr, k_spmmA, false);
+        // replication reuse: the SDDMM pass has replicated the stationary operand, except with additive attention,
+        // which has no SDDMM pass
+        d_ops->algorithm(projected, neighbours, scores, nullptr, k_spmmA, additive_);
         output.setMiddleColsRelu((int64_t)j * projected.cols(), projected);
     }
 
     void forwardPass() {
         if (softmax_) d_ops->check_full_rows("GAT softmax attention");
+        if (additive_) d_ops->check_full_rows("GAT additive attention");
         for (size_t i = 0; i < layers.size(); i++)
             for (int j = 0; j < layers[i].num_heads; j++) computeSelfAttentionHead((int)i, j);
         activations_current = true;
@@ -129,20 +162,22 @@ public:
     // file).  Decided from global quantities only, so every rank throws together and no collective is left waiting.
     void check_backward_supported() const { d_ops->check_full_rows("GAT::backwardPass"); }
 
-    // "leaky" (the reference's attention, the default) or "softmax" (see the top of this file).  Changing it makes
-    // the activations stale.
+    // "leaky" (the reference's attention, the default), "softmax" or "additive" (see the top of this file).  Changing
+    // it makes the activations stale.
     const string &attention() const { return attention_; }
     void set_attention(const string &kind) {
-        if (kind != "leaky" && kind != "softmax")
-            throw hnh::Error(HNH_E_INVALID, "GAT: attention must be \"leaky\" or \"softmax\", not \"" + kind + "\"");
+        if (kind != "leaky" && kind != "softmax" && kind != "additive")
+            throw hnh::Error(HNH_E_INVALID, "GAT: attention must be \"leaky\", \"softmax\" or \"additive\", not \"" + kind + "\"");
         if (kind != attention_) activations_current = false;
         attention_ = kind;
         softmax_ = kind == "softmax";
+        additive_ = kind == "additive";
     }
 
-    // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d wMats in layers[i].wGrads (summed over all
-    // ranks: identical everywhere) and dL/d buffers[0] in input_grad.  Collective.  Reads buffers, wMats and
-    // leaky_relu_alpha and changes none of them; gradient storage is allocated on the first call.
+    // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d wMats in layers[i].wGrads and dL/d a1 / a2
+    // in layers[i].a1Grads / a2Grads (summed over all ranks: identical everywhere), and dL/d buffers[0] in
+    // input_grad.  Collective.  Reads buffers, wMats, a1, a2 and leaky_relu_alpha and changes none of them; gradient
+    // storage is allocated on the first call.
     void backwardPass(const DenseMatrix &output_grad) {
         check_backward_supported();
         if (!activations_current)
@@ -156,6 +191,11 @@ public:
             if (layer.wGrads.size() != layer.wMats.size()) {
                 layer.wGrads.clear();
                 for (const DenseMatrix &w : layer.wMats) layer.wGrads.emplace_back(w.rows(), w.cols());
+            }
+        for (GATLayer &layer : layers)
+            if (layer.a1Grads.size() != layer.a1.size() || !additive_) {  // the other kinds do not read a1 / a2
+                layer.a1Grads = VectorXd::Constant(layer.a1.size(), 0.0);
+                layer.a2Grads = VectorXd::Constant(layer.a2.size(), 0.0);
             }
         // two layer gradients are live at a time: that of the layer's output (upstream) and that of its input
         DenseMatrix upstream;
@@ -172,6 +212,7 @@ public:
     // head j of layer i: G = dL/d buffers[i + 1]; writes layers[i].wGrads[j] and adds (or, accumulate == false,
     // writes) the head's share of dL/d buffers[i] into dX
     void backwardHead(int i, int j, const DenseMatrix &G, DenseMatrix &dX, bool accumulate) {
+        if (additive_) return backwardHeadAdditive(i, j, G, dX, accumulate);
         GATLayer &layer = layers.at((size_t)i);
         const DenseMatrix &input = buffers[(size_t)i], &output = buffers[(size_t)i + 1];
         const DenseMatrix &W = layer.wMats.at((size_t)j);
@@ -230,21 +271,96 @@ public:
         dX.setTimesTranspose(dP, W, accumulate);
     }
 
+    // backwardHead with additive attention (see the top of this file)
+    void backwardHeadAdditive(int i, int j, const DenseMatrix &G, DenseMatrix &dX, bool accumulate) {
+        GATLayer &layer = layers.at((size_t)i);
+        const DenseMatrix &input = buffers[(size_t)i], &output = buffers[(size_t)i + 1];
+        const DenseMatrix &W = layer.wMats.at((size_t)j);
+        d_ops->setRValue(layer.features_per_head);
+        cudaStream_t st = hnh::Runtime::get().compute_stream();
+        DenseMatrix P = input * W;
+        VectorXd s, t;
+        node_scalars(layer, j, P, s, t);
+
+        // alpha in both orders, each from s and t
+        VectorXd alpha_A = d_ops->like_S_values(0.0), alpha_B = d_ops->like_ST_values(0.0);
+        d_ops->additiveScores(s, t, alpha_A, k_sddmmA, leaky_relu_alpha, false);
+        d_ops->edgeSoftmax(alpha_A, k_sddmmA);
+        d_ops->additiveScores(s, t, alpha_B, k_sddmmB, leaky_relu_alpha, false);
+        d_ops->edgeSoftmax(alpha_B, k_sddmmB);
+
+        // de = x' o edgeSoftmaxBackward(alpha, S o (dZ P^T)), A order
+        DenseMatrix dZ(P.rows(), P.cols());
+        dZ.setMiddleColsReluGrad(G, output, (int64_t)j * layer.features_per_head);
+        VectorXd ones_A = d_ops->like_S_values(1.0), de = d_ops->like_S_values(0.0), x_grad = d_ops->like_S_values(0.0);
+        d_ops->sddmmA(dZ, P, ones_A, de);
+        d_ops->edgeSoftmaxBackward(alpha_A, de, k_sddmmA);
+        d_ops->additiveScores(s, t, x_grad, k_sddmmA, leaky_relu_alpha, true);
+        scale_in_place(de, x_grad);
+
+        // ds, dt: the row and column sums of de over all ranks, in the node vectors' layout (s and t are done with)
+        VectorXd &ds = s, &dt = t;
+        d_ops->edgeSums(de, ds, dt);
+
+        // dP = S_alpha^T dZ + ds a1^T + dt a2^T on this rank's rows (A- and B-shaped rows coincide where this runs)
+        const int64_t top = d_ops->aSubmatrices.at(0).topRow, off = (int64_t)j * layer.features_per_head;
+        DenseMatrix dP = d_ops->like_B_matrix(0.0);
+        d_ops->spmmB(dZ, dP, alpha_B);
+        hnh::abi_check(hnh_gat_rank2_update_f64(dP.data(), ds.data() + top, dt.data() + top, layer.a1.data() + off,
+                                                layer.a2.data() + off, dP.rows(), dP.cols(), st),
+                       "gat_rank2_update");
+
+        // [da1 da2] = P^T [ds dt] over this rank's rows, summed over the ranks
+        const size_t d = sizeof(double);
+        DenseMatrix dst(P.rows(), 2), da(P.cols(), 2);
+        hnh::cuda_check(cudaMemcpy2DAsync(dst.data(), 2 * d, ds.data() + top, d, d, (size_t)P.rows(), cudaMemcpyDeviceToDevice, st), "ds column");
+        hnh::cuda_check(cudaMemcpy2DAsync(dst.data() + 1, 2 * d, dt.data() + top, d, d, (size_t)P.rows(), cudaMemcpyDeviceToDevice, st), "dt column");
+        da.setTransposeTimes(P, dst);
+        allreduce_world(da);
+        hnh::cuda_check(cudaMemcpy2DAsync(layer.a1Grads.data() + off, d, da.data(), 2 * d, d, (size_t)P.cols(), cudaMemcpyDeviceToDevice, st), "da1");
+        hnh::cuda_check(cudaMemcpy2DAsync(layer.a2Grads.data() + off, d, da.data() + 1, 2 * d, d, (size_t)P.cols(), cudaMemcpyDeviceToDevice, st), "da2");
+
+        DenseMatrix &dW = layer.wGrads.at((size_t)j);
+        dW.setTransposeTimes(input, dP);
+        allreduce_world(dW);
+        dX.setTimesTranspose(dP, W, accumulate);
+    }
+
 private:
     string attention_ = "leaky";
     bool softmax_ = false;
+    bool additive_ = false;
+
+    // Head j's node scalars s = P a1 and t = P a2 as whole node vectors (localArows * p entries, at least M and N;
+    // those at or past M are 0): each rank writes its own rows at aSubmatrices[0].topRow into zeros, and a sum
+    // all-reduce -- exact, every entry has one contributor -- gives every rank all of them.
+    void node_scalars(const GATLayer &layer, int j, const DenseMatrix &P, VectorXd &s, VectorXd &t) {
+        const int64_t len = std::max<int64_t>((int64_t)d_ops->localArows * d_ops->p, std::max(d_ops->M, d_ops->N));
+        const int64_t top = d_ops->aSubmatrices.at(0).topRow, off = (int64_t)j * layer.features_per_head;
+        if (top + P.rows() > len || P.cols() != layer.features_per_head)
+            throw hnh::Error(HNH_E_INVALID, "GAT additive attention: the projection does not fit the node vectors");
+        s = VectorXd::Constant(len, 0.0);
+        t = VectorXd::Constant(len, 0.0);
+        hnh::abi_check(hnh_gat_node_scalars_f64(s.data() + top, t.data() + top, P.data(), layer.a1.data() + off,
+                                                layer.a2.data() + off, P.rows(), P.cols(), hnh::Runtime::get().compute_stream()),
+                       "gat_node_scalars");
+        allreduce_world(s);
+        allreduce_world(t);
+    }
 
     // v[i] *= s[i]
     static void scale_in_place(VectorXd &v, const VectorXd &s) {
         hnh::abi_check(hnh_hadamard_f64(v.data(), v.data(), s.data(), v.size(), hnh::Runtime::get().compute_stream()), "hadamard");
     }
 
-    static void allreduce_world(DenseMatrix &m) {
+    static void allreduce_world(DenseMatrix &m) { allreduce_world(m.data(), m.size()); }
+    static void allreduce_world(VectorXd &v) { allreduce_world(v.data(), v.size()); }
+    static void allreduce_world(double *p, int64_t n) {
         std::shared_ptr<hnh::Comm> world = hnh::Comm::world();
         if (world->size() == 1) return;
         hnh::Runtime &rt = hnh::Runtime::get();
         rt.chain(rt.compute_stream(), rt.comm_stream());
-        world->allreduce_sum_f64(m.data(), (size_t)m.size(), rt.comm_stream());
+        world->allreduce_sum_f64(p, (size_t)n, rt.comm_stream());
         rt.chain(rt.comm_stream(), rt.compute_stream());
     }
 };

@@ -217,6 +217,25 @@ int hnh_edge_softmax_dot_f64(const double *alpha, const double *grad, const int3
 /* dx[i] = alpha[i] * (grad[i] - row_dot[keys[i]])   (dx may alias grad) */
 int hnh_edge_softmax_backward_f64(double *dx, const double *alpha, const double *grad, const int32_t *keys,
                                   int64_t n, const double *row_dot, void *stream);
+/* row_sum[u] = sum over row u of x[i] (0 for a row without entries), in the order of hnh_edge_softmax_dot_f64;
+ * piece_sum: num_pieces doubles of workspace.  With a plan keyed by column, the column sums. */
+int hnh_edge_sum_f64(const double *x, const int32_t *perm, const int32_t *row_start, const int32_t *piece_first,
+                     const int32_t *piece_row, int64_t num_rows, int64_t num_pieces, double *piece_sum,
+                     double *row_sum, void *stream);
+
+/* ---- additive graph attention (GAT::set_attention("additive"); csrc/gat_additive.cu) ------------------
+ * s[i] = sum_k P[i, k] a1[k] and t[i] = sum_k P[i, k] a2[k] for a row-major n x d P, in one read of P; the
+ * summation order is fixed (repeated calls are bit-identical) */
+int hnh_gat_node_scalars_f64(double *s, double *t, const double *P, const double *a1, const double *a2, int64_t n,
+                             int64_t d, void *stream);
+/* out[k] = LeakyReLU(s[row_key[k]] + t[col_key[k]]) (hnh_leaky_relu_f64's formula), or, derivative != 0, its
+ * derivative: 1 where s + t > 0, alpha elsewhere (hnh_leaky_relu_grad_f64's convention).  Elementwise in the order
+ * of the keys. */
+int hnh_gat_edge_scores_f64(double *out, const double *s, const double *t, const int32_t *row_key,
+                            const int32_t *col_key, int64_t n, double alpha, int derivative, void *stream);
+/* dP[i, :] += ds[i] * a1 + dt[i] * a2 for a row-major n x d dP (the backward's rank-2 row update) */
+int hnh_gat_rank2_update_f64(double *dP, const double *ds, const double *dt, const double *a1, const double *a2,
+                             int64_t n, int64_t d, void *stream);
 
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of

@@ -159,6 +159,15 @@ int hnhd_alg_fused_host(hnhd_alg_t *alg, hnhd_dense_t *A, hnhd_dense_t *B, hnhd_
  * full-width rows (R-split layouts at p > 1; 1.5D dense shift with local kernel fusion at c > 1). */
 int hnhd_alg_edge_softmax(hnhd_alg_t *alg, hnhd_vec_t *vec, int mode);
 int hnhd_alg_edge_softmax_backward(hnhd_alg_t *alg, const hnhd_vec_t *alpha, hnhd_vec_t *grad, int mode);
+/* Additive attention (Distributed_Sparse::additiveScores / edgeSums).  out (a value vector of `mode`, as above)
+ * becomes LeakyReLU(s[u] + t[v]) for every stored entry (u, v) of S, or with derivative != 0 its derivative (1
+ * where s[u] + t[v] > 0, alpha elsewhere); s and t are whole node vectors (at least M and N entries), indexed by
+ * global row and column.  No communication.  edge_sums: row_sums[u] / col_sums[v] become the sums of `values`
+ * (A order) over row u / column v of S on all ranks (entries past M / N: 0); collective.  HNH_E_INVALID where
+ * hnhd_alg_edge_softmax is. */
+int hnhd_alg_additive_scores(hnhd_alg_t *alg, const hnhd_vec_t *s, const hnhd_vec_t *t, hnhd_vec_t *out, int mode,
+                             double alpha, int derivative);
+int hnhd_alg_edge_sums(hnhd_alg_t *alg, const hnhd_vec_t *values, hnhd_vec_t *row_sums, hnhd_vec_t *col_sums);
 
 /* CUDA-event timing on the library's compute stream: start, ..., stop -> milliseconds. */
 int hnhd_timer_start(void);
@@ -209,10 +218,19 @@ int hnhd_gat_get_weight_grad(hnhd_gat_t *g, int layer, int head, double *host);
 /* dL/d buffer 0 (this rank's rows); hnhd_gat_buffer_shape(0)'s shape */
 int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host);
 /* attention of every head (GAT::set_attention): "leaky" (the default: LeakyReLU of the scores, the
- * reference's formula) or "softmax" (their edge softmax over each row of S).  Makes the activations stale.
+ * reference's formula), "softmax" (their edge softmax over each row of S) or "additive" (below).  Makes the
+ * activations stale.
  * With "softmax" the forward pass raises HNH_E_INVALID on every rank, before any launch, where the layout has
  * no edge softmax (as hnhd_alg_edge_softmax). */
 int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind);
+/* additive attention ("additive": x_uv = LeakyReLU(a1 . h_u + a2 . h_v) with h = X W the head's projection,
+ * then the edge softmax; Velickovic et al. 2018): the attention vectors of (layer, head), features_per_head
+ * doubles each (host pointers; zero after hnhd_gat_create: uniform attention).  Makes the activations stale.
+ * "additive" is defined on the layouts where "softmax" is. */
+int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const double *a1, const double *a2);
+/* dL/d a1 and dL/d a2 of (layer, head) after hnhd_gat_backward (features_per_head doubles each, summed over all
+ * ranks; zero unless the attention is additive).  HNH_E_INVALID before the first backward pass. */
+int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2);
 void hnhd_gat_destroy(hnhd_gat_t *g);
 
 #ifdef __cplusplus
