@@ -301,11 +301,12 @@ int hnh_sddmm_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
     if (scale && ((flags & HNH_FLAG_FORCE_GENERIC) || !a16 || !table_r || (const double *)scaled_out == scale || values == scale)) {
         rc = hnh_sddmm_scaled_f64(rowStart, col_idx, values, rows, nnz, X, Y, r, flags & ~HNH_FLAG_SCALE_VALUES, nullptr, nullptr, stream);
         if (rc) return rc;
-        if (scaled_out) {
-            rc = hnh_hadamard_f64(scaled_out, scale, values, nnz, stream);
-            if (rc || !(flags & HNH_FLAG_SCALE_VALUES)) return rc;
-        }
-        return hnh_hadamard_f64(values, scale, values, nnz, stream);
+        if (scaled_out && !(flags & HNH_FLAG_SCALE_VALUES)) return hnh_hadamard_f64(scaled_out, scale, values, nnz, stream);
+        // the values take the product first: scaled_out may alias scale, so it receives a copy of them afterwards
+        rc = hnh_hadamard_f64(values, scale, values, nnz, stream);
+        if (rc || !scaled_out || scaled_out == values) return rc;
+        return check_cuda(cudaMemcpyAsync(scaled_out, values, sizeof(double) * (size_t)nnz, cudaMemcpyDeviceToDevice, st),
+                          "cudaMemcpyAsync");
     }
     const bool sv = (flags & HNH_FLAG_SCALE_VALUES) != 0;
     if ((flags & HNH_FLAG_TMA_WARP) && a16 && (r == 128 || r == 256) && !(flags & HNH_FLAG_FORCE_GENERIC)) {

@@ -111,7 +111,8 @@ __global__ void keys_from_index_kernel(int32_t *__restrict__ keys, const int64_t
 }
 
 // ---- forward ------------------------------------------------------------------------------------------------
-// one warp per piece: (max, sum of exp(x - max)) over x[perm[lo .. hi)]
+// one warp per piece: (max, sum of exp(x - max)) over x[perm[lo .. hi)].  A -inf entry (a masked edge) adds nothing:
+// exp(v - m) would be NaN while the lane's running max is still -inf.
 __global__ void piece_stats_kernel(const double *__restrict__ x, const int32_t *__restrict__ perm, const int32_t *__restrict__ row_start,
                                    const int32_t *__restrict__ piece_first, const int32_t *__restrict__ piece_row, int64_t num_pieces,
                                    double *__restrict__ piece_max, double *__restrict__ piece_sum) {
@@ -126,7 +127,7 @@ __global__ void piece_stats_kernel(const double *__restrict__ x, const int32_t *
             if (v > m) {
                 s = s * exp(m - v) + 1.0;
                 m = v;
-            } else {
+            } else if (v != -INFINITY) {
                 s += exp(v - m);
             }
         }

@@ -197,7 +197,10 @@ int hnh_edge_softmax_plan(const int32_t *keys, int64_t n, int64_t num_rows, int3
                           int32_t *piece_first, int32_t *piece_row, int64_t piece_capacity, int64_t *num_pieces,
                           void *stream);
 /* row_max[u] = max of x over row u, row_sum[u] = sum of exp(x - row_max[u]) over row u, for every row
- * (-inf and 0 for a row without entries).  piece_max / piece_sum: num_pieces doubles of workspace. */
+ * (-inf and 0 for a row without entries).  A -inf entry (a masked edge) adds nothing to row_sum, so the
+ * apply step gives it alpha = 0; a row whose entries are all -inf gets (-inf, 0) like an empty row, and
+ * the apply step gives its entries NaN, as torch.softmax does.  piece_max / piece_sum: num_pieces doubles
+ * of workspace. */
 int hnh_edge_softmax_stats_f64(const double *x, const int32_t *perm, const int32_t *row_start,
                                const int32_t *piece_first, const int32_t *piece_row, int64_t num_rows,
                                int64_t num_pieces, double *piece_max, double *piece_sum, double *row_max,

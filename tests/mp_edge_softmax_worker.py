@@ -1,7 +1,8 @@
 """Multi-process worker for the multi-rank edge-softmax tests (launched through torch.distributed.run by
 tests/test_edge_softmax_multirank_gpu.py).  Every rank builds the requested algorithm through the driver ABI, then
   * finds the (row, col) of every entry of its A-order and B-order value vectors from SDDMMs of index columns,
-  * runs edge_softmax and edge_softmax_backward on scores that are a function of (row, col),
+  * runs edge_softmax and edge_softmax_backward on scores that are a function of (row, col), with -inf on the
+    entries of `masked` when the case asks for a mask,
   * runs a softmax-attention GAT forward + backward on its rows of the global inputs,
 and writes the results -- or the errors raised -- to <outdir>/<case>_rank<r>.npz.
 
@@ -23,6 +24,13 @@ def score(r, c):
     """The edge scores of a case: up to +-1000, a function of the global coordinate."""
     r, c = np.asarray(r, np.float64), np.asarray(c, np.float64)
     return 1000.0 * np.sin(0.37 * r + 1.91 * c) * np.cos(0.11 * c)
+
+
+def masked(r, c, N):
+    """The entries a masked case scores -inf: in every fifth row each entry in the first half of the columns, in the
+    next row every entry of an even column."""
+    r, c = np.asarray(r), np.asarray(c)
+    return ((r % 5 == 0) & (c < N // 2)) | ((r % 5 == 1) & (c % 2 == 0))
 
 
 def upstream(r, c):
@@ -88,7 +96,10 @@ def main():
                 r, cc = coords(alg, mode)
                 like = alg.like_S_values if mode == "A" else alg.like_ST_values
                 v, g = like(0.0), like(0.0)
-                v.from_host(score(r, cc))
+                x = score(r, cc)
+                if case.get("mask"):
+                    x[masked(r, cc, N)] = -np.inf
+                v.from_host(x)
                 alg.edge_softmax(v, mode)
                 a = v.to_host()
                 g.from_host(upstream(r, cc))
@@ -96,6 +107,10 @@ def main():
                 out.update({f"{mode}_rows": r, f"{mode}_cols": cc, f"{mode}_alpha": a, f"{mode}_dx": g.to_host()})
         except RuntimeError as e:
             out["softmax_error"] = str(e)
+        if case.get("mask"):  # the masked case checks the edge softmax only
+            np.savez(os.path.join(outdir, f"{name}_rank{rank}.npz"), **out)
+            del alg, S
+            continue
         # softmax-attention GAT: this rank's rows of the global input, the global weights and output gradient
         net = D.GAT(alg, layers, case["alpha"], attention="softmax")
         topB, _, nrB, _ = alg.submatrices("B")[0]

@@ -19,7 +19,7 @@ import torch
 from oracle import hnh_oracle as orc
 from tests import gat_backward_oracle as gbo
 from tests import gat_softmax_oracle as gso
-from tests.mp_edge_softmax_worker import score, upstream
+from tests.mp_edge_softmax_worker import masked, score, upstream
 from tests.mp_gat_backward_worker import output_grad
 from tests.mp_util import ROOT, free_port
 from tests.mp_worker import gat_inputs
@@ -121,3 +121,34 @@ def test_layouts_without_a_row_softmax_are_rejected_on_every_rank():
                 assert key in d, (c["name"], r, key)
                 msg = str(d[key])
                 assert "code -1" in msg and op + ": not defined for" in msg and "p = 2" in msg, (c["name"], r, msg)
+
+
+def test_edge_softmax_masked_multirank():
+    """-inf scores at p = 2 on rows of about 70 entries: every entry of some rows in the first half of the columns, so
+    that a rank whose entries of a row are all masked has a local row maximum of -inf and its share of the row sum must
+    rescale to 0, not NaN; and every other entry of other rows, so that -inf is the first entry some lanes see."""
+    c = dict(case("15d_fusion1", 1, npr=100), name="15d_fusion1_c1_masked", mask=True)
+    ranks = run(2, [c])[c["name"]]
+    N = 1 << c["logM"]
+    rows, cols, _ = orc.er_tuples(c["logM"], c["npr"], c["seed"])
+    ri, ci = (t.numpy() for t in gbo.edges(rows, cols, N))
+    x = score(ri, ci)
+    x[masked(ri, ci, N)] = -np.inf
+    alpha = gso.edge_softmax_np(x, ri, N)  # NaN on the rows masked throughout, as torch.softmax
+    dx = gso.edge_softmax_backward_np(alpha, upstream(ri, ci), ri, N)
+    finite_rows = np.unique(ri[np.isfinite(x)])
+    local_masked = 0
+    for mode in ("A", "B"):
+        for r, d in enumerate(ranks):
+            assert "softmax_error" not in d, (r, str(d.get("softmax_error")))
+            at = np.searchsorted(ri * N + ci, d[f"{mode}_rows"] * N + d[f"{mode}_cols"])
+            for got, want in ((d[f"{mode}_alpha"], alpha[at]), (d[f"{mode}_dx"], dx[at])):
+                nan = np.isnan(want)
+                assert np.array_equal(np.isnan(got), nan), (mode, r)
+                assert rel_err(got[~nan], want[~nan]) < 1e-13, (mode, r)
+            assert np.all(d[f"{mode}_alpha"][np.isneginf(x[at]) & np.isin(d[f"{mode}_rows"], finite_rows)] == 0), (mode, r)
+            # rows this rank holds only masked entries of, while another rank holds finite ones
+            mine = np.unique(d[f"{mode}_rows"])
+            live = np.unique(d[f"{mode}_rows"][np.isfinite(x[at])])
+            local_masked += len(np.intersect1d(np.setdiff1d(mine, live), finite_rows))
+    assert local_masked > 0
