@@ -59,6 +59,10 @@ ABI = {
     "hnh_gat_node_scalars_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I64, _P]),
     "hnh_gat_edge_scores_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, C.c_double, C.c_int, _P]),
     "hnh_gat_rank2_update_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I64, _P]),
+    "hnh_gatv2_scores_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, C.c_int, C.c_double, _P, _P]),
+    "hnh_gatv2_grad_workspace_bytes": (C.c_int64, [_I64, C.c_int]),
+    "hnh_gatv2_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, C.c_int, C.c_double, _P, _I64, _P, _P,
+                                     C.c_size_t, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -209,6 +213,8 @@ ABI.update({
     "hnhd_alg_edge_softmax_backward": (C.c_int, [_P, _P, _P, C.c_int]),
     "hnhd_alg_additive_scores": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_double, C.c_int]),
     "hnhd_alg_edge_sums": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_alg_gatv2_scores": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double]),
+    "hnhd_alg_gatv2_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_double]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),

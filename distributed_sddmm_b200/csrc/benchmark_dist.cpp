@@ -39,8 +39,9 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
     std::unique_ptr<GAT> gnn;
     DenseMatrix gat_output_grad;
     const bool gat_app = app == "gat" || app == "gat_train" || app == "gat_softmax" || app == "gat_softmax_train" ||
-                         app == "gat_additive" || app == "gat_additive_train";
-    const bool gat_train = app == "gat_train" || app == "gat_softmax_train" || app == "gat_additive_train";
+                         app == "gat_additive" || app == "gat_additive_train" || app == "gat_v2" || app == "gat_v2_train";
+    const bool gat_train =
+        app == "gat_train" || app == "gat_softmax_train" || app == "gat_additive_train" || app == "gat_v2_train";
     if (gat_app) {
         // the three layers of the reference's GAT benchmark: (input width, width per head, heads)
         vector<GATLayer> layers{GATLayer(256, 256, 4), GATLayer(1024, 256, 4), GATLayer(1024, 256, 6)};
@@ -55,7 +56,12 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
             d_ops->check_full_rows("GAT additive attention");
             gnn->set_attention("additive");
         }
-        // gat_train / gat_softmax_train / gat_additive_train: forwardPass() then backwardPass(dL/d output = ones) per call
+        // gat_v2*: GATv2 attention (the attention vectors stay zero, as the weights do)
+        if (app == "gat_v2" || app == "gat_v2_train") {
+            d_ops->check_full_rows("GAT GATv2 attention");
+            gnn->set_attention("gatv2");
+        }
+        // gat_train / gat_softmax_train / gat_additive_train / gat_v2_train: forwardPass() then backwardPass(dL/d output = ones) per call
         if (gat_train) {
             gnn->check_backward_supported();
             gat_output_grad = DenseMatrix::Constant(gnn->buffers.back().rows(), gnn->buffers.back().cols(), 1.0);
@@ -64,7 +70,8 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
         d_als.reset(new Distributed_ALS(d_ops.get(), true));
     } else if (app != "vanilla") {
         throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\", \"gat\", \"gat_train\", \"gat_softmax\", "
-                                        "\"gat_softmax_train\", \"gat_additive\" or \"gat_additive_train\"");
+                                        "\"gat_softmax_train\", \"gat_additive\", \"gat_additive_train\", \"gat_v2\" or "
+                                        "\"gat_v2_train\"");
     }
 
     DenseMatrix A = d_ops->like_A_matrix(0.001);

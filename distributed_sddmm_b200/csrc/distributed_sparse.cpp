@@ -438,6 +438,177 @@ void Distributed_Sparse::edgeSums(const VectorXd &values, VectorXd &row_sums, Ve
     allreduce_rows(col_sums.data(), N, false);
 }
 
+// ---- GATv2 attention -----------------------------------------------------------------------------------------
+namespace {
+// dst[:, dst_col0 .. + cols) = src[:, src_col0 .. + cols) for matrices of the same height, on the compute stream
+void copy_cols(DenseMatrix &dst, int64_t dst_col0, const DenseMatrix &src, int64_t src_col0, int64_t cols) {
+    if (dst.rows() == 0 || cols == 0) return;
+    const size_t d = sizeof(double);
+    hnh::cuda_check(cudaMemcpy2DAsync(dst.data() + dst_col0, d * (size_t)dst.cols(), src.data() + src_col0, d * (size_t)src.cols(),
+                                      d * (size_t)cols, (size_t)dst.rows(), cudaMemcpyDeviceToDevice, Runtime::get().compute_stream()),
+                    "gatv2 column copy");
+}
+}  // namespace
+
+void Distributed_Sparse::gatv2_pass(KernelMode order, DenseMatrix &localA, DenseMatrix &localB, DenseMatrix *dA, DenseMatrix *dB,
+                                    const Gatv2Kernel &kernel) {
+    SpmatLocal &m = *values_matrix(*this, order);
+    const bool is_ST = &m == ST.get();
+    const int64_t r = localA.cols();
+    // block b with its entries, or null when it has none
+    auto block = [&](int b) -> CSRLocal * {
+        const int64_t nb = (int64_t)m.blockStarts[(size_t)b + 1] - (int64_t)m.blockStarts[(size_t)b];
+        if (nb == 0) return nullptr;
+        CSRLocal *blk = m.csr_blocks[(size_t)b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, "gatv2: block " + to_string(b) + " does not match its value range");
+        return blk;
+    };
+    auto run = [&](int b, CSRLocal &blk, const double *R, int64_t ldr, int64_t R_rows, const double *Y, int64_t Y_rows, double *dR,
+                   int64_t lddr) {
+        if (blk.rows > R_rows || blk.cols > Y_rows)
+            throw hnh::Error(HNH_E_INVALID, "gatv2: block " + to_string(b) + " (" + to_string(blk.rows) + " x " + to_string(blk.cols) +
+                                                ") does not fit its dense operands (" + to_string(R_rows) + " and " +
+                                                to_string(Y_rows) + " rows)");
+        kernel(b, blk, R, ldr, Y, r, dR, lddr);
+    };
+    if (p == 1) {
+        for (int b = 0; b + 1 < (int)m.blockStarts.size(); b++) {
+            CSRLocal *blk = block(b);
+            if (blk == nullptr) continue;
+            // S stores its rows as rows, ST as columns; a transposed block swaps the two
+            const bool rows_are_A = is_ST == blk->transpose;
+            DenseMatrix &Rm = rows_are_A ? localA : localB, &Ym = rows_are_A ? localB : localA;
+            DenseMatrix *dR = rows_are_A ? dA : dB;
+            run(b, *blk, Rm.data(), r, Rm.rows(), Ym.data(), Ym.rows(), dR ? dR->data() : nullptr, r);
+        }
+        return;
+    }
+    // check_full_rows has passed: 1.5D dense shift, fusion 1 at any c or fusion 2 at c = 1.  Its blocks are stored
+    // transposed exactly under fusion 1 (Sparse15D_Dense_Shift's constructor).
+    Sparse15D_Dense_Shift &ds = dynamic_cast<Sparse15D_Dense_Shift &>(*this);
+    const bool fusion1 = ds.fusionApproach == 1;
+    const bool rows_are_A = is_ST == fusion1;
+    DenseMatrix &rowSide = rows_are_A ? localA : localB, &gathered = rows_are_A ? localB : localA;
+    DenseMatrix *dRow = rows_are_A ? dA : dB;
+    if (!fusion1) {
+        // local kernel fusion, c = 1: the stored-row side (and its gradient) stays, the gathered side rides read-only
+        if (c != 1) throw hnh::Error(HNH_E_INVALID, "gatv2: local kernel fusion at c > 1");
+        ring_dense(gathered, grid->col_world, true, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
+            const int b = ds.block_at(step);
+            if (CSRLocal *blk = block(b))
+                run(b, *blk, rowSide.data(), r, rowSide.rows(), shard.data(), shard.rows(), dRow ? dRow->data() : nullptr, r);
+        });
+        return;
+    }
+    // replication reuse: the gathered side is stationary, all-gathered over the layer (row_world); the stored-row side
+    // rides the column ring
+    DenseMatrix replicated;
+    DenseMatrix *fixed = &gathered;
+    if (c > 1) {
+        Runtime &rt = Runtime::get();
+        replicated.resize(gathered.rows() * c, r);
+        rt.chain(compute(), comm());
+        region_begin("Replication Time", comm());
+        grid->row_world->allgather(gathered.data(), replicated.data(), sizeof(double) * (size_t)gathered.size(), comm());
+        region_end("Replication Time", comm());
+        rt.chain(comm(), compute());
+        fixed = &replicated;
+    }
+    if (dRow == nullptr) {
+        ring_dense(rowSide, grid->col_world, true, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
+            const int b = ds.block_at(step);
+            if (CSRLocal *blk = block(b)) run(b, *blk, shard.data(), r, shard.rows(), fixed->data(), fixed->rows(), nullptr, r);
+        });
+        return;
+    }
+    // the gradient has to ride with the rows it belongs to: [row side | gradient] travels as one 2r-wide matrix on the
+    // output-riding ring (kernel and shift alternate) and is back home after the last shift
+    DenseMatrix packed(rowSide.rows(), 2 * r);
+    copy_cols(packed, 0, rowSide, 0, r);
+    copy_cols(packed, r, *dRow, 0, r);
+    ring_dense(packed, grid->col_world, false, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
+        const int b = ds.block_at(step);
+        if (CSRLocal *blk = block(b))
+            run(b, *blk, shard.data(), 2 * r, shard.rows(), fixed->data(), fixed->rows(), shard.data() + r, 2 * r);
+    });
+    copy_cols(*dRow, 0, packed, r, r);
+}
+
+namespace {
+void check_gatv2_operands(const Distributed_Sparse &d, const char *who, const DenseMatrix &A, const DenseMatrix &B, const VectorXd &a) {
+    const int64_t r = a.size();
+    if (r < 1 || r > INT32_MAX || A.cols() != r || B.cols() != r)
+        throw hnh::Error(HNH_E_INVALID, string(who) + ": the operands are " + to_string(A.cols()) + " and " + to_string(B.cols()) +
+                                            " wide, the attention vector has " + to_string(r) + " entries");
+    if (A.rows() != d.localArows || B.rows() != d.localBrows)
+        throw hnh::Error(HNH_E_INVALID, string(who) + ": the operands have " + to_string(A.rows()) + " and " + to_string(B.rows()) +
+                                            " rows; like_A_matrix / like_B_matrix have " + to_string(d.localArows) + " and " +
+                                            to_string(d.localBrows));
+}
+int64_t order_size(Distributed_Sparse &d, const char *who, KernelMode order) {
+    if (order != k_sddmmA && order != k_sddmmB)
+        throw hnh::Error(HNH_E_INVALID, string(who) + ": the value order must be k_sddmmA or k_sddmmB");
+    return order == k_sddmmA ? d.num_S_values() : d.num_ST_values();
+}
+}  // namespace
+
+void Distributed_Sparse::gatv2Scores(DenseMatrix &localA, DenseMatrix &localB, const VectorXd &a, VectorXd &out, KernelMode order,
+                                     double alpha) {
+    check_full_rows("gatv2Scores");
+    check_gatv2_operands(*this, "gatv2Scores", localA, localB, a);
+    const int64_t want = order_size(*this, "gatv2Scores", order);
+    if (out.size() != want)
+        throw hnh::Error(HNH_E_INVALID, "gatv2Scores: the value vector has " + to_string(out.size()) + " entries, this order " + to_string(want));
+    SpmatLocal &m = *values_matrix(*this, order);
+    const int r = (int)a.size();
+    gatv2_pass(order, localA, localB, nullptr, nullptr,
+               [&](int b, CSRLocal &blk, const double *R, int64_t ldr, const double *Y, int64_t ldy, double *, int64_t) {
+                   CSRHandle *h = blk.getActive();
+                   hnh::abi_check(hnh_gatv2_scores_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords, R, ldr, Y, ldy,
+                                                       a.data(), r, alpha, out.data() + (int64_t)m.blockStarts[(size_t)b], compute()),
+                                  "gatv2_scores");
+               });
+}
+
+void Distributed_Sparse::gatv2Backward(DenseMatrix &localA, DenseMatrix &localB, const VectorXd &a, const VectorXd &grad_A,
+                                       const VectorXd &grad_B, DenseMatrix &dA, DenseMatrix &dB, VectorXd &da, double alpha) {
+    check_full_rows("gatv2Backward");
+    check_gatv2_operands(*this, "gatv2Backward", localA, localB, a);
+    check_gatv2_operands(*this, "gatv2Backward (gradients)", dA, dB, a);
+    if (grad_A.size() != num_S_values() || grad_B.size() != num_ST_values())
+        throw hnh::Error(HNH_E_INVALID, "gatv2Backward: the gradients have " + to_string(grad_A.size()) + " and " +
+                                            to_string(grad_B.size()) + " entries, the A and B orders " + to_string(num_S_values()) +
+                                            " and " + to_string(num_ST_values()));
+    const int r = (int)a.size();
+    VectorXd da_local = VectorXd::Constant(r, 0.0);
+    // the da partials of the A-order blocks (one kernel at a time uses it)
+    int64_t most_rows = 0;
+    for (CSRLocal *blk : values_matrix(*this, k_sddmmA)->csr_blocks)
+        if (blk) most_rows = std::max(most_rows, blk->rows);
+    const int64_t ws_bytes = hnh_gatv2_grad_workspace_bytes(most_rows, r);
+    if (ws_bytes < 0) hnh::abi_check((int)ws_bytes, "gatv2_grad_workspace_bytes");
+    VectorXd workspace(std::max<int64_t>((ws_bytes + 7) / 8, 1));
+    for (KernelMode order : {k_sddmmA, k_sddmmB}) {
+        SpmatLocal &m = *values_matrix(*this, order);
+        const VectorXd &g = order == k_sddmmA ? grad_A : grad_B;
+        // da counts every stored entry once over all ranks: from the A order only
+        const bool with_da = order == k_sddmmA;
+        gatv2_pass(order, localA, localB, &dA, &dB,
+                   [&](int b, CSRLocal &blk, const double *R, int64_t ldr, const double *Y, int64_t ldy, double *dR, int64_t lddr) {
+                       const size_t ws = with_da ? (size_t)workspace.size() * sizeof(double) : 0;
+                       CSRHandle *h = blk.getActive();
+                       hnh::abi_check(hnh_gatv2_grad_f64(h->rowStart.data(), h->col_idx.data(), g.data() + (int64_t)m.blockStarts[(size_t)b],
+                                                         blk.rows, blk.num_coords, R, ldr, Y, ldy, a.data(), r, alpha, dR, lddr,
+                                                         with_da ? da_local.data() : nullptr, with_da ? workspace.data() : nullptr, ws,
+                                                         compute()),
+                                      "gatv2_grad");
+                   });
+    }
+    allreduce_rows(da_local.data(), r, false);
+    da = std::move(da_local);
+}
+
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {
     if (peer_ring_broken_ || !hnh::PeerRing::enabled() || world->size() < 2) return nullptr;
     auto key = std::make_pair(world.get(), bytes);

@@ -349,6 +349,22 @@ int hnhd_alg_edge_sums(hnhd_alg_t *a, const hnhd_vec_t *values, hnhd_vec_t *row_
     });
 }
 
+int hnhd_alg_gatv2_scores(hnhd_alg_t *a, hnhd_dense_t *A, hnhd_dense_t *B, const hnhd_vec_t *va, hnhd_vec_t *out, int mode,
+                          double alpha) {
+    return guarded([&] {
+        if (!a || !A || !B || !va || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_gatv2_scores: null argument");
+        a->alg->gatv2Scores(A->m, B->m, va->v, out->v, value_order(mode), alpha);
+    });
+}
+int hnhd_alg_gatv2_backward(hnhd_alg_t *a, hnhd_dense_t *A, hnhd_dense_t *B, const hnhd_vec_t *va, const hnhd_vec_t *grad_A,
+                            const hnhd_vec_t *grad_B, hnhd_dense_t *dA, hnhd_dense_t *dB, hnhd_vec_t *da, double alpha) {
+    return guarded([&] {
+        if (!a || !A || !B || !va || !grad_A || !grad_B || !dA || !dB || !da)
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_gatv2_backward: null argument");
+        a->alg->gatv2Backward(A->m, B->m, va->v, grad_A->v, grad_B->v, dA->m, dB->m, da->v, alpha);
+    });
+}
+
 int hnhd_timer_start(void) {
     return guarded([] {
         if (!g_t0) {

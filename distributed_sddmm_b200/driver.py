@@ -275,6 +275,19 @@ class Algorithm:
         """Collective: the row and column sums of an A-order value vector over all ranks (Distributed_Sparse::edgeSums)."""
         check(lib().hnhd_alg_edge_sums(self.h, values.h, row_sums.h, col_sums.h), "edge_sums")
 
+    def gatv2_scores(self, A: Dense, B: Dense, a: Vec, out: Vec, mode: str = "A", alpha: float = 0.2):
+        """Collective: out (a value vector of `mode`) = sum_k a_k LeakyReLU(A[u, k] + B[v, k]) per stored entry (u, v)
+        of S, with A and B this rank's A- and B-shaped operands (Distributed_Sparse::gatv2Scores)."""
+        check(lib().hnhd_alg_gatv2_scores(self.h, A.h, B.h, a.h, out.h, _value_order(mode), float(alpha)), "gatv2_scores")
+
+    def gatv2_backward(self, A: Dense, B: Dense, a: Vec, grad_A: Vec, grad_B: Vec, dA: Dense, dB: Dense, da: Vec,
+                       alpha: float = 0.2):
+        """Collective: given dL/d scores in both value orders, dA += the gradient of the A side, dB += that of the B side
+        (dA and dB may be the same Dense), and da (resized to len(a)) = dL/da summed over all ranks
+        (Distributed_Sparse::gatv2Backward)."""
+        check(lib().hnhd_alg_gatv2_backward(self.h, A.h, B.h, a.h, grad_A.h, grad_B.h, dA.h, dB.h, da.h, float(alpha)),
+              "gatv2_backward")
+
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
 
@@ -368,13 +381,14 @@ class GAT:
     features_per_head, num_heads), ...].  attention: "leaky" (LeakyReLU of the scores, the reference's formula),
     "softmax" (their softmax over each node's neighbours) or "additive" (the softmax of LeakyReLU(a1 . h_u + a2 . h_v),
     Velickovic et al. 2018; a1 and a2 per head through set_attention_vectors, zero by default).  The algorithm object
-    must outlive this one."""
+    must outlive this one.  "gatv2" is GATv2 attention (Brody, Alon and Yahav 2022, shared weights): the softmax of
+    a1 . LeakyReLU(h_u + h_v), with a1 set through set_attention_vectors (a2 is not read)."""
 
-    ATTENTIONS = ("leaky", "softmax", "additive")
+    ATTENTIONS = ("leaky", "softmax", "additive", "gatv2")
 
     def __init__(self, alg: Algorithm, layers, leaky_relu_alpha: float = 0.2, attention: str = "leaky"):
         if attention not in self.ATTENTIONS:
-            raise ValueError(f'attention must be "leaky", "softmax" or "additive", not {attention!r}')
+            raise ValueError(f'attention must be "leaky", "softmax", "additive" or "gatv2", not {attention!r}')
         self.alg = alg
         self.layers = [tuple(int(x) for x in l) for l in layers]
         flat = (C.c_int * (3 * len(self.layers)))(*[x for l in self.layers for x in l])
@@ -383,7 +397,7 @@ class GAT:
         self.set_attention(attention)
 
     def set_attention(self, kind: str):
-        """"leaky", "softmax" or "additive"; the next backward pass needs a forward pass first."""
+        """"leaky", "softmax", "additive" or "gatv2"; the next backward pass needs a forward pass first."""
         check(lib().hnhd_gat_set_attention(self.h, kind.encode()), "gat_set_attention")
         self.attention = kind
 
@@ -424,8 +438,8 @@ class GAT:
         check(lib().hnhd_gat_backward(self.h, g.ctypes.data), "gat_backward")
 
     def set_attention_vectors(self, layer: int, head: int, a1, a2):
-        """The additive attention vectors of (layer, head), features_per_head long each; the next backward pass needs
-        a forward pass first."""
+        """The attention vectors of (layer, head), features_per_head long each (additive attention reads both, GATv2
+        attention a1 only); the next backward pass needs a forward pass first."""
         fph = self.layers[layer][1]
         a1, a2 = (np.ascontiguousarray(a, dtype=np.float64) for a in (a1, a2))
         assert a1.shape == (fph,) and a2.shape == (fph,), (a1.shape, a2.shape, fph)
@@ -433,8 +447,8 @@ class GAT:
               "gat_set_attention_vectors")
 
     def attention_grads(self, layer: int, head: int):
-        """(dL/d a1, dL/d a2) of (layer, head) after a backward pass, summed over all ranks (zero unless the
-        attention is additive)."""
+        """(dL/d a1, dL/d a2) of (layer, head) after a backward pass, summed over all ranks (zero for the vectors the
+        attention kind does not read)."""
         fph = self.layers[layer][1]
         da1, da2 = np.empty(fph), np.empty(fph)
         check(lib().hnhd_gat_get_attention_grads(self.h, layer, head, da1.ctypes.data, da2.ctypes.data),

@@ -16,6 +16,7 @@
 //     keys and JSON schema are kept (distributed_sparse.h:131-179,205-261).
 #pragma once
 #include <cassert>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -178,6 +179,26 @@ public:
     // edgeSoftmax's row grouping.  Defined where check_full_rows passes; HNH_E_INVALID on every rank elsewhere.
     void additiveScores(const VectorXd &s, const VectorXd &t, VectorXd &out, KernelMode order, double alpha, bool derivative);
     void edgeSums(const VectorXd &values, VectorXd &row_sums, VectorXd &col_sums);
+
+    // ---- GATv2 attention (GAT::set_attention("gatv2")) --------------------------------------------------------
+    // With sigma = LeakyReLU(., alpha), u = S-row and v = S-column, localA the A-shaped operand (rows u) and
+    // localB the B-shaped one (rows v), both r = a.size() wide, as in sddmmA / sddmmB:
+    // gatv2Scores: out (a value vector of `order`: k_sddmmA for like_S_values, k_sddmmB for like_ST_values) becomes
+    //     x_uv = sum_k a_k sigma(localA[u, k] + localB[v, k]) for every stored (u, v) of S (overwritten).
+    // gatv2Backward: with grad_A / grad_B = dL/dx in the A and B orders,
+    //     dA[u] += a o sum_v g_uv sigma'(localA[u] + localB[v]),  dB[v] += a o sum_u g_uv sigma'(...),
+    //     da = sum_uv g_uv sigma(localA[u] + localB[v]) over all ranks (overwritten; resized to r; the same on
+    //     every rank).  sigma'(z) = 1 where z > 0, alpha elsewhere.  dA and dB may be the same matrix.
+    // Each gradient comes from the order whose CSR blocks hold that side as stored rows, through a kernel that owns
+    // those rows: no scatter, no atomic.  Where the operands travel: p = 1, none; 1.5D dense shift with local kernel
+    // fusion (c = 1): the stored-row side stays, the gathered side rides read-only; with replication reuse (any c):
+    // the gathered side is replicated over the layer and the stored-row side rides -- for gatv2Backward together
+    // with its gradient, as one 2r-wide matrix that ends at home.  Collective; defined where check_full_rows
+    // passes, HNH_E_INVALID on every rank elsewhere.
+    void gatv2Scores(DenseMatrix &localA, DenseMatrix &localB, const VectorXd &a, VectorXd &out, KernelMode order,
+                     double alpha);
+    void gatv2Backward(DenseMatrix &localA, DenseMatrix &localB, const VectorXd &a, const VectorXd &grad_A,
+                       const VectorXd &grad_B, DenseMatrix &dA, DenseMatrix &dB, VectorXd &da, double alpha);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 
@@ -214,6 +235,14 @@ protected:
     template <class Body>
     void ring_dense(DenseMatrix &home, std::shared_ptr<hnh::Comm> world_ptr, bool riding_is_input, const string &shift_key,
                     const string &compute_key, Body body);
+
+    // One GATv2 pass over the CSR blocks of a value order (gatv2Scores, gatv2Backward): kernel(block, blk, R, ldr,
+    // Y, ldy, dR, lddr) runs once per block with entries, with R the stored-row side, Y the gathered side and dR
+    // the stored-row side's gradient (dA or dB; null when both are null), each at the rank and ring step where the
+    // block meets them.
+    using Gatv2Kernel = std::function<void(int, CSRLocal &, const double *, int64_t, const double *, int64_t, double *, int64_t)>;
+    void gatv2_pass(KernelMode order, DenseMatrix &localA, DenseMatrix &localB, DenseMatrix *dA, DenseMatrix *dB,
+                    const Gatv2Kernel &kernel);
 };
 
 // ------------------------------------------------------------------ ring driver ----------

@@ -50,10 +50,22 @@
 // Per head: forward 1 SpMM pass, backward 1 SDDMM and 1 SpMM pass, against 1 + 1 and 4 + 3 for the dot-product
 // attention.  The forward stores nothing extra: P, s, t and alpha are recomputed.
 //
+// GATv2 attention (set_attention("gatv2"), Brody, Alon and Yahav 2022; the shared-weights form) applies the
+// nonlinearity before the attention vector, so that a node's ranking of its neighbours depends on the node.  With a
+// the head's slice of layer.a1 (a2 is not read; its gradient stays zero) and sigma = LeakyReLU(., leaky_relu_alpha):
+//     x_uv  = sum_k a_k sigma(P_uk + P_vk)                     (Distributed_Sparse::gatv2Scores, A order)
+//     alpha = edge softmax of x, Z = S_alpha P, X_out[:, head window] = ReLU(Z)
+// Backward, with z_uv = P_u + P_v:
+//     dalpha = S o (dZ P^T), de = edgeSoftmaxBackward(alpha, dalpha)         both orders
+//     dP     = S_alpha^T dZ + sum_v de_uv a o sigma'(z_uv) (rows u) + sum_u de_uv a o sigma'(z_uv) (rows v)
+//     da     = sum_uv de_uv sigma(z_uv), summed over all ranks (layer.a1Grads)  (Distributed_Sparse::gatv2Backward)
+// Per head: forward 1 score pass + 1 SpMM; backward 2 score passes (alpha recomputed in both orders), 2 SDDMMs,
+// 2 gradient passes and 1 SpMM -- 7 sparse passes, as for the dot-product attention.  The forward stores nothing extra.
+//
 // The forward pass is the GAT formula only where every rank holds full-width rows and the A and B layouts coincide:
 // p = 1 (any algorithm), 1.5D dense shift with replication reuse (fusion 1) at any c, and with local kernel fusion
-// (fusion 2) at c = 1 (Distributed_Sparse::check_full_rows).  Only there are the backward pass and softmax and additive
-// attention defined; elsewhere they throw HNH_E_INVALID on every rank.
+// (fusion 2) at c = 1 (Distributed_Sparse::check_full_rows).  Only there are the backward pass and softmax, additive
+// and GATv2 attention defined; elsewhere they throw HNH_E_INVALID on every rank.
 #pragma once
 #include <string>
 #include <vector>
@@ -72,11 +84,11 @@ public:
     vector<DenseMatrix> wGrads; // dL/d wMats[j] after GAT::backwardPass (empty before the first one); same on every rank
     // attention vectors (declared by the reference, unused by its forward pass): num_heads * features_per_head
     // doubles each, head j's at [j * features_per_head, (j + 1) * features_per_head).  GAT allocates them as zeros;
-    // only additive attention reads them.
+    // additive attention reads both, GATv2 attention a1 only.
     VectorXd a1;
     VectorXd a2;
-    VectorXd a1Grads;  // dL/d a1, dL/d a2 after GAT::backwardPass (empty before the first one; zero unless the
-    VectorXd a2Grads;  // attention is additive); same on every rank
+    VectorXd a1Grads;  // dL/d a1, dL/d a2 after GAT::backwardPass (empty before the first one; zero for the attention
+    VectorXd a2Grads;  // kinds that do not read them); same on every rank
 
     GATLayer(int in_width, int head_width, int heads)
         : input_features(in_width), features_per_head(head_width), num_heads(heads) {}
@@ -125,7 +137,10 @@ public:
         d_ops->de_shift(&neighbours, nullptr, k_spmmA);
 
         VectorXd scores = d_ops->like_S_values(1.0);
-        if (additive_) {
+        if (gatv2_) {
+            d_ops->gatv2Scores(projected, neighbours, head_vector(layer.a1, layer, j), scores, k_sddmmA, leaky_relu_alpha);
+            d_ops->edgeSoftmax(scores, k_sddmmA);
+        } else if (additive_) {
             VectorXd s, t;
             node_scalars(layer, j, projected, s, t);
             d_ops->additiveScores(s, t, scores, k_sddmmA, leaky_relu_alpha, false);
@@ -138,15 +153,16 @@ public:
         }
 
         projected.setZero();  // becomes the SpMM accumulator
-        // replication reuse: the SDDMM pass has replicated the stationary operand, except with additive attention,
-        // which has no SDDMM pass
-        d_ops->algorithm(projected, neighbours, scores, nullptr, k_spmmA, additive_);
+        // replication reuse: the SDDMM pass has replicated the stationary operand, except with additive and GATv2
+        // attention, which have no SDDMM pass
+        d_ops->algorithm(projected, neighbours, scores, nullptr, k_spmmA, additive_ || gatv2_);
         output.setMiddleColsRelu((int64_t)j * projected.cols(), projected);
     }
 
     void forwardPass() {
         if (softmax_) d_ops->check_full_rows("GAT softmax attention");
         if (additive_) d_ops->check_full_rows("GAT additive attention");
+        if (gatv2_) d_ops->check_full_rows("GAT GATv2 attention");
         for (size_t i = 0; i < layers.size(); i++)
             for (int j = 0; j < layers[i].num_heads; j++) computeSelfAttentionHead((int)i, j);
         activations_current = true;
@@ -162,16 +178,18 @@ public:
     // file).  Decided from global quantities only, so every rank throws together and no collective is left waiting.
     void check_backward_supported() const { d_ops->check_full_rows("GAT::backwardPass"); }
 
-    // "leaky" (the reference's attention, the default), "softmax" or "additive" (see the top of this file).  Changing
-    // it makes the activations stale.
+    // "leaky" (the reference's attention, the default), "softmax", "additive" or "gatv2" (see the top of this file).
+    // Changing it makes the activations stale.
     const string &attention() const { return attention_; }
     void set_attention(const string &kind) {
-        if (kind != "leaky" && kind != "softmax" && kind != "additive")
-            throw hnh::Error(HNH_E_INVALID, "GAT: attention must be \"leaky\", \"softmax\" or \"additive\", not \"" + kind + "\"");
+        if (kind != "leaky" && kind != "softmax" && kind != "additive" && kind != "gatv2")
+            throw hnh::Error(HNH_E_INVALID, "GAT: attention must be \"leaky\", \"softmax\", \"additive\" or \"gatv2\", not \"" +
+                                                kind + "\"");
         if (kind != attention_) activations_current = false;
         attention_ = kind;
         softmax_ = kind == "softmax";
         additive_ = kind == "additive";
+        gatv2_ = kind == "gatv2";
     }
 
     // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d wMats in layers[i].wGrads and dL/d a1 / a2
@@ -193,7 +211,9 @@ public:
                 for (const DenseMatrix &w : layer.wMats) layer.wGrads.emplace_back(w.rows(), w.cols());
             }
         for (GATLayer &layer : layers)
-            if (layer.a1Grads.size() != layer.a1.size() || !additive_) {  // the other kinds do not read a1 / a2
+            // additive attention writes every entry of both, GATv2 attention every entry of a1Grads; a2Grads and the
+            // kinds that do not read the vectors leave zeros
+            if (layer.a1Grads.size() != layer.a1.size() || !additive_) {
                 layer.a1Grads = VectorXd::Constant(layer.a1.size(), 0.0);
                 layer.a2Grads = VectorXd::Constant(layer.a2.size(), 0.0);
             }
@@ -213,6 +233,7 @@ public:
     // writes) the head's share of dL/d buffers[i] into dX
     void backwardHead(int i, int j, const DenseMatrix &G, DenseMatrix &dX, bool accumulate) {
         if (additive_) return backwardHeadAdditive(i, j, G, dX, accumulate);
+        if (gatv2_) return backwardHeadGatv2(i, j, G, dX, accumulate);
         GATLayer &layer = layers.at((size_t)i);
         const DenseMatrix &input = buffers[(size_t)i], &output = buffers[(size_t)i + 1];
         const DenseMatrix &W = layer.wMats.at((size_t)j);
@@ -326,10 +347,63 @@ public:
         dX.setTimesTranspose(dP, W, accumulate);
     }
 
+    // backwardHead with GATv2 attention (see the top of this file)
+    void backwardHeadGatv2(int i, int j, const DenseMatrix &G, DenseMatrix &dX, bool accumulate) {
+        GATLayer &layer = layers.at((size_t)i);
+        const DenseMatrix &input = buffers[(size_t)i], &output = buffers[(size_t)i + 1];
+        const DenseMatrix &W = layer.wMats.at((size_t)j);
+        d_ops->setRValue(layer.features_per_head);
+        DenseMatrix P = input * W;
+        const VectorXd a = head_vector(layer.a1, layer, j);
+
+        // alpha in both orders, each from its own score pass
+        VectorXd alpha_A = d_ops->like_S_values(0.0), alpha_B = d_ops->like_ST_values(0.0);
+        d_ops->gatv2Scores(P, P, a, alpha_A, k_sddmmA, leaky_relu_alpha);
+        d_ops->edgeSoftmax(alpha_A, k_sddmmA);
+        d_ops->gatv2Scores(P, P, a, alpha_B, k_sddmmB, leaky_relu_alpha);
+        d_ops->edgeSoftmax(alpha_B, k_sddmmB);
+
+        // de = edgeSoftmaxBackward(alpha, S o (dZ P^T)) in both orders
+        DenseMatrix dZ(P.rows(), P.cols());
+        dZ.setMiddleColsReluGrad(G, output, (int64_t)j * layer.features_per_head);
+        VectorXd ones_A = d_ops->like_S_values(1.0), ones_B = d_ops->like_ST_values(1.0);
+        VectorXd de_A = d_ops->like_S_values(0.0), de_B = d_ops->like_ST_values(0.0);
+        d_ops->sddmmA(dZ, P, ones_A, de_A);
+        d_ops->sddmmB(dZ, P, ones_B, de_B);
+        d_ops->edgeSoftmaxBackward(alpha_A, de_A, k_sddmmA);
+        d_ops->edgeSoftmaxBackward(alpha_B, de_B, k_sddmmB);
+
+        // dP = S_alpha^T dZ, then the score gradient of both endpoints (P is both of them: shared weights); da
+        DenseMatrix dP = d_ops->like_B_matrix(0.0);
+        d_ops->spmmB(dZ, dP, alpha_B);
+        VectorXd da;
+        d_ops->gatv2Backward(P, P, a, de_A, de_B, dP, dP, da, leaky_relu_alpha);
+        const int64_t off = (int64_t)j * layer.features_per_head;
+        hnh::abi_check(hnh_axpby_f64(layer.a1Grads.data() + off, 1.0, da.data(), 0.0, nullptr, da.size(),
+                                     hnh::Runtime::get().compute_stream()),
+                       "da");
+
+        DenseMatrix &dW = layer.wGrads.at((size_t)j);
+        dW.setTransposeTimes(input, dP);
+        allreduce_world(dW);
+        dX.setTimesTranspose(dP, W, accumulate);
+    }
+
 private:
     string attention_ = "leaky";
     bool softmax_ = false;
     bool additive_ = false;
+    bool gatv2_ = false;
+
+    // head j's slice [j * features_per_head, (j + 1) * features_per_head) of an attention vector, as its own vector
+    // (copied by a library kernel: the forward pass stays free of direct CUDA runtime calls)
+    static VectorXd head_vector(const VectorXd &v, const GATLayer &layer, int j) {
+        VectorXd out(layer.features_per_head);
+        hnh::abi_check(hnh_axpby_f64(out.data(), 1.0, v.data() + (int64_t)j * layer.features_per_head, 0.0, nullptr,
+                                     layer.features_per_head, hnh::Runtime::get().compute_stream()),
+                       "attention vector slice");
+        return out;
+    }
 
     // Head j's node scalars s = P a1 and t = P a2 as whole node vectors (localArows * p entries, at least M and N;
     // those at or past M are 0): each rank writes its own rows at aSubmatrices[0].topRow into zeros, and a sum

@@ -240,6 +240,28 @@ int hnh_gat_edge_scores_f64(double *out, const double *s, const double *t, const
 int hnh_gat_rank2_update_f64(double *dP, const double *ds, const double *dt, const double *a1, const double *a2,
                              int64_t n, int64_t d, void *stream);
 
+/* ---- GATv2 attention (GAT::set_attention("gatv2"); csrc/gatv2.cu) ----------------------------------------
+ * One CSR block (rowStart: rows + 1 offsets from 0, col_idx: nnz column indices).  The "row side" R is the
+ * dense operand indexed by the stored row, the "gathered side" Y the one indexed by col_idx; both are row-major
+ * r-wide rows with their own leading dimensions (ldr, ldy >= r), so either may be the left or right half of a
+ * 2r-wide matrix.  sigma(z) = LeakyReLU(z) = z > 0 ? z : alpha z, sigma'(z) = z > 0 ? 1 : alpha
+ * (hnh_leaky_relu_grad_f64's convention); a holds r doubles.  The formulas are symmetric in R and Y.  No
+ * floating-point atomics: repeated calls give bit-identical results.  Empty input is a no-op.
+ *
+ * out[i] = sum_k a[k] sigma(R[row(i), k] + Y[col_idx[i], k]) for every entry i (overwritten, not accumulated) */
+int hnh_gatv2_scores_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                         const double *R, int64_t ldr, const double *Y, int64_t ldy, const double *a, int r,
+                         double alpha, double *out, void *stream);
+/* dR[row, :] += a o sum_{i in row} g[i] sigma'(R[row] + Y[col_idx[i]]) (dR: leading dimension lddr >= r; it
+ * may share rows with R, e.g. R = Q and dR = Q + r for Q = [R | dR] with ldr = lddr = 2r).  With da != NULL,
+ * also da[k] += sum_i g[i] sigma(R[row(i), k] + Y[col_idx[i], k]): per-CTA partials go to `workspace`, of at
+ * least hnh_gatv2_grad_workspace_bytes(rows, r) bytes, and a second kernel adds them in a fixed order. */
+int64_t hnh_gatv2_grad_workspace_bytes(int64_t rows, int r);
+int hnh_gatv2_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const double *g, int64_t rows, int64_t nnz,
+                       const double *R, int64_t ldr, const double *Y, int64_t ldy, const double *a, int r,
+                       double alpha, double *dR, int64_t lddr, double *da, void *workspace, size_t workspace_bytes,
+                       void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

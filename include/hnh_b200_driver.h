@@ -168,6 +168,18 @@ int hnhd_alg_edge_softmax_backward(hnhd_alg_t *alg, const hnhd_vec_t *alpha, hnh
 int hnhd_alg_additive_scores(hnhd_alg_t *alg, const hnhd_vec_t *s, const hnhd_vec_t *t, hnhd_vec_t *out, int mode,
                              double alpha, int derivative);
 int hnhd_alg_edge_sums(hnhd_alg_t *alg, const hnhd_vec_t *values, hnhd_vec_t *row_sums, hnhd_vec_t *col_sums);
+/* GATv2 attention (Distributed_Sparse::gatv2Scores / gatv2Backward), with A and B this rank's A- and B-shaped
+ * operands (u = S-row, v = S-column), r = a's length wide, and sigma = LeakyReLU(., alpha):
+ * gatv2_scores: out (a value vector of `mode`, as above) becomes sum_k a_k sigma(A[u, k] + B[v, k]) for every
+ * stored (u, v) of S.  gatv2_backward: with grad_A / grad_B = dL/d scores in the A and B orders, dA += the
+ * row-side gradient, dB += the column-side one, and da (resized to r) = the gradient of a summed over all ranks.
+ * dA and dB may be the same matrix.  Collective; HNH_E_INVALID where hnhd_alg_edge_softmax is, and for
+ * mismatched shapes. */
+int hnhd_alg_gatv2_scores(hnhd_alg_t *alg, hnhd_dense_t *A, hnhd_dense_t *B, const hnhd_vec_t *a, hnhd_vec_t *out,
+                          int mode, double alpha);
+int hnhd_alg_gatv2_backward(hnhd_alg_t *alg, hnhd_dense_t *A, hnhd_dense_t *B, const hnhd_vec_t *a,
+                            const hnhd_vec_t *grad_A, const hnhd_vec_t *grad_B, hnhd_dense_t *dA, hnhd_dense_t *dB,
+                            hnhd_vec_t *da, double alpha);
 
 /* CUDA-event timing on the library's compute stream: start, ..., stop -> milliseconds. */
 int hnhd_timer_start(void);
@@ -223,6 +235,9 @@ int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host);
  * With "softmax" the forward pass raises HNH_E_INVALID on every rank, before any launch, where the layout has
  * no edge softmax (as hnhd_alg_edge_softmax). */
 int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind);
+/* "gatv2": x_uv = a1 . LeakyReLU(h_u + h_v) (GATv2 with shared weights, Brody, Alon and Yahav 2022), then the edge
+ * softmax; a1 is set with hnhd_gat_set_attention_vectors (a2 is not read, its gradient stays zero).  Defined on
+ * the layouts where "softmax" is. */
 /* additive attention ("additive": x_uv = LeakyReLU(a1 . h_u + a2 . h_v) with h = X W the head's projection,
  * then the edge softmax; Velickovic et al. 2018): the attention vectors of (layer, head), features_per_head
  * doubles each (host pointers; zero after hnhd_gat_create: uniform attention).  Makes the activations stale.

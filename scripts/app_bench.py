@@ -4,9 +4,10 @@ knows -- vanilla FusedMM, one ALS-CG round (run_cg(1): 2 x 10 batched CG iterati
 forward pass ("gat"), and one GAT training step ("gat_train": forward pass, then the backward pass for an all-ones
 output gradient; the weights stay as "gat" leaves them), and both again with softmax attention ("gat_softmax",
 "gat_softmax_train": the scores of every head go through the edge softmax over each row of S) and with additive
-attention ("gat_additive", "gat_additive_train": the edge softmax of LeakyReLU(a1 . h_u + a2 . h_v)) -- at the
-launched world size (torchrun).  One JSON record per (application, algorithm) on rank 0.  Environment: LOGM, NPR, R,
-C, ALGS, APPS (e.g. APPS=gat,gat_softmax,gat_additive,gat_train,gat_softmax_train,gat_additive_train), TRIALS,
+attention ("gat_additive", "gat_additive_train": the edge softmax of LeakyReLU(a1 . h_u + a2 . h_v)) and with GATv2
+attention ("gat_v2", "gat_v2_train": the edge softmax of a1 . LeakyReLU(h_u + h_v)) -- at the launched world size
+(torchrun).  One JSON record per (application, algorithm) on rank 0.  Environment: LOGM, NPR, R, C, ALGS, APPS (e.g.
+APPS=gat,gat_softmax,gat_additive,gat_v2,gat_train,gat_softmax_train,gat_additive_train,gat_v2_train), TRIALS,
 WARMUP."""
 import json
 import os
