@@ -63,6 +63,13 @@ ABI = {
     "hnh_gatv2_grad_workspace_bytes": (C.c_int64, [_I64, C.c_int]),
     "hnh_gatv2_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, C.c_int, C.c_double, _P, _I64, _P, _P,
                                      C.c_size_t, _P]),
+    "hnh_sparse_attention_step_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, C.c_double, _P, _I64,
+                                                _P, _I64, _P, _I64, _P]),
+    "hnh_sparse_attention_finish_f64": (C.c_int, [_I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64, _P, _I64, _P]),
+    "hnh_sparse_attention_grad_q_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
+                                                  _P, _I64, C.c_double, _P, _I64, _P]),
+    "hnh_sparse_attention_grad_kv_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
+                                                   _P, _I64, C.c_double, _P, _I64, _P, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -215,6 +222,8 @@ ABI.update({
     "hnhd_alg_edge_sums": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_alg_gatv2_scores": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double]),
     "hnhd_alg_gatv2_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_double]),
+    "hnhd_alg_sparse_attention": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_double]),
+    "hnhd_alg_sparse_attention_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),

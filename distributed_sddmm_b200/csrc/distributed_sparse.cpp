@@ -3,8 +3,10 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <iostream>
 #include <mutex>
+#include <optional>
 
 #include "hnh/15D_dense_shift.hpp"
 #include "hnh/25D_cannon_dense.hpp"
@@ -446,41 +448,47 @@ void copy_cols(DenseMatrix &dst, int64_t dst_col0, const DenseMatrix &src, int64
     const size_t d = sizeof(double);
     hnh::cuda_check(cudaMemcpy2DAsync(dst.data() + dst_col0, d * (size_t)dst.cols(), src.data() + src_col0, d * (size_t)src.cols(),
                                       d * (size_t)cols, (size_t)dst.rows(), cudaMemcpyDeviceToDevice, Runtime::get().compute_stream()),
-                    "gatv2 column copy");
+                    "column copy");
 }
 }  // namespace
 
-void Distributed_Sparse::gatv2_pass(KernelMode order, DenseMatrix &localA, DenseMatrix &localB, DenseMatrix *dA, DenseMatrix *dB,
-                                    const Gatv2Kernel &kernel) {
+void Distributed_Sparse::gather_pass(KernelMode order, const vector<PassOperand> &A_side, const vector<PassOperand> &B_side,
+                                     const PassKernel &kernel) {
     SpmatLocal &m = *values_matrix(*this, order);
     const bool is_ST = &m == ST.get();
-    const int64_t r = localA.cols();
     // block b with its entries, or null when it has none
     auto block = [&](int b) -> CSRLocal * {
         const int64_t nb = (int64_t)m.blockStarts[(size_t)b + 1] - (int64_t)m.blockStarts[(size_t)b];
         if (nb == 0) return nullptr;
         CSRLocal *blk = m.csr_blocks[(size_t)b];
         if (blk == nullptr || blk->num_coords != nb)
-            throw hnh::Error(HNH_E_INVALID, "gatv2: block " + to_string(b) + " does not match its value range");
+            throw hnh::Error(HNH_E_INVALID, "gather_pass: block " + to_string(b) + " does not match its value range");
         return blk;
     };
-    auto run = [&](int b, CSRLocal &blk, const double *R, int64_t ldr, int64_t R_rows, const double *Y, int64_t Y_rows, double *dR,
-                   int64_t lddr) {
+    // the operands' views at home
+    auto home = [](const vector<PassOperand> &ops, bool gathered) {
+        vector<PassView> v;
+        for (const PassOperand &o : ops)
+            v.push_back(gathered && o.written ? PassView{nullptr, 0} : PassView{o.m->data() + o.col0, o.m->cols()});
+        return v;
+    };
+    auto run = [&](int b, CSRLocal &blk, bool rows_are_A, const vector<PassView> &R, int64_t R_rows, const vector<PassView> &Y,
+                   int64_t Y_rows) {
         if (blk.rows > R_rows || blk.cols > Y_rows)
-            throw hnh::Error(HNH_E_INVALID, "gatv2: block " + to_string(b) + " (" + to_string(blk.rows) + " x " + to_string(blk.cols) +
-                                                ") does not fit its dense operands (" + to_string(R_rows) + " and " +
-                                                to_string(Y_rows) + " rows)");
-        kernel(b, blk, R, ldr, Y, r, dR, lddr);
+            throw hnh::Error(HNH_E_INVALID, "gather_pass: block " + to_string(b) + " (" + to_string(blk.rows) + " x " +
+                                                to_string(blk.cols) + ") does not fit its dense operands (" + to_string(R_rows) +
+                                                " and " + to_string(Y_rows) + " rows)");
+        kernel(b, blk, rows_are_A, R.data(), Y.data());
     };
     if (p == 1) {
+        const vector<PassView> hA = home(A_side, false), hB = home(B_side, false), gA = home(A_side, true), gB = home(B_side, true);
         for (int b = 0; b + 1 < (int)m.blockStarts.size(); b++) {
             CSRLocal *blk = block(b);
             if (blk == nullptr) continue;
             // S stores its rows as rows, ST as columns; a transposed block swaps the two
             const bool rows_are_A = is_ST == blk->transpose;
-            DenseMatrix &Rm = rows_are_A ? localA : localB, &Ym = rows_are_A ? localB : localA;
-            DenseMatrix *dR = rows_are_A ? dA : dB;
-            run(b, *blk, Rm.data(), r, Rm.rows(), Ym.data(), Ym.rows(), dR ? dR->data() : nullptr, r);
+            run(b, *blk, rows_are_A, rows_are_A ? hA : hB, (rows_are_A ? A_side : B_side).front().m->rows(), rows_are_A ? gB : gA,
+                (rows_are_A ? B_side : A_side).front().m->rows());
         }
         return;
     }
@@ -489,50 +497,97 @@ void Distributed_Sparse::gatv2_pass(KernelMode order, DenseMatrix &localA, Dense
     Sparse15D_Dense_Shift &ds = dynamic_cast<Sparse15D_Dense_Shift &>(*this);
     const bool fusion1 = ds.fusionApproach == 1;
     const bool rows_are_A = is_ST == fusion1;
-    DenseMatrix &rowSide = rows_are_A ? localA : localB, &gathered = rows_are_A ? localB : localA;
-    DenseMatrix *dRow = rows_are_A ? dA : dB;
+    const vector<PassOperand> &rowOps = rows_are_A ? A_side : B_side, &gathOps = rows_are_A ? B_side : A_side;
+    // A side as one matrix that can travel: the operand itself when it is the side's only one (written ones left
+    // out with `skip_written`) and a whole matrix, else the windows packed side by side.  offset[i]: operand i's
+    // first column in it (-1: left out).
+    struct Travelling {
+        DenseMatrix packed;
+        DenseMatrix *whole = nullptr;
+        vector<int64_t> offset;
+        Travelling(const vector<PassOperand> &ops, bool skip_written) {
+            int64_t width = 0, n = 0;
+            const PassOperand *only = nullptr;
+            for (const PassOperand &o : ops) {
+                const bool in = !(skip_written && o.written);
+                offset.push_back(in ? width : -1);
+                if (in) {
+                    width += o.cols;
+                    n++;
+                    only = &o;
+                }
+            }
+            if (n == 1 && only->col0 == 0 && only->cols == only->m->cols()) {
+                whole = only->m;
+                return;
+            }
+            packed.resize(ops.front().m->rows(), width);
+            for (size_t i = 0; i < ops.size(); i++)
+                if (offset[i] >= 0) copy_cols(packed, offset[i], *ops[i].m, ops[i].col0, ops[i].cols);
+        }
+        DenseMatrix &mat() { return whole ? *whole : packed; }
+        vector<PassView> views(DenseMatrix &at) const {
+            vector<PassView> v;
+            for (int64_t off : offset) v.push_back(off < 0 ? PassView{nullptr, 0} : PassView{at.data() + off, at.cols()});
+            return v;
+        }
+    };
     if (!fusion1) {
-        // local kernel fusion, c = 1: the stored-row side (and its gradient) stays, the gathered side rides read-only
-        if (c != 1) throw hnh::Error(HNH_E_INVALID, "gatv2: local kernel fusion at c > 1");
-        ring_dense(gathered, grid->col_world, true, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
+        // local kernel fusion, c = 1: the stored-row side stays, the gathered side rides read-only
+        if (c != 1) throw hnh::Error(HNH_E_INVALID, "gather_pass: local kernel fusion at c > 1");
+        const vector<PassView> R = home(rowOps, false);
+        Travelling g(gathOps, true);
+        ring_dense(g.mat(), grid->col_world, true, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
             const int b = ds.block_at(step);
-            if (CSRLocal *blk = block(b))
-                run(b, *blk, rowSide.data(), r, rowSide.rows(), shard.data(), shard.rows(), dRow ? dRow->data() : nullptr, r);
+            if (CSRLocal *blk = block(b)) run(b, *blk, rows_are_A, R, rowOps.front().m->rows(), g.views(shard), shard.rows());
         });
         return;
     }
     // replication reuse: the gathered side is stationary, all-gathered over the layer (row_world); the stored-row side
     // rides the column ring
+    vector<PassView> Y = home(gathOps, true);
+    int64_t Y_rows = gathOps.front().m->rows();
+    std::optional<Travelling> g;
     DenseMatrix replicated;
-    DenseMatrix *fixed = &gathered;
     if (c > 1) {
+        g.emplace(gathOps, true);
         Runtime &rt = Runtime::get();
-        replicated.resize(gathered.rows() * c, r);
+        replicated.resize(g->mat().rows() * c, g->mat().cols());
         rt.chain(compute(), comm());
         region_begin("Replication Time", comm());
-        grid->row_world->allgather(gathered.data(), replicated.data(), sizeof(double) * (size_t)gathered.size(), comm());
+        grid->row_world->allgather(g->mat().data(), replicated.data(), sizeof(double) * (size_t)g->mat().size(), comm());
         region_end("Replication Time", comm());
         rt.chain(comm(), compute());
-        fixed = &replicated;
+        Y = g->views(replicated);
+        Y_rows = replicated.rows();
     }
-    if (dRow == nullptr) {
-        ring_dense(rowSide, grid->col_world, true, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
-            const int b = ds.block_at(step);
-            if (CSRLocal *blk = block(b)) run(b, *blk, shard.data(), r, shard.rows(), fixed->data(), fixed->rows(), nullptr, r);
-        });
-        return;
-    }
-    // the gradient has to ride with the rows it belongs to: [row side | gradient] travels as one 2r-wide matrix on the
-    // output-riding ring (kernel and shift alternate) and is back home after the last shift
-    DenseMatrix packed(rowSide.rows(), 2 * r);
-    copy_cols(packed, 0, rowSide, 0, r);
-    copy_cols(packed, r, *dRow, 0, r);
-    ring_dense(packed, grid->col_world, false, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
+    // written operands ride with the rows they belong to, on the output-riding ring (kernel and shift alternate), and
+    // are back home after the last shift
+    bool written = false;
+    for (const PassOperand &o : rowOps) written = written || o.written;
+    Travelling r(rowOps, false);
+    ring_dense(r.mat(), grid->col_world, !written, "Cyclic Shift Time", "Computation Time", [&](int step, DenseMatrix &shard) {
         const int b = ds.block_at(step);
-        if (CSRLocal *blk = block(b))
-            run(b, *blk, shard.data(), 2 * r, shard.rows(), fixed->data(), fixed->rows(), shard.data() + r, 2 * r);
+        if (CSRLocal *blk = block(b)) run(b, *blk, rows_are_A, r.views(shard), shard.rows(), Y, Y_rows);
     });
-    copy_cols(*dRow, 0, packed, r, r);
+    if (r.whole == nullptr)
+        for (size_t i = 0; i < rowOps.size(); i++)
+            if (rowOps[i].written) copy_cols(*rowOps[i].m, rowOps[i].col0, r.packed, r.offset[i], rowOps[i].cols);
+}
+
+void Distributed_Sparse::gatv2_pass(KernelMode order, DenseMatrix &localA, DenseMatrix &localB, DenseMatrix *dA, DenseMatrix *dB,
+                                    const Gatv2Kernel &kernel) {
+    const int64_t r = localA.cols();
+    // each side: its operand, then its gradient; the gradients ride with the stored rows as one 2r-wide matrix
+    vector<PassOperand> A_side{{&localA, 0, r, false}}, B_side{{&localB, 0, r, false}};
+    const bool grads = dA != nullptr || dB != nullptr;
+    if (grads) {
+        A_side.push_back({dA, 0, r, true});
+        B_side.push_back({dB, 0, r, true});
+    }
+    gather_pass(order, A_side, B_side, [&](int b, CSRLocal &blk, bool, const PassView *R, const PassView *Y) {
+        kernel(b, blk, R[0].p, R[0].ld, Y[0].p, Y[0].ld, grads ? R[1].p : nullptr, grads ? R[1].ld : r);
+    });
 }
 
 namespace {
@@ -607,6 +662,104 @@ void Distributed_Sparse::gatv2Backward(DenseMatrix &localA, DenseMatrix &localB,
     }
     allreduce_rows(da_local.data(), r, false);
     da = std::move(da_local);
+}
+
+// ---- fused sparse attention ------------------------------------------------------------------------------------
+namespace {
+// the shape checks of sparseAttention / sparseAttentionBackward; returns the head width d = r / heads
+int64_t check_attention(const Distributed_Sparse &dist, const string &who, std::initializer_list<const DenseMatrix *> A_like,
+                        std::initializer_list<const DenseMatrix *> B_like, const DenseMatrix &L, int heads, double scale) {
+    const int64_t r = (*A_like.begin())->cols();
+    for (const DenseMatrix *m : A_like)
+        if (m->rows() != dist.localArows || m->cols() != r)
+            throw hnh::Error(HNH_E_INVALID, who + ": an A-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                "; like_A_matrix has " + to_string(dist.localArows) + " rows, Q is " + to_string(r) +
+                                                " wide");
+    for (const DenseMatrix *m : B_like)
+        if (m->rows() != dist.localBrows || m->cols() != r)
+            throw hnh::Error(HNH_E_INVALID, who + ": a B-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                "; like_B_matrix has " + to_string(dist.localBrows) + " rows, Q is " + to_string(r) +
+                                                " wide");
+    if (heads < 1 || r < 1 || r % heads != 0 || r / heads > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": " + to_string(heads) + " heads do not divide the width " + to_string(r));
+    if (!std::isfinite(scale)) throw hnh::Error(HNH_E_INVALID, who + ": the scale must be finite");
+    if (L.rows() != dist.localArows || L.cols() != heads)
+        throw hnh::Error(HNH_E_INVALID, who + ": L is " + to_string(L.rows()) + " x " + to_string(L.cols()) + ", not localArows x heads = " +
+                                            to_string(dist.localArows) + " x " + to_string(heads));
+    return r / heads;
+}
+void need_rows(bool rows_are_A, bool want, const char *who) {
+    if (rows_are_A != want)
+        throw hnh::Error(HNH_E_INVALID, string(who) + ": a block of this order does not hold the " + (want ? "query" : "key") +
+                                            " side as its stored rows");
+}
+}  // namespace
+
+void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                                         double scale) {
+    check_full_rows("sparseAttention");
+    const int64_t d = check_attention(*this, "sparseAttention", {&Q, &Z}, {&K, &V}, L, heads, scale);
+    // the online-softmax state of row u, head h: acc in Z's window, m in L[u, h], s in s[u, h]; m is not read while
+    // s = 0, and the finish turns (acc, m, s) into (Z, L) in place
+    Z.setZero();
+    DenseMatrix s(localArows, heads);
+    s.setZero();
+    for (int h = 0; h < heads; h++) {
+        const vector<PassOperand> A_side{{&Q, h * d, d, false}, {&Z, h * d, d, true}, {&L, h, 1, true}, {&s, h, 1, true}};
+        const vector<PassOperand> B_side{{&K, h * d, d, false}, {&V, h * d, d, false}};
+        gather_pass(k_sddmmA, A_side, B_side, [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+            need_rows(rows_are_A, true, "sparseAttention");
+            CSRHandle *hd = blk.getActive();
+            hnh::abi_check(hnh_sparse_attention_step_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d,
+                                                         R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale, R[1].p, R[1].ld,
+                                                         R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
+                           "sparse_attention_step");
+        });
+        hnh::abi_check(hnh_sparse_attention_finish_f64(localArows, (int)d, Z.data() + h * d, Z.cols(), L.data() + h, heads,
+                                                       s.data() + h, heads, Z.data() + h * d, Z.cols(), L.data() + h, heads,
+                                                       compute()),
+                       "sparse_attention_finish");
+    }
+}
+
+void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                                 double scale) {
+    check_full_rows("sparseAttentionBackward");
+    const int64_t d = check_attention(*this, "sparseAttentionBackward", {&Q, &Z, &dZ, &dQ}, {&K, &V, &dK, &dV}, L, heads, scale);
+    // t[u, h] = <dZ_u,h, Z_u,h>: Z and dZ read as localArows * heads rows of d
+    DenseMatrix t(localArows, heads);
+    hnh::abi_check(hnh_batch_dot_f64(t.data(), dZ.data(), Z.data(), localArows * heads, (int)d, compute()), "batch_dot");
+    dQ.setZero();
+    dK.setZero();
+    dV.setZero();
+    for (int h = 0; h < heads; h++) {
+        const int64_t w = h * d;
+        // query rows own dQ (A order)
+        gather_pass(k_sddmmA, {{&Q, w, d, false}, {&dZ, w, d, false}, {&L, h, 1, false}, {&t, h, 1, false}, {&dQ, w, d, true}},
+                    {{&K, w, d, false}, {&V, w, d, false}},
+                    [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                        need_rows(rows_are_A, true, "sparseAttentionBackward");
+                        CSRHandle *hd = blk.getActive();
+                        hnh::abi_check(hnh_sparse_attention_grad_q_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
+                                                                       (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p,
+                                                                       R[3].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale, R[4].p, R[4].ld,
+                                                                       compute()),
+                                       "sparse_attention_grad_q");
+                    });
+        // key rows own dK and dV (B order)
+        gather_pass(k_sddmmB, {{&Q, w, d, false}, {&dZ, w, d, false}, {&L, h, 1, false}, {&t, h, 1, false}},
+                    {{&K, w, d, false}, {&V, w, d, false}, {&dK, w, d, true}, {&dV, w, d, true}},
+                    [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                        need_rows(rows_are_A, false, "sparseAttentionBackward");
+                        CSRHandle *hd = blk.getActive();
+                        hnh::abi_check(hnh_sparse_attention_grad_kv_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
+                                                                        blk.num_coords, (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld, Y[0].p,
+                                                                        Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p, Y[3].ld, scale,
+                                                                        R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
+                                       "sparse_attention_grad_kv");
+                    });
+    }
 }
 
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {

@@ -1,6 +1,7 @@
 // driver.cpp -- extern "C" driver ABI (include/hnh_b200_driver.h) over the C++ host classes.
 #include "hnh_b200_driver.h"
 
+#include <cmath>
 #include <cstring>
 #include <memory>
 
@@ -362,6 +363,25 @@ int hnhd_alg_gatv2_backward(hnhd_alg_t *a, hnhd_dense_t *A, hnhd_dense_t *B, con
         if (!a || !A || !B || !va || !grad_A || !grad_B || !dA || !dB || !da)
             throw hnh::Error(HNH_E_INVALID, "hnhd_alg_gatv2_backward: null argument");
         a->alg->gatv2Backward(A->m, B->m, va->v, grad_A->v, grad_B->v, dA->m, dB->m, da->v, alpha);
+    });
+}
+
+int hnhd_alg_sparse_attention(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z, hnhd_dense_t *L,
+                              int heads, double scale) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention: null argument");
+        if (!std::isfinite(scale)) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention: the scale must be finite");
+        a->alg->sparseAttention(Q->m, K->m, V->m, Z->m, L->m, heads, scale);
+    });
+}
+int hnhd_alg_sparse_attention_backward(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                       hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ, hnhd_dense_t *dK, hnhd_dense_t *dV,
+                                       int heads, double scale) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L || !dZ || !dQ || !dK || !dV)
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward: null argument");
+        if (!std::isfinite(scale)) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward: the scale must be finite");
+        a->alg->sparseAttentionBackward(Q->m, K->m, V->m, Z->m, L->m, dZ->m, dQ->m, dK->m, dV->m, heads, scale);
     });
 }
 

@@ -13,11 +13,7 @@
 // with a grid-stride loop.  Widths 4..256 (powers of two) with 16-byte aligned operands and even leading dimensions
 // take these; every other case (any r >= 1, any leading dimension, any alignment) takes the one-warp-per-row generic
 // kernels.  No floating-point atomics: two calls on the same device give bit-identical results.
-#include <algorithm>
-#include <cstdint>
-
-#include "hnh_b200.h"
-#include "launch.h"
+#include "row_gather.cuh"
 
 namespace {
 
@@ -25,49 +21,6 @@ using hnh::check_cuda;
 using hnh::count_launch;
 using hnh::set_error;
 
-// the load / store forms of kernels.cuh (not included here: it defines non-template kernels of c_abi.cu).  Gathers
-// use the read-only path at the normal L2 policy; index and value streams do not allocate in L1.
-template <int VW>
-__device__ __forceinline__ void ld_gather(double (&d)[VW], const double *p) {
-    static_assert(VW == 2, "128-bit loads only");
-    asm("ld.global.nc.L1::no_allocate.v2.f64 {%0,%1}, [%2];" : "=d"(d[0]), "=d"(d[1]) : "l"(p));
-}
-template <int VW>
-__device__ __forceinline__ void ld_rw(double (&d)[VW], const double *p) {
-    static_assert(VW == 2, "128-bit loads only");
-    asm volatile("ld.global.L1::no_allocate.v2.f64 {%0,%1}, [%2];" : "=d"(d[0]), "=d"(d[1]) : "l"(p) : "memory");
-}
-template <int VW>
-__device__ __forceinline__ void st_rw(double *p, const double (&d)[VW]) {
-    static_assert(VW == 2, "128-bit stores only");
-    asm volatile("st.global.L1::no_allocate.v2.f64 [%0], {%1,%2};" ::"l"(p), "d"(d[0]), "d"(d[1]) : "memory");
-}
-__device__ __forceinline__ int64_t ld_stream_i64(const int64_t *p) {
-    int64_t v;
-    asm volatile("ld.global.nc.L1::no_allocate.s64 %0, [%1];" : "=l"(v) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ double ld_stream_f64(const double *p) {
-    double v;
-    asm volatile("ld.global.nc.L1::no_allocate.f64 %0, [%1];" : "=d"(v) : "l"(p));
-    return v;
-}
-template <int G>
-__device__ __forceinline__ unsigned group_mask(int lane) {
-    if constexpr (G == 32) {
-        return 0xffffffffu;
-    } else {
-        return ((1u << G) - 1u) << (lane & ~(G - 1));
-    }
-}
-template <int G>
-__device__ __forceinline__ double group_allreduce(double d, unsigned mask) {
-#pragma unroll
-    for (int o = G / 2; o > 0; o >>= 1) d += __shfl_xor_sync(mask, d, o, G);
-    return d;
-}
-
-constexpr int kBlock = 256;
 // most CTAs a gradient launch uses (the da workspace holds one r-wide partial per CTA)
 constexpr int64_t kMaxGradCtas = 2048;
 
@@ -300,37 +253,6 @@ __global__ void gatv2_da_reduce_kernel(double *__restrict__ da, const double *__
 }
 
 // ---- launch ----------------------------------------------------------------------------------------------------
-// grid for a grid-stride kernel: at most the CTAs resident at once, at most one per `per_cta` work items, at most `cap`
-template <typename K>
-int grid_for(K kernel, int64_t per_cta, int64_t work, int64_t cap, int *grid) {
-    int sms = 0;
-    int rc = hnh::device_sm_count(&sms);
-    if (rc) return rc;
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kBlock, 0);
-    if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
-    const int64_t need = (work + per_cta - 1) / per_cta;
-    *grid = (int)std::max<int64_t>(1, std::min({need, (int64_t)sms * std::max(occ, 1), cap}));
-    return HNH_OK;
-}
-
-bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
-
-// the width table of the fast kernels: R -> (G lanes per row, VW doubles per load, UN rows in flight), as
-// HNH_DISPATCH_R in c_abi.cu
-#define GATV2_DISPATCH(r, CALL)               \
-    switch (r) {                              \
-        case 4:   CALL(4, 2, 2, 2); break;    \
-        case 8:   CALL(8, 4, 2, 4); break;    \
-        case 16:  CALL(16, 8, 2, 4); break;   \
-        case 32:  CALL(32, 16, 2, 4); break;  \
-        case 64:  CALL(64, 32, 2, 4); break;  \
-        case 128: CALL(128, 32, 2, 4); break; \
-        case 256: CALL(256, 32, 2, 2); break; \
-        default: break;                       \
-    }
-
-bool table_width(int r) { return r >= 4 && r <= 256 && (r & (r - 1)) == 0; }
 
 template <int R, int G, int VW, int UN>
 int launch_scores(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, const double *X, int64_t ldx,
@@ -383,7 +305,7 @@ int hnh_gatv2_scores_f64(const int64_t *rowStart, const int64_t *col_idx, int64_
     if (table_width(r) && aligned16(R) && aligned16(Y) && aligned16(a) && ldr % 2 == 0 && ldy % 2 == 0) {
         int rc = HNH_OK;
 #define SC(RR, G, VW, UN) rc = launch_scores<RR, G, VW, UN>(rowStart, col_idx, rows, R, ldr, Y, ldy, a, alpha, out, st)
-        GATV2_DISPATCH(r, SC)
+        ROW_GATHER_DISPATCH(r, SC)
 #undef SC
         return rc;
     }
@@ -419,7 +341,7 @@ int hnh_gatv2_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const do
         lddr % 2 == 0) {
 #define GR(RR, G, VW, UN) \
     rc = launch_grad<RR, G, VW, UN>(rowStart, col_idx, g, rows, R, ldr, Y, ldy, a, alpha, dR, lddr, part, &ctas, st)
-        GATV2_DISPATCH(r, GR)
+        ROW_GATHER_DISPATCH(r, GR)
 #undef GR
     } else {
         rc = grid_for(gatv2_grad_generic_kernel, kBlock / 32, rows, kMaxGradCtas, &ctas);

@@ -15,6 +15,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import math
 import os
 
 import numpy as np
@@ -124,6 +125,13 @@ class SpmatLocal:
 class Dense:
     def __init__(self, handle):
         self.h = handle
+
+    @classmethod
+    def create(cls, rows: int, cols: int, value: float = 0.0):
+        """A rows x cols device matrix filled with `value` (e.g. the L of Algorithm.sparse_attention)."""
+        h = C.c_void_p()
+        check(lib().hnhd_dense_create(rows, cols, value, C.byref(h)), "hnhd_dense_create")
+        return cls(h)
 
     @property
     def shape(self):
@@ -287,6 +295,31 @@ class Algorithm:
         (Distributed_Sparse::gatv2Backward)."""
         check(lib().hnhd_alg_gatv2_backward(self.h, A.h, B.h, a.h, grad_A.h, grad_B.h, dA.h, dB.h, da.h, float(alpha)),
               "gatv2_backward")
+
+    @staticmethod
+    def _attention_scale(Q: Dense, heads: int, scale):
+        if scale is not None:
+            return float(scale)
+        r = Q.shape[1]
+        if heads < 1 or r % heads:
+            raise ValueError(f"heads = {heads} must divide the width {r}")
+        return 1.0 / math.sqrt(r // heads)
+
+    def sparse_attention(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, heads: int = 1, scale=None):
+        """Collective: fused attention over the pattern of S (its values are not read).  Q and Z are A-shaped, K and V
+        B-shaped, all r wide; per head h of width d = r / heads, Z_u,h = sum over the stored (u, v) of
+        softmax_v(scale <Q_u,h, K_v,h>) V_v,h, and L (Dense.create(localArows, heads)) = the rows' log-sum-exp (-inf,
+        and Z = 0, for a row without entries).  scale=None means 1/sqrt(d) (Distributed_Sparse::sparseAttention)."""
+        s = self._attention_scale(Q, heads, scale)
+        check(lib().hnhd_alg_sparse_attention(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s), "sparse_attention")
+
+    def sparse_attention_backward(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, dZ: Dense, dQ: Dense, dK: Dense,
+                                  dV: Dense, heads: int = 1, scale=None):
+        """Collective: given dZ = dLoss/dZ and the forward's Z and L, overwrites dQ, dK and dV with the gradients of
+        sparse_attention (Distributed_Sparse::sparseAttentionBackward)."""
+        s = self._attention_scale(Q, heads, scale)
+        check(lib().hnhd_alg_sparse_attention_backward(self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h, int(heads), s),
+              "sparse_attention_backward")
 
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])

@@ -199,6 +199,24 @@ public:
                      double alpha);
     void gatv2Backward(DenseMatrix &localA, DenseMatrix &localB, const VectorXd &a, const VectorXd &grad_A,
                        const VectorXd &grad_B, DenseMatrix &dA, DenseMatrix &dB, VectorXd &da, double alpha);
+
+    // ---- fused sparse attention over the pattern of S --------------------------------------------------------
+    // Q (A-shaped: this rank's S-rows) and K, V (B-shaped: its S-columns) are r wide, r = heads * d.  For head h,
+    // over the column window [h d, (h + 1) d), and every stored (u, v) of S (duplicates count; S's values are not
+    // read):  x_uv = scale <Q_u,h, K_v,h>,  L_u,h = log sum_v exp(x_uv),  Z_u,h = sum_v exp(x_uv - L_u,h) V_v,h.
+    // sparseAttention overwrites Z (A-shaped, r wide) and L (localArows x heads); a row without entries gets Z = 0
+    // and L = -inf.  sparseAttentionBackward, given dZ and the forward's Z and L, overwrites dQ, dK and dV:
+    //     t_u,h = <dZ_u,h, Z_u,h>,  dx_uv = alpha_uv (<dZ_u,h, V_v,h> - t_u,h),
+    //     dQ_u,h = scale sum_v dx_uv K_v,h,  dK_v,h = scale sum_u dx_uv Q_u,h,  dV_v,h = sum_u alpha_uv dZ_u,h.
+    // One fused pass per head for the forward (an online softmax carried from block to block), two for the
+    // backward (A order for dQ, B order for dK and dV); no score vector, no row grouping, and no collective beyond
+    // the ring shifts of gather_pass.  `scale` must be finite.  Collective; defined where check_full_rows passes,
+    // HNH_E_INVALID on every rank elsewhere.
+    void sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                         double scale);
+    void sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                 double scale);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 
@@ -235,6 +253,29 @@ protected:
     template <class Body>
     void ring_dense(DenseMatrix &home, std::shared_ptr<hnh::Comm> world_ptr, bool riding_is_input, const string &shift_key,
                     const string &compute_key, Body body);
+
+    // One pass of a row-owning kernel over the CSR blocks of a value order (gatv2_pass, sparseAttention): each
+    // side of S has a list of operands, column windows of A-shaped (A_side) or B-shaped (B_side) matrices.  For
+    // every block with entries, kernel(block, blk, rows_are_A, rows, gathered) runs where the block meets them, with
+    // rows[i] the view of operand i of the side whose rows the block stores and gathered[i] that of operand i of
+    // the other side (null for a written one: a kernel writes the stored-row side only).  Where the operands
+    // travel: p = 1, none; 1.5D dense shift with local kernel fusion (c = 1): the stored-row side stays, the
+    // gathered side rides read-only; with replication reuse (any c): the gathered side is stationary, all-gathered
+    // over the layer when c > 1, and the stored-row side rides -- with its written operands on the output-riding
+    // ring, complete when it comes home.  A side that moves travels as its one operand when that is a whole matrix,
+    // else packed into one matrix of the operands' windows side by side.
+    struct PassOperand {
+        DenseMatrix *m;
+        int64_t col0, cols;
+        bool written;  // the kernel accumulates into it
+    };
+    struct PassView {
+        double *p;  // row 0 of the window
+        int64_t ld;
+    };
+    using PassKernel = std::function<void(int, CSRLocal &, bool, const PassView *, const PassView *)>;
+    void gather_pass(KernelMode order, const vector<PassOperand> &A_side, const vector<PassOperand> &B_side,
+                     const PassKernel &kernel);
 
     // One GATv2 pass over the CSR blocks of a value order (gatv2Scores, gatv2Backward): kernel(block, blk, R, ldr,
     // Y, ldy, dR, lddr) runs once per block with entries, with R the stored-row side, Y the gathered side and dR

@@ -262,6 +262,41 @@ int hnh_gatv2_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const do
                        double alpha, double *dR, int64_t lddr, double *da, void *workspace, size_t workspace_bytes,
                        void *stream);
 
+/* ---- fused sparse attention (Distributed_Sparse::sparseAttention; csrc/sparse_attention.cu) ---------------
+ * One CSR block (rowStart, col_idx as above) with stored row u and gathered row v = col_idx[i].  Every dense
+ * operand is a pointer plus its own leading dimension: d-wide rows (ld >= d) or one scalar per row (ld >= 1,
+ * e.g. column h of a rows x H matrix is L + h with ld = H), so head windows of an H*d-wide matrix and packed
+ * matrices are views.  x_uv = scale <Q_u, K_v>; scale must be finite.  No floating-point atomics: repeated
+ * calls give bit-identical results.  No rows or no entries: a no-op.
+ *
+ * step: continues the online softmax of every stored row over the block's entries (a row whose entries lie in
+ * several blocks is carried from call to call):
+ *     m' = max(m, max_i x_i),  s' = e^(m - m') s + sum_i e^(x_i - m'),  acc' = e^(m - m') acc + sum_i e^(x_i - m') V_v
+ * Start from acc = 0, s = 0 (m = -inf; m is not read while s = 0).  Rows without entries are not touched. */
+int hnh_sparse_attention_step_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                  const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V,
+                                  int64_t ldv, double scale, double *acc, int64_t ldacc, double *m, int64_t ldm,
+                                  double *s, int64_t lds, void *stream);
+/* finish: Z = acc / s and L = m + log s per row; Z = 0 and L = -inf where s = 0.  In place allowed: Z may be acc
+ * and L may be m (same pointer and leading dimension). */
+int hnh_sparse_attention_finish_f64(int64_t rows, int d, const double *acc, int64_t ldacc, const double *m,
+                                    int64_t ldm, const double *s, int64_t lds, double *Z, int64_t ldz, double *L,
+                                    int64_t ldl, void *stream);
+/* Backward, with L the finished log-sum-exp and t_u = <dZ_u, Z_u>; alpha_uv = exp(x_uv - L_u) and
+ * dx_uv = alpha_uv (<dZ_u, V_v> - t_u).
+ * grad_q (stored rows are query rows u): dQ_u += scale sum_v dx_uv K_v.
+ * grad_kv (stored rows are key rows v; L and t gathered by col_idx): dK_v += scale sum_u dx_uv Q_u and
+ * dV_v += sum_u alpha_uv dZ_u. */
+int hnh_sparse_attention_grad_q_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                    const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
+                                    int64_t ldl, const double *t, int64_t ldt, const double *K, int64_t ldk,
+                                    const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq, void *stream);
+int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                     const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q,
+                                     int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
+                                     const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
+                                     int64_t lddv, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

@@ -180,6 +180,17 @@ int hnhd_alg_gatv2_scores(hnhd_alg_t *alg, hnhd_dense_t *A, hnhd_dense_t *B, con
 int hnhd_alg_gatv2_backward(hnhd_alg_t *alg, hnhd_dense_t *A, hnhd_dense_t *B, const hnhd_vec_t *a,
                             const hnhd_vec_t *grad_A, const hnhd_vec_t *grad_B, hnhd_dense_t *dA, hnhd_dense_t *dB,
                             hnhd_vec_t *da, double alpha);
+/* Fused sparse attention (Distributed_Sparse::sparseAttention / sparseAttentionBackward): per head h of width
+ * d = r / heads, Z_u,h = sum over the stored (u, v) of S of softmax_v(scale <Q_u,h, K_v,h>) V_v,h, with Q and Z
+ * A-shaped, K and V B-shaped, all r wide; L (localArows x heads, from hnhd_dense_create) receives the rows'
+ * log-sum-exp (-inf, and Z = 0, for a row without entries).  The backward, given dZ (A-shaped), overwrites dQ, dK
+ * and dV.  S's values are not read.  `scale` must be finite.  Collective; HNH_E_INVALID where hnhd_alg_edge_softmax
+ * is, and for mismatched shapes. */
+int hnhd_alg_sparse_attention(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                              hnhd_dense_t *L, int heads, double scale);
+int hnhd_alg_sparse_attention_backward(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V,
+                                       hnhd_dense_t *Z, hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ,
+                                       hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale);
 
 /* CUDA-event timing on the library's compute stream: start, ..., stop -> milliseconds. */
 int hnhd_timer_start(void);

@@ -1,0 +1,201 @@
+#!/usr/bin/env python
+"""CUDA-event time of fused sparse attention on one GPU, at the kernel level and at the op level.
+
+Kernels, on the A-order CSR block of an Erdos-Renyi 2^LOGM x 2^LOGM S with NPR draws per row under ALG at p = 1
+(15d_fusion1: 2^20 rows and 33 553 937 entries at the defaults) and, for the key-side gradient, the B-order block,
+at each d of WIDTHS: the step (hnh_sparse_attention_step_f64), the finish, and the two gradients, beside the
+overwrite-form SDDMM (hnh_sddmm_f64 with HNH_FLAG_BETA0) and the accumulating SpMM (hnh_spmm_f64) on the same block.
+Algorithmic bytes per call (int64 indices, fp64 values; a gathered row counted once per entry, as if no cache held it):
+    sddmm (overwrite)  nnz (8 col + 8 value + 8 d gathered) + rows (8 row start + 8 d row side)
+    spmm (accumulate)  nnz (8 col + 8 value + 8 d gathered) + rows (8 row start + 16 d output read and write)
+    step               nnz (8 col + 16 d K and V) + rows (8 row start + 8 d Q + 16 d acc read and write + 32 m, s)
+    finish             rows (24 d + 32)
+    grad_q             nnz (8 col + 16 d K and V) + rows (8 row start + 16 d Q, dZ + 16 L, t + 16 d dQ read and write)
+    grad_kv            nnz (8 col + 16 d Q and dZ + 16 L, t) + rows (8 row start + 16 d K, V + 32 d dK, dV read and write)
+set against the H100 SXM's 3.35 TB/s.  Op level, one head of width d: Algorithm.sparse_attention and
+sparse_attention_backward beside the composed public ops -- forward: scaled sddmmA, edge_softmax, spmmA; backward:
+alpha in both orders (2 scaled SDDMMs, 2 softmaxes), dalpha in both orders (2 SDDMMs), 2 softmax backwards and the
+dV, dQ, dK SpMMs -- with the composed path's first edge_softmax per order (which builds its row grouping) timed
+separately, and the largest relative difference between the two.  Prints the card name and power limit, then one
+JSON line per measurement.  Environment: LOGM (20), NPR (32), WIDTHS (128,256), ALG (15d_fusion1), REPS (20)."""
+import json
+import math
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from bench import SEED  # noqa: E402
+from distributed_sddmm_b200 import driver as D  # noqa: E402
+from distributed_sddmm_b200 import lib  # noqa: E402
+
+logM = int(os.environ.get("LOGM", "20"))
+npr = int(os.environ.get("NPR", "32"))
+widths = [int(x) for x in os.environ.get("WIDTHS", "128,256").split(",")]
+alg_name = os.environ.get("ALG", "15d_fusion1")
+reps = int(os.environ.get("REPS", "20"))
+HBM = 3.35e12
+BETA0 = 4
+
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                      capture_output=True, text=True, timeout=30).stdout.strip()
+print(json.dumps({"card": card}), flush=True)
+torch.cuda.set_device(0)
+dev = torch.device("cuda:0")
+D.world_init("self")
+L = lib()
+S = D.SpmatLocal.load_er(logM, npr, SEED)
+st = torch.cuda.current_stream().cuda_stream
+f64 = dict(dtype=torch.float64, device=dev)
+
+
+def timed(call):
+    call()
+    torch.cuda.synchronize()
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    for _ in range(reps):
+        call()
+    t1.record()
+    torch.cuda.synchronize()
+    return t0.elapsed_time(t1) / reps
+
+
+def timed_op(call):
+    """The same on the library's compute stream, where the operations run."""
+    call()
+    D.timer_start()
+    for _ in range(reps):
+        call()
+    return D.timer_stop() / reps
+
+
+def once_op(call):
+    D.timer_start()
+    call()
+    return D.timer_stop()
+
+
+def report(kernel, d, ms, nbytes=None, **extra):
+    rec = dict(kernel=kernel, logM=logM, nnz_per_row=npr, d=d, ms_per_call=round(ms, 4), **extra)
+    if nbytes:
+        rec.update(min_bytes=nbytes, tb_per_s=round(nbytes / (ms * 1e-3) / 1e12, 3),
+                   share_of_3_35_tb_s=round(nbytes / (ms * 1e-3) / HBM, 3))
+    print(json.dumps(rec), flush=True)
+    return ms
+
+
+def block(alg, which):
+    blocks = [b for b in alg.blocks(which) if b is not None]
+    assert len(blocks) == 1, "one local block at p = 1"
+    b = blocks[0]
+    return int(b["rows"]), len(b["col_idx"]), torch.from_numpy(b["rowStart"]).to(dev), torch.from_numpy(b["col_idx"]).to(dev)
+
+
+def kernels(alg, d):
+    # fusion 1 keeps the A order in ST's block (S-rows as stored rows) and the B order in S's
+    a_blk, b_blk = ("ST", "S") if alg_name == "15d_fusion1" else ("S", "ST")
+    rows, nnz, rs, ci = block(alg, a_blk)
+    rowsT, nnzT, rsT, ciT = block(alg, b_blk)
+    g = torch.Generator(device=dev).manual_seed(1)
+    Q, K, V, dZ = (torch.rand((max(rows, rowsT), d), generator=g, **f64) * 2 - 1 for _ in range(4))
+    acc, dQ, dK, dV = (torch.zeros((max(rows, rowsT), d), **f64) for _ in range(4))
+    ms_ = torch.zeros((rows, 2), **f64)
+    Lt = torch.zeros((max(rows, rowsT), 2), **f64)
+    values = torch.rand(nnz, generator=g, **f64)
+    out = torch.empty(nnz, **f64)
+    scale = 1 / math.sqrt(d)
+    p = lambda t: t.data_ptr()  # noqa: E731
+    sddmm = report("sddmm_overwrite", d, timed(lambda: D.check(L.hnh_sddmm_f64(
+        p(rs), p(ci), p(out), rows, nnz, p(Q), p(K), d, BETA0, st))), nnz * (16 + 8 * d) + rows * (8 + 8 * d))
+    spmm = report("spmm_accumulate", d, timed(lambda: D.check(L.hnh_spmm_f64(
+        p(rs), p(ci), p(values), rows, nnz, p(V), p(acc), d, 0, st))), nnz * (16 + 8 * d) + rows * (8 + 16 * d))
+    base = sddmm + spmm
+
+    def step():
+        D.check(L.hnh_sparse_attention_step_f64(p(rs), p(ci), rows, nnz, d, p(Q), d, p(K), d, p(V), d, scale, p(acc), d,
+                                                p(ms_), 2, p(ms_) + 8, 2, st))
+    acc.zero_()
+    ms_.zero_()
+    st_ms = report("step", d, timed(step), nnz * (8 + 16 * d) + rows * (8 + 24 * d + 32))
+    finish = report("finish", d, timed(lambda: D.check(L.hnh_sparse_attention_finish_f64(
+        rows, d, p(acc), d, p(ms_), 2, p(ms_) + 8, 2, p(dQ), d, p(Lt), 2, st))), rows * (24 * d + 32))
+    gq = report("grad_q", d, timed(lambda: D.check(L.hnh_sparse_attention_grad_q_f64(
+        p(rs), p(ci), rows, nnz, d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, p(K), d, p(V), d, scale, p(dQ), d, st))),
+        nnz * (8 + 16 * d) + rows * (8 + 32 * d + 16))
+    gkv = report("grad_kv", d, timed(lambda: D.check(L.hnh_sparse_attention_grad_kv_f64(
+        p(rsT), p(ciT), rowsT, nnzT, d, p(K), d, p(V), d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, scale, p(dK), d, p(dV), d,
+        st))), nnzT * (24 + 16 * d) + rowsT * (8 + 48 * d))
+    print(json.dumps(dict(d=d, entries=nnz, rows=rows, step_over_sddmm_plus_spmm=round(st_ms / base, 3),
+                          step_plus_finish_over_sddmm_plus_spmm=round((st_ms + finish) / base, 3),
+                          grad_q_over_sddmm_plus_spmm=round(gq / base, 3),
+                          grad_kv_over_sddmm_plus_spmm=round(gkv / base, 3))), flush=True)
+
+
+def rel(a, b):
+    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-300))
+
+
+def ops(d):
+    alg = D.Algorithm(alg_name, S, d, 1)
+    dims = alg.dims
+    rng = np.random.default_rng(SEED)
+    mats = {}
+    for name, which in (("Q", "A"), ("dZ", "A"), ("K", "B"), ("V", "B")):
+        m = alg.like_A_matrix() if which == "A" else alg.like_B_matrix()
+        m.from_host(rng.uniform(-1, 1, m.shape))
+        mats[name] = m
+    Q, K, V, dZ = (mats[k] for k in ("Q", "K", "V", "dZ"))
+    Z, dQ, dK, dV = alg.like_A_matrix(), alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix()
+    Lm = D.Dense.create(dims.localArows, 1)
+    scale = 1 / math.sqrt(d)
+    fwd = report("op_fused_forward", d, timed_op(lambda: alg.sparse_attention(Q, K, V, Z, Lm)))
+    bwd = report("op_fused_backward", d, timed_op(lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV)))
+    # composed: the first edge_softmax per order builds its row grouping
+    sA, sB, oneA, oneB = alg.like_S_values(scale), alg.like_ST_values(scale), alg.like_S_values(1.0), alg.like_ST_values(1.0)
+    xA, xB, gA, gB = alg.like_S_values(), alg.like_ST_values(), alg.like_S_values(), alg.like_ST_values()
+    Zc, dQc, dKc, dVc = alg.like_A_matrix(), alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix()
+    alg.sddmmA(Q, K, sA, xA)
+    alg.sddmmB(Q, K, sB, xB)
+    plan_a = once_op(lambda: alg.edge_softmax(xA, "A"))
+    plan_b = once_op(lambda: alg.edge_softmax(xB, "B"))
+
+    def c_forward():
+        alg.sddmmA(Q, K, sA, xA)
+        alg.edge_softmax(xA, "A")
+        alg.spmmA(Zc, V, xA)
+
+    def c_backward():
+        alg.sddmmA(Q, K, sA, xA)
+        alg.edge_softmax(xA, "A")
+        alg.sddmmB(Q, K, sB, xB)
+        alg.edge_softmax(xB, "B")
+        alg.sddmmA(dZ, V, oneA, gA)
+        alg.sddmmB(dZ, V, oneB, gB)
+        alg.edge_softmax_backward(xA, gA, "A")
+        alg.edge_softmax_backward(xB, gB, "B")
+        alg.spmmB(dZ, dVc, xB)
+        alg.spmmA(dQc, K, gA)
+        alg.spmmB(Q, dKc, gB)
+
+    cf = report("op_composed_forward", d, timed_op(c_forward), first_edge_softmax_ms=dict(A=round(plan_a, 3), B=round(plan_b, 3)))
+    cb = report("op_composed_backward", d, timed_op(c_backward))
+    # the composed dQ and dK leave out the final factor scale
+    agree = dict(Z=rel(Z.to_host(), Zc.to_host()), dV=rel(dV.to_host(), dVc.to_host()),
+                 dQ=rel(dQ.to_host(), scale * dQc.to_host()), dK=rel(dK.to_host(), scale * dKc.to_host()))
+    print(json.dumps(dict(d=d, forward_fused_over_composed=round(fwd / cf, 3), backward_fused_over_composed=round(bwd / cb, 3),
+                          max_rel_difference=agree, agree_within_1e_12=all(v < 1e-12 for v in agree.values()))), flush=True)
+    del alg
+
+
+for d in widths:
+    alg = D.Algorithm(alg_name, S, d, 1)
+    kernels(alg, d)
+    del alg
+    torch.cuda.empty_cache()
+    ops(d)
+D.world_finalize()
