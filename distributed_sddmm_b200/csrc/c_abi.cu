@@ -1,8 +1,6 @@
 // c_abi.cu -- extern "C" layer of libhnh_b200.so: argument validation, kernel selection
 // and launch for the entry points declared in include/hnh_b200.h.
-#include "hnh_b200.h"
 #include "kernels.cuh"
-#include "launch.h"
 
 #include <atomic>
 #include <cstdio>
@@ -55,120 +53,115 @@ int device_sm_count(int *out) {
     return HNH_OK;
 }
 
-// Grid for a grid-stride kernel: a whole number of resident CTAs per SM (multiple of the SM
-// count), never more CTAs than there are work items.
-template <typename K>
-int grid_for(K kernel, int block, int64_t work_items_per_block_capacity, int64_t work_items,
-             int *grid_out) {
-    int sms = 0;
-    int rc = device_sm_count(&sms);
-    if (rc) return rc;
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, block, 0);
-    if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
-    if (occ < 1) occ = 1;
-    int64_t need = (work_items + work_items_per_block_capacity - 1) / work_items_per_block_capacity;
-    int64_t cap = (int64_t)sms * occ;
-    int64_t g = need < cap ? need : cap;
-    if (g < 1) g = 1;
-    *grid_out = (int)g;
-    return HNH_OK;
+// ------------------------------------------------------------------ K4 + row algebra -----
+__global__ void fill_kernel(double *__restrict__ dst, int64_t n, double value) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        dst[i] = value;
 }
 
-static inline bool aligned(const void *p, size_t a) { return ((uintptr_t)p & (a - 1)) == 0; }
-
-constexpr int kBlock = 256;
-
-// ---- templated launchers ------------------------------------------------------------------
-template <int R, int G, int VW, int UN>
-int launch_sddmm(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows,
-                 const double *X, const double *Y, bool beta0, const double *scale, double *scaled_out, bool sv,
-                 cudaStream_t st) {
-    int grid;
-    auto k = beta0 ? sddmm_row_kernel<R, G, VW, UN, true> : sddmm_row_kernel<R, G, VW, UN, false>;
-    int rc = grid_for(k, kBlock, kBlock / G, rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y, scale, scaled_out, sv);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "sddmm_row_kernel launch");
-}
-template <int R, int G, int VW, int UN>
-int launch_spmm(const int64_t *rowStart, const int64_t *col_idx, const double *values,
-                int64_t rows, const double *X, double *Y, bool beta0, cudaStream_t st) {
-    int grid;
-    auto k = beta0 ? spmm_row_kernel<R, G, VW, UN, true> : spmm_row_kernel<R, G, VW, UN, false>;
-    int rc = grid_for(k, kBlock, kBlock / G, rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "spmm_row_kernel launch");
-}
-template <int R, int G, int VW, int UN>
-int launch_fused(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows,
-                 const double *X, const double *Y, double *Out, bool bv, bool bo, cudaStream_t st,
-                 const double *scale = nullptr, double *scaled_out = nullptr) {
-    int grid;
-    auto k = bv ? (bo ? fused_row_kernel<R, G, VW, UN, true, true> : fused_row_kernel<R, G, VW, UN, true, false>)
-                : (bo ? fused_row_kernel<R, G, VW, UN, false, true> : fused_row_kernel<R, G, VW, UN, false, false>);
-    if (scale)  // scaled epilogue: first-visit form only (hnh_fused_scaled_f64 checks)
-        k = bo ? fused_row_kernel<R, G, VW, UN, true, true, true> : fused_row_kernel<R, G, VW, UN, true, false, true>;
-    int rc = grid_for(k, kBlock, kBlock / G, rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y, Out, scale, scaled_out);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "fused_row_kernel launch");
-}
-template <int R, int G, int VW, int UN>
-int launch_sddmm_coo(const int64_t *row_idx, const int64_t *col_idx, double *values,
-                     int64_t nnz, const double *X, const double *Y, cudaStream_t st) {
-    int grid;
-    auto k = sddmm_coo_kernel<R, G, VW, UN>;
-    int rc = grid_for(k, kBlock, (int64_t)(kBlock / G) * G, nnz, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(row_idx, col_idx, values, nnz, X, Y);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "sddmm_coo_kernel launch");
+// uniform(-1, 1) from a counter-based hash of (seed, i): Eigen's setRandom() stand-in
+__global__ void random_uniform_kernel(double *__restrict__ dst, int64_t n, uint64_t seed) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        uint64_t z = seed + (uint64_t)i * 0x9E3779B97F4A7C15ull + 0x9E3779B97F4A7C15ull;
+        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+        z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+        z ^= z >> 31;
+        dst[i] = (double)(z >> 11) * (2.0 / 9007199254740992.0) - 1.0;
+    }
 }
 
-// ---- small-r ("split") launchers: G = GK*GN lanes per row ----------------------------------
-template <int R, int GK, int GN, int VW, int UN>
-int launch_sddmm_split(const int64_t *rowStart, const int64_t *col_idx, double *values,
-                       int64_t rows, const double *X, const double *Y, bool beta0, const double *scale, double *scaled_out,
-                       bool sv, cudaStream_t st) {
-    int grid;
-    auto k = beta0 ? sddmm_split_kernel<R, GK, GN, VW, UN, true> : sddmm_split_kernel<R, GK, GN, VW, UN, false>;
-    int rc = grid_for(k, kBlock, kBlock / (GK * GN), rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y, scale, scaled_out, sv);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "sddmm_split_kernel launch");
+__global__ void hadamard_kernel(double *__restrict__ dst, const double *__restrict__ a,
+                                const double *__restrict__ b, int64_t n) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        dst[i] = a[i] * b[i];
 }
-template <int R, int GK, int GN, int VW, int UN>
-int launch_spmm_split(const int64_t *rowStart, const int64_t *col_idx, const double *values,
-                      int64_t rows, const double *X, double *Y, bool beta0, cudaStream_t st) {
-    int grid;
-    auto k = beta0 ? spmm_split_kernel<R, GK, GN, VW, UN, true> : spmm_split_kernel<R, GK, GN, VW, UN, false>;
-    int rc = grid_for(k, kBlock, kBlock / (GK * GN), rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "spmm_split_kernel launch");
+
+__global__ void expand_row_idx_kernel(const int64_t *__restrict__ rowStart, int64_t rows,
+                                      int64_t *__restrict__ row_idx) {
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows;
+         row += nwarps) {
+        const int64_t s = rowStart[row], e = rowStart[row + 1];
+        for (int64_t j = s + lane; j < e; j += 32) row_idx[j] = row;
+    }
 }
-template <int R, int GK, int GN, int VW, int UN>
-int launch_fused_split(const int64_t *rowStart, const int64_t *col_idx, double *values,
-                       int64_t rows, const double *X, const double *Y, double *Out, bool bv, bool bo,
-                       cudaStream_t st, const double *scale = nullptr, double *scaled_out = nullptr) {
-    int grid;
-    auto k = bv ? (bo ? fused_split_kernel<R, GK, GN, VW, UN, true, true> : fused_split_kernel<R, GK, GN, VW, UN, true, false>)
-                : (bo ? fused_split_kernel<R, GK, GN, VW, UN, false, true> : fused_split_kernel<R, GK, GN, VW, UN, false, false>);
-    if (scale)
-        k = bo ? fused_split_kernel<R, GK, GN, VW, UN, true, true, true> : fused_split_kernel<R, GK, GN, VW, UN, true, false, true>;
-    int rc = grid_for(k, kBlock, kBlock / (GK * GN), rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y, Out, scale, scaled_out);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "fused_split_kernel launch");
+
+__global__ void batch_dot_kernel(double *__restrict__ out, const double *__restrict__ A,
+                                 const double *__restrict__ B, int64_t rows, int r) {
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows;
+         row += nwarps) {
+        double d = 0.0;
+        for (int k = lane; k < r; k += 32)
+            d = fma(A[row * (int64_t)r + k], B[row * (int64_t)r + k], d);
+        d = group_allreduce<32>(d, 0xffffffffu);
+        if (lane == 0) out[row] = d;
+    }
 }
+
+__global__ void row_axpy_kernel(double *D, const double *C, double alpha,
+                                const double *__restrict__ s, const double *M, int64_t rows,
+                                int r) {
+    const int64_t n = rows * (int64_t)r;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const double sc = s ? s[i / r] : 1.0;
+        D[i] = (C ? C[i] : 0.0) + alpha * sc * M[i];
+    }
+}
+
+__global__ void vec_quotient_kernel(double *out, const double *a, double ca, const double *b,
+                                    double cb, int64_t n) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        out[i] = b ? (a[i] + ca) / (b[i] + cb) : (a[i] + ca);
+}
+
+__global__ void axpby_kernel(double *dst, double alpha, const double *x, double beta,
+                             const double *y, int64_t n) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        dst[i] = alpha * x[i] + (y ? beta * y[i] : 0.0);
+}
+
+// Deterministic two-pass sum of squares (fingerprints and residuals must be bit-stable run to run): pass 1 leaves
+// one partial per CTA (fixed grid-stride assignment, fixed shuffle tree), pass 2 -- one CTA -- adds the partials
+// in a fixed order.  No atomics.
+__global__ void squared_norm_partial_kernel(double *__restrict__ partial, const double *__restrict__ x, int64_t n) {
+    __shared__ double warp_sums[8];
+    double acc = 0.0;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        acc = fma(x[i], x[i], acc);
+    acc = group_allreduce<32>(acc, 0xffffffffu);
+    if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += warp_sums[w];
+        partial[blockIdx.x] = t;
+    }
+}
+
+__global__ void sum_partials_kernel(double *__restrict__ out, const double *__restrict__ partial, int n) {
+    __shared__ double warp_sums[8];
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) acc += partial[i];
+    acc = group_allreduce<32>(acc, 0xffffffffu);
+    if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += warp_sums[w];
+        *out = t;
+    }
+}
+
 
 // Narrow factors (r <= split_max_r()) use the split kernels.  Shape table:
 // R -> (GK lanes across r, GN lanes across the row's nonzeros, VW, UN).
@@ -190,38 +183,11 @@ static int split_max_r() {
     return v;
 }
 
-// ---- TMA-staged launchers (HNH_FLAG_TMA_STAGE; r in {128, 256}, 16-byte aligned operands) -----
-template <int R, bool FUSED>
-int launch_tma(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows, const double *X,
-               const double *Y, double *Out, bool bv, bool bo, cudaStream_t st, const double *scale = nullptr,
-               double *scaled_out = nullptr, bool sv = false) {
-    int grid;
-    auto k = bv ? (bo ? tma_row_kernel<R, 4, FUSED, true, true> : tma_row_kernel<R, 4, FUSED, true, false>)
-                : (bo ? tma_row_kernel<R, 4, FUSED, false, true> : tma_row_kernel<R, 4, FUSED, false, false>);
-    int rc = grid_for(k, kBlock, 8, rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y, Out, scale, scaled_out, sv);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "tma_row_kernel launch");
-}
+// ---- TMA-staged kernels (HNH_FLAG_TMA_STAGE / HNH_FLAG_TMA_WARP; r in {128, 256}, 16-byte aligned operands) -----------
 // Default choice between the TMA-staged and the direct-load row kernels: TMA staging for SDDMM at
 // r = 128 and 256 and for the overwriting fused kernel at r = 256; the direct kernel for the fused
 // kernel at r = 128, where the per-tile barrier makes the 8 warps of a CTA wait for the longest of
 // their rows.  HNH_TMA=0 / 1 forces one or the other everywhere.
-template <int R, bool FUSED>
-int launch_tma_warp(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows, const double *X,
-                    const double *Y, double *Out, bool bv, bool bo, cudaStream_t st, const double *scale = nullptr,
-                    double *scaled_out = nullptr, bool sv = false) {
-    int grid;
-    auto k = bv ? (bo ? tma_warp_kernel<R, 4, FUSED, true, true> : tma_warp_kernel<R, 4, FUSED, true, false>)
-                : (bo ? tma_warp_kernel<R, 4, FUSED, false, true> : tma_warp_kernel<R, 4, FUSED, false, false>);
-    int rc = grid_for(k, kBlock, 8, rows, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, Y, Out, scale, scaled_out, sv);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "tma_warp_kernel launch");
-}
-
 static bool tma_default(bool fused, int r, bool overwrite_out) {
     static int v = -2;
     if (v == -2) {
@@ -232,19 +198,15 @@ static bool tma_default(bool fused, int r, bool overwrite_out) {
     return fused ? (r == 256 && overwrite_out) : true;
 }
 
-// Shape table: R -> (G lanes per row, VW doubles per vector load, UN rows in flight).
-// 128-bit loads (VW=2, the widest on sm_90) need 16-byte aligned operand rows.
-#define HNH_DISPATCH_R(r, CALL, FALLBACK)     \
-    switch (r) {                              \
-        case 4:   CALL(4, 2, 2, 2); break;    \
-        case 8:   CALL(8, 4, 2, 4); break;    \
-        case 16:  CALL(16, 8, 2, 4); break;   \
-        case 32:  CALL(32, 16, 2, 4); break;  \
-        case 64:  CALL(64, 32, 2, 4); break;  \
-        case 128: CALL(128, 32, 2, 4); break; \
-        case 256: CALL(256, 32, 2, 2); break; \
-        default: FALLBACK; break;             \
-    }
+// the tile-staged (tma_row_kernel) or per-warp (tma_warp_kernel) instantiation for the overwrite flags
+template <int R, bool FUSED>
+auto tma_kernel(bool per_warp, bool bv, bool bo) {
+    if (per_warp)
+        return bv ? (bo ? tma_warp_kernel<R, 4, FUSED, true, true> : tma_warp_kernel<R, 4, FUSED, true, false>)
+                  : (bo ? tma_warp_kernel<R, 4, FUSED, false, true> : tma_warp_kernel<R, 4, FUSED, false, false>);
+    return bv ? (bo ? tma_row_kernel<R, 4, FUSED, true, true> : tma_row_kernel<R, 4, FUSED, true, false>)
+              : (bo ? tma_row_kernel<R, 4, FUSED, false, true> : tma_row_kernel<R, 4, FUSED, false, false>);
+}
 
 static int validate_common(const void *a, const void *b, const void *c, int64_t rows,
                            int64_t nnz, int r, const char *who) {
@@ -280,25 +242,12 @@ int hnh_sddmm_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
     if (v == 1) return HNH_OK;
     if (!X || !Y) return set_error(HNH_E_INVALID, "hnh_sddmm_f64: null dense operand");
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = HNH_OK;
-    bool beta0 = (flags & HNH_FLAG_BETA0) != 0;
-    const bool a16 = aligned(X, 16) && aligned(Y, 16);
-#define S4(R, G, VW, UN) rc = launch_sddmm<R, G, VW, UN>(rowStart, col_idx, values, rows, X, Y, beta0, scale, scaled_out, sv, st)
-#define SGEN                                                                                 \
-    {                                                                                        \
-        int grid;                                                                            \
-        rc = grid_for(sddmm_generic_kernel, kBlock, kBlock / 32, rows, &grid);               \
-        if (!rc) {                                                                           \
-            sddmm_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, \
-                                                          Y, r);                             \
-            count_launch(1);                                                                 \
-            rc = check_cuda(cudaGetLastError(), "sddmm_generic_kernel launch");              \
-        }                                                                                    \
-    }
-    const bool table_r = r == 4 || r == 8 || r == 16 || r == 32 || r == 64 || r == 128 || r == 256;
+    int grid = 0, rc = HNH_OK;
+    const bool beta0 = (flags & HNH_FLAG_BETA0) != 0;
+    const bool generic = (flags & HNH_FLAG_FORCE_GENERIC) || !aligned16(X) || !aligned16(Y) || !table_width(r);
     // The epilogue form needs a table kernel and distinct arrays (scale is read through the read-only path); otherwise
     // the product is one more elementwise pass after the plain SDDMM.
-    if (scale && ((flags & HNH_FLAG_FORCE_GENERIC) || !a16 || !table_r || (const double *)scaled_out == scale || values == scale)) {
+    if (scale && (generic || (const double *)scaled_out == scale || values == scale)) {
         rc = hnh_sddmm_scaled_f64(rowStart, col_idx, values, rows, nnz, X, Y, r, flags & ~HNH_FLAG_SCALE_VALUES, nullptr, nullptr, stream);
         if (rc) return rc;
         if (scaled_out && !(flags & HNH_FLAG_SCALE_VALUES)) return hnh_hadamard_f64(scaled_out, scale, values, nnz, stream);
@@ -309,32 +258,45 @@ int hnh_sddmm_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
                           "cudaMemcpyAsync");
     }
     const bool sv = (flags & HNH_FLAG_SCALE_VALUES) != 0;
-    if ((flags & HNH_FLAG_TMA_WARP) && a16 && (r == 128 || r == 256) && !(flags & HNH_FLAG_FORCE_GENERIC)) {
-        return r == 128 ? launch_tma_warp<128, false>(rowStart, col_idx, values, rows, X, Y, nullptr, beta0, false, st, scale, scaled_out, sv)
-                        : launch_tma_warp<256, false>(rowStart, col_idx, values, rows, X, Y, nullptr, beta0, false, st, scale, scaled_out, sv);
+    const bool warp = (flags & HNH_FLAG_TMA_WARP) != 0;
+    if (!generic && (r == 128 || r == 256) &&
+        (warp || (flags & HNH_FLAG_TMA_STAGE) || (tma_default(false, r, beta0) && !(flags & HNH_FLAG_FORCE_DIRECT)))) {
+        auto k = r == 128 ? tma_kernel<128, false>(warp, beta0, false) : tma_kernel<256, false>(warp, beta0, false);
+        rc = grid_for(k, rows, 8, &grid);
+        return rc ? rc : launch(k, grid, kBlock, st, warp ? "tma_warp_kernel" : "tma_row_kernel", rowStart, col_idx, values, rows,
+                                X, Y, nullptr, scale, scaled_out, sv);
     }
-    if (((flags & HNH_FLAG_TMA_STAGE) || (tma_default(false, r, beta0) && !(flags & HNH_FLAG_FORCE_DIRECT))) && a16 &&
-        (r == 128 || r == 256) && !(flags & HNH_FLAG_FORCE_GENERIC)) {
-        return r == 128 ? launch_tma<128, false>(rowStart, col_idx, values, rows, X, Y, nullptr, beta0, false, st, scale, scaled_out, sv)
-                        : launch_tma<256, false>(rowStart, col_idx, values, rows, X, Y, nullptr, beta0, false, st, scale, scaled_out, sv);
-    }
-    if ((flags & HNH_FLAG_FORCE_GENERIC) || !a16 || !table_r) {
+    if (generic) {
         if (beta0) {  // the any-r kernel accumulates: clear first
             rc = check_cuda(cudaMemsetAsync(values, 0, sizeof(double) * (size_t)nnz, st), "cudaMemsetAsync");
             if (rc) return rc;
         }
-        SGEN
-    } else if (r <= split_max_r() && r <= 32) {
-#define SP(R, GK, GN, VW, UN) \
-    rc = launch_sddmm_split<R, GK, GN, VW, UN>(rowStart, col_idx, values, rows, X, Y, beta0, scale, scaled_out, sv, st)
+        rc = grid_for(sddmm_generic_kernel, rows, kBlock / 32, &grid);
+        return rc ? rc : launch(sddmm_generic_kernel, grid, kBlock, st, "sddmm_generic_kernel", rowStart, col_idx, values, rows, X, Y, r);
+    }
+    decltype(&sddmm_row_kernel<4, 2, 2, 2, true>) k = nullptr;
+    int64_t per_cta = 0;
+    const char *name = "sddmm_split_kernel";
+    if (r <= split_max_r() && r <= 32) {
+#define SP(R, GK, GN, VW, UN)                                                                                    \
+    {                                                                                                            \
+        k = beta0 ? sddmm_split_kernel<R, GK, GN, VW, UN, true> : sddmm_split_kernel<R, GK, GN, VW, UN, false>;  \
+        per_cta = kBlock / (GK * GN);                                                                            \
+    }
         HNH_DISPATCH_SPLIT(r, SP)
 #undef SP
     } else {
-        HNH_DISPATCH_R(r, S4, SGEN)
+        name = "sddmm_row_kernel";
+#define S4(R, G, VW, UN)                                                                         \
+    {                                                                                            \
+        k = beta0 ? sddmm_row_kernel<R, G, VW, UN, true> : sddmm_row_kernel<R, G, VW, UN, false>; \
+        per_cta = kBlock / G;                                                                    \
     }
+        HNH_DISPATCH_R(r, S4, )
 #undef S4
-#undef SGEN
-    return rc;
+    }
+    rc = grid_for(k, rows, per_cta, &grid);
+    return rc ? rc : launch(k, grid, kBlock, st, name, rowStart, col_idx, values, rows, X, Y, scale, scaled_out, sv);
 }
 
 int hnh_sddmm_f64(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows,
@@ -350,21 +312,21 @@ int hnh_sddmm_coo_f64(const int64_t *row_idx, const int64_t *col_idx, double *va
     if (v == 1) return HNH_OK;
     if (!X || !Y) return set_error(HNH_E_INVALID, "hnh_sddmm_coo_f64: null dense operand");
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = HNH_OK;
-    const bool a16 = aligned(X, 16) && aligned(Y, 16);
-#define S4(R, G, VW, UN) rc = launch_sddmm_coo<R, G, VW, (UN > 2 ? 2 : UN)>(row_idx, col_idx, values, nnz, X, Y, st)
-#define SGEN                                                                                    \
-    {                                                                                           \
-        int grid;                                                                               \
-        rc = grid_for(sddmm_coo_generic_kernel, kBlock, kBlock / 32, nnz, &grid);               \
-        if (!rc) {                                                                              \
-            sddmm_coo_generic_kernel<<<grid, kBlock, 0, st>>>(row_idx, col_idx, values, nnz, X, \
-                                                              Y, r);                            \
-            count_launch(1);                                                                    \
-            rc = check_cuda(cudaGetLastError(), "sddmm_coo_generic_kernel launch");             \
-        }                                                                                       \
+    int grid = 0, rc = HNH_OK;
+#define S4(R, G, VW, UN)                                                                                     \
+    {                                                                                                        \
+        auto k = sddmm_coo_kernel<R, G, VW, (UN > 2 ? 2 : UN)>;                                              \
+        rc = grid_for(k, nnz, (int64_t)(kBlock / G) * G, &grid);                                             \
+        if (!rc) rc = launch(k, grid, kBlock, st, "sddmm_coo_kernel", row_idx, col_idx, values, nnz, X, Y);  \
     }
-    if ((flags & HNH_FLAG_FORCE_GENERIC) || !a16) {
+#define SGEN                                                                                                 \
+    {                                                                                                        \
+        rc = grid_for(sddmm_coo_generic_kernel, nnz, kBlock / 32, &grid);                                    \
+        if (!rc)                                                                                             \
+            rc = launch(sddmm_coo_generic_kernel, grid, kBlock, st, "sddmm_coo_generic_kernel", row_idx,     \
+                        col_idx, values, nnz, X, Y, r);                                                      \
+    }
+    if ((flags & HNH_FLAG_FORCE_GENERIC) || !aligned16(X) || !aligned16(Y)) {
         SGEN
     } else {
         HNH_DISPATCH_R(r, S4, SGEN)
@@ -389,39 +351,39 @@ int hnh_spmm_f64(const int64_t *rowStart, const int64_t *col_idx, const double *
         return HNH_OK;
     }
     if (!X || !Y) return set_error(HNH_E_INVALID, "hnh_spmm_f64: null dense operand");
-    int rc = HNH_OK;
-    bool beta0 = (flags & HNH_FLAG_BETA0) != 0;
-    const bool a16 = aligned(X, 16) && aligned(Y, 16);
-#define S4(R, G, VW, UN) rc = launch_spmm<R, G, VW, UN>(rowStart, col_idx, values, rows, X, Y, beta0, st)
-#define SGEN                                                                                \
-    {                                                                                       \
-        int grid;                                                                           \
-        rc = grid_for(spmm_generic_kernel, kBlock, kBlock / 32, rows, &grid);               \
-        if (!rc) {                                                                          \
-            spmm_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, \
-                                                         Y, r);                             \
-            count_launch(1);                                                                \
-            rc = check_cuda(cudaGetLastError(), "spmm_generic_kernel launch");              \
-        }                                                                                   \
-    }
-    const bool table_r = r == 4 || r == 8 || r == 16 || r == 32 || r == 64 || r == 128 || r == 256;
-    if ((flags & HNH_FLAG_FORCE_GENERIC) || !a16 || !table_r) {
+    int grid = 0, rc = HNH_OK;
+    const bool beta0 = (flags & HNH_FLAG_BETA0) != 0;
+    if ((flags & HNH_FLAG_FORCE_GENERIC) || !aligned16(X) || !aligned16(Y) || !table_width(r)) {
         if (beta0) {
             rc = check_cuda(cudaMemsetAsync(Y, 0, sizeof(double) * (size_t)rows * r, st), "cudaMemsetAsync");
             if (rc) return rc;
         }
-        SGEN
-    } else if (r <= split_max_r() && r <= 32) {
-#define SP(R, GK, GN, VW, UN) \
-    rc = launch_spmm_split<R, GK, GN, VW, UN>(rowStart, col_idx, values, rows, X, Y, beta0, st)
+        rc = grid_for(spmm_generic_kernel, rows, kBlock / 32, &grid);
+        return rc ? rc : launch(spmm_generic_kernel, grid, kBlock, st, "spmm_generic_kernel", rowStart, col_idx, values, rows, X, Y, r);
+    }
+    decltype(&spmm_row_kernel<4, 2, 2, 2, true>) k = nullptr;
+    int64_t per_cta = 0;
+    const char *name = "spmm_split_kernel";
+    if (r <= split_max_r() && r <= 32) {
+#define SP(R, GK, GN, VW, UN)                                                                                  \
+    {                                                                                                          \
+        k = beta0 ? spmm_split_kernel<R, GK, GN, VW, UN, true> : spmm_split_kernel<R, GK, GN, VW, UN, false>;  \
+        per_cta = kBlock / (GK * GN);                                                                          \
+    }
         HNH_DISPATCH_SPLIT(r, SP)
 #undef SP
     } else {
-        HNH_DISPATCH_R(r, S4, SGEN)
+        name = "spmm_row_kernel";
+#define S4(R, G, VW, UN)                                                                       \
+    {                                                                                          \
+        k = beta0 ? spmm_row_kernel<R, G, VW, UN, true> : spmm_row_kernel<R, G, VW, UN, false>; \
+        per_cta = kBlock / G;                                                                  \
     }
+        HNH_DISPATCH_R(r, S4, )
 #undef S4
-#undef SGEN
-    return rc;
+    }
+    rc = grid_for(k, rows, per_cta, &grid);
+    return rc ? rc : launch(k, grid, kBlock, st, name, rowStart, col_idx, values, rows, X, Y);
 }
 
 int hnh_fused_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows,
@@ -440,30 +402,17 @@ int hnh_fused_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
         return HNH_OK;
     }
     if (!X || !Y || !Out) return set_error(HNH_E_INVALID, "hnh_fused_f64: null dense operand");
-    int rc = HNH_OK;
+    int grid = 0, rc = HNH_OK;
     const bool bv = (flags & (HNH_FLAG_BETA0 | HNH_FLAG_BETA0_VALUES)) != 0;
     const bool bo = (flags & (HNH_FLAG_BETA0 | HNH_FLAG_BETA0_OUT)) != 0;
     if (X == Out && !bo)
         return set_error(HNH_E_INVALID, "hnh_fused_f64: Out may alias X only when Out is overwritten (BETA0_OUT)");
-    const bool a16 = aligned(X, 16) && aligned(Y, 16) && aligned(Out, 16);
-#define S4(R, G, VW, UN) \
-    rc = launch_fused<R, G, VW, UN>(rowStart, col_idx, values, rows, X, Y, Out, bv, bo, st, scale, scaled_out)
-#define SGEN                                                                                 \
-    {                                                                                        \
-        int grid;                                                                            \
-        rc = grid_for(fused_generic_kernel, kBlock, kBlock / 32, rows, &grid);               \
-        if (!rc) {                                                                           \
-            fused_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, values, rows, X, \
-                                                          Y, Out, r);                        \
-            count_launch(1);                                                                 \
-            rc = check_cuda(cudaGetLastError(), "fused_generic_kernel launch");              \
-        }                                                                                    \
-    }
-    const bool table_r = r == 4 || r == 8 || r == 16 || r == 32 || r == 64 || r == 128 || r == 256;
+    const bool generic =
+        (flags & HNH_FLAG_FORCE_GENERIC) || !aligned16(X) || !aligned16(Y) || !aligned16(Out) || !table_width(r);
     if (scale) {
         // the scaled epilogue exists in the first-visit form of the direct-load table kernels only
         if (!bv) return set_error(HNH_E_INVALID, "hnh_fused_scaled_f64: scale needs HNH_FLAG_BETA0_VALUES");
-        if (!a16 || !table_r || (flags & HNH_FLAG_FORCE_GENERIC))
+        if (generic)
             return set_error(HNH_E_INVALID, "hnh_fused_scaled_f64: scale needs a table width (4..256, power of two) and 16-byte "
                                             "aligned operands");
         if (values == scale || (const double *)scaled_out == scale)
@@ -472,34 +421,51 @@ int hnh_fused_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
     }
     // in place (Out == X) is not offered with TMA staging: the next tile of X is prefetched while
     // the current one is still being written
-    if ((flags & HNH_FLAG_TMA_WARP) && a16 && (r == 128 || r == 256) && X != Out && !(flags & HNH_FLAG_FORCE_GENERIC)) {
-        return r == 128 ? launch_tma_warp<128, true>(rowStart, col_idx, values, rows, X, Y, Out, bv, bo, st)
-                        : launch_tma_warp<256, true>(rowStart, col_idx, values, rows, X, Y, Out, bv, bo, st);
+    const bool warp = (flags & HNH_FLAG_TMA_WARP) != 0;
+    if (!generic && (r == 128 || r == 256) && X != Out &&
+        (warp || (flags & HNH_FLAG_TMA_STAGE) || (tma_default(true, r, bo) && !(flags & HNH_FLAG_FORCE_DIRECT)))) {
+        auto k = r == 128 ? tma_kernel<128, true>(warp, bv, bo) : tma_kernel<256, true>(warp, bv, bo);
+        rc = grid_for(k, rows, 8, &grid);
+        return rc ? rc : launch(k, grid, kBlock, st, warp ? "tma_warp_kernel" : "tma_row_kernel", rowStart, col_idx, values, rows,
+                                X, Y, Out, nullptr, nullptr, false);
     }
-    if (((flags & HNH_FLAG_TMA_STAGE) || (tma_default(true, r, bo) && !(flags & HNH_FLAG_FORCE_DIRECT))) && a16 &&
-        (r == 128 || r == 256) && X != Out && !(flags & HNH_FLAG_FORCE_GENERIC)) {
-        return r == 128 ? launch_tma<128, true>(rowStart, col_idx, values, rows, X, Y, Out, bv, bo, st)
-                        : launch_tma<256, true>(rowStart, col_idx, values, rows, X, Y, Out, bv, bo, st);
-    }
-    if ((flags & HNH_FLAG_FORCE_GENERIC) || !a16 || !table_r) {
+    if (generic) {
         if (X == Out)
             return set_error(HNH_E_INVALID, "hnh_fused_f64: in-place (Out == X) needs a table r "
                                             "(4..256, power of two) and 16-byte aligned operands");
         if (bv) rc = check_cuda(cudaMemsetAsync(values, 0, sizeof(double) * (size_t)nnz, st), "cudaMemsetAsync");
         if (!rc && bo) rc = check_cuda(cudaMemsetAsync(Out, 0, sizeof(double) * (size_t)rows * r, st), "cudaMemsetAsync");
-        if (rc) return rc;
-        SGEN
-    } else if (r <= split_max_r() && r <= 32) {
-#define SP(R, GK, GN, VW, UN) \
-    rc = launch_fused_split<R, GK, GN, VW, UN>(rowStart, col_idx, values, rows, X, Y, Out, bv, bo, st, scale, scaled_out)
+        if (!rc) rc = grid_for(fused_generic_kernel, rows, kBlock / 32, &grid);
+        return rc ? rc : launch(fused_generic_kernel, grid, kBlock, st, "fused_generic_kernel", rowStart, col_idx, values, rows, X, Y, Out, r);
+    }
+    // the scaled epilogue is a first-visit (BETA0_VALUES) form
+    decltype(&fused_row_kernel<4, 2, 2, 2, true, true>) k = nullptr;
+    int64_t per_cta = 0;
+    const char *name = "fused_split_kernel";
+    if (r <= split_max_r() && r <= 32) {
+#define SP(R, GK, GN, VW, UN)                                                                                                \
+    {                                                                                                                        \
+        k = scale ? (bo ? fused_split_kernel<R, GK, GN, VW, UN, true, true, true> : fused_split_kernel<R, GK, GN, VW, UN, true, false, true>) \
+            : bv  ? (bo ? fused_split_kernel<R, GK, GN, VW, UN, true, true> : fused_split_kernel<R, GK, GN, VW, UN, true, false>)             \
+                  : (bo ? fused_split_kernel<R, GK, GN, VW, UN, false, true> : fused_split_kernel<R, GK, GN, VW, UN, false, false>);          \
+        per_cta = kBlock / (GK * GN);                                                                                        \
+    }
         HNH_DISPATCH_SPLIT(r, SP)
 #undef SP
     } else {
-        HNH_DISPATCH_R(r, S4, SGEN)
+        name = "fused_row_kernel";
+#define S4(R, G, VW, UN)                                                                                                     \
+    {                                                                                                                        \
+        k = scale ? (bo ? fused_row_kernel<R, G, VW, UN, true, true, true> : fused_row_kernel<R, G, VW, UN, true, false, true>)   \
+            : bv  ? (bo ? fused_row_kernel<R, G, VW, UN, true, true> : fused_row_kernel<R, G, VW, UN, true, false>)               \
+                  : (bo ? fused_row_kernel<R, G, VW, UN, false, true> : fused_row_kernel<R, G, VW, UN, false, false>);            \
+        per_cta = kBlock / G;                                                                                                \
     }
+        HNH_DISPATCH_R(r, S4, )
 #undef S4
-#undef SGEN
-    return rc;
+    }
+    rc = grid_for(k, rows, per_cta, &grid);
+    return rc ? rc : launch(k, grid, kBlock, st, name, rowStart, col_idx, values, rows, X, Y, Out, scale, scaled_out);
 }
 
 int hnh_fused_f64(const int64_t *rowStart, const int64_t *col_idx, double *values, int64_t rows,
@@ -508,35 +474,34 @@ int hnh_fused_f64(const int64_t *rowStart, const int64_t *col_idx, double *value
     return hnh_fused_scaled_f64(rowStart, col_idx, values, rows, nnz, X, Y, Out, r, flags, nullptr, nullptr, stream);
 }
 
-// ---- K4 + row algebra -----------------------------------------------------------------------
-#define HNH_ELEMENTWISE_LAUNCH(kernel, n, ...)                                       \
-    do {                                                                             \
-        if ((n) < 0) return set_error(HNH_E_INVALID, #kernel ": negative size");     \
-        if ((n) == 0) return HNH_OK;                                                 \
-        int grid;                                                                    \
-        int rc_ = grid_for(kernel, kBlock, kBlock * 4, (n), &grid);                  \
-        if (rc_) return rc_;                                                         \
-        kernel<<<grid, kBlock, 0, (cudaStream_t)stream>>>(__VA_ARGS__);              \
-        count_launch(1);                                                             \
-        return check_cuda(cudaGetLastError(), #kernel " launch");                    \
-    } while (0)
-
+// ---- K4 + row algebra: one thread per element, kBlock * 4 elements per CTA ------------------------------------------
 int hnh_fill_f64(double *dst, int64_t n, double value, void *stream) {
-    if (n > 0 && !dst) return set_error(HNH_E_INVALID, "hnh_fill_f64: null pointer");
-    if (n > 0 && value == 0.0)
-        return check_cuda(cudaMemsetAsync(dst, 0, sizeof(double) * (size_t)n, (cudaStream_t)stream),
-                          "cudaMemsetAsync");
-    HNH_ELEMENTWISE_LAUNCH(fill_kernel, n, dst, n, value);
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_fill_f64: negative size");
+    if (n == 0) return HNH_OK;
+    if (!dst) return set_error(HNH_E_INVALID, "hnh_fill_f64: null pointer");
+    if (value == 0.0)
+        return check_cuda(cudaMemsetAsync(dst, 0, sizeof(double) * (size_t)n, (cudaStream_t)stream), "cudaMemsetAsync");
+    int grid;
+    int rc = grid_for(fill_kernel, n, kBlock * 4, &grid);
+    return rc ? rc : launch(fill_kernel, grid, kBlock, (cudaStream_t)stream, "fill_kernel", dst, n, value);
 }
 
 int hnh_random_uniform_f64(double *dst, int64_t n, uint64_t seed, void *stream) {
-    if (n > 0 && !dst) return set_error(HNH_E_INVALID, "hnh_random_uniform_f64: null pointer");
-    HNH_ELEMENTWISE_LAUNCH(random_uniform_kernel, n, dst, n, seed);
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_random_uniform_f64: negative size");
+    if (n == 0) return HNH_OK;
+    if (!dst) return set_error(HNH_E_INVALID, "hnh_random_uniform_f64: null pointer");
+    int grid;
+    int rc = grid_for(random_uniform_kernel, n, kBlock * 4, &grid);
+    return rc ? rc : launch(random_uniform_kernel, grid, kBlock, (cudaStream_t)stream, "random_uniform_kernel", dst, n, seed);
 }
 
 int hnh_hadamard_f64(double *dst, const double *a, const double *b, int64_t n, void *stream) {
-    if (n > 0 && (!dst || !a || !b)) return set_error(HNH_E_INVALID, "hnh_hadamard_f64: null pointer");
-    HNH_ELEMENTWISE_LAUNCH(hadamard_kernel, n, dst, a, b, n);
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_hadamard_f64: negative size");
+    if (n == 0) return HNH_OK;
+    if (!dst || !a || !b) return set_error(HNH_E_INVALID, "hnh_hadamard_f64: null pointer");
+    int grid;
+    int rc = grid_for(hadamard_kernel, n, kBlock * 4, &grid);
+    return rc ? rc : launch(hadamard_kernel, grid, kBlock, (cudaStream_t)stream, "hadamard_kernel", dst, a, b, n);
 }
 
 int hnh_expand_row_idx(const int64_t *rowStart, int64_t rows, int64_t nnz, int64_t *row_idx,
@@ -545,11 +510,8 @@ int hnh_expand_row_idx(const int64_t *rowStart, int64_t rows, int64_t nnz, int64
     if (rows == 0 || nnz == 0) return HNH_OK;
     if (!rowStart || !row_idx) return set_error(HNH_E_INVALID, "hnh_expand_row_idx: null pointer");
     int grid;
-    int rc = grid_for(expand_row_idx_kernel, kBlock, kBlock / 32, rows, &grid);
-    if (rc) return rc;
-    expand_row_idx_kernel<<<grid, kBlock, 0, (cudaStream_t)stream>>>(rowStart, rows, row_idx);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "expand_row_idx_kernel launch");
+    int rc = grid_for(expand_row_idx_kernel, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(expand_row_idx_kernel, grid, kBlock, (cudaStream_t)stream, "expand_row_idx_kernel", rowStart, rows, row_idx);
 }
 
 int hnh_batch_dot_f64(double *out, const double *A, const double *B, int64_t rows, int r,
@@ -558,31 +520,39 @@ int hnh_batch_dot_f64(double *out, const double *A, const double *B, int64_t row
     if (rows == 0) return HNH_OK;
     if (!out || !A || !B) return set_error(HNH_E_INVALID, "hnh_batch_dot_f64: null pointer");
     int grid;
-    int rc = grid_for(batch_dot_kernel, kBlock, kBlock / 32, rows, &grid);
-    if (rc) return rc;
-    batch_dot_kernel<<<grid, kBlock, 0, (cudaStream_t)stream>>>(out, A, B, rows, r);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "batch_dot_kernel launch");
+    int rc = grid_for(batch_dot_kernel, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(batch_dot_kernel, grid, kBlock, (cudaStream_t)stream, "batch_dot_kernel", out, A, B, rows, r);
 }
 
 int hnh_row_axpy_f64(double *D, const double *C, double alpha, const double *s, const double *M,
                      int64_t rows, int r, void *stream) {
     if (rows < 0 || r <= 0) return set_error(HNH_E_INVALID, "hnh_row_axpy_f64: bad size");
     const int64_t n = rows * (int64_t)r;
-    if (n > 0 && (!D || !M)) return set_error(HNH_E_INVALID, "hnh_row_axpy_f64: null pointer");
-    HNH_ELEMENTWISE_LAUNCH(row_axpy_kernel, n, D, C, alpha, s, M, rows, r);
+    if (n == 0) return HNH_OK;
+    if (!D || !M) return set_error(HNH_E_INVALID, "hnh_row_axpy_f64: null pointer");
+    int grid;
+    int rc = grid_for(row_axpy_kernel, n, kBlock * 4, &grid);
+    return rc ? rc : launch(row_axpy_kernel, grid, kBlock, (cudaStream_t)stream, "row_axpy_kernel", D, C, alpha, s, M, rows, r);
 }
 
 int hnh_vec_quotient_f64(double *out, const double *a, double ca, const double *b, double cb,
                          int64_t n, void *stream) {
-    if (n > 0 && (!out || !a)) return set_error(HNH_E_INVALID, "hnh_vec_quotient_f64: null pointer");
-    HNH_ELEMENTWISE_LAUNCH(vec_quotient_kernel, n, out, a, ca, b, cb, n);
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_vec_quotient_f64: negative size");
+    if (n == 0) return HNH_OK;
+    if (!out || !a) return set_error(HNH_E_INVALID, "hnh_vec_quotient_f64: null pointer");
+    int grid;
+    int rc = grid_for(vec_quotient_kernel, n, kBlock * 4, &grid);
+    return rc ? rc : launch(vec_quotient_kernel, grid, kBlock, (cudaStream_t)stream, "vec_quotient_kernel", out, a, ca, b, cb, n);
 }
 
 int hnh_axpby_f64(double *dst, double alpha, const double *x, double beta, const double *y,
                   int64_t n, void *stream) {
-    if (n > 0 && (!dst || !x)) return set_error(HNH_E_INVALID, "hnh_axpby_f64: null pointer");
-    HNH_ELEMENTWISE_LAUNCH(axpby_kernel, n, dst, alpha, x, beta, y, n);
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_axpby_f64: negative size");
+    if (n == 0) return HNH_OK;
+    if (!dst || !x) return set_error(HNH_E_INVALID, "hnh_axpby_f64: null pointer");
+    int grid;
+    int rc = grid_for(axpby_kernel, n, kBlock * 4, &grid);
+    return rc ? rc : launch(axpby_kernel, grid, kBlock, (cudaStream_t)stream, "axpby_kernel", dst, alpha, x, beta, y, n);
 }
 
 int hnh_squared_norm_f64(double *out, const double *x, int64_t n, void *stream) {
@@ -592,16 +562,14 @@ int hnh_squared_norm_f64(double *out, const double *x, int64_t n, void *stream) 
     if (n == 0) return check_cuda(cudaMemsetAsync(out, 0, sizeof(double), st), "cudaMemsetAsync");
     if (!x) return set_error(HNH_E_INVALID, "hnh_squared_norm_f64: null pointer");
     int grid;
-    int rc = grid_for(squared_norm_partial_kernel, kBlock, kBlock * 4, n, &grid);
+    int rc = grid_for(squared_norm_partial_kernel, n, kBlock * 4, &grid);
     if (rc) return rc;
     // per-call scratch, stream-ordered: concurrent calls on different streams never share partials
     double *partial = nullptr;
     rc = check_cuda(cudaMallocAsync((void **)&partial, sizeof(double) * (size_t)grid, st), "cudaMallocAsync");
     if (rc) return rc;
-    squared_norm_partial_kernel<<<grid, kBlock, 0, st>>>(partial, x, n);
-    sum_partials_kernel<<<1, kBlock, 0, st>>>(out, partial, grid);
-    count_launch(2);
-    rc = check_cuda(cudaGetLastError(), "squared_norm launch");
+    rc = launch(squared_norm_partial_kernel, grid, kBlock, st, "squared_norm_partial_kernel", partial, x, n);
+    if (!rc) rc = launch(sum_partials_kernel, 1, kBlock, st, "sum_partials_kernel", out, partial, grid);
     cudaError_t e = cudaFreeAsync(partial, st);
     return rc ? rc : check_cuda(e, "cudaFreeAsync");
 }

@@ -6,18 +6,19 @@
 // with the host path; these entry points are the building blocks of a device-resident setup.
 #include <cub/cub.cuh>
 
-#include <algorithm>
-
-#include "hnh_b200.h"
 #include "launch.h"
 
 namespace {
 
+using hnh::bits_for;
 using hnh::check_cuda;
-using hnh::count_launch;
+using hnh::grid_for;
+using hnh::kBlock;
+using hnh::launch;
+using hnh::Scratch;
 using hnh::set_error;
 
-constexpr int kThreads = 256;
+constexpr int kCtasPerSm = 8;  // grid cap of every grid-stride kernel here
 constexpr int kMaxPerRow = 128;  // columns drawn per row that one thread sorts in local memory
 
 __host__ __device__ inline uint64_t mix64(uint64_t z) {
@@ -168,30 +169,6 @@ __global__ void lower_bounds_kernel(const K *__restrict__ key, int64_t n, uint64
     starts[k] = lo;
 }
 
-int grid_for(int64_t n) {
-    int sms = 132;
-    hnh::device_sm_count(&sms);
-    const int64_t want = (n + kThreads - 1) / kThreads;
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)sms * 8));
-}
-
-struct Scratch {  // cudaMalloc'ed temporaries of one call, released on every exit path
-    void *p[12] = {};
-    int n = 0;
-    cudaError_t get(void **out, size_t bytes) {
-        cudaError_t e = cudaMalloc(out, std::max<size_t>(bytes, 256));
-        if (e == cudaSuccess) p[n++] = *out;
-        return e;
-    }
-    ~Scratch() { for (int i = 0; i < n; i++) cudaFree(p[i]); }
-};
-
-int bits_for(uint64_t max_value) {
-    int b = 1;
-    while (b < 64 && (max_value >> b) != 0) b++;
-    return b;
-}
-
 }  // namespace
 
 extern "C" {
@@ -213,10 +190,10 @@ int64_t hnh_er_generate_device(int logM, int nnz_per_row, uint64_t seed, int64_t
     size_t tmp_bytes = 0;
     int rc = check_cuda(s.get((void **)&counts, sizeof(int64_t) * (size_t)(nrows + 1)), "cudaMalloc");
     if (!rc) rc = check_cuda(s.get((void **)&offsets, sizeof(int64_t) * (size_t)(nrows + 1)), "cudaMalloc");
-    if (rc) return rc;
-    er_count_kernel<<<grid_for(nrows), kThreads, 0, st>>>(seed, row_lo, nrows, nnz_per_row, mask, counts);
-    count_launch(1);
-    rc = check_cuda(cudaMemsetAsync(counts + nrows, 0, sizeof(int64_t), st), "cudaMemsetAsync");
+    int grid = 0;
+    if (!rc) rc = grid_for(er_count_kernel, nrows, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(er_count_kernel, grid, kBlock, st, "er_count_kernel", seed, row_lo, nrows, nnz_per_row, mask, counts);
+    if (!rc) rc = check_cuda(cudaMemsetAsync(counts + nrows, 0, sizeof(int64_t), st), "cudaMemsetAsync");
     if (rc) return rc;
     rc = check_cuda(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offsets, (int)(nrows + 1), st), "cub scan size");
     if (!rc) rc = check_cuda(s.get(&tmp, tmp_bytes), "cudaMalloc");
@@ -228,9 +205,8 @@ int64_t hnh_er_generate_device(int logM, int nnz_per_row, uint64_t seed, int64_t
     if (rc) return rc;
     if (total > capacity)
         return set_error(HNH_E_INVALID, "hnh_er_generate_device: capacity %lld < %lld", (long long)capacity, (long long)total);
-    er_write_kernel<<<grid_for(nrows), kThreads, 0, st>>>(seed, row_lo, nrows, nnz_per_row, mask, offsets, rows_out, cols_out, vals_out);
-    count_launch(1);
-    rc = check_cuda(cudaGetLastError(), "er_write_kernel launch");
+    rc = launch(er_write_kernel, grid, kBlock, st, "er_write_kernel", seed, row_lo, nrows, nnz_per_row, mask, offsets, rows_out, cols_out,
+                vals_out);
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");  // the scratch is freed on return
     return rc ? rc : total;
 }
@@ -256,9 +232,10 @@ int hnh_coo_to_csr_device(int64_t rows, int64_t cols, int64_t nnz, const uint64_
     if (!rc) rc = check_cuda(s.get((void **)&idx_sorted, sizeof(int64_t) * (size_t)nnz), "cudaMalloc");
     if (!rc) rc = check_cuda(s.get((void **)&bad, sizeof(int)), "cudaMalloc");
     if (!rc) rc = check_cuda(cudaMemsetAsync(bad, 0, sizeof(int), st), "cudaMemsetAsync");
+    int grid = 0;
+    if (!rc) rc = grid_for(csr_keys_kernel, nnz, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(csr_keys_kernel, grid, kBlock, st, "csr_keys_kernel", sr, sc, nnz, (uint64_t)out_rows, (uint64_t)out_cols, key, idx, bad);
     if (rc) return rc;
-    csr_keys_kernel<<<grid_for(nnz), kThreads, 0, st>>>(sr, sc, nnz, (uint64_t)out_rows, (uint64_t)out_cols, key, idx, bad);
-    count_launch(1);
     int host_bad = 0;
     rc = check_cuda(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");
@@ -272,11 +249,9 @@ int hnh_coo_to_csr_device(int64_t rows, int64_t cols, int64_t nnz, const uint64_
     if (!rc) rc = check_cuda(s.get(&tmp, tmp_bytes), "cudaMalloc");
     if (!rc) rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key, key_sorted, idx, idx_sorted, (int)nnz, 0, end_bit, st),
                              "cub sort");
-    if (rc) return rc;
-    csr_gather_kernel<<<grid_for(nnz), kThreads, 0, st>>>(key_sorted, idx_sorted, sc, v, nnz, col_idx, row_idx, values);
-    csr_row_start_kernel<<<grid_for(out_rows + 1), kThreads, 0, st>>>(key_sorted, nnz, out_rows, rowStart);
-    count_launch(2);
-    rc = check_cuda(cudaGetLastError(), "csr kernels launch");
+    if (!rc) rc = launch(csr_gather_kernel, grid, kBlock, st, "csr_gather_kernel", key_sorted, idx_sorted, sc, v, nnz, col_idx, row_idx, values);
+    if (!rc) rc = grid_for(csr_row_start_kernel, out_rows + 1, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(csr_row_start_kernel, grid, kBlock, st, "csr_row_start_kernel", key_sorted, nnz, out_rows, rowStart);
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");  // the scratch is freed on return
     return rc;
 }
@@ -310,22 +285,24 @@ int hnh_tuples_bucket_by_owner_device(const uint64_t *r, const uint64_t *c, cons
     if (!rc) rc = check_cuda(s.get((void **)&starts, sizeof(int64_t) * (size_t)(nbuckets + 1)), "cudaMalloc");
     if (!rc) rc = check_cuda(cudaMemcpyAsync(table, owner_table_host, tb, cudaMemcpyHostToDevice, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaMemsetAsync(bad, 0, sizeof(int), st), "cudaMemsetAsync");
+    int grid = 0;
+    if (!rc) rc = grid_for(tuple_owner_kernel, n, kBlock, &grid, kCtasPerSm);
+    if (!rc)
+        rc = launch(tuple_owner_kernel, grid, kBlock, st, "tuple_owner_kernel", r, c, n, transpose, (uint64_t)rows_in_block,
+                    (uint64_t)cols_in_block, table, table_rows, table_cols, owner, idx, bad);
     if (rc) return rc;
-    tuple_owner_kernel<<<grid_for(n), kThreads, 0, st>>>(r, c, n, transpose, (uint64_t)rows_in_block, (uint64_t)cols_in_block, table,
-                                                         table_rows, table_cols, owner, idx, bad);
-    count_launch(1);
     const int end_bit = bits_for((uint64_t)std::max(nbuckets - 1, 1));
     rc = check_cuda(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, owner, owner_sorted, idx, idx_sorted, (int)n, 0, end_bit, st),
                     "cub sort size");
     if (!rc) rc = check_cuda(s.get(&tmp, tmp_bytes), "cudaMalloc");
     if (!rc) rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, owner, owner_sorted, idx, idx_sorted, (int)n, 0, end_bit, st),
                              "cub sort");
-    if (rc) return rc;
-    tuple_gather_kernel<<<grid_for(n), kThreads, 0, st>>>(r, c, v, idx_sorted, n, transpose, r_out, c_out, v_out);
-    lower_bounds_kernel<unsigned><<<(nbuckets + 1 + kThreads - 1) / kThreads, kThreads, 0, st>>>(owner_sorted, n, 1, nbuckets, starts);
-    count_launch(2);
+    if (!rc) rc = launch(tuple_gather_kernel, grid, kBlock, st, "tuple_gather_kernel", r, c, v, idx_sorted, n, transpose, r_out, c_out, v_out);
+    if (!rc)
+        rc = launch(lower_bounds_kernel<unsigned>, (nbuckets + 1 + kBlock - 1) / kBlock, kBlock, st, "lower_bounds_kernel", owner_sorted, n,
+                    1, nbuckets, starts);
     int host_bad = 0;
-    rc = check_cuda(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
+    if (!rc) rc = check_cuda(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaMemcpyAsync(starts_host, starts, sizeof(int64_t) * (size_t)(nbuckets + 1), cudaMemcpyDeviceToHost, st),
                              "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");
@@ -362,15 +339,14 @@ int hnh_tuples_sort_colmajor_device(uint64_t *r, uint64_t *c, double *v, int64_t
     if (!rc) rc = check_cuda(s.get(&tmp, tmp_bytes), "cudaMalloc");
     if (rc) return rc;
     // LSD over the pair: stable by row first, then stable by column  =>  ordered by (column, row), ties in input order
-    iota_kernel<<<grid_for(n), kThreads, 0, st>>>(idx_a, n);
-    rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, r, key_b, idx_a, idx_b, (int)n, 0, bits_r, st), "cub sort (rows)");
-    if (rc) return rc;
-    key_gather_kernel<<<grid_for(n), kThreads, 0, st>>>(c, idx_b, n, key_a);
-    rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_a, key_b, idx_b, idx_a, (int)n, 0, bits_c, st), "cub sort (cols)");
-    if (rc) return rc;
-    tuple_gather_kernel<<<grid_for(n), kThreads, 0, st>>>(r, c, v, idx_a, n, 0, r2, c2, v2);
-    count_launch(3);
-    rc = check_cuda(cudaMemcpyAsync(r, r2, b8, cudaMemcpyDeviceToDevice, st), "cudaMemcpyAsync");
+    int grid = 0;
+    rc = grid_for(iota_kernel, n, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(iota_kernel, grid, kBlock, st, "iota_kernel", idx_a, n);
+    if (!rc) rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, r, key_b, idx_a, idx_b, (int)n, 0, bits_r, st), "cub sort (rows)");
+    if (!rc) rc = launch(key_gather_kernel, grid, kBlock, st, "key_gather_kernel", c, idx_b, n, key_a);
+    if (!rc) rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_a, key_b, idx_b, idx_a, (int)n, 0, bits_c, st), "cub sort (cols)");
+    if (!rc) rc = launch(tuple_gather_kernel, grid, kBlock, st, "tuple_gather_kernel", r, c, v, idx_a, n, 0, r2, c2, v2);
+    if (!rc) rc = check_cuda(cudaMemcpyAsync(r, r2, b8, cudaMemcpyDeviceToDevice, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaMemcpyAsync(c, c2, b8, cudaMemcpyDeviceToDevice, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaMemcpyAsync(v, v2, b8, cudaMemcpyDeviceToDevice, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");
@@ -381,9 +357,9 @@ int hnh_tuples_mod_device(uint64_t *r, uint64_t *c, int64_t n, uint64_t mod_r, u
     if (n < 0) return set_error(HNH_E_INVALID, "hnh_tuples_mod_device: bad argument");
     if (n == 0 || (mod_r == 0 && mod_c == 0)) return HNH_OK;
     if (!r || !c) return set_error(HNH_E_INVALID, "hnh_tuples_mod_device: null pointer");
-    tuple_mod_kernel<<<grid_for(n), kThreads, 0, (cudaStream_t)stream>>>(r, c, n, mod_r, mod_c);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "tuple_mod_kernel launch");
+    int grid = 0;
+    int rc = grid_for(tuple_mod_kernel, n, kBlock, &grid, kCtasPerSm);
+    return rc ? rc : launch(tuple_mod_kernel, grid, kBlock, (cudaStream_t)stream, "tuple_mod_kernel", r, c, n, mod_r, mod_c);
 }
 
 int hnh_tuples_block_starts_device(const uint64_t *c_sorted, int64_t n, uint64_t block_width, int divisions, int64_t *starts_host,
@@ -398,10 +374,10 @@ int hnh_tuples_block_starts_device(const uint64_t *c_sorted, int64_t n, uint64_t
     Scratch s;
     int64_t *starts = nullptr;
     int rc = check_cuda(s.get((void **)&starts, sizeof(int64_t) * (size_t)(divisions + 1)), "cudaMalloc");
-    if (rc) return rc;
-    lower_bounds_kernel<uint64_t><<<(divisions + 1 + kThreads - 1) / kThreads, kThreads, 0, st>>>(c_sorted, n, block_width, divisions, starts);
-    count_launch(1);
-    rc = check_cuda(cudaMemcpyAsync(starts_host, starts, sizeof(int64_t) * (size_t)(divisions + 1), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
+    if (!rc)
+        rc = launch(lower_bounds_kernel<uint64_t>, (divisions + 1 + kBlock - 1) / kBlock, kBlock, st, "lower_bounds_kernel", c_sorted, n,
+                    block_width, divisions, starts);
+    if (!rc) rc = check_cuda(cudaMemcpyAsync(starts_host, starts, sizeof(int64_t) * (size_t)(divisions + 1), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");
     return rc;
 }

@@ -12,27 +12,21 @@
 // in the vector's own order.
 #include <cub/cub.cuh>
 
-#include <algorithm>
 #include <cmath>
 
-#include "hnh_b200.h"
-#include "launch.h"
+#include "row_gather.cuh"
 
 namespace {
 
+using hnh::bits_for;
 using hnh::check_cuda;
-using hnh::count_launch;
+using hnh::grid_for;
+using hnh::launch;
+using hnh::Scratch;
 using hnh::set_error;
 
-constexpr int kThreads = 256;
-constexpr int kPiece = 1024;  // entries of a row that one warp reduces
-
-int grid_for(int64_t work_items, int64_t per_block) {
-    int sms = 132;
-    hnh::device_sm_count(&sms);
-    const int64_t want = (work_items + per_block - 1) / per_block;
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)sms * 16));
-}
+constexpr int kCtasPerSm = 16;  // grid cap of every kernel here
+constexpr int kPiece = 1024;    // entries of a row that one warp reduces
 
 // (m, s) <- the (max, sum of exp(x - max)) of the union of two sets; (-inf, 0) is the empty set
 __device__ __forceinline__ void ms_merge(double &m, double &s, double m2, double s2) {
@@ -54,12 +48,6 @@ __device__ __forceinline__ void ms_warp_reduce(double &m, double &s) {
         const double m2 = __shfl_down_sync(0xffffffffu, m, off), s2 = __shfl_down_sync(0xffffffffu, s, off);
         ms_merge(m, s, m2, s2);
     }
-}
-
-__device__ __forceinline__ double sum_warp_reduce(double v) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
-    return v;
 }
 
 // the positions [lo, hi) in perm order of piece q
@@ -188,7 +176,7 @@ __global__ void piece_dot_kernel(const double *__restrict__ a, const double *__r
             const int32_t i = perm[p];
             t += a[i] * b[i];
         }
-        t = sum_warp_reduce(t);
+        t = warp_sum(t);
         if (lane == 0) piece_dot[q] = t;
     }
 }
@@ -204,7 +192,7 @@ __global__ void piece_sum_kernel(const double *__restrict__ x, const int32_t *__
         piece_range(q, row_start, piece_first, piece_row, &lo, &hi);
         double t = 0.0;
         for (int64_t p = lo + lane; p < hi; p += 32) t += x[perm[p]];
-        t = sum_warp_reduce(t);
+        t = warp_sum(t);
         if (lane == 0) piece_val[q] = t;
     }
 }
@@ -216,7 +204,7 @@ __global__ void row_sum_kernel(const int32_t *__restrict__ piece_first, int64_t 
     for (int64_t u = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; u < num_rows; u += warps) {
         double t = 0.0;
         for (int64_t q = piece_first[u] + lane; q < piece_first[u + 1]; q += 32) t += piece_val[q];
-        t = sum_warp_reduce(t);
+        t = warp_sum(t);
         if (lane == 0) row_val[u] = t;
     }
 }
@@ -226,23 +214,6 @@ __global__ void backward_apply_kernel(double *dx, const double *__restrict__ alp
                                       int64_t n, const double *__restrict__ row_dot) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) dx[i] = alpha[i] * (grad[i] - row_dot[keys[i]]);
-}
-
-struct Scratch {  // cudaMalloc'ed temporaries of one call, released on every exit path
-    void *p[6] = {};
-    int n = 0;
-    cudaError_t get(void **out, size_t bytes) {
-        cudaError_t e = cudaMalloc(out, std::max<size_t>(bytes, 256));
-        if (e == cudaSuccess) p[n++] = *out;
-        return e;
-    }
-    ~Scratch() { for (int i = 0; i < n; i++) cudaFree(p[i]); }
-};
-
-int bits_for(uint64_t max_value) {
-    int b = 1;
-    while (b < 64 && (max_value >> b) != 0) b++;
-    return b;
 }
 
 int check_plan(const char *who, const int32_t *perm, const int32_t *row_start, const int32_t *piece_first, const int32_t *piece_row,
@@ -261,9 +232,9 @@ int hnh_edge_keys_from_index(int32_t *keys, const int64_t *idx, int64_t n, int64
     if (n < 0) return set_error(HNH_E_INVALID, "hnh_edge_keys_from_index: negative size");
     if (n == 0) return HNH_OK;
     if (!keys || !idx) return set_error(HNH_E_INVALID, "hnh_edge_keys_from_index: null pointer");
-    keys_from_index_kernel<<<grid_for(n, kThreads * 4), kThreads, 0, (cudaStream_t)stream>>>(keys, idx, n, offset);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "keys_from_index_kernel launch");
+    int grid = 0;
+    int rc = grid_for(keys_from_index_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(keys_from_index_kernel, grid, kBlock, (cudaStream_t)stream, "keys_from_index_kernel", keys, idx, n, offset);
 }
 
 int64_t hnh_edge_softmax_piece_bound(int64_t n, int64_t num_rows) {
@@ -298,9 +269,10 @@ int hnh_edge_softmax_plan(const int32_t *keys, int64_t n, int64_t num_rows, int3
     if (!rc) rc = check_cuda(s.get((void **)&count, offsets_bytes), "cudaMalloc");
     if (!rc) rc = check_cuda(s.get((void **)&bad, sizeof(int)), "cudaMalloc");
     if (!rc) rc = check_cuda(cudaMemsetAsync(bad, 0, sizeof(int), st), "cudaMemsetAsync");
+    int grid = 0;
+    if (!rc) rc = grid_for(keys_check_iota_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    if (!rc) rc = launch(keys_check_iota_kernel, grid, kBlock, st, "keys_check_iota_kernel", keys, n, num_rows, idx, bad);
     if (rc) return rc;
-    keys_check_iota_kernel<<<grid_for(n, kThreads * 4), kThreads, 0, st>>>(keys, n, num_rows, idx, bad);
-    count_launch(1);
     int host_bad = 0;
     rc = check_cuda(cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");
@@ -312,20 +284,18 @@ int hnh_edge_softmax_plan(const int32_t *keys, int64_t n, int64_t num_rows, int3
     if (!rc) rc = check_cuda(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, count, piece_first, (int)(num_rows + 1), st), "cub scan size");
     if (!rc) rc = check_cuda(s.get(&tmp, std::max(sort_bytes, scan_bytes)), "cudaMalloc");
     if (!rc) rc = check_cuda(cub::DeviceRadixSort::SortPairs(tmp, sort_bytes, keys, sorted, idx, perm, (int)n, 0, end_bit, st), "cub sort");
-    if (rc) return rc;
-    row_start_kernel<<<grid_for(num_rows + 1, kThreads), kThreads, 0, st>>>(sorted, n, num_rows, row_start);
-    piece_count_kernel<<<grid_for(num_rows + 1, kThreads), kThreads, 0, st>>>(row_start, num_rows, count);
-    count_launch(2);
-    rc = check_cuda(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, count, piece_first, (int)(num_rows + 1), st), "cub scan");
+    if (!rc) rc = grid_for(row_start_kernel, num_rows + 1, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(row_start_kernel, grid, kBlock, st, "row_start_kernel", sorted, n, num_rows, row_start);
+    if (!rc) rc = launch(piece_count_kernel, grid, kBlock, st, "piece_count_kernel", row_start, num_rows, count);
+    if (!rc) rc = check_cuda(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, count, piece_first, (int)(num_rows + 1), st), "cub scan");
     int32_t total = 0;
     if (!rc) rc = check_cuda(cudaMemcpyAsync(&total, piece_first + num_rows, sizeof(int32_t), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");
     if (rc) return rc;
     if (total > piece_capacity)
         return set_error(HNH_E_INVALID, "hnh_edge_softmax_plan: %lld pieces, room for %lld", (long long)total, (long long)piece_capacity);
-    piece_row_kernel<<<grid_for(num_rows, kThreads), kThreads, 0, st>>>(piece_first, num_rows, piece_row);
-    count_launch(1);
-    rc = check_cuda(cudaGetLastError(), "edge softmax plan kernels launch");
+    rc = grid_for(piece_row_kernel, num_rows, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(piece_row_kernel, grid, kBlock, st, "piece_row_kernel", piece_first, num_rows, piece_row);
     if (!rc) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize");  // the scratch is freed on return
     if (!rc) *num_pieces = total;
     return rc;
@@ -340,23 +310,26 @@ int hnh_edge_softmax_stats_f64(const double *x, const int32_t *perm, const int32
     if (!row_max || !row_sum || (num_pieces > 0 && (!x || !piece_max || !piece_sum)))
         return set_error(HNH_E_INVALID, "hnh_edge_softmax_stats_f64: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0;
     if (num_pieces > 0) {
-        piece_stats_kernel<<<grid_for(num_pieces, kThreads / 32), kThreads, 0, st>>>(x, perm, row_start, piece_first, piece_row,
-                                                                                      num_pieces, piece_max, piece_sum);
-        count_launch(1);
+        rc = grid_for(piece_stats_kernel, num_pieces, kBlock / 32, &grid, kCtasPerSm);
+        if (!rc)
+            rc = launch(piece_stats_kernel, grid, kBlock, st, "piece_stats_kernel", x, perm, row_start, piece_first, piece_row, num_pieces,
+                        piece_max, piece_sum);
+        if (rc) return rc;
     }
-    row_stats_kernel<<<grid_for(num_rows, kThreads / 32), kThreads, 0, st>>>(piece_first, num_rows, piece_max, piece_sum, row_max, row_sum);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "edge softmax stats kernels launch");
+    rc = grid_for(row_stats_kernel, num_rows, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(row_stats_kernel, grid, kBlock, st, "row_stats_kernel", piece_first, num_rows, piece_max, piece_sum, row_max,
+                            row_sum);
 }
 
 int hnh_edge_softmax_rescale_f64(double *row_sum, const double *local_max, const double *global_max, int64_t num_rows, void *stream) {
     if (num_rows < 0) return set_error(HNH_E_INVALID, "hnh_edge_softmax_rescale_f64: negative size");
     if (num_rows == 0) return HNH_OK;
     if (!row_sum || !local_max || !global_max) return set_error(HNH_E_INVALID, "hnh_edge_softmax_rescale_f64: null pointer");
-    rescale_kernel<<<grid_for(num_rows, kThreads * 4), kThreads, 0, (cudaStream_t)stream>>>(row_sum, local_max, global_max, num_rows);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "rescale_kernel launch");
+    int grid = 0;
+    int rc = grid_for(rescale_kernel, num_rows, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(rescale_kernel, grid, kBlock, (cudaStream_t)stream, "rescale_kernel", row_sum, local_max, global_max, num_rows);
 }
 
 int hnh_edge_softmax_apply_f64(double *alpha, const double *x, const int32_t *keys, int64_t n, const double *row_max,
@@ -364,9 +337,9 @@ int hnh_edge_softmax_apply_f64(double *alpha, const double *x, const int32_t *ke
     if (n < 0) return set_error(HNH_E_INVALID, "hnh_edge_softmax_apply_f64: negative size");
     if (n == 0) return HNH_OK;
     if (!alpha || !x || !keys || !row_max || !row_sum) return set_error(HNH_E_INVALID, "hnh_edge_softmax_apply_f64: null pointer");
-    apply_kernel<<<grid_for(n, kThreads * 4), kThreads, 0, (cudaStream_t)stream>>>(alpha, x, keys, n, row_max, row_sum);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "apply_kernel launch");
+    int grid = 0;
+    int rc = grid_for(apply_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(apply_kernel, grid, kBlock, (cudaStream_t)stream, "apply_kernel", alpha, x, keys, n, row_max, row_sum);
 }
 
 int hnh_edge_softmax_dot_f64(const double *alpha, const double *grad, const int32_t *perm, const int32_t *row_start,
@@ -378,14 +351,16 @@ int hnh_edge_softmax_dot_f64(const double *alpha, const double *grad, const int3
     if (!row_dot || (num_pieces > 0 && (!alpha || !grad || !piece_dot)))
         return set_error(HNH_E_INVALID, "hnh_edge_softmax_dot_f64: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0;
     if (num_pieces > 0) {
-        piece_dot_kernel<<<grid_for(num_pieces, kThreads / 32), kThreads, 0, st>>>(alpha, grad, perm, row_start, piece_first, piece_row,
-                                                                                    num_pieces, piece_dot);
-        count_launch(1);
+        rc = grid_for(piece_dot_kernel, num_pieces, kBlock / 32, &grid, kCtasPerSm);
+        if (!rc)
+            rc = launch(piece_dot_kernel, grid, kBlock, st, "piece_dot_kernel", alpha, grad, perm, row_start, piece_first, piece_row,
+                        num_pieces, piece_dot);
+        if (rc) return rc;
     }
-    row_sum_kernel<<<grid_for(num_rows, kThreads / 32), kThreads, 0, st>>>(piece_first, num_rows, piece_dot, row_dot);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "edge softmax dot kernels launch");
+    rc = grid_for(row_sum_kernel, num_rows, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(row_sum_kernel, grid, kBlock, st, "row_sum_kernel", piece_first, num_rows, piece_dot, row_dot);
 }
 
 int hnh_edge_sum_f64(const double *x, const int32_t *perm, const int32_t *row_start, const int32_t *piece_first,
@@ -396,14 +371,16 @@ int hnh_edge_sum_f64(const double *x, const int32_t *perm, const int32_t *row_st
     if (num_rows == 0) return HNH_OK;
     if (!row_sum || (num_pieces > 0 && (!x || !piece_sum))) return set_error(HNH_E_INVALID, "hnh_edge_sum_f64: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0;
     if (num_pieces > 0) {
-        piece_sum_kernel<<<grid_for(num_pieces, kThreads / 32), kThreads, 0, st>>>(x, perm, row_start, piece_first, piece_row,
-                                                                                    num_pieces, piece_sum);
-        count_launch(1);
+        rc = grid_for(piece_sum_kernel, num_pieces, kBlock / 32, &grid, kCtasPerSm);
+        if (!rc)
+            rc = launch(piece_sum_kernel, grid, kBlock, st, "piece_sum_kernel", x, perm, row_start, piece_first, piece_row, num_pieces,
+                        piece_sum);
+        if (rc) return rc;
     }
-    row_sum_kernel<<<grid_for(num_rows, kThreads / 32), kThreads, 0, st>>>(piece_first, num_rows, piece_sum, row_sum);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "edge sum kernels launch");
+    rc = grid_for(row_sum_kernel, num_rows, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(row_sum_kernel, grid, kBlock, st, "row_sum_kernel", piece_first, num_rows, piece_sum, row_sum);
 }
 
 int hnh_edge_softmax_backward_f64(double *dx, const double *alpha, const double *grad, const int32_t *keys, int64_t n,
@@ -411,9 +388,10 @@ int hnh_edge_softmax_backward_f64(double *dx, const double *alpha, const double 
     if (n < 0) return set_error(HNH_E_INVALID, "hnh_edge_softmax_backward_f64: negative size");
     if (n == 0) return HNH_OK;
     if (!dx || !alpha || !grad || !keys || !row_dot) return set_error(HNH_E_INVALID, "hnh_edge_softmax_backward_f64: null pointer");
-    backward_apply_kernel<<<grid_for(n, kThreads * 4), kThreads, 0, (cudaStream_t)stream>>>(dx, alpha, grad, keys, n, row_dot);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "backward_apply_kernel launch");
+    int grid = 0;
+    int rc = grid_for(backward_apply_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(backward_apply_kernel, grid, kBlock, (cudaStream_t)stream, "backward_apply_kernel", dx, alpha, grad, keys, n,
+                            row_dot);
 }
 
 }  // extern "C"

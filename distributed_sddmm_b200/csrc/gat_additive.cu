@@ -8,41 +8,19 @@
 // The two row kernels run one warp per row: lanes stride the row in 16-byte pairs (scalars when a row or a vector is
 // not 16-byte aligned), and a row's dot products end in a fixed shuffle tree.  No floating-point atomics: repeated
 // calls give bit-identical results.
-#include <algorithm>
-#include <cstdint>
-
-#include "hnh_b200.h"
-#include "launch.h"
+#include "row_gather.cuh"
 
 namespace {
 
-using hnh::check_cuda;
-using hnh::count_launch;
+using hnh::grid_for;
+using hnh::launch;
 using hnh::set_error;
 
-constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
-
-int grid_for(int64_t work_items, int64_t per_block, int *grid) {
-    int sms = 0;
-    int rc = hnh::device_sm_count(&sms);
-    if (rc) return rc;
-    const int64_t want = (work_items + per_block - 1) / per_block;
-    *grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)sms * 16));
-    return HNH_OK;
-}
-
-bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
-
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
-    return v;
-}
+constexpr int kCtasPerSm = 16;  // grid cap of every kernel here
 
 // s[i] = <P[i, :], a1>, t[i] = <P[i, :], a2>.  P is read once, with streaming loads; a1 and a2 stay in L1.
 template <bool kPairs>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kBlock)
 node_scalars_kernel(double *__restrict__ s, double *__restrict__ t, const double *__restrict__ P, const double *__restrict__ a1,
                     const double *__restrict__ a2, int64_t n, int64_t d) {
     const int lane = threadIdx.x & 31;
@@ -90,7 +68,7 @@ __global__ void edge_scores_kernel(double *__restrict__ out, const double *__res
 
 // dP[i, :] += ds[i] a1 + dt[i] a2
 template <bool kPairs>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kBlock)
 rank2_update_kernel(double *__restrict__ dP, const double *__restrict__ ds, const double *__restrict__ dt,
                     const double *__restrict__ a1, const double *__restrict__ a2, int64_t n, int64_t d) {
     const int lane = threadIdx.x & 31;
@@ -123,16 +101,10 @@ int hnh_gat_node_scalars_f64(double *s, double *t, const double *P, const double
     if (n < 0 || d < 0) return set_error(HNH_E_INVALID, "hnh_gat_node_scalars_f64: negative size");
     if (n == 0) return HNH_OK;
     if (!s || !t || (d > 0 && (!P || !a1 || !a2))) return set_error(HNH_E_INVALID, "hnh_gat_node_scalars_f64: null pointer");
+    auto k = d % 2 == 0 && aligned16(P) && aligned16(a1) && aligned16(a2) ? node_scalars_kernel<true> : node_scalars_kernel<false>;
     int grid;
-    int rc = grid_for(n, kWarps, &grid);
-    if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (d % 2 == 0 && aligned16(P) && aligned16(a1) && aligned16(a2))
-        node_scalars_kernel<true><<<grid, kThreads, 0, st>>>(s, t, P, a1, a2, n, d);
-    else
-        node_scalars_kernel<false><<<grid, kThreads, 0, st>>>(s, t, P, a1, a2, n, d);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "node_scalars_kernel launch");
+    int rc = grid_for(k, n, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "node_scalars_kernel", s, t, P, a1, a2, n, d);
 }
 
 int hnh_gat_edge_scores_f64(double *out, const double *s, const double *t, const int32_t *row_key, const int32_t *col_key,
@@ -140,16 +112,10 @@ int hnh_gat_edge_scores_f64(double *out, const double *s, const double *t, const
     if (n < 0) return set_error(HNH_E_INVALID, "hnh_gat_edge_scores_f64: negative size");
     if (n == 0) return HNH_OK;
     if (!out || !s || !t || !row_key || !col_key) return set_error(HNH_E_INVALID, "hnh_gat_edge_scores_f64: null pointer");
+    auto k = derivative ? edge_scores_kernel<true> : edge_scores_kernel<false>;
     int grid;
-    int rc = grid_for(n, kThreads * 4, &grid);
-    if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (derivative)
-        edge_scores_kernel<true><<<grid, kThreads, 0, st>>>(out, s, t, row_key, col_key, n, alpha);
-    else
-        edge_scores_kernel<false><<<grid, kThreads, 0, st>>>(out, s, t, row_key, col_key, n, alpha);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "edge_scores_kernel launch");
+    int rc = grid_for(k, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "edge_scores_kernel", out, s, t, row_key, col_key, n, alpha);
 }
 
 int hnh_gat_rank2_update_f64(double *dP, const double *ds, const double *dt, const double *a1, const double *a2, int64_t n,
@@ -157,16 +123,10 @@ int hnh_gat_rank2_update_f64(double *dP, const double *ds, const double *dt, con
     if (n < 0 || d < 0) return set_error(HNH_E_INVALID, "hnh_gat_rank2_update_f64: negative size");
     if (n == 0 || d == 0) return HNH_OK;
     if (!dP || !ds || !dt || !a1 || !a2) return set_error(HNH_E_INVALID, "hnh_gat_rank2_update_f64: null pointer");
+    auto k = d % 2 == 0 && aligned16(dP) && aligned16(a1) && aligned16(a2) ? rank2_update_kernel<true> : rank2_update_kernel<false>;
     int grid;
-    int rc = grid_for(n, kWarps, &grid);
-    if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (d % 2 == 0 && aligned16(dP) && aligned16(a1) && aligned16(a2))
-        rank2_update_kernel<true><<<grid, kThreads, 0, st>>>(dP, ds, dt, a1, a2, n, d);
-    else
-        rank2_update_kernel<false><<<grid, kThreads, 0, st>>>(dP, ds, dt, a1, a2, n, d);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "rank2_update_kernel launch");
+    int rc = grid_for(k, n, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "rank2_update_kernel", dP, ds, dt, a1, a2, n, d);
 }
 
 }  // extern "C"

@@ -9,18 +9,17 @@
 // The backward pass (GAT::backwardPass) adds the two other products of a projection on the same DMMA tiling --
 // dW = X^T dP (dgemm_tn_kernel, split over the long k and reduced in a fixed order) and dX += dP W^T
 // (dgemm_nt_kernel) -- and the derivatives of the two activations.
-#include <algorithm>
-
-#include "hnh_b200.h"
 #include "launch.h"
 
 namespace {
 
 using hnh::check_cuda;
-using hnh::count_launch;
+using hnh::grid_for;
+using hnh::kBlock;
+using hnh::launch;
 using hnh::set_error;
 
-constexpr int kThreads = 256;
+constexpr int kCtasPerSm = 8;  // grid cap of every grid-stride kernel here
 
 // x -> max(x, 0) + alpha * min(x, 0)
 __global__ void leaky_relu_kernel(double *__restrict__ dst, const double *__restrict__ src, int64_t n, double alpha) {
@@ -40,15 +39,6 @@ __global__ void relu_cols_kernel(double *__restrict__ dst, int64_t ld_dst, int64
         const int64_t i = t / cols, j = t - i * cols;
         dst[i * ld_dst + col0 + j] = fmax(src[t], 0.0);
     }
-}
-
-int grid_for_elements(int64_t n, int *grid) {
-    int sms = 0;
-    int rc = hnh::device_sm_count(&sms);
-    if (rc) return rc;
-    const int64_t want = (n + (int64_t)kThreads * 4 - 1) / ((int64_t)kThreads * 4);
-    *grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)sms * 8));
-    return HNH_OK;
 }
 
 // ---- fp64 GEMM on DMMA ---------------------------------------------------------------------------------
@@ -294,11 +284,8 @@ int hnh_leaky_relu_f64(double *dst, const double *src, int64_t n, double alpha, 
     if (n == 0) return HNH_OK;
     if (!dst || !src) return set_error(HNH_E_INVALID, "hnh_leaky_relu_f64: null pointer");
     int grid;
-    int rc = grid_for_elements(n, &grid);
-    if (rc) return rc;
-    leaky_relu_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(dst, src, n, alpha);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "leaky_relu_kernel launch");
+    int rc = grid_for(leaky_relu_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(leaky_relu_kernel, grid, kBlock, (cudaStream_t)stream, "leaky_relu_kernel", dst, src, n, alpha);
 }
 
 int hnh_relu_cols_f64(double *dst, int64_t ld_dst, int64_t col0, const double *src, int64_t rows, int64_t cols, void *stream) {
@@ -308,11 +295,8 @@ int hnh_relu_cols_f64(double *dst, int64_t ld_dst, int64_t col0, const double *s
     if (rows == 0 || cols == 0) return HNH_OK;
     if (!dst || !src) return set_error(HNH_E_INVALID, "hnh_relu_cols_f64: null pointer");
     int grid;
-    int rc = grid_for_elements(rows * cols, &grid);
-    if (rc) return rc;
-    relu_cols_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(dst, ld_dst, col0, src, rows, cols);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "relu_cols_kernel launch");
+    int rc = grid_for(relu_cols_kernel, rows * cols, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(relu_cols_kernel, grid, kBlock, (cudaStream_t)stream, "relu_cols_kernel", dst, ld_dst, col0, src, rows, cols);
 }
 
 int hnh_dgemm_f64(double *C, const double *A, const double *B, int64_t m, int64_t n, int64_t k, void *stream) {
@@ -322,16 +306,10 @@ int hnh_dgemm_f64(double *C, const double *A, const double *B, int64_t m, int64_
     if (!C || (k > 0 && (!A || !B))) return set_error(HNH_E_INVALID, "hnh_dgemm_f64: null pointer");
     if (k == 0)
         return check_cuda(cudaMemsetAsync(C, 0, sizeof(double) * (size_t)(m * n), (cudaStream_t)stream), "cudaMemsetAsync");
-    int sms = 0;
-    int rc = hnh::device_sm_count(&sms);
-    if (rc) return rc;
     const int64_t tiles = ((m + GM - 1) / GM) * ((n + GN - 1) / GN);
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, (int64_t)sms * 8));
-    dgemm_dmma_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(C, A, B, m, (int)n, (int)k);
-    rc = check_cuda(cudaGetLastError(), "dgemm_dmma_kernel launch");
-    if (rc) return rc;
-    count_launch(1);
-    return HNH_OK;
+    int grid;
+    int rc = grid_for(dgemm_dmma_kernel, tiles, 1, &grid, kCtasPerSm);
+    return rc ? rc : launch(dgemm_dmma_kernel, grid, 128, (cudaStream_t)stream, "dgemm_dmma_kernel", C, A, B, m, (int)n, (int)k);
 }
 
 int hnh_leaky_relu_grad_f64(double *dst, const double *src, int64_t n, double alpha, void *stream) {
@@ -339,11 +317,8 @@ int hnh_leaky_relu_grad_f64(double *dst, const double *src, int64_t n, double al
     if (n == 0) return HNH_OK;
     if (!dst || !src) return set_error(HNH_E_INVALID, "hnh_leaky_relu_grad_f64: null pointer");
     int grid;
-    int rc = grid_for_elements(n, &grid);
-    if (rc) return rc;
-    leaky_relu_grad_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(dst, src, n, alpha);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "leaky_relu_grad_kernel launch");
+    int rc = grid_for(leaky_relu_grad_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(leaky_relu_grad_kernel, grid, kBlock, (cudaStream_t)stream, "leaky_relu_grad_kernel", dst, src, n, alpha);
 }
 
 int hnh_relu_cols_backward_f64(double *dst, const double *grad, const double *out, int64_t ld, int64_t col0, int64_t rows,
@@ -354,11 +329,8 @@ int hnh_relu_cols_backward_f64(double *dst, const double *grad, const double *ou
     if (rows == 0 || cols == 0) return HNH_OK;
     if (!dst || !grad || !out) return set_error(HNH_E_INVALID, "hnh_relu_cols_backward_f64: null pointer");
     int grid;
-    int rc = grid_for_elements(rows * cols, &grid);
-    if (rc) return rc;
-    relu_cols_backward_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(dst, grad, out, ld, col0, rows, cols);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "relu_cols_backward_kernel launch");
+    int rc = grid_for(relu_cols_backward_kernel, rows * cols, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(relu_cols_backward_kernel, grid, kBlock, (cudaStream_t)stream, "relu_cols_backward_kernel", dst, grad, out, ld, col0, rows, cols);
 }
 
 int64_t hnh_dgemm_tn_workspace_bytes(int64_t m, int64_t n, int64_t k) {
@@ -386,17 +358,12 @@ int hnh_dgemm_tn_f64(double *C, const double *A, const double *B, int64_t m, int
     tn_plan(m, n, k, &splits, &chunk);
     const int64_t tiles = ((m + GM - 1) / GM) * ((n + GN - 1) / GN);
     double *part = splits > 1 ? (double *)workspace : C;
-    dgemm_tn_kernel<<<dim3((unsigned)tiles, (unsigned)splits), 128, 0, (cudaStream_t)stream>>>(part, A, B, (int)m, (int)n, k, chunk);
-    int rc = check_cuda(cudaGetLastError(), "dgemm_tn_kernel launch");
-    if (rc) return rc;
-    count_launch(1);
-    if (splits == 1) return HNH_OK;
+    int rc = launch(dgemm_tn_kernel, dim3((unsigned)tiles, (unsigned)splits), 128, (cudaStream_t)stream, "dgemm_tn_kernel", part, A, B,
+                    (int)m, (int)n, k, chunk);
+    if (rc || splits == 1) return rc;
     int grid;
-    rc = grid_for_elements(m * n, &grid);
-    if (rc) return rc;
-    tn_reduce_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(C, part, m * n, splits);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "tn_reduce_kernel launch");
+    rc = grid_for(tn_reduce_kernel, m * n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(tn_reduce_kernel, grid, kBlock, (cudaStream_t)stream, "tn_reduce_kernel", C, part, m * n, splits);
 }
 
 int hnh_dgemm_nt_f64(double *C, const double *A, const double *B, int64_t m, int64_t n, int64_t k, int accumulate, void *stream) {
@@ -406,16 +373,10 @@ int hnh_dgemm_nt_f64(double *C, const double *A, const double *B, int64_t m, int
     if (!C || (k > 0 && (!A || !B))) return set_error(HNH_E_INVALID, "hnh_dgemm_nt_f64: null pointer");
     if (k == 0)
         return check_cuda(cudaMemsetAsync(C, 0, sizeof(double) * (size_t)(m * n), (cudaStream_t)stream), "cudaMemsetAsync");
-    int sms = 0;
-    int rc = hnh::device_sm_count(&sms);
-    if (rc) return rc;
     const int64_t tiles = ((m + GM - 1) / GM) * ((n + GN - 1) / GN);
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, (int64_t)sms * 8));
-    dgemm_nt_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(C, A, B, m, (int)n, (int)k, accumulate ? 1 : 0);
-    rc = check_cuda(cudaGetLastError(), "dgemm_nt_kernel launch");
-    if (rc) return rc;
-    count_launch(1);
-    return HNH_OK;
+    int grid;
+    int rc = grid_for(dgemm_nt_kernel, tiles, 1, &grid, kCtasPerSm);
+    return rc ? rc : launch(dgemm_nt_kernel, grid, 128, (cudaStream_t)stream, "dgemm_nt_kernel", C, A, B, m, (int)n, (int)k, accumulate ? 1 : 0);
 }
 
 }  // extern "C"

@@ -17,8 +17,9 @@
 
 namespace {
 
-using hnh::check_cuda;
-using hnh::count_launch;
+using hnh::grid_for;
+using hnh::kResident;
+using hnh::launch;
 using hnh::set_error;
 
 // most CTAs a gradient launch uses (the da workspace holds one r-wide partial per CTA)
@@ -252,32 +253,6 @@ __global__ void gatv2_da_reduce_kernel(double *__restrict__ da, const double *__
     }
 }
 
-// ---- launch ----------------------------------------------------------------------------------------------------
-
-template <int R, int G, int VW, int UN>
-int launch_scores(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, const double *X, int64_t ldx,
-                  const double *Y, int64_t ldy, const double *a, double alpha, double *out, cudaStream_t st) {
-    auto k = gatv2_scores_kernel<R, G, VW, UN>;
-    int grid;
-    int rc = grid_for(k, kBlock / G, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, X, ldx, Y, ldy, a, alpha, out);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "gatv2_scores_kernel launch");
-}
-
-template <int R, int G, int VW, int UN>
-int launch_grad(const int64_t *rowStart, const int64_t *col_idx, const double *g, int64_t rows, const double *X,
-                int64_t ldx, const double *Y, int64_t ldy, const double *a, double alpha, double *dX, int64_t lddx,
-                double *part, int *ctas, cudaStream_t st) {
-    auto k = part ? gatv2_grad_kernel<R, G, VW, UN, true> : gatv2_grad_kernel<R, G, VW, UN, false>;
-    int rc = grid_for(k, kBlock / G, rows, kMaxGradCtas, ctas);
-    if (rc) return rc;
-    k<<<*ctas, kBlock, 0, st>>>(rowStart, col_idx, g, rows, X, ldx, Y, ldy, a, alpha, dX, lddx, part);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "gatv2_grad_kernel launch");
-}
-
 int check_block(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
                 const double *X, int64_t ldx, const double *Y, int64_t ldy, const double *a, int r) {
     if (rows < 0 || nnz < 0) return set_error(HNH_E_INVALID, "%s: negative size", who);
@@ -302,19 +277,21 @@ int hnh_gatv2_scores_f64(const int64_t *rowStart, const int64_t *col_idx, int64_
     if (v == 1) return HNH_OK;
     if (!out) return set_error(HNH_E_INVALID, "hnh_gatv2_scores_f64: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
     if (table_width(r) && aligned16(R) && aligned16(Y) && aligned16(a) && ldr % 2 == 0 && ldy % 2 == 0) {
-        int rc = HNH_OK;
-#define SC(RR, G, VW, UN) rc = launch_scores<RR, G, VW, UN>(rowStart, col_idx, rows, R, ldr, Y, ldy, a, alpha, out, st)
-        ROW_GATHER_DISPATCH(r, SC)
+#define SC(RR, G, VW, UN)                                                                                                  \
+    {                                                                                                                      \
+        auto k = gatv2_scores_kernel<RR, G, VW, UN>;                                                                       \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc) rc = launch(k, grid, kBlock, st, "gatv2_scores_kernel", rowStart, col_idx, rows, R, ldr, Y, ldy, a, alpha, out); \
+    }
+        HNH_DISPATCH_R(r, SC, )
 #undef SC
         return rc;
     }
-    int grid = 1;
-    int rc = grid_for(gatv2_scores_generic_kernel, kBlock / 32, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    gatv2_scores_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, R, ldr, Y, ldy, a, r, alpha, out);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "gatv2_scores_generic_kernel launch");
+    rc = grid_for(gatv2_scores_generic_kernel, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(gatv2_scores_generic_kernel, grid, kBlock, st, "gatv2_scores_generic_kernel", rowStart, col_idx, rows, R, ldr,
+                            Y, ldy, a, r, alpha, out);
 }
 
 int64_t hnh_gatv2_grad_workspace_bytes(int64_t rows, int r) {
@@ -339,22 +316,23 @@ int hnh_gatv2_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const do
     int ctas = 0, rc = HNH_OK;
     if (table_width(r) && aligned16(R) && aligned16(Y) && aligned16(a) && aligned16(dR) && ldr % 2 == 0 && ldy % 2 == 0 &&
         lddr % 2 == 0) {
-#define GR(RR, G, VW, UN) \
-    rc = launch_grad<RR, G, VW, UN>(rowStart, col_idx, g, rows, R, ldr, Y, ldy, a, alpha, dR, lddr, part, &ctas, st)
-        ROW_GATHER_DISPATCH(r, GR)
+#define GR(RR, G, VW, UN)                                                                                                  \
+    {                                                                                                                      \
+        auto k = part ? gatv2_grad_kernel<RR, G, VW, UN, true> : gatv2_grad_kernel<RR, G, VW, UN, false>;                  \
+        rc = grid_for(k, rows, kBlock / G, &ctas, kResident, kMaxGradCtas);                                                \
+        if (!rc)                                                                                                           \
+            rc = launch(k, ctas, kBlock, st, "gatv2_grad_kernel", rowStart, col_idx, g, rows, R, ldr, Y, ldy, a, alpha, dR, lddr, part); \
+    }
+        HNH_DISPATCH_R(r, GR, )
 #undef GR
     } else {
-        rc = grid_for(gatv2_grad_generic_kernel, kBlock / 32, rows, kMaxGradCtas, &ctas);
-        if (rc) return rc;
-        gatv2_grad_generic_kernel<<<ctas, kBlock, 0, st>>>(rowStart, col_idx, g, rows, R, ldr, Y, ldy, a, r, alpha, dR, lddr,
-                                                            part);
-        count_launch(1);
-        rc = check_cuda(cudaGetLastError(), "gatv2_grad_generic_kernel launch");
+        rc = grid_for(gatv2_grad_generic_kernel, rows, kBlock / 32, &ctas, kResident, kMaxGradCtas);
+        if (!rc)
+            rc = launch(gatv2_grad_generic_kernel, ctas, kBlock, st, "gatv2_grad_generic_kernel", rowStart, col_idx, g, rows, R, ldr, Y,
+                        ldy, a, r, alpha, dR, lddr, part);
     }
     if (rc || !da) return rc;
-    gatv2_da_reduce_kernel<<<(r + kBlock - 1) / kBlock, kBlock, 0, st>>>(da, part, ctas, r);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "gatv2_da_reduce_kernel launch");
+    return launch(gatv2_da_reduce_kernel, (r + kBlock - 1) / kBlock, kBlock, st, "gatv2_da_reduce_kernel", da, part, ctas, r);
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 // kernels.cuh -- sm_90a device code for the HnH local kernels (K1 SDDMM, K2 SpMM,
-// K3 fused SDDMM->SpMM) and the small value-plumbing / row-algebra kernels.
+// K3 fused SDDMM->SpMM).
 //
 // What these replace (reference, CPU): StandardKernel::sddmm_local
 // (sparse_kernels.cpp:13-57, an OpenMP loop over nonzeros) and
@@ -17,78 +17,9 @@
 // SpMM / fused accumulate the output row in registers in stored CSR order (bit-compatible
 // with the row-major CSR restatement in oracle/hnh_oracle.c) and touch Y[row] once.
 #pragma once
-#include <cstdint>
-#include <cuda_runtime.h>
+#include "row_gather.cuh"
 
 namespace hnh {
-
-// ------------------------------------------------------------------ vector loads --------
-// Gather loads: read-only path, normal L2 policy (gathered factor rows are the only data
-// with any reuse).  Stream loads: read-only, do not allocate in L1, evict-first in L2.
-template <int VW>
-__device__ __forceinline__ void ld_gather(double (&d)[VW], const double *p);
-template <>
-__device__ __forceinline__ void ld_gather<2>(double (&d)[2], const double *p) {
-    asm volatile("ld.global.nc.L1::no_allocate.v2.f64 {%0,%1}, [%2];"
-                 : "=d"(d[0]), "=d"(d[1])
-                 : "l"(p));
-}
-template <>
-__device__ __forceinline__ void ld_gather<1>(double (&d)[1], const double *p) {
-    d[0] = __ldg(p);
-}
-
-// plain (coherent) vector load / store for read-modify-write of output rows
-template <int VW>
-__device__ __forceinline__ void ld_rw(double (&d)[VW], const double *p);
-template <>
-__device__ __forceinline__ void ld_rw<2>(double (&d)[2], const double *p) {
-    asm volatile("ld.global.L1::no_allocate.v2.f64 {%0,%1}, [%2];"
-                 : "=d"(d[0]), "=d"(d[1])
-                 : "l"(p)
-                 : "memory");
-}
-template <int VW>
-__device__ __forceinline__ void st_rw(double *p, const double (&d)[VW]);
-template <>
-__device__ __forceinline__ void st_rw<2>(double *p, const double (&d)[2]) {
-    asm volatile("st.global.L1::no_allocate.v2.f64 [%0], {%1,%2};" ::"l"(p), "d"(d[0]), "d"(d[1])
-                 : "memory");
-}
-
-__device__ __forceinline__ int64_t ld_stream_i64(const int64_t *p) {
-    int64_t v;
-    asm volatile("ld.global.nc.L1::no_allocate.s64 %0, [%1];" : "=l"(v) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ double ld_stream_f64(const double *p) {
-    double v;
-    asm volatile("ld.global.nc.L1::no_allocate.f64 %0, [%1];" : "=d"(v) : "l"(p));
-    return v;
-}
-
-// coherent (non-.nc) streaming load: for `values`, which the same kernel overwrites
-__device__ __forceinline__ double ld_rw_f64(const double *p) {
-    double v;
-    asm volatile("ld.global.L1::no_allocate.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
-    return v;
-}
-
-template <int G>
-__device__ __forceinline__ unsigned group_mask(int lane) {
-    if constexpr (G == 32) {
-        return 0xffffffffu;
-    } else {
-        return ((1u << G) - 1u) << (lane & ~(G - 1));
-    }
-}
-
-template <int G>
-__device__ __forceinline__ double group_allreduce(double d, unsigned mask) {
-#pragma unroll
-    for (int o = G / 2; o > 0; o >>= 1) d += __shfl_xor_sync(mask, d, o, G);
-    return d;
-}
 
 // SDDMM epilogue.  Plain: values[j] = d.  With `scale` (the caller's S values, aligned with `values`) the Hadamard
 // product of the reference's `SValues.cwiseProduct(getCSRValues())` (15D_dense_shift.hpp:364-368) is applied at the
@@ -970,115 +901,6 @@ fused_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__rest
                 acc = fma(values[j], Y[col_idx[j] * (int64_t)r + k], acc);
             Out[row * (int64_t)r + k] = acc;
         }
-    }
-}
-
-// ------------------------------------------------------------------ K4 + row algebra -----
-__global__ void fill_kernel(double *__restrict__ dst, int64_t n, double value) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-        dst[i] = value;
-}
-
-// uniform(-1, 1) from a counter-based hash of (seed, i): Eigen's setRandom() stand-in
-__global__ void random_uniform_kernel(double *__restrict__ dst, int64_t n, uint64_t seed) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        uint64_t z = seed + (uint64_t)i * 0x9E3779B97F4A7C15ull + 0x9E3779B97F4A7C15ull;
-        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-        z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-        z ^= z >> 31;
-        dst[i] = (double)(z >> 11) * (2.0 / 9007199254740992.0) - 1.0;
-    }
-}
-
-__global__ void hadamard_kernel(double *__restrict__ dst, const double *__restrict__ a,
-                                const double *__restrict__ b, int64_t n) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-        dst[i] = a[i] * b[i];
-}
-
-__global__ void expand_row_idx_kernel(const int64_t *__restrict__ rowStart, int64_t rows,
-                                      int64_t *__restrict__ row_idx) {
-    const int lane = threadIdx.x & 31;
-    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-    for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows;
-         row += nwarps) {
-        const int64_t s = rowStart[row], e = rowStart[row + 1];
-        for (int64_t j = s + lane; j < e; j += 32) row_idx[j] = row;
-    }
-}
-
-__global__ void batch_dot_kernel(double *__restrict__ out, const double *__restrict__ A,
-                                 const double *__restrict__ B, int64_t rows, int r) {
-    const int lane = threadIdx.x & 31;
-    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-    for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows;
-         row += nwarps) {
-        double d = 0.0;
-        for (int k = lane; k < r; k += 32)
-            d = fma(A[row * (int64_t)r + k], B[row * (int64_t)r + k], d);
-        d = group_allreduce<32>(d, 0xffffffffu);
-        if (lane == 0) out[row] = d;
-    }
-}
-
-__global__ void row_axpy_kernel(double *D, const double *C, double alpha,
-                                const double *__restrict__ s, const double *M, int64_t rows,
-                                int r) {
-    const int64_t n = rows * (int64_t)r;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const double sc = s ? s[i / r] : 1.0;
-        D[i] = (C ? C[i] : 0.0) + alpha * sc * M[i];
-    }
-}
-
-__global__ void vec_quotient_kernel(double *out, const double *a, double ca, const double *b,
-                                    double cb, int64_t n) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-        out[i] = b ? (a[i] + ca) / (b[i] + cb) : (a[i] + ca);
-}
-
-__global__ void axpby_kernel(double *dst, double alpha, const double *x, double beta,
-                             const double *y, int64_t n) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-        dst[i] = alpha * x[i] + (y ? beta * y[i] : 0.0);
-}
-
-// Deterministic two-pass sum of squares (fingerprints and residuals must be bit-stable run to run): pass 1 leaves
-// one partial per CTA (fixed grid-stride assignment, fixed shuffle tree), pass 2 -- one CTA -- adds the partials
-// in a fixed order.  No atomics.
-__global__ void squared_norm_partial_kernel(double *__restrict__ partial, const double *__restrict__ x, int64_t n) {
-    __shared__ double warp_sums[8];
-    double acc = 0.0;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-        acc = fma(x[i], x[i], acc);
-    acc = group_allreduce<32>(acc, 0xffffffffu);
-    if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0.0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += warp_sums[w];
-        partial[blockIdx.x] = t;
-    }
-}
-
-__global__ void sum_partials_kernel(double *__restrict__ out, const double *__restrict__ partial, int n) {
-    __shared__ double warp_sums[8];
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) acc += partial[i];
-    acc = group_allreduce<32>(acc, 0xffffffffu);
-    if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0.0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += warp_sums[w];
-        *out = t;
     }
 }
 

@@ -21,8 +21,8 @@
 
 namespace {
 
-using hnh::check_cuda;
-using hnh::count_launch;
+using hnh::grid_for;
+using hnh::launch;
 using hnh::set_error;
 
 template <int G>
@@ -416,48 +416,6 @@ __global__ void attn_finish_kernel(int64_t rows, int d, const double *acc, int64
     }
 }
 
-// ---- launch ----------------------------------------------------------------------------------------------------
-template <int R, int G, int VW, int UN>
-int launch_step(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, const double *Q, int64_t ldq, const double *K,
-                int64_t ldk, const double *V, int64_t ldv, double scale, double *acc, int64_t ldacc, double *m, int64_t ldm,
-                double *s, int64_t lds, cudaStream_t st) {
-    auto k = attn_step_kernel<R, G, VW, UN>;
-    int grid;
-    int rc = grid_for(k, kBlock / G, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_step_kernel launch");
-}
-
-template <int R, int G, int VW, int UN>
-int launch_grad_q(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, const double *Q, int64_t ldq,
-                  const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt, const double *K,
-                  int64_t ldk, const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq, cudaStream_t st) {
-    auto k = attn_grad_q_kernel<R, G, VW, UN>;
-    int grid;
-    int rc = grid_for(k, kBlock / G, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_grad_q_kernel launch");
-}
-
-template <int R, int G, int VW, int UN>
-int launch_grad_kv(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, const double *K, int64_t ldk,
-                   const double *V, int64_t ldv, const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
-                   int64_t ldl, const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV, int64_t lddv,
-                   cudaStream_t st) {
-    auto k = attn_grad_kv_kernel<R, G, VW, UN>;
-    int grid;
-    int rc = grid_for(k, kBlock / G, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    k<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV,
-                               lddv);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_grad_kv_kernel launch");
-}
-
 // A d-wide row operand (vector) or a per-row scalar column (scalar): its pointer and leading dimension
 struct Operand {
     const void *p;
@@ -503,21 +461,23 @@ int hnh_sparse_attention_step_f64(const int64_t *rowStart, const int64_t *col_id
     if (v < 0) return v;
     if (v == 1) return HNH_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
     if (fast_path(d, ops)) {
-        int rc = HNH_OK;
-#define STEP(RR, G, VW, UN) \
-    rc = launch_step<RR, G, VW, UN>(rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds, st)
-        ROW_GATHER_DISPATCH(d, STEP)
+#define STEP(RR, G, VW, UN)                                                                                                \
+    {                                                                                                                      \
+        auto k = attn_step_kernel<RR, G, VW, UN>;                                                                          \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc)                                                                                                           \
+            rc = launch(k, grid, kBlock, st, "attn_step_kernel", rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, \
+                        ldm, s, lds);                                                                                      \
+    }
+        HNH_DISPATCH_R(d, STEP, )
 #undef STEP
         return rc;
     }
-    int grid = 1;
-    int rc = grid_for(attn_step_generic_kernel, kBlock / 32, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    attn_step_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m,
-                                                      ldm, s, lds);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_step_generic_kernel launch");
+    rc = grid_for(attn_step_generic_kernel, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(attn_step_generic_kernel, grid, kBlock, st, "attn_step_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, K,
+                            ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds);
 }
 
 int hnh_sparse_attention_finish_f64(int64_t rows, int d, const double *acc, int64_t ldacc, const double *m, int64_t ldm,
@@ -530,12 +490,10 @@ int hnh_sparse_attention_finish_f64(int64_t rows, int d, const double *acc, int6
         return set_error(HNH_E_INVALID, "%s: leading dimension below d = %d (rows) or 1 (scalars)", who, d);
     if (rows == 0) return HNH_OK;
     if (!acc || !m || !s || !Z || !L) return set_error(HNH_E_INVALID, "%s: null pointer", who);
-    int grid = 1;
-    int rc = grid_for(attn_finish_kernel, kBlock, rows * d, INT32_MAX, &grid);
-    if (rc) return rc;
-    attn_finish_kernel<<<grid, kBlock, 0, (cudaStream_t)stream>>>(rows, d, acc, ldacc, m, ldm, s, lds, Z, ldz, L, ldl);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_finish_kernel launch");
+    int grid = 0;
+    int rc = grid_for(attn_finish_kernel, rows * d, kBlock, &grid);
+    return rc ? rc : launch(attn_finish_kernel, grid, kBlock, (cudaStream_t)stream, "attn_finish_kernel", rows, d, acc, ldacc, m, ldm, s,
+                            lds, Z, ldz, L, ldl);
 }
 
 int hnh_sparse_attention_grad_q_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -548,21 +506,23 @@ int hnh_sparse_attention_grad_q_f64(const int64_t *rowStart, const int64_t *col_
     if (v < 0) return v;
     if (v == 1) return HNH_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
     if (fast_path(d, ops)) {
-        int rc = HNH_OK;
-#define GQ(RR, G, VW, UN) \
-    rc = launch_grad_q<RR, G, VW, UN>(rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq, st)
-        ROW_GATHER_DISPATCH(d, GQ)
+#define GQ(RR, G, VW, UN)                                                                                                  \
+    {                                                                                                                      \
+        auto k = attn_grad_q_kernel<RR, G, VW, UN>;                                                                        \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc)                                                                                                           \
+            rc = launch(k, grid, kBlock, st, "attn_grad_q_kernel", rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, \
+                        V, ldv, scale, dQ, lddq);                                                                          \
+    }
+        HNH_DISPATCH_R(d, GQ, )
 #undef GQ
         return rc;
     }
-    int grid = 1;
-    int rc = grid_for(attn_grad_q_generic_kernel, kBlock / 32, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    attn_grad_q_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V,
-                                                        ldv, scale, dQ, lddq);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_grad_q_generic_kernel launch");
+    rc = grid_for(attn_grad_q_generic_kernel, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(attn_grad_q_generic_kernel, grid, kBlock, st, "attn_grad_q_generic_kernel", rowStart, col_idx, rows, d, Q, ldq,
+                            dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq);
 }
 
 int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -575,22 +535,23 @@ int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col
     if (v < 0) return v;
     if (v == 1) return HNH_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
     if (fast_path(d, ops)) {
-        int rc = HNH_OK;
-#define GKV(RR, G, VW, UN)                                                                                                  \
-    rc = launch_grad_kv<RR, G, VW, UN>(rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, \
-                                       lddk, dV, lddv, st)
-        ROW_GATHER_DISPATCH(d, GKV)
+#define GKV(RR, G, VW, UN)                                                                                                 \
+    {                                                                                                                      \
+        auto k = attn_grad_kv_kernel<RR, G, VW, UN>;                                                                       \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc)                                                                                                           \
+            rc = launch(k, grid, kBlock, st, "attn_grad_kv_kernel", rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, \
+                        ldl, t, ldt, scale, dK, lddk, dV, lddv);                                                           \
+    }
+        HNH_DISPATCH_R(d, GKV, )
 #undef GKV
         return rc;
     }
-    int grid = 1;
-    int rc = grid_for(attn_grad_kv_generic_kernel, kBlock / 32, rows, INT32_MAX, &grid);
-    if (rc) return rc;
-    attn_grad_kv_generic_kernel<<<grid, kBlock, 0, st>>>(rowStart, col_idx, rows, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t,
-                                                         ldt, scale, dK, lddk, dV, lddv);
-    count_launch(1);
-    return check_cuda(cudaGetLastError(), "attn_grad_kv_generic_kernel launch");
+    rc = grid_for(attn_grad_kv_generic_kernel, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(attn_grad_kv_generic_kernel, grid, kBlock, st, "attn_grad_kv_generic_kernel", rowStart, col_idx, rows, d, K,
+                            ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv);
 }
 
 }  // extern "C"

@@ -2,7 +2,7 @@
 shared by tests/test_kernel_waves_gpu.py (in process) and its child processes (`python -m tests.kernel_waves_worker
 <group>`, for the paths that HNH_SPLIT_MAX_R and HNH_TMA select: the library reads them once per process).
 
-Every kernel walks its work with a grid-stride loop, and grid_for (csrc/c_abi.cu) caps the grid at the CTAs resident
+Every kernel walks its work with a grid-stride loop, and grid_for (csrc/launch.h) caps the grid at the CTAs resident
 at once, at most 8 per SM for 256-thread CTAs.  Each case is sized from its kernel's work unit per CTA so that every
 CTA runs at least WAVES iterations, which is where the later iterations, the TMA next-tile prefetch and the second
 mbarrier phase run.
@@ -21,7 +21,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-# ---- the launchers' constants (csrc/c_abi.cu; tests/test_kernel_waves.py reads them back from the source) ------------
+# ---- the launchers' constants (csrc/launch.h, row_gather.cuh, c_abi.cu; tests/test_kernel_waves.py reads them back) --
 BLOCK = 256                # kBlock: threads per CTA
 CTAS_PER_SM = 2048 // BLOCK  # the most 256-thread CTAs an SM holds, so the most grid_for ever launches per SM
 WAVES = 3                  # grid-stride iterations every CTA must run at least

@@ -16,8 +16,8 @@ from tests import gat_softmax_oracle as gso
 pytestmark = pytest.mark.gpu
 
 WAVES = 3
-GRID_PER_SM = 16  # grid_for in csrc/edge_softmax.cu and csrc/gat_additive.cu
-THREADS = 256     # kThreads
+GRID_PER_SM = 16  # kCtasPerSm in csrc/edge_softmax.cu and csrc/gat_additive.cu
+THREADS = 256     # kBlock (csrc/launch.h)
 PIECE = 1024      # kPiece: entries of a row one warp reduces
 ALPHA = 0.2
 

@@ -10,6 +10,7 @@ import pytest
 from distributed_sddmm_b200 import driver as D
 from oracle import hnh_oracle as orc
 from tests import gatv2_oracle as g2
+from tests.kernel_waves_worker import CTAS_PER_SM
 from tests.mp_edge_softmax_worker import coords
 from tests.mp_worker import gat_inputs
 
@@ -20,8 +21,6 @@ LAYERS = [[12, 8, 2], [16, 5, 3]]  # the second layer's heads are 5 wide: the ge
 ALPHA = 0.2
 EXACT_ALPHA = 0.25  # with small-integer operands every product and sum below is exact in fp64
 WIDTHS = [4, 8, 16, 32, 64, 128, 256, 7]
-# the most CTAs of 256 threads an SM holds (2048 threads per SM on sm_90)
-MAX_CTAS_PER_SM = 8
 
 
 def rel_err(got, ref):
@@ -167,8 +166,8 @@ def test_kernels_past_one_resident_wave(world, r):
     L = lib()
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     rows_per_cta = 256 // {4: 2, 64: 32}.get(r, 32)  # lanes per row: the width table, 32 for the generic kernels
-    M = 3 * MAX_CTAS_PER_SM * sms * rows_per_cta + 5
-    assert M // (MAX_CTAS_PER_SM * sms * rows_per_cta) >= 3
+    M = 3 * CTAS_PER_SM * sms * rows_per_cta + 5
+    assert M // (CTAS_PER_SM * sms * rows_per_cta) >= 3
     rng = np.random.default_rng(SEED + 100 + r)
     N = 1000
     lens = rng.integers(0, 4, M)

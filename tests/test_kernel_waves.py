@@ -1,6 +1,6 @@
 """The fixtures of the past-one-wave GPU tests, checked without a GPU: the row-length profile holds every boundary
 it claims, the operands keep every result exact in fp64, and the wave arithmetic uses the launchers' own constants
-(read back from csrc/c_abi.cu, csrc/edge_softmax.cu and csrc/gat_additive.cu)."""
+(read back from csrc/launch.h, csrc/row_gather.cuh, csrc/c_abi.cu, csrc/edge_softmax.cu and csrc/gat_additive.cu)."""
 import os
 import re
 
@@ -26,31 +26,38 @@ def _macro(src, name):
             for a in [tuple(x for x in a if x != "")]}
 
 
-def test_dispatch_tables_match_the_launchers():
-    src = _src("c_abi.cu")
-    assert re.search(r"constexpr int kBlock = (\d+);", src).group(1) == str(kw.BLOCK)
+def test_dispatch_tables_match_the_shared_launch_path():
+    launch, src = _src("launch.h"), _src("c_abi.cu")
+    assert re.search(r"constexpr int kBlock = (\d+);", launch).group(1) == str(kw.BLOCK)
     split = _macro(src, "HNH_DISPATCH_SPLIT")
     assert {r: (gk, gn, un) for r, (_, gk, gn, _, un) in split.items()} == kw.SPLIT
-    row = _macro(src, "HNH_DISPATCH_R")
+    row = _macro(_src("row_gather.cuh"), "HNH_DISPATCH_R")
     assert {r: g for r, (_, g, _, _) in row.items()} == kw.ROW_G
     # work per CTA iteration: kBlock / G rows (row kernels), kBlock / (GK * GN) (split), 8-row tiles (TMA), one row per
     # warp (generic), kBlock / G groups of G entries (COO)
-    assert "grid_for(k, kBlock, kBlock / G, rows, &grid)" in src
-    assert "grid_for(k, kBlock, kBlock / (GK * GN), rows, &grid)" in src
-    assert src.count("grid_for(k, kBlock, %d, rows, &grid)" % kw.TILE) == 2
-    assert "grid_for(sddmm_generic_kernel, kBlock, kBlock / 32, rows, &grid)" in src
-    assert "grid_for(k, kBlock, (int64_t)(kBlock / G) * G, nnz, &grid)" in src
+    assert src.count("per_cta = kBlock / G;") == 3 and src.count("grid_for(k, rows, per_cta, &grid);") == 3
+    assert src.count("per_cta = kBlock / (GK * GN);") == 3
+    assert src.count("grid_for(k, rows, %d, &grid)" % kw.TILE) == 2
+    assert "grid_for(sddmm_generic_kernel, rows, kBlock / 32, &grid)" in src
+    assert "grid_for(k, nnz, (int64_t)(kBlock / G) * G, &grid)" in src
     assert "constexpr int G = 32, VW = 2, TR = %d;" % kw.TILE in _src("kernels.cuh")
-    # grid_for never launches more than SMs x occupancy CTAs, and a 2048-thread SM holds at most 8 CTAs of 256
-    assert "int64_t cap = (int64_t)sms * occ;" in src
+    # grid_for never launches more than SMs x occupancy CTAs unless given a smaller per-SM count (the calls above are
+    # not), and a 2048-thread SM holds at most 8 CTAs of 256
+    assert "int per_sm = kResident" in launch
+    assert "cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kBlock, 0)" in launch
+    assert "(int64_t)sms * per_sm" in launch
+    assert "kCtasPerSm" not in src
     assert kw.CTAS_PER_SM * kw.BLOCK == 2048
 
 
-def test_attention_grid_caps_match_the_launchers():
+def test_attention_grid_caps_match_the_shared_launch_path():
+    assert "constexpr int kBlock = %d;" % aw.THREADS in _src("launch.h")
     for name in ("edge_softmax.cu", "gat_additive.cu"):
         src = _src(name)
-        assert "(int64_t)sms * %d" % aw.GRID_PER_SM in src, name
-        assert "constexpr int kThreads = %d;" % aw.THREADS in src, name
+        assert "constexpr int kCtasPerSm = %d;" % aw.GRID_PER_SM in src, name
+        # every grid of the file is capped at kCtasPerSm per SM, and every launch has kBlock threads
+        assert src.count("grid_for(") == src.count("&grid, kCtasPerSm)") > 0, name
+        assert src.count("launch(") == src.count(", grid, kBlock, ") > 0, name
     assert "constexpr int kPiece = %d;" % aw.PIECE in _src("edge_softmax.cu")
 
 

@@ -11,14 +11,13 @@ import pytest
 
 from distributed_sddmm_b200 import driver as D
 from tests import sparse_attention_oracle as sa
+from tests.kernel_waves_worker import CTAS_PER_SM
 from tests.mp_edge_softmax_worker import coords
 
 pytestmark = pytest.mark.gpu
 SEED = 0xC0FFEE + 21
 ALGS = ["15d_fusion1", "15d_fusion2", "15d_sparse", "25d_dense_replicate", "25d_sparse_replicate"]
 WIDTHS = [4, 8, 16, 32, 64, 128, 256, 7]
-# the most CTAs of 256 threads an SM holds (2048 threads per SM on sm_90)
-MAX_CTAS_PER_SM = 8
 KERNEL_TOL = 1e-12
 
 
@@ -280,8 +279,8 @@ def test_kernels_past_one_resident_wave(world, d):
     import torch
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     rows_per_cta = 256 // {4: 2, 64: 32}.get(d, 32)  # lanes per row: the width table, 32 for the generic kernels
-    M = 3 * MAX_CTAS_PER_SM * sms * rows_per_cta + 5
-    assert M // (MAX_CTAS_PER_SM * sms * rows_per_cta) >= 3
+    M = 3 * CTAS_PER_SM * sms * rows_per_cta + 5
+    assert M // (CTAS_PER_SM * sms * rows_per_cta) >= 3
     rng = np.random.default_rng(SEED + 100 + d)
     N = M  # the key-side pass walks N rows
     lens = rng.integers(0, 4, M)
