@@ -70,6 +70,14 @@ ABI = {
                                                   _P, _I64, C.c_double, _P, _I64, _P]),
     "hnh_sparse_attention_grad_kv_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
                                                    _P, _I64, C.c_double, _P, _I64, _P, _I64, _P]),
+    "hnh_sparse_attention_step_dropout_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, C.c_double,
+                                                        _P, _I64, _P, _I64, _P, _I64, C.c_double, C.c_uint64, _I64, _I64, _P]),
+    "hnh_sparse_attention_grad_q_dropout_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
+                                                          _P, _I64, _P, _I64, C.c_double, _P, _I64, C.c_double, C.c_uint64,
+                                                          _I64, _I64, _P]),
+    "hnh_sparse_attention_grad_kv_dropout_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
+                                                           _P, _I64, _P, _I64, C.c_double, _P, _I64, _P, _I64, C.c_double,
+                                                           C.c_uint64, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -224,6 +232,9 @@ ABI.update({
     "hnhd_alg_gatv2_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_double]),
     "hnhd_alg_sparse_attention": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_double]),
     "hnhd_alg_sparse_attention_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double]),
+    "hnhd_alg_sparse_attention_dropout": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_double, C.c_uint64]),
+    "hnhd_alg_sparse_attention_backward_dropout": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double,
+                                                             C.c_double, C.c_uint64]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),

@@ -7,6 +7,7 @@
 #include <cub/cub.cuh>
 
 #include "launch.h"
+#include "mix64.cuh"
 
 namespace {
 
@@ -20,13 +21,6 @@ using hnh::set_error;
 
 constexpr int kCtasPerSm = 8;  // grid cap of every grid-stride kernel here
 constexpr int kMaxPerRow = 128;  // columns drawn per row that one thread sorts in local memory
-
-__host__ __device__ inline uint64_t mix64(uint64_t z) {
-    z += 0x9E3779B97F4A7C15ull;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
 
 // the sorted, de-duplicated column draws of one row; returns how many are left
 __device__ inline int draw_row(uint64_t seed, uint64_t row, int per_row, uint64_t mask, uint64_t *tmp) {

@@ -693,12 +693,42 @@ void need_rows(bool rows_are_A, bool want, const char *who) {
         throw hnh::Error(HNH_E_INVALID, string(who) + ": a block of this order does not hold the " + (want ? "query" : "key") +
                                             " side as its stored rows");
 }
+// the dropout checks: a probability in [0, 1), and global S-rows and S-columns that fit the mask's 32-bit halves
+void check_dropout(const Distributed_Sparse &dist, const string &who, double dropout) {
+    if (!(dropout >= 0.0 && dropout < 1.0))
+        throw hnh::Error(HNH_E_INVALID, who + ": the dropout probability must lie in [0, 1), got " + std::to_string(dropout));
+    if (dropout > 0.0 && (dist.M > ((int64_t)1 << 32) || dist.N > ((int64_t)1 << 32)))
+        throw hnh::Error(HNH_E_INVALID, who + ": dropout keys S-rows and S-columns by 32 bits; S is " + to_string(dist.M) + " x " +
+                                            to_string(dist.N));
+}
+// The (u0, v0) of block b of `order`'s values matrix: the global S-row and S-column of its local row and column 0,
+// as the edge softmax keys its entries (entry_keys)
+struct BlockOrigin {
+    const Distributed_Sparse &dist;
+    const SpmatLocal &m;
+    BlockOrigin(const Distributed_Sparse &d, KernelMode order) : dist(d), m(*values_matrix(d, order)) {}
+    int64_t u0(int b) const { return values_row_offset(dist, m, b); }
+    int64_t v0(int b) const { return values_col_offset(dist, m, b); }
+};
 }  // namespace
 
 void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
                                          double scale) {
+    sparseAttention(Q, K, V, Z, L, heads, scale, 0.0, 0);
+}
+
+void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                                 double scale) {
+    sparseAttentionBackward(Q, K, V, Z, L, dZ, dQ, dK, dV, heads, scale, 0.0, 0);
+}
+
+void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                                         double scale, double dropout, uint64_t seed) {
     check_full_rows("sparseAttention");
     const int64_t d = check_attention(*this, "sparseAttention", {&Q, &Z}, {&K, &V}, L, heads, scale);
+    check_dropout(*this, "sparseAttention", dropout);
+    const BlockOrigin at(*this, k_sddmmA);
     // the online-softmax state of row u, head h: acc in Z's window, m in L[u, h], s in s[u, h]; m is not read while
     // s = 0, and the finish turns (acc, m, s) into (Z, L) in place
     Z.setZero();
@@ -707,13 +737,21 @@ void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMa
     for (int h = 0; h < heads; h++) {
         const vector<PassOperand> A_side{{&Q, h * d, d, false}, {&Z, h * d, d, true}, {&L, h, 1, true}, {&s, h, 1, true}};
         const vector<PassOperand> B_side{{&K, h * d, d, false}, {&V, h * d, d, false}};
-        gather_pass(k_sddmmA, A_side, B_side, [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+        gather_pass(k_sddmmA, A_side, B_side, [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
             need_rows(rows_are_A, true, "sparseAttention");
             CSRHandle *hd = blk.getActive();
-            hnh::abi_check(hnh_sparse_attention_step_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d,
-                                                         R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale, R[1].p, R[1].ld,
-                                                         R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
-                           "sparse_attention_step");
+            if (dropout == 0.0)
+                hnh::abi_check(hnh_sparse_attention_step_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
+                                                             (int)d, R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale, R[1].p,
+                                                             R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
+                               "sparse_attention_step");
+            else
+                hnh::abi_check(hnh_sparse_attention_step_dropout_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
+                                                                     blk.num_coords, (int)d, R[0].p, R[0].ld, Y[0].p, Y[0].ld,
+                                                                     Y[1].p, Y[1].ld, scale, R[1].p, R[1].ld, R[2].p, R[2].ld,
+                                                                     R[3].p, R[3].ld, dropout, seed + (uint64_t)h, at.u0(b),
+                                                                     at.v0(b), compute()),
+                               "sparse_attention_step_dropout");
         });
         hnh::abi_check(hnh_sparse_attention_finish_f64(localArows, (int)d, Z.data() + h * d, Z.cols(), L.data() + h, heads,
                                                        s.data() + h, heads, Z.data() + h * d, Z.cols(), L.data() + h, heads,
@@ -724,9 +762,11 @@ void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMa
 
 void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
                                                  DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
-                                                 double scale) {
+                                                 double scale, double dropout, uint64_t seed) {
     check_full_rows("sparseAttentionBackward");
     const int64_t d = check_attention(*this, "sparseAttentionBackward", {&Q, &Z, &dZ, &dQ}, {&K, &V, &dK, &dV}, L, heads, scale);
+    check_dropout(*this, "sparseAttentionBackward", dropout);
+    const BlockOrigin atA(*this, k_sddmmA), atB(*this, k_sddmmB);
     // t[u, h] = <dZ_u,h, Z_u,h>: Z and dZ read as localArows * heads rows of d
     DenseMatrix t(localArows, heads);
     hnh::abi_check(hnh_batch_dot_f64(t.data(), dZ.data(), Z.data(), localArows * heads, (int)d, compute()), "batch_dot");
@@ -738,26 +778,42 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
         // query rows own dQ (A order)
         gather_pass(k_sddmmA, {{&Q, w, d, false}, {&dZ, w, d, false}, {&L, h, 1, false}, {&t, h, 1, false}, {&dQ, w, d, true}},
                     {{&K, w, d, false}, {&V, w, d, false}},
-                    [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
                         need_rows(rows_are_A, true, "sparseAttentionBackward");
                         CSRHandle *hd = blk.getActive();
-                        hnh::abi_check(hnh_sparse_attention_grad_q_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
-                                                                       (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p,
-                                                                       R[3].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale, R[4].p, R[4].ld,
-                                                                       compute()),
-                                       "sparse_attention_grad_q");
+                        if (dropout == 0.0)
+                            hnh::abi_check(hnh_sparse_attention_grad_q_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
+                                                                           blk.num_coords, (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld,
+                                                                           R[2].p, R[2].ld, R[3].p, R[3].ld, Y[0].p, Y[0].ld, Y[1].p,
+                                                                           Y[1].ld, scale, R[4].p, R[4].ld, compute()),
+                                           "sparse_attention_grad_q");
+                        else
+                            hnh::abi_check(hnh_sparse_attention_grad_q_dropout_f64(
+                                               hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
+                                               R[0].ld, R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, Y[0].p, Y[0].ld, Y[1].p,
+                                               Y[1].ld, scale, R[4].p, R[4].ld, dropout, seed + (uint64_t)h, atA.u0(b), atA.v0(b),
+                                               compute()),
+                                           "sparse_attention_grad_q_dropout");
                     });
         // key rows own dK and dV (B order)
         gather_pass(k_sddmmB, {{&Q, w, d, false}, {&dZ, w, d, false}, {&L, h, 1, false}, {&t, h, 1, false}},
                     {{&K, w, d, false}, {&V, w, d, false}, {&dK, w, d, true}, {&dV, w, d, true}},
-                    [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
                         need_rows(rows_are_A, false, "sparseAttentionBackward");
                         CSRHandle *hd = blk.getActive();
-                        hnh::abi_check(hnh_sparse_attention_grad_kv_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
-                                                                        blk.num_coords, (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld, Y[0].p,
-                                                                        Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p, Y[3].ld, scale,
-                                                                        R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
-                                       "sparse_attention_grad_kv");
+                        if (dropout == 0.0)
+                            hnh::abi_check(hnh_sparse_attention_grad_kv_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
+                                                                            blk.num_coords, (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld,
+                                                                            Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p,
+                                                                            Y[3].ld, scale, R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
+                                           "sparse_attention_grad_kv");
+                        else
+                            hnh::abi_check(hnh_sparse_attention_grad_kv_dropout_f64(
+                                               hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
+                                               R[0].ld, R[1].p, R[1].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p,
+                                               Y[3].ld, scale, R[2].p, R[2].ld, R[3].p, R[3].ld, dropout, seed + (uint64_t)h,
+                                               atB.u0(b), atB.v0(b), compute()),
+                                           "sparse_attention_grad_kv_dropout");
                     });
     }
 }

@@ -384,6 +384,25 @@ int hnhd_alg_sparse_attention_backward(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dens
         a->alg->sparseAttentionBackward(Q->m, K->m, V->m, Z->m, L->m, dZ->m, dQ->m, dK->m, dV->m, heads, scale);
     });
 }
+int hnhd_alg_sparse_attention_dropout(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                      hnhd_dense_t *L, int heads, double scale, double dropout, uint64_t seed) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_dropout: null argument");
+        if (!std::isfinite(scale)) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_dropout: the scale must be finite");
+        a->alg->sparseAttention(Q->m, K->m, V->m, Z->m, L->m, heads, scale, dropout, seed);
+    });
+}
+int hnhd_alg_sparse_attention_backward_dropout(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                               hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ, hnhd_dense_t *dK,
+                                               hnhd_dense_t *dV, int heads, double scale, double dropout, uint64_t seed) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L || !dZ || !dQ || !dK || !dV)
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward_dropout: null argument");
+        if (!std::isfinite(scale))
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward_dropout: the scale must be finite");
+        a->alg->sparseAttentionBackward(Q->m, K->m, V->m, Z->m, L->m, dZ->m, dQ->m, dK->m, dV->m, heads, scale, dropout, seed);
+    });
+}
 
 int hnhd_timer_start(void) {
     return guarded([] {

@@ -15,8 +15,18 @@
 // (acc, s) to the chunk's new maximum, then the V rows.  Widths 4..256 (powers of two) with 16-byte aligned d-wide
 // operands and even leading dimensions take these; every other case takes the one-warp-per-row generic kernels.  No
 // floating-point atomics: two calls on the same device give bit-identical results.
+//
+// Attention dropout (DROP = true; the *_dropout_f64 entry points): with D_uv the keep bit of entry (u, v) and
+// w = 1 / (1 - p), the step adds D_uv w e^(x_uv - m') V_v to acc but every e^(x_uv - m') to s (L stays the
+// log-sum-exp of all scores), and the gradients use dx_uv = alpha_uv (D_uv w <dZ_u, V_v> - t_u) and
+// dV_v += sum_u D_uv w alpha_uv dZ_u.  D_uv is a hash of (seed, global u, global v) only (keep(), below), so the
+// three passes, whatever their value order, block or ring step, see the same mask.  In the fast kernels the lane
+// that loads entry k's column index hashes it and sends the bit along with what it already broadcasts: the sign of
+// its weight (step) or its column index, complemented (gradients).  A dropped entry's V row (step), V row (grad_q)
+// or dZ row (grad_kv) is not loaded.  The instantiations with DROP = false are the kernels without dropout.
 #include <cmath>
 
+#include "mix64.cuh"
 #include "row_gather.cuh"
 
 namespace {
@@ -24,6 +34,20 @@ namespace {
 using hnh::grid_for;
 using hnh::launch;
 using hnh::set_error;
+
+// The dropout of one call (include/hnh_b200.h): entry (u, v) is kept iff the high word of mix64(key ^ (u << 32 | v))
+// is at least `threshold`, key = mix64(seed); u0 and v0 are the global S-row and S-column of the block's row and
+// column 0.  The kernels without dropout receive it and do not read it.
+struct Dropout {
+    uint64_t key;
+    int64_t u0, v0;
+    double inv_keep;  // 1 / (1 - p)
+    uint32_t threshold;
+};
+
+__device__ __forceinline__ bool keep(const Dropout &dr, int64_t u, int64_t v) {
+    return (uint32_t)(mix64(dr.key ^ ((uint64_t)u << 32 | (uint64_t)v)) >> 32) >= dr.threshold;
+}
 
 template <int G>
 __device__ __forceinline__ double group_max(double d, unsigned mask) {
@@ -33,12 +57,12 @@ __device__ __forceinline__ double group_max(double d, unsigned mask) {
 }
 
 // ---- fast row kernels ----------------------------------------------------------------------------------------
-template <int R, int G, int VW, int UN>
+template <int R, int G, int VW, int UN, bool DROP>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                  const double *__restrict__ Q, int64_t ldq, const double *__restrict__ K, int64_t ldk,
                  const double *__restrict__ V, int64_t ldv, double scale, double *__restrict__ acc, int64_t ldacc,
-                 double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds) {
+                 double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds, Dropout dr) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -100,7 +124,10 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                 for (int w = 0; w < VW; w++) a[v][w] *= f;
             srow *= f;
             mrow = mnew;
-            const double pmine = gl < cnt ? exp(mine - mnew) : 0.0;
+            double pmine = gl < cnt ? exp(mine - mnew) : 0.0;
+            // a dropped entry's weight travels with its sign bit set (-0.0 included): it counts in s, not in acc
+            if constexpr (DROP)
+                if (!keep(dr, dr.u0 + row, dr.v0 + mycol)) pmine = -pmine;
             // sweep 2: the V rows, weighted
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double y[UN][NV][VW];
@@ -111,7 +138,7 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                     const int src = k < G ? k : G - 1;
                     const int64_t c = __shfl_sync(gmask, mycol, src, G);
                     pv[u] = __shfl_sync(gmask, pmine, src, G);
-                    if (k < cnt) {
+                    if (k < cnt && !(DROP && signbit(pv[u]))) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) ld_gather<VW>(y[u][v], V + c * ldv + (v * G + gl) * VW);
                     }
@@ -119,11 +146,22 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
 #pragma unroll
                 for (int u = 0; u < UN; u++) {
                     if (k0 + u < cnt) {
+                        if constexpr (DROP) {
+                            if (!signbit(pv[u])) {
+                                const double pw = pv[u] * dr.inv_keep;
 #pragma unroll
-                        for (int v = 0; v < NV; v++)
+                                for (int v = 0; v < NV; v++)
 #pragma unroll
-                            for (int w = 0; w < VW; w++) a[v][w] = fma(pv[u], y[u][v][w], a[v][w]);
-                        srow += pv[u];
+                                    for (int w = 0; w < VW; w++) a[v][w] = fma(pw, y[u][v][w], a[v][w]);
+                            }
+                            srow += fabs(pv[u]);
+                        } else {
+#pragma unroll
+                            for (int v = 0; v < NV; v++)
+#pragma unroll
+                                for (int w = 0; w < VW; w++) a[v][w] = fma(pv[u], y[u][v][w], a[v][w]);
+                            srow += pv[u];
+                        }
                     }
                 }
             }
@@ -137,13 +175,13 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
     }
 }
 
-template <int R, int G, int VW, int UN>
+template <int R, int G, int VW, int UN, bool DROP>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                    const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                    const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                    const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv, double scale,
-                   double *__restrict__ dQ, int64_t lddq) {
+                   double *__restrict__ dQ, int64_t lddq, Dropout dr) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -167,17 +205,28 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
             const int cnt = (e - j < G) ? (int)(e - j) : G;
             int64_t mycol = 0;
             if (gl < cnt) mycol = ld_stream_i64(col_idx + j + gl);
+            // a dropped entry's column index travels complemented (negative)
+            if constexpr (DROP)
+                if (!keep(dr, dr.u0 + row, dr.v0 + mycol)) mycol = ~mycol;
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double yk[UN][NV][VW], yv[UN][NV][VW];
 #pragma unroll
                 for (int u = 0; u < UN; u++) {
                     const int k = k0 + u;
-                    const int64_t c = __shfl_sync(gmask, mycol, k < G ? k : G - 1, G);
+                    int64_t c = __shfl_sync(gmask, mycol, k < G ? k : G - 1, G);
+                    const bool dropped = DROP && c < 0;
+                    if (dropped) c = ~c;
                     if (k < cnt) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) {
                             ld_gather<VW>(yk[u][v], K + c * ldk + (v * G + gl) * VW);
-                            ld_gather<VW>(yv[u][v], V + c * ldv + (v * G + gl) * VW);
+                            // a dropped entry needs no <dZ_u, V_v>: a zero V row makes it 0
+                            if (!dropped) {
+                                ld_gather<VW>(yv[u][v], V + c * ldv + (v * G + gl) * VW);
+                            } else {
+#pragma unroll
+                                for (int w = 0; w < VW; w++) yv[u][v][w] = 0.0;
+                            }
                         }
                     } else {
 #pragma unroll
@@ -199,7 +248,7 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
                     d1 = group_allreduce<G>(d1, gmask);
                     d2 = group_allreduce<G>(d2, gmask);
                     if (k0 + u < cnt) {
-                        const double dx = exp(scale * d1 - Lr) * (d2 - tr);
+                        const double dx = exp(scale * d1 - Lr) * ((DROP ? dr.inv_keep * d2 : d2) - tr);
 #pragma unroll
                         for (int v = 0; v < NV; v++)
 #pragma unroll
@@ -220,13 +269,13 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
     }
 }
 
-template <int R, int G, int VW, int UN>
+template <int R, int G, int VW, int UN, bool DROP>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                     const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
                     const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                     const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt, double scale,
-                    double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv) {
+                    double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv, Dropout dr) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -254,6 +303,9 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                 myL = L[mycol * ldl];
                 myt = t[mycol * ldt];
             }
+            // a dropped entry's column index travels complemented (negative); here u = u0 + col_idx, v = v0 + row
+            if constexpr (DROP)
+                if (!keep(dr, dr.u0 + mycol, dr.v0 + row)) mycol = ~mycol;
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double yq[UN][NV][VW], yd[UN][NV][VW];
                 double Lu[UN], tu[UN];
@@ -261,14 +313,22 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                 for (int u = 0; u < UN; u++) {
                     const int k = k0 + u;
                     const int src = k < G ? k : G - 1;
-                    const int64_t c = __shfl_sync(gmask, mycol, src, G);
+                    int64_t c = __shfl_sync(gmask, mycol, src, G);
                     Lu[u] = __shfl_sync(gmask, myL, src, G);
                     tu[u] = __shfl_sync(gmask, myt, src, G);
+                    const bool dropped = DROP && c < 0;
+                    if (dropped) c = ~c;
                     if (k < cnt) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) {
                             ld_gather<VW>(yq[u][v], Q + c * ldq + (v * G + gl) * VW);
-                            ld_gather<VW>(yd[u][v], dZ + c * lddz + (v * G + gl) * VW);
+                            // a dropped entry adds nothing to dV and needs no <V_v, dZ_u>: a zero dZ row
+                            if (!dropped) {
+                                ld_gather<VW>(yd[u][v], dZ + c * lddz + (v * G + gl) * VW);
+                            } else {
+#pragma unroll
+                                for (int w = 0; w < VW; w++) yd[u][v][w] = 0.0;
+                            }
                         }
                     } else {
 #pragma unroll
@@ -291,13 +351,14 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                     d2 = group_allreduce<G>(d2, gmask);
                     if (k0 + u < cnt) {
                         const double al = exp(scale * d1 - Lu[u]);
-                        const double dx = al * (d2 - tu[u]);
+                        const double dx = al * ((DROP ? dr.inv_keep * d2 : d2) - tu[u]);
+                        const double aw = DROP ? al * dr.inv_keep : al;
 #pragma unroll
                         for (int v = 0; v < NV; v++)
 #pragma unroll
                             for (int w = 0; w < VW; w++) {
                                 ak[v][w] = fma(dx, yq[u][v][w], ak[v][w]);
-                                av[v][w] = fma(al, yd[u][v][w], av[v][w]);
+                                av[v][w] = fma(aw, yd[u][v][w], av[v][w]);
                             }
                     }
                 }
@@ -327,11 +388,13 @@ __device__ __forceinline__ double warp_dot(const double *x, const double *y, int
     return group_allreduce<32>(acc, 0xffffffffu);
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(kBlock)
 attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                          const double *__restrict__ Q, int64_t ldq, const double *__restrict__ K, int64_t ldk,
                          const double *__restrict__ V, int64_t ldv, double scale, double *__restrict__ acc,
-                         int64_t ldacc, double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds) {
+                         int64_t ldacc, double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds,
+                         Dropout dr) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -345,7 +408,12 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
             const double x = scale * warp_dot(Q + row * ldq, K + c * ldk, d, lane);
             const double mnew = fmax(mrow, x);
             const double f = exp(mrow - mnew), pj = exp(x - mnew);
-            for (int k = lane; k < d; k += 32) a[k] = fma(pj, V[c * ldv + k], a[k] * f);
+            if (DROP && !keep(dr, dr.u0 + row, dr.v0 + c)) {
+                for (int k = lane; k < d; k += 32) a[k] *= f;
+            } else {
+                const double pw = DROP ? pj * dr.inv_keep : pj;
+                for (int k = lane; k < d; k += 32) a[k] = fma(pw, V[c * ldv + k], a[k] * f);
+            }
             srow = fma(srow, f, pj);
             mrow = mnew;
         }
@@ -356,12 +424,13 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
     }
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(kBlock)
 attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                            const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                            const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                            const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
-                           double scale, double *__restrict__ dQ, int64_t lddq) {
+                           double scale, double *__restrict__ dQ, int64_t lddq, Dropout dr) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -371,19 +440,25 @@ attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *
         for (int64_t j = s0; j < e; j++) {
             const int64_t c = col_idx[j];
             const double d1 = warp_dot(Q + row * ldq, K + c * ldk, d, lane);
-            const double d2 = warp_dot(dZ + row * lddz, V + c * ldv, d, lane);
+            double d2;  // D_uv w <dZ_u, V_v>
+            if constexpr (DROP)
+                d2 = keep(dr, dr.u0 + row, dr.v0 + c) ? dr.inv_keep * warp_dot(dZ + row * lddz, V + c * ldv, d, lane) : 0.0;
+            else
+                d2 = warp_dot(dZ + row * lddz, V + c * ldv, d, lane);
             const double g = scale * (exp(scale * d1 - Lr) * (d2 - tr));
             for (int k = lane; k < d; k += 32) dQ[row * lddq + k] = fma(g, K[c * ldk + k], dQ[row * lddq + k]);
         }
     }
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(kBlock)
 attn_grad_kv_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                             const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
                             const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                             const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
-                            double scale, double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv) {
+                            double scale, double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv,
+                            Dropout dr) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -391,12 +466,18 @@ attn_grad_kv_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t 
         for (int64_t j = s0; j < e; j++) {
             const int64_t u = col_idx[j];
             const double d1 = warp_dot(K + row * ldk, Q + u * ldq, d, lane);
+            if (DROP && !keep(dr, dr.u0 + u, dr.v0 + row)) {  // here the stored row is the key v
+                const double g = scale * (exp(scale * d1 - L[u * ldl]) * -t[u * ldt]);
+                for (int k = lane; k < d; k += 32) dK[row * lddk + k] = fma(g, Q[u * ldq + k], dK[row * lddk + k]);
+                continue;
+            }
             const double d2 = warp_dot(V + row * ldv, dZ + u * lddz, d, lane);
             const double al = exp(scale * d1 - L[u * ldl]);
-            const double g = scale * (al * (d2 - t[u * ldt]));
+            const double aw = DROP ? al * dr.inv_keep : al;
+            const double g = scale * (al * ((DROP ? dr.inv_keep * d2 : d2) - t[u * ldt]));
             for (int k = lane; k < d; k += 32) {
                 dK[row * lddk + k] = fma(g, Q[u * ldq + k], dK[row * lddk + k]);
-                dV[row * lddv + k] = fma(al, dZ[u * lddz + k], dV[row * lddv + k]);
+                dV[row * lddv + k] = fma(aw, dZ[u * lddz + k], dV[row * lddv + k]);
             }
         }
     }
@@ -447,6 +528,111 @@ bool fast_path(int d, std::initializer_list<Operand> ops) {
     return true;
 }
 
+// The Dropout of a call: HNH_OK, or HNH_E_INVALID for p outside [0, 1) (NaN included) or a negative offset
+int make_dropout(const char *who, double p, uint64_t seed, int64_t u0, int64_t v0, Dropout *dr) {
+    if (!(p >= 0.0 && p < 1.0)) return set_error(HNH_E_INVALID, "%s: the dropout probability must lie in [0, 1) (got %g)", who, p);
+    if (u0 < 0 || v0 < 0) return set_error(HNH_E_INVALID, "%s: negative row or column offset", who);
+    const double T = std::ceil(p * 4294967296.0);  // p 2^32 is exact
+    dr->threshold = T >= 4294967295.0 ? 0xffffffffu : (uint32_t)T;
+    dr->key = mix64(seed);
+    dr->u0 = u0;
+    dr->v0 = v0;
+    dr->inv_keep = 1.0 / (1.0 - p);
+    return HNH_OK;
+}
+
+template <bool DROP>
+int step(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *Q,
+         int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv, double scale, double *acc, int64_t ldacc,
+         double *m, int64_t ldm, double *s, int64_t lds, const Dropout &dr, void *stream) {
+    const std::initializer_list<Operand> ops = {{Q, ldq, true}, {K, ldk, true},   {V, ldv, true},
+                                                {acc, ldacc, true}, {m, ldm, false}, {s, lds, false}};
+    int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
+    if (v < 0) return v;
+    if (v == 1) return HNH_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
+    if (fast_path(d, ops)) {
+#define STEP(RR, G, VW, UN)                                                                                                \
+    {                                                                                                                      \
+        auto k = attn_step_kernel<RR, G, VW, UN, DROP>;                                                                    \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc)                                                                                                           \
+            rc = launch(k, grid, kBlock, st, "attn_step_kernel", rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, \
+                        ldm, s, lds, dr);                                                                                  \
+    }
+        HNH_DISPATCH_R(d, STEP, )
+#undef STEP
+        return rc;
+    }
+    auto k = attn_step_generic_kernel<DROP>;
+    rc = grid_for(k, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(k, grid, kBlock, st, "attn_step_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, K, ldk, V, ldv,
+                            scale, acc, ldacc, m, ldm, s, lds, dr);
+}
+
+template <bool DROP>
+int grad_q(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *Q,
+           int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
+           const double *K, int64_t ldk, const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq,
+           const Dropout &dr, void *stream) {
+    const std::initializer_list<Operand> ops = {{Q, ldq, true}, {dZ, lddz, true}, {L, ldl, false}, {t, ldt, false},
+                                                {K, ldk, true}, {V, ldv, true},   {dQ, lddq, true}};
+    int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
+    if (v < 0) return v;
+    if (v == 1) return HNH_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
+    if (fast_path(d, ops)) {
+#define GQ(RR, G, VW, UN)                                                                                                  \
+    {                                                                                                                      \
+        auto k = attn_grad_q_kernel<RR, G, VW, UN, DROP>;                                                                  \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc)                                                                                                           \
+            rc = launch(k, grid, kBlock, st, "attn_grad_q_kernel", rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, \
+                        V, ldv, scale, dQ, lddq, dr);                                                                      \
+    }
+        HNH_DISPATCH_R(d, GQ, )
+#undef GQ
+        return rc;
+    }
+    auto k = attn_grad_q_generic_kernel<DROP>;
+    rc = grid_for(k, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(k, grid, kBlock, st, "attn_grad_q_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, dZ, lddz, L,
+                            ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq, dr);
+}
+
+template <bool DROP>
+int grad_kv(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *K,
+            int64_t ldk, const double *V, int64_t ldv, const double *Q, int64_t ldq, const double *dZ, int64_t lddz,
+            const double *L, int64_t ldl, const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
+            int64_t lddv, const Dropout &dr, void *stream) {
+    const std::initializer_list<Operand> ops = {{K, ldk, true},   {V, ldv, true},   {Q, ldq, true},   {dZ, lddz, true},
+                                                {L, ldl, false},  {t, ldt, false},  {dK, lddk, true}, {dV, lddv, true}};
+    int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
+    if (v < 0) return v;
+    if (v == 1) return HNH_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int grid = 0, rc = HNH_OK;
+    if (fast_path(d, ops)) {
+#define GKV(RR, G, VW, UN)                                                                                                 \
+    {                                                                                                                      \
+        auto k = attn_grad_kv_kernel<RR, G, VW, UN, DROP>;                                                                 \
+        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
+        if (!rc)                                                                                                           \
+            rc = launch(k, grid, kBlock, st, "attn_grad_kv_kernel", rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, \
+                        ldl, t, ldt, scale, dK, lddk, dV, lddv, dr);                                                       \
+    }
+        HNH_DISPATCH_R(d, GKV, )
+#undef GKV
+        return rc;
+    }
+    auto k = attn_grad_kv_generic_kernel<DROP>;
+    rc = grid_for(k, rows, kBlock / 32, &grid);
+    return rc ? rc : launch(k, grid, kBlock, st, "attn_grad_kv_generic_kernel", rowStart, col_idx, rows, d, K, ldk, V, ldv, Q,
+                            ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, dr);
+}
+
 }  // namespace
 
 extern "C" {
@@ -455,29 +641,20 @@ int hnh_sparse_attention_step_f64(const int64_t *rowStart, const int64_t *col_id
                                   const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv,
                                   double scale, double *acc, int64_t ldacc, double *m, int64_t ldm, double *s, int64_t lds,
                                   void *stream) {
-    const std::initializer_list<Operand> ops = {{Q, ldq, true}, {K, ldk, true},   {V, ldv, true},
-                                                {acc, ldacc, true}, {m, ldm, false}, {s, lds, false}};
-    int v = check_call("hnh_sparse_attention_step_f64", rowStart, col_idx, rows, nnz, d, scale, ops);
-    if (v < 0) return v;
-    if (v == 1) return HNH_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    int grid = 0, rc = HNH_OK;
-    if (fast_path(d, ops)) {
-#define STEP(RR, G, VW, UN)                                                                                                \
-    {                                                                                                                      \
-        auto k = attn_step_kernel<RR, G, VW, UN>;                                                                          \
-        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
-        if (!rc)                                                                                                           \
-            rc = launch(k, grid, kBlock, st, "attn_step_kernel", rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, \
-                        ldm, s, lds);                                                                                      \
-    }
-        HNH_DISPATCH_R(d, STEP, )
-#undef STEP
-        return rc;
-    }
-    rc = grid_for(attn_step_generic_kernel, rows, kBlock / 32, &grid);
-    return rc ? rc : launch(attn_step_generic_kernel, grid, kBlock, st, "attn_step_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, K,
-                            ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds);
+    return step<false>("hnh_sparse_attention_step_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc,
+                       ldacc, m, ldm, s, lds, Dropout{}, stream);
+}
+
+int hnh_sparse_attention_step_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                          const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V,
+                                          int64_t ldv, double scale, double *acc, int64_t ldacc, double *m, int64_t ldm,
+                                          double *s, int64_t lds, double p, uint64_t seed, int64_t u0, int64_t v0,
+                                          void *stream) {
+    const char *who = "hnh_sparse_attention_step_dropout_f64";
+    Dropout dr;
+    const int rc = make_dropout(who, p, seed, u0, v0, &dr);
+    return rc ? rc : step<true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds,
+                                dr, stream);
 }
 
 int hnh_sparse_attention_finish_f64(int64_t rows, int d, const double *acc, int64_t ldacc, const double *m, int64_t ldm,
@@ -500,58 +677,40 @@ int hnh_sparse_attention_grad_q_f64(const int64_t *rowStart, const int64_t *col_
                                     const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
                                     const double *t, int64_t ldt, const double *K, int64_t ldk, const double *V, int64_t ldv,
                                     double scale, double *dQ, int64_t lddq, void *stream) {
-    const std::initializer_list<Operand> ops = {{Q, ldq, true}, {dZ, lddz, true}, {L, ldl, false}, {t, ldt, false},
-                                                {K, ldk, true}, {V, ldv, true},   {dQ, lddq, true}};
-    int v = check_call("hnh_sparse_attention_grad_q_f64", rowStart, col_idx, rows, nnz, d, scale, ops);
-    if (v < 0) return v;
-    if (v == 1) return HNH_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    int grid = 0, rc = HNH_OK;
-    if (fast_path(d, ops)) {
-#define GQ(RR, G, VW, UN)                                                                                                  \
-    {                                                                                                                      \
-        auto k = attn_grad_q_kernel<RR, G, VW, UN>;                                                                        \
-        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
-        if (!rc)                                                                                                           \
-            rc = launch(k, grid, kBlock, st, "attn_grad_q_kernel", rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, \
-                        V, ldv, scale, dQ, lddq);                                                                          \
-    }
-        HNH_DISPATCH_R(d, GQ, )
-#undef GQ
-        return rc;
-    }
-    rc = grid_for(attn_grad_q_generic_kernel, rows, kBlock / 32, &grid);
-    return rc ? rc : launch(attn_grad_q_generic_kernel, grid, kBlock, st, "attn_grad_q_generic_kernel", rowStart, col_idx, rows, d, Q, ldq,
-                            dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq);
+    return grad_q<false>("hnh_sparse_attention_grad_q_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K,
+                         ldk, V, ldv, scale, dQ, lddq, Dropout{}, stream);
+}
+
+int hnh_sparse_attention_grad_q_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                            const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
+                                            int64_t ldl, const double *t, int64_t ldt, const double *K, int64_t ldk,
+                                            const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq, double p,
+                                            uint64_t seed, int64_t u0, int64_t v0, void *stream) {
+    const char *who = "hnh_sparse_attention_grad_q_dropout_f64";
+    Dropout dr;
+    const int rc = make_dropout(who, p, seed, u0, v0, &dr);
+    return rc ? rc : grad_q<true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale,
+                                  dQ, lddq, dr, stream);
 }
 
 int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
                                      const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q, int64_t ldq,
                                      const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
                                      double scale, double *dK, int64_t lddk, double *dV, int64_t lddv, void *stream) {
-    const std::initializer_list<Operand> ops = {{K, ldk, true},   {V, ldv, true},   {Q, ldq, true},   {dZ, lddz, true},
-                                                {L, ldl, false},  {t, ldt, false},  {dK, lddk, true}, {dV, lddv, true}};
-    int v = check_call("hnh_sparse_attention_grad_kv_f64", rowStart, col_idx, rows, nnz, d, scale, ops);
-    if (v < 0) return v;
-    if (v == 1) return HNH_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    int grid = 0, rc = HNH_OK;
-    if (fast_path(d, ops)) {
-#define GKV(RR, G, VW, UN)                                                                                                 \
-    {                                                                                                                      \
-        auto k = attn_grad_kv_kernel<RR, G, VW, UN>;                                                                       \
-        rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
-        if (!rc)                                                                                                           \
-            rc = launch(k, grid, kBlock, st, "attn_grad_kv_kernel", rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, \
-                        ldl, t, ldt, scale, dK, lddk, dV, lddv);                                                           \
-    }
-        HNH_DISPATCH_R(d, GKV, )
-#undef GKV
-        return rc;
-    }
-    rc = grid_for(attn_grad_kv_generic_kernel, rows, kBlock / 32, &grid);
-    return rc ? rc : launch(attn_grad_kv_generic_kernel, grid, kBlock, st, "attn_grad_kv_generic_kernel", rowStart, col_idx, rows, d, K,
-                            ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv);
+    return grad_kv<false>("hnh_sparse_attention_grad_kv_f64", rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz,
+                          L, ldl, t, ldt, scale, dK, lddk, dV, lddv, Dropout{}, stream);
+}
+
+int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                             const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q,
+                                             int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
+                                             const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
+                                             int64_t lddv, double p, uint64_t seed, int64_t u0, int64_t v0, void *stream) {
+    const char *who = "hnh_sparse_attention_grad_kv_dropout_f64";
+    Dropout dr;
+    const int rc = make_dropout(who, p, seed, u0, v0, &dr);
+    return rc ? rc : grad_kv<true>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale,
+                                   dK, lddk, dV, lddv, dr, stream);
 }
 
 }  // extern "C"

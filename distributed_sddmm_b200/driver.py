@@ -16,6 +16,7 @@ from __future__ import annotations
 import ctypes as C
 import json
 import math
+import numbers
 import os
 
 import numpy as np
@@ -305,20 +306,42 @@ class Algorithm:
             raise ValueError(f"heads = {heads} must divide the width {r}")
         return 1.0 / math.sqrt(r // heads)
 
-    def sparse_attention(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, heads: int = 1, scale=None):
+    @staticmethod
+    def _dropout_args(dropout, seed):
+        """(dropout, seed) as the C ABI takes them: a probability in [0, 1) and an integer in [0, 2^64)."""
+        p = float(dropout)
+        if not 0.0 <= p < 1.0:
+            raise ValueError(f"dropout = {dropout} must lie in [0, 1)")
+        if isinstance(seed, bool) or not isinstance(seed, numbers.Integral) or not 0 <= seed < 1 << 64:
+            raise ValueError(f"seed = {seed!r} must be an integer in [0, 2^64)")
+        return p, int(seed)
+
+    def sparse_attention(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, heads: int = 1, scale=None,
+                         dropout: float = 0.0, seed: int = 0):
         """Collective: fused attention over the pattern of S (its values are not read).  Q and Z are A-shaped, K and V
         B-shaped, all r wide; per head h of width d = r / heads, Z_u,h = sum over the stored (u, v) of
         softmax_v(scale <Q_u,h, K_v,h>) V_v,h, and L (Dense.create(localArows, heads)) = the rows' log-sum-exp (-inf,
-        and Z = 0, for a row without entries).  scale=None means 1/sqrt(d) (Distributed_Sparse::sparseAttention)."""
+        and Z = 0, for a row without entries).  scale=None means 1/sqrt(d) (Distributed_Sparse::sparseAttention).
+
+        dropout in [0, 1) drops each attention coefficient with that probability and scales the kept ones by
+        1 / (1 - dropout), as torch.nn.functional.dropout(softmax(x)) @ V does; L is still the log-sum-exp of all
+        scores.  The mask is a hash of (seed, head, global S-row, global S-column), so it does not depend on the
+        algorithm or the number of ranks, and duplicate stored (u, v) share one keep bit.  Every rank must pass the
+        same dropout and seed, and sparse_attention_backward must get the ones its forward got."""
         s = self._attention_scale(Q, heads, scale)
-        check(lib().hnhd_alg_sparse_attention(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s), "sparse_attention")
+        p, sd = self._dropout_args(dropout, seed)
+        check(lib().hnhd_alg_sparse_attention_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s, p, sd),
+              "sparse_attention")
 
     def sparse_attention_backward(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, dZ: Dense, dQ: Dense, dK: Dense,
-                                  dV: Dense, heads: int = 1, scale=None):
+                                  dV: Dense, heads: int = 1, scale=None, dropout: float = 0.0, seed: int = 0):
         """Collective: given dZ = dLoss/dZ and the forward's Z and L, overwrites dQ, dK and dV with the gradients of
-        sparse_attention (Distributed_Sparse::sparseAttentionBackward)."""
+        sparse_attention (Distributed_Sparse::sparseAttentionBackward).  dropout and seed must be the ones the forward
+        got, and the same on every rank: the backward regenerates the forward's mask from them."""
         s = self._attention_scale(Q, heads, scale)
-        check(lib().hnhd_alg_sparse_attention_backward(self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h, int(heads), s),
+        p, sd = self._dropout_args(dropout, seed)
+        check(lib().hnhd_alg_sparse_attention_backward_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h,
+                                                               int(heads), s, p, sd),
               "sparse_attention_backward")
 
     def initial_shift(self, A, B, mode):

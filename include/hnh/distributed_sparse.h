@@ -217,6 +217,20 @@ public:
     void sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
                                  DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
                                  double scale);
+    // The same with attention dropout of probability `dropout` in [0, 1): with D_uv,h the keep bit of the stored
+    // (u, v) in head h and w = 1 / (1 - dropout),
+    //     Z_u,h = sum_v D_uv,h w alpha_uv V_v,h,  with L_u,h still the log-sum-exp of all scores, and
+    //     dx_uv = alpha_uv (D_uv,h w <dZ_u,h, V_v,h> - t_u,h),  dV_v,h = sum_u D_uv,h w alpha_uv dZ_u,h.
+    // D_uv,h is the mask of hnh_sparse_attention_step_dropout_f64 (include/hnh_b200.h) at seed + h and the global
+    // S-row u and S-column v, so it is the same on every layout, and stored duplicates of (u, v) share it.  A
+    // backward must get the forward's dropout and seed, and every rank the same values.  dropout = 0 runs the
+    // kernels without dropout (the overloads above forward here with (0, 0)).  dropout outside [0, 1), NaN, or,
+    // with dropout > 0, S wider or taller than 2^32: HNH_E_INVALID on every rank before any launch.
+    void sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                         double scale, double dropout, uint64_t seed);
+    void sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                 double scale, double dropout, uint64_t seed);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

@@ -296,6 +296,38 @@ int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col
                                      int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
                                      const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
                                      int64_t lddv, void *stream);
+/* Attention dropout: the same three calls with (p, seed, u0, v0) before the stream.  Entry (u, v) has the global
+ * query row u and key row v: step and grad_q, u = u0 + stored row, v = v0 + col_idx[i]; grad_kv, u = u0 + col_idx[i],
+ * v = v0 + stored row; u and v below 2^32.  Its keep bit is
+ *     D_uv = (uint32_t)(mix64(mix64(seed) ^ ((uint64_t)u << 32 | (uint64_t)v)) >> 32) >= T,
+ *     T = min(ceil(p 2^32), 2^32 - 1),
+ * with mix64 the splitmix64 finaliser: z += 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ * z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31).  So p = 0 keeps every entry, the keep probability
+ * is exactly 1 - T / 2^32, and the mask is a function of (seed, u, v) alone: not of an entry's position, its block
+ * or the call, so the three passes see the same mask, and stored duplicates of one (u, v) share one bit.
+ * Distributed_Sparse::sparseAttention passes seed + h for head h.  With w = 1 / (1 - p):
+ * step: s' as above (every entry counts, so L stays the log-sum-exp of all scores), and
+ *     acc' = e^(m - m') acc + sum_i D_i w e^(x_i - m') V_v   (finish is unchanged: Z = sum_v D_uv w alpha_uv V_v);
+ * grad_q, grad_kv: dx_uv = alpha_uv (D_uv w <dZ_u, V_v> - t_u), and dV_v += sum_u D_uv w alpha_uv dZ_u.
+ * p < 0, p >= 1, NaN, u0 < 0 or v0 < 0: HNH_E_INVALID before any launch.  At p = 0 the results are bit-identical
+ * to the calls without dropout. */
+int hnh_sparse_attention_step_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                                          int d, const double *Q, int64_t ldq, const double *K, int64_t ldk,
+                                          const double *V, int64_t ldv, double scale, double *acc, int64_t ldacc,
+                                          double *m, int64_t ldm, double *s, int64_t lds, double p, uint64_t seed,
+                                          int64_t u0, int64_t v0, void *stream);
+int hnh_sparse_attention_grad_q_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows,
+                                            int64_t nnz, int d, const double *Q, int64_t ldq, const double *dZ,
+                                            int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
+                                            const double *K, int64_t ldk, const double *V, int64_t ldv, double scale,
+                                            double *dQ, int64_t lddq, double p, uint64_t seed, int64_t u0, int64_t v0,
+                                            void *stream);
+int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows,
+                                             int64_t nnz, int d, const double *K, int64_t ldk, const double *V,
+                                             int64_t ldv, const double *Q, int64_t ldq, const double *dZ, int64_t lddz,
+                                             const double *L, int64_t ldl, const double *t, int64_t ldt, double scale,
+                                             double *dK, int64_t lddk, double *dV, int64_t lddv, double p,
+                                             uint64_t seed, int64_t u0, int64_t v0, void *stream);
 
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of

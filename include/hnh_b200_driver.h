@@ -191,6 +191,18 @@ int hnhd_alg_sparse_attention(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K,
 int hnhd_alg_sparse_attention_backward(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V,
                                        hnhd_dense_t *Z, hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ,
                                        hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale);
+/* The same with attention dropout of probability `dropout` in [0, 1) (Distributed_Sparse::sparseAttention with
+ * dropout and seed): the kept entries' alpha is scaled by 1 / (1 - dropout), L stays the log-sum-exp of all scores,
+ * and the mask of head h is that of hnh_sparse_attention_step_dropout_f64 at seed + h and the global S-row and
+ * S-column.  The backward must get its forward's dropout and seed, and every rank the same values.  dropout = 0
+ * equals the calls above.  HNH_E_INVALID as above, and for dropout outside [0, 1) or NaN. */
+int hnhd_alg_sparse_attention_dropout(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V,
+                                      hnhd_dense_t *Z, hnhd_dense_t *L, int heads, double scale, double dropout,
+                                      uint64_t seed);
+int hnhd_alg_sparse_attention_backward_dropout(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V,
+                                               hnhd_dense_t *Z, hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ,
+                                               hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale,
+                                               double dropout, uint64_t seed);
 
 /* CUDA-event timing on the library's compute stream: start, ..., stop -> milliseconds. */
 int hnhd_timer_start(void);

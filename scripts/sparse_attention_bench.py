@@ -17,7 +17,13 @@ sparse_attention_backward beside the composed public ops -- forward: scaled sddm
 alpha in both orders (2 scaled SDDMMs, 2 softmaxes), dalpha in both orders (2 SDDMMs), 2 softmax backwards and the
 dV, dQ, dK SpMMs -- with the composed path's first edge_softmax per order (which builds its row grouping) timed
 separately, and the largest relative difference between the two.  Prints the card name and power limit, then one
-JSON line per measurement.  Environment: LOGM (20), NPR (32), WIDTHS (128,256), ALG (15d_fusion1), REPS (20)."""
+JSON line per measurement.
+
+Attention dropout at DROPOUT (0.1): each of the three dropout kernels (hnh_sparse_attention_*_dropout_f64) beside its
+kernel without dropout on the same block and operands, the two timed in alternation ROUNDS (5) times, REPS launches
+each, with the median of each and their ratio; then Algorithm.sparse_attention and sparse_attention_backward with and
+without dropout, alternated the same way.  PARTS (kernels,ops,dropout) picks the sections.
+Environment: LOGM (20), NPR (32), WIDTHS (128,256), ALG (15d_fusion1), REPS (20), DROPOUT (0.1), ROUNDS (5), PARTS."""
 import json
 import math
 import os
@@ -38,6 +44,9 @@ npr = int(os.environ.get("NPR", "32"))
 widths = [int(x) for x in os.environ.get("WIDTHS", "128,256").split(",")]
 alg_name = os.environ.get("ALG", "15d_fusion1")
 reps = int(os.environ.get("REPS", "20"))
+dropout = float(os.environ.get("DROPOUT", "0.1"))
+rounds = int(os.environ.get("ROUNDS", "5"))
+parts = os.environ.get("PARTS", "kernels,ops,dropout").split(",")
 HBM = 3.35e12
 BETA0 = 4
 
@@ -192,10 +201,85 @@ def ops(d):
     del alg
 
 
+def alternate(name, d, plain, dropped, timer=timed, nbytes=None):
+    """plain and dropped timed in turn `rounds` times; their medians and ratio."""
+    a, b = [], []
+    for _ in range(rounds):
+        a.append(timer(plain))
+        b.append(timer(dropped))
+    ma, mb = float(np.median(a)), float(np.median(b))
+    report(name, d, ma, nbytes, dropout=0.0, spread=[round(min(a), 4), round(max(a), 4)])
+    report(name + "_dropout", d, mb, nbytes, dropout=dropout, spread=[round(min(b), 4), round(max(b), 4)])
+    return mb / ma
+
+
+def dropout_kernels(alg, d):
+    a_blk, b_blk = ("ST", "S") if alg_name == "15d_fusion1" else ("S", "ST")
+    rows, nnz, rs, ci = block(alg, a_blk)
+    rowsT, nnzT, rsT, ciT = block(alg, b_blk)
+    g = torch.Generator(device=dev).manual_seed(1)
+    n = max(rows, rowsT)
+    Q, K, V, dZ = (torch.rand((n, d), generator=g, **f64) * 2 - 1 for _ in range(4))
+    acc, dQ, dK, dV = (torch.zeros((n, d), **f64) for _ in range(4))
+    ms_ = torch.zeros((rows, 2), **f64)
+    Lt = torch.rand((n, 2), generator=g, **f64) + 4  # L, t: a plausible log-sum-exp of 32 entries, and <dZ, Z>
+    scale = 1 / math.sqrt(d)
+    p = lambda t: t.data_ptr()  # noqa: E731
+    drop = (dropout, SEED, 0, 0)
+
+    def step(*dr):
+        fn = L.hnh_sparse_attention_step_dropout_f64 if dr else L.hnh_sparse_attention_step_f64
+        D.check(fn(p(rs), p(ci), rows, nnz, d, p(Q), d, p(K), d, p(V), d, scale, p(acc), d, p(ms_), 2, p(ms_) + 8, 2, *dr, st))
+
+    def grad_q(*dr):
+        fn = L.hnh_sparse_attention_grad_q_dropout_f64 if dr else L.hnh_sparse_attention_grad_q_f64
+        D.check(fn(p(rs), p(ci), rows, nnz, d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, p(K), d, p(V), d, scale, p(dQ), d,
+                   *dr, st))
+
+    def grad_kv(*dr):
+        fn = L.hnh_sparse_attention_grad_kv_dropout_f64 if dr else L.hnh_sparse_attention_grad_kv_f64
+        D.check(fn(p(rsT), p(ciT), rowsT, nnzT, d, p(K), d, p(V), d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, scale, p(dK), d,
+                   p(dV), d, *dr, st))
+
+    ratios = {}
+    for name, fn, nbytes in (("step", step, nnz * (8 + 16 * d) + rows * (8 + 24 * d + 32)),
+                             ("grad_q", grad_q, nnz * (8 + 16 * d) + rows * (8 + 32 * d + 16)),
+                             ("grad_kv", grad_kv, nnzT * (24 + 16 * d) + rowsT * (8 + 48 * d))):
+        ratios[name] = round(alternate(name, d, fn, lambda fn=fn: fn(*drop), nbytes=nbytes), 3)
+    print(json.dumps(dict(d=d, dropout=dropout, dropout_kernel_over_kernel=ratios)), flush=True)
+
+
+def dropout_ops(d):
+    alg = D.Algorithm(alg_name, S, d, 1)
+    dims = alg.dims
+    rng = np.random.default_rng(SEED)
+    Q, dZ = (alg.like_A_matrix() for _ in range(2))
+    K, V = (alg.like_B_matrix() for _ in range(2))
+    for m in (Q, dZ, K, V):
+        m.from_host(rng.uniform(-1, 1, m.shape))
+    Z, dQ, dK, dV = alg.like_A_matrix(), alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix()
+    Lm = D.Dense.create(dims.localArows, 1)
+    kw = dict(dropout=dropout, seed=SEED)
+    fwd = alternate("op_fused_forward", d, lambda: alg.sparse_attention(Q, K, V, Z, Lm),
+                    lambda: alg.sparse_attention(Q, K, V, Z, Lm, **kw), timer=timed_op)
+    alg.sparse_attention(Q, K, V, Z, Lm, **kw)
+    bwd = alternate("op_fused_backward", d, lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV),
+                    lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV, **kw), timer=timed_op)
+    print(json.dumps(dict(d=d, dropout=dropout, forward_dropout_over_forward=round(fwd, 3),
+                          backward_dropout_over_backward=round(bwd, 3))), flush=True)
+    del alg
+
+
 for d in widths:
     alg = D.Algorithm(alg_name, S, d, 1)
-    kernels(alg, d)
+    if "kernels" in parts:
+        kernels(alg, d)
+    if "dropout" in parts:
+        dropout_kernels(alg, d)
     del alg
     torch.cuda.empty_cache()
-    ops(d)
+    if "ops" in parts:
+        ops(d)
+    if "dropout" in parts:
+        dropout_ops(d)
 D.world_finalize()
