@@ -265,25 +265,33 @@ int64_t values_col_offset(const Distributed_Sparse &d, const SpmatLocal &m, int 
     return &m == d.ST.get() ? (int64_t)d.grid->i * d.localBrows * d.c : (int64_t)block * d.localBrows;
 }
 
-// keys[i] = the global S-row (columns == false) or S-column (columns == true) of entry i of a value vector of `order`
-// with n entries, from the CSR blocks that hold that order
-void entry_keys(Distributed_Sparse &d, KernelMode order, int64_t n, int32_t *keys, bool columns, cudaStream_t s) {
+// For each block of a value vector of `order` with n entries that has entries: fn(its first entry, its entry count,
+// the index array that holds its entries' local S-rows (columns == false) or S-columns (columns == true), and the
+// offset that makes them global), from the CSR blocks that hold that order
+template <typename F>
+void for_entry_index(Distributed_Sparse &d, KernelMode order, int64_t n, bool columns, const string &who, F fn) {
     SpmatLocal &m = *values_matrix(d, order);
     const bool is_ST = &m == d.ST.get();
-    if ((int64_t)m.blockStarts.back() != n)
-        throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: the value vector does not cover the local blocks");
+    if ((int64_t)m.blockStarts.back() != n) throw hnh::Error(HNH_E_INVALID, who + ": the value vector does not cover the local blocks");
     for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
         const int64_t off = (int64_t)m.blockStarts[b], nb = (int64_t)m.blockStarts[b + 1] - off;
         if (nb == 0) continue;
         CSRLocal *blk = m.csr_blocks[b];
         if (blk == nullptr || blk->num_coords != nb)
-            throw hnh::Error(HNH_E_INVALID, "edgeSoftmax: block " + to_string(b) + " does not match its value range");
+            throw hnh::Error(HNH_E_INVALID, who + ": block " + to_string(b) + " does not match its value range");
         // S stores its rows as rows, ST as columns; a transposed block swaps the two
         const bool stored_row = (is_ST == blk->transpose) != columns;
         const int64_t *idx = stored_row ? blk->row_idx_device() : blk->getActive()->col_idx.data();
-        const int64_t offset = columns ? values_col_offset(d, m, (int)b) : values_row_offset(d, m, (int)b);
-        hnh::abi_check(hnh_edge_keys_from_index(keys + off, idx, nb, offset, s), "edge_keys_from_index");
+        fn(off, nb, idx, columns ? values_col_offset(d, m, (int)b) : values_row_offset(d, m, (int)b));
     }
+}
+
+// keys[i] = the global S-row (columns == false) or S-column (columns == true) of entry i of a value vector of `order`
+// with n entries
+void entry_keys(Distributed_Sparse &d, KernelMode order, int64_t n, int32_t *keys, bool columns, cudaStream_t s) {
+    for_entry_index(d, order, n, columns, "edgeSoftmax", [&](int64_t off, int64_t nb, const int64_t *idx, int64_t offset) {
+        hnh::abi_check(hnh_edge_keys_from_index(keys + off, idx, nb, offset, s), "edge_keys_from_index");
+    });
 }
 
 EdgeRows &edge_rows(Distributed_Sparse &d, KernelMode order, int64_t n) {
@@ -352,6 +360,21 @@ EdgeRows &edge_col_plan(Distributed_Sparse &d, int64_t n) {
 }
 
 }  // namespace
+
+void Distributed_Sparse::entryCoordinates(KernelMode order, VectorXd &rows, VectorXd &cols) {
+    check_full_rows("entryCoordinates");
+    if (order != k_sddmmA && order != k_sddmmB)
+        throw hnh::Error(HNH_E_INVALID, "entryCoordinates: the value order must be k_sddmmA or k_sddmmB");
+    const int64_t n = order == k_sddmmA ? num_S_values() : num_ST_values();
+    rows.resize(n);
+    cols.resize(n);
+    for (bool columns : {false, true}) {
+        double *out = columns ? cols.data() : rows.data();
+        for_entry_index(*this, order, n, columns, "entryCoordinates", [&](int64_t off, int64_t nb, const int64_t *idx, int64_t offset) {
+            hnh::abi_check(hnh_entry_coords_from_index_f64(out + off, idx, nb, offset, compute()), "entry_coords_from_index");
+        });
+    }
+}
 
 void Distributed_Sparse::release_edge_softmax() {
     std::lock_guard<std::mutex> lock(edge_rows_mutex);
@@ -710,6 +733,36 @@ struct BlockOrigin {
     int64_t u0(int b) const { return values_row_offset(dist, m, b); }
     int64_t v0(int b) const { return values_col_offset(dist, m, b); }
 };
+// A bias vector of `order` as sparseAttention reads it: block b of head h starts at at(h, b)
+struct BiasView {
+    const VectorXd *v = nullptr;
+    VectorXd *grad = nullptr;
+    const SpmatLocal *m = nullptr;
+    int64_t head_stride = 0;  // n for a per-head bias, 0 for a shared one
+    const double *at(int h, int b) const { return v->data() + h * head_stride + (int64_t)m->blockStarts[(size_t)b]; }
+    double *grad_at(int h, int b) const {
+        return grad ? grad->data() + h * head_stride + (int64_t)m->blockStarts[(size_t)b] : nullptr;
+    }
+};
+// The head multiplicity of a bias of `order`: 1 (shared), heads (per head) or 0 (either: the order has no local
+// entries); HNH_E_INVALID for any other length
+int64_t bias_heads(Distributed_Sparse &d, const string &who, const char *name, const VectorXd &b, KernelMode order, int heads) {
+    const int64_t n = order == k_sddmmA ? d.num_S_values() : d.num_ST_values();
+    if (n == 0 && b.size() == 0) return 0;
+    if (b.size() == n) return 1;
+    if (b.size() == (int64_t)heads * n) return heads;
+    throw hnh::Error(HNH_E_INVALID, who + ": " + name + " has " + to_string(b.size()) + " entries; its order has " + to_string(n) +
+                                        " per head and there are " + to_string(heads) + " heads");
+}
+BiasView bias_view(Distributed_Sparse &d, const VectorXd *b, VectorXd *grad, KernelMode order, int64_t multiplicity) {
+    BiasView v;
+    if (b == nullptr) return v;
+    v.v = b;
+    v.grad = grad;
+    v.m = values_matrix(d, order);
+    v.head_stride = multiplicity > 1 ? (order == k_sddmmA ? d.num_S_values() : d.num_ST_values()) : 0;
+    return v;
+}
 }  // namespace
 
 void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
@@ -725,9 +778,22 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
 
 void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
                                          double scale, double dropout, uint64_t seed) {
+    sparseAttention(Q, K, V, Z, L, heads, scale, dropout, seed, nullptr);
+}
+
+void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                                 double scale, double dropout, uint64_t seed) {
+    sparseAttentionBackward(Q, K, V, Z, L, dZ, dQ, dK, dV, heads, scale, dropout, seed, nullptr, nullptr, nullptr, nullptr);
+}
+
+void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                                         double scale, double dropout, uint64_t seed, const VectorXd *bias) {
     check_full_rows("sparseAttention");
     const int64_t d = check_attention(*this, "sparseAttention", {&Q, &Z}, {&K, &V}, L, heads, scale);
     check_dropout(*this, "sparseAttention", dropout);
+    const BiasView bv =
+        bias_view(*this, bias, nullptr, k_sddmmA, bias ? bias_heads(*this, "sparseAttention", "the bias", *bias, k_sddmmA, heads) : 0);
     const BlockOrigin at(*this, k_sddmmA);
     // the online-softmax state of row u, head h: acc in Z's window, m in L[u, h], s in s[u, h]; m is not read while
     // s = 0, and the finish turns (acc, m, s) into (Z, L) in place
@@ -740,7 +806,13 @@ void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMa
         gather_pass(k_sddmmA, A_side, B_side, [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
             need_rows(rows_are_A, true, "sparseAttention");
             CSRHandle *hd = blk.getActive();
-            if (dropout == 0.0)
+            if (bias)
+                hnh::abi_check(hnh_sparse_attention_step_bias_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
+                                                                  (int)d, R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale,
+                                                                  R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, dropout,
+                                                                  seed + (uint64_t)h, at.u0(b), at.v0(b), bv.at(h, b), compute()),
+                               "sparse_attention_step_bias");
+            else if (dropout == 0.0)
                 hnh::abi_check(hnh_sparse_attention_step_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
                                                              (int)d, R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale, R[1].p,
                                                              R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, compute()),
@@ -762,11 +834,34 @@ void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMa
 
 void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
                                                  DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
-                                                 double scale, double dropout, uint64_t seed) {
-    check_full_rows("sparseAttentionBackward");
-    const int64_t d = check_attention(*this, "sparseAttentionBackward", {&Q, &Z, &dZ, &dQ}, {&K, &V, &dK, &dV}, L, heads, scale);
-    check_dropout(*this, "sparseAttentionBackward", dropout);
+                                                 double scale, double dropout, uint64_t seed, const VectorXd *bias_A,
+                                                 const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B) {
+    const string who = "sparseAttentionBackward";
+    check_full_rows(who);
+    const int64_t d = check_attention(*this, who, {&Q, &Z, &dZ, &dQ}, {&K, &V, &dK, &dV}, L, heads, scale);
+    check_dropout(*this, who, dropout);
+    if ((bias_A == nullptr) != (bias_B == nullptr))
+        throw hnh::Error(HNH_E_INVALID, who + ": a bias needs both orders, bias_A and bias_B");
+    if ((dbias_A && !bias_A) || (dbias_B && !bias_B)) throw hnh::Error(HNH_E_INVALID, who + ": a bias gradient without its bias");
+    for (const VectorXd *g : {(const VectorXd *)dbias_A, (const VectorXd *)dbias_B})
+        if (g && (g == bias_A || g == bias_B)) throw hnh::Error(HNH_E_INVALID, who + ": a bias gradient may not be a bias");
+    if (dbias_A && dbias_A == dbias_B) throw hnh::Error(HNH_E_INVALID, who + ": dbias_A and dbias_B are one vector");
+    const bool with_bias = bias_A != nullptr;
+    int64_t mA = 0, mB = 0;
+    if (with_bias) {
+        mA = bias_heads(*this, who, "bias_A", *bias_A, k_sddmmA, heads);
+        mB = bias_heads(*this, who, "bias_B", *bias_B, k_sddmmB, heads);
+        if (mA != 0 && mB != 0 && mA != mB)
+            throw hnh::Error(HNH_E_INVALID, who + ": bias_A is " + (mA > 1 ? "per head" : "shared") + ", bias_B " +
+                                                (mB > 1 ? "per head" : "shared"));
+    }
     const BlockOrigin atA(*this, k_sddmmA), atB(*this, k_sddmmB);
+    for (auto [g, b] : {std::make_pair(dbias_A, bias_A), std::make_pair(dbias_B, bias_B)})
+        if (g) {
+            g->resize(b->size());
+            g->setZero();
+        }
+    const BiasView bvA = bias_view(*this, bias_A, dbias_A, k_sddmmA, mA), bvB = bias_view(*this, bias_B, dbias_B, k_sddmmB, mB);
     // t[u, h] = <dZ_u,h, Z_u,h>: Z and dZ read as localArows * heads rows of d
     DenseMatrix t(localArows, heads);
     hnh::abi_check(hnh_batch_dot_f64(t.data(), dZ.data(), Z.data(), localArows * heads, (int)d, compute()), "batch_dot");
@@ -781,7 +876,14 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
                     [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
                         need_rows(rows_are_A, true, "sparseAttentionBackward");
                         CSRHandle *hd = blk.getActive();
-                        if (dropout == 0.0)
+                        if (with_bias)
+                            hnh::abi_check(hnh_sparse_attention_grad_q_bias_f64(
+                                               hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
+                                               R[0].ld, R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, Y[0].p, Y[0].ld, Y[1].p,
+                                               Y[1].ld, scale, R[4].p, R[4].ld, dropout, seed + (uint64_t)h, atA.u0(b), atA.v0(b),
+                                               bvA.at(h, b), bvA.grad_at(h, b), compute()),
+                                           "sparse_attention_grad_q_bias");
+                        else if (dropout == 0.0)
                             hnh::abi_check(hnh_sparse_attention_grad_q_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
                                                                            blk.num_coords, (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld,
                                                                            R[2].p, R[2].ld, R[3].p, R[3].ld, Y[0].p, Y[0].ld, Y[1].p,
@@ -801,7 +903,14 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
                     [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
                         need_rows(rows_are_A, false, "sparseAttentionBackward");
                         CSRHandle *hd = blk.getActive();
-                        if (dropout == 0.0)
+                        if (with_bias)
+                            hnh::abi_check(hnh_sparse_attention_grad_kv_bias_f64(
+                                               hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
+                                               R[0].ld, R[1].p, R[1].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p,
+                                               Y[3].ld, scale, R[2].p, R[2].ld, R[3].p, R[3].ld, dropout, seed + (uint64_t)h,
+                                               atB.u0(b), atB.v0(b), bvB.at(h, b), bvB.grad_at(h, b), compute()),
+                                           "sparse_attention_grad_kv_bias");
+                        else if (dropout == 0.0)
                             hnh::abi_check(hnh_sparse_attention_grad_kv_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows,
                                                                             blk.num_coords, (int)d, R[0].p, R[0].ld, R[1].p, R[1].ld,
                                                                             Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p,

@@ -403,6 +403,37 @@ int hnhd_alg_sparse_attention_backward_dropout(hnhd_alg_t *a, hnhd_dense_t *Q, h
         a->alg->sparseAttentionBackward(Q->m, K->m, V->m, Z->m, L->m, dZ->m, dQ->m, dK->m, dV->m, heads, scale, dropout, seed);
     });
 }
+int hnhd_alg_sparse_attention_bias(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                   hnhd_dense_t *L, int heads, double scale, double dropout, uint64_t seed,
+                                   const hnhd_vec_t *bias) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_bias: null argument");
+        if (!std::isfinite(scale)) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_bias: the scale must be finite");
+        a->alg->sparseAttention(Q->m, K->m, V->m, Z->m, L->m, heads, scale, dropout, seed, bias ? &bias->v : nullptr);
+    });
+}
+int hnhd_alg_sparse_attention_backward_bias(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                            hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ, hnhd_dense_t *dK,
+                                            hnhd_dense_t *dV, int heads, double scale, double dropout, uint64_t seed,
+                                            const hnhd_vec_t *bias_A, const hnhd_vec_t *bias_B, hnhd_vec_t *dbias_A,
+                                            hnhd_vec_t *dbias_B) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L || !dZ || !dQ || !dK || !dV)
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward_bias: null argument");
+        if (!std::isfinite(scale))
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward_bias: the scale must be finite");
+        a->alg->sparseAttentionBackward(Q->m, K->m, V->m, Z->m, L->m, dZ->m, dQ->m, dK->m, dV->m, heads, scale, dropout, seed,
+                                        bias_A ? &bias_A->v : nullptr, bias_B ? &bias_B->v : nullptr,
+                                        dbias_A ? &dbias_A->v : nullptr, dbias_B ? &dbias_B->v : nullptr);
+    });
+}
+int hnhd_alg_entry_coordinates(hnhd_alg_t *a, int mode, hnhd_vec_t *rows, hnhd_vec_t *cols) {
+    return guarded([&] {
+        if (!a || !rows || !cols) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_entry_coordinates: null argument");
+        if (rows == cols) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_entry_coordinates: rows and cols are one vector");
+        a->alg->entryCoordinates(value_order(mode), rows->v, cols->v);
+    });
+}
 
 int hnhd_timer_start(void) {
     return guarded([] {

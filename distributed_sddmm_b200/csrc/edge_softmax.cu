@@ -97,6 +97,10 @@ __global__ void keys_from_index_kernel(int32_t *__restrict__ keys, const int64_t
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) keys[i] = (int32_t)(idx[i] + offset);
 }
+__global__ void coords_from_index_kernel(double *__restrict__ out, const int64_t *__restrict__ idx, int64_t n, int64_t offset) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = (double)(idx[i] + offset);
+}
 
 // ---- forward ------------------------------------------------------------------------------------------------
 // one warp per piece: (max, sum of exp(x - max)) over x[perm[lo .. hi)].  A -inf entry (a masked edge) adds nothing:
@@ -235,6 +239,15 @@ int hnh_edge_keys_from_index(int32_t *keys, const int64_t *idx, int64_t n, int64
     int grid = 0;
     int rc = grid_for(keys_from_index_kernel, n, kBlock * 4, &grid, kCtasPerSm);
     return rc ? rc : launch(keys_from_index_kernel, grid, kBlock, (cudaStream_t)stream, "keys_from_index_kernel", keys, idx, n, offset);
+}
+
+int hnh_entry_coords_from_index_f64(double *out, const int64_t *idx, int64_t n, int64_t offset, void *stream) {
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_entry_coords_from_index_f64: negative size");
+    if (n == 0) return HNH_OK;
+    if (!out || !idx) return set_error(HNH_E_INVALID, "hnh_entry_coords_from_index_f64: null pointer");
+    int grid = 0;
+    int rc = grid_for(coords_from_index_kernel, n, kBlock * 4, &grid, kCtasPerSm);
+    return rc ? rc : launch(coords_from_index_kernel, grid, kBlock, (cudaStream_t)stream, "coords_from_index_kernel", out, idx, n, offset);
 }
 
 int64_t hnh_edge_softmax_piece_bound(int64_t n, int64_t num_rows) {

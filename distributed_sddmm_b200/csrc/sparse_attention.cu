@@ -24,6 +24,16 @@
 // that loads entry k's column index hashes it and sends the bit along with what it already broadcasts: the sign of
 // its weight (step) or its column index, complemented (gradients).  A dropped entry's V row (step), V row (grad_q)
 // or dZ row (grad_kv) is not loaded.  The instantiations with DROP = false are the kernels without dropout.
+//
+// Additive score bias (BIAS = true; the *_bias_f64 entry points): x_uv = sigma <Q_u, K_v> + b_i for the block's entry
+// i, and the gradient kernels add dx_i to db[i] when db is not null (dx_i is the bias gradient).  b = -inf masks an
+// entry: it adds nothing to (acc, m, s), alpha = 0 (so dx = 0) even where L = -inf, and its V or dZ row is not
+// loaded; a chunk whose entries are all masked leaves (acc, m, s) as they are, so a row masked throughout keeps s = 0
+// and finishes with Z = 0, L = -inf.  In the fast kernels the lane that loads entry k's column index loads b_k: the
+// step adds it to the lane's own score and sends a masked entry's weight with its sign bit set; the gradients
+// broadcast it with one shuffle, send a masked entry's column index complemented, and lane k keeps dx_k and adds it
+// to db[k] once per chunk.  The gradients compute x - L as (sigma <.,.> - L) + b, so a bias of zeros gives the bits
+// of the kernels without bias.  The instantiations with BIAS = false are the kernels without bias.
 #include <cmath>
 
 #include "mix64.cuh"
@@ -45,6 +55,13 @@ struct Dropout {
     uint32_t threshold;
 };
 
+// The bias of one call: entry i of the block reads b[i]; the gradient kernels add dx_i to db[i] unless db is null.
+// Passed after the Dropout, so the kernels without bias keep their parameter layout.
+struct Bias {
+    const double *b;
+    double *db;
+};
+
 __device__ __forceinline__ bool keep(const Dropout &dr, int64_t u, int64_t v) {
     return (uint32_t)(mix64(dr.key ^ ((uint64_t)u << 32 | (uint64_t)v)) >> 32) >= dr.threshold;
 }
@@ -57,12 +74,12 @@ __device__ __forceinline__ double group_max(double d, unsigned mask) {
 }
 
 // ---- fast row kernels ----------------------------------------------------------------------------------------
-template <int R, int G, int VW, int UN, bool DROP>
+template <int R, int G, int VW, int UN, bool DROP, bool BIAS>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                  const double *__restrict__ Q, int64_t ldq, const double *__restrict__ K, int64_t ldk,
                  const double *__restrict__ V, int64_t ldv, double scale, double *__restrict__ acc, int64_t ldacc,
-                 double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds, Dropout dr) {
+                 double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds, Dropout dr, Bias bs) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -84,7 +101,11 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
         for (int64_t j = s0; j < e; j += G) {
             const int cnt = (e - j < G) ? (int)(e - j) : G;
             int64_t mycol = 0;
-            if (gl < cnt) mycol = ld_stream_i64(col_idx + j + gl);
+            double mybias = 0.0;
+            if (gl < cnt) {
+                mycol = ld_stream_i64(col_idx + j + gl);
+                if constexpr (BIAS) mybias = ld_stream_f64(bs.b + j + gl);
+            }
             // sweep 1: the chunk's scores, entry k's on lane k
             double mine = -INFINITY;
             for (int k0 = 0; k0 < cnt; k0 += UN) {
@@ -112,12 +133,13 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                         for (int w = 0; w < VW; w++) d = fma(q[v][w], y[u][v][w], d);
                     d = group_allreduce<G>(d, gmask);
                     // padding slots past cnt (zero rows) must not enter the chunk's maximum
-                    if (gl == k0 + u && k0 + u < cnt) mine = scale * d;
+                    if (gl == k0 + u && k0 + u < cnt) mine = BIAS ? scale * d + mybias : scale * d;
                 }
             }
-            // one rescale to the chunk's maximum (exp(-inf) = 0 for a row's first chunk)
+            // one rescale to the chunk's maximum (exp(-inf) = 0 for a row's first chunk); a chunk whose entries are all
+            // masked, with no earlier entry, has mnew = -inf and leaves the state as it is
             const double mnew = fmax(mrow, group_max<G>(mine, gmask));
-            const double f = exp(mrow - mnew);
+            const double f = (BIAS && mnew == -INFINITY) ? 1.0 : exp(mrow - mnew);
 #pragma unroll
             for (int v = 0; v < NV; v++)
 #pragma unroll
@@ -128,6 +150,9 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
             // a dropped entry's weight travels with its sign bit set (-0.0 included): it counts in s, not in acc
             if constexpr (DROP)
                 if (!keep(dr, dr.u0 + row, dr.v0 + mycol)) pmine = -pmine;
+            // a masked entry's weight is -0.0: it counts in neither s nor acc
+            if constexpr (BIAS)
+                if (mine == -INFINITY) pmine = -0.0;
             // sweep 2: the V rows, weighted
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double y[UN][NV][VW];
@@ -138,7 +163,7 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                     const int src = k < G ? k : G - 1;
                     const int64_t c = __shfl_sync(gmask, mycol, src, G);
                     pv[u] = __shfl_sync(gmask, pmine, src, G);
-                    if (k < cnt && !(DROP && signbit(pv[u]))) {
+                    if (k < cnt && !((DROP || BIAS) && signbit(pv[u]))) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) ld_gather<VW>(y[u][v], V + c * ldv + (v * G + gl) * VW);
                     }
@@ -155,6 +180,14 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                                     for (int w = 0; w < VW; w++) a[v][w] = fma(pw, y[u][v][w], a[v][w]);
                             }
                             srow += fabs(pv[u]);
+                        } else if constexpr (BIAS) {
+                            if (!signbit(pv[u])) {
+#pragma unroll
+                                for (int v = 0; v < NV; v++)
+#pragma unroll
+                                    for (int w = 0; w < VW; w++) a[v][w] = fma(pv[u], y[u][v][w], a[v][w]);
+                            }
+                            srow += pv[u];
                         } else {
 #pragma unroll
                             for (int v = 0; v < NV; v++)
@@ -175,13 +208,13 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
     }
 }
 
-template <int R, int G, int VW, int UN, bool DROP>
+template <int R, int G, int VW, int UN, bool DROP, bool BIAS>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                    const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                    const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                    const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv, double scale,
-                   double *__restrict__ dQ, int64_t lddq, Dropout dr) {
+                   double *__restrict__ dQ, int64_t lddq, Dropout dr, Bias bs) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -204,17 +237,26 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
         for (int64_t j = s0; j < e; j += G) {
             const int cnt = (e - j < G) ? (int)(e - j) : G;
             int64_t mycol = 0;
-            if (gl < cnt) mycol = ld_stream_i64(col_idx + j + gl);
+            double mybias = 0.0, mydx = 0.0;
+            if (gl < cnt) {
+                mycol = ld_stream_i64(col_idx + j + gl);
+                if constexpr (BIAS) mybias = ld_stream_f64(bs.b + j + gl);
+            }
             // a dropped entry's column index travels complemented (negative)
             if constexpr (DROP)
                 if (!keep(dr, dr.u0 + row, dr.v0 + mycol)) mycol = ~mycol;
+            // and so does a masked one's: it needs no V row either
+            if constexpr (BIAS)
+                if (mybias == -INFINITY && mycol >= 0) mycol = ~mycol;
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double yk[UN][NV][VW], yv[UN][NV][VW];
+                double bu[UN];
 #pragma unroll
                 for (int u = 0; u < UN; u++) {
                     const int k = k0 + u;
                     int64_t c = __shfl_sync(gmask, mycol, k < G ? k : G - 1, G);
-                    const bool dropped = DROP && c < 0;
+                    if constexpr (BIAS) bu[u] = __shfl_sync(gmask, mybias, k < G ? k : G - 1, G);
+                    const bool dropped = (DROP || BIAS) && c < 0;
                     if (dropped) c = ~c;
                     if (k < cnt) {
 #pragma unroll
@@ -248,7 +290,14 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
                     d1 = group_allreduce<G>(d1, gmask);
                     d2 = group_allreduce<G>(d2, gmask);
                     if (k0 + u < cnt) {
-                        const double dx = exp(scale * d1 - Lr) * ((DROP ? dr.inv_keep * d2 : d2) - tr);
+                        double al;
+                        if constexpr (BIAS) {
+                            al = bu[u] == -INFINITY ? 0.0 : exp((scale * d1 - Lr) + bu[u]);
+                        } else {
+                            al = exp(scale * d1 - Lr);
+                        }
+                        const double dx = al * ((DROP ? dr.inv_keep * d2 : d2) - tr);
+                        if (BIAS && gl == k0 + u) mydx = dx;
 #pragma unroll
                         for (int v = 0; v < NV; v++)
 #pragma unroll
@@ -256,6 +305,8 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
                     }
                 }
             }
+            if constexpr (BIAS)
+                if (bs.db != nullptr && gl < cnt) bs.db[j + gl] += mydx;
         }
 #pragma unroll
         for (int v = 0; v < NV; v++) {
@@ -269,13 +320,13 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
     }
 }
 
-template <int R, int G, int VW, int UN, bool DROP>
+template <int R, int G, int VW, int UN, bool DROP, bool BIAS>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                     const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
                     const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                     const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt, double scale,
-                    double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv, Dropout dr) {
+                    double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv, Dropout dr, Bias bs) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -297,18 +348,22 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
         for (int64_t j = s0; j < e; j += G) {
             const int cnt = (e - j < G) ? (int)(e - j) : G;
             int64_t mycol = 0;
-            double myL = 0.0, myt = 0.0;
+            double myL = 0.0, myt = 0.0, mybias = 0.0, mydx = 0.0;
             if (gl < cnt) {
                 mycol = ld_stream_i64(col_idx + j + gl);
+                if constexpr (BIAS) mybias = ld_stream_f64(bs.b + j + gl);
                 myL = L[mycol * ldl];
                 myt = t[mycol * ldt];
             }
             // a dropped entry's column index travels complemented (negative); here u = u0 + col_idx, v = v0 + row
             if constexpr (DROP)
                 if (!keep(dr, dr.u0 + mycol, dr.v0 + row)) mycol = ~mycol;
+            // and so does a masked one's: it needs no dZ row either
+            if constexpr (BIAS)
+                if (mybias == -INFINITY && mycol >= 0) mycol = ~mycol;
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double yq[UN][NV][VW], yd[UN][NV][VW];
-                double Lu[UN], tu[UN];
+                double Lu[UN], tu[UN], bu[UN];
 #pragma unroll
                 for (int u = 0; u < UN; u++) {
                     const int k = k0 + u;
@@ -316,7 +371,8 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                     int64_t c = __shfl_sync(gmask, mycol, src, G);
                     Lu[u] = __shfl_sync(gmask, myL, src, G);
                     tu[u] = __shfl_sync(gmask, myt, src, G);
-                    const bool dropped = DROP && c < 0;
+                    if constexpr (BIAS) bu[u] = __shfl_sync(gmask, mybias, src, G);
+                    const bool dropped = (DROP || BIAS) && c < 0;
                     if (dropped) c = ~c;
                     if (k < cnt) {
 #pragma unroll
@@ -350,9 +406,15 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                     d1 = group_allreduce<G>(d1, gmask);
                     d2 = group_allreduce<G>(d2, gmask);
                     if (k0 + u < cnt) {
-                        const double al = exp(scale * d1 - Lu[u]);
+                        double al;
+                        if constexpr (BIAS) {
+                            al = bu[u] == -INFINITY ? 0.0 : exp((scale * d1 - Lu[u]) + bu[u]);
+                        } else {
+                            al = exp(scale * d1 - Lu[u]);
+                        }
                         const double dx = al * ((DROP ? dr.inv_keep * d2 : d2) - tu[u]);
                         const double aw = DROP ? al * dr.inv_keep : al;
+                        if (BIAS && gl == k0 + u) mydx = dx;
 #pragma unroll
                         for (int v = 0; v < NV; v++)
 #pragma unroll
@@ -363,6 +425,8 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                     }
                 }
             }
+            if constexpr (BIAS)
+                if (bs.db != nullptr && gl < cnt) bs.db[j + gl] += mydx;
         }
 #pragma unroll
         for (int v = 0; v < NV; v++) {
@@ -388,13 +452,13 @@ __device__ __forceinline__ double warp_dot(const double *x, const double *y, int
     return group_allreduce<32>(acc, 0xffffffffu);
 }
 
-template <bool DROP>
+template <bool DROP, bool BIAS>
 __global__ void __launch_bounds__(kBlock)
 attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                          const double *__restrict__ Q, int64_t ldq, const double *__restrict__ K, int64_t ldk,
                          const double *__restrict__ V, int64_t ldv, double scale, double *__restrict__ acc,
                          int64_t ldacc, double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds,
-                         Dropout dr) {
+                         Dropout dr, Bias bs) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -405,7 +469,13 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
         double *a = acc + row * ldacc;
         for (int64_t j = s0; j < e; j++) {
             const int64_t c = col_idx[j];
-            const double x = scale * warp_dot(Q + row * ldq, K + c * ldk, d, lane);
+            double x;
+            if constexpr (BIAS) {
+                if (bs.b[j] == -INFINITY) continue;  // masked: adds nothing
+                x = scale * warp_dot(Q + row * ldq, K + c * ldk, d, lane) + bs.b[j];
+            } else {
+                x = scale * warp_dot(Q + row * ldq, K + c * ldk, d, lane);
+            }
             const double mnew = fmax(mrow, x);
             const double f = exp(mrow - mnew), pj = exp(x - mnew);
             if (DROP && !keep(dr, dr.u0 + row, dr.v0 + c)) {
@@ -424,13 +494,13 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
     }
 }
 
-template <bool DROP>
+template <bool DROP, bool BIAS>
 __global__ void __launch_bounds__(kBlock)
 attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                            const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                            const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                            const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
-                           double scale, double *__restrict__ dQ, int64_t lddq, Dropout dr) {
+                           double scale, double *__restrict__ dQ, int64_t lddq, Dropout dr, Bias bs) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -439,42 +509,62 @@ attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *
         const double Lr = L[row * ldl], tr = t[row * ldt];
         for (int64_t j = s0; j < e; j++) {
             const int64_t c = col_idx[j];
+            double bj = 0.0;
+            if constexpr (BIAS) {
+                bj = bs.b[j];
+                if (bj == -INFINITY) continue;  // masked: alpha = 0, dx = 0 (db[j] += 0)
+            }
             const double d1 = warp_dot(Q + row * ldq, K + c * ldk, d, lane);
             double d2;  // D_uv w <dZ_u, V_v>
             if constexpr (DROP)
                 d2 = keep(dr, dr.u0 + row, dr.v0 + c) ? dr.inv_keep * warp_dot(dZ + row * lddz, V + c * ldv, d, lane) : 0.0;
             else
                 d2 = warp_dot(dZ + row * lddz, V + c * ldv, d, lane);
-            const double g = scale * (exp(scale * d1 - Lr) * (d2 - tr));
+            double g;
+            if constexpr (BIAS) {
+                // L and t read at their use: held across the row, they spill in this instantiation
+                const double dx = exp((scale * d1 - L[row * ldl]) + bj) * (d2 - t[row * ldt]);
+                if (bs.db != nullptr && lane == 0) bs.db[j] += dx;
+                g = scale * dx;
+            } else {
+                g = scale * (exp(scale * d1 - Lr) * (d2 - tr));
+            }
             for (int k = lane; k < d; k += 32) dQ[row * lddq + k] = fma(g, K[c * ldk + k], dQ[row * lddq + k]);
         }
     }
 }
 
-template <bool DROP>
+template <bool DROP, bool BIAS>
 __global__ void __launch_bounds__(kBlock)
 attn_grad_kv_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                             const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
                             const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                             const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                             double scale, double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv,
-                            Dropout dr) {
+                            Dropout dr, Bias bs) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
         const int64_t s0 = rowStart[row], e = rowStart[row + 1];
         for (int64_t j = s0; j < e; j++) {
             const int64_t u = col_idx[j];
+            if (BIAS && bs.b[j] == -INFINITY) continue;  // masked: alpha = 0, dx = 0 (db[j] += 0)
             const double d1 = warp_dot(K + row * ldk, Q + u * ldq, d, lane);
+            // x_uv - L_u
+            auto xl = [&] { return BIAS ? (scale * d1 - L[u * ldl]) + bs.b[j] : scale * d1 - L[u * ldl]; };
             if (DROP && !keep(dr, dr.u0 + u, dr.v0 + row)) {  // here the stored row is the key v
-                const double g = scale * (exp(scale * d1 - L[u * ldl]) * -t[u * ldt]);
+                const double dx = exp(xl()) * -t[u * ldt];
+                if (BIAS && bs.db != nullptr && lane == 0) bs.db[j] += dx;
+                const double g = scale * dx;
                 for (int k = lane; k < d; k += 32) dK[row * lddk + k] = fma(g, Q[u * ldq + k], dK[row * lddk + k]);
                 continue;
             }
             const double d2 = warp_dot(V + row * ldv, dZ + u * lddz, d, lane);
-            const double al = exp(scale * d1 - L[u * ldl]);
+            const double al = exp(xl());
             const double aw = DROP ? al * dr.inv_keep : al;
-            const double g = scale * (al * ((DROP ? dr.inv_keep * d2 : d2) - t[u * ldt]));
+            const double dx = al * ((DROP ? dr.inv_keep * d2 : d2) - t[u * ldt]);
+            if (BIAS && bs.db != nullptr && lane == 0) bs.db[j] += dx;
+            const double g = scale * dx;
             for (int k = lane; k < d; k += 32) {
                 dK[row * lddk + k] = fma(g, Q[u * ldq + k], dK[row * lddk + k]);
                 dV[row * lddv + k] = fma(aw, dZ[u * lddz + k], dV[row * lddv + k]);
@@ -541,10 +631,10 @@ int make_dropout(const char *who, double p, uint64_t seed, int64_t u0, int64_t v
     return HNH_OK;
 }
 
-template <bool DROP>
+template <bool DROP, bool BIAS>
 int step(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *Q,
          int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv, double scale, double *acc, int64_t ldacc,
-         double *m, int64_t ldm, double *s, int64_t lds, const Dropout &dr, void *stream) {
+         double *m, int64_t ldm, double *s, int64_t lds, const Dropout &dr, const Bias &bs, void *stream) {
     const std::initializer_list<Operand> ops = {{Q, ldq, true}, {K, ldk, true},   {V, ldv, true},
                                                 {acc, ldacc, true}, {m, ldm, false}, {s, lds, false}};
     int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
@@ -555,27 +645,27 @@ int step(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64
     if (fast_path(d, ops)) {
 #define STEP(RR, G, VW, UN)                                                                                                \
     {                                                                                                                      \
-        auto k = attn_step_kernel<RR, G, VW, UN, DROP>;                                                                    \
+        auto k = attn_step_kernel<RR, G, VW, UN, DROP, BIAS>;                                                              \
         rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
         if (!rc)                                                                                                           \
             rc = launch(k, grid, kBlock, st, "attn_step_kernel", rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, \
-                        ldm, s, lds, dr);                                                                                  \
+                        ldm, s, lds, dr, bs);                                                                              \
     }
         HNH_DISPATCH_R(d, STEP, )
 #undef STEP
         return rc;
     }
-    auto k = attn_step_generic_kernel<DROP>;
+    auto k = attn_step_generic_kernel<DROP, BIAS>;
     rc = grid_for(k, rows, kBlock / 32, &grid);
     return rc ? rc : launch(k, grid, kBlock, st, "attn_step_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, K, ldk, V, ldv,
-                            scale, acc, ldacc, m, ldm, s, lds, dr);
+                            scale, acc, ldacc, m, ldm, s, lds, dr, bs);
 }
 
-template <bool DROP>
+template <bool DROP, bool BIAS>
 int grad_q(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *Q,
            int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
            const double *K, int64_t ldk, const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq,
-           const Dropout &dr, void *stream) {
+           const Dropout &dr, const Bias &bs, void *stream) {
     const std::initializer_list<Operand> ops = {{Q, ldq, true}, {dZ, lddz, true}, {L, ldl, false}, {t, ldt, false},
                                                 {K, ldk, true}, {V, ldv, true},   {dQ, lddq, true}};
     int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
@@ -586,27 +676,27 @@ int grad_q(const char *who, const int64_t *rowStart, const int64_t *col_idx, int
     if (fast_path(d, ops)) {
 #define GQ(RR, G, VW, UN)                                                                                                  \
     {                                                                                                                      \
-        auto k = attn_grad_q_kernel<RR, G, VW, UN, DROP>;                                                                  \
+        auto k = attn_grad_q_kernel<RR, G, VW, UN, DROP, BIAS>;                                                            \
         rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
         if (!rc)                                                                                                           \
             rc = launch(k, grid, kBlock, st, "attn_grad_q_kernel", rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, \
-                        V, ldv, scale, dQ, lddq, dr);                                                                      \
+                        V, ldv, scale, dQ, lddq, dr, bs);                                                                  \
     }
         HNH_DISPATCH_R(d, GQ, )
 #undef GQ
         return rc;
     }
-    auto k = attn_grad_q_generic_kernel<DROP>;
+    auto k = attn_grad_q_generic_kernel<DROP, BIAS>;
     rc = grid_for(k, rows, kBlock / 32, &grid);
     return rc ? rc : launch(k, grid, kBlock, st, "attn_grad_q_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, dZ, lddz, L,
-                            ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq, dr);
+                            ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq, dr, bs);
 }
 
-template <bool DROP>
+template <bool DROP, bool BIAS>
 int grad_kv(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *K,
             int64_t ldk, const double *V, int64_t ldv, const double *Q, int64_t ldq, const double *dZ, int64_t lddz,
             const double *L, int64_t ldl, const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
-            int64_t lddv, const Dropout &dr, void *stream) {
+            int64_t lddv, const Dropout &dr, const Bias &bs, void *stream) {
     const std::initializer_list<Operand> ops = {{K, ldk, true},   {V, ldv, true},   {Q, ldq, true},   {dZ, lddz, true},
                                                 {L, ldl, false},  {t, ldt, false},  {dK, lddk, true}, {dV, lddv, true}};
     int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
@@ -617,20 +707,28 @@ int grad_kv(const char *who, const int64_t *rowStart, const int64_t *col_idx, in
     if (fast_path(d, ops)) {
 #define GKV(RR, G, VW, UN)                                                                                                 \
     {                                                                                                                      \
-        auto k = attn_grad_kv_kernel<RR, G, VW, UN, DROP>;                                                                 \
+        auto k = attn_grad_kv_kernel<RR, G, VW, UN, DROP, BIAS>;                                                           \
         rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
         if (!rc)                                                                                                           \
             rc = launch(k, grid, kBlock, st, "attn_grad_kv_kernel", rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, \
-                        ldl, t, ldt, scale, dK, lddk, dV, lddv, dr);                                                       \
+                        ldl, t, ldt, scale, dK, lddk, dV, lddv, dr, bs);                                                   \
     }
         HNH_DISPATCH_R(d, GKV, )
 #undef GKV
         return rc;
     }
-    auto k = attn_grad_kv_generic_kernel<DROP>;
+    auto k = attn_grad_kv_generic_kernel<DROP, BIAS>;
     rc = grid_for(k, rows, kBlock / 32, &grid);
     return rc ? rc : launch(k, grid, kBlock, st, "attn_grad_kv_generic_kernel", rowStart, col_idx, rows, d, K, ldk, V, ldv, Q,
-                            ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, dr);
+                            ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, dr, bs);
+}
+
+// The Dropout of a bias call (p = 0: the kernels without dropout) with its bias checked: HNH_OK or HNH_E_INVALID
+int make_bias_call(const char *who, double p, uint64_t seed, int64_t u0, int64_t v0, const double *bias, Dropout *dr) {
+    const int rc = make_dropout(who, p, seed, u0, v0, dr);
+    if (rc) return rc;
+    if (!bias) return set_error(HNH_E_INVALID, "%s: null bias", who);
+    return HNH_OK;
 }
 
 }  // namespace
@@ -641,8 +739,8 @@ int hnh_sparse_attention_step_f64(const int64_t *rowStart, const int64_t *col_id
                                   const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv,
                                   double scale, double *acc, int64_t ldacc, double *m, int64_t ldm, double *s, int64_t lds,
                                   void *stream) {
-    return step<false>("hnh_sparse_attention_step_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc,
-                       ldacc, m, ldm, s, lds, Dropout{}, stream);
+    return step<false, false>("hnh_sparse_attention_step_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale,
+                              acc, ldacc, m, ldm, s, lds, Dropout{}, Bias{}, stream);
 }
 
 int hnh_sparse_attention_step_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -653,8 +751,23 @@ int hnh_sparse_attention_step_dropout_f64(const int64_t *rowStart, const int64_t
     const char *who = "hnh_sparse_attention_step_dropout_f64";
     Dropout dr;
     const int rc = make_dropout(who, p, seed, u0, v0, &dr);
-    return rc ? rc : step<true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds,
-                                dr, stream);
+    return rc ? rc : step<true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
+                                       lds, dr, Bias{}, stream);
+}
+
+int hnh_sparse_attention_step_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                       const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv,
+                                       double scale, double *acc, int64_t ldacc, double *m, int64_t ldm, double *s, int64_t lds,
+                                       double p, uint64_t seed, int64_t u0, int64_t v0, const double *bias, void *stream) {
+    const char *who = "hnh_sparse_attention_step_bias_f64";
+    Dropout dr;
+    const int rc = make_bias_call(who, p, seed, u0, v0, bias, &dr);
+    if (rc) return rc;
+    const Bias bs{bias, nullptr};
+    return p == 0.0 ? step<false, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
+                                        lds, dr, bs, stream)
+                    : step<true, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
+                                       lds, dr, bs, stream);
 }
 
 int hnh_sparse_attention_finish_f64(int64_t rows, int d, const double *acc, int64_t ldacc, const double *m, int64_t ldm,
@@ -677,8 +790,8 @@ int hnh_sparse_attention_grad_q_f64(const int64_t *rowStart, const int64_t *col_
                                     const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
                                     const double *t, int64_t ldt, const double *K, int64_t ldk, const double *V, int64_t ldv,
                                     double scale, double *dQ, int64_t lddq, void *stream) {
-    return grad_q<false>("hnh_sparse_attention_grad_q_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K,
-                         ldk, V, ldv, scale, dQ, lddq, Dropout{}, stream);
+    return grad_q<false, false>("hnh_sparse_attention_grad_q_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t,
+                                ldt, K, ldk, V, ldv, scale, dQ, lddq, Dropout{}, Bias{}, stream);
 }
 
 int hnh_sparse_attention_grad_q_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -689,16 +802,33 @@ int hnh_sparse_attention_grad_q_dropout_f64(const int64_t *rowStart, const int64
     const char *who = "hnh_sparse_attention_grad_q_dropout_f64";
     Dropout dr;
     const int rc = make_dropout(who, p, seed, u0, v0, &dr);
-    return rc ? rc : grad_q<true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale,
-                                  dQ, lddq, dr, stream);
+    return rc ? rc : grad_q<true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
+                                         scale, dQ, lddq, dr, Bias{}, stream);
+}
+
+int hnh_sparse_attention_grad_q_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                         const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
+                                         int64_t ldl, const double *t, int64_t ldt, const double *K, int64_t ldk,
+                                         const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq, double p,
+                                         uint64_t seed, int64_t u0, int64_t v0, const double *bias, double *dbias,
+                                         void *stream) {
+    const char *who = "hnh_sparse_attention_grad_q_bias_f64";
+    Dropout dr;
+    const int rc = make_bias_call(who, p, seed, u0, v0, bias, &dr);
+    if (rc) return rc;
+    const Bias bs{bias, dbias};
+    return p == 0.0 ? grad_q<false, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
+                                          scale, dQ, lddq, dr, bs, stream)
+                    : grad_q<true, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
+                                         scale, dQ, lddq, dr, bs, stream);
 }
 
 int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
                                      const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q, int64_t ldq,
                                      const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
                                      double scale, double *dK, int64_t lddk, double *dV, int64_t lddv, void *stream) {
-    return grad_kv<false>("hnh_sparse_attention_grad_kv_f64", rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz,
-                          L, ldl, t, ldt, scale, dK, lddk, dV, lddv, Dropout{}, stream);
+    return grad_kv<false, false>("hnh_sparse_attention_grad_kv_f64", rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ,
+                                 lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, Dropout{}, Bias{}, stream);
 }
 
 int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -709,8 +839,25 @@ int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int6
     const char *who = "hnh_sparse_attention_grad_kv_dropout_f64";
     Dropout dr;
     const int rc = make_dropout(who, p, seed, u0, v0, &dr);
-    return rc ? rc : grad_kv<true>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale,
-                                   dK, lddk, dV, lddv, dr, stream);
+    return rc ? rc : grad_kv<true, false>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
+                                          scale, dK, lddk, dV, lddv, dr, Bias{}, stream);
+}
+
+int hnh_sparse_attention_grad_kv_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                          const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q,
+                                          int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
+                                          const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
+                                          int64_t lddv, double p, uint64_t seed, int64_t u0, int64_t v0, const double *bias,
+                                          double *dbias, void *stream) {
+    const char *who = "hnh_sparse_attention_grad_kv_bias_f64";
+    Dropout dr;
+    const int rc = make_bias_call(who, p, seed, u0, v0, bias, &dr);
+    if (rc) return rc;
+    const Bias bs{bias, dbias};
+    return p == 0.0 ? grad_kv<false, true>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
+                                           scale, dK, lddk, dV, lddv, dr, bs, stream)
+                    : grad_kv<true, true>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
+                                          scale, dK, lddk, dV, lddv, dr, bs, stream);
 }
 
 }  // extern "C"

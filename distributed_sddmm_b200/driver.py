@@ -167,6 +167,13 @@ class Vec:
     def __init__(self, handle):
         self.h = handle
 
+    @classmethod
+    def create(cls, n: int, value: float = 0.0):
+        """A device vector of n doubles filled with `value` (e.g. a per-head bias of heads * len(like_S_values()))."""
+        h = C.c_void_p()
+        check(lib().hnhd_vec_create(int(n), float(value), C.byref(h)), "hnhd_vec_create")
+        return cls(h)
+
     def __len__(self):
         return int(lib().hnhd_vec_size(self.h))
 
@@ -317,7 +324,7 @@ class Algorithm:
         return p, int(seed)
 
     def sparse_attention(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, heads: int = 1, scale=None,
-                         dropout: float = 0.0, seed: int = 0):
+                         dropout: float = 0.0, seed: int = 0, bias: Vec = None):
         """Collective: fused attention over the pattern of S (its values are not read).  Q and Z are A-shaped, K and V
         B-shaped, all r wide; per head h of width d = r / heads, Z_u,h = sum over the stored (u, v) of
         softmax_v(scale <Q_u,h, K_v,h>) V_v,h, and L (Dense.create(localArows, heads)) = the rows' log-sum-exp (-inf,
@@ -327,22 +334,70 @@ class Algorithm:
         1 / (1 - dropout), as torch.nn.functional.dropout(softmax(x)) @ V does; L is still the log-sum-exp of all
         scores.  The mask is a hash of (seed, head, global S-row, global S-column), so it does not depend on the
         algorithm or the number of ranks, and duplicate stored (u, v) share one keep bit.  Every rank must pass the
-        same dropout and seed, and sparse_attention_backward must get the ones its forward got."""
+        same dropout and seed, and sparse_attention_backward must get the ones its forward got.
+
+        bias (a Vec, or None) adds b_uv,h to the score of the stored (u, v) in head h, after the scale:
+        x_uv,h = scale <Q_u,h, K_v,h> + b_uv,h.  It is an A-order value vector (like_S_values' order) of length n
+        (every head reads it) or heads * n (head h reads [h n, (h + 1) n)), n = len(like_S_values()).  b = -inf
+        masks an entry (the attn_mask of torch's scaled_dot_product_attention); a row masked throughout gets Z = 0
+        and L = -inf, as a row without entries (edge_softmax gives NaN there).  +inf or NaN are not checked and make
+        the row NaN.  Contract, not checked: b is a function of the global S-row and S-column (entry_coordinates
+        gives them), so stored duplicates of (u, v) share one bias, and every rank passes its part of the same
+        bias.  A bias of zeros gives the bits of the call without bias."""
         s = self._attention_scale(Q, heads, scale)
         p, sd = self._dropout_args(dropout, seed)
-        check(lib().hnhd_alg_sparse_attention_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s, p, sd),
-              "sparse_attention")
+        if bias is None:
+            check(lib().hnhd_alg_sparse_attention_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s, p, sd),
+                  "sparse_attention")
+        else:
+            check(lib().hnhd_alg_sparse_attention_bias(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s, p, sd,
+                                                       self._vec_arg(bias, "bias")),
+                  "sparse_attention")
 
     def sparse_attention_backward(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, dZ: Dense, dQ: Dense, dK: Dense,
-                                  dV: Dense, heads: int = 1, scale=None, dropout: float = 0.0, seed: int = 0):
+                                  dV: Dense, heads: int = 1, scale=None, dropout: float = 0.0, seed: int = 0,
+                                  bias: Vec = None, bias_B: Vec = None, dbias: Vec = None, dbias_B: Vec = None):
         """Collective: given dZ = dLoss/dZ and the forward's Z and L, overwrites dQ, dK and dV with the gradients of
         sparse_attention (Distributed_Sparse::sparseAttentionBackward).  dropout and seed must be the ones the forward
-        got, and the same on every rank: the backward regenerates the forward's mask from them."""
+        got, and the same on every rank: the backward regenerates the forward's mask from them.
+
+        With a bias, the backward needs it in both value orders: `bias` (the forward's, A order) for the dQ pass and
+        `bias_B` (B order, like_ST_values' order, of the same head multiplicity) for the dK, dV pass.  Both must
+        hold the same b(u, v) for every stored (u, v); build bias_B from entry_coordinates("B").  dbias / dbias_B
+        (optional Vecs, resized to their bias's length) receive dLoss/dbias in each order:
+        dx_uv,h = alpha_uv (D w <dZ_u,h, V_v,h> - t_u,h), summed over the heads for a shared bias, in a fixed order
+        (repeats are bit-identical); 0 at a masked entry."""
         s = self._attention_scale(Q, heads, scale)
         p, sd = self._dropout_args(dropout, seed)
-        check(lib().hnhd_alg_sparse_attention_backward_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h,
-                                                               int(heads), s, p, sd),
-              "sparse_attention_backward")
+        if bias is None and bias_B is None:
+            if dbias is not None or dbias_B is not None:
+                raise ValueError("dbias / dbias_B need their bias")
+            check(lib().hnhd_alg_sparse_attention_backward_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h,
+                                                                   int(heads), s, p, sd),
+                  "sparse_attention_backward")
+            return
+        if bias is None or bias_B is None:
+            raise ValueError("a bias needs both value orders: bias (A order) and bias_B (B order)")
+        check(lib().hnhd_alg_sparse_attention_backward_bias(
+            self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h, int(heads), s, p, sd, self._vec_arg(bias, "bias"),
+            self._vec_arg(bias_B, "bias_B"), self._vec_arg(dbias, "dbias"), self._vec_arg(dbias_B, "dbias_B")),
+            "sparse_attention_backward")
+
+    @staticmethod
+    def _vec_arg(v, name):
+        if v is None:
+            return None
+        if not isinstance(v, Vec):
+            raise TypeError(f"{name} must be a Vec, not {type(v).__name__}")
+        return v.h
+
+    def entry_coordinates(self, mode: str = "A"):
+        """(rows, cols): int64 numpy arrays with the global S-row and S-column of every entry of this rank's value
+        vector of `mode` ("A": like_S_values, "B": like_ST_values), in that vector's order -- what a bias of that
+        order is built from (Distributed_Sparse::entryCoordinates)."""
+        rows, cols = Vec.create(0), Vec.create(0)
+        check(lib().hnhd_alg_entry_coordinates(self.h, _value_order(mode), rows.h, cols.h), "entry_coordinates")
+        return rows.to_host().astype(np.int64), cols.to_host().astype(np.int64)
 
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])

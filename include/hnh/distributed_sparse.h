@@ -231,6 +231,33 @@ public:
     void sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
                                  DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
                                  double scale, double dropout, uint64_t seed);
+    // The same with an additive score bias: x_uv,h = scale <Q_u,h, K_v,h> + b_uv,h (added after the scale, not
+    // scaled); L, Z, t and the dropout mask are the above on these scores, and dQ, dK, dV keep their formulas with
+    // alpha from the biased x.  The backward also writes dbias_uv,h = dx_uv,h = alpha_uv (D w <dZ_u, V_v> - t_u).
+    // A bias is a value vector of the order it is used in (like_S_values for the A order, like_ST_values for the
+    // B order) of length n (every head reads it; its gradient is sum_h dx_h) or heads * n (head h reads
+    // [h n, (h + 1) n)), n that order's local entry count.  The forward and the backward's dQ pass read `bias` /
+    // `bias_A` (A order), the backward's dK, dV pass `bias_B` (B order).  Contract, not checked: bias_A and bias_B
+    // hold the same b(u, v), a function of the global S-row and S-column (entryCoordinates gives them), so stored
+    // duplicates of (u, v) share one bias; the backward gets the forward's bias; every rank passes matching vectors.
+    // b = -inf masks an entry: alpha = 0, nothing added to Z, dbias = 0.  A row masked throughout gets Z = 0,
+    // L = -inf and zero gradients, as a row without entries (edgeSoftmax gives NaN there).  +inf or NaN: not
+    // checked, the row's results are NaN.  dbias_A / dbias_B (nullable) are resized to their bias's length and
+    // overwritten; the heads accumulate into a shared bias's gradient in a fixed order (bit-identical repeats).
+    // A null bias (both null in the backward) runs the kernels without bias: the overloads above forward here with
+    // null pointers.  HNH_E_INVALID on every rank before any launch for a bias length other than n or heads * n,
+    // bias_A and bias_B of different head multiplicity, only one of them, a dbias without its bias, or a dbias that
+    // is a bias.
+    void sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                         double scale, double dropout, uint64_t seed, const VectorXd *bias);
+    void sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                 double scale, double dropout, uint64_t seed, const VectorXd *bias_A,
+                                 const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B);
+    // rows / cols (resized to the order's local entry count) become the global S-row and S-column of every entry
+    // of this rank's value vector of `order` (k_sddmmA: like_S_values, k_sddmmB: like_ST_values), as exact
+    // doubles.  No communication.  Defined where check_full_rows passes; HNH_E_INVALID on every rank elsewhere.
+    void entryCoordinates(KernelMode order, VectorXd &rows, VectorXd &cols);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

@@ -188,6 +188,8 @@ int hnh_dgemm_nt_f64(double *C, const double *A, const double *B, int64_t m, int
  * keys[i] = (int32) (idx[i] + offset): the global row of the entries of one CSR block from its stored row or
  * column index */
 int hnh_edge_keys_from_index(int32_t *keys, const int64_t *idx, int64_t n, int64_t offset, void *stream);
+/* out[i] = (double) (idx[i] + offset): the same as doubles, exact below 2^53 (Distributed_Sparse::entryCoordinates) */
+int hnh_entry_coords_from_index_f64(double *out, const int64_t *idx, int64_t n, int64_t offset, void *stream);
 /* room for piece_row that any plan of n entries over num_rows rows fits in (negative: bad size) */
 int64_t hnh_edge_softmax_piece_bound(int64_t n, int64_t num_rows);
 /* Builds the plan of `keys` (synchronises): perm (n), row_start and piece_first (num_rows + 1 each),
@@ -328,6 +330,36 @@ int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int6
                                              const double *L, int64_t ldl, const double *t, int64_t ldt, double scale,
                                              double *dK, int64_t lddk, double *dV, int64_t lddv, double p,
                                              uint64_t seed, int64_t u0, int64_t v0, void *stream);
+/* Additive score bias: the dropout calls with `bias` (and, for the gradients, `dbias`) before the stream; p = 0
+ * means no dropout.  bias is block-local: entry i (the i-th stored entry, in col_idx order) reads bias[i], and
+ *     x_i = scale <Q_u, K_v> + bias[i]      (the bias is added after the scale and is not scaled).
+ * The step, finish, L, t and the dropout mask are those above on these scores; the gradients keep their formulas
+ * with alpha computed from the biased x, and grad_q / grad_kv add dx_i = alpha_i (D_i w <dZ_u, V_v> - t_u) (the
+ * bias gradient; D w = 1 without dropout) to dbias[i] when dbias is not null.  The caller zeroes dbias.
+ * Masking: bias[i] = -inf masks entry i: alpha_i = 0, it adds nothing to acc or s, and dx_i = 0.  A row whose
+ * entries are all masked keeps s = 0, so finish gives it Z = 0, L = -inf, and its gradients are 0 (as for a row
+ * without entries; the edge softmax gives NaN there instead).  bias = +inf or NaN is not checked: the row's results
+ * are then NaN.  A bias of zeros gives results bit-identical to the calls without bias.
+ * The backward's grad_q reads the bias of its (A-order) block and grad_kv that of its transpose (B-order): both
+ * must hold the same b(u, v) for every stored (u, v), as the step did.
+ * bias null, p < 0, p >= 1, NaN, u0 < 0 or v0 < 0: HNH_E_INVALID before any launch. */
+int hnh_sparse_attention_step_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                       const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V,
+                                       int64_t ldv, double scale, double *acc, int64_t ldacc, double *m, int64_t ldm,
+                                       double *s, int64_t lds, double p, uint64_t seed, int64_t u0, int64_t v0,
+                                       const double *bias, void *stream);
+int hnh_sparse_attention_grad_q_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                                         int d, const double *Q, int64_t ldq, const double *dZ, int64_t lddz,
+                                         const double *L, int64_t ldl, const double *t, int64_t ldt, const double *K,
+                                         int64_t ldk, const double *V, int64_t ldv, double scale, double *dQ,
+                                         int64_t lddq, double p, uint64_t seed, int64_t u0, int64_t v0,
+                                         const double *bias, double *dbias, void *stream);
+int hnh_sparse_attention_grad_kv_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                                          int d, const double *K, int64_t ldk, const double *V, int64_t ldv,
+                                          const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
+                                          int64_t ldl, const double *t, int64_t ldt, double scale, double *dK,
+                                          int64_t lddk, double *dV, int64_t lddv, double p, uint64_t seed, int64_t u0,
+                                          int64_t v0, const double *bias, double *dbias, void *stream);
 
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of

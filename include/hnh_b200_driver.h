@@ -203,6 +203,20 @@ int hnhd_alg_sparse_attention_backward_dropout(hnhd_alg_t *alg, hnhd_dense_t *Q,
                                                hnhd_dense_t *Z, hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ,
                                                hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale,
                                                double dropout, uint64_t seed);
+/* With an additive score bias (Distributed_Sparse::sparseAttention / sparseAttentionBackward with bias pointers):
+ * bias / bias_A an A-order vector, bias_B a B-order one, of length n or heads * n; dbias_A / dbias_B nullable.
+ * A null bias (both null in the backward) is the call without bias. */
+int hnhd_alg_sparse_attention_bias(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                   hnhd_dense_t *L, int heads, double scale, double dropout, uint64_t seed,
+                                   const hnhd_vec_t *bias);
+int hnhd_alg_sparse_attention_backward_bias(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V,
+                                            hnhd_dense_t *Z, hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ,
+                                            hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale, double dropout,
+                                            uint64_t seed, const hnhd_vec_t *bias_A, const hnhd_vec_t *bias_B,
+                                            hnhd_vec_t *dbias_A, hnhd_vec_t *dbias_B);
+/* rows / cols (resized) become the global S-row and S-column of every entry of this rank's value vector of `mode`
+ * (0 = A order, 1 = B order) (Distributed_Sparse::entryCoordinates). */
+int hnhd_alg_entry_coordinates(hnhd_alg_t *alg, int mode, hnhd_vec_t *rows, hnhd_vec_t *cols);
 
 /* CUDA-event timing on the library's compute stream: start, ..., stop -> milliseconds. */
 int hnhd_timer_start(void);

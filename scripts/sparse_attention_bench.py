@@ -22,7 +22,13 @@ JSON line per measurement.
 Attention dropout at DROPOUT (0.1): each of the three dropout kernels (hnh_sparse_attention_*_dropout_f64) beside its
 kernel without dropout on the same block and operands, the two timed in alternation ROUNDS (5) times, REPS launches
 each, with the median of each and their ratio; then Algorithm.sparse_attention and sparse_attention_backward with and
-without dropout, alternated the same way.  PARTS (kernels,ops,dropout) picks the sections.
+without dropout, alternated the same way.
+
+Additive score bias (PARTS=bias): each of the three bias kernels (hnh_sparse_attention_*_bias_f64, p = 0, a bias
+uniform in [-1, 1), the gradients writing dbias) beside its kernel without bias, alternated the same way; the two
+gradient kernels with and without the dbias write; then Algorithm.sparse_attention and sparse_attention_backward
+(writing both dbias vectors) with and without a bias.  The bias adds 8 bytes read per entry, and dbias 16 more (read
+and write), to the byte counts above.  PARTS (kernels,ops,dropout; also bias) picks the sections.
 Environment: LOGM (20), NPR (32), WIDTHS (128,256), ALG (15d_fusion1), REPS (20), DROPOUT (0.1), ROUNDS (5), PARTS."""
 import json
 import math
@@ -270,16 +276,114 @@ def dropout_ops(d):
     del alg
 
 
+def alternate_pair(names, d, calls, timer=timed, nbytes=(None, None)):
+    """calls[0] and calls[1] timed in turn `rounds` times, reported under names[0] and names[1]; the ratio of their
+    medians (second over first)."""
+    t = ([], [])
+    for _ in range(rounds):
+        for i in (0, 1):
+            t[i].append(timer(calls[i]))
+    med = [float(np.median(x)) for x in t]
+    for i in (0, 1):
+        report(names[i], d, med[i], nbytes[i], spread=[round(min(t[i]), 4), round(max(t[i]), 4)])
+    return med[1] / med[0]
+
+
+def bias_kernels(alg, d):
+    a_blk, b_blk = ("ST", "S") if alg_name == "15d_fusion1" else ("S", "ST")
+    rows, nnz, rs, ci = block(alg, a_blk)
+    rowsT, nnzT, rsT, ciT = block(alg, b_blk)
+    g = torch.Generator(device=dev).manual_seed(1)
+    n = max(rows, rowsT)
+    Q, K, V, dZ = (torch.rand((n, d), generator=g, **f64) * 2 - 1 for _ in range(4))
+    acc, dQ, dK, dV = (torch.zeros((n, d), **f64) for _ in range(4))
+    ms_ = torch.zeros((rows, 2), **f64)
+    Lt = torch.rand((n, 2), generator=g, **f64) + 4  # L, t: a plausible log-sum-exp of 32 entries, and <dZ, Z>
+    bA, bB = torch.rand(nnz, generator=g, **f64) * 2 - 1, torch.rand(nnzT, generator=g, **f64) * 2 - 1
+    dbA, dbB = torch.zeros(nnz, **f64), torch.zeros(nnzT, **f64)
+    scale = 1 / math.sqrt(d)
+    p = lambda t: t.data_ptr()  # noqa: E731
+    nob = (0.0, SEED, 0, 0)
+
+    def step(b=False):
+        if b:
+            D.check(L.hnh_sparse_attention_step_bias_f64(p(rs), p(ci), rows, nnz, d, p(Q), d, p(K), d, p(V), d, scale, p(acc), d,
+                                                         p(ms_), 2, p(ms_) + 8, 2, *nob, p(bA), st))
+        else:
+            D.check(L.hnh_sparse_attention_step_f64(p(rs), p(ci), rows, nnz, d, p(Q), d, p(K), d, p(V), d, scale, p(acc), d,
+                                                    p(ms_), 2, p(ms_) + 8, 2, st))
+
+    def grad_q(b=False, db=True):
+        args = (p(rs), p(ci), rows, nnz, d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, p(K), d, p(V), d, scale, p(dQ), d)
+        if b:
+            D.check(L.hnh_sparse_attention_grad_q_bias_f64(*args, *nob, p(bA), p(dbA) if db else None, st))
+        else:
+            D.check(L.hnh_sparse_attention_grad_q_f64(*args, st))
+
+    def grad_kv(b=False, db=True):
+        args = (p(rsT), p(ciT), rowsT, nnzT, d, p(K), d, p(V), d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, scale, p(dK), d,
+                p(dV), d)
+        if b:
+            D.check(L.hnh_sparse_attention_grad_kv_bias_f64(*args, *nob, p(bB), p(dbB) if db else None, st))
+        else:
+            D.check(L.hnh_sparse_attention_grad_kv_f64(*args, st))
+
+    ratios = {}
+    for name, fn, nbytes, nb, with_db in (
+            ("step", step, nnz * (8 + 16 * d) + rows * (8 + 24 * d + 32), nnz * 8, False),
+            ("grad_q", grad_q, nnz * (8 + 16 * d) + rows * (8 + 32 * d + 16), nnz * 24, True),
+            ("grad_kv", grad_kv, nnzT * (24 + 16 * d) + rowsT * (8 + 48 * d), nnzT * 24, True)):
+        ratios[name] = round(alternate_pair((name, name + "_bias"), d, (fn, lambda fn=fn: fn(True)),
+                                            nbytes=(nbytes, nbytes + nb)), 3)
+        if with_db:
+            ratios[name + "_dbias_write"] = round(alternate_pair((name + "_bias_no_dbias", name + "_bias"), d,
+                                                                 (lambda fn=fn: fn(True, False), lambda fn=fn: fn(True))), 3)
+    print(json.dumps(dict(d=d, bias_kernel_over_kernel=ratios)), flush=True)
+
+
+def bias_ops(d):
+    alg = D.Algorithm(alg_name, S, d, 1)
+    dims = alg.dims
+    rng = np.random.default_rng(SEED)
+    Q, dZ = (alg.like_A_matrix() for _ in range(2))
+    K, V = (alg.like_B_matrix() for _ in range(2))
+    for m in (Q, dZ, K, V):
+        m.from_host(rng.uniform(-1, 1, m.shape))
+    Z, dQ, dK, dV = alg.like_A_matrix(), alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix()
+    Lm = D.Dense.create(dims.localArows, 1)
+    bA, bB = alg.like_S_values(), alg.like_ST_values()
+    rA, cA = alg.entry_coordinates("A")
+    rB, cB = alg.entry_coordinates("B")
+    bA.from_host(np.sin(0.37 * rA + 1.3 * cA))
+    bB.from_host(np.sin(0.37 * rB + 1.3 * cB))
+    dbA, dbB = D.Vec.create(0), D.Vec.create(0)
+    fwd = alternate_pair(("op_fused_forward", "op_fused_forward_bias"), d,
+                         (lambda: alg.sparse_attention(Q, K, V, Z, Lm), lambda: alg.sparse_attention(Q, K, V, Z, Lm, bias=bA)),
+                         timer=timed_op)
+    alg.sparse_attention(Q, K, V, Z, Lm, bias=bA)
+    bwd = alternate_pair(("op_fused_backward", "op_fused_backward_bias"), d,
+                         (lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV),
+                          lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV, bias=bA, bias_B=bB, dbias=dbA,
+                                                                dbias_B=dbB)), timer=timed_op)
+    print(json.dumps(dict(d=d, forward_bias_over_forward=round(fwd, 3), backward_bias_over_backward=round(bwd, 3))),
+          flush=True)
+    del alg
+
+
 for d in widths:
     alg = D.Algorithm(alg_name, S, d, 1)
     if "kernels" in parts:
         kernels(alg, d)
     if "dropout" in parts:
         dropout_kernels(alg, d)
+    if "bias" in parts:
+        bias_kernels(alg, d)
     del alg
     torch.cuda.empty_cache()
     if "ops" in parts:
         ops(d)
     if "dropout" in parts:
         dropout_ops(d)
+    if "bias" in parts:
+        bias_ops(d)
 D.world_finalize()
