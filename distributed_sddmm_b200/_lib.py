@@ -87,6 +87,15 @@ ABI = {
     "hnh_sparse_attention_grad_kv_bias_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
                                                         _P, _I64, _P, _I64, C.c_double, _P, _I64, _P, _I64, C.c_double,
                                                         C.c_uint64, _I64, _I64, _P, _P, _P]),
+    "hnh_sparse_attention_step_edge_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, C.c_double,
+                                                     _P, _I64, _P, _I64, _P, _I64, C.c_double, C.c_uint64, _I64, _I64, _P,
+                                                     _P, _I64, _P]),
+    "hnh_sparse_attention_grad_q_edge_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
+                                                       _P, _I64, _P, _I64, C.c_double, _P, _I64, C.c_double, C.c_uint64,
+                                                       _I64, _I64, _P, _P, _P, _I64, _P, _I64, _P]),
+    "hnh_sparse_attention_grad_kv_edge_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
+                                                        _P, _I64, _P, _I64, C.c_double, _P, _I64, _P, _I64, C.c_double,
+                                                        C.c_uint64, _I64, _I64, _P, _P, _P, _I64, _P]),
     "hnh_entry_coords_from_index_f64": (C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
@@ -248,6 +257,10 @@ ABI.update({
     "hnhd_alg_sparse_attention_bias": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_double, C.c_uint64, _P]),
     "hnhd_alg_sparse_attention_backward_bias": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double,
                                                           C.c_double, C.c_uint64, _P, _P, _P, _P]),
+    "hnhd_alg_sparse_attention_edge": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_double, C.c_uint64, _P,
+                                                 _P]),
+    "hnhd_alg_sparse_attention_backward_edge": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double,
+                                                          C.c_double, C.c_uint64, _P, _P, _P, _P, _P, _P, _P]),
     "hnhd_alg_entry_coordinates": (C.c_int, [_P, C.c_int, _P, _P]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),

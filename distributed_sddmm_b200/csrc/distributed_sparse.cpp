@@ -763,6 +763,33 @@ BiasView bias_view(Distributed_Sparse &d, const VectorXd *b, VectorXd *grad, Ker
     v.head_stride = multiplicity > 1 ? (order == k_sddmmA ? d.num_S_values() : d.num_ST_values()) : 0;
     return v;
 }
+// Edge features of `order` as sparseAttention reads them: block b of head h starts at at(h, b), leading dimension r
+// (its gradient likewise); a null E gives null pointers
+struct EdgeView {
+    const DenseMatrix *E = nullptr;
+    DenseMatrix *grad = nullptr;
+    const SpmatLocal *m = nullptr;
+    int64_t d = 0;
+    int64_t offset(int h, int b) const { return (int64_t)m->blockStarts[(size_t)b] * E->cols() + h * d; }
+    const double *at(int h, int b) const { return E ? E->data() + offset(h, b) : nullptr; }
+    int64_t ld() const { return E ? E->cols() : d; }
+    double *grad_at(int h, int b) const { return grad ? grad->data() + offset(h, b) : nullptr; }
+};
+// The view of edge features of `order`, checked to be n x r (n that order's local entry count); HNH_E_INVALID else
+EdgeView edge_view(Distributed_Sparse &dist, const string &who, const char *name, const DenseMatrix *E, DenseMatrix *grad,
+                   KernelMode order, int64_t r, int64_t d) {
+    EdgeView v;
+    if (E == nullptr) return v;
+    const int64_t n = order == k_sddmmA ? dist.num_S_values() : dist.num_ST_values();
+    if (E->rows() != n || E->cols() != r)
+        throw hnh::Error(HNH_E_INVALID, who + ": " + name + " is " + to_string(E->rows()) + " x " + to_string(E->cols()) +
+                                            "; its order has " + to_string(n) + " entries and Q is " + to_string(r) + " wide");
+    v.E = E;
+    v.grad = grad;
+    v.m = values_matrix(dist, order);
+    v.d = d;
+    return v;
+}
 }  // namespace
 
 void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
@@ -789,11 +816,25 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
 
 void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
                                          double scale, double dropout, uint64_t seed, const VectorXd *bias) {
+    sparseAttention(Q, K, V, Z, L, heads, scale, dropout, seed, bias, nullptr);
+}
+
+void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                                 double scale, double dropout, uint64_t seed, const VectorXd *bias_A,
+                                                 const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B) {
+    sparseAttentionBackward(Q, K, V, Z, L, dZ, dQ, dK, dV, heads, scale, dropout, seed, bias_A, bias_B, dbias_A, dbias_B, nullptr,
+                            nullptr, nullptr);
+}
+
+void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                                         double scale, double dropout, uint64_t seed, const VectorXd *bias, const DenseMatrix *edge) {
     check_full_rows("sparseAttention");
     const int64_t d = check_attention(*this, "sparseAttention", {&Q, &Z}, {&K, &V}, L, heads, scale);
     check_dropout(*this, "sparseAttention", dropout);
     const BiasView bv =
         bias_view(*this, bias, nullptr, k_sddmmA, bias ? bias_heads(*this, "sparseAttention", "the bias", *bias, k_sddmmA, heads) : 0);
+    const EdgeView ev = edge_view(*this, "sparseAttention", "the edge features", edge, nullptr, k_sddmmA, Q.cols(), d);
     const BlockOrigin at(*this, k_sddmmA);
     // the online-softmax state of row u, head h: acc in Z's window, m in L[u, h], s in s[u, h]; m is not read while
     // s = 0, and the finish turns (acc, m, s) into (Z, L) in place
@@ -806,7 +847,14 @@ void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMa
         gather_pass(k_sddmmA, A_side, B_side, [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
             need_rows(rows_are_A, true, "sparseAttention");
             CSRHandle *hd = blk.getActive();
-            if (bias)
+            if (edge)
+                hnh::abi_check(hnh_sparse_attention_step_edge_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
+                                                                  (int)d, R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale,
+                                                                  R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, dropout,
+                                                                  seed + (uint64_t)h, at.u0(b), at.v0(b),
+                                                                  bias ? bv.at(h, b) : nullptr, ev.at(h, b), ev.ld(), compute()),
+                               "sparse_attention_step_edge");
+            else if (bias)
                 hnh::abi_check(hnh_sparse_attention_step_bias_f64(hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords,
                                                                   (int)d, R[0].p, R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, scale,
                                                                   R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, dropout,
@@ -835,7 +883,8 @@ void Distributed_Sparse::sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMa
 void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
                                                  DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
                                                  double scale, double dropout, uint64_t seed, const VectorXd *bias_A,
-                                                 const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B) {
+                                                 const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B,
+                                                 const DenseMatrix *edge_A, const DenseMatrix *edge_B, DenseMatrix *dedge) {
     const string who = "sparseAttentionBackward";
     check_full_rows(who);
     const int64_t d = check_attention(*this, who, {&Q, &Z, &dZ, &dQ}, {&K, &V, &dK, &dV}, L, heads, scale);
@@ -855,6 +904,17 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
             throw hnh::Error(HNH_E_INVALID, who + ": bias_A is " + (mA > 1 ? "per head" : "shared") + ", bias_B " +
                                                 (mB > 1 ? "per head" : "shared"));
     }
+    if ((edge_A == nullptr) != (edge_B == nullptr))
+        throw hnh::Error(HNH_E_INVALID, who + ": edge features need both orders, edge_A and edge_B");
+    if (dedge && !edge_A) throw hnh::Error(HNH_E_INVALID, who + ": an edge-feature gradient without edge features");
+    for (const DenseMatrix *o : {(const DenseMatrix *)&Q, (const DenseMatrix *)&K, (const DenseMatrix *)&V, (const DenseMatrix *)&Z,
+                                 (const DenseMatrix *)&L, (const DenseMatrix *)&dZ, (const DenseMatrix *)&dQ, (const DenseMatrix *)&dK,
+                                 (const DenseMatrix *)&dV, edge_A, edge_B})
+        if (dedge && dedge == o) throw hnh::Error(HNH_E_INVALID, who + ": dedge may not be another operand of the call");
+    const bool with_edge = edge_A != nullptr;
+    const EdgeView evA = edge_view(*this, who, "edge_A", edge_A, dedge, k_sddmmA, Q.cols(), d),
+                   evB = edge_view(*this, who, "edge_B", edge_B, nullptr, k_sddmmB, Q.cols(), d);
+    if (dedge) dedge->resize(edge_A->rows(), edge_A->cols());
     const BlockOrigin atA(*this, k_sddmmA), atB(*this, k_sddmmB);
     for (auto [g, b] : {std::make_pair(dbias_A, bias_A), std::make_pair(dbias_B, bias_B)})
         if (g) {
@@ -876,7 +936,15 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
                     [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
                         need_rows(rows_are_A, true, "sparseAttentionBackward");
                         CSRHandle *hd = blk.getActive();
-                        if (with_bias)
+                        if (with_edge)
+                            hnh::abi_check(hnh_sparse_attention_grad_q_edge_f64(
+                                               hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
+                                               R[0].ld, R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, Y[0].p, Y[0].ld, Y[1].p,
+                                               Y[1].ld, scale, R[4].p, R[4].ld, dropout, seed + (uint64_t)h, atA.u0(b), atA.v0(b),
+                                               with_bias ? bvA.at(h, b) : nullptr, bvA.grad_at(h, b), evA.at(h, b), evA.ld(),
+                                               evA.grad_at(h, b), evA.ld(), compute()),
+                                           "sparse_attention_grad_q_edge");
+                        else if (with_bias)
                             hnh::abi_check(hnh_sparse_attention_grad_q_bias_f64(
                                                hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
                                                R[0].ld, R[1].p, R[1].ld, R[2].p, R[2].ld, R[3].p, R[3].ld, Y[0].p, Y[0].ld, Y[1].p,
@@ -903,7 +971,15 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
                     [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
                         need_rows(rows_are_A, false, "sparseAttentionBackward");
                         CSRHandle *hd = blk.getActive();
-                        if (with_bias)
+                        if (with_edge)
+                            hnh::abi_check(hnh_sparse_attention_grad_kv_edge_f64(
+                                               hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
+                                               R[0].ld, R[1].p, R[1].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p,
+                                               Y[3].ld, scale, R[2].p, R[2].ld, R[3].p, R[3].ld, dropout, seed + (uint64_t)h,
+                                               atB.u0(b), atB.v0(b), with_bias ? bvB.at(h, b) : nullptr, bvB.grad_at(h, b),
+                                               evB.at(h, b), evB.ld(), compute()),
+                                           "sparse_attention_grad_kv_edge");
+                        else if (with_bias)
                             hnh::abi_check(hnh_sparse_attention_grad_kv_bias_f64(
                                                hd->rowStart.data(), hd->col_idx.data(), blk.rows, blk.num_coords, (int)d, R[0].p,
                                                R[0].ld, R[1].p, R[1].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, Y[2].p, Y[2].ld, Y[3].p,

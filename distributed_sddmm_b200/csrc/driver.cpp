@@ -427,6 +427,33 @@ int hnhd_alg_sparse_attention_backward_bias(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd
                                         dbias_A ? &dbias_A->v : nullptr, dbias_B ? &dbias_B->v : nullptr);
     });
 }
+int hnhd_alg_sparse_attention_edge(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                   hnhd_dense_t *L, int heads, double scale, double dropout, uint64_t seed,
+                                   const hnhd_vec_t *bias, const hnhd_dense_t *edge) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_edge: null argument");
+        if (!std::isfinite(scale)) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_edge: the scale must be finite");
+        a->alg->sparseAttention(Q->m, K->m, V->m, Z->m, L->m, heads, scale, dropout, seed, bias ? &bias->v : nullptr,
+                                edge ? &edge->m : nullptr);
+    });
+}
+int hnhd_alg_sparse_attention_backward_edge(hnhd_alg_t *a, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                            hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ, hnhd_dense_t *dK,
+                                            hnhd_dense_t *dV, int heads, double scale, double dropout, uint64_t seed,
+                                            const hnhd_vec_t *bias_A, const hnhd_vec_t *bias_B, hnhd_vec_t *dbias_A,
+                                            hnhd_vec_t *dbias_B, const hnhd_dense_t *edge_A, const hnhd_dense_t *edge_B,
+                                            hnhd_dense_t *dedge) {
+    return guarded([&] {
+        if (!a || !Q || !K || !V || !Z || !L || !dZ || !dQ || !dK || !dV)
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward_edge: null argument");
+        if (!std::isfinite(scale))
+            throw hnh::Error(HNH_E_INVALID, "hnhd_alg_sparse_attention_backward_edge: the scale must be finite");
+        a->alg->sparseAttentionBackward(Q->m, K->m, V->m, Z->m, L->m, dZ->m, dQ->m, dK->m, dV->m, heads, scale, dropout, seed,
+                                        bias_A ? &bias_A->v : nullptr, bias_B ? &bias_B->v : nullptr,
+                                        dbias_A ? &dbias_A->v : nullptr, dbias_B ? &dbias_B->v : nullptr,
+                                        edge_A ? &edge_A->m : nullptr, edge_B ? &edge_B->m : nullptr, dedge ? &dedge->m : nullptr);
+    });
+}
 int hnhd_alg_entry_coordinates(hnhd_alg_t *a, int mode, hnhd_vec_t *rows, hnhd_vec_t *cols) {
     return guarded([&] {
         if (!a || !rows || !cols) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_entry_coordinates: null argument");

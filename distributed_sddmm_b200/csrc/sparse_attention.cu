@@ -34,6 +34,16 @@
 // broadcast it with one shuffle, send a masked entry's column index complemented, and lane k keeps dx_k and adds it
 // to db[k] once per chunk.  The gradients compute x - L as (sigma <.,.> - L) + b, so a bias of zeros gives the bits
 // of the kernels without bias.  The instantiations with BIAS = false are the kernels without bias.
+//
+// Edge features (EDGE = true; the *_edge_f64 entry points): entry i of the block reads a d-wide row E_i, added to the
+// key and to the value: x_i = sigma <Q_u, K_v + E_i> (+ b_i), the step accumulates alpha_i (V_v + E_i), the gradients
+// use g_i = <dZ_u, V_v + E_i>, dQ_u += sigma dx_i (K_v + E_i), and grad_q writes dE_i = sigma dx_i Q_u + D_i w
+// alpha_i dZ_u (0 for a masked entry) once per entry when dE is not null.  The rows of a chunk's entries are
+// contiguous: every lane loads its own slice of E_i beside the K (step sweep 1, grad_q) or Q (grad_kv) row it gathers,
+// and adds it to the gathered row before any product, so E = 0 gives the bits of the kernels without E.  The step
+// reads E_i twice, once per sweep; the first read allocates in L1 so that the second, a chunk later, hits a cache.
+// grad_q writes the dE row from the Q_u and dZ_u it already holds, every lane its own slice.  The instantiations with
+// EDGE = false are the kernels without edge features.
 #include <cmath>
 
 #include "mix64.cuh"
@@ -62,6 +72,22 @@ struct Bias {
     double *db;
 };
 
+// The edge features of one call: entry i of the block reads E + i lde; grad_q writes dE_i to dE + i ldde unless dE
+// is null.  Passed after the Bias, so the kernels without edge features keep their parameter layout.
+struct Edge {
+    const double *E;
+    int64_t lde;
+    double *dE;
+    int64_t ldde;
+};
+
+// E_i's slice in the step's first sweep: read-only, allocating in L1 for the second sweep's read of the same row
+template <int VW>
+__device__ __forceinline__ void ld_edge(double (&d)[VW], const double *p) {
+    static_assert(VW == 2, "128-bit loads only");
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(d[0]), "=d"(d[1]) : "l"(p));
+}
+
 __device__ __forceinline__ bool keep(const Dropout &dr, int64_t u, int64_t v) {
     return (uint32_t)(mix64(dr.key ^ ((uint64_t)u << 32 | (uint64_t)v)) >> 32) >= dr.threshold;
 }
@@ -74,12 +100,12 @@ __device__ __forceinline__ double group_max(double d, unsigned mask) {
 }
 
 // ---- fast row kernels ----------------------------------------------------------------------------------------
-template <int R, int G, int VW, int UN, bool DROP, bool BIAS>
+template <int R, int G, int VW, int UN, bool DROP, bool BIAS, bool EDGE>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                  const double *__restrict__ Q, int64_t ldq, const double *__restrict__ K, int64_t ldk,
                  const double *__restrict__ V, int64_t ldv, double scale, double *__restrict__ acc, int64_t ldacc,
-                 double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds, Dropout dr, Bias bs) {
+                 double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds, Dropout dr, Bias bs, Edge eg) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -117,6 +143,15 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                     if (k < cnt) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) ld_gather<VW>(y[u][v], K + c * ldk + (v * G + gl) * VW);
+                        if constexpr (EDGE) {
+#pragma unroll
+                            for (int v = 0; v < NV; v++) {
+                                double ev[VW];
+                                ld_edge<VW>(ev, eg.E + (j + k) * eg.lde + (v * G + gl) * VW);
+#pragma unroll
+                                for (int w = 0; w < VW; w++) y[u][v][w] += ev[w];
+                            }
+                        }
                     } else {
 #pragma unroll
                         for (int v = 0; v < NV; v++)
@@ -166,6 +201,15 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
                     if (k < cnt && !((DROP || BIAS) && signbit(pv[u]))) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) ld_gather<VW>(y[u][v], V + c * ldv + (v * G + gl) * VW);
+                        if constexpr (EDGE) {
+#pragma unroll
+                            for (int v = 0; v < NV; v++) {
+                                double ev[VW];
+                                ld_gather<VW>(ev, eg.E + (j + k) * eg.lde + (v * G + gl) * VW);
+#pragma unroll
+                                for (int w = 0; w < VW; w++) y[u][v][w] += ev[w];
+                            }
+                        }
                     }
                 }
 #pragma unroll
@@ -208,13 +252,13 @@ attn_step_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
     }
 }
 
-template <int R, int G, int VW, int UN, bool DROP, bool BIAS>
+template <int R, int G, int VW, int UN, bool DROP, bool BIAS, bool EDGE>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                    const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                    const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                    const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv, double scale,
-                   double *__restrict__ dQ, int64_t lddq, Dropout dr, Bias bs) {
+                   double *__restrict__ dQ, int64_t lddq, Dropout dr, Bias bs, Edge eg) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -251,6 +295,7 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
             for (int k0 = 0; k0 < cnt; k0 += UN) {
                 double yk[UN][NV][VW], yv[UN][NV][VW];
                 double bu[UN];
+                bool kept[UN];  // EDGE: D_i = 1 and not masked (the weight of dZ_u in dE_i is nonzero)
 #pragma unroll
                 for (int u = 0; u < UN; u++) {
                     const int k = k0 + u;
@@ -258,6 +303,7 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
                     if constexpr (BIAS) bu[u] = __shfl_sync(gmask, mybias, k < G ? k : G - 1, G);
                     const bool dropped = (DROP || BIAS) && c < 0;
                     if (dropped) c = ~c;
+                    if constexpr (EDGE) kept[u] = !dropped;
                     if (k < cnt) {
 #pragma unroll
                         for (int v = 0; v < NV; v++) {
@@ -268,6 +314,15 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
                             } else {
 #pragma unroll
                                 for (int w = 0; w < VW; w++) yv[u][v][w] = 0.0;
+                            }
+                            if constexpr (EDGE) {
+                                double ev[VW];
+                                ld_gather<VW>(ev, eg.E + (j + k) * eg.lde + (v * G + gl) * VW);
+#pragma unroll
+                                for (int w = 0; w < VW; w++) {
+                                    yk[u][v][w] += ev[w];
+                                    if (!dropped) yv[u][v][w] += ev[w];
+                                }
                             }
                         }
                     } else {
@@ -302,6 +357,19 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
                         for (int v = 0; v < NV; v++)
 #pragma unroll
                             for (int w = 0; w < VW; w++) a[v][w] = fma(dx, yk[u][v][w], a[v][w]);
+                        if constexpr (EDGE) {
+                            if (eg.dE != nullptr) {
+                                // dE_i = sigma dx_i Q_u + D_i w alpha_i dZ_u
+                                const double g = scale * dx, aw = kept[u] ? (DROP ? al * dr.inv_keep : al) : 0.0;
+#pragma unroll
+                                for (int v = 0; v < NV; v++) {
+                                    double o[VW];
+#pragma unroll
+                                    for (int w = 0; w < VW; w++) o[w] = fma(g, q[v][w], aw * dz[v][w]);
+                                    st_rw<VW>(eg.dE + (j + k0 + u) * eg.ldde + (v * G + gl) * VW, o);
+                                }
+                            }
+                        }
                     }
                 }
             }
@@ -320,13 +388,14 @@ attn_grad_q_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restri
     }
 }
 
-template <int R, int G, int VW, int UN, bool DROP, bool BIAS>
+template <int R, int G, int VW, int UN, bool DROP, bool BIAS, bool EDGE>
 __global__ void __launch_bounds__(kBlock, 1)
 attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows,
                     const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
                     const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                     const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt, double scale,
-                    double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv, Dropout dr, Bias bs) {
+                    double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv, Dropout dr, Bias bs,
+                    Edge eg) {
     constexpr int NV = R / (G * VW);
     static_assert(NV * G * VW == R, "R must equal NV*G*VW");
     const int lane = threadIdx.x & 31;
@@ -362,7 +431,7 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
             if constexpr (BIAS)
                 if (mybias == -INFINITY && mycol >= 0) mycol = ~mycol;
             for (int k0 = 0; k0 < cnt; k0 += UN) {
-                double yq[UN][NV][VW], yd[UN][NV][VW];
+                double yq[UN][NV][VW], yd[UN][NV][VW], ye[UN][NV][VW];
                 double Lu[UN], tu[UN], bu[UN];
 #pragma unroll
                 for (int u = 0; u < UN; u++) {
@@ -385,12 +454,18 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
 #pragma unroll
                                 for (int w = 0; w < VW; w++) yd[u][v][w] = 0.0;
                             }
+                            if constexpr (EDGE) ld_gather<VW>(ye[u][v], eg.E + (j + k) * eg.lde + (v * G + gl) * VW);
                         }
                     } else {
 #pragma unroll
                         for (int v = 0; v < NV; v++)
 #pragma unroll
                             for (int w = 0; w < VW; w++) yq[u][v][w] = yd[u][v][w] = 0.0;
+                        if constexpr (EDGE)
+#pragma unroll
+                            for (int v = 0; v < NV; v++)
+#pragma unroll
+                                for (int w = 0; w < VW; w++) ye[u][v][w] = 0.0;
                     }
                 }
 #pragma unroll
@@ -400,8 +475,13 @@ attn_grad_kv_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restr
                     for (int v = 0; v < NV; v++)
 #pragma unroll
                         for (int w = 0; w < VW; w++) {
-                            d1 = fma(kr[v][w], yq[u][v][w], d1);
-                            d2 = fma(vr[v][w], yd[u][v][w], d2);
+                            if constexpr (EDGE) {
+                                d1 = fma(kr[v][w] + ye[u][v][w], yq[u][v][w], d1);
+                                d2 = fma(vr[v][w] + ye[u][v][w], yd[u][v][w], d2);
+                            } else {
+                                d1 = fma(kr[v][w], yq[u][v][w], d1);
+                                d2 = fma(vr[v][w], yd[u][v][w], d2);
+                            }
                         }
                     d1 = group_allreduce<G>(d1, gmask);
                     d2 = group_allreduce<G>(d2, gmask);
@@ -451,14 +531,20 @@ __device__ __forceinline__ double warp_dot(const double *x, const double *y, int
     for (int k = lane; k < d; k += 32) acc = fma(x[k], y[k], acc);
     return group_allreduce<32>(acc, 0xffffffffu);
 }
+// <x, y + e>, with the bits of warp_dot(x, y) where e = 0
+__device__ __forceinline__ double warp_dot_plus(const double *x, const double *y, const double *e, int d, int lane) {
+    double acc = 0.0;
+    for (int k = lane; k < d; k += 32) acc = fma(x[k], y[k] + e[k], acc);
+    return group_allreduce<32>(acc, 0xffffffffu);
+}
 
-template <bool DROP, bool BIAS>
+template <bool DROP, bool BIAS, bool EDGE>
 __global__ void __launch_bounds__(kBlock)
 attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                          const double *__restrict__ Q, int64_t ldq, const double *__restrict__ K, int64_t ldk,
                          const double *__restrict__ V, int64_t ldv, double scale, double *__restrict__ acc,
                          int64_t ldacc, double *__restrict__ m, int64_t ldm, double *__restrict__ s, int64_t lds,
-                         Dropout dr, Bias bs) {
+                         Dropout dr, Bias bs, Edge eg) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -469,12 +555,16 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
         double *a = acc + row * ldacc;
         for (int64_t j = s0; j < e; j++) {
             const int64_t c = col_idx[j];
+            const double *Ej = EDGE ? eg.E + j * eg.lde : nullptr;
             double x;
             if constexpr (BIAS) {
                 if (bs.b[j] == -INFINITY) continue;  // masked: adds nothing
-                x = scale * warp_dot(Q + row * ldq, K + c * ldk, d, lane) + bs.b[j];
+                x = scale * (EDGE ? warp_dot_plus(Q + row * ldq, K + c * ldk, Ej, d, lane)
+                                  : warp_dot(Q + row * ldq, K + c * ldk, d, lane)) +
+                    bs.b[j];
             } else {
-                x = scale * warp_dot(Q + row * ldq, K + c * ldk, d, lane);
+                x = scale * (EDGE ? warp_dot_plus(Q + row * ldq, K + c * ldk, Ej, d, lane)
+                                  : warp_dot(Q + row * ldq, K + c * ldk, d, lane));
             }
             const double mnew = fmax(mrow, x);
             const double f = exp(mrow - mnew), pj = exp(x - mnew);
@@ -482,7 +572,10 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
                 for (int k = lane; k < d; k += 32) a[k] *= f;
             } else {
                 const double pw = DROP ? pj * dr.inv_keep : pj;
-                for (int k = lane; k < d; k += 32) a[k] = fma(pw, V[c * ldv + k], a[k] * f);
+                if constexpr (EDGE)
+                    for (int k = lane; k < d; k += 32) a[k] = fma(pw, V[c * ldv + k] + Ej[k], a[k] * f);
+                else
+                    for (int k = lane; k < d; k += 32) a[k] = fma(pw, V[c * ldv + k], a[k] * f);
             }
             srow = fma(srow, f, pj);
             mrow = mnew;
@@ -494,13 +587,13 @@ attn_step_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__
     }
 }
 
-template <bool DROP, bool BIAS>
+template <bool DROP, bool BIAS, bool EDGE>
 __global__ void __launch_bounds__(kBlock)
 attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                            const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                            const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                            const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
-                           double scale, double *__restrict__ dQ, int64_t lddq, Dropout dr, Bias bs) {
+                           double scale, double *__restrict__ dQ, int64_t lddq, Dropout dr, Bias bs, Edge eg) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -509,6 +602,31 @@ attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *
         const double Lr = L[row * ldl], tr = t[row * ldt];
         for (int64_t j = s0; j < e; j++) {
             const int64_t c = col_idx[j];
+            if constexpr (EDGE) {
+                const double *Ej = eg.E + j * eg.lde;
+                double *dEj = eg.dE != nullptr ? eg.dE + j * eg.ldde : nullptr;
+                const double bj = BIAS ? bs.b[j] : 0.0;
+                if (BIAS && bj == -INFINITY) {  // masked: alpha = 0, dx = 0 (db[j] += 0), dE_j = 0
+                    if (dEj != nullptr)
+                        for (int k = lane; k < d; k += 32) dEj[k] = 0.0;
+                    continue;
+                }
+                const double d1 = warp_dot_plus(Q + row * ldq, K + c * ldk, Ej, d, lane);
+                const bool kept = !DROP || keep(dr, dr.u0 + row, dr.v0 + c);
+                // D_j w <dZ_u, V_v + E_j>
+                const double d2 = kept ? (DROP ? dr.inv_keep : 1.0) * warp_dot_plus(dZ + row * lddz, V + c * ldv, Ej, d, lane) : 0.0;
+                // L and t read at their use, as in the bias instantiation
+                const double al = BIAS ? exp((scale * d1 - L[row * ldl]) + bj) : exp(scale * d1 - L[row * ldl]);
+                const double dx = al * (d2 - t[row * ldt]);
+                if (BIAS && bs.db != nullptr && lane == 0) bs.db[j] += dx;
+                const double g = scale * dx;
+                if (dEj != nullptr) {
+                    const double aw = kept ? (DROP ? al * dr.inv_keep : al) : 0.0;
+                    for (int k = lane; k < d; k += 32) dEj[k] = fma(g, Q[row * ldq + k], aw * dZ[row * lddz + k]);
+                }
+                for (int k = lane; k < d; k += 32) dQ[row * lddq + k] = fma(g, K[c * ldk + k] + Ej[k], dQ[row * lddq + k]);
+                continue;
+            }
             double bj = 0.0;
             if constexpr (BIAS) {
                 bj = bs.b[j];
@@ -534,14 +652,14 @@ attn_grad_q_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *
     }
 }
 
-template <bool DROP, bool BIAS>
+template <bool DROP, bool BIAS, bool EDGE>
 __global__ void __launch_bounds__(kBlock)
 attn_grad_kv_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx, int64_t rows, int d,
                             const double *__restrict__ K, int64_t ldk, const double *__restrict__ V, int64_t ldv,
                             const double *__restrict__ Q, int64_t ldq, const double *__restrict__ dZ, int64_t lddz,
                             const double *__restrict__ L, int64_t ldl, const double *__restrict__ t, int64_t ldt,
                             double scale, double *__restrict__ dK, int64_t lddk, double *__restrict__ dV, int64_t lddv,
-                            Dropout dr, Bias bs) {
+                            Dropout dr, Bias bs, Edge eg) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
@@ -549,7 +667,9 @@ attn_grad_kv_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t 
         for (int64_t j = s0; j < e; j++) {
             const int64_t u = col_idx[j];
             if (BIAS && bs.b[j] == -INFINITY) continue;  // masked: alpha = 0, dx = 0 (db[j] += 0)
-            const double d1 = warp_dot(K + row * ldk, Q + u * ldq, d, lane);
+            const double *Ej = EDGE ? eg.E + j * eg.lde : nullptr;
+            // <K_v + E_j, Q_u>
+            const double d1 = EDGE ? warp_dot_plus(Q + u * ldq, K + row * ldk, Ej, d, lane) : warp_dot(K + row * ldk, Q + u * ldq, d, lane);
             // x_uv - L_u
             auto xl = [&] { return BIAS ? (scale * d1 - L[u * ldl]) + bs.b[j] : scale * d1 - L[u * ldl]; };
             if (DROP && !keep(dr, dr.u0 + u, dr.v0 + row)) {  // here the stored row is the key v
@@ -559,7 +679,7 @@ attn_grad_kv_generic_kernel(const int64_t *__restrict__ rowStart, const int64_t 
                 for (int k = lane; k < d; k += 32) dK[row * lddk + k] = fma(g, Q[u * ldq + k], dK[row * lddk + k]);
                 continue;
             }
-            const double d2 = warp_dot(V + row * ldv, dZ + u * lddz, d, lane);
+            const double d2 = EDGE ? warp_dot_plus(dZ + u * lddz, V + row * ldv, Ej, d, lane) : warp_dot(V + row * ldv, dZ + u * lddz, d, lane);
             const double al = exp(xl());
             const double aw = DROP ? al * dr.inv_keep : al;
             const double dx = al * ((DROP ? dr.inv_keep * d2 : d2) - t[u * ldt]);
@@ -618,6 +738,11 @@ bool fast_path(int d, std::initializer_list<Operand> ops) {
     return true;
 }
 
+// fast_path's condition on the edge operands: E and, when written, dE
+bool edge_fast(const Edge &eg) {
+    return aligned16(eg.E) && eg.lde % 2 == 0 && (eg.dE == nullptr || (aligned16(eg.dE) && eg.ldde % 2 == 0));
+}
+
 // The Dropout of a call: HNH_OK, or HNH_E_INVALID for p outside [0, 1) (NaN included) or a negative offset
 int make_dropout(const char *who, double p, uint64_t seed, int64_t u0, int64_t v0, Dropout *dr) {
     if (!(p >= 0.0 && p < 1.0)) return set_error(HNH_E_INVALID, "%s: the dropout probability must lie in [0, 1) (got %g)", who, p);
@@ -631,10 +756,10 @@ int make_dropout(const char *who, double p, uint64_t seed, int64_t u0, int64_t v
     return HNH_OK;
 }
 
-template <bool DROP, bool BIAS>
+template <bool DROP, bool BIAS, bool EDGE>
 int step(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *Q,
          int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv, double scale, double *acc, int64_t ldacc,
-         double *m, int64_t ldm, double *s, int64_t lds, const Dropout &dr, const Bias &bs, void *stream) {
+         double *m, int64_t ldm, double *s, int64_t lds, const Dropout &dr, const Bias &bs, const Edge &eg, void *stream) {
     const std::initializer_list<Operand> ops = {{Q, ldq, true}, {K, ldk, true},   {V, ldv, true},
                                                 {acc, ldacc, true}, {m, ldm, false}, {s, lds, false}};
     int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
@@ -642,30 +767,30 @@ int step(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64
     if (v == 1) return HNH_OK;
     cudaStream_t st = (cudaStream_t)stream;
     int grid = 0, rc = HNH_OK;
-    if (fast_path(d, ops)) {
+    if (fast_path(d, ops) && (!EDGE || edge_fast(eg))) {
 #define STEP(RR, G, VW, UN)                                                                                                \
     {                                                                                                                      \
-        auto k = attn_step_kernel<RR, G, VW, UN, DROP, BIAS>;                                                              \
+        auto k = attn_step_kernel<RR, G, VW, UN, DROP, BIAS, EDGE>;                                                              \
         rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
         if (!rc)                                                                                                           \
             rc = launch(k, grid, kBlock, st, "attn_step_kernel", rowStart, col_idx, rows, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, \
-                        ldm, s, lds, dr, bs);                                                                              \
+                        ldm, s, lds, dr, bs, eg);                                                                              \
     }
         HNH_DISPATCH_R(d, STEP, )
 #undef STEP
         return rc;
     }
-    auto k = attn_step_generic_kernel<DROP, BIAS>;
+    auto k = attn_step_generic_kernel<DROP, BIAS, EDGE>;
     rc = grid_for(k, rows, kBlock / 32, &grid);
     return rc ? rc : launch(k, grid, kBlock, st, "attn_step_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, K, ldk, V, ldv,
-                            scale, acc, ldacc, m, ldm, s, lds, dr, bs);
+                            scale, acc, ldacc, m, ldm, s, lds, dr, bs, eg);
 }
 
-template <bool DROP, bool BIAS>
+template <bool DROP, bool BIAS, bool EDGE>
 int grad_q(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *Q,
            int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
            const double *K, int64_t ldk, const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq,
-           const Dropout &dr, const Bias &bs, void *stream) {
+           const Dropout &dr, const Bias &bs, const Edge &eg, void *stream) {
     const std::initializer_list<Operand> ops = {{Q, ldq, true}, {dZ, lddz, true}, {L, ldl, false}, {t, ldt, false},
                                                 {K, ldk, true}, {V, ldv, true},   {dQ, lddq, true}};
     int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
@@ -673,30 +798,30 @@ int grad_q(const char *who, const int64_t *rowStart, const int64_t *col_idx, int
     if (v == 1) return HNH_OK;
     cudaStream_t st = (cudaStream_t)stream;
     int grid = 0, rc = HNH_OK;
-    if (fast_path(d, ops)) {
+    if (fast_path(d, ops) && (!EDGE || edge_fast(eg))) {
 #define GQ(RR, G, VW, UN)                                                                                                  \
     {                                                                                                                      \
-        auto k = attn_grad_q_kernel<RR, G, VW, UN, DROP, BIAS>;                                                            \
+        auto k = attn_grad_q_kernel<RR, G, VW, UN, DROP, BIAS, EDGE>;                                                            \
         rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
         if (!rc)                                                                                                           \
             rc = launch(k, grid, kBlock, st, "attn_grad_q_kernel", rowStart, col_idx, rows, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, \
-                        V, ldv, scale, dQ, lddq, dr, bs);                                                                  \
+                        V, ldv, scale, dQ, lddq, dr, bs, eg);                                                                  \
     }
         HNH_DISPATCH_R(d, GQ, )
 #undef GQ
         return rc;
     }
-    auto k = attn_grad_q_generic_kernel<DROP, BIAS>;
+    auto k = attn_grad_q_generic_kernel<DROP, BIAS, EDGE>;
     rc = grid_for(k, rows, kBlock / 32, &grid);
     return rc ? rc : launch(k, grid, kBlock, st, "attn_grad_q_generic_kernel", rowStart, col_idx, rows, d, Q, ldq, dZ, lddz, L,
-                            ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq, dr, bs);
+                            ldl, t, ldt, K, ldk, V, ldv, scale, dQ, lddq, dr, bs, eg);
 }
 
-template <bool DROP, bool BIAS>
+template <bool DROP, bool BIAS, bool EDGE>
 int grad_kv(const char *who, const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d, const double *K,
             int64_t ldk, const double *V, int64_t ldv, const double *Q, int64_t ldq, const double *dZ, int64_t lddz,
             const double *L, int64_t ldl, const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
-            int64_t lddv, const Dropout &dr, const Bias &bs, void *stream) {
+            int64_t lddv, const Dropout &dr, const Bias &bs, const Edge &eg, void *stream) {
     const std::initializer_list<Operand> ops = {{K, ldk, true},   {V, ldv, true},   {Q, ldq, true},   {dZ, lddz, true},
                                                 {L, ldl, false},  {t, ldt, false},  {dK, lddk, true}, {dV, lddv, true}};
     int v = check_call(who, rowStart, col_idx, rows, nnz, d, scale, ops);
@@ -704,23 +829,23 @@ int grad_kv(const char *who, const int64_t *rowStart, const int64_t *col_idx, in
     if (v == 1) return HNH_OK;
     cudaStream_t st = (cudaStream_t)stream;
     int grid = 0, rc = HNH_OK;
-    if (fast_path(d, ops)) {
+    if (fast_path(d, ops) && (!EDGE || edge_fast(eg))) {
 #define GKV(RR, G, VW, UN)                                                                                                 \
     {                                                                                                                      \
-        auto k = attn_grad_kv_kernel<RR, G, VW, UN, DROP, BIAS>;                                                           \
+        auto k = attn_grad_kv_kernel<RR, G, VW, UN, DROP, BIAS, EDGE>;                                                           \
         rc = grid_for(k, rows, kBlock / G, &grid);                                                                         \
         if (!rc)                                                                                                           \
             rc = launch(k, grid, kBlock, st, "attn_grad_kv_kernel", rowStart, col_idx, rows, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, \
-                        ldl, t, ldt, scale, dK, lddk, dV, lddv, dr, bs);                                                   \
+                        ldl, t, ldt, scale, dK, lddk, dV, lddv, dr, bs, eg);                                                   \
     }
         HNH_DISPATCH_R(d, GKV, )
 #undef GKV
         return rc;
     }
-    auto k = attn_grad_kv_generic_kernel<DROP, BIAS>;
+    auto k = attn_grad_kv_generic_kernel<DROP, BIAS, EDGE>;
     rc = grid_for(k, rows, kBlock / 32, &grid);
     return rc ? rc : launch(k, grid, kBlock, st, "attn_grad_kv_generic_kernel", rowStart, col_idx, rows, d, K, ldk, V, ldv, Q,
-                            ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, dr, bs);
+                            ldq, dZ, lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, dr, bs, eg);
 }
 
 // The Dropout of a bias call (p = 0: the kernels without dropout) with its bias checked: HNH_OK or HNH_E_INVALID
@@ -731,6 +856,25 @@ int make_bias_call(const char *who, double p, uint64_t seed, int64_t u0, int64_t
     return HNH_OK;
 }
 
+// The Dropout of an edge call (p = 0: the kernels without dropout) with its edge operands and nullable bias checked:
+// HNH_OK or HNH_E_INVALID
+int make_edge_call(const char *who, int d, double p, uint64_t seed, int64_t u0, int64_t v0, const double *bias,
+                   const double *dbias, const Edge &eg, Dropout *dr) {
+    const int rc = make_dropout(who, p, seed, u0, v0, dr);
+    if (rc) return rc;
+    if (dbias && !bias) return set_error(HNH_E_INVALID, "%s: dbias without a bias", who);
+    if (!eg.E) return set_error(HNH_E_INVALID, "%s: null E", who);
+    if (eg.lde < d) return set_error(HNH_E_INVALID, "%s: lde %lld below d = %d", who, (long long)eg.lde, d);
+    if (eg.dE && eg.ldde < d) return set_error(HNH_E_INVALID, "%s: ldde %lld below d = %d", who, (long long)eg.ldde, d);
+    if (eg.dE && (const double *)eg.dE == eg.E) return set_error(HNH_E_INVALID, "%s: dE is E", who);
+    return HNH_OK;
+}
+
+// The (DROP, BIAS) instantiation with EDGE = true of an edge call: DROP iff p > 0, BIAS iff a bias is given
+#define HNH_EDGE_CALL(FN, ...)                                                                                             \
+    (p == 0.0 ? (bias ? FN<false, true, true>(__VA_ARGS__) : FN<false, false, true>(__VA_ARGS__))                        \
+              : (bias ? FN<true, true, true>(__VA_ARGS__) : FN<true, false, true>(__VA_ARGS__)))
+
 }  // namespace
 
 extern "C" {
@@ -739,8 +883,8 @@ int hnh_sparse_attention_step_f64(const int64_t *rowStart, const int64_t *col_id
                                   const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv,
                                   double scale, double *acc, int64_t ldacc, double *m, int64_t ldm, double *s, int64_t lds,
                                   void *stream) {
-    return step<false, false>("hnh_sparse_attention_step_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale,
-                              acc, ldacc, m, ldm, s, lds, Dropout{}, Bias{}, stream);
+    return step<false, false, false>("hnh_sparse_attention_step_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale,
+                              acc, ldacc, m, ldm, s, lds, Dropout{}, Bias{}, Edge{}, stream);
 }
 
 int hnh_sparse_attention_step_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -751,8 +895,8 @@ int hnh_sparse_attention_step_dropout_f64(const int64_t *rowStart, const int64_t
     const char *who = "hnh_sparse_attention_step_dropout_f64";
     Dropout dr;
     const int rc = make_dropout(who, p, seed, u0, v0, &dr);
-    return rc ? rc : step<true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
-                                       lds, dr, Bias{}, stream);
+    return rc ? rc : step<true, false, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
+                                       lds, dr, Bias{}, Edge{}, stream);
 }
 
 int hnh_sparse_attention_step_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -764,10 +908,10 @@ int hnh_sparse_attention_step_bias_f64(const int64_t *rowStart, const int64_t *c
     const int rc = make_bias_call(who, p, seed, u0, v0, bias, &dr);
     if (rc) return rc;
     const Bias bs{bias, nullptr};
-    return p == 0.0 ? step<false, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
-                                        lds, dr, bs, stream)
-                    : step<true, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
-                                       lds, dr, bs, stream);
+    return p == 0.0 ? step<false, true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
+                                        lds, dr, bs, Edge{}, stream)
+                    : step<true, true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s,
+                                       lds, dr, bs, Edge{}, stream);
 }
 
 int hnh_sparse_attention_finish_f64(int64_t rows, int d, const double *acc, int64_t ldacc, const double *m, int64_t ldm,
@@ -790,8 +934,8 @@ int hnh_sparse_attention_grad_q_f64(const int64_t *rowStart, const int64_t *col_
                                     const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
                                     const double *t, int64_t ldt, const double *K, int64_t ldk, const double *V, int64_t ldv,
                                     double scale, double *dQ, int64_t lddq, void *stream) {
-    return grad_q<false, false>("hnh_sparse_attention_grad_q_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t,
-                                ldt, K, ldk, V, ldv, scale, dQ, lddq, Dropout{}, Bias{}, stream);
+    return grad_q<false, false, false>("hnh_sparse_attention_grad_q_f64", rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t,
+                                ldt, K, ldk, V, ldv, scale, dQ, lddq, Dropout{}, Bias{}, Edge{}, stream);
 }
 
 int hnh_sparse_attention_grad_q_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -802,8 +946,8 @@ int hnh_sparse_attention_grad_q_dropout_f64(const int64_t *rowStart, const int64
     const char *who = "hnh_sparse_attention_grad_q_dropout_f64";
     Dropout dr;
     const int rc = make_dropout(who, p, seed, u0, v0, &dr);
-    return rc ? rc : grad_q<true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
-                                         scale, dQ, lddq, dr, Bias{}, stream);
+    return rc ? rc : grad_q<true, false, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
+                                         scale, dQ, lddq, dr, Bias{}, Edge{}, stream);
 }
 
 int hnh_sparse_attention_grad_q_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -817,18 +961,18 @@ int hnh_sparse_attention_grad_q_bias_f64(const int64_t *rowStart, const int64_t 
     const int rc = make_bias_call(who, p, seed, u0, v0, bias, &dr);
     if (rc) return rc;
     const Bias bs{bias, dbias};
-    return p == 0.0 ? grad_q<false, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
-                                          scale, dQ, lddq, dr, bs, stream)
-                    : grad_q<true, true>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
-                                         scale, dQ, lddq, dr, bs, stream);
+    return p == 0.0 ? grad_q<false, true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
+                                          scale, dQ, lddq, dr, bs, Edge{}, stream)
+                    : grad_q<true, true, false>(who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv,
+                                         scale, dQ, lddq, dr, bs, Edge{}, stream);
 }
 
 int hnh_sparse_attention_grad_kv_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
                                      const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q, int64_t ldq,
                                      const double *dZ, int64_t lddz, const double *L, int64_t ldl, const double *t, int64_t ldt,
                                      double scale, double *dK, int64_t lddk, double *dV, int64_t lddv, void *stream) {
-    return grad_kv<false, false>("hnh_sparse_attention_grad_kv_f64", rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ,
-                                 lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, Dropout{}, Bias{}, stream);
+    return grad_kv<false, false, false>("hnh_sparse_attention_grad_kv_f64", rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ,
+                                 lddz, L, ldl, t, ldt, scale, dK, lddk, dV, lddv, Dropout{}, Bias{}, Edge{}, stream);
 }
 
 int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -839,8 +983,8 @@ int hnh_sparse_attention_grad_kv_dropout_f64(const int64_t *rowStart, const int6
     const char *who = "hnh_sparse_attention_grad_kv_dropout_f64";
     Dropout dr;
     const int rc = make_dropout(who, p, seed, u0, v0, &dr);
-    return rc ? rc : grad_kv<true, false>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
-                                          scale, dK, lddk, dV, lddv, dr, Bias{}, stream);
+    return rc ? rc : grad_kv<true, false, false>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
+                                          scale, dK, lddk, dV, lddv, dr, Bias{}, Edge{}, stream);
 }
 
 int hnh_sparse_attention_grad_kv_bias_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
@@ -854,10 +998,57 @@ int hnh_sparse_attention_grad_kv_bias_f64(const int64_t *rowStart, const int64_t
     const int rc = make_bias_call(who, p, seed, u0, v0, bias, &dr);
     if (rc) return rc;
     const Bias bs{bias, dbias};
-    return p == 0.0 ? grad_kv<false, true>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
-                                           scale, dK, lddk, dV, lddv, dr, bs, stream)
-                    : grad_kv<true, true>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
-                                          scale, dK, lddk, dV, lddv, dr, bs, stream);
+    return p == 0.0 ? grad_kv<false, true, false>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
+                                           scale, dK, lddk, dV, lddv, dr, bs, Edge{}, stream)
+                    : grad_kv<true, true, false>(who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt,
+                                          scale, dK, lddk, dV, lddv, dr, bs, Edge{}, stream);
+}
+
+int hnh_sparse_attention_step_edge_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                       const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V, int64_t ldv,
+                                       double scale, double *acc, int64_t ldacc, double *m, int64_t ldm, double *s, int64_t lds,
+                                       double p, uint64_t seed, int64_t u0, int64_t v0, const double *bias, const double *E,
+                                       int64_t lde, void *stream) {
+    const char *who = "hnh_sparse_attention_step_edge_f64";
+    const Edge eg{E, lde, nullptr, 0};
+    Dropout dr;
+    const int rc = make_edge_call(who, d, p, seed, u0, v0, bias, nullptr, eg, &dr);
+    if (rc) return rc;
+    const Bias bs{bias, nullptr};
+    return HNH_EDGE_CALL(step, who, rowStart, col_idx, rows, nnz, d, Q, ldq, K, ldk, V, ldv, scale, acc, ldacc, m, ldm, s, lds,
+                         dr, bs, eg, stream);
+}
+
+int hnh_sparse_attention_grad_q_edge_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                         const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
+                                         int64_t ldl, const double *t, int64_t ldt, const double *K, int64_t ldk,
+                                         const double *V, int64_t ldv, double scale, double *dQ, int64_t lddq, double p,
+                                         uint64_t seed, int64_t u0, int64_t v0, const double *bias, double *dbias,
+                                         const double *E, int64_t lde, double *dE, int64_t ldde, void *stream) {
+    const char *who = "hnh_sparse_attention_grad_q_edge_f64";
+    const Edge eg{E, lde, dE, ldde};
+    Dropout dr;
+    const int rc = make_edge_call(who, d, p, seed, u0, v0, bias, dbias, eg, &dr);
+    if (rc) return rc;
+    const Bias bs{bias, dbias};
+    return HNH_EDGE_CALL(grad_q, who, rowStart, col_idx, rows, nnz, d, Q, ldq, dZ, lddz, L, ldl, t, ldt, K, ldk, V, ldv, scale,
+                         dQ, lddq, dr, bs, eg, stream);
+}
+
+int hnh_sparse_attention_grad_kv_edge_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                          const double *K, int64_t ldk, const double *V, int64_t ldv, const double *Q,
+                                          int64_t ldq, const double *dZ, int64_t lddz, const double *L, int64_t ldl,
+                                          const double *t, int64_t ldt, double scale, double *dK, int64_t lddk, double *dV,
+                                          int64_t lddv, double p, uint64_t seed, int64_t u0, int64_t v0, const double *bias,
+                                          double *dbias, const double *E, int64_t lde, void *stream) {
+    const char *who = "hnh_sparse_attention_grad_kv_edge_f64";
+    const Edge eg{E, lde, nullptr, 0};
+    Dropout dr;
+    const int rc = make_edge_call(who, d, p, seed, u0, v0, bias, dbias, eg, &dr);
+    if (rc) return rc;
+    const Bias bs{bias, dbias};
+    return HNH_EDGE_CALL(grad_kv, who, rowStart, col_idx, rows, nnz, d, K, ldk, V, ldv, Q, ldq, dZ, lddz, L, ldl, t, ldt, scale,
+                         dK, lddk, dV, lddv, dr, bs, eg, stream);
 }
 
 }  // extern "C"

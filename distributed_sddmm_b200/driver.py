@@ -324,7 +324,7 @@ class Algorithm:
         return p, int(seed)
 
     def sparse_attention(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, heads: int = 1, scale=None,
-                         dropout: float = 0.0, seed: int = 0, bias: Vec = None):
+                         dropout: float = 0.0, seed: int = 0, bias: Vec = None, edge: Dense = None):
         """Collective: fused attention over the pattern of S (its values are not read).  Q and Z are A-shaped, K and V
         B-shaped, all r wide; per head h of width d = r / heads, Z_u,h = sum over the stored (u, v) of
         softmax_v(scale <Q_u,h, K_v,h>) V_v,h, and L (Dense.create(localArows, heads)) = the rows' log-sum-exp (-inf,
@@ -343,10 +343,22 @@ class Algorithm:
         and L = -inf, as a row without entries (edge_softmax gives NaN there).  +inf or NaN are not checked and make
         the row NaN.  Contract, not checked: b is a function of the global S-row and S-column (entry_coordinates
         gives them), so stored duplicates of (u, v) share one bias, and every rank passes its part of the same
-        bias.  A bias of zeros gives the bits of the call without bias."""
+        bias.  A bias of zeros gives the bits of the call without bias.
+
+        edge (a Dense, or None) holds edge features added to the keys and the values, as PyG's TransformerConv with
+        edge_dim does: x_uv,h = scale <Q_u,h, K_v,h + E_uv,h> (+ b_uv,h) and Z_u,h = sum_v softmax(x)_uv (V_v,h +
+        E_uv,h) (with dropout's weights).  It is Dense.create(len(like_S_values()), r): row i belongs to entry i of the
+        A-order value vector, filled in the order of entry_coordinates("A"), and head h reads its columns
+        [h d, (h + 1) d).  It stays on this rank (no ring carries it).  Contract, not checked: E is a function of the
+        global S-row and S-column, so stored duplicates of (u, v) share one row, and every rank passes its part of the
+        same E.  E = 0 gives the bits of the call without it."""
         s = self._attention_scale(Q, heads, scale)
         p, sd = self._dropout_args(dropout, seed)
-        if bias is None:
+        if edge is not None:
+            check(lib().hnhd_alg_sparse_attention_edge(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s, p, sd,
+                                                       self._vec_arg(bias, "bias"), self._dense_arg(edge, "edge")),
+                  "sparse_attention")
+        elif bias is None:
             check(lib().hnhd_alg_sparse_attention_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, int(heads), s, p, sd),
                   "sparse_attention")
         else:
@@ -356,7 +368,8 @@ class Algorithm:
 
     def sparse_attention_backward(self, Q: Dense, K: Dense, V: Dense, Z: Dense, L: Dense, dZ: Dense, dQ: Dense, dK: Dense,
                                   dV: Dense, heads: int = 1, scale=None, dropout: float = 0.0, seed: int = 0,
-                                  bias: Vec = None, bias_B: Vec = None, dbias: Vec = None, dbias_B: Vec = None):
+                                  bias: Vec = None, bias_B: Vec = None, dbias: Vec = None, dbias_B: Vec = None,
+                                  edge: Dense = None, edge_B: Dense = None, dedge: Dense = None):
         """Collective: given dZ = dLoss/dZ and the forward's Z and L, overwrites dQ, dK and dV with the gradients of
         sparse_attention (Distributed_Sparse::sparseAttentionBackward).  dropout and seed must be the ones the forward
         got, and the same on every rank: the backward regenerates the forward's mask from them.
@@ -366,22 +379,48 @@ class Algorithm:
         hold the same b(u, v) for every stored (u, v); build bias_B from entry_coordinates("B").  dbias / dbias_B
         (optional Vecs, resized to their bias's length) receive dLoss/dbias in each order:
         dx_uv,h = alpha_uv (D w <dZ_u,h, V_v,h> - t_u,h), summed over the heads for a shared bias, in a fixed order
-        (repeats are bit-identical); 0 at a masked entry."""
+        (repeats are bit-identical); 0 at a masked entry.
+
+        With edge features, the backward needs them in both value orders as well: `edge` (the forward's, A order)
+        for the dQ pass and `edge_B` (Dense.create(len(like_ST_values()), r), B order, filled from
+        entry_coordinates("B")) for the dK, dV pass, holding the same e(u, v) for every stored (u, v).  dedge (an
+        optional Dense, resized to edge's shape and overwritten) receives dLoss/dE in the A order:
+        dE_uv,h = scale dx_uv,h Q_u,h + D w alpha_uv,h dZ_u,h, 0 at a masked entry."""
         s = self._attention_scale(Q, heads, scale)
         p, sd = self._dropout_args(dropout, seed)
+        if edge is None and edge_B is None:
+            if dedge is not None:
+                raise ValueError("dedge needs the edge features")
+        elif edge is None or edge_B is None:
+            raise ValueError("edge features need both value orders: edge (A order) and edge_B (B order)")
+        if (bias is None) != (bias_B is None):
+            raise ValueError("a bias needs both value orders: bias (A order) and bias_B (B order)")
+        if bias is None and (dbias is not None or dbias_B is not None):
+            raise ValueError("dbias / dbias_B need their bias")
+        if edge is not None:
+            check(lib().hnhd_alg_sparse_attention_backward_edge(
+                self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h, int(heads), s, p, sd, self._vec_arg(bias, "bias"),
+                self._vec_arg(bias_B, "bias_B"), self._vec_arg(dbias, "dbias"), self._vec_arg(dbias_B, "dbias_B"),
+                self._dense_arg(edge, "edge"), self._dense_arg(edge_B, "edge_B"), self._dense_arg(dedge, "dedge")),
+                "sparse_attention_backward")
+            return
         if bias is None and bias_B is None:
-            if dbias is not None or dbias_B is not None:
-                raise ValueError("dbias / dbias_B need their bias")
             check(lib().hnhd_alg_sparse_attention_backward_dropout(self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h,
                                                                    int(heads), s, p, sd),
                   "sparse_attention_backward")
             return
-        if bias is None or bias_B is None:
-            raise ValueError("a bias needs both value orders: bias (A order) and bias_B (B order)")
         check(lib().hnhd_alg_sparse_attention_backward_bias(
             self.h, Q.h, K.h, V.h, Z.h, L.h, dZ.h, dQ.h, dK.h, dV.h, int(heads), s, p, sd, self._vec_arg(bias, "bias"),
             self._vec_arg(bias_B, "bias_B"), self._vec_arg(dbias, "dbias"), self._vec_arg(dbias_B, "dbias_B")),
             "sparse_attention_backward")
+
+    @staticmethod
+    def _dense_arg(m, name):
+        if m is None:
+            return None
+        if not isinstance(m, Dense):
+            raise TypeError(f"{name} must be a Dense, not {type(m).__name__}")
+        return m.h
 
     @staticmethod
     def _vec_arg(v, name):

@@ -254,6 +254,28 @@ public:
                                  DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
                                  double scale, double dropout, uint64_t seed, const VectorXd *bias_A,
                                  const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B);
+    // The same with edge features added to the keys and values (TransformerConv with edge_dim): per entry i = (u, v)
+    // and head h, x_i,h = scale <Q_u,h, K_v,h + E_i,h> + b_i,h and Z_u,h = sum_i D_i w alpha_i (V_v,h + E_i,h); the
+    // backward uses g_i = <dZ_u, V_v + E_i> in dx_i = alpha_i (D_i w g_i - t_u), dQ_u = scale sum_i dx_i (K_v + E_i),
+    // dK_v and dV_v keep their formulas, and it writes dE_i = scale dx_i Q_u + D_i w alpha_i dZ_u.  E is a
+    // DenseMatrix of n x r, n the local entry count of the order it is used in (num_S_values / num_ST_values, the
+    // order of like_S_values / like_ST_values): row i belongs to entry i of that order's value vector and head h
+    // reads its columns [h d, (h + 1) d).  It stays on the rank that owns the entry; no ring carries it.  The forward
+    // and the dQ pass read `edge` / `edge_A` (A order), the dK, dV pass `edge_B` (B order).  `dedge` (nullable) is
+    // resized to edge_A's shape and overwritten in the A order; a masked entry's row is 0.  Contract, not checked:
+    // edge_A and edge_B hold the same e(u, v), a function of the global S-row and S-column (entryCoordinates), so
+    // stored duplicates of (u, v) share one row; the backward gets the forward's E; every rank passes its part of
+    // the same E.  E = 0 gives the bits of the call without E.  A null edge (both null in the backward) is the call
+    // without E: the overloads above forward here with null pointers.  HNH_E_INVALID on every rank before any
+    // launch for an E that is not n x r, only one of edge_A / edge_B, a dedge without E, or a dedge that is another
+    // operand of the call.
+    void sparseAttention(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L, int heads,
+                         double scale, double dropout, uint64_t seed, const VectorXd *bias, const DenseMatrix *edge);
+    void sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K, DenseMatrix &V, DenseMatrix &Z, DenseMatrix &L,
+                                 DenseMatrix &dZ, DenseMatrix &dQ, DenseMatrix &dK, DenseMatrix &dV, int heads,
+                                 double scale, double dropout, uint64_t seed, const VectorXd *bias_A,
+                                 const VectorXd *bias_B, VectorXd *dbias_A, VectorXd *dbias_B, const DenseMatrix *edge_A,
+                                 const DenseMatrix *edge_B, DenseMatrix *dedge);
     // rows / cols (resized to the order's local entry count) become the global S-row and S-column of every entry
     // of this rank's value vector of `order` (k_sddmmA: like_S_values, k_sddmmB: like_ST_values), as exact
     // doubles.  No communication.  Defined where check_full_rows passes; HNH_E_INVALID on every rank elsewhere.

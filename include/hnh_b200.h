@@ -360,6 +360,39 @@ int hnh_sparse_attention_grad_kv_bias_f64(const int64_t *rowStart, const int64_t
                                           int64_t ldl, const double *t, int64_t ldt, double scale, double *dK,
                                           int64_t lddk, double *dV, int64_t lddv, double p, uint64_t seed, int64_t u0,
                                           int64_t v0, const double *bias, double *dbias, void *stream);
+/* Edge features: the bias calls with a nullable bias (null: no bias; p = 0: no dropout) and, before the stream, a
+ * d-wide row per entry, E_i at E + i lde (block-local, in col_idx order), added to the key and to the value:
+ *     x_i = scale <Q_u, K_v + E_i> + bias[i],     Z_u = sum_i D_i w alpha_i (V_v + E_i)
+ * (D w = 1 without dropout).  The gradients use g_i = <dZ_u, V_v + E_i> and dx_i = alpha_i (D_i w g_i - t_u):
+ *     dQ_u += scale sum_i dx_i (K_v + E_i),  dK_v += scale sum_i dx_i Q_u,  dV_v += sum_i D_i w alpha_i dZ_u,
+ * dbias as above, and grad_q also writes (overwrites, once per entry)
+ *     dE_i = scale dx_i Q_u + D_i w alpha_i dZ_u
+ * to dE + i ldde when dE is not null (0 for a masked entry; scale dx_i Q_u for a dropped one).  grad_q reads E in
+ * the order of its (A-order) block, grad_kv in that of its transpose (B order): both must hold the same e(u, v) for
+ * every stored (u, v), as the step did.  Masking and rows without live entries are as for the bias.  E = 0 gives
+ * results bit-identical to the calls without E (finite inputs, no signed zeros).  The fast kernels need E (and dE)
+ * 16-byte aligned with an even leading dimension, as the other d-wide operands; else the generic kernels run.
+ * E null, lde < d, dE with ldde < d, dE == E, dbias without bias, p < 0, p >= 1, NaN, u0 < 0 or v0 < 0:
+ * HNH_E_INVALID before any launch. */
+int hnh_sparse_attention_step_edge_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, int d,
+                                       const double *Q, int64_t ldq, const double *K, int64_t ldk, const double *V,
+                                       int64_t ldv, double scale, double *acc, int64_t ldacc, double *m, int64_t ldm,
+                                       double *s, int64_t lds, double p, uint64_t seed, int64_t u0, int64_t v0,
+                                       const double *bias, const double *E, int64_t lde, void *stream);
+int hnh_sparse_attention_grad_q_edge_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                                         int d, const double *Q, int64_t ldq, const double *dZ, int64_t lddz,
+                                         const double *L, int64_t ldl, const double *t, int64_t ldt, const double *K,
+                                         int64_t ldk, const double *V, int64_t ldv, double scale, double *dQ,
+                                         int64_t lddq, double p, uint64_t seed, int64_t u0, int64_t v0,
+                                         const double *bias, double *dbias, const double *E, int64_t lde, double *dE,
+                                         int64_t ldde, void *stream);
+int hnh_sparse_attention_grad_kv_edge_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                                          int d, const double *K, int64_t ldk, const double *V, int64_t ldv,
+                                          const double *Q, int64_t ldq, const double *dZ, int64_t lddz, const double *L,
+                                          int64_t ldl, const double *t, int64_t ldt, double scale, double *dK,
+                                          int64_t lddk, double *dV, int64_t lddv, double p, uint64_t seed, int64_t u0,
+                                          int64_t v0, const double *bias, double *dbias, const double *E, int64_t lde,
+                                          void *stream);
 
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of

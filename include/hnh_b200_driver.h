@@ -214,6 +214,19 @@ int hnhd_alg_sparse_attention_backward_bias(hnhd_alg_t *alg, hnhd_dense_t *Q, hn
                                             hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale, double dropout,
                                             uint64_t seed, const hnhd_vec_t *bias_A, const hnhd_vec_t *bias_B,
                                             hnhd_vec_t *dbias_A, hnhd_vec_t *dbias_B);
+/* With edge features added to the keys and values (Distributed_Sparse::sparseAttention / sparseAttentionBackward with
+ * edge pointers): edge / edge_A an A-order matrix, edge_B a B-order one, each n x r (n the order's local entry
+ * count); dedge (nullable) is resized to edge_A's shape and overwritten.  Bias pointers as in the _bias calls,
+ * nullable.  A null edge (both null in the backward) is the call without edge features. */
+int hnhd_alg_sparse_attention_edge(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V, hnhd_dense_t *Z,
+                                   hnhd_dense_t *L, int heads, double scale, double dropout, uint64_t seed,
+                                   const hnhd_vec_t *bias, const hnhd_dense_t *edge);
+int hnhd_alg_sparse_attention_backward_edge(hnhd_alg_t *alg, hnhd_dense_t *Q, hnhd_dense_t *K, hnhd_dense_t *V,
+                                            hnhd_dense_t *Z, hnhd_dense_t *L, hnhd_dense_t *dZ, hnhd_dense_t *dQ,
+                                            hnhd_dense_t *dK, hnhd_dense_t *dV, int heads, double scale, double dropout,
+                                            uint64_t seed, const hnhd_vec_t *bias_A, const hnhd_vec_t *bias_B,
+                                            hnhd_vec_t *dbias_A, hnhd_vec_t *dbias_B, const hnhd_dense_t *edge_A,
+                                            const hnhd_dense_t *edge_B, hnhd_dense_t *dedge);
 /* rows / cols (resized) become the global S-row and S-column of every entry of this rank's value vector of `mode`
  * (0 = A order, 1 = B order) (Distributed_Sparse::entryCoordinates). */
 int hnhd_alg_entry_coordinates(hnhd_alg_t *alg, int mode, hnhd_vec_t *rows, hnhd_vec_t *cols);

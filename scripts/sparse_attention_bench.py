@@ -28,7 +28,13 @@ Additive score bias (PARTS=bias): each of the three bias kernels (hnh_sparse_att
 uniform in [-1, 1), the gradients writing dbias) beside its kernel without bias, alternated the same way; the two
 gradient kernels with and without the dbias write; then Algorithm.sparse_attention and sparse_attention_backward
 (writing both dbias vectors) with and without a bias.  The bias adds 8 bytes read per entry, and dbias 16 more (read
-and write), to the byte counts above.  PARTS (kernels,ops,dropout; also bias) picks the sections.
+and write), to the byte counts above.
+Edge features (PARTS=edge): each of the three edge kernels (hnh_sparse_attention_*_edge_f64, p = 0, no bias, E
+uniform in [-1, 1), grad_q writing dE) beside its kernel without E, alternated the same way, with the ratio of their
+bytes/s; then Algorithm.sparse_attention and sparse_attention_backward (writing dE) with and without E.  E adds 8d
+bytes read per entry to the step and to grad_kv, and 16d (E read, dE written) to grad_q; a gathered row still counts
+once per entry.  E, its B-order copy and dE take 3 x 8 d bytes per entry (51 GB at 2^20 rows, 32 per row and d = 64),
+so run this part at WIDTHS=32,64.  PARTS (kernels,ops,dropout; also bias, edge) picks the sections.
 Environment: LOGM (20), NPR (32), WIDTHS (128,256), ALG (15d_fusion1), REPS (20), DROPOUT (0.1), ROUNDS (5), PARTS."""
 import json
 import math
@@ -370,6 +376,86 @@ def bias_ops(d):
     del alg
 
 
+def edge_kernels(alg, d):
+    a_blk, b_blk = ("ST", "S") if alg_name == "15d_fusion1" else ("S", "ST")
+    rows, nnz, rs, ci = block(alg, a_blk)
+    rowsT, nnzT, rsT, ciT = block(alg, b_blk)
+    g = torch.Generator(device=dev).manual_seed(1)
+    n = max(rows, rowsT)
+    Q, K, V, dZ = (torch.rand((n, d), generator=g, **f64) * 2 - 1 for _ in range(4))
+    acc, dQ, dK, dV = (torch.zeros((n, d), **f64) for _ in range(4))
+    ms_ = torch.zeros((rows, 2), **f64)
+    Lt = torch.rand((n, 2), generator=g, **f64) + 4  # L, t: a plausible log-sum-exp of 32 entries, and <dZ, Z>
+    EA, EB = torch.rand((nnz, d), generator=g, **f64) * 2 - 1, torch.rand((nnzT, d), generator=g, **f64) * 2 - 1
+    dE = torch.zeros((nnz, d), **f64)
+    scale = 1 / math.sqrt(d)
+    p = lambda t: t.data_ptr()  # noqa: E731
+    noe = (0.0, SEED, 0, 0, None)
+
+    def step(e=False):
+        args = (p(rs), p(ci), rows, nnz, d, p(Q), d, p(K), d, p(V), d, scale, p(acc), d, p(ms_), 2, p(ms_) + 8, 2)
+        if e:
+            D.check(L.hnh_sparse_attention_step_edge_f64(*args, *noe, p(EA), d, st))
+        else:
+            D.check(L.hnh_sparse_attention_step_f64(*args, st))
+
+    def grad_q(e=False):
+        args = (p(rs), p(ci), rows, nnz, d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, p(K), d, p(V), d, scale, p(dQ), d)
+        if e:
+            D.check(L.hnh_sparse_attention_grad_q_edge_f64(*args, *noe, None, p(EA), d, p(dE), d, st))
+        else:
+            D.check(L.hnh_sparse_attention_grad_q_f64(*args, st))
+
+    def grad_kv(e=False):
+        args = (p(rsT), p(ciT), rowsT, nnzT, d, p(K), d, p(V), d, p(Q), d, p(dZ), d, p(Lt), 2, p(Lt) + 8, 2, scale, p(dK), d,
+                p(dV), d)
+        if e:
+            D.check(L.hnh_sparse_attention_grad_kv_edge_f64(*args, *noe, None, p(EB), d, st))
+        else:
+            D.check(L.hnh_sparse_attention_grad_kv_f64(*args, st))
+
+    time_ratio, rate_ratio = {}, {}
+    for name, fn, nbytes, ne in (("step", step, nnz * (8 + 16 * d) + rows * (8 + 24 * d + 32), nnz * 8 * d),
+                                 ("grad_q", grad_q, nnz * (8 + 16 * d) + rows * (8 + 32 * d + 16), nnz * 16 * d),
+                                 ("grad_kv", grad_kv, nnzT * (24 + 16 * d) + rowsT * (8 + 48 * d), nnzT * 8 * d)):
+        r = alternate_pair((name, name + "_edge"), d, (fn, lambda fn=fn: fn(True)), nbytes=(nbytes, nbytes + ne))
+        time_ratio[name] = round(r, 3)
+        rate_ratio[name] = round((nbytes + ne) / nbytes / r, 3)
+    print(json.dumps(dict(d=d, entries=nnz, edge_kernel_over_kernel_time=time_ratio,
+                          edge_kernel_over_kernel_bytes_per_s=rate_ratio)), flush=True)
+
+
+def edge_ops(d):
+    alg = D.Algorithm(alg_name, S, d, 1)
+    dims = alg.dims
+    rng = np.random.default_rng(SEED)
+    Q, dZ = (alg.like_A_matrix() for _ in range(2))
+    K, V = (alg.like_B_matrix() for _ in range(2))
+    for m in (Q, dZ, K, V):
+        m.from_host(rng.uniform(-1, 1, m.shape))
+    Z, dQ, dK, dV = alg.like_A_matrix(), alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix()
+    Lm = D.Dense.create(dims.localArows, 1)
+    edges = []
+    for mode in ("A", "B"):
+        r_, c_ = alg.entry_coordinates(mode)
+        e = D.Dense.create(len(r_), d)
+        e.from_host(np.cos(0.31 * r_[:, None] + 0.73 * c_[:, None] + 0.45 * np.arange(d)[None, :]))
+        edges.append(e)
+        del r_, c_
+    dE = D.Dense.create(1, 1)
+    fwd = alternate_pair(("op_fused_forward", "op_fused_forward_edge"), d,
+                         (lambda: alg.sparse_attention(Q, K, V, Z, Lm), lambda: alg.sparse_attention(Q, K, V, Z, Lm, edge=edges[0])),
+                         timer=timed_op)
+    alg.sparse_attention(Q, K, V, Z, Lm, edge=edges[0])
+    bwd = alternate_pair(("op_fused_backward", "op_fused_backward_edge"), d,
+                         (lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV),
+                          lambda: alg.sparse_attention_backward(Q, K, V, Z, Lm, dZ, dQ, dK, dV, edge=edges[0], edge_B=edges[1],
+                                                                dedge=dE)), timer=timed_op)
+    print(json.dumps(dict(d=d, forward_edge_over_forward=round(fwd, 3), backward_edge_over_backward=round(bwd, 3))),
+          flush=True)
+    del alg
+
+
 for d in widths:
     alg = D.Algorithm(alg_name, S, d, 1)
     if "kernels" in parts:
@@ -378,6 +464,8 @@ for d in widths:
         dropout_kernels(alg, d)
     if "bias" in parts:
         bias_kernels(alg, d)
+    if "edge" in parts:
+        edge_kernels(alg, d)
     del alg
     torch.cuda.empty_cache()
     if "ops" in parts:
@@ -386,4 +474,6 @@ for d in widths:
         dropout_ops(d)
     if "bias" in parts:
         bias_ops(d)
+    if "edge" in parts:
+        edge_ops(d)
 D.world_finalize()
