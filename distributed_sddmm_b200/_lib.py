@@ -96,6 +96,10 @@ ABI = {
     "hnh_sparse_attention_grad_kv_edge_f64": (C.c_int, [_P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, _P, _I64,
                                                         _P, _I64, _P, _I64, C.c_double, _P, _I64, _P, _I64, C.c_double,
                                                         C.c_uint64, _I64, _I64, _P, _P, _P, _I64, _P]),
+    "hnh_row_bias_add_f64": (C.c_int, [_P, _P, _I64, _I64, _P]),
+    "hnh_gt_gate_f64": (C.c_int, [_P, _P, _P, _P, _I64, _I64, C.c_int, _P]),
+    "hnh_gt_gate_backward_workspace_bytes": (C.c_int64, [_I64, _I64]),
+    "hnh_gt_gate_backward_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, C.c_int, _P, C.c_size_t, _P]),
     "hnh_entry_coords_from_index_f64": (C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
@@ -263,6 +267,19 @@ ABI.update({
                                                           C.c_double, C.c_uint64, _P, _P, _P, _P, _P, _P, _P]),
     "hnhd_alg_entry_coordinates": (C.c_int, [_P, C.c_int, _P, _P]),
     "hnhd_gat_destroy": (None, [_P]),
+    "hnhd_gt_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, _PP]),
+    "hnhd_gt_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_gt_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_gt_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_gt_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_gt_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_gt_set_input": (C.c_int, [_P, _P]),
+    "hnhd_gt_get_buffer": (C.c_int, [_P, C.c_int, _P]),
+    "hnhd_gt_set_edge_attributes": (C.c_int, [_P, _P, _I64, _P, _I64]),
+    "hnhd_gt_forward": (C.c_int, [_P, C.c_double, C.c_uint64]),
+    "hnhd_gt_backward": (C.c_int, [_P, _P]),
+    "hnhd_gt_get_input_grad": (C.c_int, [_P, _P]),
+    "hnhd_gt_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

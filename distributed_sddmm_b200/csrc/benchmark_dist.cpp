@@ -17,6 +17,7 @@
 #include "hnh/25D_cannon_sparse.hpp"
 #include "hnh/als_conjugate_gradients.h"
 #include "hnh/gat.hpp"
+#include "hnh/graph_transformer.hpp"
 #include "hnh_b200.h"
 
 Distributed_Sparse *hnh_make_algorithm(const string &name, SpmatLocal *spmat, int R, int c, KernelImplementation *k) {
@@ -37,12 +38,22 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
     std::unique_ptr<Distributed_Sparse> d_ops(hnh_make_algorithm(algorithm_name, spmat, R, c, &local_ops));
     std::unique_ptr<Distributed_ALS> d_als;
     std::unique_ptr<GAT> gnn;
+    std::unique_ptr<GraphTransformer> transformer;
     DenseMatrix gat_output_grad;
     const bool gat_app = app == "gat" || app == "gat_train" || app == "gat_softmax" || app == "gat_softmax_train" ||
                          app == "gat_additive" || app == "gat_additive_train" || app == "gat_v2" || app == "gat_v2_train";
     const bool gat_train =
         app == "gat_train" || app == "gat_softmax_train" || app == "gat_additive_train" || app == "gat_v2_train";
-    if (gat_app) {
+    const bool gt_app = app == "graph_transformer" || app == "graph_transformer_train";
+    if (gt_app) {
+        // GAT's three layer shapes as TransformerConv layers (no edge features, no gate; the parameters stay zero,
+        // as GAT's weights do); graph_transformer_train: forwardPass() then backwardPass(dL/d output = ones) per call
+        vector<GraphTransformerLayer> layers{GraphTransformerLayer(256, 256, 4), GraphTransformerLayer(1024, 256, 4),
+                                             GraphTransformerLayer(1024, 256, 6)};
+        transformer.reset(new GraphTransformer(layers, d_ops.get(), 0, false));
+        if (app == "graph_transformer_train")
+            gat_output_grad = DenseMatrix::Constant(transformer->buffers.back().rows(), transformer->buffers.back().cols(), 1.0);
+    } else if (gat_app) {
         // the three layers of the reference's GAT benchmark: (input width, width per head, heads)
         vector<GATLayer> layers{GATLayer(256, 256, 4), GATLayer(1024, 256, 4), GATLayer(1024, 256, 6)};
         gnn.reset(new GAT(layers, d_ops.get()));
@@ -70,8 +81,8 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
         d_als.reset(new Distributed_ALS(d_ops.get(), true));
     } else if (app != "vanilla") {
         throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\", \"gat\", \"gat_train\", \"gat_softmax\", "
-                                        "\"gat_softmax_train\", \"gat_additive\", \"gat_additive_train\", \"gat_v2\" or "
-                                        "\"gat_v2_train\"");
+                                        "\"gat_softmax_train\", \"gat_additive\", \"gat_additive_train\", \"gat_v2\", "
+                                        "\"gat_v2_train\", \"graph_transformer\" or \"graph_transformer_train\"");
     }
 
     DenseMatrix A = d_ops->like_A_matrix(0.001);
@@ -89,6 +100,9 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
                 d_ops->sddmmA(A, B, Sv, sddmm_result);
                 d_ops->spmmA(A, B, Sv);
             }
+        } else if (gt_app) {
+            transformer->forwardPass(0.0, 0);
+            if (app == "graph_transformer_train") transformer->backwardPass(gat_output_grad);
         } else if (gat_app) {
             gnn->forwardPass();
             if (gat_train) gnn->backwardPass(gat_output_grad);

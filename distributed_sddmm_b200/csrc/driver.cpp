@@ -13,6 +13,7 @@
 #include "hnh/benchmark_dist.hpp"
 #include "hnh/distributed_sparse.h"
 #include "hnh/gat.hpp"
+#include "hnh/graph_transformer.hpp"
 #include "hnh_b200.h"
 #include "launch.h"
 
@@ -33,6 +34,9 @@ struct hnhd_vec {
 };
 struct hnhd_gat {
     std::unique_ptr<GAT> g;
+};
+struct hnhd_gt {
+    std::unique_ptr<GraphTransformer> g;
 };
 
 namespace {
@@ -670,5 +674,132 @@ int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1
     });
 }
 void hnhd_gat_destroy(hnhd_gat_t *g) { delete g; }
+
+// ---- graph transformer -----------------------------------------------------------------------------
+int hnhd_gt_create(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_gt_t **out) {
+    return guarded([&] {
+        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_create: bad argument");
+        vector<GraphTransformerLayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
+        std::unique_ptr<hnhd_gt> g(new hnhd_gt);
+        g->g.reset(new GraphTransformer(layers, a->alg.get(), edge_dim, beta != 0));
+        *out = g.release();
+    });
+}
+// The parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
+struct GtParam {
+    int64_t offset, rows, cols;
+};
+static GtParam gt_param(hnhd_gt_t *g, int layer, const char *name) {
+    if (!g || !name) throw hnh::Error(HNH_E_INVALID, "graph transformer: null argument");
+    GraphTransformer &m = *g->g;
+    if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no such layer");
+    const GraphTransformerLayer &l = m.layers[(size_t)layer];
+    const int64_t f = l.input_features, r = l.output_features();
+    static const char *const projections[4] = {"query", "key", "value", "skip"};
+    const string s = name;
+    for (int j = 0; j < 4; j++) {
+        if (s == projections[j]) return {l.projection_offset(j), f, r};
+        if (s == string(projections[j]) + "_bias") return {l.projection_offset(j) + f * r, r, 1};
+    }
+    if (s == "edge" && m.edge_dim > 0) return {l.edge_offset(), m.edge_dim, r};
+    if (s == "beta" && m.beta) return {l.beta_offset(m.edge_dim), 3 * r, 1};
+    throw hnh::Error(HNH_E_INVALID, "graph transformer: no parameter \"" + s + "\" in this model");
+}
+// copy n doubles between host and device on the compute stream and wait for the copy
+static void gt_copy(double *dst, const double *src, int64_t n, cudaMemcpyKind kind) {
+    cudaStream_t s = hnh::Runtime::get().compute_stream();
+    if (n > 0) hnh::cuda_check(cudaMemcpyAsync(dst, src, sizeof(double) * (size_t)n, kind, s), "graph transformer copy");
+    hnh::cuda_check(cudaStreamSynchronize(s), "graph transformer copy");
+}
+static DenseMatrix &gt_buffer(hnhd_gt_t *g, int buffer) {
+    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no such buffer");
+    return g->g->buffers[(size_t)buffer];
+}
+int hnhd_gt_param_shape(hnhd_gt_t *g, int layer, const char *name, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        const GtParam p = gt_param(g, layer, name);
+        if (rows) *rows = p.rows;
+        if (cols) *cols = p.cols;
+    });
+}
+int hnhd_gt_set_param(hnhd_gt_t *g, int layer, const char *name, const double *host) {
+    return guarded([&] {
+        const GtParam p = gt_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gt_copy(g->g->layers[(size_t)layer].params.data() + p.offset, host, p.rows * p.cols, cudaMemcpyHostToDevice);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_gt_get_param(hnhd_gt_t *g, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const GtParam p = gt_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gt_copy(host, g->g->layers[(size_t)layer].params.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_gt_get_param_grad(hnhd_gt_t *g, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const GtParam p = gt_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const GraphTransformerLayer &l = g->g->layers[(size_t)layer];
+        if (l.grads.size() != l.params.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no backward pass has run");
+        gt_copy(host, l.grads.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_gt_buffer_shape(hnhd_gt_t *g, int buffer, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        DenseMatrix &b = gt_buffer(g, buffer);
+        if (rows) *rows = b.rows();
+        if (cols) *cols = b.cols();
+    });
+}
+int hnhd_gt_set_input(hnhd_gt_t *g, const double *host) {
+    return guarded([&] {
+        DenseMatrix &b = gt_buffer(g, 0);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        b.copy_from_host(host);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_gt_set_edge_attributes(hnhd_gt_t *g, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
+        if ((n_A > 0 && !attr_A) || (n_B > 0 && !attr_B)) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        g->g->setEdgeAttributes(attr_A, n_A, attr_B, n_B);
+    });
+}
+int hnhd_gt_get_buffer(hnhd_gt_t *g, int buffer, double *host) {
+    return guarded([&] {
+        DenseMatrix &b = gt_buffer(g, buffer);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        b.copy_to_host(host);
+    });
+}
+int hnhd_gt_forward(hnhd_gt_t *g, double dropout, uint64_t seed) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
+        g->g->forwardPass(dropout, seed);
+    });
+}
+int hnhd_gt_backward(hnhd_gt_t *g, const double *host_output_grad) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
+        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const DenseMatrix &out = g->g->buffers.back();
+        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
+        g->g->backwardPass(grad);
+    });
+}
+int hnhd_gt_get_input_grad(hnhd_gt_t *g, double *host) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (g->g->input_grad.size() != g->g->buffers[0].size())
+            throw hnh::Error(HNH_E_INVALID, "graph transformer: no backward pass has run");
+        g->g->input_grad.copy_to_host(host);
+    });
+}
+void hnhd_gt_destroy(hnhd_gt_t *g) { delete g; }
 
 }  // extern "C"

@@ -1,0 +1,295 @@
+// graph_transformer.cu -- the row-wise device operations of the graph transformer (include/hnh/graph_transformer.hpp)
+// beyond the projections (hnh_dgemm_f64 and friends) and fused sparse attention.  All matrices are row-major n x r
+// and contiguous; w_beta (nullable) holds 3r doubles [w1 | w2 | w3]:
+//     X[i, :] += b                                            projection bias                 (row_bias_kernel)
+//     s_i = <w1, M_i> + <w2, R_i> + <w3, M_i - R_i>,  beta_i = sigmoid(s_i)
+//     Y_i = beta_i R_i + (1 - beta_i) M_i   (M_i + R_i without w_beta),  then ReLU when asked
+//                                                             the gate forward                (gate_kernel)
+// Backward, with dY = G, or G where Y > 0 after a ReLU, and ds_i = <dY_i, R_i - M_i> beta_i (1 - beta_i):
+//     dM_i = (1 - beta_i) dY_i + ds_i (w1 + w3),  dR_i = beta_i dY_i + ds_i (w2 - w3)   (dM = dR = dY without w_beta)
+//                                                             one row pass                    (gate_backward_kernel)
+//     dw_beta = sum_i ds_i [M_i, R_i, M_i - R_i]              two stages: fixed row chunks     (gate_dw_partial_kernel)
+//                                                             then the chunks in order         (gate_dw_final_kernel)
+//
+// The row kernels run one warp per row: lanes stride the row in 16-byte pairs when r is even and every row pointer is
+// 16-byte aligned, in scalars otherwise, and a row's dot products end in the warp's xor butterfly, which leaves the
+// same bits on every lane.  The dw_beta chunks depend on n only, never on the device, so repeated calls are
+// bit-identical everywhere.  No floating-point atomics.
+#include "row_gather.cuh"
+
+namespace {
+
+using hnh::grid_for;
+using hnh::launch;
+using hnh::set_error;
+
+constexpr int kCtasPerSm = 16;         // grid cap of the row kernels
+constexpr int64_t kMaxChunks = 128;    // dw_beta partial sums: at most this many row chunks ...
+constexpr int64_t kMinChunkRows = 512; // ... of at least this many rows (fewer chunks for small n)
+
+int64_t dw_chunks(int64_t n) { return std::max<int64_t>(1, std::min<int64_t>(kMaxChunks, (n + kMinChunkRows - 1) / kMinChunkRows)); }
+
+__device__ __forceinline__ double sigmoid(double s) { return 1.0 / (1.0 + exp(-s)); }
+
+// X[i, :] += b
+template <bool kPairs>
+__global__ void __launch_bounds__(kBlock) row_bias_kernel(double *__restrict__ X, const double *__restrict__ b, int64_t n, int64_t r) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        if (kPairs) {
+            double2 *row = reinterpret_cast<double2 *>(X + i * r);
+            const double2 *bb = reinterpret_cast<const double2 *>(b);
+#pragma unroll 2  // ptxas spills 8 bytes at its default unroll of this loop
+            for (int64_t k = lane; k < r / 2; k += 32) {
+                const double2 v = row[k], c = __ldg(bb + k);
+                row[k] = make_double2(v.x + c.x, v.y + c.y);
+            }
+        } else {
+            double *row = X + i * r;
+            for (int64_t k = lane; k < r; k += 32) row[k] += __ldg(b + k);
+        }
+    }
+}
+
+// s_i of row i: the gate's logit, the same bits on every lane
+template <bool kPairs>
+__device__ __forceinline__ double gate_logit(const double *m, const double *rr, const double *w, int64_t r, int lane) {
+    double x = 0.0;
+    if (kPairs) {
+        const double2 *m2 = reinterpret_cast<const double2 *>(m), *r2 = reinterpret_cast<const double2 *>(rr);
+        const double2 *w1 = reinterpret_cast<const double2 *>(w), *w2 = reinterpret_cast<const double2 *>(w + r),
+                      *w3 = reinterpret_cast<const double2 *>(w + 2 * r);
+        for (int64_t k = lane; k < r / 2; k += 32) {
+            const double2 a = m2[k], c = r2[k], u = __ldg(w1 + k), v = __ldg(w2 + k), z = __ldg(w3 + k);
+            x = fma(u.x, a.x, x);
+            x = fma(v.x, c.x, x);
+            x = fma(z.x, a.x - c.x, x);
+            x = fma(u.y, a.y, x);
+            x = fma(v.y, c.y, x);
+            x = fma(z.y, a.y - c.y, x);
+        }
+    } else {
+        for (int64_t k = lane; k < r; k += 32) {
+            const double a = m[k], c = rr[k];
+            x = fma(__ldg(w + k), a, x);
+            x = fma(__ldg(w + r + k), c, x);
+            x = fma(__ldg(w + 2 * r + k), a - c, x);
+        }
+    }
+    return group_allreduce<32>(x, 0xffffffffu);
+}
+
+// Y = beta R + (1 - beta) M (M + R when !kBeta), ReLU when kRelu.  With the gate, the logit pass reads M and R
+// through L1 and the combine pass rereads them there.
+template <bool kPairs, bool kBeta, bool kRelu>
+__global__ void __launch_bounds__(kBlock)
+gate_kernel(double *__restrict__ Y, const double *__restrict__ M, const double *__restrict__ R, const double *__restrict__ w,
+            int64_t n, int64_t r) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const double *m = M + i * r, *rr = R + i * r;
+        double beta = 0.0;
+        if (kBeta) beta = sigmoid(gate_logit<kPairs>(m, rr, w, r, lane));
+        auto combine = [&](double a, double c) {
+            const double y = kBeta ? fma(beta, c, (1.0 - beta) * a) : a + c;
+            return kRelu ? fmax(y, 0.0) : y;
+        };
+        if (kPairs) {
+            const double2 *m2 = reinterpret_cast<const double2 *>(m), *r2 = reinterpret_cast<const double2 *>(rr);
+            double2 *y2 = reinterpret_cast<double2 *>(Y + i * r);
+            for (int64_t k = lane; k < r / 2; k += 32) {
+                const double2 a = __ldcs(m2 + k), c = __ldcs(r2 + k);
+                __stcs(y2 + k, make_double2(combine(a.x, c.x), combine(a.y, c.y)));
+            }
+        } else {
+            double *y = Y + i * r;
+            for (int64_t k = lane; k < r; k += 32) __stcs(y + k, combine(__ldcs(m + k), __ldcs(rr + k)));
+        }
+    }
+}
+
+// dM, dR (dR nullable without the gate) and ds_i (with the gate) of every row
+template <bool kPairs, bool kBeta, bool kRelu>
+__global__ void __launch_bounds__(kBlock)
+gate_backward_kernel(double *__restrict__ dM, double *__restrict__ dR, double *__restrict__ ds_out, const double *__restrict__ G,
+                     const double *__restrict__ Y, const double *__restrict__ M, const double *__restrict__ R,
+                     const double *__restrict__ w, int64_t n, int64_t r) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const double *g = G + i * r, *y = kRelu ? Y + i * r : nullptr, *m = M + i * r, *rr = R + i * r;
+        auto dy = [&](double gk, double yk) { return kRelu ? (yk > 0.0 ? gk : 0.0) : gk; };
+        double beta = 0.0, ds = 0.0;
+        if (kBeta) {
+            beta = sigmoid(gate_logit<kPairs>(m, rr, w, r, lane));
+            double t = 0.0;
+            if (kPairs) {
+                const double2 *g2 = reinterpret_cast<const double2 *>(g), *y2 = reinterpret_cast<const double2 *>(y),
+                              *m2 = reinterpret_cast<const double2 *>(m), *r2 = reinterpret_cast<const double2 *>(rr);
+                for (int64_t k = lane; k < r / 2; k += 32) {
+                    const double2 gk = g2[k], a = m2[k], c = r2[k];
+                    double2 yk = make_double2(0.0, 0.0);
+                    if (kRelu) yk = y2[k];
+                    t = fma(dy(gk.x, yk.x), c.x - a.x, t);
+                    t = fma(dy(gk.y, yk.y), c.y - a.y, t);
+                }
+            } else {
+                for (int64_t k = lane; k < r; k += 32) t = fma(dy(g[k], kRelu ? y[k] : 0.0), rr[k] - m[k], t);
+            }
+            ds = group_allreduce<32>(t, 0xffffffffu) * beta * (1.0 - beta);
+            if (lane == 0) ds_out[i] = ds;
+        }
+        if (kPairs) {
+            const double2 *g2 = reinterpret_cast<const double2 *>(g), *y2 = reinterpret_cast<const double2 *>(y);
+            double2 *dm2 = reinterpret_cast<double2 *>(dM + i * r), *dr2 = dR ? reinterpret_cast<double2 *>(dR + i * r) : nullptr;
+            for (int64_t k = lane; k < r / 2; k += 32) {
+                const double2 gk = __ldcs(g2 + k);
+                double2 yk = make_double2(0.0, 0.0);
+                if (kRelu) yk = __ldcs(y2 + k);
+                const double ax = dy(gk.x, yk.x), ay = dy(gk.y, yk.y);
+                if (kBeta) {
+                    const double2 u = __ldg(reinterpret_cast<const double2 *>(w) + k),
+                                  v = __ldg(reinterpret_cast<const double2 *>(w + r) + k),
+                                  z = __ldg(reinterpret_cast<const double2 *>(w + 2 * r) + k);
+                    __stcs(dm2 + k, make_double2(fma(ds, u.x + z.x, (1.0 - beta) * ax), fma(ds, u.y + z.y, (1.0 - beta) * ay)));
+                    __stcs(dr2 + k, make_double2(fma(ds, v.x - z.x, beta * ax), fma(ds, v.y - z.y, beta * ay)));
+                } else {
+                    __stcs(dm2 + k, make_double2(ax, ay));
+                    if (dr2) __stcs(dr2 + k, make_double2(ax, ay));
+                }
+            }
+        } else {
+            double *dm = dM + i * r, *dr = dR ? dR + i * r : nullptr;
+            for (int64_t k = lane; k < r; k += 32) {
+                const double a = dy(__ldcs(g + k), kRelu ? __ldcs(y + k) : 0.0);
+                if (kBeta) {
+                    const double u = __ldg(w + k), v = __ldg(w + r + k), z = __ldg(w + 2 * r + k);
+                    __stcs(dm + k, fma(ds, u + z, (1.0 - beta) * a));
+                    __stcs(dr + k, fma(ds, v - z, beta * a));
+                } else {
+                    __stcs(dm + k, a);
+                    if (dr) __stcs(dr + k, a);
+                }
+            }
+        }
+    }
+}
+
+// partial[c, :] = sum over the rows of chunk c (in row order) of ds_i [M_i, R_i, M_i - R_i]; one thread per column,
+// blockIdx.y the chunk
+__global__ void __launch_bounds__(kBlock)
+gate_dw_partial_kernel(double *__restrict__ partial, const double *__restrict__ ds, const double *__restrict__ M,
+                       const double *__restrict__ R, int64_t n, int64_t r, int64_t chunk_rows) {
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= r) return;
+    const int64_t c = blockIdx.y, i0 = c * chunk_rows, i1 = n < i0 + chunk_rows ? n : i0 + chunk_rows;
+    double a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    for (int64_t i = i0; i < i1; i++) {
+        const double s = __ldg(ds + i), a = ld_stream_f64(M + i * r + k), b = ld_stream_f64(R + i * r + k);
+        a1 = fma(s, a, a1);
+        a2 = fma(s, b, a2);
+        a3 = fma(s, a - b, a3);
+    }
+    double *out = partial + c * 3 * r;
+    out[k] = a1;
+    out[r + k] = a2;
+    out[2 * r + k] = a3;
+}
+
+// dw[j] = sum over the chunks, in order, of partial[c, j]
+__global__ void __launch_bounds__(kBlock)
+gate_dw_final_kernel(double *__restrict__ dw, const double *__restrict__ partial, int64_t chunks, int64_t len) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < len; j += stride) {
+        double s = 0.0;
+        for (int64_t c = 0; c < chunks; c++) s += partial[c * len + j];
+        dw[j] = s;
+    }
+}
+
+template <bool kPairs, bool kBeta>
+auto pick_gate(bool relu) {
+    return relu ? gate_kernel<kPairs, kBeta, true> : gate_kernel<kPairs, kBeta, false>;
+}
+template <bool kPairs, bool kBeta>
+auto pick_gate_backward(bool relu) {
+    return relu ? gate_backward_kernel<kPairs, kBeta, true> : gate_backward_kernel<kPairs, kBeta, false>;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hnh_row_bias_add_f64(double *X, const double *b, int64_t n, int64_t r, void *stream) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_row_bias_add_f64: negative size");
+    if (n == 0 || r == 0) return HNH_OK;
+    if (!X || !b) return set_error(HNH_E_INVALID, "hnh_row_bias_add_f64: null pointer");
+    auto k = r % 2 == 0 && aligned16(X) && aligned16(b) ? row_bias_kernel<true> : row_bias_kernel<false>;
+    int grid;
+    int rc = grid_for(k, n, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "row_bias_kernel", X, b, n, r);
+}
+
+int hnh_gt_gate_f64(double *Y, const double *M, const double *R, const double *w_beta, int64_t n, int64_t r, int relu,
+                    void *stream) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_gt_gate_f64: negative size");
+    if (n == 0 || r == 0) return HNH_OK;
+    if (!Y || !M || !R) return set_error(HNH_E_INVALID, "hnh_gt_gate_f64: null pointer");
+    if (Y == M || Y == R) return set_error(HNH_E_INVALID, "hnh_gt_gate_f64: Y may not be M or R");
+    const bool pairs = r % 2 == 0 && aligned16(Y) && aligned16(M) && aligned16(R) && (!w_beta || aligned16(w_beta));
+    auto k = w_beta ? (pairs ? pick_gate<true, true>(relu) : pick_gate<false, true>(relu))
+                    : (pairs ? pick_gate<true, false>(relu) : pick_gate<false, false>(relu));
+    int grid;
+    int rc = grid_for(k, n, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "gate_kernel", Y, M, R, w_beta, n, r);
+}
+
+int64_t hnh_gt_gate_backward_workspace_bytes(int64_t n, int64_t r) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_workspace_bytes: negative size");
+    return (int64_t)sizeof(double) * (n + dw_chunks(n) * 3 * r);
+}
+
+int hnh_gt_gate_backward_f64(double *dM, double *dR, double *dw_beta, const double *G, const double *Y, const double *M,
+                             const double *R, const double *w_beta, int64_t n, int64_t r, int relu, void *workspace,
+                             size_t workspace_bytes, void *stream) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: negative size");
+    const bool beta = w_beta != nullptr;
+    if (beta && !dw_beta) return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: the gate needs dw_beta");
+    if (!beta && dw_beta) return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: dw_beta without the gate");
+    if (r == 0) return HNH_OK;
+    if (n == 0) {  // no rows: dw_beta = 0
+        if (!beta) return HNH_OK;
+        return hnh::check_cuda(cudaMemsetAsync(dw_beta, 0, sizeof(double) * 3 * (size_t)r, (cudaStream_t)stream), "dw_beta");
+    }
+    if (!dM || !G || !M || !R || (relu && !Y) || (beta && !dR))
+        return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: null pointer");
+    const double *ins[] = {G, relu ? Y : nullptr, M, R, w_beta};
+    for (const double *o : {(const double *)dM, (const double *)dR, (const double *)dw_beta})
+        for (const double *in : ins)
+            if (o && o == in) return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: an output may not be an input");
+    if (dR && dR == dM) return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: dM and dR are one matrix");
+    const int64_t need = beta ? hnh_gt_gate_backward_workspace_bytes(n, r) : 0;
+    if (beta && (!workspace || (int64_t)workspace_bytes < need))
+        return set_error(HNH_E_INVALID, "hnh_gt_gate_backward_f64: the workspace needs %lld bytes", (long long)need);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool pairs = r % 2 == 0 && aligned16(dM) && (!dR || aligned16(dR)) && aligned16(G) && (!relu || aligned16(Y)) &&
+                       aligned16(M) && aligned16(R) && (!beta || aligned16(w_beta));
+    auto k = beta ? (pairs ? pick_gate_backward<true, true>(relu) : pick_gate_backward<false, true>(relu))
+                  : (pairs ? pick_gate_backward<true, false>(relu) : pick_gate_backward<false, false>(relu));
+    double *ds = beta ? (double *)workspace : nullptr;
+    int grid;
+    int rc = grid_for(k, n, kBlock / 32, &grid, kCtasPerSm);
+    if (!rc) rc = launch(k, grid, kBlock, st, "gate_backward_kernel", dM, dR, ds, G, relu ? Y : nullptr, M, R, w_beta, n, r);
+    if (rc || !beta) return rc;
+    const int64_t chunks = dw_chunks(n), chunk_rows = (n + chunks - 1) / chunks;
+    double *partial = ds + n;
+    rc = launch(gate_dw_partial_kernel, dim3((unsigned)((r + kBlock - 1) / kBlock), (unsigned)chunks), kBlock, st,
+                "gate_dw_partial_kernel", partial, (const double *)ds, M, R, n, r, chunk_rows);
+    if (rc) return rc;
+    rc = grid_for(gate_dw_final_kernel, 3 * r, kBlock, &grid, kCtasPerSm);
+    return rc ? rc : launch(gate_dw_final_kernel, grid, kBlock, st, "gate_dw_final_kernel", dw_beta, (const double *)partial, chunks, 3 * r);
+}
+
+}  // extern "C"

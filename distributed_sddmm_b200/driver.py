@@ -624,6 +624,121 @@ class GAT:
             pass
 
 
+class GraphTransformer:
+    """A graph transformer on fused sparse attention: layers of PyG's TransformerConv(concat=True, root_weight=True)
+    with the heads concatenated, forward and backward (include/hnh/graph_transformer.hpp).  layers: [(input_features,
+    features_per_head, num_heads), ...]; every layer but the last ends in a ReLU.  edge_dim > 0 adds edge features
+    (per-entry attributes, set with set_edge_attributes, projected by each layer's "edge" weight onto the keys and
+    values); beta=True the gated skip connection.  The algorithm object must outlive this one.
+
+    Parameters (zero after construction), by layer and name: "query", "key", "value", "skip" (input_features x r),
+    "query_bias", "key_bias", "value_bias", "skip_bias" (r), "edge" (edge_dim x r) and "beta" (3r).  A TransformerConv
+    state dict maps onto them as lin_query.weight.T -> "query", lin_query.bias -> "query_bias", ..., lin_edge.weight.T
+    -> "edge", lin_beta.weight[0] -> "beta"."""
+
+    PROJECTIONS = ("query", "key", "value", "skip")
+    VECTORS = ("query_bias", "key_bias", "value_bias", "skip_bias", "beta")
+
+    def __init__(self, alg: Algorithm, layers, edge_dim: int = 0, beta: bool = False):
+        self.alg = alg
+        self.layers = [tuple(int(x) for x in l) for l in layers]
+        if any(len(l) != 3 for l in self.layers):
+            raise ValueError("layers are (input_features, features_per_head, num_heads) triples")
+        if isinstance(edge_dim, bool) or not isinstance(edge_dim, numbers.Integral) or edge_dim < 0:
+            raise ValueError(f"edge_dim = {edge_dim!r} must be a non-negative integer")
+        self.edge_dim, self.beta = int(edge_dim), bool(beta)
+        flat = (C.c_int * (3 * len(self.layers)))(*[x for l in self.layers for x in l])
+        self.h = C.c_void_p()
+        check(lib().hnhd_gt_create(alg.h, len(self.layers), flat, self.edge_dim, int(self.beta), C.byref(self.h)),
+              "gt_create")
+
+    def param_names(self):
+        names = [n for p in self.PROJECTIONS for n in (p, p + "_bias")]
+        return names + (["edge"] if self.edge_dim else []) + (["beta"] if self.beta else [])
+
+    def param_shape(self, layer: int, name: str):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_gt_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "gt_param_shape")
+        return (r.value,) if name in self.VECTORS else (r.value, c.value)
+
+    def set_param(self, layer: int, name: str, value):
+        """Make the activations stale: the next backward pass needs a forward pass first."""
+        shape = self.param_shape(layer, name)
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        if v.shape != shape:
+            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
+        check(lib().hnhd_gt_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "gt_set_param")
+
+    def param(self, layer: int, name: str):
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        check(lib().hnhd_gt_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "gt_get_param")
+        return out
+
+    def param_grad(self, layer: int, name: str):
+        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        check(lib().hnhd_gt_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "gt_get_param_grad")
+        return out
+
+    def buffer_shape(self, i: int):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_gt_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "gt_buffer_shape")
+        return r.value, c.value
+
+    def set_input(self, x):
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.shape != self.buffer_shape(0):
+            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
+        check(lib().hnhd_gt_set_input(self.h, x.ctypes.data), "gt_set_input")
+
+    def set_edge_attributes(self, attr_A, attr_B):
+        """The edge attributes of this rank's entries: attr_A (len(like_S_values()) x edge_dim) in the order of
+        alg.entry_coordinates("A"), attr_B (len(like_ST_values()) x edge_dim) in that of entry_coordinates("B"), both
+        holding the same attribute for every stored (u, v)."""
+        if not self.edge_dim:
+            raise ValueError("the model has no edge features (edge_dim = 0)")
+        a, b = (np.ascontiguousarray(x, dtype=np.float64) for x in (attr_A, attr_B))
+        for name, x in (("attr_A", a), ("attr_B", b)):
+            if x.ndim != 2 or x.shape[1] != self.edge_dim:
+                raise ValueError(f"{name} must be n x {self.edge_dim}, got {x.shape}")
+        check(lib().hnhd_gt_set_edge_attributes(self.h, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0]),
+              "gt_set_edge_attributes")
+
+    def buffer(self, i: int):
+        out = np.empty(self.buffer_shape(i), dtype=np.float64)
+        check(lib().hnhd_gt_get_buffer(self.h, int(i), out.ctypes.data), "gt_get_buffer")
+        return out
+
+    def forward(self, dropout: float = 0.0, seed: int = 0):
+        """Collective.  dropout in [0, 1) is the attention dropout of every layer; layer l draws its masks at seed +
+        the heads of the layers before it, so no two (layer, head) pairs share one.  Every rank passes the same
+        values."""
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        check(lib().hnhd_gt_forward(self.h, p, sd), "gt_forward")
+
+    def backward(self, grad_out):
+        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the last
+        set_param / set_input / set_edge_attributes and regenerates its dropout masks; the gradients are then read
+        with param_grad / input_grad."""
+        g = np.ascontiguousarray(grad_out, dtype=np.float64)
+        last = len(self.layers)
+        if g.shape != self.buffer_shape(last):
+            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
+        check(lib().hnhd_gt_backward(self.h, g.ctypes.data), "gt_backward")
+
+    def input_grad(self):
+        """dL/d(network input), this rank's rows."""
+        out = np.empty(self.buffer_shape(0), dtype=np.float64)
+        check(lib().hnhd_gt_get_input_grad(self.h, out.ctypes.data), "gt_get_input_grad")
+        return out
+
+    def __del__(self):
+        try:
+            lib().hnhd_gt_destroy(self.h)
+        except Exception:
+            pass
+
+
 def als_run(alg: Algorithm, Agt, Bgt, A0, B0, steps: int = 1, cg_iters: int = 10):
     """Distributed_ALS on caller inputs (this rank's local shards, numpy float64): ground truth from (Agt, Bgt),
     embeddings (A0, B0), `steps` alternating cg_optimizer rounds.  Returns ((residual before, after), A, B)."""

@@ -72,6 +72,7 @@
 
 #include "hnh/15D_dense_shift.hpp"
 #include "hnh/distributed_sparse.h"
+#include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
 
 class GATLayer {
@@ -427,14 +428,4 @@ private:
         hnh::abi_check(hnh_hadamard_f64(v.data(), v.data(), s.data(), v.size(), hnh::Runtime::get().compute_stream()), "hadamard");
     }
 
-    static void allreduce_world(DenseMatrix &m) { allreduce_world(m.data(), m.size()); }
-    static void allreduce_world(VectorXd &v) { allreduce_world(v.data(), v.size()); }
-    static void allreduce_world(double *p, int64_t n) {
-        std::shared_ptr<hnh::Comm> world = hnh::Comm::world();
-        if (world->size() == 1) return;
-        hnh::Runtime &rt = hnh::Runtime::get();
-        rt.chain(rt.compute_stream(), rt.comm_stream());
-        world->allreduce_sum_f64(p, (size_t)n, rt.comm_stream());
-        rt.chain(rt.comm_stream(), rt.compute_stream());
-    }
 };

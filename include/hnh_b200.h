@@ -394,6 +394,30 @@ int hnh_sparse_attention_grad_kv_edge_f64(const int64_t *rowStart, const int64_t
                                           int64_t v0, const double *bias, double *dbias, const double *E, int64_t lde,
                                           void *stream);
 
+/* ---- graph transformer (GraphTransformer, include/hnh/graph_transformer.hpp; csrc/graph_transformer.cu) --------
+ * Row-major contiguous n x r matrices; w_beta (nullable: no gate) holds 3r doubles [w1 | w2 | w3].  Rows take
+ * 16-byte pair loads when r is even and every matrix and vector is 16-byte aligned, scalars otherwise.  Fixed
+ * summation orders: repeated calls give bit-identical results.  Empty input is a no-op.
+ *
+ * X[i, :] += b for every row i (the projection biases; b holds r doubles) */
+int hnh_row_bias_add_f64(double *X, const double *b, int64_t n, int64_t r, void *stream);
+/* The gate forward: with beta_i = sigmoid(<w1, M_i> + <w2, R_i> + <w3, M_i - R_i>),
+ *     Y_i = beta_i R_i + (1 - beta_i) M_i    (Y = M + R when w_beta is null),
+ * then Y = max(Y, 0) when relu != 0.  Y may be neither M nor R. */
+int hnh_gt_gate_f64(double *Y, const double *M, const double *R, const double *w_beta, int64_t n, int64_t r, int relu,
+                    void *stream);
+/* The gate backward, given G = dL/dY (after the ReLU when relu != 0; Y is then the forward's output and dY = G
+ * where Y > 0, else 0): with ds_i = <dY_i, R_i - M_i> beta_i (1 - beta_i),
+ *     dM_i = (1 - beta_i) dY_i + ds_i (w1 + w3),  dR_i = beta_i dY_i + ds_i (w2 - w3),
+ *     dw_beta = sum_i ds_i [M_i, R_i, M_i - R_i]    (3r doubles, overwritten; 0 for n = 0),
+ * or, with a null w_beta, dM = dY and dR (nullable) = dY, and dw_beta must be null.  dw_beta is reduced in two
+ * stages, over fixed row chunks (depending on n only) and then over the chunks in order, in a workspace of
+ * hnh_gt_gate_backward_workspace_bytes(n, r) bytes (needed with the gate only).  Outputs may not alias inputs. */
+int64_t hnh_gt_gate_backward_workspace_bytes(int64_t n, int64_t r);
+int hnh_gt_gate_backward_f64(double *dM, double *dR, double *dw_beta, const double *G, const double *Y, const double *M,
+                             const double *R, const double *w_beta, int64_t n, int64_t r, int relu, void *workspace,
+                             size_t workspace_bytes, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

@@ -298,6 +298,44 @@ int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const dou
 int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2);
 void hnhd_gat_destroy(hnhd_gat_t *g);
 
+/* ---- graph transformer (include/hnh/graph_transformer.hpp): TransformerConv layers on fused sparse attention ---
+ * layers3: n_layers triples (input_features, features_per_head, num_heads); every layer concatenates its heads, so
+ * layer i + 1 takes features_per_head * num_heads of layer i.  edge_dim > 0 adds edge features (attributes of S's
+ * entries projected by each layer's "edge" weight onto the keys and values), beta != 0 the gated skip connection.
+ * The object keeps a pointer to `alg`, which must outlive it.  HNH_E_INVALID on every rank, before any launch,
+ * where the layout has no fused sparse attention (as hnhd_alg_edge_softmax), and for bad layer sizes. */
+typedef struct hnhd_gt hnhd_gt_t;
+int hnhd_gt_create(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_gt_t **out);
+/* Parameters by layer and name: "query", "key", "value", "skip" (input_features x r, row-major: the transpose of
+ * PyG's lin_*.weight), "query_bias", "key_bias", "value_bias", "skip_bias" (r x 1), "edge" (edge_dim x r; models
+ * with edge features only), "beta" (3r x 1, the weight of PyG's lin_beta; gated models only).  All zero after
+ * hnhd_gt_create.  set_param makes the activations stale; get_param_grad reads dL/d param after hnhd_gt_backward,
+ * summed over all ranks (identical on every rank). */
+int hnhd_gt_param_shape(hnhd_gt_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
+int hnhd_gt_set_param(hnhd_gt_t *g, int layer, const char *name, const double *host);
+int hnhd_gt_get_param(hnhd_gt_t *g, int layer, const char *name, double *host);
+int hnhd_gt_get_param_grad(hnhd_gt_t *g, int layer, const char *name, double *host);
+/* buffer 0 is the network input, buffer i + 1 the output of layer i (this rank's rows) */
+int hnhd_gt_buffer_shape(hnhd_gt_t *g, int buffer, int64_t *rows, int64_t *cols);
+int hnhd_gt_set_input(hnhd_gt_t *g, const double *host);
+int hnhd_gt_get_buffer(hnhd_gt_t *g, int buffer, double *host); /* synchronises */
+/* Edge attributes of this rank's entries in both value orders: attr_A is n_A x edge_dim in the order of
+ * hnhd_vec_like(.., 0, ..) (hnhd_alg_entry_coordinates mode 0), attr_B n_B x edge_dim in the B order; n_A and n_B
+ * must be this rank's entry counts.  Both hold the same attribute for every stored (u, v).  Makes the activations
+ * stale.  HNH_E_INVALID for a model without edge features or wrong counts. */
+int hnhd_gt_set_edge_attributes(hnhd_gt_t *g, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B);
+/* Forward pass with attention dropout `dropout` in [0, 1): layer l uses the dropout seed seed + the heads of the
+ * layers before it.  Collective, stream-ordered.  HNH_E_INVALID before any launch for a bad dropout or a model with
+ * edge features whose attributes were not set. */
+int hnhd_gt_forward(hnhd_gt_t *g, double dropout, uint64_t seed);
+/* Backward pass: host_output_grad = dL/d(last buffer), this rank's rows; regenerates the forward's dropout masks.
+ * Collective.  HNH_E_INVALID when no forward pass has run since the last set_param / set_input /
+ * set_edge_attributes. */
+int hnhd_gt_backward(hnhd_gt_t *g, const double *host_output_grad);
+/* dL/d buffer 0 (this rank's rows) after hnhd_gt_backward */
+int hnhd_gt_get_input_grad(hnhd_gt_t *g, double *host);
+void hnhd_gt_destroy(hnhd_gt_t *g);
+
 #ifdef __cplusplus
 }
 #endif
