@@ -100,6 +100,10 @@ ABI = {
     "hnh_gt_gate_f64": (C.c_int, [_P, _P, _P, _P, _I64, _I64, C.c_int, _P]),
     "hnh_gt_gate_backward_workspace_bytes": (C.c_int64, [_I64, _I64]),
     "hnh_gt_gate_backward_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, C.c_int, _P, C.c_size_t, _P]),
+    "hnh_row_bias_relu_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P]),
+    "hnh_layer_norm_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, C.c_double, _P]),
+    "hnh_layer_norm_backward_workspace_bytes": (C.c_int64, [_I64, _I64]),
+    "hnh_layer_norm_backward_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, C.c_int, _P, C.c_size_t, _P]),
     "hnh_entry_coords_from_index_f64": (C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
@@ -268,6 +272,7 @@ ABI.update({
     "hnhd_alg_entry_coordinates": (C.c_int, [_P, C.c_int, _P, _P]),
     "hnhd_gat_destroy": (None, [_P]),
     "hnhd_gt_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, _PP]),
+    "hnhd_gt_create_block": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.c_double, _PP]),
     "hnhd_gt_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "hnhd_gt_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
     "hnhd_gt_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),

@@ -44,14 +44,17 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
                          app == "gat_additive" || app == "gat_additive_train" || app == "gat_v2" || app == "gat_v2_train";
     const bool gat_train =
         app == "gat_train" || app == "gat_softmax_train" || app == "gat_additive_train" || app == "gat_v2_train";
-    const bool gt_app = app == "graph_transformer" || app == "graph_transformer_train";
+    const bool gt_block = app == "graph_transformer_block" || app == "graph_transformer_block_train";
+    const bool gt_train = app == "graph_transformer_train" || app == "graph_transformer_block_train";
+    const bool gt_app = app == "graph_transformer" || app == "graph_transformer_train" || gt_block;
     if (gt_app) {
         // GAT's three layer shapes as TransformerConv layers (no edge features, no gate; the parameters stay zero,
-        // as GAT's weights do); graph_transformer_train: forwardPass() then backwardPass(dL/d output = ones) per call
+        // as GAT's weights do); graph_transformer_block*: as transformer blocks with ffn_ratio = 2 (LayerNorm gains
+        // 1); *_train: forwardPass() then backwardPass(dL/d output = ones) per call
         vector<GraphTransformerLayer> layers{GraphTransformerLayer(256, 256, 4), GraphTransformerLayer(1024, 256, 4),
                                              GraphTransformerLayer(1024, 256, 6)};
-        transformer.reset(new GraphTransformer(layers, d_ops.get(), 0, false));
-        if (app == "graph_transformer_train")
+        transformer.reset(new GraphTransformer(layers, d_ops.get(), 0, false, gt_block ? 2 : 0));
+        if (gt_train)
             gat_output_grad = DenseMatrix::Constant(transformer->buffers.back().rows(), transformer->buffers.back().cols(), 1.0);
     } else if (gat_app) {
         // the three layers of the reference's GAT benchmark: (input width, width per head, heads)
@@ -82,7 +85,8 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
     } else if (app != "vanilla") {
         throw hnh::Error(HNH_E_INVALID, "app must be \"vanilla\", \"als\", \"gat\", \"gat_train\", \"gat_softmax\", "
                                         "\"gat_softmax_train\", \"gat_additive\", \"gat_additive_train\", \"gat_v2\", "
-                                        "\"gat_v2_train\", \"graph_transformer\" or \"graph_transformer_train\"");
+                                        "\"gat_v2_train\", \"graph_transformer\", \"graph_transformer_train\", "
+                                        "\"graph_transformer_block\" or \"graph_transformer_block_train\"");
     }
 
     DenseMatrix A = d_ops->like_A_matrix(0.001);
@@ -102,7 +106,7 @@ json benchmark_algorithm_ex(SpmatLocal *spmat, string algorithm_name, string out
             }
         } else if (gt_app) {
             transformer->forwardPass(0.0, 0);
-            if (app == "graph_transformer_train") transformer->backwardPass(gat_output_grad);
+            if (gt_train) transformer->backwardPass(gat_output_grad);
         } else if (gat_app) {
             gnn->forwardPass();
             if (gat_train) gnn->backwardPass(gat_output_grad);

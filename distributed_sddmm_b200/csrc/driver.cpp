@@ -686,6 +686,17 @@ int hnhd_gt_create(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim
         *out = g.release();
     });
 }
+int hnhd_gt_create_block(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, int beta, int ffn_ratio, double norm_eps,
+                         hnhd_gt_t **out) {
+    return guarded([&] {
+        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_create_block: bad argument");
+        vector<GraphTransformerLayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
+        std::unique_ptr<hnhd_gt> g(new hnhd_gt);
+        g->g.reset(new GraphTransformer(layers, a->alg.get(), edge_dim, beta != 0, ffn_ratio, norm_eps));
+        *out = g.release();
+    });
+}
 // The parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
 struct GtParam {
     int64_t offset, rows, cols;
@@ -704,6 +715,13 @@ static GtParam gt_param(hnhd_gt_t *g, int layer, const char *name) {
     }
     if (s == "edge" && m.edge_dim > 0) return {l.edge_offset(), m.edge_dim, r};
     if (s == "beta" && m.beta) return {l.beta_offset(m.edge_dim), 3 * r, 1};
+    if (m.ffn_ratio > 0) {
+        const int64_t h = l.hidden_features(m.ffn_ratio);
+        static const char *const block[6] = {"norm1", "norm1_bias", "ffn1", "ffn2", "norm2", "norm2_bias"};
+        const int64_t rows[6] = {r, r, r + 1, h + 1, r, r}, cols[6] = {1, 1, h, r, 1, 1};
+        for (int j = 0; j < 6; j++)
+            if (s == block[j]) return {l.block_part_offset(m.edge_dim, m.beta, m.ffn_ratio, j), rows[j], cols[j]};
+    }
     throw hnh::Error(HNH_E_INVALID, "graph transformer: no parameter \"" + s + "\" in this model");
 }
 // copy n doubles between host and device on the compute stream and wait for the copy

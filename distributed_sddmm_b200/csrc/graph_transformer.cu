@@ -15,6 +15,20 @@
 // 16-byte aligned, in scalars otherwise, and a row's dot products end in the warp's xor butterfly, which leaves the
 // same bits on every lane.  The dw_beta chunks depend on n only, never on the device, so repeated calls are
 // bit-identical everywhere.  No floating-point atomics.
+//
+// The transformer block (ffn_ratio > 0) adds, on rows of width r (or h for the feed-forward hidden layer):
+//     Z[i, :] = max(A[i, :] + b, 0)                           first FFN layer's bias and ReLU (row_bias_relu_kernel)
+//     Y_i = gamma (x_i - mean_i) rstd_i + beta,  x = X + Res (Res nullable),  rstd_i = 1 / sqrt(var_i + eps)
+//                                                             LayerNorm; (mean, rstd) per row   (layer_norm_kernel)
+//     dX_i = rstd_i (g_i - mean(g_i) - xh_i mean(g_i xh_i)),  g = G gamma,  xh = (x - mean) rstd
+//                                                             one row pass, dX overwritten or added to
+//                                                                                       (layer_norm_backward_kernel)
+//     dgamma = sum_i G_i xh_i,  dbeta = sum_i G_i              the dw_beta scheme: fixed row chunks
+//                                                             (layer_norm_dw_partial_kernel), then gate_dw_final_kernel
+// The LayerNorm kernels hold a row in registers (r <= 1536 forward, r <= 1024 backward), so it is read from HBM once; the
+// variance is taken from the centred values.  Wider rows reread the row from L1 / L2 in every pass.
+#include <cmath>
+
 #include "row_gather.cuh"
 
 namespace {
@@ -26,6 +40,9 @@ using hnh::set_error;
 constexpr int kCtasPerSm = 16;         // grid cap of the row kernels
 constexpr int64_t kMaxChunks = 128;    // dw_beta partial sums: at most this many row chunks ...
 constexpr int64_t kMinChunkRows = 512; // ... of at least this many rows (fewer chunks for small n)
+// register rows of the LayerNorm kernels up to r = 64 * this: the forward keeps one row (x), the backward two (G and
+// xh), and ptxas spills the backward's at 24
+constexpr int kLnWidest = 24, kLnBackwardWidest = 16;
 
 int64_t dw_chunks(int64_t n) { return std::max<int64_t>(1, std::min<int64_t>(kMaxChunks, (n + kMinChunkRows - 1) / kMinChunkRows)); }
 
@@ -209,6 +226,251 @@ gate_dw_final_kernel(double *__restrict__ dw, const double *__restrict__ partial
     }
 }
 
+// ---- the transformer block (GraphTransformer with ffn_ratio > 0) ----------------------------------------------------
+// Z[i, :] = max(A[i, :] + b, 0): the first feed-forward layer's bias and ReLU
+template <bool kPairs>
+__global__ void __launch_bounds__(kBlock)
+row_bias_relu_kernel(double *__restrict__ Z, const double *__restrict__ A, const double *__restrict__ b, int64_t n, int64_t r) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        if (kPairs) {
+            const double2 *a2 = reinterpret_cast<const double2 *>(A + i * r), *b2 = reinterpret_cast<const double2 *>(b);
+            double2 *z2 = reinterpret_cast<double2 *>(Z + i * r);
+#pragma unroll 2
+            for (int64_t k = lane; k < r / 2; k += 32) {
+                const double2 v = __ldcs(a2 + k), c = __ldg(b2 + k);
+                z2[k] = make_double2(fmax(v.x + c.x, 0.0), fmax(v.y + c.y, 0.0));
+            }
+        } else {
+            const double *a = A + i * r;
+            double *z = Z + i * r;
+            for (int64_t k = lane; k < r; k += 32) z[k] = fmax(__ldcs(a + k) + __ldg(b + k), 0.0);
+        }
+    }
+}
+
+// LayerNorm rows.  kN > 0: a lane keeps 2 kN elements of the row in registers (r <= 64 kN), so the row is read once;
+// with kPairs they are the pairs lane + 32 j (j < kN), else the scalars lane + 32 j (j < 2 kN).  kN = 0: any r, every
+// pass rereads the row (from L1 / L2).  Slot j of a lane holds column ln_col<kPairs>(j, lane).
+template <bool kPairs>
+__device__ __forceinline__ int64_t ln_col(int j, int lane) {
+    return kPairs ? 2 * (int64_t)(lane + 32 * (j >> 1)) + (j & 1) : (int64_t)lane + 32 * j;
+}
+
+// v = p[row] (+ q[row] when q is not null), zero past the row end
+template <bool kPairs, int kN>
+__device__ __forceinline__ void ln_load(double (&v)[2 * kN], const double *p, const double *q, int64_t r, int lane) {
+    if (kPairs) {
+        const double2 *p2 = reinterpret_cast<const double2 *>(p), *q2 = reinterpret_cast<const double2 *>(q);
+#pragma unroll
+        for (int j = 0; j < kN; j++) {
+            const int64_t k = lane + 32 * j;
+            double2 a = make_double2(0.0, 0.0);
+            if (k < r / 2) {
+                a = __ldcs(p2 + k);
+                if (q) {
+                    const double2 c = __ldcs(q2 + k);
+                    a = make_double2(a.x + c.x, a.y + c.y);
+                }
+            }
+            v[2 * j] = a.x;
+            v[2 * j + 1] = a.y;
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < 2 * kN; j++) {
+            const int64_t k = lane + 32 * j;
+            v[j] = k < r ? (q ? __ldcs(p + k) + __ldcs(q + k) : __ldcs(p + k)) : 0.0;
+        }
+    }
+}
+
+// Y = gamma * (x - mean) * rstd + beta with x = X + Res (Res nullable), mean and rstd = 1 / sqrt(var + eps) of each
+// row (biased variance, from the centred values), written to stats[2i], stats[2i + 1]
+template <bool kPairs, int kN>
+__global__ void __launch_bounds__(kBlock, 1)
+layer_norm_kernel(double *__restrict__ Y, double *__restrict__ stats, const double *__restrict__ X, const double *__restrict__ Res,
+                  const double *__restrict__ gamma, const double *__restrict__ beta, int64_t n, int64_t r, double eps) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const double inv_r = 1.0 / (double)r;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const double *x = X + i * r, *res = Res ? Res + i * r : nullptr;
+        double *y = Y + i * r;
+        double mean, rstd;
+        if constexpr (kN > 0) {
+            double v[2 * kN];
+            ln_load<kPairs, kN>(v, x, res, r, lane);
+            double s = 0.0;
+#pragma unroll
+            for (int j = 0; j < 2 * kN; j++) s += v[j];
+            mean = group_allreduce<32>(s, 0xffffffffu) * inv_r;
+            double q = 0.0;
+#pragma unroll
+            for (int j = 0; j < 2 * kN; j++) {
+                const double c = v[j] - mean;
+                if (ln_col<kPairs>(j, lane) < r) q = fma(c, c, q);
+            }
+            rstd = 1.0 / sqrt(group_allreduce<32>(q, 0xffffffffu) * inv_r + eps);
+            if (kPairs) {
+                const double2 *g2 = reinterpret_cast<const double2 *>(gamma), *b2 = reinterpret_cast<const double2 *>(beta);
+                double2 *y2 = reinterpret_cast<double2 *>(y);
+#pragma unroll
+                for (int j = 0; j < kN; j++) {
+                    const int64_t k = lane + 32 * j;
+                    if (k < r / 2) {
+                        const double2 g = __ldg(g2 + k), b = __ldg(b2 + k);
+                        y2[k] = make_double2(fma((v[2 * j] - mean) * rstd, g.x, b.x), fma((v[2 * j + 1] - mean) * rstd, g.y, b.y));
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 2 * kN; j++) {
+                    const int64_t k = lane + 32 * j;
+                    if (k < r) y[k] = fma((v[j] - mean) * rstd, __ldg(gamma + k), __ldg(beta + k));
+                }
+            }
+        } else {
+            auto at = [&](int64_t k) { return res ? x[k] + res[k] : x[k]; };
+            double s = 0.0;
+            for (int64_t k = lane; k < r; k += 32) s += at(k);
+            mean = group_allreduce<32>(s, 0xffffffffu) * inv_r;
+            double q = 0.0;
+            for (int64_t k = lane; k < r; k += 32) {
+                const double c = at(k) - mean;
+                q = fma(c, c, q);
+            }
+            rstd = 1.0 / sqrt(group_allreduce<32>(q, 0xffffffffu) * inv_r + eps);
+            for (int64_t k = lane; k < r; k += 32) y[k] = fma((at(k) - mean) * rstd, __ldg(gamma + k), __ldg(beta + k));
+        }
+        if (lane == 0) {
+            stats[2 * i] = mean;
+            stats[2 * i + 1] = rstd;
+        }
+    }
+}
+
+// dX = rstd (g - mean(g) - xh mean(g xh)) with g = G gamma and xh = (X + Res - mean) rstd from stats; added to dX
+// when accumulate.  kN as in layer_norm_kernel, for G and xh both.
+template <bool kPairs, int kN>
+__global__ void __launch_bounds__(kBlock, 1)
+layer_norm_backward_kernel(double *__restrict__ dX, const double *__restrict__ G, const double *__restrict__ X,
+                           const double *__restrict__ Res, const double *__restrict__ stats, const double *__restrict__ gamma,
+                           int64_t n, int64_t r, int accumulate) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const double inv_r = 1.0 / (double)r;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const double *x = X + i * r, *res = Res ? Res + i * r : nullptr, *gr = G + i * r;
+        double *dx = dX + i * r;
+        const double mean = __ldg(stats + 2 * i), rstd = __ldg(stats + 2 * i + 1);
+        auto out = [&](int64_t k, double v) { return accumulate ? dx[k] + v : v; };
+        if constexpr (kN > 0) {
+            constexpr int N = kN;
+            double g[2 * N], xh[2 * N];
+            ln_load<kPairs, N>(g, gr, nullptr, r, lane);
+            ln_load<kPairs, N>(xh, x, res, r, lane);
+            double s1 = 0.0, s2 = 0.0;
+            if (kPairs) {
+                const double2 *g2 = reinterpret_cast<const double2 *>(gamma);
+#pragma unroll
+                for (int j = 0; j < N; j++) {
+                    const int64_t k = lane + 32 * j;
+                    const double2 w = k < r / 2 ? __ldg(g2 + k) : make_double2(0.0, 0.0);
+                    g[2 * j] *= w.x;
+                    g[2 * j + 1] *= w.y;
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 2 * N; j++) {
+                    const int64_t k = lane + 32 * j;
+                    g[j] *= k < r ? __ldg(gamma + k) : 0.0;
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < 2 * N; j++) {
+                xh[j] = (xh[j] - mean) * rstd;
+                s1 += g[j];
+                s2 = fma(g[j], xh[j], s2);
+            }
+            const double m1 = group_allreduce<32>(s1, 0xffffffffu) * inv_r, m2 = group_allreduce<32>(s2, 0xffffffffu) * inv_r;
+            if (kPairs) {
+                double2 *d2 = reinterpret_cast<double2 *>(dx);
+#pragma unroll
+                for (int j = 0; j < N; j++) {
+                    const int64_t k = lane + 32 * j;
+                    if (k < r / 2) {
+                        double2 v = make_double2(rstd * (g[2 * j] - m1 - xh[2 * j] * m2), rstd * (g[2 * j + 1] - m1 - xh[2 * j + 1] * m2));
+                        if (accumulate) {
+                            const double2 o = d2[k];
+                            v = make_double2(o.x + v.x, o.y + v.y);
+                        }
+                        d2[k] = v;
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 2 * N; j++) {
+                    const int64_t k = lane + 32 * j;
+                    if (k < r) dx[k] = out(k, rstd * (g[j] - m1 - xh[j] * m2));
+                }
+            }
+        } else {
+            auto xhat = [&](int64_t k) { return ((res ? x[k] + res[k] : x[k]) - mean) * rstd; };
+            double s1 = 0.0, s2 = 0.0;
+            for (int64_t k = lane; k < r; k += 32) {
+                const double gk = gr[k] * __ldg(gamma + k);
+                s1 += gk;
+                s2 = fma(gk, xhat(k), s2);
+            }
+            const double m1 = group_allreduce<32>(s1, 0xffffffffu) * inv_r, m2 = group_allreduce<32>(s2, 0xffffffffu) * inv_r;
+            for (int64_t k = lane; k < r; k += 32) dx[k] = out(k, rstd * (gr[k] * __ldg(gamma + k) - m1 - xhat(k) * m2));
+        }
+    }
+}
+
+// partial[c, k] = sum over the rows of chunk c (in row order) of G_ik xh_ik, partial[chunks + c, k] = of G_ik; one
+// thread per column, blockIdx.y the chunk.  The chunks are then summed in order by gate_dw_final_kernel.
+__global__ void __launch_bounds__(kBlock)
+layer_norm_dw_partial_kernel(double *__restrict__ partial, const double *__restrict__ G, const double *__restrict__ X,
+                             const double *__restrict__ Res, const double *__restrict__ stats, int64_t n, int64_t r,
+                             int64_t chunk_rows) {
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= r) return;
+    const int64_t c = blockIdx.y, i0 = c * chunk_rows, i1 = n < i0 + chunk_rows ? n : i0 + chunk_rows;
+    double a1 = 0.0, a2 = 0.0;
+    for (int64_t i = i0; i < i1; i++) {
+        const double x = Res ? ld_stream_f64(X + i * r + k) + ld_stream_f64(Res + i * r + k) : ld_stream_f64(X + i * r + k);
+        const double g = ld_stream_f64(G + i * r + k);
+        a1 = fma(g, (x - __ldg(stats + 2 * i)) * __ldg(stats + 2 * i + 1), a1);
+        a2 += g;
+    }
+    partial[c * r + k] = a1;
+    partial[((int64_t)gridDim.y + c) * r + k] = a2;
+}
+
+// the register-row instantiation for width r (kN = 0 past the widest)
+template <int kWidest, typename K>
+K pick_ln(int64_t r, K k1, K k2, K k4, K k8, K k12, K k16, K k24, K k0) {
+    const int64_t per = (r + 63) / 64;
+    K k = per <= 1 ? k1 : per <= 2 ? k2 : per <= 4 ? k4 : per <= 8 ? k8 : per <= 12 ? k12 : per <= 16 ? k16 : per <= 24 ? k24 : k0;
+    return per <= kWidest ? k : k0;
+}
+template <bool kPairs>
+auto layer_norm_for(int64_t r) {
+    return pick_ln<kLnWidest>(r, layer_norm_kernel<kPairs, 1>, layer_norm_kernel<kPairs, 2>, layer_norm_kernel<kPairs, 4>,
+                               layer_norm_kernel<kPairs, 8>, layer_norm_kernel<kPairs, 12>, layer_norm_kernel<kPairs, 16>,
+                               layer_norm_kernel<kPairs, 24>, layer_norm_kernel<kPairs, 0>);
+}
+template <bool kPairs>
+auto layer_norm_backward_for(int64_t r) {
+    return pick_ln<kLnBackwardWidest>(
+        r, layer_norm_backward_kernel<kPairs, 1>, layer_norm_backward_kernel<kPairs, 2>, layer_norm_backward_kernel<kPairs, 4>,
+        layer_norm_backward_kernel<kPairs, 8>, layer_norm_backward_kernel<kPairs, 12>, layer_norm_backward_kernel<kPairs, 16>,
+        layer_norm_backward_kernel<kPairs, 0>, layer_norm_backward_kernel<kPairs, 0>);  // past kLnBackwardWidest: kN = 0
+}
+
 template <bool kPairs, bool kBeta>
 auto pick_gate(bool relu) {
     return relu ? gate_kernel<kPairs, kBeta, true> : gate_kernel<kPairs, kBeta, false>;
@@ -290,6 +552,76 @@ int hnh_gt_gate_backward_f64(double *dM, double *dR, double *dw_beta, const doub
     if (rc) return rc;
     rc = grid_for(gate_dw_final_kernel, 3 * r, kBlock, &grid, kCtasPerSm);
     return rc ? rc : launch(gate_dw_final_kernel, grid, kBlock, st, "gate_dw_final_kernel", dw_beta, (const double *)partial, chunks, 3 * r);
+}
+
+int hnh_row_bias_relu_f64(double *Z, const double *A, const double *b, int64_t n, int64_t r, void *stream) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_row_bias_relu_f64: negative size");
+    if (n == 0 || r == 0) return HNH_OK;
+    if (!Z || !A || !b) return set_error(HNH_E_INVALID, "hnh_row_bias_relu_f64: null pointer");
+    if (Z == A || Z == b) return set_error(HNH_E_INVALID, "hnh_row_bias_relu_f64: Z may not be A or b");
+    auto k = r % 2 == 0 && aligned16(Z) && aligned16(A) && aligned16(b) ? row_bias_relu_kernel<true> : row_bias_relu_kernel<false>;
+    int grid;
+    int rc = grid_for(k, n, kBlock / 32, &grid, kCtasPerSm);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "row_bias_relu_kernel", Z, A, b, n, r);
+}
+
+int hnh_layer_norm_f64(double *Y, double *stats, const double *X, const double *Res, const double *gamma, const double *beta,
+                       int64_t n, int64_t r, double eps, void *stream) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_layer_norm_f64: negative size");
+    if (!(eps > 0.0) || !std::isfinite(eps)) return set_error(HNH_E_INVALID, "hnh_layer_norm_f64: eps must be finite and > 0");
+    if (n == 0 || r == 0) return HNH_OK;
+    if (!Y || !stats || !X || !gamma || !beta) return set_error(HNH_E_INVALID, "hnh_layer_norm_f64: null pointer");
+    for (const double *o : {(const double *)Y, (const double *)stats})
+        for (const double *in : {X, Res, gamma, beta})
+            if (o == in) return set_error(HNH_E_INVALID, "hnh_layer_norm_f64: an output may not be an input");
+    if (Y == stats) return set_error(HNH_E_INVALID, "hnh_layer_norm_f64: Y and stats are one buffer");
+    const bool pairs = r % 2 == 0 && aligned16(Y) && aligned16(X) && (!Res || aligned16(Res)) && aligned16(gamma) && aligned16(beta);
+    auto k = pairs ? layer_norm_for<true>(r) : layer_norm_for<false>(r);
+    int grid;
+    int rc = grid_for(k, n, kBlock / 32, &grid);
+    return rc ? rc : launch(k, grid, kBlock, (cudaStream_t)stream, "layer_norm_kernel", Y, stats, X, Res, gamma, beta, n, r, eps);
+}
+
+int64_t hnh_layer_norm_backward_workspace_bytes(int64_t n, int64_t r) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_workspace_bytes: negative size");
+    return (int64_t)sizeof(double) * dw_chunks(n) * 2 * r;
+}
+
+int hnh_layer_norm_backward_f64(double *dX, double *dgamma, double *dbeta, const double *G, const double *X, const double *Res,
+                                const double *stats, const double *gamma, int64_t n, int64_t r, int accumulate,
+                                void *workspace, size_t workspace_bytes, void *stream) {
+    if (n < 0 || r < 0) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: negative size");
+    if (r == 0) return HNH_OK;
+    if (!dgamma || !dbeta) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: null pointer");
+    if (dgamma == dbeta) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: dgamma and dbeta are one vector");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) {  // no rows: dgamma = dbeta = 0
+        int rc = hnh::check_cuda(cudaMemsetAsync(dgamma, 0, sizeof(double) * (size_t)r, st), "dgamma");
+        return rc ? rc : hnh::check_cuda(cudaMemsetAsync(dbeta, 0, sizeof(double) * (size_t)r, st), "dbeta");
+    }
+    if (!dX || !G || !X || !stats || !gamma) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: null pointer");
+    const double *ins[] = {G, X, Res, stats, gamma};
+    for (const double *o : {(const double *)dX, (const double *)dgamma, (const double *)dbeta})
+        for (const double *in : ins)
+            if (o == in) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: an output may not be an input");
+    if (dX == dgamma || dX == dbeta) return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: dX and dgamma / dbeta are one buffer");
+    const int64_t need = hnh_layer_norm_backward_workspace_bytes(n, r);
+    if (!workspace || (int64_t)workspace_bytes < need)
+        return set_error(HNH_E_INVALID, "hnh_layer_norm_backward_f64: the workspace needs %lld bytes", (long long)need);
+    const bool pairs = r % 2 == 0 && aligned16(dX) && aligned16(G) && aligned16(X) && (!Res || aligned16(Res)) && aligned16(gamma);
+    auto k = pairs ? layer_norm_backward_for<true>(r) : layer_norm_backward_for<false>(r);
+    int grid;
+    int rc = grid_for(k, n, kBlock / 32, &grid);
+    if (!rc) rc = launch(k, grid, kBlock, st, "layer_norm_backward_kernel", dX, G, X, Res, stats, gamma, n, r, accumulate ? 1 : 0);
+    if (rc) return rc;
+    const int64_t chunks = dw_chunks(n), chunk_rows = (n + chunks - 1) / chunks;
+    double *partial = (double *)workspace;
+    rc = launch(layer_norm_dw_partial_kernel, dim3((unsigned)((r + kBlock - 1) / kBlock), (unsigned)chunks), kBlock, st,
+                "layer_norm_dw_partial_kernel", partial, G, X, Res, stats, n, r, chunk_rows);
+    if (!rc) rc = grid_for(gate_dw_final_kernel, r, kBlock, &grid, kCtasPerSm);
+    if (!rc) rc = launch(gate_dw_final_kernel, grid, kBlock, st, "gate_dw_final_kernel", dgamma, (const double *)partial, chunks, r);
+    return rc ? rc : launch(gate_dw_final_kernel, grid, kBlock, st, "gate_dw_final_kernel", dbeta,
+                            (const double *)(partial + chunks * r), chunks, r);
 }
 
 }  // extern "C"

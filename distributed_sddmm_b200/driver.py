@@ -629,32 +629,48 @@ class GraphTransformer:
     with the heads concatenated, forward and backward (include/hnh/graph_transformer.hpp).  layers: [(input_features,
     features_per_head, num_heads), ...]; every layer but the last ends in a ReLU.  edge_dim > 0 adds edge features
     (per-entry attributes, set with set_edge_attributes, projected by each layer's "edge" weight onto the keys and
-    values); beta=True the gated skip connection.  The algorithm object must outlive this one.
+    values); beta=True the gated skip connection.  ffn_ratio = k >= 1 makes every layer a post-norm transformer block,
+    norm2(h + lin2(relu(lin1(h)))) with h = norm1(the TransformerConv output), LayerNorms of epsilon norm_eps and a
+    feed-forward network of hidden width k r, and drops the ReLU between layers.  The algorithm object must outlive this
+    one.
 
     Parameters (zero after construction), by layer and name: "query", "key", "value", "skip" (input_features x r),
     "query_bias", "key_bias", "value_bias", "skip_bias" (r), "edge" (edge_dim x r) and "beta" (3r).  A TransformerConv
     state dict maps onto them as lin_query.weight.T -> "query", lin_query.bias -> "query_bias", ..., lin_edge.weight.T
-    -> "edge", lin_beta.weight[0] -> "beta"."""
+    -> "edge", lin_beta.weight[0] -> "beta".  With blocks: "norm1", "norm1_bias", "norm2", "norm2_bias" (r; the
+    LayerNorm weights start at 1) and "ffn1" ((r + 1) x h: vstack(lin1.weight.T, lin1.bias)), "ffn2" ((h + 1) x r)."""
 
     PROJECTIONS = ("query", "key", "value", "skip")
-    VECTORS = ("query_bias", "key_bias", "value_bias", "skip_bias", "beta")
+    VECTORS = ("query_bias", "key_bias", "value_bias", "skip_bias", "beta", "norm1", "norm1_bias", "norm2", "norm2_bias")
+    BLOCK = ("norm1", "norm1_bias", "ffn1", "ffn2", "norm2", "norm2_bias")
 
-    def __init__(self, alg: Algorithm, layers, edge_dim: int = 0, beta: bool = False):
+    def __init__(self, alg: Algorithm, layers, edge_dim: int = 0, beta: bool = False, ffn_ratio: int = 0,
+                 norm_eps: float = 1e-5):
         self.alg = alg
         self.layers = [tuple(int(x) for x in l) for l in layers]
         if any(len(l) != 3 for l in self.layers):
             raise ValueError("layers are (input_features, features_per_head, num_heads) triples")
         if isinstance(edge_dim, bool) or not isinstance(edge_dim, numbers.Integral) or edge_dim < 0:
             raise ValueError(f"edge_dim = {edge_dim!r} must be a non-negative integer")
+        if isinstance(ffn_ratio, bool) or not isinstance(ffn_ratio, numbers.Integral) or ffn_ratio < 0:
+            raise ValueError(f"ffn_ratio = {ffn_ratio!r} must be a non-negative integer")
+        if isinstance(norm_eps, bool) or not isinstance(norm_eps, numbers.Real) or not (math.isfinite(norm_eps) and norm_eps > 0):
+            raise ValueError(f"norm_eps = {norm_eps!r} must be finite and > 0")
         self.edge_dim, self.beta = int(edge_dim), bool(beta)
+        self.ffn_ratio, self.norm_eps = int(ffn_ratio), float(norm_eps)
         flat = (C.c_int * (3 * len(self.layers)))(*[x for l in self.layers for x in l])
         self.h = C.c_void_p()
-        check(lib().hnhd_gt_create(alg.h, len(self.layers), flat, self.edge_dim, int(self.beta), C.byref(self.h)),
-              "gt_create")
+        if self.ffn_ratio:
+            check(lib().hnhd_gt_create_block(alg.h, len(self.layers), flat, self.edge_dim, int(self.beta), self.ffn_ratio,
+                                             self.norm_eps, C.byref(self.h)), "gt_create_block")
+        else:
+            check(lib().hnhd_gt_create(alg.h, len(self.layers), flat, self.edge_dim, int(self.beta), C.byref(self.h)),
+                  "gt_create")
 
     def param_names(self):
         names = [n for p in self.PROJECTIONS for n in (p, p + "_bias")]
-        return names + (["edge"] if self.edge_dim else []) + (["beta"] if self.beta else [])
+        names += (["edge"] if self.edge_dim else []) + (["beta"] if self.beta else [])
+        return names + (list(self.BLOCK) if getattr(self, "ffn_ratio", 0) else [])
 
     def param_shape(self, layer: int, name: str):
         r, c = C.c_int64(), C.c_int64()

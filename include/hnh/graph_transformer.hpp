@@ -28,6 +28,20 @@
 // All are zero after construction.  Weights are stored input-major (f x r): a PyG TransformerConv state dict maps
 // onto them by transposing lin_*.weight.
 //
+// Transformer blocks (ffn_ratio = k >= 1; 0, the default, is the model above): every layer becomes a post-norm
+// transformer block with hidden width h = k r.  Y is the gate's output without the ReLU, and no ReLU follows a layer:
+//     H1 = LN1(Y),  Z = ReLU(H1 W1 + b1),  F = Z W2 + b2,  X_{l+1} = LN2(H1 + F)
+// with LN(x) = gamma (x - mean(x)) / sqrt(var(x) + norm_eps) + beta per row (biased variance over r), as torch's
+// norm2(h + lin2(relu(lin1(h)))) with h = norm1(conv(x)).  Backward, before the gate's (which then runs with no ReLU):
+//     dU, dgamma2, dbeta2 = LN2 backward of G                  (hnh_layer_norm_backward_f64, on H1 + F)
+//     [dW2; db2] = [Z 1]^T dU,  dA = dU W2^T where Z > 0        (TN GEMM; NT GEMM and hnh_relu_cols_backward_f64)
+//     [dW1; db1] = [H1 1]^T dA,  dH1 = dU + dA W1^T             (TN GEMM; NT GEMM accumulating into dU)
+//     dY, dgamma1, dbeta1 = LN1 backward of dH1
+// The forward keeps (mean, rstd) of both norms per row (4 doubles per row per layer) beside M and L; the backward
+// recomputes Y, H1, Z and F (rewriting the same statistics) and uses them.  The block's parameters follow w_beta, in
+// the order of their gradients: gamma1 (r), beta1 (r), [W1; b1] ((r + 1) x h), [W2; b2] ((h + 1) x r), gamma2 (r),
+// beta2 (r); the gammas are 1 after construction (as torch's), the rest 0.  One all-reduce still covers the layer.
+//
 // Defined where Distributed_Sparse::check_full_rows passes (every rank holds full-width rows and the A and B layouts
 // coincide); elsewhere the constructor throws HNH_E_INVALID on every rank before any launch.
 #pragma once
@@ -56,7 +70,19 @@ public:
     int64_t projection_offset(int j) const { return (int64_t)j * (input_features + 1) * output_features(); }
     int64_t edge_offset() const { return projection_offset(4); }
     int64_t beta_offset(int edge_dim) const { return edge_offset() + (int64_t)edge_dim * output_features(); }
-    int64_t param_count(int edge_dim, bool beta) const { return beta_offset(edge_dim) + (beta ? 3 * output_features() : 0); }
+    int64_t block_offset(int edge_dim, bool beta) const { return beta_offset(edge_dim) + (beta ? 3 * output_features() : 0); }
+    int64_t hidden_features(int ffn_ratio) const { return (int64_t)ffn_ratio * output_features(); }
+    // offset of block part j (0 gamma1, 1 beta1, 2 [W1; b1], 3 [W2; b2], 4 gamma2, 5 beta2) in params / grads
+    int64_t block_part_offset(int edge_dim, bool beta, int ffn_ratio, int j) const {
+        const int64_t r = output_features(), h = hidden_features(ffn_ratio);
+        const int64_t sizes[6] = {r, r, (r + 1) * h, (h + 1) * r, r, r};
+        int64_t off = block_offset(edge_dim, beta);
+        for (int k = 0; k < j; k++) off += sizes[k];
+        return off;
+    }
+    int64_t param_count(int edge_dim, bool beta, int ffn_ratio = 0) const {
+        return ffn_ratio > 0 ? block_part_offset(edge_dim, beta, ffn_ratio, 6) : block_offset(edge_dim, beta);
+    }
 };
 
 class GraphTransformer {
@@ -66,24 +92,32 @@ public:
     vector<DenseMatrix> buffers;  // [0] network input (B-shaped), [i + 1] output of layer i (A-shaped)
     const int edge_dim;
     const bool beta;
+    const int ffn_ratio;    // > 0: transformer blocks with hidden width ffn_ratio * r
+    const double norm_eps;  // their LayerNorms' epsilon
     DenseMatrix edge_attr_A, edge_attr_B;  // num_S_values x edge_dim and num_ST_values x edge_dim
     bool has_edge_attributes = false;
     vector<DenseMatrix> attention, lse;   // M and L of every layer from the last forward pass
+    vector<DenseMatrix> norm_stats;       // with blocks: (mean, rstd) per row of LN1 and LN2 of layer i at [2i], [2i + 1]
     DenseMatrix input_grad;               // dL/d buffers[0] after backwardPass
     // The activations belong to the current parameters, input and edge attributes: forwardPass sets it, whoever
     // changes one of them clears it, and backwardPass refuses to run on stale activations.
     bool activations_current = false;
 
-    GraphTransformer(vector<GraphTransformerLayer> &l_input, Distributed_Sparse *ops, int edge_features, bool gate)
-        : d_ops(ops), layers(l_input), edge_dim(edge_features), beta(gate) {
+    GraphTransformer(vector<GraphTransformerLayer> &l_input, Distributed_Sparse *ops, int edge_features, bool gate,
+                     int ffn = 0, double eps = 1e-5)
+        : d_ops(ops), layers(l_input), edge_dim(edge_features), beta(gate), ffn_ratio(ffn), norm_eps(eps) {
         d_ops->check_full_rows("GraphTransformer");
         if (layers.empty()) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: no layers");
         if (edge_dim < 0) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: edge_dim must not be negative");
+        if (ffn_ratio < 0) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: ffn_ratio must not be negative");
+        if (!(norm_eps > 0.0) || !std::isfinite(norm_eps))
+            throw hnh::Error(HNH_E_INVALID, "GraphTransformer: norm_eps must be finite and > 0");
         for (size_t i = 0; i < layers.size(); i++) {
             const GraphTransformerLayer &l = layers[i];
             if (l.input_features <= 0 || l.features_per_head <= 0 || l.num_heads <= 0)
                 throw hnh::Error(HNH_E_INVALID, "GraphTransformer: layer " + std::to_string(i) + ": sizes must be positive");
-            if ((int64_t)l.features_per_head * l.num_heads > INT32_MAX)
+            if ((int64_t)l.features_per_head * l.num_heads > INT32_MAX ||
+                (int64_t)l.features_per_head * l.num_heads * std::max(ffn_ratio, 1) > INT32_MAX)
                 throw hnh::Error(HNH_E_INVALID, "GraphTransformer: layer " + std::to_string(i) + " is too wide");
             if (i > 0 && l.input_features != layers[i - 1].output_features())
                 throw hnh::Error(HNH_E_INVALID, "GraphTransformer: layer " + std::to_string(i) + " does not take the width layer " +
@@ -96,7 +130,9 @@ public:
         for (GraphTransformerLayer &layer : layers) {
             d_ops->setRValue(layer.output_features());
             buffers.push_back(d_ops->like_A_matrix(0.0));
-            layer.params = VectorXd::Constant(layer.param_count(edge_dim, beta), 0.0);
+            layer.params = VectorXd::Constant(layer.param_count(edge_dim, beta, ffn_ratio), 0.0);
+            if (ffn_ratio > 0)
+                for (int j : {0, 4}) block_vector(layer.params, layer, j).setConstant(1.0);  // the LayerNorm gains
         }
     }
 
@@ -109,6 +145,16 @@ public:
     }
     DenseMatrix edge_weight(VectorXd &v, const GraphTransformerLayer &l) const {
         return DenseMatrix::view(v.data() + l.edge_offset(), edge_dim, l.output_features());
+    }
+    // block part j of a layer (see block_part_offset): the vectors (j = 0, 1, 4, 5) as 1 x r, the FFN layers (j = 2, 3)
+    // as their (input + 1) x output blocks, and those blocks' weights without the bias row
+    DenseMatrix block_vector(VectorXd &v, const GraphTransformerLayer &l, int j) const {
+        return DenseMatrix::view(v.data() + l.block_part_offset(edge_dim, beta, ffn_ratio, j), 1, l.output_features());
+    }
+    DenseMatrix ffn_block(VectorXd &v, const GraphTransformerLayer &l, int j, bool with_bias) const {
+        const int64_t r = l.output_features(), h = l.hidden_features(ffn_ratio);
+        const int64_t in = j == 2 ? r : h, out = j == 2 ? h : r;
+        return DenseMatrix::view(v.data() + l.block_part_offset(edge_dim, beta, ffn_ratio, j), in + (with_bias ? 1 : 0), out);
     }
 
     // Edge attributes of S's entries in both value orders (row i belongs to entry i of like_S_values /
@@ -133,6 +179,7 @@ public:
         uint64_t seed_l = seed;
         attention.resize(layers.size());
         lse.resize(layers.size());
+        if (ffn_ratio > 0) norm_stats.resize(2 * layers.size());
         for (size_t i = 0; i < layers.size(); i++) {
             GraphTransformerLayer &layer = layers[i];
             const DenseMatrix &X = buffers[i];
@@ -146,10 +193,19 @@ public:
                                        edge_dim > 0 ? &E : nullptr);
             }
             DenseMatrix R = project(X, layer, 3);
-            hnh::abi_check(hnh_gt_gate_f64(buffers[i + 1].data(), attention[i].data(), R.data(),
-                                           beta ? layer.params.data() + layer.beta_offset(edge_dim) : nullptr, n, r,
-                                           i + 1 < layers.size() ? 1 : 0, stream()),
-                           "gt_gate");
+            if (ffn_ratio == 0) {
+                hnh::abi_check(hnh_gt_gate_f64(buffers[i + 1].data(), attention[i].data(), R.data(),
+                                               beta ? layer.params.data() + layer.beta_offset(edge_dim) : nullptr, n, r,
+                                               i + 1 < layers.size() ? 1 : 0, stream()),
+                               "gt_gate");
+            } else {
+                DenseMatrix Y = gate(layer, attention[i], R);
+                R = DenseMatrix();
+                DenseMatrix H1, F;
+                blockHidden(i, Y, H1, F);
+                Y = DenseMatrix();
+                layerNorm(buffers[i + 1], norm_stats[2 * i + 1], F, &H1, layer, 4);
+            }
             seed_l += (uint64_t)layer.num_heads;
         }
         dropout_ = dropout;
@@ -206,32 +262,129 @@ private:
         return P;
     }
 
+    // The gate's output without a ReLU: Y = M + R, or beta R + (1 - beta) M
+    DenseMatrix gate(GraphTransformerLayer &layer, const DenseMatrix &M, const DenseMatrix &R) const {
+        DenseMatrix Y(M.rows(), M.cols());
+        hnh::abi_check(hnh_gt_gate_f64(Y.data(), M.data(), R.data(), beta ? layer.params.data() + layer.beta_offset(edge_dim) : nullptr,
+                                       M.rows(), M.cols(), 0, stream()),
+                       "gt_gate");
+        return Y;
+    }
+
+    // out = LN(X + Res) with the gain and bias at block part j (0: LN1, 4: LN2); (mean, rstd) per row into stats
+    void layerNorm(DenseMatrix &out, DenseMatrix &stats, const DenseMatrix &X, const DenseMatrix *Res, GraphTransformerLayer &layer,
+                   int j) const {
+        const int64_t n = X.rows(), r = X.cols();
+        if (out.rows() != n || out.cols() != r) out.resize(n, r);
+        stats.resize(n, 2);
+        hnh::abi_check(hnh_layer_norm_f64(out.data(), stats.data(), X.data(), Res ? Res->data() : nullptr,
+                                          block_vector(layer.params, layer, j).data(), block_vector(layer.params, layer, j + 1).data(),
+                                          n, r, norm_eps, stream()),
+                       "layer_norm");
+    }
+
+    // The block from the gate's output Y up to LN2's input: H1 = LN1(Y) (its statistics into norm_stats[2i]) and
+    // F = ReLU(H1 W1 + b1) W2 + b2.  With Z given, Z = ReLU(H1 W1 + b1) is kept there.
+    void blockHidden(size_t i, const DenseMatrix &Y, DenseMatrix &H1, DenseMatrix &F, DenseMatrix *keep_Z = nullptr) {
+        GraphTransformerLayer &layer = layers[i];
+        layerNorm(H1, norm_stats[2 * i], Y, nullptr, layer, 0);
+        const int64_t n = Y.rows(), r = Y.cols(), h = layer.hidden_features(ffn_ratio);
+        DenseMatrix Z(n, h);
+        {
+            DenseMatrix A = H1 * ffn_block(layer.params, layer, 2, false);
+            hnh::abi_check(hnh_row_bias_relu_f64(Z.data(), A.data(), layer.params.data() + layer.block_part_offset(edge_dim, beta, ffn_ratio, 2) + r * h,
+                                                 n, h, stream()),
+                           "row_bias_relu");
+        }
+        F = Z * ffn_block(layer.params, layer, 3, false);
+        hnh::abi_check(hnh_row_bias_add_f64(F.data(), layer.params.data() + layer.block_part_offset(edge_dim, beta, ffn_ratio, 3) + h * r,
+                                            n, r, stream()),
+                       "row_bias_add");
+        if (keep_Z) *keep_Z = std::move(Z);
+    }
+
+    // [A 1]: the bias gradients are the products with its ones column
+    static DenseMatrix with_ones(const DenseMatrix &A) {
+        const int64_t n = A.rows(), f = A.cols();
+        DenseMatrix Aa = DenseMatrix::Constant(n, f + 1, 1.0);
+        const size_t dsz = sizeof(double);
+        hnh::cuda_check(cudaMemcpy2DAsync(Aa.data(), (f + 1) * dsz, A.data(), f * dsz, f * dsz, (size_t)n, cudaMemcpyDeviceToDevice,
+                                          stream()),
+                        "[A 1]");
+        return Aa;
+    }
+
+    // LN backward of G for block part j (0: LN1 on X, 4: LN2 on X + Res) into dX, its gain and bias gradients into grads
+    void layerNormBackward(DenseMatrix &dX, const DenseMatrix &G, const DenseMatrix &X, const DenseMatrix *Res,
+                           const DenseMatrix &stats, GraphTransformerLayer &layer, int j) const {
+        const int64_t n = X.rows(), r = X.cols();
+        dX.resize(n, r);
+        const int64_t ws_bytes = hnh_layer_norm_backward_workspace_bytes(n, r);
+        if (ws_bytes < 0) hnh::abi_check((int)ws_bytes, "layer_norm_backward");
+        hnh::DeviceBuffer<char> ws((size_t)ws_bytes);
+        hnh::abi_check(hnh_layer_norm_backward_f64(dX.data(), block_vector(layer.grads, layer, j).data(),
+                                                   block_vector(layer.grads, layer, j + 1).data(), G.data(), X.data(),
+                                                   Res ? Res->data() : nullptr, stats.data(), block_vector(layer.params, layer, j).data(),
+                                                   n, r, 0, ws.data(), (size_t)ws_bytes, stream()),
+                       "layer_norm_backward");
+    }
+
+    // The block's backward of layer i from G = dL/d buffers[i + 1] down to dL/dY, given the gate's output Y; writes
+    // the block's part of layers[i].grads
+    DenseMatrix blockBackward(size_t i, const DenseMatrix &G, const DenseMatrix &Y) {
+        GraphTransformerLayer &layer = layers[i];
+        const int64_t n = Y.rows(), h = layer.hidden_features(ffn_ratio);
+        DenseMatrix H1, F, Z, dU;
+        blockHidden(i, Y, H1, F, &Z);
+        layerNormBackward(dU, G, F, &H1, norm_stats[2 * i + 1], layer, 4);
+        F = DenseMatrix();
+        {
+            DenseMatrix Za = with_ones(Z);
+            ffn_block(layer.grads, layer, 3, true).setTransposeTimes(Za, dU);
+        }
+        DenseMatrix dA(n, h);
+        {
+            DenseMatrix dZ;
+            dZ.setTimesTranspose(dU, ffn_block(layer.params, layer, 3, false), false);
+            dA.setMiddleColsReluGrad(dZ, Z, 0);  // Z > 0 exactly where H1 W1 + b1 > 0
+        }
+        Z = DenseMatrix();
+        {
+            DenseMatrix H1a = with_ones(H1);
+            ffn_block(layer.grads, layer, 2, true).setTransposeTimes(H1a, dA);
+        }
+        H1 = DenseMatrix();
+        dU.setTimesTranspose(dA, ffn_block(layer.params, layer, 2, false), true);  // dH1 = dU + dA W1^T
+        dA = DenseMatrix();
+        DenseMatrix dY;
+        layerNormBackward(dY, dU, Y, nullptr, norm_stats[2 * i], layer, 0);
+        return dY;
+    }
+
     // layer i: G = dL/d buffers[i + 1]; writes layers[i].grads and dX = dL/d buffers[i]
     void backwardLayer(int i, const DenseMatrix &G, DenseMatrix &dX, uint64_t seed_l) {
         GraphTransformerLayer &layer = layers[(size_t)i];
         const DenseMatrix &X = buffers[(size_t)i], &out = buffers[(size_t)i + 1];
         const int64_t n = X.rows(), f = X.cols(), r = layer.output_features();
         if (layer.grads.size() != layer.params.size()) layer.grads = VectorXd(layer.params.size());
-        const bool relu = i + 1 < (int)layers.size();
+        const bool relu = ffn_ratio == 0 && i + 1 < (int)layers.size();
 
-        // [X 1]: the bias gradients are the products with its ones column
-        DenseMatrix Xa = DenseMatrix::Constant(n, f + 1, 1.0);
-        const size_t dsz = sizeof(double);
-        hnh::cuda_check(cudaMemcpy2DAsync(Xa.data(), (f + 1) * dsz, X.data(), f * dsz, f * dsz, (size_t)n, cudaMemcpyDeviceToDevice,
-                                          stream()),
-                        "[X 1]");
+        DenseMatrix Xa = with_ones(X);
         auto grad_block = [&](int j) { return DenseMatrix::view(layer.grads.data() + layer.projection_offset(j), f + 1, r); };
 
         // the gate: dM, dR (dR = dM without it) and dw_beta
         DenseMatrix dM(n, r), dR;
         {
             DenseMatrix R = project(X, layer, 3);
+            DenseMatrix dY;  // with blocks: dL/d the gate's output
+            if (ffn_ratio > 0) dY = blockBackward((size_t)i, G, gate(layer, attention[(size_t)i], R));
             if (beta) dR.resize(n, r);
             const int64_t ws_bytes = beta ? hnh_gt_gate_backward_workspace_bytes(n, r) : 0;
             if (ws_bytes < 0) hnh::abi_check((int)ws_bytes, "gt_gate_backward");
             hnh::DeviceBuffer<char> ws((size_t)ws_bytes);
             hnh::abi_check(hnh_gt_gate_backward_f64(dM.data(), beta ? dR.data() : nullptr,
-                                                    beta ? layer.grads.data() + layer.beta_offset(edge_dim) : nullptr, G.data(),
+                                                    beta ? layer.grads.data() + layer.beta_offset(edge_dim) : nullptr,
+                                                    ffn_ratio > 0 ? dY.data() : G.data(),
                                                     relu ? out.data() : nullptr, attention[(size_t)i].data(), R.data(),
                                                     beta ? layer.params.data() + layer.beta_offset(edge_dim) : nullptr, n, r,
                                                     relu ? 1 : 0, ws.data(), (size_t)ws_bytes, stream()),

@@ -417,6 +417,26 @@ int64_t hnh_gt_gate_backward_workspace_bytes(int64_t n, int64_t r);
 int hnh_gt_gate_backward_f64(double *dM, double *dR, double *dw_beta, const double *G, const double *Y, const double *M,
                              const double *R, const double *w_beta, int64_t n, int64_t r, int relu, void *workspace,
                              size_t workspace_bytes, void *stream);
+/* The transformer block (GraphTransformer with ffn_ratio > 0).  Z = max(A + b, 0) row by row (the first feed-forward
+ * layer's bias and ReLU; b holds r doubles).  Z may be neither A nor b. */
+int hnh_row_bias_relu_f64(double *Z, const double *A, const double *b, int64_t n, int64_t r, void *stream);
+/* LayerNorm of every row of x = X + Res (Res nullable: x = X):
+ *     Y_i = gamma (x_i - mean_i) rstd_i + beta,  rstd_i = 1 / sqrt(var_i + eps)   (biased variance over the r columns),
+ * as torch.nn.functional.layer_norm.  stats (2n doubles) receives (mean_i, rstd_i) at [2i, 2i + 1].  The variance is
+ * taken from the centred values.  eps must be finite and > 0; Y and stats may not be inputs.  One warp per row; up to
+ * r = 1536 a row is read once and kept in registers. */
+int hnh_layer_norm_f64(double *Y, double *stats, const double *X, const double *Res, const double *gamma, const double *beta,
+                       int64_t n, int64_t r, double eps, void *stream);
+/* Its backward, given G = dL/dY and the forward's X, Res and stats: with g = G gamma and xh = (x - mean) rstd,
+ *     dX_i = rstd_i (g_i - mean(g_i) - xh_i mean(g_i xh_i))   (written, or added to dX when accumulate != 0),
+ *     dgamma = sum_i G_i xh_i,  dbeta = sum_i G_i            (r doubles each, overwritten; 0 for n = 0).
+ * dX is also the gradient of Res.  dgamma and dbeta are reduced as dw_beta is, over fixed row chunks and then the
+ * chunks in order, in a workspace of hnh_layer_norm_backward_workspace_bytes(n, r) bytes: no atomics, repeated calls
+ * are bit-identical.  Outputs may not alias inputs or each other. */
+int64_t hnh_layer_norm_backward_workspace_bytes(int64_t n, int64_t r);
+int hnh_layer_norm_backward_f64(double *dX, double *dgamma, double *dbeta, const double *G, const double *X, const double *Res,
+                                const double *stats, const double *gamma, int64_t n, int64_t r, int accumulate,
+                                void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of

@@ -306,10 +306,17 @@ void hnhd_gat_destroy(hnhd_gat_t *g);
  * where the layout has no fused sparse attention (as hnhd_alg_edge_softmax), and for bad layer sizes. */
 typedef struct hnhd_gt hnhd_gt_t;
 int hnhd_gt_create(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_gt_t **out);
+/* The same with transformer blocks: ffn_ratio = k >= 1 makes every layer a post-norm block, LN2(H1 + FFN(H1)) with
+ * H1 = LN1(the layer's output without ReLU) and a ReLU FFN of hidden width k r; LayerNorm epsilon norm_eps.  ffn_ratio
+ * = 0 is hnhd_gt_create.  HNH_E_INVALID for ffn_ratio < 0 or a norm_eps that is not finite and > 0. */
+int hnhd_gt_create_block(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, int ffn_ratio,
+                         double norm_eps, hnhd_gt_t **out);
 /* Parameters by layer and name: "query", "key", "value", "skip" (input_features x r, row-major: the transpose of
  * PyG's lin_*.weight), "query_bias", "key_bias", "value_bias", "skip_bias" (r x 1), "edge" (edge_dim x r; models
- * with edge features only), "beta" (3r x 1, the weight of PyG's lin_beta; gated models only).  All zero after
- * hnhd_gt_create.  set_param makes the activations stale; get_param_grad reads dL/d param after hnhd_gt_backward,
+ * with edge features only), "beta" (3r x 1, the weight of PyG's lin_beta; gated models only).  Models with blocks
+ * (ffn_ratio > 0, hidden width h) add "norm1", "norm1_bias" (r x 1; LN1's weight and bias), "ffn1" ((r + 1) x h:
+ * lin1.weight^T with lin1.bias as the last row), "ffn2" ((h + 1) x r), "norm2", "norm2_bias".  All zero after
+ * hnhd_gt_create, except the LayerNorm weights, which are 1.  set_param makes the activations stale; get_param_grad reads dL/d param after hnhd_gt_backward,
  * summed over all ranks (identical on every rank). */
 int hnhd_gt_param_shape(hnhd_gt_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
 int hnhd_gt_set_param(hnhd_gt_t *g, int layer, const char *name, const double *host);
