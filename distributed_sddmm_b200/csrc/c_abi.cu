@@ -198,6 +198,33 @@ static bool tma_default(bool fused, int r, bool overwrite_out) {
     return fused ? (r == 256 && overwrite_out) : true;
 }
 
+// ---- the direct-load fused kernel of a table width ------------------------------------------------------------------
+// fused_ring_kernel's shape at the widths where it runs (DESIGN.md section 3, chosen by a sweep at 2^20 rows x 32
+// entries): UN rows per batch, S ring slots, CTAs per SM in its __launch_bounds__ -- all without spills, and the ring
+// within the 48 KB of static shared memory of a CTA.  Every other width keeps fused_row_kernel (S = 0).
+template <int R> struct FusedRing { static constexpr int UN = 0, S = 0, MINB = 0; };
+template <> struct FusedRing<64> { static constexpr int UN = 2, S = 4, MINB = 3; };
+template <> struct FusedRing<128> { static constexpr int UN = 2, S = 3, MINB = 3; };
+template <> struct FusedRing<256> { static constexpr int UN = 1, S = 3, MINB = 2; };
+
+using FusedKernel = decltype(&fused_row_kernel<4, 2, 2, 2, true, true>);
+template <int R, int G, int VW, int UN>
+static FusedKernel fused_direct_kernel(bool scale, bool bv, bool bo, const char **name) {
+    using F = FusedRing<R>;
+    if constexpr (F::S > 0) {
+        *name = "fused_ring_kernel";
+        return scale ? (bo ? fused_ring_kernel<R, F::UN, F::S, F::MINB, true, true, true>
+                           : fused_ring_kernel<R, F::UN, F::S, F::MINB, true, false, true>)
+             : bv   ? (bo ? fused_ring_kernel<R, F::UN, F::S, F::MINB, true, true> : fused_ring_kernel<R, F::UN, F::S, F::MINB, true, false>)
+                    : (bo ? fused_ring_kernel<R, F::UN, F::S, F::MINB, false, true> : fused_ring_kernel<R, F::UN, F::S, F::MINB, false, false>);
+    } else {
+        *name = "fused_row_kernel";
+        return scale ? (bo ? fused_row_kernel<R, G, VW, UN, true, true, true> : fused_row_kernel<R, G, VW, UN, true, false, true>)
+             : bv   ? (bo ? fused_row_kernel<R, G, VW, UN, true, true> : fused_row_kernel<R, G, VW, UN, true, false>)
+                    : (bo ? fused_row_kernel<R, G, VW, UN, false, true> : fused_row_kernel<R, G, VW, UN, false, false>);
+    }
+}
+
 // the tile-staged (tma_row_kernel) or per-warp (tma_warp_kernel) instantiation for the overwrite flags
 template <int R, bool FUSED>
 auto tma_kernel(bool per_warp, bool bv, bool bo) {
@@ -439,7 +466,7 @@ int hnh_fused_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
         return rc ? rc : launch(fused_generic_kernel, grid, kBlock, st, "fused_generic_kernel", rowStart, col_idx, values, rows, X, Y, Out, r);
     }
     // the scaled epilogue is a first-visit (BETA0_VALUES) form
-    decltype(&fused_row_kernel<4, 2, 2, 2, true, true>) k = nullptr;
+    FusedKernel k = nullptr;
     int64_t per_cta = 0;
     const char *name = "fused_split_kernel";
     if (r <= split_max_r() && r <= 32) {
@@ -453,13 +480,10 @@ int hnh_fused_scaled_f64(const int64_t *rowStart, const int64_t *col_idx, double
         HNH_DISPATCH_SPLIT(r, SP)
 #undef SP
     } else {
-        name = "fused_row_kernel";
-#define S4(R, G, VW, UN)                                                                                                     \
-    {                                                                                                                        \
-        k = scale ? (bo ? fused_row_kernel<R, G, VW, UN, true, true, true> : fused_row_kernel<R, G, VW, UN, true, false, true>)   \
-            : bv  ? (bo ? fused_row_kernel<R, G, VW, UN, true, true> : fused_row_kernel<R, G, VW, UN, true, false>)               \
-                  : (bo ? fused_row_kernel<R, G, VW, UN, false, true> : fused_row_kernel<R, G, VW, UN, false, false>);            \
-        per_cta = kBlock / G;                                                                                                \
+#define S4(R, G, VW, UN)                                                    \
+    {                                                                       \
+        k = fused_direct_kernel<R, G, VW, UN>(scale != nullptr, bv, bo, &name); \
+        per_cta = kBlock / G;                                               \
     }
         HNH_DISPATCH_R(r, S4, )
 #undef S4

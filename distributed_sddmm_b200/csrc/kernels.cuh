@@ -11,7 +11,7 @@
 //   * a chunk of G nonzeros' (col, value) is read coalesced, one per lane, and broadcast
 //     inside the group with shuffles;
 //   * each gathered Y row is read with 128-bit loads (the widest global load on sm_90),
-//     UN rows in flight per lane;
+//     UN rows in flight per lane (K3 at G = 32: through a per-warp cp.async ring, fused_ring_kernel);
 //   * the r-wide dot is reduced with an xor-butterfly of width G;
 //   * results of a chunk are written back coalesced (lane k owns nonzero k).
 // SpMM / fused accumulate the output row in registers in stored CSR order (bit-compatible
@@ -263,6 +263,175 @@ fused_row_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
     }
 }
 
+__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
+// 16 bytes global -> shared, bypassing L1 (SASS LDGSTS); completion is tracked per thread in commit groups
+__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gmem_src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// K3 with the gathered rows staged through a per-warp shared-memory ring (the G = 32 widths; see DESIGN.md section 3).
+// Same contract, lane shape (one warp per CSR row, VW = 2) and arithmetic as fused_row_kernel: per entry the same FMA
+// order over (v, w), the same xor-butterfly, the same accumulator FMAs in stored CSR order, so the results are
+// bit-identical.  What differs is where a gathered row waits: each lane copies its own 16-byte slices of the warp's
+// next batches of UN rows into a ring of S slots with cp.async (one commit group per batch), and reads back only the
+// bytes it wrote itself -- so no barrier or __syncwarp is needed and the LDS.128 reads are bank-conflict-free.  While
+// batch k is reduced, batches k+1 .. k+S-1 are in flight.  The copy side walks the warp's own stream of entries
+// (its rows, row += grid stride) independently of the compute side, so the ring runs across row ends; it keeps the
+// bounds of its next two rows and the next row's first chunk of column indices loaded ahead, so starting a row costs
+// no dependent index round trip.
+template <int R, int UN, int S, int MINB, bool BV, bool BO, bool SC = false>
+__global__ void __launch_bounds__(256, MINB)
+fused_ring_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict__ col_idx,
+                  double *__restrict__ values, int64_t rows, const double *X,
+                  const double *__restrict__ Y, double *Out, const double *__restrict__ scale = nullptr,
+                  double *__restrict__ scaled_out = nullptr) {
+    constexpr int G = 32, VW = 2, NV = R / (G * VW);
+    static_assert(NV * G * VW == R, "R must be a multiple of 64");
+    static_assert(G % UN == 0 && S >= 2, "a batch never straddles a chunk of G entries; the ring has 2+ slots");
+    __shared__ alignas(16) double ring[kBlock / 32][S][UN][R];
+    const int lane = threadIdx.x & 31;
+    double(*const my)[UN][R] = ring[threadIdx.x >> 5];
+    const unsigned gmask = 0xffffffffu;
+    const int64_t ngroups = (int64_t)gridDim.x * (blockDim.x / G);
+    const int64_t first = (int64_t)blockIdx.x * (blockDim.x / G) + threadIdx.x / G;
+
+    // ---- copy side: p_row's entries [p_j, p_e), chunk of G column indices at p_c0 (lane k holds entry p_c0 + k);
+    // the next row's bounds and first chunk (n1_*) and the bounds of the row after it (n2_*) are already loaded
+    int64_t p_row = first - ngroups, p_j = 0, p_e = 0, p_c0 = 0, p_col = 0;
+    int64_t n1_s = 0, n1_e = 0, n1_col = 0, n2_s = 0, n2_e = 0;
+    if (first < rows) {
+        n1_s = ld_stream_i64(rowStart + first);
+        n1_e = ld_stream_i64(rowStart + first + 1);
+        if (lane < n1_e - n1_s) n1_col = ld_stream_i64(col_idx + n1_s + lane);
+    }
+    if (first + ngroups < rows) {
+        n2_s = ld_stream_i64(rowStart + first + ngroups);
+        n2_e = ld_stream_i64(rowStart + first + ngroups + 1);
+    }
+    int p_slot = 0;
+    // one commit group per call: the next batch of up to UN entries of the stream, or nothing once it has ended
+    auto issue_batch = [&]() {
+        while (p_j == p_e && p_row < rows) {  // row done (or empty): step to the next one
+            p_row += ngroups;
+            if (p_row >= rows) break;
+            p_j = p_c0 = n1_s;
+            p_e = n1_e;
+            p_col = n1_col;
+            n1_s = n2_s;
+            n1_e = n2_e;
+            n1_col = 0;
+            if (p_row + ngroups < rows && lane < n1_e - n1_s) n1_col = ld_stream_i64(col_idx + n1_s + lane);
+            if (p_row + 2 * ngroups < rows) {
+                n2_s = ld_stream_i64(rowStart + p_row + 2 * ngroups);
+                n2_e = ld_stream_i64(rowStart + p_row + 2 * ngroups + 1);
+            }
+        }
+        if (p_j < p_e) {
+            if (p_j == p_c0 + G) {  // the row's next chunk of G entries
+                p_c0 = p_j;
+                p_col = lane < p_e - p_j ? ld_stream_i64(col_idx + p_j + lane) : 0;
+            }
+            const int k0 = (int)(p_j - p_c0);
+            const int64_t left = (p_e < p_c0 + G ? p_e : p_c0 + G) - p_j;
+            const int n = left < UN ? (int)left : UN;
+#pragma unroll
+            for (int u = 0; u < UN; u++) {
+                const int64_t c = __shfl_sync(gmask, p_col, k0 + u);
+                if (u < n) {
+#pragma unroll
+                    for (int v = 0; v < NV; v++)
+                        cp_async16(&my[p_slot][u][(v * G + lane) * VW], Y + c * R + (v * G + lane) * VW);
+                }
+            }
+            p_j += n;
+        }
+        cp_async_commit();
+        p_slot = p_slot + 1 == S ? 0 : p_slot + 1;
+    };
+#pragma unroll
+    for (int b = 0; b < S - 1; b++) issue_batch();
+
+    // ---- compute side: fused_row_kernel's row loop, reading each batch from the ring
+    int c_slot = 0;
+    int64_t s = 0, e = 0;
+    if (first < rows) {
+        s = ld_stream_i64(rowStart + first);
+        e = ld_stream_i64(rowStart + first + 1);
+    }
+    for (int64_t row = first; row < rows; row += ngroups) {
+        const int64_t rs = s, re = e;
+        if (row + ngroups < rows) {  // the next row's bounds, used one row later
+            s = ld_stream_i64(rowStart + row + ngroups);
+            e = ld_stream_i64(rowStart + row + ngroups + 1);
+        }
+        if (!BO && rs == re) continue;
+        double x[NV][VW], acc[NV][VW];
+#pragma unroll
+        for (int v = 0; v < NV; v++) {
+            ld_rw<VW>(x[v], X + row * R + (v * G + lane) * VW);
+            if (BO) {
+#pragma unroll
+                for (int w = 0; w < VW; w++) acc[v][w] = 0.0;
+            } else {
+                ld_rw<VW>(acc[v], Out + row * R + (v * G + lane) * VW);
+            }
+        }
+        for (int64_t j = rs; j < re; j += G) {
+            const int cnt = (re - j < G) ? (int)(re - j) : G;
+            double myval = 0.0, mysc = 1.0;
+            if (lane < cnt) {
+                if (!BV) myval = values[j + lane];
+                if (SC) mysc = ld_stream_f64(scale + j + lane);
+            }
+            for (int k0 = 0; k0 < cnt; k0 += UN) {
+                issue_batch();
+                cp_async_wait<S - 1>();  // this lane's slices of batch (row, j, k0) have landed
+                const double(*const yb)[R] = my[c_slot];
+                c_slot = c_slot + 1 == S ? 0 : c_slot + 1;
+#pragma unroll
+                for (int u = 0; u < UN; u++) {
+                    if (k0 + u < cnt) {
+                        double y[NV][VW];
+#pragma unroll
+                        for (int v = 0; v < NV; v++) {
+                            const double2 t = *reinterpret_cast<const double2 *>(&yb[u][(v * G + lane) * VW]);
+                            y[v][0] = t.x;
+                            y[v][1] = t.y;
+                        }
+                        // BV: the old value is 0.0; the addition stays, so that a -0.0 dot is stored as +0.0
+                        const double vold = BV ? 0.0 : __shfl_sync(gmask, myval, k0 + u);
+                        double d = 0.0;
+#pragma unroll
+                        for (int v = 0; v < NV; v++)
+#pragma unroll
+                            for (int w = 0; w < VW; w++) d = fma(x[v][w], y[v][w], d);
+                        d = group_allreduce<G>(d, gmask);
+                        const double vnew = SC ? (vold + d) * __shfl_sync(gmask, mysc, k0 + u) : vold + d;
+                        if (lane == k0 + u) myval = vnew;
+#pragma unroll
+                        for (int v = 0; v < NV; v++)
+#pragma unroll
+                            for (int w = 0; w < VW; w++) acc[v][w] = fma(vnew, y[v][w], acc[v][w]);
+                    }
+                }
+            }
+            if (lane < cnt) {
+                values[j + lane] = myval;
+                if (SC && scaled_out != nullptr) scaled_out[j + lane] = myval;
+            }
+        }
+#pragma unroll
+        for (int v = 0; v < NV; v++) st_rw<VW>(Out + row * R + (v * G + lane) * VW, acc[v]);
+    }
+    cp_async_wait<0>();
+}
+
 // ------------------------------------------------------------------ TMA-staged variants ---
 // The row-side factor tile X[row0 .. row0+TR) of the TR = 8 rows a CTA works on is one contiguous
 // TR*R*8-byte span: a single elected thread fetches it with ONE bulk asynchronous copy
@@ -273,7 +442,6 @@ fused_row_kernel(const int64_t *__restrict__ rowStart, const int64_t *__restrict
 // into registers (random 8R-byte rows consumed once: staging them would add a shared-memory hop
 // and remove no HBM traffic).  Selected with HNH_FLAG_TMA_STAGE; compared with the direct-load
 // kernels.  G and VW equal the direct kernels' (32, 2), so both compute in the same order.
-__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, unsigned count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
