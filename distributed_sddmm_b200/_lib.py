@@ -104,7 +104,12 @@ ABI = {
     "hnh_layer_norm_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, C.c_double, _P]),
     "hnh_layer_norm_backward_workspace_bytes": (C.c_int64, [_I64, _I64]),
     "hnh_layer_norm_backward_f64": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, C.c_int, _P, C.c_size_t, _P]),
-    "hnh_entry_coords_from_index_f64": (C.c_int, [_P, _P, _I64, _I64, _P]),
+    "hnh_cross_entropy_workspace_bytes": (C.c_int64, [_I64]),
+    "hnh_cross_entropy_f64": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _I64, C.c_double, _P, C.c_size_t, _P]),
+    "hnh_adamw_f64": (C.c_int, [_P, _P, _P, _P, _I64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
+                                C.c_double, C.c_double, _P, _P]),
+    "hnh_clip_coef_f64": (C.c_int, [_P, _P, _I64, C.c_double, _P]),
+    "hnh_entry_coords_from_index_f64":(C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -241,6 +246,8 @@ ABI.update({
     "hnhd_gat_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_double, _PP]),
     "hnhd_gat_weight_shape": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "hnhd_gat_set_weight": (C.c_int, [_P, C.c_int, C.c_int, _P]),
+    "hnhd_gat_get_weight": (C.c_int, [_P, C.c_int, C.c_int, _P]),
+    "hnhd_gat_get_attention_vectors": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
     "hnhd_gat_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "hnhd_gat_set_input": (C.c_int, [_P, _P]),
     "hnhd_gat_get_buffer": (C.c_int, [_P, C.c_int, _P]),
@@ -285,6 +292,13 @@ ABI.update({
     "hnhd_gt_backward": (C.c_int, [_P, _P]),
     "hnhd_gt_get_input_grad": (C.c_int, [_P, _P]),
     "hnhd_gt_destroy": (None, [_P]),
+    "hnhd_labels_create": (C.c_int, [_P, _P, _I64, C.c_int, _PP]),
+    "hnhd_labels_destroy": (None, [_P]),
+    "hnhd_adamw_create": (C.c_int, [C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _PP]),
+    "hnhd_adamw_set_lr": (C.c_int, [_P, C.c_double]),
+    "hnhd_adamw_destroy": (None, [_P]),
+    "hnhd_gt_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
+    "hnhd_gat_train_step": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

@@ -14,6 +14,7 @@
 #include "hnh/distributed_sparse.h"
 #include "hnh/gat.hpp"
 #include "hnh/graph_transformer.hpp"
+#include "hnh/training.hpp"
 #include "hnh_b200.h"
 #include "launch.h"
 
@@ -37,6 +38,12 @@ struct hnhd_gat {
 };
 struct hnhd_gt {
     std::unique_ptr<GraphTransformer> g;
+};
+struct hnhd_labels {
+    std::unique_ptr<hnh::NodeLabels> l;
+};
+struct hnhd_adamw {
+    std::unique_ptr<hnh::AdamW> o;
 };
 
 namespace {
@@ -586,6 +593,12 @@ int hnhd_gat_set_weight(hnhd_gat_t *g, int layer, int head, const double *host) 
         g->g->activations_current = false;
     });
 }
+int hnhd_gat_get_weight(hnhd_gat_t *g, int layer, int head, double *host) {
+    return guarded([&] {
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_weight(g, layer, head).copy_to_host(host);
+    });
+}
 int hnhd_gat_buffer_shape(hnhd_gat_t *g, int buffer, int64_t *rows, int64_t *cols) {
     return guarded([&] {
         DenseMatrix &b = gat_buffer(g, buffer);
@@ -659,6 +672,16 @@ int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const dou
         gat_copy(l.a1.data() + off, a1, l.features_per_head, cudaMemcpyHostToDevice);
         gat_copy(l.a2.data() + off, a2, l.features_per_head, cudaMemcpyHostToDevice);
         g->g->activations_current = false;
+    });
+}
+int hnhd_gat_get_attention_vectors(hnhd_gat_t *g, int layer, int head, double *a1, double *a2) {
+    return guarded([&] {
+        if (!a1 || !a2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_weight(g, layer, head);  // validates layer and head
+        GATLayer &l = g->g->layers[(size_t)layer];
+        const int64_t off = (int64_t)head * l.features_per_head;
+        gat_copy(a1, l.a1.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
+        gat_copy(a2, l.a2.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
     });
 }
 int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2) {
@@ -819,5 +842,52 @@ int hnhd_gt_get_input_grad(hnhd_gt_t *g, double *host) {
     });
 }
 void hnhd_gt_destroy(hnhd_gt_t *g) { delete g; }
+
+// ---- training ------------------------------------------------------------------------------------------
+int hnhd_labels_create(hnhd_alg_t *a, const int32_t *host, int64_t n, int num_classes, hnhd_labels_t **out) {
+    return guarded([&] {
+        if (!a || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_labels_create: null argument");
+        std::unique_ptr<hnhd_labels> l(new hnhd_labels);
+        l->l.reset(new hnh::NodeLabels(host, n, a->alg->localArows, num_classes));
+        *out = l.release();
+    });
+}
+void hnhd_labels_destroy(hnhd_labels_t *l) { delete l; }
+
+int hnhd_adamw_create(double lr, double beta1, double beta2, double eps, double weight_decay, double max_grad_norm,
+                      hnhd_adamw_t **out) {
+    return guarded([&] {
+        if (!out) throw hnh::Error(HNH_E_INVALID, "hnhd_adamw_create: null argument");
+        std::unique_ptr<hnhd_adamw> o(new hnhd_adamw);
+        o->o.reset(new hnh::AdamW(lr, beta1, beta2, eps, weight_decay, max_grad_norm));
+        *out = o.release();
+    });
+}
+int hnhd_adamw_set_lr(hnhd_adamw_t *opt, double lr) {
+    return guarded([&] {
+        if (!opt) throw hnh::Error(HNH_E_INVALID, "hnhd_adamw_set_lr: null optimizer");
+        opt->o->set_lr(lr);
+    });
+}
+void hnhd_adamw_destroy(hnhd_adamw_t *opt) { delete opt; }
+
+static void train_out(const hnh::TrainResult &r, double out[4]) {
+    out[0] = r.loss;
+    out[1] = (double)r.correct;
+    out[2] = (double)r.labelled;
+    out[3] = r.grad_norm;
+}
+int hnhd_gt_train_step(hnhd_gt_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double dropout, uint64_t seed, double out[4]) {
+    return guarded([&] {
+        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_train_step: null argument");
+        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o, dropout, seed), out);
+    });
+}
+int hnhd_gat_train_step(hnhd_gat_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]) {
+    return guarded([&] {
+        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_train_step: null argument");
+        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
+    });
+}
 
 }  // extern "C"

@@ -18,6 +18,7 @@ import json
 import math
 import numbers
 import os
+from typing import NamedTuple
 
 import numpy as np
 
@@ -561,6 +562,12 @@ class GAT:
         assert w.shape == self.weight_shape(layer, head), (w.shape, self.weight_shape(layer, head))
         check(lib().hnhd_gat_set_weight(self.h, layer, head, w.ctypes.data), "gat_set_weight")
 
+    def weight(self, layer: int, head: int):
+        """The weight of (layer, head) as the model holds it (e.g. after train steps)."""
+        out = np.empty(self.weight_shape(layer, head), dtype=np.float64)
+        check(lib().hnhd_gat_get_weight(self.h, layer, head, out.ctypes.data), "gat_get_weight")
+        return out
+
     def buffer_shape(self, i: int):
         r, c = C.c_int64(), C.c_int64()
         check(lib().hnhd_gat_buffer_shape(self.h, i, C.byref(r), C.byref(c)), "gat_buffer_shape")
@@ -596,6 +603,14 @@ class GAT:
         check(lib().hnhd_gat_set_attention_vectors(self.h, layer, head, a1.ctypes.data, a2.ctypes.data),
               "gat_set_attention_vectors")
 
+    def attention_vectors(self, layer: int, head: int):
+        """(a1, a2) of (layer, head) as the model holds them (e.g. after train steps)."""
+        fph = self.layers[layer][1]
+        a1, a2 = np.empty(fph), np.empty(fph)
+        check(lib().hnhd_gat_get_attention_vectors(self.h, layer, head, a1.ctypes.data, a2.ctypes.data),
+              "gat_get_attention_vectors")
+        return a1, a2
+
     def attention_grads(self, layer: int, head: int):
         """(dL/d a1, dL/d a2) of (layer, head) after a backward pass, summed over all ranks (zero for the vectors the
         attention kind does not read)."""
@@ -604,6 +619,14 @@ class GAT:
         check(lib().hnhd_gat_get_attention_grads(self.h, layer, head, da1.ctypes.data, da2.ctypes.data),
               "gat_get_attention_grads")
         return da1, da2
+
+    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
+        """One collective training step on the device: forward, the mean cross-entropy of the output buffer against
+        labels over all ranks, backward, clipping and AdamW (see AdamW).  The forward's activations are stale
+        afterwards.  Returns TrainStep(loss, correct, labelled, grad_norm)."""
+        out = (C.c_double * 4)()
+        check(lib().hnhd_gat_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "gat_train_step")
+        return TrainStep._of(out)
 
     def weight_grad(self, layer: int, head: int):
         """dL/d weight (layer, head), summed over all ranks."""
@@ -742,6 +765,15 @@ class GraphTransformer:
             raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
         check(lib().hnhd_gt_backward(self.h, g.ctypes.data), "gt_backward")
 
+    def train_step(self, labels: "NodeLabels", opt: "AdamW", dropout: float = 0.0, seed: int = 0) -> "TrainStep":
+        """One collective training step on the device: forward(dropout, seed), the mean cross-entropy of the output
+        buffer against labels over all ranks, backward, clipping and AdamW (see AdamW).  The forward's activations are
+        stale afterwards.  Returns TrainStep(loss, correct, labelled, grad_norm)."""
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        out = (C.c_double * 4)()
+        check(lib().hnhd_gt_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), p, sd, out), "gt_train_step")
+        return TrainStep._of(out)
+
     def input_grad(self):
         """dL/d(network input), this rank's rows."""
         out = np.empty(self.buffer_shape(0), dtype=np.float64)
@@ -753,6 +785,93 @@ class GraphTransformer:
             lib().hnhd_gt_destroy(self.h)
         except Exception:
             pass
+
+
+class TrainStep(NamedTuple):
+    """What a train step reports: the mean loss over the labelled rows of all ranks, how many of them the model's
+    argmax gets right, how many there are, and the gradient norm before clipping."""
+    loss: float
+    correct: int
+    labelled: int
+    grad_norm: float
+
+    @classmethod
+    def _of(cls, out):
+        return cls(float(out[0]), int(out[1]), int(out[2]), float(out[3]))
+
+
+class NodeLabels:
+    """The node-classification labels of this rank's rows of a model's output buffer, on the device.  labels: an
+    integer array of net.buffer_shape(last)[0] entries, each a class in [0, num_classes) or negative for "ignored"
+    (padding rows and unlabelled nodes must be negative).  Collective: a bad label on one rank is refused on every
+    rank.  The model's algorithm object must outlive this one."""
+
+    def __init__(self, net, labels, num_classes: int):
+        lab = np.asarray(labels)
+        if lab.dtype.kind not in "iu" or lab.ndim != 1:
+            raise ValueError(f"labels must be a 1-D integer array, got {lab.dtype} of shape {lab.shape}")
+        rows = net.buffer_shape(len(net.layers))[0]
+        if len(lab) != rows:
+            raise ValueError(f"{len(lab)} labels for {rows} output rows")
+        if len(lab) and (lab.max() > np.iinfo(np.int32).max or lab.min() < np.iinfo(np.int32).min):
+            raise ValueError("labels must fit in int32")
+        if isinstance(num_classes, bool) or not isinstance(num_classes, numbers.Integral):
+            raise ValueError(f"num_classes = {num_classes!r} must be an integer")
+        self.num_classes = int(num_classes)
+        self._host = np.ascontiguousarray(lab, np.int32)
+        self.h = C.c_void_p()
+        check(lib().hnhd_labels_create(net.alg.h, self._host.ctypes.data, len(self._host), self.num_classes,
+                                       C.byref(self.h)), "labels_create")
+
+    def __del__(self):
+        try:
+            lib().hnhd_labels_destroy(self.h)
+        except Exception:
+            pass
+
+
+class AdamW:
+    """torch.optim.AdamW(lr, betas, eps, weight_decay, amsgrad=False, foreach=False) on the device, with one parameter
+    group and torch's defaults; max_grad_norm (None: off) clips as torch.nn.utils.clip_grad_norm_ before every step.
+    Weight decay applies to every parameter.  An optimizer belongs to the parameters of the first model it steps; the
+    lr property may change between steps (a warm-up or decay schedule)."""
+
+    def __init__(self, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 1e-2,
+                 max_grad_norm=None):
+        b1, b2 = (float(b) for b in betas)
+        mg = 0.0 if max_grad_norm is None else float(max_grad_norm)
+        if max_grad_norm is not None and not mg > 0:
+            raise ValueError(f"max_grad_norm = {max_grad_norm!r} must be > 0 (None: no clipping)")
+        self._lr = float(lr)
+        self.h = C.c_void_p()
+        check(lib().hnhd_adamw_create(self._lr, b1, b2, float(eps), float(weight_decay), mg, C.byref(self.h)), "adamw_create")
+
+    @property
+    def lr(self) -> float:
+        return self._lr
+
+    @lr.setter
+    def lr(self, value: float):
+        check(lib().hnhd_adamw_set_lr(self.h, float(value)), "adamw_set_lr")
+        self._lr = float(value)
+
+    def __del__(self):
+        try:
+            lib().hnhd_adamw_destroy(self.h)
+        except Exception:
+            pass
+
+
+def _labels_arg(labels):
+    if not isinstance(labels, NodeLabels):
+        raise TypeError(f"labels must be a NodeLabels, not {type(labels).__name__}")
+    return labels.h
+
+
+def _adamw_arg(opt):
+    if not isinstance(opt, AdamW):
+        raise TypeError(f"opt must be an AdamW, not {type(opt).__name__}")
+    return opt.h
 
 
 def als_run(alg: Algorithm, Agt, Bgt, A0, B0, steps: int = 1, cg_iters: int = 10):

@@ -75,6 +75,8 @@
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
 
+struct ParamSpan;  // hnh/training.hpp
+
 class GATLayer {
 public:
     int input_features;
@@ -178,6 +180,10 @@ public:
     // Throws HNH_E_INVALID unless the backward pass is defined on this algorithm object (see the top of this
     // file).  Decided from global quantities only, so every rank throws together and no collective is left waiting.
     void check_backward_supported() const { d_ops->check_full_rows("GAT::backwardPass"); }
+
+    // Every (layer, head) weight with its gradient, then a1 and a2 of every layer with theirs; grad is null before the
+    // first backward pass.  Defined in hnh/training.hpp.  Read afresh for every use: set_weight may replace storage.
+    std::vector<ParamSpan> parameters();
 
     // "leaky" (the reference's attention, the default), "softmax", "additive" or "gatv2" (see the top of this file).
     // Changing it makes the activations stale.

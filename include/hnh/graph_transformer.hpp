@@ -53,6 +53,8 @@
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
 
+struct ParamSpan;  // hnh/training.hpp
+
 class GraphTransformerLayer {
 public:
     int input_features;
@@ -171,6 +173,10 @@ public:
         has_edge_attributes = true;
         activations_current = false;
     }
+
+    // Each layer's params with its grads, one span per layer; grad is null before the first backward pass.  Defined in
+    // hnh/training.hpp.
+    std::vector<ParamSpan> parameters();
 
     // Collective.  dropout in [0, 1) and seed go to every layer's attention (seed_l as above); the backward pass
     // regenerates the same masks.

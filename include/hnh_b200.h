@@ -438,6 +438,35 @@ int hnh_layer_norm_backward_f64(double *dX, double *dgamma, double *dbeta, const
                                 const double *stats, const double *gamma, int64_t n, int64_t r, int accumulate,
                                 void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- training (include/hnh/training.hpp; csrc/training.cu) ---------------------------------------------------------
+ * Cross-entropy of n rows of logits (n x C, leading dimension ld >= C) against int32 labels: a row is labelled when
+ * 0 <= labels[i] < C and ignored otherwise.  With lse_i = max_i + log sum_k exp(x_ik - max_i):
+ *     dlogits_ik = (exp(x_ik - lse_i) - [k == labels[i]]) * inv_count   (0 on ignored rows; same ld as logits),
+ *     sums[0] = sum over labelled rows of lse_i - x_i,labels[i],
+ *     sums[1] = the number of labelled rows whose argmax (ties to the lowest index, as torch.argmax) is their label.
+ * inv_count is the caller's 1 / (labelled rows), e.g. over all ranks; sums are not scaled by it.  The label is only
+ * compared with column indices, never used to address memory.  One warp per row; up to C = 1536 the row is read once.
+ * sums are reduced over per-row values in the fixed two-stage order of hnh_layer_norm_backward_f64, in a workspace of
+ * hnh_cross_entropy_workspace_bytes(n) bytes: repeated calls are bit-identical.  dlogits may not be logits; n = 0
+ * writes sums = 0. */
+int64_t hnh_cross_entropy_workspace_bytes(int64_t n);
+int hnh_cross_entropy_f64(double *dlogits, double *sums, const double *logits, const int32_t *labels, int64_t n, int64_t C,
+                          int64_t ld, double inv_count, void *workspace, size_t workspace_bytes, void *stream);
+/* One AdamW step on one tensor of n doubles, in place on param, m and v, as torch.optim.AdamW(foreach=False,
+ * amsgrad=False) with g = grad * (*clip_coef) (clip_coef: a nullable DEVICE scalar, so a clip coefficient computed on
+ * the device needs no host round trip; null = 1):
+ *     param *= 1 - lr weight_decay;  m = lerp(m, g, 1 - beta1);  v = v beta2 + (1 - beta2) g g;
+ *     param -= lr / bias_correction1 * m / (sqrt(v) / sqrt(bias_correction2) + eps),
+ * with bias_correction_k = 1 - beta_k^t from the caller.  grad is not written.  lr, weight_decay >= 0, betas in [0, 1),
+ * eps > 0, bias corrections in (0, 1], all finite; param, m, v, grad distinct. */
+int hnh_adamw_f64(double *param, double *m, double *v, const double *grad, int64_t n, double lr, double beta1, double beta2,
+                  double eps, double weight_decay, double bias_correction1, double bias_correction2, const double *clip_coef,
+                  void *stream);
+/* The coefficient of torch.nn.utils.clip_grad_norm_ from per-tensor squared norms (hnh_squared_norm_f64 of each):
+ * total_coef[0] = sqrt(sum of squared_norms[0 .. count) in order), total_coef[1] = min(1, max_norm / (total + 1e-6)).
+ * max_norm >= 0; +inf gives coef = 1. */
+int hnh_clip_coef_f64(double *total_coef, const double *squared_norms, int64_t count, double max_norm, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

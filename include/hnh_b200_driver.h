@@ -266,6 +266,7 @@ int hnhd_gat_create(hnhd_alg_t *alg, int n_layers, const int *layers3, double le
                     hnhd_gat_t **out);
 int hnhd_gat_weight_shape(hnhd_gat_t *g, int layer, int head, int64_t *rows, int64_t *cols);
 int hnhd_gat_set_weight(hnhd_gat_t *g, int layer, int head, const double *host);
+int hnhd_gat_get_weight(hnhd_gat_t *g, int layer, int head, double *host); /* synchronises (e.g. after train steps) */
 int hnhd_gat_buffer_shape(hnhd_gat_t *g, int buffer, int64_t *rows, int64_t *cols);
 int hnhd_gat_set_input(hnhd_gat_t *g, const double *host);          /* buffer 0 */
 int hnhd_gat_get_buffer(hnhd_gat_t *g, int buffer, double *host);   /* synchronises */
@@ -293,6 +294,7 @@ int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind);
  * doubles each (host pointers; zero after hnhd_gat_create: uniform attention).  Makes the activations stale.
  * "additive" is defined on the layouts where "softmax" is. */
 int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const double *a1, const double *a2);
+int hnhd_gat_get_attention_vectors(hnhd_gat_t *g, int layer, int head, double *a1, double *a2); /* synchronises */
 /* dL/d a1 and dL/d a2 of (layer, head) after hnhd_gat_backward (features_per_head doubles each, summed over all
  * ranks; zero unless the attention is additive).  HNH_E_INVALID before the first backward pass. */
 int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2);
@@ -342,6 +344,33 @@ int hnhd_gt_backward(hnhd_gt_t *g, const double *host_output_grad);
 /* dL/d buffer 0 (this rank's rows) after hnhd_gt_backward */
 int hnhd_gt_get_input_grad(hnhd_gt_t *g, double *host);
 void hnhd_gt_destroy(hnhd_gt_t *g);
+
+/* ---- training (include/hnh/training.hpp): cross-entropy, clipping and AdamW on the device -------------------------
+ * Labels of this rank's rows of the model's output buffer (alg's localArows of them), one int32 per row: a class in
+ * [0, num_classes) or negative for "ignored" (padding rows and unlabelled nodes must be negative).  Collective: a bad
+ * label or count on one rank is refused with HNH_E_INVALID on every rank.  The host array is copied. */
+typedef struct hnhd_labels hnhd_labels_t;
+int hnhd_labels_create(hnhd_alg_t *alg, const int32_t *host_labels, int64_t n, int num_classes, hnhd_labels_t **out);
+void hnhd_labels_destroy(hnhd_labels_t *labels);
+/* torch.optim.AdamW(lr, (beta1, beta2), eps, weight_decay, amsgrad=False, foreach=False) with one parameter group, and
+ * max_grad_norm > 0: torch.nn.utils.clip_grad_norm_(max_grad_norm) before every step (0: no clipping).  HNH_E_INVALID
+ * for lr < 0, a beta outside [0, 1), eps <= 0, weight_decay < 0, max_grad_norm < 0, or any of them NaN or infinite
+ * (max_grad_norm may be +inf).  The moments are allocated on the first step; an optimizer is tied to the parameter
+ * sizes of its first model, and a train step with another is refused.  set_lr changes lr from the next step on. */
+typedef struct hnhd_adamw hnhd_adamw_t;
+int hnhd_adamw_create(double lr, double beta1, double beta2, double eps, double weight_decay, double max_grad_norm,
+                      hnhd_adamw_t **out);
+int hnhd_adamw_set_lr(hnhd_adamw_t *opt, double lr);
+void hnhd_adamw_destroy(hnhd_adamw_t *opt);
+/* One training step: forward (the graph transformer with attention dropout `dropout` and `seed`), the mean
+ * cross-entropy of the output buffer against the labels over all ranks, the backward pass, clipping and AdamW.
+ * out = {loss, correct, labelled, grad_norm}: the loss, the labelled rows whose argmax is their label and the labelled
+ * rows (all ranks), and the gradient norm before clipping.  With no labelled row the loss and the gradient are 0.
+ * Collective; afterwards the activations are stale.  HNH_E_INVALID on every rank before any launch for labels of
+ * another row or class count, an optimizer of other parameter sizes, and layouts without a backward pass. */
+int hnhd_gt_train_step(hnhd_gt_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double dropout, uint64_t seed,
+                       double out[4]);
+int hnhd_gat_train_step(hnhd_gat_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
 
 #ifdef __cplusplus
 }
