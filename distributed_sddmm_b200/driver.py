@@ -247,8 +247,10 @@ class Algorithm:
         check(lib().hnhd_dense_dummy_initialize(self.h, m.h, 0 if which == "A" else 1), "dummyInitialize")
 
     def _op(self, op, A, B, S=None, R=None, aux=0):
-        check(lib().hnhd_alg_op(self.h, OP[op], A.h if A else None, B.h if B else None, S.h if S else None,
-                                R.h if R else None, aux), op)
+        # `is not None`, not truth: a Vec has a length, and a rank whose share of S is empty holds vectors of length 0,
+        # which must still reach the collective op (the other ranks wait for this one in the ring)
+        h = lambda x: x.h if x is not None else None  # noqa: E731
+        check(lib().hnhd_alg_op(self.h, OP[op], h(A), h(B), h(S), h(R), aux), op)
 
     def sddmmA(self, A, B, S, R):
         self._op("sddmmA", A, B, S, R)

@@ -1,0 +1,321 @@
+"""Worker of the skewed-graph tests (tests/test_skewed_graphs_multirank_gpu.py launches it through
+torch.distributed.run; tests/test_skewed_graphs_gpu.py calls run_case in-process at p = 1).  Per case every rank builds
+the pattern of tests/skewed_graph.py, hands its round-robin share of the tuples to SpmatLocal.from_tuples, builds the
+algorithm and runs the case's kind:
+
+  base     the case's script of sddmmA/B, spmmA/B and fusedSpMM A/B on global A and B
+  softmax  edge_softmax and edge_softmax_backward in both value orders, optionally with -inf scores
+  attn     sparse_attention and sparse_attention_backward: plain, with dropout, with a per-head bias that masks, with
+           edge features
+  gat      GAT forward and backward with the case's attention kind
+  train    GAT train steps
+
+Every op runs twice and the worker records whether the repeat gave the same bits.  It writes its rows of the results
+-- or the error the layout must raise -- to <outdir>/<case>_rank<r>.npz.
+
+Transports as in tests/mp_worker.py: "gloo" (ranks sharing one GPU), "nccl" (one GPU per rank)."""
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from tests import gat_additive_oracle as gao  # noqa: E402
+from tests.mp_edge_softmax_worker import score, upstream  # noqa: E402
+from tests.mp_sparse_attention_edge_worker import edge_of  # noqa: E402
+from tests.mp_worker import gather_local, sval  # noqa: E402
+from tests.skewed_graph import DEFAULT_N, landmarks, rank_slice, skewed_tuples  # noqa: E402
+
+
+def sizes(case):
+    return case.get("m") or DEFAULT_N, case.get("n") or DEFAULT_N
+
+
+def base_inputs(M, N, R, seed):
+    """A (M x R) and B (N x R)."""
+    rng = np.random.default_rng(seed + 11)
+    return rng.uniform(-1, 1, (M, R)), rng.uniform(-1, 1, (N, R))
+
+
+def attn_inputs(M, N, r, seed):
+    """Q, dZ (M x r) and K, V (N x r)."""
+    rng = np.random.default_rng(seed + 13)
+    return rng.uniform(-1, 1, (M, r)), rng.uniform(-1, 1, (M, r)), rng.uniform(-1, 1, (N, r)), rng.uniform(-1, 1, (N, r))
+
+
+def masked(rows, cols, M, N):
+    """The entries a masking case scores -inf: every entry of the first wide hub row in the first of 4 column blocks
+    (so one rank's share of that row is masked throughout while the others' is not), and in every fifth row every
+    entry of an even column."""
+    lm = landmarks(M, N)
+    rows, cols = np.asarray(rows), np.asarray(cols)
+    return ((rows == lm["wide_hubs"][0]) & (cols < lm["w"])) | ((rows % 5 == 1) & (cols % 2 == 0))
+
+
+def bias_of(rows, cols, h, M, N):
+    """b(u, v) of head h, a function of the global coordinates: up to +-30, -inf on masked(); head 1 also masks row 0
+    throughout."""
+    rows, cols = np.asarray(rows), np.asarray(cols)
+    b = 30.0 * np.sin(0.37 * rows + 1.3 * cols + 0.5 * h)
+    b[masked(rows, cols, M, N) | ((rows == 0) & (h == 1))] = -np.inf
+    return b
+
+
+def labels_of(N, classes, seed):
+    """Labels on about 30 % of the nodes (40 % of the first three of 4 row blocks): every hub row labelled, the last
+    row block unlabelled."""
+    rng = np.random.default_rng(seed + 17)
+    lm = landmarks(N, N)
+    lab = rng.integers(0, classes, N)
+    lab[rng.random(N) >= 0.4] = -1
+    for u in (*lm["wide_hubs"], lm["last_block_hub"]):
+        lab[u] = u % classes
+    lab[lm["narrow_rows"][0]:] = -1
+    return lab
+
+
+def gat_inputs(N, layers, seed):
+    """(X0, weights[layer][head], a1, a2, G) of a GAT case: weights scaled by 1 / sqrt(fan-in) so that the scores of a
+    2000-entry row stay in exp's range."""
+    rng = np.random.default_rng(seed + 19)
+    X0 = rng.uniform(-1, 1, (N, layers[0][0]))
+    ws = [[rng.uniform(-1, 1, (f, d)) / np.sqrt(f) for _ in range(H)] for f, d, H in layers]
+    a1, a2 = gao.attention_inputs(layers, seed)
+    G = rng.uniform(-1, 1, (N, layers[-1][1] * layers[-1][2]))
+    return X0, ws, a1, a2, G
+
+
+def coords_by_sddmm(alg, A, B, mode):
+    """(row, col) of every entry of this rank's value vector of `mode` on any layout: SDDMMs of a global-index column
+    against a column of ones (the column lives on the ranks whose submatrix starts at column 0)."""
+    d = alg.dims
+    like, sddmm = (alg.like_S_values, alg.sddmmA) if mode == "A" else (alg.like_ST_values, alg.sddmmB)
+    ones, res = like(1.0), like(0.0)
+    out = []
+    for first in ("A", "B"):
+        for m, which, shape in ((A, "A", (d.localArows, d.localAcols)), (B, "B", (d.localBrows, d.localBcols))):
+            x = np.zeros(shape)
+            flat, at = x.reshape(-1), 0
+            for top, left, nr, nc in alg.submatrices(which):
+                blk = np.zeros((nr, nc))
+                if left == 0:
+                    blk[:, 0] = np.arange(top, top + nr) if which == first else 1.0
+                flat[at:at + nr * nc] = blk.reshape(-1)
+                at += nr * nc
+            m.from_host(x)
+        alg.initial_shift(A, B, "sddmm" + mode)
+        sddmm(A, B, ones, res)
+        alg.de_shift(A, B, "sddmm" + mode)
+        out.append(np.rint(res.to_host()).astype(np.int64))
+    return out
+
+
+def run_base(D, alg, case, M, N, out):
+    d = alg.dims
+    shapeA, shapeB = (d.localArows, d.localAcols), (d.localBrows, d.localBcols)
+    subsA, subsB = alg.submatrices("A"), alg.submatrices("B")
+    out.update(aSubmatrices=subsA, bSubmatrices=subsB, shapeA=shapeA, shapeB=shapeB)
+    A, B = alg.like_A_matrix(), alg.like_B_matrix()
+    vals, res = {}, {}
+    for mode, like in (("A", alg.like_S_values), ("B", alg.like_ST_values)):
+        r, c = coords_by_sddmm(alg, A, B, mode)
+        out[f"{mode}_rows"], out[f"{mode}_cols"] = r, c
+        vals[mode], res[mode] = like(0.0), like(0.0)
+        vals[mode].from_host(sval(r, c))
+    GA, GB = base_inputs(M, N, case["R"], case["seed"])
+    hA, hB = gather_local(GA, subsA, shapeA), gather_local(GB, subsB, shapeB)
+    for op in case["script"]:
+        mode = op[-1]
+        got = []
+        for _ in range(2):
+            A.from_host(hA)
+            B.from_host(hB)
+            res[mode].fill(0.0)
+            shift = "spmm" + mode if op.startswith("spmm") else "sddmm" + mode
+            alg.initial_shift(A, B, shift)
+            if op.startswith("sddmm"):
+                (alg.sddmmA if mode == "A" else alg.sddmmB)(A, B, vals[mode], res[mode])
+            elif op.startswith("spmm"):
+                (alg.spmmA if mode == "A" else alg.spmmB)(A, B, vals[mode])
+            else:
+                alg.fusedSpMM(A, B, vals[mode], res[mode], mode)
+            alg.de_shift(A, B, shift)
+            got.append(((A if mode == "A" else B).to_host(), res[mode].to_host()))
+        out[op + "_repeat"] = all(np.array_equal(a, b, equal_nan=True) for a, b in zip(*got))
+        if not op.startswith("sddmm"):
+            out[op + "_dense"] = got[0][0]
+        if not op.startswith("spmm"):
+            out[op + "_values"] = got[0][1]
+
+
+def run_softmax(D, alg, case, M, N, out):
+    for mode in ("A", "B"):
+        r, c = alg.entry_coordinates(mode)
+        like = alg.like_S_values if mode == "A" else alg.like_ST_values
+        x = score(r, c)
+        if case.get("mask"):
+            x[masked(r, c, M, N)] = -np.inf
+        got = []
+        for _ in range(2):
+            v, g = like(0.0), like(0.0)
+            v.from_host(x)
+            alg.edge_softmax(v, mode)
+            a = v.to_host()
+            g.from_host(upstream(r, c))
+            alg.edge_softmax_backward(v, g, mode)
+            got.append((a, g.to_host()))
+        out[f"{mode}_repeat"] = all(np.array_equal(a, b, equal_nan=True) for a, b in zip(*got))
+        out.update({f"{mode}_rows": r, f"{mode}_cols": c, f"{mode}_alpha": got[0][0], f"{mode}_dx": got[0][1]})
+
+
+def run_attn(D, alg, case, M, N, out):
+    heads, d, variant, p = case["heads"], case["d"], case["variant"], case["dropout"]
+    r = heads * d
+    dims = alg.dims
+    Q, K, V, dZ = alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix(), alg.like_A_matrix()
+    Z, dQ, dK, dV = alg.like_A_matrix(), alg.like_A_matrix(), alg.like_B_matrix(), alg.like_B_matrix()
+    L = D.Dense.create(dims.localArows, heads)
+    if case.get("rejected"):  # a layout without sparse attention must refuse before any launch
+        alg.sparse_attention(Q, K, V, Z, L, heads)
+        return
+    Qg, dZg, Kg, Vg = attn_inputs(M, N, r, case["seed"])
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    out.update(topA=topA, nrA=nrA, topB=topB, nrB=nrB)
+    for m, g, top, nr in ((Q, Qg, topA, nrA), (dZ, dZg, topA, nrA), (K, Kg, topB, nrB), (V, Vg, topB, nrB)):
+        m.from_host(gather_local(g, [(top, 0, nr, r)], m.shape))
+    rA, cA = alg.entry_coordinates("A")
+    rB, cB = alg.entry_coordinates("B")
+    out.update(rA=rA, cA=cA, rB=rB, cB=cB)
+    fwd, bwd, extra = dict(dropout=p, seed=case["mask_seed"]), {}, []
+    if variant == "bias":
+        vecs = []
+        for rr, cc in ((rA, cA), (rB, cB)):
+            b = np.concatenate([bias_of(rr, cc, h, M, N) for h in range(heads)])
+            vecs.append(D.Vec.create(len(b)))
+            vecs[-1].from_host(b)
+        dbA, dbB = D.Vec.create(0), D.Vec.create(0)
+        fwd.update(bias=vecs[0])
+        bwd.update(bias_B=vecs[1], dbias=dbA, dbias_B=dbB)
+        extra = [("dbA", dbA), ("dbB", dbB)]
+    elif variant == "edge":
+        edges = []
+        for rr, cc in ((rA, cA), (rB, cB)):
+            e = edge_of(rr, cc, r)
+            edges.append(D.Dense.create(*e.shape))
+            edges[-1].from_host(e)
+        dE = D.Dense.create(1, 1)
+        fwd.update(edge=edges[0])
+        bwd.update(edge_B=edges[1], dedge=dE)
+        extra = [("dE", dE)]
+    got = []
+    for _ in range(2):
+        alg.sparse_attention(Q, K, V, Z, L, heads, **fwd)
+        alg.sparse_attention_backward(Q, K, V, Z, L, dZ, dQ, dK, dV, heads, **fwd, **bwd)
+        got.append({key: m.to_host() for key, m in [("Z", Z), ("L", L), ("dQ", dQ), ("dK", dK), ("dV", dV)] + extra})
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k], equal_nan=True) for k in got[0])
+    out.update(got[0])
+
+
+def _gat(D, alg, case, N):
+    layers = [tuple(l) for l in case["layers"]]
+    X0, ws, a1, a2, G = gat_inputs(N, layers, case["seed"])
+    net = D.GAT(alg, layers, 0.2, attention=case["attention"])
+    if not case.get("rejected"):  # layouts that split R hold other weight shapes; they must refuse before reading them
+        for l, (_, fph, H) in enumerate(layers):
+            for h in range(H):
+                net.set_weight(l, h, ws[l][h])
+                if case["attention"] in ("additive", "gatv2"):
+                    net.set_attention_vectors(l, h, a1[l][h], a2[l][h] if case["attention"] == "additive" else np.zeros(fph))
+    return layers, X0, G, net
+
+
+def run_gat(D, alg, case, M, N, out):
+    layers, X0, G, net = _gat(D, alg, case, N)
+    if case.get("rejected"):
+        net.forward()
+        return
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    out.update(topA=topA, nrA=nrA, topB=topB, nrB=nrB)
+    net.set_input(gather_local(X0, [(topB, 0, nrB, layers[0][0])], net.buffer_shape(0)))
+    width = layers[-1][1] * layers[-1][2]
+    Gl = gather_local(G, [(topA, 0, nrA, width)], net.buffer_shape(len(layers)))
+    got = []
+    for _ in range(2):
+        net.forward()
+        o = dict(out=net.buffer(len(layers)))
+        net.backward(Gl)
+        o["dX0"] = net.input_grad()
+        for l, (_, _, H) in enumerate(layers):
+            for h in range(H):
+                o[f"dW_{l}_{h}"] = net.weight_grad(l, h)
+                o[f"da1_{l}_{h}"], o[f"da2_{l}_{h}"] = net.attention_grads(l, h)
+        got.append(o)
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k], equal_nan=True) for k in got[0])
+    out.update(got[0])
+
+
+def run_train(D, alg, case, M, N, out):
+    layers, X0, _, net = _gat(D, alg, case, N)
+    topA = alg.submatrices("A")[0][0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    net.set_input(gather_local(X0, [(topB, 0, nrB, layers[0][0])], net.buffer_shape(0)))
+    rows = net.buffer_shape(len(layers))[0]
+    classes = layers[-1][1] * layers[-1][2]
+    lab = -np.ones(rows, np.int64)
+    hi = min(topA + rows, N)
+    lab[:hi - topA] = labels_of(N, classes, case["seed"])[topA:hi]
+    nl = D.NodeLabels(net, lab, classes)
+    opt = D.AdamW(lr=1e-2)
+    out["local_rows"] = rows
+    out["steps"] = np.array([list(net.train_step(nl, opt)) for _ in range(case["steps"])])
+    for l, (_, _, H) in enumerate(layers):
+        for h in range(H):
+            out[f"w{l}_{h}"] = net.weight(l, h)
+            out[f"a1_{l}_{h}"], out[f"a2_{l}_{h}"] = net.attention_vectors(l, h)
+
+
+KINDS = dict(base=run_base, softmax=run_softmax, attn=run_attn, gat=run_gat, train=run_train)
+
+
+def run_case(D, case, rank, world):
+    """The case on this rank: {key: array}, with "error" = the message if the library refused."""
+    M, N = sizes(case)
+    rows, cols = skewed_tuples(M, N, case["seed"])
+    tr, tc = rank_slice(rows, cols, rank, world)
+    S = D.SpmatLocal.from_tuples(M, N, tr, tc, sval(tr, tc) if case["kind"] == "base" else np.ones(len(tr)))
+    alg = D.Algorithm(case["alg"], S, case["R"], case["c"])
+    out = {}
+    try:
+        KINDS[case["kind"]](D, alg, case, M, N, out)
+    except RuntimeError as e:
+        out["error"] = str(e)
+        if not case.get("rejected"):  # shown by the launcher if the other ranks then wait for this one
+            print(f"rank {rank}: {case['name']}: {e}", flush=True)
+    del alg, S
+    return out
+
+
+def main():
+    cases = json.loads(sys.argv[1])
+    outdir = sys.argv[2]
+    transport = sys.argv[3]
+    import torch
+    ngpu = torch.cuda.device_count()
+    if ngpu:
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")) % ngpu if transport == "nccl" else 0)
+    from distributed_sddmm_b200 import driver as D
+    rank, world = D.world_init(transport)
+    for case in cases:
+        if rank == 0:  # progress, shown when the launcher reports a failure or a timeout
+            print("case", case["name"], flush=True)
+        np.savez(os.path.join(outdir, f"{case['name']}_rank{rank}.npz"), **run_case(D, case, rank, world))
+    D.world_finalize()
+
+
+if __name__ == "__main__":
+    main()

@@ -1,0 +1,490 @@
+"""The distributed ops on a skewed graph (tests/skewed_graph.py: hub rows of more than two softmax pieces spread over
+every rank's column block, a hub column, a rank whose row block is empty, a column band nothing touches, duplicates and
+self-loops, 4200 nodes so that 4 ranks hold 1050 rows each) at the kernels' table widths, on 1, 2 and 4 ranks
+(tests/mp_skewed_worker.py): the base ops at R = 64, 128, 256 and 100 on every layout, the edge softmax with and without
+-inf scores, fused sparse attention (plain, dropout, a masking per-head bias, edge features) at heads x d = 2 x 64,
+1 x 128 and 4 x 7, GAT forward and backward with the four attention kinds and GAT train steps, each against the fp64
+models written per stored entry, rank by rank.  Beyond parity: rows without entries give Z = 0, L = -inf and zero dQ,
+untouched columns zero dK and dV; a repeat gives the same bits; the results at p = 2 and 4 equal those at p = 1 to
+1e-12; per-entry gradients (dbias, dE) of the two copies of a duplicate agree, with dropout too (one keep bit per
+(row, column), whatever the layout); trained parameters are bit-identical across ranks.
+
+One worker launch per rank count serves every test of that count.  Ranks share cuda:0 over the gloo-backed transport
+unless there is one GPU per rank (then NCCL)."""
+import json
+import math
+import os
+import subprocess
+import sys
+import tempfile
+
+import numpy as np
+import pytest
+import torch
+
+from tests import gat_additive_oracle as gao
+from tests import gat_backward_oracle as gbk
+from tests import gat_softmax_oracle as gso
+from tests import gatv2_oracle as gv2
+from tests import mp_skewed_worker as W
+from tests import sparse_attention_bias_oracle as sb
+from tests import sparse_attention_dropout_oracle as sd
+from tests import sparse_attention_edge_oracle as se
+from tests import sparse_attention_oracle as sa
+from tests import training_oracle as tro
+from tests.mp_edge_softmax_worker import score, upstream
+from tests.mp_sparse_attention_edge_worker import edge_of
+from tests.mp_util import ROOT, free_port
+from tests.mp_worker import gather_local, sval
+from tests.skewed_graph import landmarks, skewed_tuples
+from tests.test_sparse_attention_multirank_gpu import rel_err
+
+pytestmark = pytest.mark.gpu
+SEED = 0xC0FFEE + 211
+GAT_LAYERS = [[64, 32, 2], [64, 16, 4]]  # per-head products at table widths 32 and 16 from inputs 64 wide
+# widths per layout: every layout sees table widths inside its shift loops, the dense-shift layouts the generic kernels too
+BASE_WIDTHS = {"15d_fusion1": [64, 128, 256, 100], "15d_fusion2": [128, 100], "15d_sparse": [256, 128],
+               "25d_dense_replicate": [256, 128], "25d_sparse_replicate": [64, 128]}
+REPLICATION = {1: {a: [1] for a in BASE_WIDTHS},
+               2: {"15d_fusion1": [1, 2], "15d_fusion2": [1, 2], "15d_sparse": [1, 2], "25d_sparse_replicate": [2]},
+               4: {"15d_fusion1": [1, 2], "15d_fusion2": [1, 2], "15d_sparse": [1, 2], "25d_dense_replicate": [1],
+                   "25d_sparse_replicate": [1]}}
+ALL_OPS = ["sddmmA", "spmmA", "spmmB", "fusedA", "sddmmB", "fusedB"]
+
+
+def _case(kind, alg, c, R, **kw):
+    tag = "_".join(f"{k}{v}" for k, v in sorted(kw.items()) if k not in ("layers", "script", "mask_seed", "steps"))
+    return dict(name=f"{kind}_{alg}_c{c}_R{R}" + ("_" + tag if tag else ""), kind=kind, alg=alg, c=c, R=R, seed=SEED, **kw)
+
+
+def cases_for(p):
+    out = []
+    for alg, cs in REPLICATION[p].items():
+        for i, R in enumerate(BASE_WIDTHS[alg]):
+            c = cs[i % len(cs)]
+            # local kernel fusion with c > 1 accumulates its fused output onto the gathered operand: not what the global
+            # model states, and covered against the reference's own code in tests/test_multirank_gpu.py
+            script = [op for op in ALL_OPS if not (alg == "15d_fusion2" and c > 1 and op.startswith("fused"))]
+            out.append(_case("base", alg, c, R, script=script))
+    c2 = 2 if p > 1 else 1  # replication needs at least 2 ranks
+    out += [_case("softmax", "15d_fusion1", 1, 8), _case("softmax", "15d_fusion1", c2, 8, mask=1),
+            _case("softmax", "15d_fusion2", 1, 8), _case("softmax", "15d_fusion1", 1, 8, mask=1)]
+
+    def attn(alg, c, heads, d, variant, dropout=0.0):
+        return _case("attn", alg, c, heads * d, heads=heads, d=d, variant=variant, dropout=dropout, mask_seed=29)
+
+    out += [attn("15d_fusion1", 1, 2, 64, "plain"), attn("15d_fusion2", 1, 1, 128, "plain"), attn("15d_fusion1", c2, 4, 7, "plain"),
+            attn("15d_fusion1", 1, 1, 128, "plain", 0.4), attn("15d_fusion2", 1, 2, 64, "plain", 0.4),
+            attn("15d_fusion1", 1, 2, 64, "bias", 0.4), attn("15d_fusion2", 1, 4, 7, "bias"),
+            attn("15d_fusion1", c2, 1, 128, "bias"),
+            attn("15d_fusion1", 1, 1, 128, "edge"), attn("15d_fusion1", c2, 2, 64, "edge", 0.4),
+            attn("15d_fusion2", 1, 4, 7, "edge")]
+    for kind, alg, c in (("leaky", "15d_fusion1", 1), ("softmax", "15d_fusion2", 1), ("additive", "15d_fusion1", c2),
+                         ("gatv2", "15d_fusion1", 1)):
+        out.append(_case("gat", alg, c, 64, attention=kind, layers=GAT_LAYERS))
+    out += [_case("train", "15d_fusion1", 1, 64, attention="additive", layers=GAT_LAYERS, steps=3),
+            _case("train", "15d_fusion2", 1, 64, attention="softmax", layers=GAT_LAYERS, steps=3)]
+    if p > 1:  # the layouts that split R have no row softmax, attention or GAT backward
+        out += [dict(attn("15d_sparse", 1, 2, 64, "plain"), rejected=1),
+                dict(_case("gat", "15d_sparse", 1, 64, attention="softmax", layers=GAT_LAYERS), rejected=1)]
+    return list({c["name"]: c for c in out}.values())  # at p = 1 the c = 2 cases fall onto their c = 1 twins
+
+
+CASES = {p: cases_for(p) for p in (1, 2, 4)}
+
+
+def params(kind, ps=(1, 2, 4), **match):
+    return [pytest.param(p, c, id=f"p{p}-{c['name']}") for p in ps for c in CASES[p]
+            if c["kind"] == kind and not c.get("rejected") and all(c.get(k) == v for k, v in match.items())]
+
+
+_RESULTS = {}
+
+
+def results(nproc, timeout=2400):
+    """{case name: [per-rank dict]} of every case of this rank count: one launch, kept for the module."""
+    if nproc in _RESULTS:
+        return _RESULTS[nproc]
+    cases = CASES[nproc]
+    transport = "self" if nproc == 1 else "nccl" if torch.cuda.device_count() >= nproc else "gloo"
+    with tempfile.TemporaryDirectory() as td:
+        cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={nproc}",
+               "--master-addr", "127.0.0.1", "--master-port", str(free_port()),
+               os.path.join(ROOT, "tests", "mp_skewed_worker.py"), json.dumps(cases), td, transport]
+        env = dict(os.environ, OMP_NUM_THREADS="2")
+        p = subprocess.run(cmd, cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=timeout, text=True)
+        if p.returncode != 0 and "Address already in use" in p.stdout:  # lost the race for the rendezvous port
+            cmd[cmd.index("--master-port") + 1] = str(free_port())
+            p = subprocess.run(cmd, cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=timeout, text=True)
+        assert p.returncode == 0, "worker failed:\n" + p.stdout[-6000:]
+        out = {}
+        for c in cases:
+            out[c["name"]] = []
+            for r in range(nproc):
+                z = np.load(os.path.join(td, f"{c['name']}_rank{r}.npz"), allow_pickle=False)
+                out[c["name"]].append({k: z[k] for k in z.files})
+    _RESULTS[nproc] = out
+    return out
+
+
+_GRAPH = {}
+
+
+def graph(case):
+    """(M, N, rows, cols) of a case as int64, sorted by (row, col) with the duplicates kept."""
+    M, N = W.sizes(case)
+    if (M, N) not in _GRAPH:
+        r, c = (x.astype(np.int64) for x in skewed_tuples(M, N, case["seed"]))
+        order = np.lexsort((c, r))
+        _GRAPH[M, N] = (r[order], c[order])
+    return (M, N, *_GRAPH[M, N])
+
+
+def lookup(N, rows, cols, values, qr, qc):
+    """values (one per stored entry of the sorted rows, cols) at the entries (qr, qc); the copies of a duplicate are
+    equal in every per-entry model (inputs that are functions of (row, col)), so the first copy stands for all."""
+    key = rows * N + cols
+    at = np.searchsorted(key, qr * N + qc)
+    assert np.array_equal(key[at], qr * N + qc)
+    return values[at]
+
+
+def ranks_ok(ranks, name):
+    for r, d in enumerate(ranks):
+        assert "error" not in d, (name, r, str(d.get("error")))
+    return ranks
+
+
+def assemble(ranks, key, top, nr, total):
+    """The global matrix from every rank's rows [top, top + nr) of `key`; all rows must be covered."""
+    first = ranks[0][key]
+    G = np.full((total,) + first.shape[1:], np.nan)
+    covered = np.zeros(total, bool)
+    for d in ranks:
+        t, n = int(d[top]), min(int(d[nr]), total - int(d[top]))
+        G[t:t + n] = d[key][:n]
+        covered[t:t + n] = True
+    assert covered.all(), key
+    return G
+
+
+def check_rows(ranks, name, key, want, top, nr, tol=1e-10):
+    """Every rank's rows of `key` against the model's, +-inf matched exactly; returns the assembled global matrix."""
+    total = len(want)
+    for r, d in enumerate(ranks):
+        t, n = int(d[top]), min(int(d[nr]), total - int(d[top]))
+        got, w = d[key][:n], want[t:t + n]
+        fin = np.isfinite(w)
+        assert np.array_equal(fin, np.isfinite(got)) and np.array_equal(got[~fin], w[~fin]), (name, r, key)
+        err = np.abs(got[fin] - w[fin]).max(initial=0.0) / max(np.abs(want[np.isfinite(want)]).max(initial=0.0), 1e-300)
+        assert err < tol, (name, r, key, err)
+    return assemble(ranks, key, top, nr, total)
+
+
+# ---- base ops ------------------------------------------------------------------------------------------------------
+_BASE_REF = {}
+
+
+def base_reference(case, ones):
+    """Dense results of the global model for the case's width: S's value at (u, v) is sval(u, v) per stored copy (ones:
+    1 per copy), so duplicates add up, as in the scipy matrix of oracle.hnh_oracle.global_reference."""
+    import scipy.sparse as sp
+    M, N, rows, cols = graph(case)
+    key = (M, N, case["R"], ones)
+    if key not in _BASE_REF:
+        A, B = W.base_inputs(M, N, case["R"], case["seed"])
+        v = np.ones(len(rows)) if ones else sval(rows, cols)
+        S = sp.csr_matrix((v, (rows, cols)), shape=(M, N))  # sums the copies of a duplicate
+        ri = np.repeat(np.arange(M), np.diff(S.indptr))
+        Sd = sp.csr_matrix((S.data * np.einsum("ij,ij->i", A[ri], B[S.indices]), S.indices, S.indptr), shape=(M, N))
+        _BASE_REF[key] = dict(spmmA=S @ B, spmmB=S.T @ A, fusedA=Sd @ B, fusedB=Sd.T @ A)
+    return _BASE_REF[key]
+
+
+def check_base(ranks, case, nproc):
+    ranks = ranks_ok(ranks, case["name"])
+    M, N, rows, cols = graph(case)
+    A, B = W.base_inputs(M, N, case["R"], case["seed"])
+    for mode in ("A", "B"):  # every stored pair is held by some rank, in both value orders
+        keys = np.concatenate([d[f"{mode}_rows"] * N + d[f"{mode}_cols"] for d in ranks])
+        assert np.array_equal(np.unique(keys), np.unique(rows * N + cols)), (case["name"], mode)
+        if case["c"] == 1 and not case["alg"].startswith("25d"):
+            assert np.array_equal(np.sort(keys), rows * N + cols), (case["name"], mode, "copies of duplicates")
+    for op in case["script"]:
+        mode = op[-1]
+        # local kernel fusion treats S as an all-ones pattern and leaves the SDDMM buffer unfilled
+        ones = case["alg"] == "15d_fusion2" and op.startswith("fused")
+        for r, d in enumerate(ranks):
+            where = (case["name"], op, r)
+            assert bool(d[op + "_repeat"]), where
+            if not op.startswith("spmm") and not ones:
+                u, v = d[f"{mode}_rows"], d[f"{mode}_cols"]
+                want = sval(u, v) * np.einsum("ij,ij->i", A[u], B[v])
+                assert np.abs(d[op + "_values"] - want).max(initial=0.0) <= 1e-10 * np.abs(want).max(initial=1e-300), where
+            if not op.startswith("sddmm"):
+                G = base_reference(case, ones)[op]
+                subs, shape = (d["aSubmatrices"], d["shapeA"]) if mode == "A" else (d["bSubmatrices"], d["shapeB"])
+                want = gather_local(G, [tuple(int(x) for x in s) for s in subs], tuple(int(x) for x in shape))
+                assert np.abs(d[op + "_dense"] - want).max() <= 1e-10 * np.abs(G).max(), where
+
+
+# ---- edge softmax --------------------------------------------------------------------------------------------------
+def check_softmax(ranks, case, nproc):
+    ranks = ranks_ok(ranks, case["name"])
+    M, N, rows, cols = graph(case)
+    x = score(rows, cols)
+    if case.get("mask"):
+        x[W.masked(rows, cols, M, N)] = -np.inf
+    alpha = gso.edge_softmax_np(x, rows, M)
+    # a row masked throughout is NaN, as torch.softmax gives (fused sparse attention defines Z = 0, L = -inf there)
+    dx = gso.edge_softmax_backward_np(alpha, upstream(rows, cols), rows, M)
+    hub = landmarks(M, N)["wide_hubs"][0]
+    for mode in ("A", "B"):
+        keys = []
+        for r, d in enumerate(ranks):
+            where = (case["name"], mode, r)
+            assert bool(d[f"{mode}_repeat"]), where
+            u, v = d[f"{mode}_rows"], d[f"{mode}_cols"]
+            for got, w in ((d[f"{mode}_alpha"], lookup(N, rows, cols, alpha, u, v)), (d[f"{mode}_dx"], lookup(N, rows, cols, dx, u, v))):
+                nan = np.isnan(w)
+                assert np.array_equal(np.isnan(got), nan) and nan.sum() <= 0.01 * len(nan), where
+                assert rel_err(got[~nan], w[~nan]) < 1e-13, where
+            keys.append(u * N + v)
+        assert np.array_equal(np.sort(np.concatenate(keys)), rows * N + cols), (case["name"], mode)  # duplicates included
+        assert (rows == hub).sum() > 2 * 1024 + 37  # the hub row is more than two pieces long
+
+
+# ---- fused sparse attention ----------------------------------------------------------------------------------------
+_ATTN_REF = {}
+
+
+def attention_reference(case):
+    """The model's Z, L, dQ, dK, dV and per-entry gradients for a case (the same at every rank count)."""
+    key = (W.sizes(case), case["heads"], case["d"], case["variant"], case["dropout"])
+    if key in _ATTN_REF:
+        return _ATTN_REF[key]
+    M, N, rows, cols = graph(case)
+    heads, d, p, seed = case["heads"], case["d"], case["dropout"], case["mask_seed"]
+    Q, dZ, K, V = W.attn_inputs(M, N, heads * d, case["seed"])
+    scale = 1 / math.sqrt(d)
+    want = {}
+    if case["variant"] == "plain" and p == 0.0:
+        want["Z"], want["L"] = sa.forward_np(rows, cols, M, Q, K, V, heads, scale)
+        want["dQ"], want["dK"], want["dV"] = sa.backward_np(rows, cols, M, Q, K, V, dZ, heads, scale)
+    elif case["variant"] == "plain":
+        want["Z"], want["L"] = sd.forward_np(rows, cols, M, Q, K, V, heads, scale, p, seed)
+        want["dQ"], want["dK"], want["dV"] = sd.backward_np(rows, cols, M, Q, K, V, dZ, heads, scale, p, seed)
+    elif case["variant"] == "bias":
+        bias = np.concatenate([W.bias_of(rows, cols, h, M, N) for h in range(heads)])
+        want["Z"], want["L"] = sb.forward_np(rows, cols, M, Q, K, V, bias, heads, scale, p, seed)
+        want["dQ"], want["dK"], want["dV"], want["db"] = sb.backward_np(rows, cols, M, Q, K, V, dZ, bias, heads, scale, p, seed)
+    else:
+        E = edge_of(rows, cols, heads * d)
+        want["Z"], want["L"] = se.forward_np(rows, cols, M, Q, K, V, E, heads, scale, p, seed)
+        want["dQ"], want["dK"], want["dV"], want["dE"], _ = se.backward_np(rows, cols, M, Q, K, V, E, dZ, heads, scale, p, seed)
+    _ATTN_REF[key] = want
+    return want
+
+
+def check_attention(ranks, case, nproc):
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    M, N, rows, cols = graph(case)
+    want = attention_reference(case)
+    heads = case["heads"]
+    for r, d in enumerate(ranks):
+        assert bool(d["repeat"]), (name, r)
+    got = {}
+    for key in ("Z", "L", "dQ"):
+        got[key] = check_rows(ranks, name, key, want[key], "topA", "nrA")
+    for key in ("dK", "dV"):
+        got[key] = check_rows(ranks, name, key, want[key], "topB", "nrB")
+    # rows without entries, and the columns nothing points to
+    empty = np.bincount(rows, minlength=M) == 0
+    lm = landmarks(M, N)
+    assert empty[lm["empty_rows"][0]:lm["empty_rows"][1]].all() and empty.mean() > 0.25
+    assert not got["Z"][empty].any() and np.isneginf(got["L"][empty]).all() and not got["dQ"][empty].any(), name
+    untouched = np.bincount(cols, minlength=N) == 0
+    assert untouched[lm["empty_cols"][0]:lm["empty_cols"][1]].all()
+    assert not got["dK"][untouched].any() and not got["dV"][untouched].any(), name
+    if case["variant"] == "bias" and heads > 1:
+        assert np.isneginf(want["L"][0, 1]) and np.isfinite(want["L"][0, 0])  # row 0 is masked throughout in head 1 only
+    # per-entry gradients, matched by (row, col): the copies of a duplicate agree (with dropout: they share one keep bit)
+    nnz = len(rows)
+    dup = np.flatnonzero(np.diff(rows * N + cols) == 0)
+    assert len(dup) >= 50 and (rows[dup] == lm["dup_row"]).sum() >= 3
+    for r, d in enumerate(ranks):
+        if case["variant"] == "bias":
+            for order, u, v in (("dbA", d["rA"], d["cA"]), ("dbB", d["rB"], d["cB"])):
+                n = len(u)
+                assert d[order].shape == (heads * n,), (name, r, order)
+                for h in range(heads):
+                    w = lookup(N, rows, cols, want["db"][h * nnz:(h + 1) * nnz], u, v)
+                    assert rel_err(d[order][h * n:(h + 1) * n], w) < 1e-10, (name, r, order, h)
+        if case["variant"] == "edge":
+            assert rel_err(d["dE"], lookup(N, rows, cols, want["dE"], d["rA"], d["cA"])) < 1e-10, (name, r, "dE")
+    if case["dropout"] > 0 and case["variant"] != "plain":
+        # the dropped entries show as rows of dE (or entries of dbias) that lose their D w alpha dZ term: what the model
+        # computes from the hash of the global (row, col) is what every layout computes, copy by copy
+        key, u, v = ("dE", "rA", "cA") if case["variant"] == "edge" else ("dbA", "rA", "cA")
+        allk = np.concatenate([d[u] * N + d[v] for d in ranks])
+        vals = np.concatenate([d[key] if key == "dE" else d[key][:len(d[u])] for d in ranks])
+        order = np.argsort(allk, kind="stable")
+        allk, vals = allk[order], vals[order]
+        same = np.flatnonzero(np.diff(allk) == 0)
+        assert len(same) >= 50 and np.array_equal(vals[same], vals[same + 1]), (name, "copies of a duplicate differ")
+
+
+# ---- GAT -----------------------------------------------------------------------------------------------------------
+def gat_forward(kind, ri, ci, N, layers, ws, u1, u2, x):
+    if kind == "leaky":
+        return gbk.gat_forward_torch(ri, ci, N, layers, ws, 0.2, x)
+    if kind == "softmax":
+        return gso.gat_softmax_forward_torch(ri, ci, N, layers, ws, 0.2, x)
+    if kind == "additive":
+        return gao.gat_additive_forward_torch(ri, ci, N, layers, ws, u1, u2, 0.2, x)
+    return gv2.gatv2_forward_torch(ri, ci, N, layers, ws, u1, 0.2, x)
+
+
+def gat_tensors(case, grad=True):
+    """The case's inputs as torch leaves, and the stored entries with their duplicates (the models' edges() would
+    merge them; the forward functions take any edge list)."""
+    M, N, rows, cols = graph(case)
+    layers = [tuple(l) for l in case["layers"]]
+    X0, ws, a1, a2, G = W.gat_inputs(N, layers, case["seed"])
+    t = lambda v: torch.tensor(np.asarray(v, np.float64), requires_grad=grad)  # noqa: E731
+    nest = lambda n: [[t(v) for v in l] for l in n]  # noqa: E731
+    return N, layers, torch.from_numpy(rows), torch.from_numpy(cols), t(X0), nest(ws), nest(a1), nest(a2), G
+
+
+_GAT_REF = {}
+
+
+def gat_reference(case):
+    if case["attention"] not in _GAT_REF:
+        N, layers, ri, ci, x, ws, u1, u2, G = gat_tensors(case)
+        out = gat_forward(case["attention"], ri, ci, N, layers, ws, u1, u2, x)
+        out.backward(torch.from_numpy(G))
+        g = lambda v: v.grad.numpy() if v.grad is not None else np.zeros(v.shape)  # noqa: E731
+        want = dict(out=out.detach().numpy(), dX0=g(x))
+        for l, (_, _, H) in enumerate(layers):
+            for h in range(H):
+                want[f"dW_{l}_{h}"] = g(ws[l][h])
+                if case["attention"] in ("additive", "gatv2"):
+                    want[f"da1_{l}_{h}"] = g(u1[l][h])
+                if case["attention"] == "additive":
+                    want[f"da2_{l}_{h}"] = g(u2[l][h])
+        _GAT_REF[case["attention"]] = want
+    return _GAT_REF[case["attention"]]
+
+
+def check_gat(ranks, case, nproc):
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    want = gat_reference(case)
+    assert np.abs(want["out"]).max() > 0 and np.abs(want["dX0"]).max() > 0
+    for r, d in enumerate(ranks):
+        assert bool(d["repeat"]), (name, r)
+    check_rows(ranks, name, "out", want["out"], "topA", "nrA")
+    check_rows(ranks, name, "dX0", want["dX0"], "topB", "nrB")
+    for key, w in want.items():
+        if key[0] == "d" and key != "dX0":
+            assert np.abs(w).max() > 0, (name, key)
+            for r, d in enumerate(ranks):
+                assert np.array_equal(d[key], ranks[0][key]), (name, r, key, "differs across ranks")
+            assert rel_err(ranks[0][key], w) < 1e-10, (name, key)
+
+
+def check_training(ranks, case, nproc):
+    """3 train steps: the cross-entropy and the parameter-gradient reductions run over 1050 local rows at p = 4 (more
+    than two row chunks of 512), with one rank's row block unlabelled and another's without entries."""
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    if nproc == 4:
+        assert all(int(d["local_rows"]) >= 2 * 512 + 1 for d in ranks)
+    for r, d in enumerate(ranks):
+        for k in d:
+            assert np.array_equal(d[k], ranks[0][k]), (name, r, k, "differs across ranks")
+    N, layers, ri, ci, x, ws, u1, u2, _ = gat_tensors(case)
+    x = x.detach()
+    labels = W.labels_of(N, layers[-1][1] * layers[-1][2], case["seed"])
+    lm = landmarks(N, N)
+    assert 0.2 < (labels >= 0).mean() < 0.4 and (labels[lm["narrow_rows"][0]:] < 0).all() and labels[lm["wide_hubs"][0]] >= 0
+    leaves = [w for l in ws for w in l]
+    if case["attention"] == "additive":
+        leaves += [v for l1, l2 in zip(u1, u2) for v in l1 + l2]
+    res = tro.train(lambda _: gat_forward(case["attention"], ri, ci, N, layers, ws, u1, u2, x), leaves, labels, case["steps"],
+                    lr=1e-2)
+    steps = ranks[0]["steps"]
+    for t, w in enumerate(res):
+        assert abs(steps[t][0] - w[0]) <= 1e-10 * abs(w[0]) and abs(steps[t][3] - w[3]) <= 1e-10 * abs(w[3]), (name, t)
+        assert (int(steps[t][1]), int(steps[t][2])) == (w[1], w[2]), (name, t)
+    for l, (_, _, H) in enumerate(layers):
+        for h in range(H):
+            read = [(f"a1_{l}_{h}", u1[l][h]), (f"a2_{l}_{h}", u2[l][h])] if case["attention"] == "additive" else []
+            for key, w in [(f"w{l}_{h}", ws[l][h])] + read:  # vectors the attention does not read are never set
+                w = w.detach().numpy()
+                err = np.abs(ranks[0][key] - w).max()
+                assert err <= 1e-9 * max(np.abs(w).max(), 1.0), (name, key, err)
+
+
+# ---- across rank counts --------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("nproc", [2, 4])
+def test_results_do_not_depend_on_the_rank_count(nproc):
+    """Every attention, GAT and training case that also runs at p = 1: the assembled global result equals p = 1's to
+    1e-12 of its largest entry (the sums run in another order), +-inf exactly."""
+    one, many = results(1), results(nproc)
+    checked = 0
+    for case in CASES[nproc]:
+        name = case["name"]
+        if name not in one or case["kind"] not in ("attn", "gat", "train") or case.get("rejected"):
+            continue
+        a, b = ranks_ok(one[name], name), ranks_ok(many[name], name)
+        M, N = W.sizes(case)
+        if case["kind"] == "train":
+            pairs = [(a[0][k], b[0][k]) for k in a[0] if k != "local_rows"]
+        else:
+            keysA, keysB = (("Z", "L", "dQ"), ("dK", "dV")) if case["kind"] == "attn" else (("out",), ("dX0",))
+            pairs = [(assemble(a, k, "topA", "nrA", M), assemble(b, k, "topA", "nrA", M)) for k in keysA]
+            pairs += [(assemble(a, k, "topB", "nrB", N), assemble(b, k, "topB", "nrB", N)) for k in keysB]
+        for x, y in pairs:
+            # trained parameters: AdamW's g / (sqrt(v) + eps) amplifies the last bits of small gradients, as against the model
+            assert rel_err(y, x) < (1e-9 if case["kind"] == "train" else 1e-12), (name, nproc)
+        checked += 1
+    assert checked >= 10
+
+
+@pytest.mark.parametrize("nproc", [2, 4])
+def test_layouts_without_the_op_still_refuse_on_every_rank(nproc):
+    got = results(nproc)
+    rejected = [c for c in CASES[nproc] if c.get("rejected")]
+    assert rejected
+    for c in rejected:
+        for r, d in enumerate(got[c["name"]]):
+            msg = str(d.get("error"))
+            assert "error" in d and "code -1" in msg and "not defined for" in msg and f"p = {nproc}" in msg, (c["name"], r, msg)
+
+
+@pytest.mark.parametrize("nproc,case", params("base"))
+def test_base_ops_on_the_skewed_graph(nproc, case):
+    check_base(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("softmax"))
+def test_edge_softmax_on_the_skewed_graph(nproc, case):
+    check_softmax(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("attn"))
+def test_sparse_attention_on_the_skewed_graph(nproc, case):
+    check_attention(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gat"))
+def test_gat_on_the_skewed_graph(nproc, case):
+    check_gat(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("train"))
+def test_gat_training_on_the_skewed_graph(nproc, case):
+    check_training(results(nproc)[case["name"]], case, nproc)
