@@ -109,6 +109,10 @@ ABI = {
     "hnh_adamw_f64": (C.c_int, [_P, _P, _P, _P, _I64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
                                 C.c_double, C.c_double, _P, _P]),
     "hnh_clip_coef_f64": (C.c_int, [_P, _P, _I64, C.c_double, _P]),
+    "hnh_pair_sums_workspace_bytes": (C.c_int64, [_I64]),
+    "hnh_pair_sums_f64": (C.c_int, [_P, _P, _I64, _P, C.c_size_t, _P]),
+    "hnh_link_bce_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, _P, _I64, C.c_int, C.c_double, _P, _I64, _P, _I64, _P, _P]),
+    "hnh_link_target_check_f64": (C.c_int, [_P, _P, _I64, _P]),
     "hnh_entry_coords_from_index_f64":(C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
@@ -299,6 +303,13 @@ ABI.update({
     "hnhd_adamw_destroy": (None, [_P]),
     "hnhd_gt_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
     "hnhd_gat_train_step": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_alg_link_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "hnhd_link_targets_create": (C.c_int, [_P, _P, _PP]),
+    "hnhd_link_targets_destroy": (None, [_P]),
+    "hnhd_gt_link_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
+    "hnhd_gat_link_train_step": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_gt_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_gat_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

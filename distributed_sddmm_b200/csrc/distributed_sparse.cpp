@@ -7,6 +7,7 @@
 #include <iostream>
 #include <mutex>
 #include <optional>
+#include <tuple>
 
 #include "hnh/15D_dense_shift.hpp"
 #include "hnh/25D_cannon_dense.hpp"
@@ -1001,6 +1002,90 @@ void Distributed_Sparse::sparseAttentionBackward(DenseMatrix &Q, DenseMatrix &K,
                                            "sparse_attention_grad_kv_dropout");
                     });
     }
+}
+
+// ---- link prediction -----------------------------------------------------------------------------------------
+void Distributed_Sparse::linkLoss(DenseMatrix &H_A, DenseMatrix &H_B, double inv_count, DenseMatrix *dH_A, DenseMatrix *dH_B,
+                                  VectorXd *scores, double *sums) {
+    const string who = "linkLoss";
+    check_full_rows(who);
+    const int64_t r = H_A.cols();
+    if (H_A.rows() != localArows || H_B.rows() != localBrows || H_B.cols() != r || r < 1 || r > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": H_A is " + to_string(H_A.rows()) + " x " + to_string(r) + " and H_B " +
+                                            to_string(H_B.rows()) + " x " + to_string(H_B.cols()) + "; like_A_matrix has " +
+                                            to_string(localArows) + " rows and like_B_matrix " + to_string(localBrows) +
+                                            ", both of one width");
+    for (auto [g, h, name] : {std::make_tuple(dH_A, &H_A, "dH_A"), std::make_tuple(dH_B, &H_B, "dH_B")}) {
+        if (g && (g == &H_A || g == &H_B)) throw hnh::Error(HNH_E_INVALID, who + ": " + name + " may not be H_A or H_B");
+        if (g && (g->rows() != h->rows() || g->cols() != r))
+            throw hnh::Error(HNH_E_INVALID, who + ": " + name + " is " + to_string(g->rows()) + " x " + to_string(g->cols()) +
+                                                ", its H " + to_string(h->rows()) + " x " + to_string(r));
+    }
+    if (scores && scores->size() != num_S_values())
+        throw hnh::Error(HNH_E_INVALID, who + ": the scores have " + to_string(scores->size()) + " entries, the A order " +
+                                            to_string(num_S_values()));
+    if (!(inv_count >= 0.0) || !std::isfinite(inv_count)) throw hnh::Error(HNH_E_INVALID, who + ": inv_count must be finite and >= 0");
+    if (sums == nullptr) throw hnh::Error(HNH_E_INVALID, who + ": null sums");
+    // the rows' (loss sum, correct count), accumulated over the ring steps
+    DenseMatrix stats(localArows, 2);
+    stats.setZero();
+    if (dH_A) dH_A->setZero();
+    if (dH_B && dH_B != dH_A) dH_B->setZero();
+    // one pass: the stored-row side is [H, its gradient (when wanted), the row statistics (A order only)]
+    auto pass = [&](KernelMode order, DenseMatrix &H, DenseMatrix *dH, DenseMatrix &G, DenseMatrix *st) {
+        const bool a_rows = order == k_sddmmA;
+        vector<PassOperand> rows{{&H, 0, r, false}}, gathered{{&G, 0, r, false}};
+        const int i_grad = dH ? (int)rows.size() : -1;
+        if (dH) rows.push_back({dH, 0, r, true});
+        const int i_stats = st ? (int)rows.size() : -1;
+        if (st) rows.push_back({st, 0, 2, true});
+        const SpmatLocal &m = *values_matrix(*this, order);
+        gather_pass(order, a_rows ? rows : gathered, a_rows ? gathered : rows,
+                    [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                        if (rows_are_A != a_rows)
+                            throw hnh::Error(HNH_E_INVALID, who + ": a block of this order does not hold the expected side as its rows");
+                        CSRHandle *h = blk.getActive();
+                        double *sc = scores && a_rows ? scores->data() + (int64_t)m.blockStarts[(size_t)b] : nullptr;
+                        hnh::abi_check(hnh_link_bce_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(), blk.rows,
+                                                        blk.num_coords, R[0].p, R[0].ld, Y[0].p, Y[0].ld, (int)r, inv_count,
+                                                        i_grad >= 0 ? R[i_grad].p : nullptr, i_grad >= 0 ? R[i_grad].ld : r,
+                                                        i_stats >= 0 ? R[i_stats].p : nullptr, i_stats >= 0 ? R[i_stats].ld : 2,
+                                                        sc, compute()),
+                                       "link_bce");
+                    });
+    };
+    pass(k_sddmmA, H_A, dH_A, H_B, &stats);
+    if (dH_B) pass(k_sddmmB, H_B, dH_B, H_A, nullptr);
+    const int64_t ws_bytes = hnh_pair_sums_workspace_bytes(localArows);
+    if (ws_bytes < 0) hnh::abi_check((int)ws_bytes, "pair_sums_workspace_bytes");
+    VectorXd ws(std::max<int64_t>(ws_bytes / 8, 1));
+    hnh::abi_check(hnh_pair_sums_f64(sums, stats.data(), localArows, ws.data(), (size_t)ws_bytes, compute()), "pair_sums");
+    allreduce_rows(sums, 2, false);
+}
+
+int64_t Distributed_Sparse::linkTargetCount() {
+    check_full_rows("linkTargetCount");
+    const int64_t n = num_S_values();
+    SpmatLocal &m = *values_matrix(*this, k_sddmmA);
+    VectorXd bad(1);
+    bad.setZero();
+    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
+        const int64_t nb = (int64_t)m.blockStarts[b + 1] - (int64_t)m.blockStarts[b];
+        if (nb == 0) continue;
+        CSRLocal *blk = m.csr_blocks[b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, "linkTargetCount: block " + to_string(b) + " does not match its value range");
+        hnh::abi_check(hnh_link_target_check_f64(bad.data(), blk->getActive()->values.data(), nb, compute()), "link_target_check");
+    }
+    double mine = 0.0;
+    hnh::cuda_check(cudaMemcpyAsync(&mine, bad.data(), sizeof mine, cudaMemcpyDeviceToHost, compute()), "target check");
+    hnh::cuda_check(cudaStreamSynchronize(compute()), "target check");
+    double x[2] = {mine > 0.0 ? 1.0 : 0.0, (double)n};
+    hnh::Comm::world()->host_allreduce_sum_f64(x, 2);
+    if (mine > 0.0)
+        throw hnh::Error(HNH_E_INVALID, "link targets: " + to_string((int64_t)mine) + " stored values of this rank are not in [0, 1]");
+    if (x[0] != 0.0) throw hnh::Error(HNH_E_INVALID, "link targets: another rank's stored values are not all in [0, 1]");
+    return (int64_t)x[1];
 }
 
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {

@@ -45,6 +45,9 @@ struct hnhd_labels {
 struct hnhd_adamw {
     std::unique_ptr<hnh::AdamW> o;
 };
+struct hnhd_link_targets {
+    std::unique_ptr<hnh::LinkTargets> t;
+};
 
 namespace {
 
@@ -887,6 +890,64 @@ int hnhd_gat_train_step(hnhd_gat_t *g, const hnhd_labels_t *labels, hnhd_adamw_t
     return guarded([&] {
         if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_train_step: null argument");
         train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
+    });
+}
+
+// ---- link prediction -----------------------------------------------------------------------------------------
+int hnhd_alg_link_loss(hnhd_alg_t *T, hnhd_dense_t *H_A, hnhd_dense_t *H_B, hnhd_dense_t *dH_A, hnhd_dense_t *dH_B,
+                       hnhd_vec_t *scores, double out[3]) {
+    return guarded([&] {
+        if (!T || !H_A || !H_B || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_link_loss: null argument");
+        const int64_t count = (int64_t)T->alg->S->dist_nnz;
+        VectorXd sums(2);
+        T->alg->linkLoss(H_A->m, H_B->m, count > 0 ? 1.0 / (double)count : 0.0, dH_A ? &dH_A->m : nullptr,
+                         dH_B ? &dH_B->m : nullptr, scores ? &scores->v : nullptr, sums.data());
+        double h[2];
+        cudaStream_t s = hnh::Runtime::get().compute_stream();
+        hnh::cuda_check(cudaMemcpyAsync(h, sums.data(), sizeof h, cudaMemcpyDeviceToHost, s), "link loss results");
+        hnh::cuda_check(cudaStreamSynchronize(s), "link loss results");
+        out[0] = count > 0 ? h[0] / (double)count : 0.0;
+        out[1] = h[1];
+        out[2] = (double)count;
+    });
+}
+int hnhd_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T, hnhd_link_targets_t **out) {
+    return guarded([&] {
+        if (!model || !T || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_link_targets_create: null argument");
+        std::unique_ptr<hnhd_link_targets> t(new hnhd_link_targets);
+        t->t.reset(new hnh::LinkTargets(*model->alg, *T->alg));
+        *out = t.release();
+    });
+}
+void hnhd_link_targets_destroy(hnhd_link_targets_t *t) { delete t; }
+int hnhd_gt_link_train_step(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double dropout, uint64_t seed,
+                            double out[4]) {
+    return guarded([&] {
+        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_link_train_step: null argument");
+        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o, dropout, seed), out);
+    });
+}
+int hnhd_gat_link_train_step(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]) {
+    return guarded([&] {
+        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_link_train_step: null argument");
+        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o), out);
+    });
+}
+static void link_out(const hnh::LinkResult &r, double out[3]) {
+    out[0] = r.loss;
+    out[1] = (double)r.correct;
+    out[2] = (double)r.count;
+}
+int hnhd_gt_link_evaluate(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
+    return guarded([&] {
+        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_link_evaluate: null argument");
+        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
+    });
+}
+int hnhd_gat_link_evaluate(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
+    return guarded([&] {
+        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_link_evaluate: null argument");
+        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
     });
 }
 

@@ -227,6 +227,27 @@ int hnh_cross_entropy_f64(double *dlogits, double *sums, const double *logits, c
     return rc ? rc : launch(gate_dw_final_kernel, 1, kBlock, st, "gate_dw_final_kernel", sums, (const double *)partial, chunks, (int64_t)2);
 }
 
+int64_t hnh_pair_sums_workspace_bytes(int64_t n) {
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_pair_sums_workspace_bytes: negative size");
+    return (int64_t)sizeof(double) * 2 * dw_chunks(n);
+}
+
+int hnh_pair_sums_f64(double *sums, const double *pairs, int64_t n, void *workspace, size_t workspace_bytes, void *stream) {
+    if (n < 0) return set_error(HNH_E_INVALID, "hnh_pair_sums_f64: negative size");
+    if (!sums) return set_error(HNH_E_INVALID, "hnh_pair_sums_f64: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) return hnh::check_cuda(cudaMemsetAsync(sums, 0, 2 * sizeof(double), st), "sums");
+    if (!pairs) return set_error(HNH_E_INVALID, "hnh_pair_sums_f64: null pointer");
+    const int64_t need = hnh_pair_sums_workspace_bytes(n);
+    if (!workspace || (int64_t)workspace_bytes < need)
+        return set_error(HNH_E_INVALID, "hnh_pair_sums_f64: the workspace needs %lld bytes", (long long)need);
+    double *partial = (double *)workspace;
+    const int64_t chunks = dw_chunks(n), chunk_rows = (n + chunks - 1) / chunks;
+    int rc = launch(cross_entropy_partial_kernel, (unsigned)((chunks * 32 + kBlock - 1) / kBlock), kBlock, st,
+                    "cross_entropy_partial_kernel", partial, pairs, n, chunks, chunk_rows);
+    return rc ? rc : launch(gate_dw_final_kernel, 1, kBlock, st, "gate_dw_final_kernel", sums, (const double *)partial, chunks, (int64_t)2);
+}
+
 int hnh_adamw_f64(double *param, double *m, double *v, const double *grad, int64_t n, double lr, double beta1, double beta2,
                   double eps, double weight_decay, double bias_correction1, double bias_correction2, const double *clip_coef,
                   void *stream) {

@@ -441,6 +441,21 @@ class Algorithm:
         check(lib().hnhd_alg_entry_coordinates(self.h, _value_order(mode), rows.h, cols.h), "entry_coordinates")
         return rows.to_host().astype(np.int64), cols.to_host().astype(np.int64)
 
+    def link_loss(self, H_A: Dense, H_B: Dense, dH_A: Dense | None = None, dH_B: Dense | None = None,
+                  scores: Vec | None = None):
+        """Link prediction on this algorithm object's S, the target matrix T (collective; Distributed_Sparse::linkLoss):
+        s_uv = <H_A[u], H_B[v]> for every stored (u, v) of T, with H_A A-shaped and H_B B-shaped (one Dense may be both),
+        and T's stored values the targets y_uv in [0, 1] (an SDDMM, SpMM or FusedMM on this object overwrites them).
+        Returns (loss, correct, count): the mean of F.binary_cross_entropy_with_logits(s, y) over T's entries on all
+        ranks, the entries with (s > 0) == (y > 0.5), and the entry count.  dH_A / dH_B (optional, the shapes of H_A /
+        H_B) are overwritten with the loss's gradients (one Dense passed as both receives their sum; a gradient may not
+        be an H); scores (optional, len(like_S_values())) receives s in the A order (entry_coordinates("A"))."""
+        out = (C.c_double * 3)()
+        check(lib().hnhd_alg_link_loss(self.h, self._dense_arg(H_A, "H_A"), self._dense_arg(H_B, "H_B"),
+                                       self._dense_arg(dH_A, "dH_A"), self._dense_arg(dH_B, "dH_B"),
+                                       self._vec_arg(scores, "scores"), out), "link_loss")
+        return float(out[0]), int(out[1]), int(out[2])
+
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
 
@@ -630,6 +645,21 @@ class GAT:
         check(lib().hnhd_gat_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "gat_train_step")
         return TrainStep._of(out)
 
+    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
+        """One collective link-prediction step on the device: forward, the mean binary cross-entropy of the dot-product
+        scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping and AdamW.
+        Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm).  The last layer keeps its ReLU (the
+        reference's formula), so GAT's scores are >= 0 and it cannot score a pair below 0.5: the graph transformer is
+        the model for link prediction."""
+        out = (C.c_double * 4)()
+        check(lib().hnhd_gat_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), out), "gat_link_train_step")
+        return TrainStep._of(out)
+
+    def link_evaluate(self, targets: "LinkTargets"):
+        """A forward pass and the link loss without gradients (collective): (loss, correct, count, scores), the scores a
+        numpy array in the order of targets.alg_T.entry_coordinates("A")."""
+        return _link_evaluate(lib().hnhd_gat_link_evaluate, self.h, targets, "gat_link_evaluate")
+
     def weight_grad(self, layer: int, head: int):
         """dL/d weight (layer, head), summed over all ranks."""
         out = np.empty(self.weight_shape(layer, head), dtype=np.float64)
@@ -776,6 +806,21 @@ class GraphTransformer:
         check(lib().hnhd_gt_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), p, sd, out), "gt_train_step")
         return TrainStep._of(out)
 
+    def link_train_step(self, targets: "LinkTargets", opt: "AdamW", dropout: float = 0.0, seed: int = 0) -> "TrainStep":
+        """One collective link-prediction step on the device: forward(dropout, seed), the mean binary cross-entropy of
+        the dot-product scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping
+        and AdamW.  Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        out = (C.c_double * 4)()
+        check(lib().hnhd_gt_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), p, sd, out),
+              "gt_link_train_step")
+        return TrainStep._of(out)
+
+    def link_evaluate(self, targets: "LinkTargets"):
+        """A forward pass without dropout and the link loss without gradients (collective): (loss, correct, count,
+        scores), the scores a numpy array in the order of targets.alg_T.entry_coordinates("A") -- for AUC or Hits@K."""
+        return _link_evaluate(lib().hnhd_gt_link_evaluate, self.h, targets, "gt_link_evaluate")
+
     def input_grad(self):
         """dL/d(network input), this rank's rows."""
         out = np.empty(self.buffer_shape(0), dtype=np.float64)
@@ -862,6 +907,42 @@ class AdamW:
             lib().hnhd_adamw_destroy(self.h)
         except Exception:
             pass
+
+
+class LinkTargets:
+    """The link-prediction targets of a model, on the device: alg_T is an Algorithm over the target matrix T, built
+    with the model's algorithm name and c over the same nodes (T is square, M = N = the model's S dimensions), whose
+    stored values are the targets y_uv in [0, 1] -- 1 for a positive pair, 0 for a negative one, soft targets allowed;
+    duplicates count.  Build T with SpmatLocal.from_tuples (e.g. with fresh negatives every epoch).  Collective: a T of
+    another layout, a T that is not square, or a target outside [0, 1] on any rank is refused on every rank.  The
+    model's and T's algorithm objects must outlive this one."""
+
+    def __init__(self, net, alg_T: Algorithm):
+        if not isinstance(alg_T, Algorithm):
+            raise TypeError(f"alg_T must be an Algorithm, not {type(alg_T).__name__}")
+        self.net, self.alg_T = net, alg_T
+        self.h = C.c_void_p()
+        check(lib().hnhd_link_targets_create(net.alg.h, alg_T.h, C.byref(self.h)), "link_targets_create")
+
+    def __del__(self):
+        try:
+            lib().hnhd_link_targets_destroy(self.h)
+        except Exception:
+            pass
+
+
+def _link_targets_arg(targets):
+    if not isinstance(targets, LinkTargets):
+        raise TypeError(f"targets must be a LinkTargets, not {type(targets).__name__}")
+    return targets.h
+
+
+def _link_evaluate(fn, h, targets, what):
+    t = _link_targets_arg(targets)
+    out = (C.c_double * 3)()
+    scores = Vec.create(0)
+    check(fn(h, t, scores.h, out), what)
+    return float(out[0]), int(out[1]), int(out[2]), scores.to_host()
 
 
 def _labels_arg(labels):

@@ -280,6 +280,29 @@ public:
     // of this rank's value vector of `order` (k_sddmmA: like_S_values, k_sddmmB: like_ST_values), as exact
     // doubles.  No communication.  Defined where check_full_rows passes; HNH_E_INVALID on every rank elsewhere.
     void entryCoordinates(KernelMode order, VectorXd &rows, VectorXd &cols);
+
+    // ---- link prediction: a dot-product edge decoder with binary cross-entropy -------------------------------------
+    // Called on the object of the target matrix T: its S holds the node pairs to score, its stored values y_uv in [0, 1]
+    // the targets (1 positive, 0 negative, soft targets allowed), as built -- an SDDMM, SpMM or FusedMM on this object
+    // overwrites its block values.  H_A (localArows x r) and H_B (localBrows x r) are the A- and B-shaped node
+    // embeddings; a model whose A and B rows are the same nodes passes its output buffer as both.  For every stored
+    // (u, v) of T (duplicates count):
+    //     s_uv = <H_A[u], H_B[v]>,  l_uv = max(s, 0) - s y + log1p(exp(-|s|)),  g_uv = (sigmoid(s_uv) - y_uv) inv_count,
+    // torch's F.binary_cross_entropy_with_logits per entry.  sums (device, 2 doubles) receives (sum l_uv, the number of
+    // entries with (s > 0) == (y > 0.5)) over all ranks, the same on every rank; dH_A (nullable) = sum_v g_uv H_B[v]
+    // and dH_B (nullable) = sum_u g_uv H_A[u], overwritten (the sum of both when they are one matrix); scores
+    // (nullable, an A-order vector: like_S_values) = s.  H_A and H_B may be one matrix.  One gather_pass in the A
+    // order (H_A, dH_A and the rows' loss and count on the stored-row side), a second in the B order only with dH_B;
+    // the row statistics are summed in a fixed order, then one world all-reduce of 2 doubles.  No atomics: repeated
+    // calls are bit-identical.  Collective; defined where check_full_rows passes.  HNH_E_INVALID on every rank before
+    // any launch for H_A / H_B that are not localArows / localBrows rows of one width r >= 1, a gradient of another
+    // shape or that is an H, scores of another length, a null sums or an inv_count that is not finite and >= 0.
+    void linkLoss(DenseMatrix &H_A, DenseMatrix &H_B, double inv_count, DenseMatrix *dH_A, DenseMatrix *dH_B,
+                  VectorXd *scores, double *sums);
+    // The number of stored entries of S over all ranks, after checking on the device that every stored value lies in
+    // [0, 1] (link targets).  Collective: one world all-reduce of 2 doubles; a value elsewhere (NaN and infinities
+    // included) on any rank is refused with HNH_E_INVALID on every rank.  Defined where check_full_rows passes.
+    int64_t linkTargetCount();
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

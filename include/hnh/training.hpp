@@ -9,6 +9,9 @@
 // all-reduces: one world all-reduce of 2 doubles (the loss sum and the correct count); the gradients are identical on
 // every rank after the backward, so the norm and the update need none.  Host traffic: 4 doubles down per step.
 //
+// Link prediction (LinkTargets, linkTrainStep, linkEvaluate, at the end) shares the step: its loss is the binary
+// cross-entropy of dot-product scores over the entries of a target matrix (Distributed_Sparse::linkLoss).
+//
 // Parameters are device spans read afresh at every step (set_weight may replace a matrix's storage), in a fixed order:
 //     GraphTransformer: each layer's params vector with its grads, one span per layer;
 //     GAT: every (layer, head) weight with its gradient, then a1 and a2 of every layer with theirs.  Where an attention
@@ -19,6 +22,7 @@
 #include <string>
 #include <vector>
 
+#include "hnh/15D_dense_shift.hpp"
 #include "hnh/comm.h"
 #include "hnh/gat.hpp"
 #include "hnh/graph_transformer.hpp"
@@ -187,12 +191,14 @@ inline void check_train(const DenseMatrix &out, const NodeLabels &labels, const 
                                        std::to_string(out.cols()) + " wide");
     opt.check_spans(spans);
 }
-// loss and dlogits, backward (by the caller's `backward`), clip and AdamW; then the 4 scalars to the host
-template <class Model, class Backward>
-TrainResult finishStep(Model &net, const NodeLabels &labels, AdamW &opt, Backward backward) {
+// the loss (by the caller's `loss`: the output buffer's gradient and the device sums (loss sum, correct) over all
+// ranks), backward (by the caller's `backward`), clip and AdamW; then the 4 scalars to the host.  count: the
+// denominator of the mean loss (labelled rows, or link targets).
+template <class Model, class Loss, class Backward>
+TrainResult finishStep(Model &net, int64_t count, AdamW &opt, Loss loss, Backward backward) {
     VectorXd stats(4);  // loss sum, correct, total norm, clip coefficient
     DenseMatrix dlogits;
-    crossEntropy(net.buffers.back(), labels, dlogits, stats.data());
+    loss(dlogits, stats.data());
     backward(dlogits);
     dlogits = DenseMatrix();
     opt.step(net.parameters(), stats.data() + 2);
@@ -201,7 +207,7 @@ TrainResult finishStep(Model &net, const NodeLabels &labels, AdamW &opt, Backwar
     cudaStream_t s = Runtime::get().compute_stream();
     cuda_check(cudaMemcpyAsync(h, stats.data(), sizeof h, cudaMemcpyDeviceToHost, s), "train step results");
     cuda_check(cudaStreamSynchronize(s), "train step results");
-    return {labels.labelled > 0 ? h[0] / (double)labels.labelled : 0.0, (int64_t)h[1], labels.labelled, h[2]};
+    return {count > 0 ? h[0] / (double)count : 0.0, (int64_t)h[1], count, h[2]};
 }
 }  // namespace detail
 
@@ -211,7 +217,9 @@ TrainResult finishStep(Model &net, const NodeLabels &labels, AdamW &opt, Backwar
 inline TrainResult trainStep(GraphTransformer &net, const NodeLabels &labels, AdamW &opt, double dropout, uint64_t seed) {
     detail::check_train(net.buffers.back(), labels, opt, net.parameters());
     net.forwardPass(dropout, seed);
-    return detail::finishStep(net, labels, opt, [&](const DenseMatrix &g) { net.backwardPass(g); });
+    return detail::finishStep(
+        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
 }
 
 // The same for GAT (no dropout).
@@ -219,7 +227,121 @@ inline TrainResult trainStep(GAT &net, const NodeLabels &labels, AdamW &opt) {
     detail::check_train(net.buffers.back(), labels, opt, net.parameters());
     net.check_backward_supported();
     net.forwardPass();
-    return detail::finishStep(net, labels, opt, [&](const DenseMatrix &g) { net.backwardPass(g); });
+    return detail::finishStep(
+        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
+// ---- link prediction ----------------------------------------------------------------------------------------------
+// The link targets of a model: T, a square sparse matrix over the model's nodes in its own algorithm object of the
+// model's layout (algorithm, fusion, p, c, M = N = the model's S dimensions, localArows, localBrows), so the dense row
+// partition is the model's.  T's stored values are the targets y_uv in [0, 1] (1 a positive pair, 0 a negative one,
+// soft targets allowed; duplicates count), as Distributed_Sparse::linkLoss reads them.  The loss is
+//     F.binary_cross_entropy_with_logits(s, y, reduction = "mean") over the stored entries of T on all ranks,
+// s_uv = <H_u, H_v> with H the model's output buffer (0 and a zero gradient when T has no entry anywhere), and the
+// correct count the entries with (s > 0) == (y > 0.5).  GAT's last layer keeps its ReLU (the reference's formula), so
+// its scores are >= 0: the graph transformer is the model for link prediction.  Collective: refuses, with
+// HNH_E_INVALID on every rank, a T of another layout, a T that is not square and a target outside [0, 1] on any rank
+// (a device check, then one world all-reduce of 2 doubles).  Both algorithm objects must outlive this one.
+class LinkTargets {
+public:
+    const Distributed_Sparse *model;
+    Distributed_Sparse *T;
+    int64_t count;     // stored entries of T over all ranks
+    double inv_count;  // 1 / count, 0 when T has no entry anywhere
+
+    LinkTargets(const Distributed_Sparse &model_ops, Distributed_Sparse &T_ops) : model(&model_ops), T(&T_ops) {
+        const string why = mismatch(model_ops, T_ops);
+        if (!why.empty()) throw Error(HNH_E_INVALID, "LinkTargets: " + why);
+        count = T_ops.linkTargetCount();
+        inv_count = count > 0 ? 1.0 / (double)count : 0.0;
+    }
+    // sums (device, 2 doubles) = (loss sum, correct count) over all ranks; dH (nullable, resized to H's shape) = dL/dH
+    // of the mean loss; scores (nullable, resized to T's A-order length) = s in the order of T's like_S_values
+    void loss(DenseMatrix &H, DenseMatrix *dH, VectorXd *scores, double *sums) const {
+        if (dH) dH->resize(H.rows(), H.cols());
+        if (scores) scores->resize(T->num_S_values());
+        T->linkLoss(H, H, inv_count, dH, dH, scores, sums);
+    }
+
+private:
+    static int fusion(const Distributed_Sparse &d) {
+        const Sparse15D_Dense_Shift *ds = dynamic_cast<const Sparse15D_Dense_Shift *>(&d);
+        return ds ? ds->fusionApproach : 0;
+    }
+    // why T's layout is not the model's ("" when it is); global quantities only, so every rank decides alike
+    static string mismatch(const Distributed_Sparse &m, const Distributed_Sparse &t) {
+        auto dims = [](const Distributed_Sparse &d) {
+            return std::to_string(d.p) + ", c = " + std::to_string(d.c) + ", " + std::to_string(d.M) + " x " + std::to_string(d.N) +
+                   ", local rows " + std::to_string(d.localArows) + " / " + std::to_string(d.localBrows);
+        };
+        if (t.algorithm_name != m.algorithm_name || fusion(t) != fusion(m) || t.p != m.p || t.c != m.c || t.M != m.M ||
+            t.N != m.N || t.localArows != m.localArows || t.localBrows != m.localBrows)
+            return "T's layout (" + t.algorithm_name + ", fusion " + std::to_string(fusion(t)) + ", p = " + dims(t) +
+                   ") is not the model's (" + m.algorithm_name + ", fusion " + std::to_string(fusion(m)) + ", p = " + dims(m) + ")";
+        if (t.M != t.N) return "T is " + std::to_string(t.M) + " x " + std::to_string(t.N) + "; link targets are square";
+        return "";
+    }
+};
+
+struct LinkResult {
+    double loss;  // mean over the stored entries of T on all ranks
+    int64_t correct, count;
+};
+
+namespace detail {
+// refusals every rank decides alike, before any launch
+inline void check_link(const Distributed_Sparse *ops, const LinkTargets &targets, const AdamW *opt, const std::vector<ParamSpan> &spans,
+                       const char *who) {
+    if (ops != targets.model) throw Error(HNH_E_INVALID, string(who) + ": the link targets were made for another model's algorithm object");
+    if (opt) opt->check_spans(spans);
+}
+inline LinkResult linkResult(DenseMatrix &H, const LinkTargets &targets, VectorXd *scores) {
+    VectorXd sums(2);
+    targets.loss(H, nullptr, scores, sums.data());
+    double h[2];
+    cudaStream_t s = Runtime::get().compute_stream();
+    cuda_check(cudaMemcpyAsync(h, sums.data(), sizeof h, cudaMemcpyDeviceToHost, s), "link results");
+    cuda_check(cudaStreamSynchronize(s), "link results");
+    return {targets.count > 0 ? h[0] / (double)targets.count : 0.0, (int64_t)h[1], targets.count};
+}
+}  // namespace detail
+
+// One link-prediction training step of the graph transformer: forward(dropout, seed), the mean binary cross-entropy of
+// the scores of T's entries (LinkTargets) with its gradient dH from Distributed_Sparse::linkLoss, backwardPass(dH),
+// clip and AdamW, as trainStep.  TrainResult's `labelled` is the entry count of T.  Collective.  Refuses, on every rank
+// before any launch, targets made for another model's algorithm object, an optimizer of other parameters and a layout
+// the model refuses.  Leaves the activations stale.
+inline TrainResult linkTrainStep(GraphTransformer &net, const LinkTargets &targets, AdamW &opt, double dropout, uint64_t seed) {
+    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
+    net.forwardPass(dropout, seed);
+    return detail::finishStep(
+        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
+// The same for GAT (no dropout).  Its last layer keeps its ReLU, so its scores are >= 0.
+inline TrainResult linkTrainStep(GAT &net, const LinkTargets &targets, AdamW &opt) {
+    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
+    net.check_backward_supported();
+    net.forwardPass();
+    return detail::finishStep(
+        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
+// A forward pass without dropout and the link loss without gradients: (mean loss, correct, count) over all ranks, and
+// scores (nullable, resized) = s in the order of T's like_S_values (Distributed_Sparse::entryCoordinates(k_sddmmA) of
+// T gives their node pairs).  Collective.
+inline LinkResult linkEvaluate(GraphTransformer &net, const LinkTargets &targets, VectorXd *scores) {
+    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
+    net.forwardPass(0.0, 0);
+    return detail::linkResult(net.buffers.back(), targets, scores);
+}
+inline LinkResult linkEvaluate(GAT &net, const LinkTargets &targets, VectorXd *scores) {
+    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
+    net.forwardPass();
+    return detail::linkResult(net.buffers.back(), targets, scores);
 }
 
 }  // namespace hnh

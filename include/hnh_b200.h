@@ -466,6 +466,26 @@ int hnh_adamw_f64(double *param, double *m, double *v, const double *grad, int64
  * total_coef[0] = sqrt(sum of squared_norms[0 .. count) in order), total_coef[1] = min(1, max_norm / (total + 1e-6)).
  * max_norm >= 0; +inf gives coef = 1. */
 int hnh_clip_coef_f64(double *total_coef, const double *squared_norms, int64_t count, double max_norm, void *stream);
+/* sums[j] = sum over i < n of pairs[2i + j], j = 0, 1 (n rows of 2 contiguous doubles), in the fixed two-stage order of
+ * hnh_cross_entropy_f64's sums, in a workspace of hnh_pair_sums_workspace_bytes(n) bytes.  n = 0 writes sums = 0. */
+int64_t hnh_pair_sums_workspace_bytes(int64_t n);
+int hnh_pair_sums_f64(double *sums, const double *pairs, int64_t n, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---- link prediction (Distributed_Sparse::linkLoss; csrc/link_prediction.cu) --------------------------------------
+ * The dot-product edge decoder with binary cross-entropy on one CSR block: X (rows x r, leading dimension ldx) is
+ * indexed by the stored row u, Y (ldy) gathered by col_idx v, and target[i] = y_uv is entry i's target.  Per entry:
+ *     s = <X_u, Y_v>,  loss = max(s, 0) - s y + log1p(exp(-|s|)),  correct = [(s > 0) == (y > 0.5)],
+ *     g = (sigmoid(s) - y) inv_count,
+ * and the nullable outputs: dX_u += sum_v g Y_v (lddx), stats[u * lds] += sum_v loss, stats[u * lds + 1] += sum_v
+ * correct (lds >= 2), scores[i] = s.  Rows without entries are not touched.  r >= 1, every leading dimension >= r (the
+ * stats' >= 2), inv_count finite and >= 0; an output may not be an input or another output.  Widths 4..256 (powers
+ * of two) with 16-byte aligned X, Y, dX and even leading dimensions take a row kernel with X_u in registers and
+ * 128-bit gathers; others a one-warp-per-row kernel.  No atomics: repeated calls are bit-identical. */
+int hnh_link_bce_f64(const int64_t *rowStart, const int64_t *col_idx, const double *target, int64_t rows, int64_t nnz,
+                     const double *X, int64_t ldx, const double *Y, int64_t ldy, int r, double inv_count, double *dX,
+                     int64_t lddx, double *stats, int64_t lds, double *scores, void *stream);
+/* bad[0] (device) += the number of target[0 .. n) that are not in [0, 1] (NaN and infinities count) */
+int hnh_link_target_check_f64(double *bad, const double *target, int64_t n, void *stream);
 
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of

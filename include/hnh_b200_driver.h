@@ -372,6 +372,36 @@ int hnhd_gt_train_step(hnhd_gt_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *
                        double out[4]);
 int hnhd_gat_train_step(hnhd_gat_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
 
+/* ---- link prediction: a dot-product edge decoder with binary cross-entropy (Distributed_Sparse::linkLoss) ---------
+ * On the algorithm object of a target matrix T (its stored values are the targets y_uv in [0, 1]; an SDDMM, SpMM or
+ * FusedMM on that object overwrites them): s_uv = <H_A[u], H_B[v]> for every stored (u, v), with H_A A-shaped and H_B
+ * B-shaped (one matrix may be both), and the mean of F.binary_cross_entropy_with_logits over T's entries on all ranks.
+ * out = {loss, correct, count}: the mean loss, the entries with (s > 0) == (y > 0.5), and T's entry count over all
+ * ranks (0 loss and gradient when there is none).  dH_A, dH_B (nullable) are overwritten with the gradients of the
+ * mean loss (the sum of both when they are one matrix); scores (nullable, of hnhd_vec_like(T, 0) length) = s in the A
+ * order.  The targets are not checked here (hnhd_link_targets_create does).  Collective; HNH_E_INVALID on every rank
+ * where hnhd_alg_edge_softmax is, and for mismatched shapes or a gradient that is an H. */
+int hnhd_alg_link_loss(hnhd_alg_t *T, hnhd_dense_t *H_A, hnhd_dense_t *H_B, hnhd_dense_t *dH_A, hnhd_dense_t *dH_B,
+                       hnhd_vec_t *scores, double out[3]);
+/* The link targets of a model (hnh::LinkTargets): T's algorithm object, of the model's layout (algorithm, fusion, p,
+ * c, M = N, local rows).  Collective; HNH_E_INVALID on every rank for another layout, a T that is not square or a
+ * target outside [0, 1] (NaN included) on any rank.  Both algorithm objects must outlive it. */
+typedef struct hnhd_link_targets hnhd_link_targets_t;
+int hnhd_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T, hnhd_link_targets_t **out);
+void hnhd_link_targets_destroy(hnhd_link_targets_t *t);
+/* One link-prediction training step: forward, the mean binary cross-entropy of the output buffer's dot-product scores
+ * over T's entries, the backward pass, clipping and AdamW.  out = {loss, correct, count, grad_norm}.  GAT's last layer
+ * keeps its ReLU, so its scores are >= 0: the graph transformer is the model for link prediction.  Collective;
+ * HNH_E_INVALID on every rank before any launch for targets of another model's algorithm object, an optimizer of
+ * other parameter sizes, and layouts without a backward pass. */
+int hnhd_gt_link_train_step(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double dropout, uint64_t seed,
+                            double out[4]);
+int hnhd_gat_link_train_step(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]);
+/* A forward pass without dropout and the link loss without gradients: out = {loss, correct, count}; scores (nullable)
+ * is resized and receives s in the A order of T (hnhd_alg_entry_coordinates(T, 0, ..) gives the pairs).  Collective. */
+int hnhd_gt_link_evaluate(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
+int hnhd_gat_link_evaluate(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
+
 #ifdef __cplusplus
 }
 #endif
