@@ -114,6 +114,10 @@ ABI = {
     "hnh_link_bce_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, _P, _I64, C.c_int, C.c_double, _P, _I64, _P, _I64, _P, _P]),
     "hnh_link_target_check_f64": (C.c_int, [_P, _P, _I64, _P]),
     "hnh_entry_coords_from_index_f64":(C.c_int, [_P, _P, _I64, _I64, _P]),
+    "hnh_max_aggregate_step_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, C.c_int, _P, _I64, _P, _I64, _P]),
+    "hnh_max_aggregate_finish_f64": (C.c_int, [_P, _P, _I64, _P]),
+    "hnh_max_aggregate_grad_scale_f64": (C.c_int, [_P, _P, _P, _I64, _P]),
+    "hnh_max_aggregate_grad_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -310,6 +314,23 @@ ABI.update({
     "hnhd_gat_link_train_step": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_gt_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_gat_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_alg_max_aggregate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_alg_max_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int]),
+    "hnhd_sage_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, _PP]),
+    "hnhd_sage_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_sage_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_sage_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_sage_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_sage_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_sage_set_input": (C.c_int, [_P, _P]),
+    "hnhd_sage_get_buffer": (C.c_int, [_P, C.c_int, _P]),
+    "hnhd_sage_forward": (C.c_int, [_P]),
+    "hnhd_sage_backward": (C.c_int, [_P, _P]),
+    "hnhd_sage_get_input_grad": (C.c_int, [_P, _P]),
+    "hnhd_sage_train_step": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_sage_link_train_step": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_sage_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_sage_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

@@ -1088,6 +1088,73 @@ int64_t Distributed_Sparse::linkTargetCount() {
     return (int64_t)x[1];
 }
 
+// ---- max aggregation -------------------------------------------------------------------------------------------------
+namespace {
+// the shape and aliasing checks of maxAggregate / maxAggregateBackward (every rank decides alike: shapes are local, but
+// a layout gives every rank the same widths and the caller passes the same matrices); returns f
+int64_t check_max_aggregate(const Distributed_Sparse &d, const string &who, const DenseMatrix &X,
+                            std::initializer_list<const DenseMatrix *> A_like, std::initializer_list<const DenseMatrix *> outs,
+                            const DenseMatrix *dX) {
+    const int64_t f = X.cols();
+    if (X.rows() != d.localBrows || f < 1 || f > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": X is " + to_string(X.rows()) + " x " + to_string(f) + "; like_B_matrix has " +
+                                            to_string(d.localBrows) + " rows and the width must be positive");
+    for (const DenseMatrix *m : A_like)
+        if (m->rows() != d.localArows || m->cols() != f)
+            throw hnh::Error(HNH_E_INVALID, who + ": an A-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                ", not localArows x f = " + to_string(d.localArows) + " x " + to_string(f));
+    if (dX && (dX->rows() != X.rows() || dX->cols() != f))
+        throw hnh::Error(HNH_E_INVALID, who + ": dX is " + to_string(dX->rows()) + " x " + to_string(dX->cols()) + ", X " +
+                                            to_string(X.rows()) + " x " + to_string(f));
+    vector<const DenseMatrix *> all{&X};
+    all.insert(all.end(), A_like.begin(), A_like.end());
+    if (dX) all.push_back(dX);
+    for (const DenseMatrix *o : outs) {
+        int same = 0;
+        for (const DenseMatrix *m : all) same += m == o || (o->size() > 0 && m->data() == o->data());
+        if (same != 1) throw hnh::Error(HNH_E_INVALID, who + ": an output may not be another operand of the call");
+    }
+    return f;
+}
+}  // namespace
+
+void Distributed_Sparse::maxAggregate(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C) {
+    const string who = "maxAggregate";
+    check_full_rows(who);
+    const int64_t f = check_max_aggregate(*this, who, X, {&Z, &C}, {&Z, &C}, nullptr);
+    Z.setConstant(-INFINITY);
+    C.setZero();
+    gather_pass(k_sddmmA, {{&Z, 0, f, true}, {&C, 0, f, true}}, {{&X, 0, f, false}},
+                [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, true, "maxAggregate");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_max_aggregate_step_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords, Y[0].p,
+                                                              Y[0].ld, (int)f, R[0].p, R[0].ld, R[1].p, R[1].ld, compute()),
+                                   "max_aggregate_step");
+                });
+    hnh::abi_check(hnh_max_aggregate_finish_f64(Z.data(), C.data(), Z.size(), compute()), "max_aggregate_finish");
+}
+
+void Distributed_Sparse::maxAggregateBackward(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C, DenseMatrix &dZ, DenseMatrix &dX,
+                                              bool accumulate) {
+    const string who = "maxAggregateBackward";
+    check_full_rows(who);
+    const int64_t f = check_max_aggregate(*this, who, X, {&Z, &C, &dZ}, {&dX}, &dX);
+    // G = dZ / C, 0 where C = 0: the share of dZ_u,k each tied entry gets
+    DenseMatrix G(localArows, f);
+    hnh::abi_check(hnh_max_aggregate_grad_scale_f64(G.data(), dZ.data(), C.data(), G.size(), compute()), "max_aggregate_grad_scale");
+    if (!accumulate) dX.setZero();
+    gather_pass(k_sddmmB, {{&Z, 0, f, false}, {&G, 0, f, false}}, {{&X, 0, f, false}, {&dX, 0, f, true}},
+                [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, false, "maxAggregateBackward");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_max_aggregate_grad_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords, R[0].p,
+                                                              R[0].ld, Y[0].p, Y[0].ld, Y[1].p, Y[1].ld, (int)f, R[1].p, R[1].ld,
+                                                              compute()),
+                                   "max_aggregate_grad");
+                });
+}
+
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {
     if (peer_ring_broken_ || !hnh::PeerRing::enabled() || world->size() < 2) return nullptr;
     auto key = std::make_pair(world.get(), bytes);

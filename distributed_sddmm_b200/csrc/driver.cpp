@@ -13,6 +13,7 @@
 #include "hnh/benchmark_dist.hpp"
 #include "hnh/distributed_sparse.h"
 #include "hnh/gat.hpp"
+#include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
 #include "hnh/training.hpp"
 #include "hnh_b200.h"
@@ -38,6 +39,9 @@ struct hnhd_gat {
 };
 struct hnhd_gt {
     std::unique_ptr<GraphTransformer> g;
+};
+struct hnhd_sage {
+    std::unique_ptr<GraphSAGE> g;
 };
 struct hnhd_labels {
     std::unique_ptr<hnh::NodeLabels> l;
@@ -950,5 +954,144 @@ int hnhd_gat_link_evaluate(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_vec
         link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
     });
 }
+
+// ---- max aggregation -------------------------------------------------------------------------------------------------
+int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C) {
+    return guarded([&] {
+        if (!a || !X || !Z || !C) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_max_aggregate: null argument");
+        a->alg->maxAggregate(X->m, Z->m, C->m);
+    });
+}
+int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C, hnhd_dense_t *dZ,
+                                    hnhd_dense_t *dX, int accumulate) {
+    return guarded([&] {
+        if (!a || !X || !Z || !C || !dZ || !dX) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_max_aggregate_backward: null argument");
+        a->alg->maxAggregateBackward(X->m, Z->m, C->m, dZ->m, dX->m, accumulate != 0);
+    });
+}
+
+// ---- GraphSAGE -------------------------------------------------------------------------------------------------------
+int hnhd_sage_create(hnhd_alg_t *a, int n_layers, const int *layers2, const char *aggr, hnhd_sage_t **out) {
+    return guarded([&] {
+        if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_create: bad argument");
+        vector<GraphSAGELayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
+        std::unique_ptr<hnhd_sage> g(new hnhd_sage);
+        g->g.reset(new GraphSAGE(layers, a->alg.get(), aggr));
+        *out = g.release();
+    });
+}
+// the parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
+static GtParam sage_param(hnhd_sage_t *g, int layer, const char *name) {
+    if (!g || !name) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: null argument");
+    GraphSAGE &m = *g->g;
+    if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no such layer");
+    const GraphSAGELayer &l = m.layers[(size_t)layer];
+    const int64_t f = l.input_features, r = l.output_features;
+    const string s = name;
+    if (s == "neigh") return {0, f, r};
+    if (s == "neigh_bias") return {f * r, r, 1};
+    if (s == "root") return {l.root_offset(), f, r};
+    throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no parameter \"" + s + "\" (neigh, neigh_bias or root)");
+}
+static DenseMatrix &sage_buffer(hnhd_sage_t *g, int buffer) {
+    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no such buffer");
+    return g->g->buffers[(size_t)buffer];
+}
+int hnhd_sage_param_shape(hnhd_sage_t *g, int layer, const char *name, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        const GtParam p = sage_param(g, layer, name);
+        if (rows) *rows = p.rows;
+        if (cols) *cols = p.cols;
+    });
+}
+int hnhd_sage_set_param(hnhd_sage_t *g, int layer, const char *name, const double *host) {
+    return guarded([&] {
+        const GtParam p = sage_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gt_copy(g->g->layers[(size_t)layer].params.data() + p.offset, host, p.rows * p.cols, cudaMemcpyHostToDevice);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_sage_get_param(hnhd_sage_t *g, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const GtParam p = sage_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gt_copy(host, g->g->layers[(size_t)layer].params.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_sage_get_param_grad(hnhd_sage_t *g, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const GtParam p = sage_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const GraphSAGELayer &l = g->g->layers[(size_t)layer];
+        if (l.grads.size() != l.params.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no backward pass has run");
+        gt_copy(host, l.grads.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_sage_buffer_shape(hnhd_sage_t *g, int buffer, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        DenseMatrix &b = sage_buffer(g, buffer);
+        if (rows) *rows = b.rows();
+        if (cols) *cols = b.cols();
+    });
+}
+int hnhd_sage_set_input(hnhd_sage_t *g, const double *host) {
+    return guarded([&] {
+        DenseMatrix &b = sage_buffer(g, 0);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        b.copy_from_host(host);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_sage_get_buffer(hnhd_sage_t *g, int buffer, double *host) {
+    return guarded([&] {
+        DenseMatrix &b = sage_buffer(g, buffer);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        b.copy_to_host(host);
+    });
+}
+int hnhd_sage_forward(hnhd_sage_t *g) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null GraphSAGE");
+        g->g->forwardPass();
+    });
+}
+int hnhd_sage_backward(hnhd_sage_t *g, const double *host_output_grad) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null GraphSAGE");
+        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const DenseMatrix &out = g->g->buffers.back();
+        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
+        g->g->backwardPass(grad);
+    });
+}
+int hnhd_sage_get_input_grad(hnhd_sage_t *g, double *host) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null GraphSAGE");
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no backward pass has run");
+        g->g->input_grad.copy_to_host(host);
+    });
+}
+int hnhd_sage_train_step(hnhd_sage_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]) {
+    return guarded([&] {
+        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_train_step: null argument");
+        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
+    });
+}
+int hnhd_sage_link_train_step(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]) {
+    return guarded([&] {
+        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_link_train_step: null argument");
+        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o), out);
+    });
+}
+int hnhd_sage_link_evaluate(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
+    return guarded([&] {
+        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_link_evaluate: null argument");
+        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
+    });
+}
+void hnhd_sage_destroy(hnhd_sage_t *g) { delete g; }
 
 }  // extern "C"

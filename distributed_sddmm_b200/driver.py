@@ -456,6 +456,24 @@ class Algorithm:
                                        self._vec_arg(scores, "scores"), out), "link_loss")
         return float(out[0]), int(out[1]), int(out[2])
 
+    def max_aggregate(self, X: Dense, Z: Dense, C: Dense):
+        """Collective: the SpMM over the (max, .) semiring (Distributed_Sparse::maxAggregate).  X is B-shaped, f wide;
+        Z and C (A-shaped, f wide: Dense.create(localArows, f)) are overwritten with Z_u,k = max_v X_v,k over the stored
+        entries (u, v) of S on all ranks (duplicates count; S's values are not read) and C_u,k = how many of them
+        attain it.  A row without entries gets Z = C = 0: torch's zeros(M, f).scatter_reduce(0, u, X[v], "amax",
+        include_self=False), PyG's MaxAggregation.  -0.0 and +0.0 tie; which of the two Z holds is not specified."""
+        check(lib().hnhd_alg_max_aggregate(self.h, self._dense_arg(X, "X"), self._dense_arg(Z, "Z"),
+                                           self._dense_arg(C, "C")), "max_aggregate")
+
+    def max_aggregate_backward(self, X: Dense, Z: Dense, C: Dense, dZ: Dense, dX: Dense, accumulate: bool = False):
+        """Collective: given the forward's Z and C and dZ = dLoss/dZ (A-shaped), dX (X's shape) is overwritten -- or,
+        with accumulate, added to -- with dX_v,k = sum_u [X_v,k == Z_u,k] dZ_u,k / C_u,k: tied entries share the
+        gradient equally, as torch's autograd of scatter_reduce "amax" (Distributed_Sparse::maxAggregateBackward)."""
+        check(lib().hnhd_alg_max_aggregate_backward(self.h, self._dense_arg(X, "X"), self._dense_arg(Z, "Z"),
+                                                    self._dense_arg(C, "C"), self._dense_arg(dZ, "dZ"),
+                                                    self._dense_arg(dX, "dX"), int(bool(accumulate))),
+              "max_aggregate_backward")
+
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
 
@@ -830,6 +848,123 @@ class GraphTransformer:
     def __del__(self):
         try:
             lib().hnhd_gt_destroy(self.h)
+        except Exception:
+            pass
+
+
+class GraphSAGE:
+    """GraphSAGE: layers of PyG's SAGEConv(aggr, root_weight=True, project=False, normalize=False), forward and backward
+    (include/hnh/graph_sage.hpp).  layers: [(input_features, output_features), ...]; aggr: "mean", "sum" or "max" over
+    the stored entries of each S-row on all ranks (duplicates count; a row without entries aggregates to 0).  Every
+    layer but the last ends in a ReLU, so the last layer's output is a valid link-prediction embedding.  The algorithm
+    object must outlive this one.
+
+    Parameters (zero after construction), by layer and name: "neigh" (input_features x r), "neigh_bias" (r) and
+    "root" (input_features x r).  A SAGEConv state dict maps onto them as lin_l.weight.T -> "neigh", lin_l.bias ->
+    "neigh_bias" and lin_r.weight.T -> "root"."""
+
+    AGGREGATIONS = ("mean", "sum", "max")
+    PARAMS = ("neigh", "neigh_bias", "root")
+
+    def __init__(self, alg: Algorithm, layers, aggr: str = "mean"):
+        self.alg = alg
+        self.layers = [tuple(int(x) for x in l) for l in layers]
+        if not self.layers or any(len(l) != 2 for l in self.layers):
+            raise ValueError("layers are a non-empty list of (input_features, output_features) pairs")
+        if aggr not in self.AGGREGATIONS:
+            raise ValueError(f"aggr = {aggr!r} must be one of {self.AGGREGATIONS}")
+        self.aggr = aggr
+        flat = (C.c_int * (2 * len(self.layers)))(*[x for l in self.layers for x in l])
+        self.h = C.c_void_p()
+        check(lib().hnhd_sage_create(alg.h, len(self.layers), flat, aggr.encode(), C.byref(self.h)), "sage_create")
+
+    def param_names(self):
+        return list(self.PARAMS)
+
+    def param_shape(self, layer: int, name: str):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_sage_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "sage_param_shape")
+        return (r.value,) if name == "neigh_bias" else (r.value, c.value)
+
+    def set_param(self, layer: int, name: str, value):
+        """Make the activations stale: the next backward pass needs a forward pass first."""
+        shape = self.param_shape(layer, name)
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        if v.shape != shape:
+            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
+        check(lib().hnhd_sage_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "sage_set_param")
+
+    def param(self, layer: int, name: str):
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        check(lib().hnhd_sage_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "sage_get_param")
+        return out
+
+    def param_grad(self, layer: int, name: str):
+        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        check(lib().hnhd_sage_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "sage_get_param_grad")
+        return out
+
+    def buffer_shape(self, i: int):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_sage_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "sage_buffer_shape")
+        return r.value, c.value
+
+    def set_input(self, x):
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.shape != self.buffer_shape(0):
+            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
+        check(lib().hnhd_sage_set_input(self.h, x.ctypes.data), "sage_set_input")
+
+    def buffer(self, i: int):
+        out = np.empty(self.buffer_shape(i), dtype=np.float64)
+        check(lib().hnhd_sage_get_buffer(self.h, int(i), out.ctypes.data), "sage_get_buffer")
+        return out
+
+    def forward(self):
+        """Collective."""
+        check(lib().hnhd_sage_forward(self.h), "sage_forward")
+
+    def backward(self, grad_out):
+        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the last set_param
+        / set_input; the gradients are then read with param_grad / input_grad."""
+        g = np.ascontiguousarray(grad_out, dtype=np.float64)
+        last = len(self.layers)
+        if g.shape != self.buffer_shape(last):
+            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
+        check(lib().hnhd_sage_backward(self.h, g.ctypes.data), "sage_backward")
+
+    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
+        """One collective training step on the device: forward, the mean cross-entropy of the output buffer against
+        labels over all ranks, backward, clipping and AdamW (see AdamW).  Returns TrainStep(loss, correct, labelled,
+        grad_norm)."""
+        out = (C.c_double * 4)()
+        check(lib().hnhd_sage_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "sage_train_step")
+        return TrainStep._of(out)
+
+    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
+        """One collective link-prediction step on the device: forward, the mean binary cross-entropy of the dot-product
+        scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping and AdamW.
+        Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
+        out = (C.c_double * 4)()
+        check(lib().hnhd_sage_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), out),
+              "sage_link_train_step")
+        return TrainStep._of(out)
+
+    def link_evaluate(self, targets: "LinkTargets"):
+        """A forward pass and the link loss without gradients (collective): (loss, correct, count, scores), the scores
+        a numpy array in the order of targets.alg_T.entry_coordinates("A")."""
+        return _link_evaluate(lib().hnhd_sage_link_evaluate, self.h, targets, "sage_link_evaluate")
+
+    def input_grad(self):
+        """dL/d(network input), this rank's rows."""
+        out = np.empty(self.buffer_shape(0), dtype=np.float64)
+        check(lib().hnhd_sage_get_input_grad(self.h, out.ctypes.data), "sage_get_input_grad")
+        return out
+
+    def __del__(self):
+        try:
+            lib().hnhd_sage_destroy(self.h)
         except Exception:
             pass
 

@@ -303,6 +303,28 @@ public:
     // [0, 1] (link targets).  Collective: one world all-reduce of 2 doubles; a value elsewhere (NaN and infinities
     // included) on any rank is refused with HNH_E_INVALID on every rank.  Defined where check_full_rows passes.
     int64_t linkTargetCount();
+
+    // ---- max aggregation: the SpMM over the (max, .) semiring (GraphSAGE's max aggregator) ---------------------------
+    // X (localBrows x f, the B-shaped operand: rows are S-columns v) is gathered over the stored entries (u, v) of S on
+    // all ranks (duplicates count; S's values are not read).  maxAggregate overwrites Z and C (localArows x f each):
+    //     Z_u,k = max_v X_v,k,   C_u,k = the number of stored entries of row u with X_v,k == Z_u,k,
+    // and Z = C = 0 on a row without entries -- torch's zeros(M, f).scatter_reduce(0, u, X[v], "amax",
+    // include_self = False), which is PyG's MaxAggregation.  -0.0 and +0.0 tie; which of the two Z holds is not
+    // specified.  NaN is not checked.  maxAggregateBackward, given the forward's Z and C and dZ (A-shaped), writes
+    //     dX_v,k = sum_u [X_v,k == Z_u,k] dZ_u,k / C_u,k
+    // (ties share the gradient equally), overwriting dX or, with `accumulate`, adding to it.  (torch's autograd of that
+    // scatter_reduce also counts the untouched zero of `self` as a tie where the maximum is exactly 0, and gives each
+    // entry dZ / (C + 1) there; this op splits dZ over the stored entries only.)  One gather_pass for the
+    // forward (A order: [Z | C] on the stored-row side, read-modify-written once per row and ring step, holding
+    // (-inf, 0) before it and finished elementwise after it), one for the backward (B order: X and dX on the stored-row
+    // side, [Z | dZ / C] gathered).  gather_pass never adds the written operands of a riding side: under replication
+    // reuse they ride the output ring from kernel to kernel and come home, and no layout where check_full_rows passes
+    // reduce-scatters.  The forward has no floating-point sum and no atomics: repeated calls are bit-identical, and so
+    // is the backward (sums in stored order).  Collective; defined where check_full_rows passes.  HNH_E_INVALID on every
+    // rank before any launch for an X that is not localBrows rows of width 1 <= f < 2^31, a Z, C or dZ that is not
+    // localArows x f, a dX that is not X's shape, or an output that is another operand of the call.
+    void maxAggregate(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C);
+    void maxAggregateBackward(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C, DenseMatrix &dZ, DenseMatrix &dX, bool accumulate);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

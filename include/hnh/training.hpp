@@ -13,7 +13,7 @@
 // cross-entropy of dot-product scores over the entries of a target matrix (Distributed_Sparse::linkLoss).
 //
 // Parameters are device spans read afresh at every step (set_weight may replace a matrix's storage), in a fixed order:
-//     GraphTransformer: each layer's params vector with its grads, one span per layer;
+//     GraphTransformer, GraphSAGE: each layer's params vector with its grads, one span per layer;
 //     GAT: every (layer, head) weight with its gradient, then a1 and a2 of every layer with theirs.  Where an attention
 //     kind does not read a1 or a2 their gradient is 0, and AdamW's decoupled decay alone moves them.
 #pragma once
@@ -25,6 +25,7 @@
 #include "hnh/15D_dense_shift.hpp"
 #include "hnh/comm.h"
 #include "hnh/gat.hpp"
+#include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
@@ -50,6 +51,13 @@ inline std::vector<ParamSpan> GAT::parameters() {
 inline std::vector<ParamSpan> GraphTransformer::parameters() {
     std::vector<ParamSpan> s;
     for (GraphTransformerLayer &l : layers)
+        s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
+    return s;
+}
+
+inline std::vector<ParamSpan> GraphSAGE::parameters() {
+    std::vector<ParamSpan> s;
+    for (GraphSAGELayer &l : layers)
         s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
     return s;
 }
@@ -232,6 +240,15 @@ inline TrainResult trainStep(GAT &net, const NodeLabels &labels, AdamW &opt) {
         [&](const DenseMatrix &g) { net.backwardPass(g); });
 }
 
+// The same for GraphSAGE (no dropout).
+inline TrainResult trainStep(GraphSAGE &net, const NodeLabels &labels, AdamW &opt) {
+    detail::check_train(net.buffers.back(), labels, opt, net.parameters());
+    net.forwardPass();
+    return detail::finishStep(
+        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
 // ---- link prediction ----------------------------------------------------------------------------------------------
 // The link targets of a model: T, a square sparse matrix over the model's nodes in its own algorithm object of the
 // model's layout (algorithm, fusion, p, c, M = N = the model's S dimensions, localArows, localBrows), so the dense row
@@ -330,6 +347,15 @@ inline TrainResult linkTrainStep(GAT &net, const LinkTargets &targets, AdamW &op
         [&](const DenseMatrix &g) { net.backwardPass(g); });
 }
 
+// The same for GraphSAGE (no dropout).  Its last layer has no ReLU, so its scores take either sign.
+inline TrainResult linkTrainStep(GraphSAGE &net, const LinkTargets &targets, AdamW &opt) {
+    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
+    net.forwardPass();
+    return detail::finishStep(
+        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
 // A forward pass without dropout and the link loss without gradients: (mean loss, correct, count) over all ranks, and
 // scores (nullable, resized) = s in the order of T's like_S_values (Distributed_Sparse::entryCoordinates(k_sddmmA) of
 // T gives their node pairs).  Collective.
@@ -339,6 +365,11 @@ inline LinkResult linkEvaluate(GraphTransformer &net, const LinkTargets &targets
     return detail::linkResult(net.buffers.back(), targets, scores);
 }
 inline LinkResult linkEvaluate(GAT &net, const LinkTargets &targets, VectorXd *scores) {
+    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
+    net.forwardPass();
+    return detail::linkResult(net.buffers.back(), targets, scores);
+}
+inline LinkResult linkEvaluate(GraphSAGE &net, const LinkTargets &targets, VectorXd *scores) {
     detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
     net.forwardPass();
     return detail::linkResult(net.buffers.back(), targets, scores);

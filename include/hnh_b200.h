@@ -487,6 +487,29 @@ int hnh_link_bce_f64(const int64_t *rowStart, const int64_t *col_idx, const doub
 /* bad[0] (device) += the number of target[0 .. n) that are not in [0, 1] (NaN and infinities count) */
 int hnh_link_target_check_f64(double *bad, const double *target, int64_t n, void *stream);
 
+/* ---- max aggregation (Distributed_Sparse::maxAggregate; csrc/graph_sage.cu) ----------------------------------------
+ * The SpMM over the (max, .) semiring on one CSR block, and its gradient.  S's values are not read; duplicates count.
+ * hnh_max_aggregate_step_f64: for every stored row u, over its entries v (X: gathered, leading dimension ldx),
+ *     (Z_u,k, C_u,k) = merge((Z_u,k, C_u,k), (max_v X_v,k, #{v : X_v,k == max}))
+ * where merge keeps the larger maximum and adds the counts of equal ones.  Z and C are read and written once per row
+ * (they may carry the state of earlier blocks); before the first block they hold (-inf, 0).  Rows without entries are
+ * not touched.  hnh_max_aggregate_finish_f64 then sets Z[i] = 0 where C[i] = 0 (n contiguous doubles).
+ * hnh_max_aggregate_grad_scale_f64: G[i] = dZ[i] / C[i], and 0 where C[i] = 0 (n contiguous doubles; G may be dZ).
+ * hnh_max_aggregate_grad_f64, on a block whose stored rows are X's (the B order): for every stored row v, over its
+ * entries u (Z, G gathered),
+ *     dX_v,k += sum_u [X_v,k == Z_u,k] G_u,k         (accumulated in stored order, then one read-modify-write of dX)
+ * f >= 1, every leading dimension >= f; outputs may not alias inputs.  Column windows of 256 run separately (max is
+ * independent per column); a window of width 4..256 (a power of two) with 16-byte aligned operands and even leading
+ * dimensions takes a row kernel with 128-bit gathers, others a one-warp-per-row kernel.  No atomics: repeated calls
+ * are bit-identical. */
+int hnh_max_aggregate_step_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, const double *X,
+                               int64_t ldx, int f, double *Z, int64_t ldz, double *C, int64_t ldc, void *stream);
+int hnh_max_aggregate_finish_f64(double *Z, const double *C, int64_t n, void *stream);
+int hnh_max_aggregate_grad_scale_f64(double *G, const double *dZ, const double *C, int64_t n, void *stream);
+int hnh_max_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, const double *X,
+                               int64_t ldx, const double *Z, int64_t ldz, const double *G, int64_t ldg, int f, double *dX,
+                               int64_t lddx, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

@@ -402,6 +402,44 @@ int hnhd_gat_link_train_step(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_a
 int hnhd_gt_link_evaluate(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
 int hnhd_gat_link_evaluate(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
 
+/* ---- GraphSAGE (include/hnh/graph_sage.hpp) ----------------------------------------------------------------------
+ * Layers of PyG's SAGEConv(aggr, root_weight = True): layers2 = {input_features, output_features} per layer; aggr is
+ * "mean", "sum" or "max".  Every layer but the last ends in a ReLU.  Parameters (zero after construction), by layer
+ * and name: "neigh" (input_features x r: lin_l.weight.T), "neigh_bias" (r x 1: lin_l.bias), "root" (input_features x
+ * r: lin_r.weight.T).  Buffers: 0 is the input (B-shaped), i + 1 the output of layer i (A-shaped).  set_param and
+ * set_input make the activations stale; get_param_grad reads dL/d param after hnhd_sage_backward, summed over all
+ * ranks.  Collective where the model's algorithm is; HNH_E_INVALID on every rank before any launch where
+ * hnhd_alg_edge_softmax is, for unknown aggregations, non-positive sizes, widths that do not chain, and a backward
+ * on stale activations.  The algorithm object must outlive the model. */
+typedef struct hnhd_sage hnhd_sage_t;
+int hnhd_sage_create(hnhd_alg_t *alg, int n_layers, const int *layers2, const char *aggr, hnhd_sage_t **out);
+int hnhd_sage_param_shape(hnhd_sage_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
+int hnhd_sage_set_param(hnhd_sage_t *g, int layer, const char *name, const double *host);
+int hnhd_sage_get_param(hnhd_sage_t *g, int layer, const char *name, double *host);
+int hnhd_sage_get_param_grad(hnhd_sage_t *g, int layer, const char *name, double *host);
+int hnhd_sage_buffer_shape(hnhd_sage_t *g, int buffer, int64_t *rows, int64_t *cols);
+int hnhd_sage_set_input(hnhd_sage_t *g, const double *host);
+int hnhd_sage_get_buffer(hnhd_sage_t *g, int buffer, double *host); /* synchronises */
+int hnhd_sage_forward(hnhd_sage_t *g);
+/* host_output_grad: dL/d(the last buffer), this rank's rows */
+int hnhd_sage_backward(hnhd_sage_t *g, const double *host_output_grad);
+/* dL/d buffer 0 (this rank's rows) after hnhd_sage_backward */
+int hnhd_sage_get_input_grad(hnhd_sage_t *g, double *host);
+/* hnhd_gt_train_step, hnhd_gt_link_train_step and hnhd_gt_link_evaluate for GraphSAGE (no dropout) */
+int hnhd_sage_train_step(hnhd_sage_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
+int hnhd_sage_link_train_step(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]);
+int hnhd_sage_link_evaluate(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
+void hnhd_sage_destroy(hnhd_sage_t *g);
+
+/* ---- max aggregation (Distributed_Sparse::maxAggregate) -------------------------------------------------------------
+ * Z, C (A-shaped, f wide) = the per-column maximum of X (B-shaped) over the stored entries of each S-row and the number
+ * of entries that attain it; Z = C = 0 on a row without entries.  The backward overwrites dX (or adds to it with
+ * accumulate != 0) with sum_u [X_v == Z_u] dZ_u / C_u.  Collective; HNH_E_INVALID on every rank where
+ * hnhd_alg_edge_softmax is, for wrong shapes, and for an output that is another operand. */
+int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C);
+int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C, hnhd_dense_t *dZ,
+                                    hnhd_dense_t *dX, int accumulate);
+
 #ifdef __cplusplus
 }
 #endif
