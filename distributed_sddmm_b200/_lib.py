@@ -118,6 +118,10 @@ ABI = {
     "hnh_max_aggregate_finish_f64": (C.c_int, [_P, _P, _I64, _P]),
     "hnh_max_aggregate_grad_scale_f64": (C.c_int, [_P, _P, _P, _I64, _P]),
     "hnh_max_aggregate_grad_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
+    "hnh_relational_aggregate_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
+    "hnh_relational_aggregate_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
+    "hnh_window_scale_f64": (C.c_int, [_P, _I64, _P, _I64, _I64, C.c_int, C.c_int, _P]),
+    "hnh_relation_check_f64": (C.c_int, [_P, _P, _I64, C.c_int, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -331,6 +335,23 @@ ABI.update({
     "hnhd_sage_link_train_step": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_sage_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_sage_destroy": (None, [_P]),
+    "hnhd_alg_relational_aggregate": (C.c_int, [_P, _P, _P, C.c_int]),
+    "hnhd_alg_relational_aggregate_backward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int]),
+    "hnhd_rgcn_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_char_p, _PP]),
+    "hnhd_rgcn_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_rgcn_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_rgcn_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_rgcn_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_rgcn_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_rgcn_set_input": (C.c_int, [_P, _P]),
+    "hnhd_rgcn_get_buffer": (C.c_int, [_P, C.c_int, _P]),
+    "hnhd_rgcn_forward": (C.c_int, [_P]),
+    "hnhd_rgcn_backward": (C.c_int, [_P, _P]),
+    "hnhd_rgcn_get_input_grad": (C.c_int, [_P, _P]),
+    "hnhd_rgcn_train_step": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_rgcn_link_train_step": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_rgcn_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_rgcn_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

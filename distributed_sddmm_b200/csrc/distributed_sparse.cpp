@@ -1155,6 +1155,88 @@ void Distributed_Sparse::maxAggregateBackward(DenseMatrix &X, DenseMatrix &Z, De
                 });
 }
 
+// ---- relational aggregation --------------------------------------------------------------------------------------------
+namespace {
+// the shape and aliasing checks of relationalAggregate / relationalAggregateBackward: X-shaped (localBrows x f) and
+// A-shaped (localArows x R f), distinct (every rank decides alike: a layout gives every rank the same widths)
+void check_relational(const Distributed_Sparse &d, const string &who, const DenseMatrix &X, const DenseMatrix &A, int num_relations) {
+    const int64_t f = X.cols();
+    if (num_relations < 1) throw hnh::Error(HNH_E_INVALID, who + ": the relation count must be positive, got " + to_string(num_relations));
+    if (X.rows() != d.localBrows || f < 1 || f * num_relations > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": the B-shaped operand is " + to_string(X.rows()) + " x " + to_string(f) +
+                                            "; like_B_matrix has " + to_string(d.localBrows) +
+                                            " rows and the width f must be positive with R f below 2^31");
+    if (A.rows() != d.localArows || A.cols() != f * num_relations)
+        throw hnh::Error(HNH_E_INVALID, who + ": the A-shaped operand is " + to_string(A.rows()) + " x " + to_string(A.cols()) +
+                                            ", not localArows x R f = " + to_string(d.localArows) + " x " + to_string(f * num_relations));
+    if (&A == &X || (A.size() > 0 && A.data() == X.data()))
+        throw hnh::Error(HNH_E_INVALID, who + ": an output may not be another operand of the call");
+}
+}  // namespace
+
+void Distributed_Sparse::relationalAggregate(DenseMatrix &X, DenseMatrix &A, int num_relations) {
+    const string who = "relationalAggregate";
+    check_full_rows(who);
+    check_relational(*this, who, X, A, num_relations);
+    const int64_t f = X.cols(), w = f * num_relations;
+    A.setZero();
+    gather_pass(k_sddmmA, {{&A, 0, w, true}}, {{&X, 0, f, false}},
+                [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, true, "relationalAggregate");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_relational_aggregate_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(), blk.rows,
+                                                                blk.num_coords, Y[0].p, Y[0].ld, (int)f, num_relations, R[0].p,
+                                                                R[0].ld, compute()),
+                                   "relational_aggregate");
+                });
+}
+
+void Distributed_Sparse::relationalAggregateBackward(DenseMatrix &dA, DenseMatrix &dX, int num_relations, bool accumulate) {
+    const string who = "relationalAggregateBackward";
+    check_full_rows(who);
+    check_relational(*this, who, dX, dA, num_relations);
+    const int64_t f = dX.cols(), w = f * num_relations;
+    if (!accumulate) dX.setZero();
+    gather_pass(k_sddmmB, {{&dA, 0, w, false}}, {{&dX, 0, f, true}},
+                [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, false, "relationalAggregateBackward");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_relational_aggregate_grad_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(),
+                                                                     blk.rows, blk.num_coords, Y[0].p, Y[0].ld, (int)f, num_relations,
+                                                                     R[0].p, R[0].ld, compute()),
+                                   "relational_aggregate_grad");
+                });
+}
+
+int64_t Distributed_Sparse::relationCheck(int num_relations) {
+    check_full_rows("relationCheck");
+    if (num_relations < 1)
+        throw hnh::Error(HNH_E_INVALID, "relationCheck: the relation count must be positive, got " + to_string(num_relations));
+    const int64_t n = num_S_values();
+    SpmatLocal &m = *values_matrix(*this, k_sddmmA);
+    VectorXd bad(1);
+    bad.setZero();
+    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
+        const int64_t nb = (int64_t)m.blockStarts[b + 1] - (int64_t)m.blockStarts[b];
+        if (nb == 0) continue;
+        CSRLocal *blk = m.csr_blocks[b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, "relationCheck: block " + to_string(b) + " does not match its value range");
+        hnh::abi_check(hnh_relation_check_f64(bad.data(), blk->getActive()->values.data(), nb, num_relations, compute()), "relation_check");
+    }
+    double mine = 0.0;
+    hnh::cuda_check(cudaMemcpyAsync(&mine, bad.data(), sizeof mine, cudaMemcpyDeviceToHost, compute()), "relation check");
+    hnh::cuda_check(cudaStreamSynchronize(compute()), "relation check");
+    double x[2] = {mine > 0.0 ? 1.0 : 0.0, (double)n};
+    hnh::Comm::world()->host_allreduce_sum_f64(x, 2);
+    if (mine > 0.0)
+        throw hnh::Error(HNH_E_INVALID, "relations: " + to_string((int64_t)mine) + " stored values of this rank are not integers in [0, " +
+                                            to_string(num_relations) + ")");
+    if (x[0] != 0.0)
+        throw hnh::Error(HNH_E_INVALID, "relations: another rank's stored values are not all integers in [0, " + to_string(num_relations) + ")");
+    return (int64_t)x[1];
+}
+
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {
     if (peer_ring_broken_ || !hnh::PeerRing::enabled() || world->size() < 2) return nullptr;
     auto key = std::make_pair(world.get(), bytes);

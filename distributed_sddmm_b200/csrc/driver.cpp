@@ -15,6 +15,7 @@
 #include "hnh/gat.hpp"
 #include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
+#include "hnh/rgcn.hpp"
 #include "hnh/training.hpp"
 #include "hnh_b200.h"
 #include "launch.h"
@@ -42,6 +43,9 @@ struct hnhd_gt {
 };
 struct hnhd_sage {
     std::unique_ptr<GraphSAGE> g;
+};
+struct hnhd_rgcn {
+    std::unique_ptr<RGCN> g;
 };
 struct hnhd_labels {
     std::unique_ptr<hnh::NodeLabels> l;
@@ -1093,5 +1097,148 @@ int hnhd_sage_link_evaluate(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_v
     });
 }
 void hnhd_sage_destroy(hnhd_sage_t *g) { delete g; }
+
+// ---- relational aggregation ------------------------------------------------------------------------------------------
+int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations) {
+    return guarded([&] {
+        if (!a || !X || !A) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_relational_aggregate: null argument");
+        a->alg->relationalAggregate(X->m, A->m, num_relations);
+    });
+}
+int hnhd_alg_relational_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dA, hnhd_dense_t *dX, int num_relations, int accumulate) {
+    return guarded([&] {
+        if (!a || !dA || !dX) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_relational_aggregate_backward: null argument");
+        a->alg->relationalAggregateBackward(dA->m, dX->m, num_relations, accumulate != 0);
+    });
+}
+
+// ---- R-GCN -----------------------------------------------------------------------------------------------------------
+int hnhd_rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, hnhd_rgcn_t **out) {
+    return guarded([&] {
+        if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_create: bad argument");
+        // refused before the device is touched
+        vector<std::pair<int, int>> widths;
+        for (int i = 0; i < n_layers; i++) widths.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
+        RGCN::parse(aggr);
+        RGCN::check_layers(widths, num_relations);
+        vector<RGCNLayer> layers;
+        for (auto [f, r] : widths) layers.emplace_back(f, r);
+        std::unique_ptr<hnhd_rgcn> g(new hnhd_rgcn);
+        g->g.reset(new RGCN(layers, a->alg.get(), num_relations, aggr));
+        *out = g.release();
+    });
+}
+// the parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
+static GtParam rgcn_param(hnhd_rgcn_t *g, int layer, const char *name) {
+    if (!g || !name) throw hnh::Error(HNH_E_INVALID, "RGCN: null argument");
+    RGCN &m = *g->g;
+    if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no such layer");
+    const RGCNLayer &l = m.layers[(size_t)layer];
+    const int64_t f = l.input_features, r = l.output_features, R = m.num_relations;
+    const string s = name;
+    if (s == "weight") return {0, R * f, r};
+    if (s == "bias") return {l.bias_offset(m.num_relations), r, 1};
+    if (s == "root") return {l.root_offset(m.num_relations), f, r};
+    throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + s + "\" (weight, bias or root)");
+}
+static DenseMatrix &rgcn_buffer(hnhd_rgcn_t *g, int buffer) {
+    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no such buffer");
+    return g->g->buffers[(size_t)buffer];
+}
+int hnhd_rgcn_param_shape(hnhd_rgcn_t *g, int layer, const char *name, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        const GtParam p = rgcn_param(g, layer, name);
+        if (rows) *rows = p.rows;
+        if (cols) *cols = p.cols;
+    });
+}
+int hnhd_rgcn_set_param(hnhd_rgcn_t *g, int layer, const char *name, const double *host) {
+    return guarded([&] {
+        const GtParam p = rgcn_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gt_copy(g->g->layers[(size_t)layer].params.data() + p.offset, host, p.rows * p.cols, cudaMemcpyHostToDevice);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_rgcn_get_param(hnhd_rgcn_t *g, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const GtParam p = rgcn_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gt_copy(host, g->g->layers[(size_t)layer].params.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_rgcn_get_param_grad(hnhd_rgcn_t *g, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const GtParam p = rgcn_param(g, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const RGCNLayer &l = g->g->layers[(size_t)layer];
+        if (l.grads.size() != l.params.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no backward pass has run");
+        gt_copy(host, l.grads.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_rgcn_buffer_shape(hnhd_rgcn_t *g, int buffer, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        DenseMatrix &b = rgcn_buffer(g, buffer);
+        if (rows) *rows = b.rows();
+        if (cols) *cols = b.cols();
+    });
+}
+int hnhd_rgcn_set_input(hnhd_rgcn_t *g, const double *host) {
+    return guarded([&] {
+        DenseMatrix &b = rgcn_buffer(g, 0);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        b.copy_from_host(host);
+        g->g->activations_current = false;
+    });
+}
+int hnhd_rgcn_get_buffer(hnhd_rgcn_t *g, int buffer, double *host) {
+    return guarded([&] {
+        DenseMatrix &b = rgcn_buffer(g, buffer);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        b.copy_to_host(host);
+    });
+}
+int hnhd_rgcn_forward(hnhd_rgcn_t *g) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null RGCN");
+        g->g->forwardPass();
+    });
+}
+int hnhd_rgcn_backward(hnhd_rgcn_t *g, const double *host_output_grad) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null RGCN");
+        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const DenseMatrix &out = g->g->buffers.back();
+        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
+        g->g->backwardPass(grad);
+    });
+}
+int hnhd_rgcn_get_input_grad(hnhd_rgcn_t *g, double *host) {
+    return guarded([&] {
+        if (!g) throw hnh::Error(HNH_E_INVALID, "null RGCN");
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no backward pass has run");
+        g->g->input_grad.copy_to_host(host);
+    });
+}
+int hnhd_rgcn_train_step(hnhd_rgcn_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]) {
+    return guarded([&] {
+        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_train_step: null argument");
+        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
+    });
+}
+int hnhd_rgcn_link_train_step(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]) {
+    return guarded([&] {
+        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_link_train_step: null argument");
+        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o), out);
+    });
+}
+int hnhd_rgcn_link_evaluate(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
+    return guarded([&] {
+        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_link_evaluate: null argument");
+        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
+    });
+}
+void hnhd_rgcn_destroy(hnhd_rgcn_t *g) { delete g; }
 
 }  // extern "C"

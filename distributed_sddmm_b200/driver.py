@@ -474,6 +474,24 @@ class Algorithm:
                                                     self._dense_arg(dX, "dX"), int(bool(accumulate))),
               "max_aggregate_backward")
 
+    def relational_aggregate(self, X: Dense, A: Dense, num_relations: int):
+        """Collective: R-GCN's aggregation (Distributed_Sparse::relationalAggregate).  The relation of each stored entry
+        (u, v) of S is its stored value (SpmatLocal.from_tuples' vals; an SDDMM, SpMM or FusedMM on this object
+        overwrites them), an integer in [0, num_relations).  X is B-shaped, f wide; A (A-shaped, num_relations * f wide:
+        Dense.create(localArows, R f)) is overwritten with A[u, rho f + k] = the sum of X[v, k] over the entries (u, v)
+        of relation rho on all ranks (duplicates count; 0 where there are none).  An entry whose value is not an integer
+        in [0, num_relations) -- negative, too large, fractional, infinite or NaN -- contributes nothing."""
+        check(lib().hnhd_alg_relational_aggregate(self.h, self._dense_arg(X, "X"), self._dense_arg(A, "A"),
+                                                  int(num_relations)), "relational_aggregate")
+
+    def relational_aggregate_backward(self, dA: Dense, dX: Dense, num_relations: int, accumulate: bool = False):
+        """Collective: given dA = dLoss/dA (A-shaped, R f wide), dX (B-shaped, f wide) is overwritten -- or, with
+        accumulate, added to -- with dX[v] = the sum of dA[u, rho f : rho f + f] over the stored entries (u, v), rho
+        their relation (Distributed_Sparse::relationalAggregateBackward)."""
+        check(lib().hnhd_alg_relational_aggregate_backward(self.h, self._dense_arg(dA, "dA"), self._dense_arg(dX, "dX"),
+                                                           int(num_relations), int(bool(accumulate))),
+              "relational_aggregate_backward")
+
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
 
@@ -965,6 +983,128 @@ class GraphSAGE:
     def __del__(self):
         try:
             lib().hnhd_sage_destroy(self.h)
+        except Exception:
+            pass
+
+
+class RGCN:
+    """R-GCN: layers of PyG's RGCNConv(in, out, num_relations, aggr, root_weight=True, bias=True) without basis or block
+    decomposition, forward and backward (include/hnh/rgcn.hpp).  The relation of each stored entry of the algorithm's S
+    is its stored value, an integer in [0, num_relations); construction refuses any other value on any rank.
+    layers: [(input_features, output_features), ...]; aggr: "mean" or "sum" over the entries of each (S-row, relation)
+    on all ranks (duplicates count; an empty one aggregates to 0).  Every layer but the last ends in a ReLU.  The
+    forward keeps num_relations * input_features doubles per row per layer.  The algorithm object must outlive this one.
+
+    Parameters (zero after construction), by layer and name: "weight" (num_relations * input_features x r), "bias" (r)
+    and "root" (input_features x r).  An RGCNConv state dict maps onto them as weight.reshape(-1, r) -> "weight",
+    bias -> "bias" and root -> "root", with no transpose."""
+
+    AGGREGATIONS = ("mean", "sum")
+    PARAMS = ("weight", "bias", "root")
+
+    def __init__(self, alg: Algorithm, layers, num_relations: int, aggr: str = "mean"):
+        self.alg = alg
+        self.layers = [tuple(int(x) for x in l) for l in layers]
+        if not self.layers or any(len(l) != 2 for l in self.layers):
+            raise ValueError("layers are a non-empty list of (input_features, output_features) pairs")
+        if any(a[1] != b[0] for a, b in zip(self.layers, self.layers[1:])):
+            raise ValueError(f"the layer widths {self.layers} do not chain")
+        if aggr not in self.AGGREGATIONS:
+            raise ValueError(f"aggr = {aggr!r} must be one of {self.AGGREGATIONS}")
+        if int(num_relations) < 1:
+            raise ValueError(f"num_relations = {num_relations} must be positive")
+        self.aggr, self.num_relations = aggr, int(num_relations)
+        flat = (C.c_int * (2 * len(self.layers)))(*[x for l in self.layers for x in l])
+        self.h = C.c_void_p()
+        check(lib().hnhd_rgcn_create(alg.h, len(self.layers), flat, self.num_relations, aggr.encode(), C.byref(self.h)),
+              "rgcn_create")
+
+    def param_names(self):
+        return list(self.PARAMS)
+
+    def param_shape(self, layer: int, name: str):
+        if name not in self.PARAMS:
+            raise ValueError(f"no parameter {name!r}: one of {self.PARAMS}")
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_rgcn_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "rgcn_param_shape")
+        return (r.value,) if name == "bias" else (r.value, c.value)
+
+    def set_param(self, layer: int, name: str, value):
+        """Make the activations stale: the next backward pass needs a forward pass first."""
+        shape = self.param_shape(layer, name)
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        if v.shape != shape:
+            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
+        check(lib().hnhd_rgcn_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "rgcn_set_param")
+
+    def param(self, layer: int, name: str):
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        check(lib().hnhd_rgcn_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "rgcn_get_param")
+        return out
+
+    def param_grad(self, layer: int, name: str):
+        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        check(lib().hnhd_rgcn_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "rgcn_get_param_grad")
+        return out
+
+    def buffer_shape(self, i: int):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_rgcn_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "rgcn_buffer_shape")
+        return r.value, c.value
+
+    def set_input(self, x):
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.shape != self.buffer_shape(0):
+            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
+        check(lib().hnhd_rgcn_set_input(self.h, x.ctypes.data), "rgcn_set_input")
+
+    def buffer(self, i: int):
+        out = np.empty(self.buffer_shape(i), dtype=np.float64)
+        check(lib().hnhd_rgcn_get_buffer(self.h, int(i), out.ctypes.data), "rgcn_get_buffer")
+        return out
+
+    def forward(self):
+        """Collective."""
+        check(lib().hnhd_rgcn_forward(self.h), "rgcn_forward")
+
+    def backward(self, grad_out):
+        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the last set_param
+        / set_input; the gradients are then read with param_grad / input_grad."""
+        g = np.ascontiguousarray(grad_out, dtype=np.float64)
+        last = len(self.layers)
+        if g.shape != self.buffer_shape(last):
+            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
+        check(lib().hnhd_rgcn_backward(self.h, g.ctypes.data), "rgcn_backward")
+
+    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
+        """One collective node-classification step on the device, as GraphSAGE.train_step."""
+        out = (C.c_double * 4)()
+        check(lib().hnhd_rgcn_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "rgcn_train_step")
+        return TrainStep._of(out)
+
+    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
+        """One collective link-prediction step on the device (the dot-product decoder on the output buffer), as
+        GraphSAGE.link_train_step."""
+        out = (C.c_double * 4)()
+        check(lib().hnhd_rgcn_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), out),
+              "rgcn_link_train_step")
+        return TrainStep._of(out)
+
+    def link_evaluate(self, targets: "LinkTargets"):
+        """A forward pass and the link loss without gradients (collective): (loss, correct, count, scores), the scores
+        a numpy array in the order of targets.alg_T.entry_coordinates("A")."""
+        return _link_evaluate(lib().hnhd_rgcn_link_evaluate, self.h, targets, "rgcn_link_evaluate")
+
+    def input_grad(self):
+        """dL/d(network input), this rank's rows."""
+        out = np.empty(self.buffer_shape(0), dtype=np.float64)
+        check(lib().hnhd_rgcn_get_input_grad(self.h, out.ctypes.data), "rgcn_get_input_grad")
+        return out
+
+    def __del__(self):
+        try:
+            lib().hnhd_rgcn_destroy(self.h)
         except Exception:
             pass
 

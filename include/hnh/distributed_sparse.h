@@ -325,6 +325,28 @@ public:
     // localArows x f, a dX that is not X's shape, or an output that is another operand of the call.
     void maxAggregate(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C);
     void maxAggregateBackward(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C, DenseMatrix &dZ, DenseMatrix &dX, bool accumulate);
+
+    // ---- relational aggregation (R-GCN): each stored entry's value picks the window its neighbour is summed into ------
+    // The relation of a stored entry (u, v) of S is its stored value (SpmatLocal::from_tuples' vals; an SDDMM or
+    // FusedMM on this object overwrites it), an integer in [0, num_relations).  An entry with any other value
+    // (negative, too large, fractional, infinite, NaN) contributes nothing.  relationalAggregate overwrites A
+    // (localArows x R f) with
+    //     A[u, rho f + k] = sum of X[v, k] over the stored entries (u, v) of relation rho on all ranks
+    // (duplicates count, each under its own relation; 0 where there are none), X being localBrows x f.
+    // relationalAggregateBackward, given dA (localArows x R f), writes
+    //     dX[v, k] = sum of dA[u, rho f + k] over the stored entries (u, v), rho their relation
+    // overwriting dX (localBrows x f) or, with `accumulate`, adding to it.  One gather_pass each: the forward in A
+    // order (A rides with the stored rows under replication reuse and accumulates across the ring steps), the backward
+    // in B order (dX with the stored rows, dA gathered: at c > 1 the all-gather carries R f columns).  Sums run in
+    // stored order without atomics: repeated calls are bit-identical.  Collective; defined where check_full_rows passes.
+    // HNH_E_INVALID on every rank before any launch for num_relations < 1, R f >= 2^31, wrong shapes, or an output that
+    // is another operand.
+    void relationalAggregate(DenseMatrix &X, DenseMatrix &A, int num_relations);
+    void relationalAggregateBackward(DenseMatrix &dA, DenseMatrix &dX, int num_relations, bool accumulate);
+    // The number of stored entries of S over all ranks, all of whose values are relations in [0, num_relations).
+    // Collective: one world all-reduce of 2 doubles; a value elsewhere on any rank is refused with HNH_E_INVALID on
+    // every rank.  Defined where check_full_rows passes.
+    int64_t relationCheck(int num_relations);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

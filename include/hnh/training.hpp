@@ -13,7 +13,7 @@
 // cross-entropy of dot-product scores over the entries of a target matrix (Distributed_Sparse::linkLoss).
 //
 // Parameters are device spans read afresh at every step (set_weight may replace a matrix's storage), in a fixed order:
-//     GraphTransformer, GraphSAGE: each layer's params vector with its grads, one span per layer;
+//     GraphTransformer, GraphSAGE, RGCN: each layer's params vector with its grads, one span per layer;
 //     GAT: every (layer, head) weight with its gradient, then a1 and a2 of every layer with theirs.  Where an attention
 //     kind does not read a1 or a2 their gradient is 0, and AdamW's decoupled decay alone moves them.
 #pragma once
@@ -27,6 +27,7 @@
 #include "hnh/gat.hpp"
 #include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
+#include "hnh/rgcn.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
 
@@ -58,6 +59,13 @@ inline std::vector<ParamSpan> GraphTransformer::parameters() {
 inline std::vector<ParamSpan> GraphSAGE::parameters() {
     std::vector<ParamSpan> s;
     for (GraphSAGELayer &l : layers)
+        s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
+    return s;
+}
+
+inline std::vector<ParamSpan> RGCN::parameters() {
+    std::vector<ParamSpan> s;
+    for (RGCNLayer &l : layers)
         s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
     return s;
 }
@@ -249,6 +257,15 @@ inline TrainResult trainStep(GraphSAGE &net, const NodeLabels &labels, AdamW &op
         [&](const DenseMatrix &g) { net.backwardPass(g); });
 }
 
+// The same for RGCN (no dropout).
+inline TrainResult trainStep(RGCN &net, const NodeLabels &labels, AdamW &opt) {
+    detail::check_train(net.buffers.back(), labels, opt, net.parameters());
+    net.forwardPass();
+    return detail::finishStep(
+        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
 // ---- link prediction ----------------------------------------------------------------------------------------------
 // The link targets of a model: T, a square sparse matrix over the model's nodes in its own algorithm object of the
 // model's layout (algorithm, fusion, p, c, M = N = the model's S dimensions, localArows, localBrows), so the dense row
@@ -356,6 +373,15 @@ inline TrainResult linkTrainStep(GraphSAGE &net, const LinkTargets &targets, Ada
         [&](const DenseMatrix &g) { net.backwardPass(g); });
 }
 
+// The same for RGCN (no dropout): the dot-product decoder on its embeddings.  Its last layer has no ReLU.
+inline TrainResult linkTrainStep(RGCN &net, const LinkTargets &targets, AdamW &opt) {
+    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
+    net.forwardPass();
+    return detail::finishStep(
+        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
+        [&](const DenseMatrix &g) { net.backwardPass(g); });
+}
+
 // A forward pass without dropout and the link loss without gradients: (mean loss, correct, count) over all ranks, and
 // scores (nullable, resized) = s in the order of T's like_S_values (Distributed_Sparse::entryCoordinates(k_sddmmA) of
 // T gives their node pairs).  Collective.
@@ -370,6 +396,12 @@ inline LinkResult linkEvaluate(GAT &net, const LinkTargets &targets, VectorXd *s
     return detail::linkResult(net.buffers.back(), targets, scores);
 }
 inline LinkResult linkEvaluate(GraphSAGE &net, const LinkTargets &targets, VectorXd *scores) {
+    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
+    net.forwardPass();
+    return detail::linkResult(net.buffers.back(), targets, scores);
+}
+
+inline LinkResult linkEvaluate(RGCN &net, const LinkTargets &targets, VectorXd *scores) {
     detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
     net.forwardPass();
     return detail::linkResult(net.buffers.back(), targets, scores);

@@ -510,6 +510,32 @@ int hnh_max_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, 
                                int64_t ldx, const double *Z, int64_t ldz, const double *G, int64_t ldg, int f, double *dX,
                                int64_t lddx, void *stream);
 
+/* ---- relational aggregation (Distributed_Sparse::relationalAggregate; csrc/rgcn.cu) ---------------------------------
+ * R-GCN's neighbour aggregation on one CSR block: the stored value of an entry is its relation rho, an integer in
+ * [0, R).  An entry whose value is anything else (negative, >= R, fractional, infinite, NaN) contributes nothing and
+ * its gathered row is not read.
+ * hnh_relational_aggregate_f64: for every stored row u and entry (v, rho) (X: gathered, leading dimension ldx),
+ *     A[u, rho f + k] += X[v, k]          (A is R f wide; the caller zeroes it before the first block)
+ * The relations present in a row are swept in increasing order, each one's entries summed in registers in stored order
+ * and added to the (row, relation) window with one read-modify-write; windows without entries are not touched.
+ * hnh_relational_aggregate_grad_f64, on a block whose stored rows are X's (the B order): for every stored row v and
+ * entry (u, rho) (dA gathered),
+ *     dX[v, k] += dA[u, rho f + k]         (accumulated in stored order, then one read-modify-write of dX)
+ * f >= 1, R >= 1, R f < 2^31, every leading dimension >= its operand's width; outputs may not alias inputs.  Column
+ * windows of 256 run separately; a window of width 4..256 (a power of two) with 16-byte aligned operands, even leading
+ * dimensions and an even f takes a row kernel with 128-bit gathers, others a one-warp-per-row kernel.  No atomics:
+ * repeated calls are bit-identical.
+ * hnh_window_scale_f64: A[u, rho f + k] = A[u, rho f + k] / C[u, rho], and 0 where C[u, rho] = 0, for u < n (the mean
+ * of R-GCN, forward and backward; C holds the per-(row, relation) entry counts).
+ * hnh_relation_check_f64: bad[0] (device) += the number of values[0 .. n) that are not integers in [0, R). */
+int hnh_relational_aggregate_f64(const int64_t *rowStart, const int64_t *col_idx, const double *values, int64_t rows, int64_t nnz,
+                                 const double *X, int64_t ldx, int f, int R, double *A, int64_t lda, void *stream);
+int hnh_relational_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const double *values, int64_t rows,
+                                      int64_t nnz, const double *dA, int64_t ldda, int f, int R, double *dX, int64_t lddx,
+                                      void *stream);
+int hnh_window_scale_f64(double *A, int64_t lda, const double *C, int64_t ldc, int64_t n, int f, int R, void *stream);
+int hnh_relation_check_f64(double *bad, const double *values, int64_t n, int R, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

@@ -440,6 +440,42 @@ int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd
 int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C, hnhd_dense_t *dZ,
                                     hnhd_dense_t *dX, int accumulate);
 
+/* ---- R-GCN (include/hnh/rgcn.hpp) ----------------------------------------------------------------------------------
+ * Layers of PyG's RGCNConv(in, out, num_relations, aggr, root_weight = True, bias = True) without basis or block
+ * decomposition: layers2 = {input_features, output_features} per layer; aggr is "mean" or "sum".  The relation of each
+ * stored entry of S is its stored value, an integer in [0, num_relations); create refuses any other value on any rank.
+ * Every layer but the last ends in a ReLU.  Parameters (zero after construction), by layer and name: "weight"
+ * (num_relations * input_features x r: RGCNConv.weight reshaped, no transpose), "bias" (r x 1), "root"
+ * (input_features x r).  Buffers, staleness and gradients as hnhd_sage_*.  Collective where the model's algorithm is;
+ * HNH_E_INVALID on every rank before any launch where hnhd_alg_edge_softmax is, for unknown aggregations,
+ * num_relations < 1, non-positive sizes, widths that do not chain, R f >= 2^31, and a backward on stale activations.
+ * The algorithm object must outlive the model. */
+typedef struct hnhd_rgcn hnhd_rgcn_t;
+int hnhd_rgcn_create(hnhd_alg_t *alg, int n_layers, const int *layers2, int num_relations, const char *aggr, hnhd_rgcn_t **out);
+int hnhd_rgcn_param_shape(hnhd_rgcn_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
+int hnhd_rgcn_set_param(hnhd_rgcn_t *g, int layer, const char *name, const double *host);
+int hnhd_rgcn_get_param(hnhd_rgcn_t *g, int layer, const char *name, double *host);
+int hnhd_rgcn_get_param_grad(hnhd_rgcn_t *g, int layer, const char *name, double *host);
+int hnhd_rgcn_buffer_shape(hnhd_rgcn_t *g, int buffer, int64_t *rows, int64_t *cols);
+int hnhd_rgcn_set_input(hnhd_rgcn_t *g, const double *host);
+int hnhd_rgcn_get_buffer(hnhd_rgcn_t *g, int buffer, double *host); /* synchronises */
+int hnhd_rgcn_forward(hnhd_rgcn_t *g);
+int hnhd_rgcn_backward(hnhd_rgcn_t *g, const double *host_output_grad);
+int hnhd_rgcn_get_input_grad(hnhd_rgcn_t *g, double *host);
+int hnhd_rgcn_train_step(hnhd_rgcn_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
+int hnhd_rgcn_link_train_step(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]);
+int hnhd_rgcn_link_evaluate(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
+void hnhd_rgcn_destroy(hnhd_rgcn_t *g);
+
+/* ---- relational aggregation (Distributed_Sparse::relationalAggregate) -----------------------------------------------
+ * A (A-shaped, num_relations * f wide) = for each S-row u and relation rho, the sum of X_v (B-shaped, f wide) over the
+ * stored entries (u, v) whose value is rho (0 where there are none; entries whose value is not an integer in
+ * [0, num_relations) count nowhere).  The backward overwrites dX (or adds to it with accumulate != 0) with
+ * dX_v = sum over the stored (u, v) of dA[u, rho f .. rho f + f).  Collective; HNH_E_INVALID on every rank where
+ * hnhd_alg_edge_softmax is, for num_relations < 1, wrong shapes, and for an output that is another operand. */
+int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations);
+int hnhd_alg_relational_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dA, hnhd_dense_t *dX, int num_relations, int accumulate);
+
 #ifdef __cplusplus
 }
 #endif
