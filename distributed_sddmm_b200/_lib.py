@@ -122,6 +122,11 @@ ABI = {
     "hnh_relational_aggregate_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_window_scale_f64": (C.c_int, [_P, _I64, _P, _I64, _I64, C.c_int, C.c_int, _P]),
     "hnh_relation_check_f64": (C.c_int, [_P, _P, _I64, C.c_int, _P]),
+    "hnh_basis_aggregate_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, _P, _I64, _P, C.c_int, C.c_int, _P, _I64,
+                                          _P]),
+    "hnh_basis_aggregate_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, C.c_int, C.c_int, _P, _I64,
+                                               C.c_int, _P, _I64, _P, _I64, _P]),
+    "hnh_relation_keys": (C.c_int, [_P, _P, _I64, C.c_int, _P]),
     "hnh_block_create_host": (C.c_int, [_P, _P, _I64, _I64, _I64, C.c_int, C.POINTER(_P)]),
     "hnh_block_destroy": (None, [_P]),
     "hnh_block_run_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
@@ -338,6 +343,9 @@ ABI.update({
     "hnhd_alg_relational_aggregate": (C.c_int, [_P, _P, _P, C.c_int]),
     "hnhd_alg_relational_aggregate_backward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int]),
     "hnhd_rgcn_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_char_p, _PP]),
+    "hnhd_rgcn_create_bases": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_char_p, _PP]),
+    "hnhd_alg_basis_aggregate": (C.c_int, [_P, _P, _P, _P, C.c_int, _P]),
+    "hnhd_alg_basis_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P, C.c_int]),
     "hnhd_rgcn_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "hnhd_rgcn_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
     "hnhd_rgcn_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),

@@ -1237,6 +1237,125 @@ int64_t Distributed_Sparse::relationCheck(int num_relations) {
     return (int64_t)x[1];
 }
 
+// ---- basis aggregation -----------------------------------------------------------------------------------------------
+namespace {
+// the shape and aliasing checks of basisAggregate / basisAggregateBackward: X-shaped (localBrows x f), A-shaped
+// (localArows x B f), comp and dcomp R x B, scale localArows x R; B = comp.cols()
+void check_basis(const Distributed_Sparse &d, const string &who, const vector<const DenseMatrix *> &X_like,
+                 const vector<const DenseMatrix *> &H_like, const DenseMatrix &comp, const DenseMatrix *dcomp, const DenseMatrix *scale,
+                 int num_relations, const vector<const DenseMatrix *> &outs) {
+    if (num_relations < 1) throw hnh::Error(HNH_E_INVALID, who + ": the relation count must be positive, got " + to_string(num_relations));
+    const int64_t B = comp.cols(), f = X_like.front()->cols();
+    if (B < 1) throw hnh::Error(HNH_E_INVALID, who + ": the basis count must be positive, got " + to_string(B));
+    if (comp.rows() != num_relations)
+        throw hnh::Error(HNH_E_INVALID, who + ": comp is " + to_string(comp.rows()) + " x " + to_string(B) + ", not R x B with R = " +
+                                            to_string(num_relations));
+    if (f < 1 || B * f > INT32_MAX || (int64_t)num_relations * B > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": the width f must be positive with B f and R B below 2^31 (f = " + to_string(f) +
+                                            ", B = " + to_string(B) + ")");
+    for (const DenseMatrix *m : X_like)
+        if (m->rows() != d.localBrows || m->cols() != f)
+            throw hnh::Error(HNH_E_INVALID, who + ": a B-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                ", not like_B_matrix's " + to_string(d.localBrows) + " rows of width f = " + to_string(f));
+    for (const DenseMatrix *m : H_like)
+        if (m->rows() != d.localArows || m->cols() != B * f)
+            throw hnh::Error(HNH_E_INVALID, who + ": an A-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                ", not localArows x B f = " + to_string(d.localArows) + " x " + to_string(B * f));
+    if (dcomp && (dcomp->rows() != num_relations || dcomp->cols() != B))
+        throw hnh::Error(HNH_E_INVALID, who + ": dcomp is " + to_string(dcomp->rows()) + " x " + to_string(dcomp->cols()) +
+                                            ", not R x B = " + to_string(num_relations) + " x " + to_string(B));
+    if (scale && (scale->rows() != d.localArows || scale->cols() != num_relations))
+        throw hnh::Error(HNH_E_INVALID, who + ": scale is " + to_string(scale->rows()) + " x " + to_string(scale->cols()) +
+                                            ", not localArows x R = " + to_string(d.localArows) + " x " + to_string(num_relations));
+    vector<const DenseMatrix *> all(X_like);
+    all.insert(all.end(), H_like.begin(), H_like.end());
+    all.push_back(&comp);
+    if (dcomp) all.push_back(dcomp);
+    if (scale) all.push_back(scale);
+    for (const DenseMatrix *o : outs) {
+        int same = 0;
+        for (const DenseMatrix *m : all) same += m == o || (o->size() > 0 && m->data() == o->data());
+        if (same != 1) throw hnh::Error(HNH_E_INVALID, who + ": an output may not be another operand of the call");
+    }
+}
+}  // namespace
+
+void Distributed_Sparse::basisAggregate(DenseMatrix &X, DenseMatrix &H, const DenseMatrix &comp, int num_relations,
+                                        const DenseMatrix *scale) {
+    const string who = "basisAggregate";
+    check_full_rows(who);
+    check_basis(*this, who, {&X}, {&H}, comp, nullptr, scale, num_relations, {&H});
+    const int64_t f = X.cols(), B = comp.cols();
+    H.setZero();
+    vector<PassOperand> A_side{{&H, 0, B * f, true}};
+    if (scale) A_side.push_back({const_cast<DenseMatrix *>(scale), 0, num_relations, false});
+    gather_pass(k_sddmmA, A_side, {{&X, 0, f, false}}, [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+        need_rows(rows_are_A, true, "basisAggregate");
+        CSRHandle *h = blk.getActive();
+        hnh::abi_check(hnh_basis_aggregate_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(), blk.rows, blk.num_coords,
+                                               Y[0].p, Y[0].ld, (int)f, scale ? R[1].p : nullptr, scale ? R[1].ld : 0, comp.data(),
+                                               num_relations, (int)B, R[0].p, R[0].ld, compute()),
+                       "basis_aggregate");
+    });
+}
+
+void Distributed_Sparse::basisAggregateBackward(DenseMatrix &dH, DenseMatrix &X, DenseMatrix &dX, const DenseMatrix &comp,
+                                                DenseMatrix &dcomp, int num_relations, const DenseMatrix *scale, bool accumulate) {
+    const string who = "basisAggregateBackward";
+    check_full_rows(who);
+    check_basis(*this, who, {&X, &dX}, {&dH}, comp, &dcomp, scale, num_relations, {&dX, &dcomp});
+    const int64_t f = X.cols(), B = comp.cols(), n = num_ST_values();
+    if (n >= INT32_MAX) throw hnh::Error(HNH_E_INVALID, who + ": " + to_string(n) + " local entries; at most 2^31 - 2");
+    if (!accumulate) dX.setZero();
+    // P[b n + j]: entry j's product for basis b, written block by block at the block's offset in the B-order values
+    SpmatLocal &m = *values_matrix(*this, k_sddmmB);
+    VectorXd P(std::max<int64_t>(n * B, 1));
+    vector<PassOperand> A_side{{&dH, 0, B * f, false}};
+    if (scale) A_side.push_back({const_cast<DenseMatrix *>(scale), 0, num_relations, false});
+    gather_pass(k_sddmmB, A_side, {{&X, 0, f, false}, {&dX, 0, f, true}},
+                [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, false, "basisAggregateBackward");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_basis_aggregate_grad_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(), blk.rows,
+                                                                blk.num_coords, Y[0].p, Y[0].ld, scale ? Y[1].p : nullptr,
+                                                                scale ? Y[1].ld : 0, comp.data(), num_relations, (int)B, R[0].p,
+                                                                R[0].ld, (int)f, R[1].p, R[1].ld,
+                                                                P.data() + (int64_t)m.blockStarts[(size_t)b], n, compute()),
+                                   "basis_aggregate_grad");
+                });
+    // dcomp: P summed by relation in the fixed order of an edge-softmax plan over R + 1 keys (key R: no relation)
+    const int64_t keys_n = (int64_t)num_relations + 1;
+    hnh::DeviceBuffer<int32_t> keys((size_t)std::max<int64_t>(n, 1)), perm((size_t)std::max<int64_t>(n, 1)),
+        row_start((size_t)keys_n + 1), piece_first((size_t)keys_n + 1);
+    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
+        const int64_t off = (int64_t)m.blockStarts[b], nb = (int64_t)m.blockStarts[b + 1] - off;
+        if (nb == 0) continue;
+        CSRLocal *blk = m.csr_blocks[b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, who + ": block " + to_string(b) + " does not match its value range");
+        hnh::abi_check(hnh_relation_keys(keys.data() + off, blk->getActive()->values.data(), nb, num_relations, compute()), "relation_keys");
+    }
+    const int64_t bound = hnh_edge_softmax_piece_bound(n, keys_n);
+    if (bound < 0) hnh::abi_check((int)bound, "edge_softmax_piece_bound");
+    hnh::DeviceBuffer<int32_t> piece_row((size_t)std::max<int64_t>(bound, 1));
+    int64_t pieces = 0;
+    hnh::abi_check(hnh_edge_softmax_plan(keys.data(), n, keys_n, perm.data(), row_start.data(), piece_first.data(), piece_row.data(),
+                                         (int64_t)piece_row.size(), &pieces, compute()),
+                   "edge_softmax_plan");
+    // sums[b (R + 1) + rho], then dcomp[rho, b] = sums[b (R + 1) + rho] for rho < R
+    VectorXd piece(std::max<int64_t>(pieces, 1)), sums(keys_n * B);
+    for (int64_t b = 0; b < B; b++)
+        hnh::abi_check(hnh_edge_sum_f64(P.data() + b * n, perm.data(), row_start.data(), piece_first.data(), piece_row.data(), keys_n,
+                                        pieces, piece.data(), sums.data() + b * keys_n, compute()),
+                       "edge_sum");
+    const size_t d = sizeof(double);
+    for (int64_t b = 0; b < B; b++)
+        hnh::cuda_check(cudaMemcpy2DAsync(dcomp.data() + b, d * (size_t)B, sums.data() + b * keys_n, d, d, (size_t)num_relations,
+                                          cudaMemcpyDeviceToDevice, compute()),
+                        "dcomp copy");
+    allreduce_rows(dcomp.data(), dcomp.size(), false);
+}
+
 hnh::PeerRing *Distributed_Sparse::peer_ring(std::shared_ptr<hnh::Comm> world, size_t bytes) {
     if (peer_ring_broken_ || !hnh::PeerRing::enabled() || world->size() < 2) return nullptr;
     auto key = std::make_pair(world.get(), bytes);

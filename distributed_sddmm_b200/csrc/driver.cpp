@@ -1112,7 +1112,44 @@ int hnhd_alg_relational_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dA, hnhd
     });
 }
 
+int hnhd_alg_basis_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *H, hnhd_dense_t *comp, int num_relations,
+                             hnhd_dense_t *scale) {
+    return guarded([&] {
+        if (!a || !X || !H || !comp) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_basis_aggregate: null argument");
+        a->alg->basisAggregate(X->m, H->m, comp->m, num_relations, scale ? &scale->m : nullptr);
+    });
+}
+int hnhd_alg_basis_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dH, hnhd_dense_t *X, hnhd_dense_t *dX, hnhd_dense_t *comp,
+                                      hnhd_dense_t *dcomp, int num_relations, hnhd_dense_t *scale, int accumulate) {
+    return guarded([&] {
+        if (!a || !dH || !X || !dX || !comp || !dcomp) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_basis_aggregate_backward: null argument");
+        a->alg->basisAggregateBackward(dH->m, X->m, dX->m, comp->m, dcomp->m, num_relations, scale ? &scale->m : nullptr,
+                                       accumulate != 0);
+    });
+}
+
 // ---- R-GCN -----------------------------------------------------------------------------------------------------------
+static int rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, int num_bases,
+                       hnhd_rgcn_t **out, const char *who) {
+    return guarded([&] {
+        if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, string(who) + ": bad argument");
+        // refused before the device is touched
+        vector<std::pair<int, int>> widths;
+        for (int i = 0; i < n_layers; i++) widths.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
+        RGCN::parse(aggr);
+        RGCN::check_layers(widths, num_relations, num_bases);
+        vector<RGCNLayer> layers;
+        for (auto [f, r] : widths) layers.emplace_back(f, r);
+        std::unique_ptr<hnhd_rgcn> g(new hnhd_rgcn);
+        g->g.reset(new RGCN(layers, a->alg.get(), num_relations, aggr, num_bases));
+        *out = g.release();
+    });
+}
+int hnhd_rgcn_create_bases(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, int num_bases, const char *aggr,
+                           hnhd_rgcn_t **out) {
+    if (num_bases < 1) return hnh::set_error(HNH_E_INVALID, "hnhd_rgcn_create_bases: the basis count must be positive (got %d)", num_bases);
+    return rgcn_create(a, n_layers, layers2, num_relations, aggr, num_bases, out, "hnhd_rgcn_create_bases");
+}
 int hnhd_rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, hnhd_rgcn_t **out) {
     return guarded([&] {
         if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_create: bad argument");
@@ -1134,11 +1171,13 @@ static GtParam rgcn_param(hnhd_rgcn_t *g, int layer, const char *name) {
     RGCN &m = *g->g;
     if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no such layer");
     const RGCNLayer &l = m.layers[(size_t)layer];
-    const int64_t f = l.input_features, r = l.output_features, R = m.num_relations;
+    const int64_t f = l.input_features, r = l.output_features, K = m.windows();
     const string s = name;
-    if (s == "weight") return {0, R * f, r};
-    if (s == "bias") return {l.bias_offset(m.num_relations), r, 1};
-    if (s == "root") return {l.root_offset(m.num_relations), f, r};
+    if (s == "weight") return {0, K * f, r};
+    if (s == "bias") return {l.bias_offset(m.windows()), r, 1};
+    if (s == "root") return {l.root_offset(m.windows()), f, r};
+    if (s == "comp" && m.num_bases > 0) return {m.comp_offset(l), m.num_relations, m.num_bases};
+    if (m.num_bases > 0) throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + s + "\" (weight, comp, bias or root)");
     throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + s + "\" (weight, bias or root)");
 }
 static DenseMatrix &rgcn_buffer(hnhd_rgcn_t *g, int buffer) {

@@ -492,6 +492,44 @@ class Algorithm:
                                                            int(num_relations), int(bool(accumulate))),
               "relational_aggregate_backward")
 
+    @staticmethod
+    def _comp_arg(comp):
+        """comp as a Dense: a Dense as it is, or an R x B array copied to the device."""
+        if isinstance(comp, Dense):
+            return comp
+        c = np.ascontiguousarray(comp, dtype=np.float64)
+        if c.ndim != 2 or c.shape[1] < 1:
+            raise ValueError(f"comp must be an R x B matrix with B >= 1, got shape {c.shape}")
+        d = Dense.create(c.shape[0], c.shape[1])
+        if c.size:
+            d.from_host(c)
+        return d
+
+    def basis_aggregate(self, X: Dense, H: Dense, comp, num_relations: int, scale: Dense | None = None):
+        """Collective: R-GCN's aggregation with basis decomposition (Distributed_Sparse::basisAggregate).  The relation
+        rho of each stored entry (u, v) of S is its stored value, as for relational_aggregate.  comp (R x B: a numpy
+        array or a Dense) mixes the relations into B bases; scale (optional Dense, A-shaped, num_relations wide) weighs
+        each (S-row, relation), e.g. 1 / |N_rho(u)| for the mean; without it every weight is 1.  X is B-shaped, f wide;
+        H (A-shaped, B f wide: Dense.create(localArows, B f)) is overwritten with
+        H[u, b f + k] = the sum of scale[u, rho] comp[rho, b] X[v, k] over the stored entries (u, v) on all ranks."""
+        args = (self._dense_arg(X, "X"), self._dense_arg(H, "H"), self._dense_arg(scale, "scale"))
+        c = self._comp_arg(comp)
+        check(lib().hnhd_alg_basis_aggregate(self.h, args[0], args[1], c.h, int(num_relations), args[2]), "basis_aggregate")
+
+    def basis_aggregate_backward(self, dH: Dense, X: Dense, dX: Dense, comp, num_relations: int, scale: Dense | None = None,
+                                 accumulate: bool = False):
+        """Collective: given dH = dLoss/dH (A-shaped, B f wide) and the forward's X, comp and scale, dX (B-shaped, f wide)
+        is overwritten -- or, with accumulate, added to -- with dX[v] = the sum of scale[u, rho] sum_b comp[rho, b]
+        dH[u, b f : b f + f] over the stored entries (u, v).  Returns dLoss/dcomp as an R x B numpy array, summed over
+        all ranks (the same on every rank): dcomp[rho, b] = the sum of scale[u, rho] <dH[u, b f : b f + f], X[v]> over
+        the stored entries of relation rho (Distributed_Sparse::basisAggregateBackward)."""
+        args = (self._dense_arg(dH, "dH"), self._dense_arg(X, "X"), self._dense_arg(dX, "dX"), self._dense_arg(scale, "scale"))
+        c = self._comp_arg(comp)
+        dcomp = Dense.create(max(int(num_relations), 0), c.shape[1])
+        check(lib().hnhd_alg_basis_aggregate_backward(self.h, args[0], args[1], args[2], c.h, dcomp.h, int(num_relations), args[3],
+                                                      int(bool(accumulate))), "basis_aggregate_backward")
+        return dcomp.to_host()
+
     def initial_shift(self, A, B, mode):
         self._op("initial_shift", A, B, aux=KMODE[mode])
 
@@ -988,21 +1026,25 @@ class GraphSAGE:
 
 
 class RGCN:
-    """R-GCN: layers of PyG's RGCNConv(in, out, num_relations, aggr, root_weight=True, bias=True) without basis or block
-    decomposition, forward and backward (include/hnh/rgcn.hpp).  The relation of each stored entry of the algorithm's S
-    is its stored value, an integer in [0, num_relations); construction refuses any other value on any rank.
-    layers: [(input_features, output_features), ...]; aggr: "mean" or "sum" over the entries of each (S-row, relation)
-    on all ranks (duplicates count; an empty one aggregates to 0).  Every layer but the last ends in a ReLU.  The
-    forward keeps num_relations * input_features doubles per row per layer.  The algorithm object must outlive this one.
+    """R-GCN: layers of PyG's RGCNConv(in, out, num_relations, num_bases, aggr, root_weight=True, bias=True) without
+    block decomposition, forward and backward (include/hnh/rgcn.hpp).  The relation of each stored entry of the
+    algorithm's S is its stored value, an integer in [0, num_relations); construction refuses any other value on any
+    rank.  layers: [(input_features, output_features), ...]; aggr: "mean" or "sum" over the entries of each (S-row,
+    relation) on all ranks (duplicates count; an empty one aggregates to 0).  Every layer but the last ends in a ReLU.
+    The forward keeps num_relations * input_features doubles per row per layer, or num_bases * input_features with
+    bases.  The algorithm object must outlive this one.
 
     Parameters (zero after construction), by layer and name: "weight" (num_relations * input_features x r), "bias" (r)
     and "root" (input_features x r).  An RGCNConv state dict maps onto them as weight.reshape(-1, r) -> "weight",
-    bias -> "bias" and root -> "root", with no transpose."""
+    bias -> "bias" and root -> "root", with no transpose.  With num_bases = B (W_rho = sum_b comp[rho, b] V_b),
+    "weight" is B * input_features x r (RGCNConv.weight.reshape(-1, r), the bases) and "comp" (num_relations x B) is
+    RGCNConv.comp."""
 
     AGGREGATIONS = ("mean", "sum")
     PARAMS = ("weight", "bias", "root")
+    BASIS_PARAMS = ("weight", "comp", "bias", "root")
 
-    def __init__(self, alg: Algorithm, layers, num_relations: int, aggr: str = "mean"):
+    def __init__(self, alg: Algorithm, layers, num_relations: int, aggr: str = "mean", num_bases: int | None = None):
         self.alg = alg
         self.layers = [tuple(int(x) for x in l) for l in layers]
         if not self.layers or any(len(l) != 2 for l in self.layers):
@@ -1013,18 +1055,28 @@ class RGCN:
             raise ValueError(f"aggr = {aggr!r} must be one of {self.AGGREGATIONS}")
         if int(num_relations) < 1:
             raise ValueError(f"num_relations = {num_relations} must be positive")
+        if num_bases is not None and int(num_bases) < 1:
+            raise ValueError(f"num_bases = {num_bases} must be positive (or None for no decomposition)")
         self.aggr, self.num_relations = aggr, int(num_relations)
+        self.num_bases = None if num_bases is None else int(num_bases)
         flat = (C.c_int * (2 * len(self.layers)))(*[x for l in self.layers for x in l])
         self.h = C.c_void_p()
-        check(lib().hnhd_rgcn_create(alg.h, len(self.layers), flat, self.num_relations, aggr.encode(), C.byref(self.h)),
-              "rgcn_create")
+        if self.num_bases is None:
+            check(lib().hnhd_rgcn_create(alg.h, len(self.layers), flat, self.num_relations, aggr.encode(), C.byref(self.h)),
+                  "rgcn_create")
+        else:
+            check(lib().hnhd_rgcn_create_bases(alg.h, len(self.layers), flat, self.num_relations, self.num_bases, aggr.encode(),
+                                               C.byref(self.h)), "rgcn_create_bases")
+
+    def _params(self):
+        return self.BASIS_PARAMS if getattr(self, "num_bases", None) else self.PARAMS
 
     def param_names(self):
-        return list(self.PARAMS)
+        return list(self._params())
 
     def param_shape(self, layer: int, name: str):
-        if name not in self.PARAMS:
-            raise ValueError(f"no parameter {name!r}: one of {self.PARAMS}")
+        if name not in self._params():
+            raise ValueError(f"no parameter {name!r}: one of {self._params()}")
         r, c = C.c_int64(), C.c_int64()
         check(lib().hnhd_rgcn_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "rgcn_param_shape")
         return (r.value,) if name == "bias" else (r.value, c.value)

@@ -347,6 +347,27 @@ public:
     // Collective: one world all-reduce of 2 doubles; a value elsewhere on any rank is refused with HNH_E_INVALID on
     // every rank.  Defined where check_full_rows passes.
     int64_t relationCheck(int num_relations);
+
+    // ---- basis aggregation (R-GCN with basis decomposition): one window per basis instead of one per relation ---------
+    // comp (R x B, every rank the same) mixes the relations into B bases; scale (nullable: all ones) is localArows x R,
+    // a weight per (S-row, relation) -- 1 / |N_rho(u)| for R-GCN's mean.  With rho the relation of a stored entry as for
+    // relationalAggregate (an entry that is no relation contributes nothing), basisAggregate overwrites H
+    // (localArows x B f) with
+    //     H[u, b f + k] = sum over the stored entries (u, v) on all ranks of scale[u, rho] comp[rho, b] X[v, k]
+    // X being localBrows x f.  basisAggregateBackward, given dH (localArows x B f), writes
+    //     dX[v, k] = sum over the stored entries (u, v) of scale[u, rho] sum_b comp[rho, b] dH[u, b f + k]
+    // overwriting dX (localBrows x f) or, with `accumulate`, adding to it, and overwrites dcomp (R x B) with
+    //     dcomp[rho, b] = sum over the stored entries of relation rho on all ranks of scale[u, rho] <dH[u, b f ..], X[v]>
+    // the same on every rank.  One gather_pass each: the forward in A order (H and scale with the stored rows, X
+    // gathered), the backward in B order (X and dX with the stored rows, dH and scale gathered) whose kernel also writes
+    // every local entry's B products; these are summed by relation with an edge-softmax plan keyed by relation, built
+    // per call (relations are S's values, which an SDDMM may overwrite), then one world all-reduce of R B doubles.  No
+    // atomics: repeated calls are bit-identical.  Collective; defined where check_full_rows passes.  HNH_E_INVALID on
+    // every rank before any launch for num_relations < 1, B < 1, B f or R B >= 2^31, wrong shapes, or an output that is
+    // another operand.
+    void basisAggregate(DenseMatrix &X, DenseMatrix &H, const DenseMatrix &comp, int num_relations, const DenseMatrix *scale);
+    void basisAggregateBackward(DenseMatrix &dH, DenseMatrix &X, DenseMatrix &dX, const DenseMatrix &comp, DenseMatrix &dcomp,
+                                int num_relations, const DenseMatrix *scale, bool accumulate);
     // frees what edgeSoftmax keeps for this object (the destructor calls it)
     void release_edge_softmax();
 

@@ -1,6 +1,6 @@
-// hnh/rgcn.hpp -- R-GCN: layers of PyG's RGCNConv(in, out, num_relations = R, aggr, root_weight = True, bias = True)
-// without basis or block decomposition, with the mean or sum aggregator, forward and backward, with the weight
-// gradients summed over all ranks.
+// hnh/rgcn.hpp -- R-GCN: layers of PyG's RGCNConv(in, out, num_relations = R, num_bases = B, aggr, root_weight = True,
+// bias = True), without decomposition or with basis decomposition, with the mean or sum aggregator, forward and backward,
+// with the weight gradients summed over all ranks.
 //
 // The relation of a stored entry (u, v) of S is its stored value (Distributed_Sparse::relationalAggregate), an integer
 // in [0, R); the constructor refuses any other value on any rank.  Layer l has input width f and output width r.  With
@@ -24,6 +24,17 @@
 // Parameters of a layer live in one device vector, in the order of its gradients: [W_0; ...; W_{R-1}; b]
 // ((R f + 1) x r), then W_root (f x r).  All are zero after construction.  A PyG RGCNConv state dict maps onto them as
 // weight.reshape(R f, r) -> "weight", bias -> "bias", root -> "root", with no transpose.
+//
+// With B >= 1 bases, W_rho = sum_b comp[rho, b] V_b (PyG's num_bases = B), and the aggregation writes one window per
+// basis instead of one per relation (Distributed_Sparse::basisAggregate), so memory and traffic depend on B, not R:
+//     H[u, b] = sum_{(u, v) stored} w(u, rho_uv) comp[rho_uv, b] X_v,   w = 1 / |N_rho(u)| (mean) or 1 (sum)
+//     Y = [H_0 | ... | H_{B-1}] [V_0; ...; V_{B-1}] + X W_root + b
+// The mean's weights 1 / |N_rho(u)| (0 where the count is 0) are computed once per model from the same counts.  The
+// forward keeps H (B f doubles per row per layer).  The backward computes dV = H^T dY, db and dW_root as above,
+// dH = dY [V_0; ...]^T, and dX = dY W_root^T + basisAggregateBackward(dH), which also gives dcomp already summed over
+// all ranks; the all-reduce of the layer's other gradients follows.  The parameter vector is [V_0; ...; V_{B-1}; b]
+// ((B f + 1) x r), W_root (f x r), then comp (R x B), so that the all-reduce covers the prefix before comp.  PyG's
+// RGCNConv(num_bases = B) maps onto it as weight.reshape(B f, r) -> "weight", comp -> "comp", bias, root.
 //
 // Defined where Distributed_Sparse::check_full_rows passes (every rank holds full-width rows and the A and B layouts
 // coincide); elsewhere the constructor throws HNH_E_INVALID on every rank before any launch.
@@ -61,18 +72,23 @@ public:
     const int num_relations;
     vector<DenseMatrix> buffers;  // [0] network input (B-shaped), [i + 1] output of layer i (A-shaped)
     const Aggregation aggr;
-    vector<DenseMatrix> aggregated;  // Ab of every layer from the last forward pass (localArows x R f)
+    vector<DenseMatrix> aggregated;  // Ab (localArows x R f), or H with bases (localArows x B f), of every layer
     DenseMatrix input_grad;          // dL/d buffers[0] after backwardPass
     // The activations belong to the current parameters and input: forwardPass sets it, whoever changes one of them
     // clears it, and backwardPass refuses to run on stale activations.
     bool activations_current = false;
+    const int num_bases;  // B >= 1: basis decomposition; 0: none
 
     // aggr: "mean" or "sum".  Collective: checks every stored value of S (Distributed_Sparse::relationCheck).
     RGCN(vector<RGCNLayer> &l_input, Distributed_Sparse *ops, int relations, const string &aggregation)
-        : d_ops(ops), layers(l_input), num_relations(relations), aggr(parse(aggregation)) {
+        : RGCN(l_input, ops, relations, aggregation, 0) {}
+
+    // The same with `bases` bases (0: without decomposition, as above).
+    RGCN(vector<RGCNLayer> &l_input, Distributed_Sparse *ops, int relations, const string &aggregation, int bases)
+        : d_ops(ops), layers(l_input), num_relations(relations), aggr(parse(aggregation)), num_bases(bases) {
         vector<std::pair<int, int>> widths;
         for (const RGCNLayer &l : layers) widths.emplace_back(l.input_features, l.output_features);
-        check_layers(widths, num_relations);
+        check_layers(widths, num_relations, num_bases);
         d_ops->check_full_rows("RGCN");
         if (d_ops->localArows != d_ops->localBrows) throw hnh::Error(HNH_E_INVALID, "RGCN: the A and B layouts hold different rows");
         d_ops->relationCheck(num_relations);
@@ -81,7 +97,7 @@ public:
         for (RGCNLayer &layer : layers) {
             d_ops->setRValue(layer.output_features);
             buffers.push_back(d_ops->like_A_matrix(0.0));
-            layer.params = VectorXd::Constant(layer.param_count(num_relations), 0.0);
+            layer.params = VectorXd::Constant(param_count(layer), 0.0);
         }
         ones = DenseMatrix::Constant(d_ops->localArows, 1, 1.0);
         if (aggr == kMean) {
@@ -89,19 +105,30 @@ public:
             DenseMatrix one_col = DenseMatrix::Constant(d_ops->localBrows, 1, 1.0);
             counts.resize(d_ops->localArows, num_relations);
             d_ops->relationalAggregate(one_col, counts, num_relations);
+            if (num_bases > 0) {
+                // basisAggregate's scale: 1 / |N_rho(u)|, 0 where the count is 0
+                DenseMatrix inv = DenseMatrix::Constant(d_ops->localArows, num_relations, 1.0);
+                hnh::abi_check(hnh_max_aggregate_grad_scale_f64(inv.data(), inv.data(), counts.data(), inv.size(), stream()),
+                               "max_aggregate_grad_scale");
+                counts.take(inv);
+            }
         }
     }
 
-    // the checks that need no device, on the (input, output) widths of the layers: a relation count >= 1 and positive
-    // widths that chain, R f < 2^31
-    static void check_layers(const vector<std::pair<int, int>> &widths, int num_relations) {
+    // the checks that need no device, on the (input, output) widths of the layers: a relation count >= 1, a basis count
+    // >= 0, positive widths that chain, R f < 2^31, and with bases B f and R B < 2^31
+    static void check_layers(const vector<std::pair<int, int>> &widths, int num_relations, int num_bases = 0) {
         if (widths.empty()) throw hnh::Error(HNH_E_INVALID, "RGCN: no layers");
         if (num_relations < 1) throw hnh::Error(HNH_E_INVALID, "RGCN: the relation count must be positive");
+        if (num_bases < 0) throw hnh::Error(HNH_E_INVALID, "RGCN: the basis count must not be negative");
+        if ((int64_t)num_relations * num_bases > INT32_MAX) throw hnh::Error(HNH_E_INVALID, "RGCN: R B must be below 2^31");
         for (size_t i = 0; i < widths.size(); i++) {
             const auto [f, r] = widths[i];
             if (f <= 0 || r <= 0) throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + ": sizes must be positive");
-            if ((int64_t)num_relations * f > INT32_MAX)
+            if (num_bases == 0 && (int64_t)num_relations * f > INT32_MAX)
                 throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + ": R f must be below 2^31");
+            if ((int64_t)num_bases * f > INT32_MAX)
+                throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + ": B f must be below 2^31");
             if (i > 0 && f != widths[i - 1].second)
                 throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + " does not take the width layer " +
                                                     std::to_string(i - 1) + " produces");
@@ -114,15 +141,25 @@ public:
         throw hnh::Error(HNH_E_INVALID, "RGCN: unknown aggregation \"" + a + "\" (mean or sum)");
     }
 
-    // [W_0; ...; W_{R-1}] (R f x r), b (1 x r) and W_root (f x r) of a layer's params or grads, as views
+    // the aggregation's windows per row: B with bases, else R
+    int windows() const { return num_bases > 0 ? num_bases : num_relations; }
+    // where comp (R x B) starts in a layer's params and grads, and their length
+    int64_t comp_offset(const RGCNLayer &l) const { return l.param_count(windows()); }
+    int64_t param_count(const RGCNLayer &l) const { return comp_offset(l) + (int64_t)num_relations * num_bases; }
+
+    // [W_0; ...; W_{R-1}] (R f x r) or [V_0; ...; V_{B-1}] (B f x r), b (1 x r), W_root (f x r) and comp (R x B) of a
+    // layer's params or grads, as views
     DenseMatrix weight(VectorXd &v, const RGCNLayer &l) const {
-        return DenseMatrix::view(v.data(), (int64_t)num_relations * l.input_features, l.output_features);
+        return DenseMatrix::view(v.data(), (int64_t)windows() * l.input_features, l.output_features);
     }
     DenseMatrix bias(VectorXd &v, const RGCNLayer &l) const {
-        return DenseMatrix::view(v.data() + l.bias_offset(num_relations), 1, l.output_features);
+        return DenseMatrix::view(v.data() + l.bias_offset(windows()), 1, l.output_features);
     }
     DenseMatrix root(VectorXd &v, const RGCNLayer &l) const {
-        return DenseMatrix::view(v.data() + l.root_offset(num_relations), l.input_features, l.output_features);
+        return DenseMatrix::view(v.data() + l.root_offset(windows()), l.input_features, l.output_features);
+    }
+    DenseMatrix comp(VectorXd &v, const RGCNLayer &l) const {
+        return DenseMatrix::view(v.data() + comp_offset(l), num_relations, num_bases);
     }
 
     // Each layer's params with its grads, one span per layer; grad is null before the first backward pass.  Defined in
@@ -137,9 +174,13 @@ public:
             RGCNLayer &layer = layers[i];
             DenseMatrix &X = buffers[i], &A = aggregated[i];
             const int64_t f = X.cols();
-            A.resize(d_ops->localArows, f * num_relations);
-            d_ops->relationalAggregate(X, A, num_relations);
-            if (aggr == kMean) window_scale(A, (int)f);
+            A.resize(d_ops->localArows, f * windows());
+            if (num_bases > 0) {
+                d_ops->basisAggregate(X, A, comp(layer.params, layer), num_relations, aggr == kMean ? &counts : nullptr);
+            } else {
+                d_ops->relationalAggregate(X, A, num_relations);
+                if (aggr == kMean) window_scale(A, (int)f);
+            }
             DenseMatrix Y = A * weight(layer.params, layer);
             hnh::abi_check(hnh_row_bias_add_f64(Y.data(), bias(layer.params, layer).data(), Y.rows(), Y.cols(), stream()), "row_bias_add");
             Y += X * root(layer.params, layer);
@@ -172,7 +213,7 @@ public:
 
 private:
     DenseMatrix ones;    // localArows x 1 of 1.0: the bias gradient is its product with dY
-    DenseMatrix counts;  // mean: |N_rho(u)| (localArows x R)
+    DenseMatrix counts;  // mean: |N_rho(u)| (localArows x R); with bases 1 / |N_rho(u)|, 0 where the count is 0
 
     static cudaStream_t stream() { return hnh::Runtime::get().compute_stream(); }
 
@@ -198,6 +239,14 @@ private:
         bias(layer.grads, layer).setTransposeTimes(ones, dY);
         root(layer.grads, layer).setTransposeTimes(X, dY);
         dX.setTimesTranspose(dY, root(layer.params, layer), false);
+        if (num_bases > 0) {
+            DenseMatrix dH, dcomp = comp(layer.grads, layer);
+            dH.setTimesTranspose(dY, weight(layer.params, layer), false);
+            d_ops->basisAggregateBackward(dH, X, dX, comp(layer.params, layer), dcomp, num_relations,
+                                          aggr == kMean ? &counts : nullptr, true);
+            allreduce_world(layer.grads.data(), comp_offset(layer));  // dcomp is summed over the ranks already
+            return;
+        }
         {
             DenseMatrix dA;
             dA.setTimesTranspose(dY, weight(layer.params, layer), false);

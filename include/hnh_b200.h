@@ -536,6 +536,35 @@ int hnh_relational_aggregate_grad_f64(const int64_t *rowStart, const int64_t *co
 int hnh_window_scale_f64(double *A, int64_t lda, const double *C, int64_t ldc, int64_t n, int f, int R, void *stream);
 int hnh_relation_check_f64(double *bad, const double *values, int64_t n, int R, void *stream);
 
+/* ---- basis aggregation (Distributed_Sparse::basisAggregate; csrc/rgcn.cu) ---------------------------------------------
+ * R-GCN with basis decomposition on one CSR block.  comp is the R x B coefficient matrix (row-major, device), scale
+ * (nullable: all ones) holds a weight per (stored row of the A order, relation) with leading dimension lds, and rho is
+ * an entry's relation as for hnh_relational_aggregate_f64 (an entry that is no relation contributes nothing and its
+ * gathered row is not read).
+ * hnh_basis_aggregate_f64: for every stored row u and entry (v, rho) (X gathered),
+ *     H[u, b f + k] += scale[u, rho] comp[rho, b] X[v, k]        (H is B f wide; the caller zeroes it first)
+ * summed in stored order in registers, up to a fixed number of bases at a time (more bases re-gather the row per chunk);
+ * every window of H of a row with entries is read and written once per call, so H may carry earlier blocks' sums.
+ * hnh_basis_aggregate_grad_f64, on a block whose stored rows are X's (the B order): for every stored row v and entry
+ * (u, rho) (dH and scale gathered),
+ *     dX[v, k] += scale[u, rho] sum_b comp[rho, b] dH[u, b f + k]   (in registers, one read-modify-write of dX per row)
+ * and with a non-null `products`, for entry j of the block (its CSR position),
+ *     products[b ldp + j] = scale[u, rho] <dH[u, b f .. b f + f), X[v, 0 .. f)>      (0 for an entry that is no relation)
+ * f, R, B >= 1, B f and R B < 2^31, every leading dimension >= its operand's width (ldp >= nnz); outputs may not alias
+ * inputs.  Column windows of 256 run separately; a window of width 4..256 (a power of two) with 16-byte aligned
+ * operands, even leading dimensions and an even f takes a row kernel with 128-bit gathers, others a one-warp-per-row
+ * kernel.  No atomics: repeated calls are bit-identical.
+ * hnh_relation_keys: keys[i] = the relation of values[i], or R for a value that is no relation (the keys of an
+ * hnh_edge_softmax_plan over R + 1 rows, which sums the products by relation). */
+int hnh_basis_aggregate_f64(const int64_t *rowStart, const int64_t *col_idx, const double *values, int64_t rows, int64_t nnz,
+                            const double *X, int64_t ldx, int f, const double *scale, int64_t lds, const double *comp, int R, int B,
+                            double *H, int64_t ldh, void *stream);
+int hnh_basis_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const double *values, int64_t rows, int64_t nnz,
+                                 const double *dH, int64_t lddh, const double *scale, int64_t lds, const double *comp, int R, int B,
+                                 const double *X, int64_t ldx, int f, double *dX, int64_t lddx, double *products, int64_t ldp,
+                                 void *stream);
+int hnh_relation_keys(int32_t *keys, const double *values, int64_t n, int R, void *stream);
+
 /* ---- host-side setup helpers (untimed; HOST pointers) --------------------------------------
  * hnh_er_generate_host replaces the CombBLAS Graph500 generator call of
  * SpmatLocal::loadTuples(false, logM, nnz_per_row) (SpmatLocal.hpp:499-516): rows

@@ -476,6 +476,25 @@ void hnhd_rgcn_destroy(hnhd_rgcn_t *g);
 int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations);
 int hnhd_alg_relational_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dA, hnhd_dense_t *dX, int num_relations, int accumulate);
 
+/* ---- R-GCN with basis decomposition (include/hnh/rgcn.hpp, Distributed_Sparse::basisAggregate) ---------------------
+ * hnhd_rgcn_create_bases: the model of hnhd_rgcn_create with PyG's num_bases = B >= 1: W_rho = sum_b comp[rho, b] V_b.
+ * Parameters by layer and name: "weight" (B f x r: RGCNConv.weight.reshape(-1, r)), "comp" (R x B), "bias" and "root"
+ * as without bases.  Refuses num_bases < 1 and B f or R B >= 2^31 besides what hnhd_rgcn_create refuses; every other
+ * hnhd_rgcn_* call works on the model unchanged.
+ * hnhd_alg_basis_aggregate: H (A-shaped, B f wide, B = comp's columns) = for each S-row u and basis b, the sum over the
+ * stored entries (u, v) of scale[u, rho] comp[rho, b] X_v (X B-shaped, f wide; comp R x B; scale A-shaped and R wide,
+ * or null for ones).  hnhd_alg_basis_aggregate_backward: dX (overwritten, or added to with accumulate != 0) =
+ * sum over the stored (u, v) of scale[u, rho] sum_b comp[rho, b] dH[u, b f .. b f + f), and dcomp (R x B, overwritten,
+ * the same on every rank) = sum over the stored entries of relation rho on all ranks of scale[u, rho]
+ * <dH[u, b f .. b f + f), X_v>.  Collective; HNH_E_INVALID on every rank where hnhd_alg_edge_softmax is, for
+ * num_relations < 1, B < 1, wrong shapes, and for an output that is another operand. */
+int hnhd_rgcn_create_bases(hnhd_alg_t *alg, int n_layers, const int *layers2, int num_relations, int num_bases, const char *aggr,
+                           hnhd_rgcn_t **out);
+int hnhd_alg_basis_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *H, hnhd_dense_t *comp, int num_relations,
+                             hnhd_dense_t *scale);
+int hnhd_alg_basis_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dH, hnhd_dense_t *X, hnhd_dense_t *dX, hnhd_dense_t *comp,
+                                      hnhd_dense_t *dcomp, int num_relations, hnhd_dense_t *scale, int accumulate);
+
 #ifdef __cplusplus
 }
 #endif
