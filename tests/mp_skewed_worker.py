@@ -9,6 +9,9 @@ algorithm and runs the case's kind:
            edge features
   gat      GAT forward and backward with the case's attention kind
   train    GAT train steps
+  gt       graph transformer forward and backward (a configuration of GT_CONFIGS)
+  gt_train graph transformer node train steps
+  gt_link  graph transformer link train steps against the targets of link_pairs, then link_evaluate
 
 Every op runs twice and the worker records whether the repeat gave the same bits.  It writes its rows of the results
 -- or the error the layout must raise -- to <outdir>/<case>_rank<r>.npz.
@@ -24,7 +27,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tests import gat_additive_oracle as gao  # noqa: E402
+from tests import graph_transformer_block_oracle as gbo  # noqa: E402
 from tests.mp_edge_softmax_worker import score, upstream  # noqa: E402
+from tests.mp_graph_transformer_worker import attr_of  # noqa: E402
 from tests.mp_sparse_attention_edge_worker import edge_of  # noqa: E402
 from tests.mp_worker import gather_local, sval  # noqa: E402
 from tests.skewed_graph import DEFAULT_N, landmarks, rank_slice, skewed_tuples  # noqa: E402
@@ -279,7 +284,151 @@ def run_train(D, alg, case, M, N, out):
             out[f"a1_{l}_{h}"], out[f"a2_{l}_{h}"] = net.attention_vectors(l, h)
 
 
-KINDS = dict(base=run_base, softmax=run_softmax, attn=run_attn, gat=run_gat, train=run_train)
+# ---- the graph transformer -----------------------------------------------------------------------------------------
+# Configurations and the paths each is meant to reach (tests/test_graph_transformer_sparse_oracle.py checks these
+# against the kernels' tables): per layer the attention kernels ("fast": d in HNH_DISPATCH_R, else "generic") and,
+# with blocks, LayerNorm forward and backward ("regs": the row in registers, else "generic").
+GT_CONFIGS = {
+    "table": dict(layers=[[64, 64, 4], [256, 128, 2]], edge_dim=3, beta=True, ffn=2, dropout=0.3,
+                  attention=("fast", "fast"), ln=(("regs", "regs"), ("regs", "regs"))),
+    "wide_heads": dict(layers=[[32, 256, 1], [256, 32, 8]], edge_dim=0, beta=False, ffn=0, dropout=0.0,
+                       attention=("fast", "fast"), ln=None),
+    "ln_backward_generic": dict(layers=[[48, 64, 17]], edge_dim=2, beta=True, ffn=1, dropout=0.3, attention=("fast",),
+                                ln=(("regs", "generic"),)),
+    "ln_generic": dict(layers=[[16, 64, 25]], edge_dim=0, beta=True, ffn=1, dropout=0.0, attention=("fast",),
+                       ln=(("generic", "generic"),)),
+    "odd": dict(layers=[[7, 5, 3], [15, 12, 2]], edge_dim=3, beta=True, ffn=1, dropout=0.3, attention=("generic", "generic"),
+                ln=(("regs", "regs"), ("regs", "regs"))),
+}
+
+
+def gt_config(case):
+    cfg = dict(GT_CONFIGS[case["gt"]])
+    cfg["layers"] = [tuple(l) for l in cfg["layers"]]
+    return cfg
+
+
+def gt_inputs(N, cfg, seed):
+    """(params, X, G) of a graph transformer case: the same on every rank."""
+    layers = cfg["layers"]
+    rng = np.random.default_rng(seed + 23)
+    params = gbo.random_params(layers, cfg["edge_dim"], cfg["beta"], cfg["ffn"], rng)
+    X = rng.uniform(-1, 1, (N, layers[0][0]))
+    G = rng.uniform(-1, 1, (N, layers[-1][1] * layers[-1][2]))
+    return params, X, G
+
+
+def link_pairs(N, seed):
+    """(rows, cols, soft targets) of the link cases' T: pairs on the wide hub rows, pairs between nodes without entries
+    (the empty third row block), pairs into the hub column, random pairs, and duplicated pairs with equal targets."""
+    rng = np.random.default_rng(seed + 29)
+    lm = landmarks(N, N)
+    e0, e1 = lm["empty_rows"]
+    groups = [(np.full(40, u), rng.integers(0, N, 40)) for u in lm["wide_hubs"]]
+    groups += [(rng.integers(e0, e1, 40), rng.integers(e0, e1, 40)), (rng.integers(0, N, 60), np.full(60, lm["hub_col"])),
+               (rng.integers(0, N, 200), rng.integers(0, N, 200))]
+    key = np.unique(np.concatenate([u * N + v for u, v in groups]))
+    tr, tc = key // N, key % N
+    y = rng.choice([0.0, 1.0, 0.25], len(tr))
+    dup = rng.choice(len(tr), 6, replace=False)
+    return np.concatenate([tr, tr[dup]]), np.concatenate([tc, tc[dup]]), np.concatenate([y, y[dup]])
+
+
+def _gt(D, alg, case, N):
+    cfg = gt_config(case)
+    layers = cfg["layers"]
+    net = D.GraphTransformer(alg, layers, edge_dim=cfg["edge_dim"], beta=cfg["beta"], ffn_ratio=cfg["ffn"])
+    params, X, G = gt_inputs(N, cfg, case["seed"])
+    for l, P in enumerate(params):
+        for k, v in P.items():
+            net.set_param(l, k, v)
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    rA, cA = alg.entry_coordinates("A")
+    rB, cB = alg.entry_coordinates("B")
+    # what the case reached on this rank: local rows, entries in each value order, the longest A-order row
+    reach = dict(topA=topA, nrA=nrA, topB=topB, nrB=nrB, local_rows=net.buffer_shape(0)[0], nA=len(rA), nB=len(rB),
+                 longest=np.bincount(np.asarray(rA, np.int64)).max(initial=0) if len(rA) else 0)
+    net.set_input(gather_local(X, [(topB, 0, nrB, layers[0][0])], net.buffer_shape(0)))
+    if cfg["edge_dim"]:
+        net.set_edge_attributes(attr_of(rA, cA, cfg["edge_dim"]), attr_of(rB, cB, cfg["edge_dim"]))
+    return cfg, net, G, reach
+
+
+def run_gt(D, alg, case, M, N, out):
+    cfg, net, G, reach = _gt(D, alg, case, N)
+    out.update(reach)
+    layers = cfg["layers"]
+    Gl = gather_local(G, [(reach["topA"], 0, reach["nrA"], G.shape[1])], net.buffer_shape(len(layers)))
+    got = []
+    for _ in range(2):
+        net.forward(cfg["dropout"], case["mask_seed"])
+        o = dict(Y=net.buffer(len(layers)))
+        net.backward(Gl)
+        o["dX"] = net.input_grad()
+        for l in range(len(layers)):
+            for k in net.param_names():
+                o[f"g{l}_{k}"] = net.param_grad(l, k)
+        got.append(o)
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k], equal_nan=True) for k in got[0])
+    out.update(got[0])
+
+
+def _gt_params(net, layers, out):
+    for l in range(len(layers)):
+        for k in net.param_names():
+            out[f"p{l}_{k}"] = net.param(l, k)
+
+
+def run_gt_train(D, alg, case, M, N, out):
+    cfg, net, _, reach = _gt(D, alg, case, N)
+    out.update(reach)
+    layers = cfg["layers"]
+    rows = net.buffer_shape(len(layers))[0]
+    classes = layers[-1][1] * layers[-1][2]
+    topA = reach["topA"]
+    lab = -np.ones(rows, np.int64)
+    hi = min(topA + rows, N)
+    lab[:hi - topA] = labels_of(N, classes, case["seed"])[topA:hi]
+    nl = D.NodeLabels(net, lab, classes)
+    opt = D.AdamW(lr=case["lrs"][0], weight_decay=0.01, max_grad_norm=case.get("clip"))
+    steps = []
+    for t, lr in enumerate(case["lrs"]):
+        opt.lr = lr
+        steps.append(list(net.train_step(nl, opt, cfg["dropout"], case["mask_seed"] + 7 * t)))
+    out["steps"] = np.array(steps)
+    _gt_params(net, layers, out)
+
+
+def run_gt_link(D, alg, case, M, N, out):
+    cfg, net, _, reach = _gt(D, alg, case, N)
+    out.update(reach)
+    layers = cfg["layers"]
+    from distributed_sddmm_b200 import lib
+    rank, world = lib().hnhd_world_rank(), lib().hnhd_world_size()
+    tr, tc, y = link_pairs(N, case["seed"])
+    sr, sc = rank_slice(tr, tc, rank, world)
+    sy = y[rank::world]
+    algT = D.Algorithm(case["alg"], D.SpmatLocal.from_tuples(N, N, sr.astype(np.uint64), sc.astype(np.uint64), sy), layers[0][0],
+                       case["c"])
+    t = D.LinkTargets(net, algT)
+    opt = D.AdamW(lr=case["lrs"][0], weight_decay=0.01)
+    steps = []
+    for s, lr in enumerate(case["lrs"]):
+        opt.lr = lr
+        steps.append(list(net.link_train_step(t, opt, cfg["dropout"], case["mask_seed"] + 7 * s)))
+    out["steps"] = np.array(steps)
+    _gt_params(net, layers, out)
+    loss, correct, count, scores = net.link_evaluate(t)
+    out["evaluate"] = np.array([loss, correct, count])
+    out["scores"] = scores
+    out["tA_rows"], out["tA_cols"] = algT.entry_coordinates("A")
+    out["H"] = net.buffer(len(layers))
+    del t, algT
+
+
+KINDS = dict(base=run_base, softmax=run_softmax, attn=run_attn, gat=run_gat, train=run_train, gt=run_gt, gt_train=run_gt_train,
+             gt_link=run_gt_link)
 
 
 def run_case(D, case, rank, world):

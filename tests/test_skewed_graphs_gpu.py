@@ -1,9 +1,10 @@
 """The skewed graph of tests/skewed_graph.py on one rank, in-process: the op table of
 tests/test_skewed_graphs_multirank_gpu.py (its cases, worker code and checks) on all five algorithms and on the
-rectangular variants, and the kernel-level entry points fed one skewed block directly -- the sparse-attention step,
-finish, grad_q and grad_kv kernels on the block and on its transpose (where the hub column is one very long row), and
-the edge-softmax plan, statistics, apply and backward kernels keyed by row and by column -- so that a failure on several
-ranks can be told apart from a kernel fault."""
+rectangular variants, every graph transformer configuration (and its refusal of the rectangular sizes), and the
+kernel-level entry points fed one skewed block directly -- the sparse-attention step, finish, grad_q and grad_kv kernels
+on the block and on its transpose (where the hub column is one very long row), and the edge-softmax plan, statistics,
+apply and backward kernels keyed by row and by column -- so that a failure on several ranks can be told apart from a
+kernel fault."""
 import numpy as np
 import pytest
 
@@ -41,9 +42,13 @@ def _cases(alg, i):
     return out
 
 
-CHECKS = dict(base=T.check_base, softmax=T.check_softmax, attn=T.check_attention, gat=T.check_gat, train=T.check_training)
+CHECKS = dict(base=T.check_base, softmax=T.check_softmax, attn=T.check_attention, gat=T.check_gat, train=T.check_training,
+              gt=T.check_gt)
 P1 = [c for i, alg in enumerate(ALGS) for c in _cases(alg, i)]
 P1 += [T._case("train", "25d_dense_replicate", 1, 64, attention="additive", layers=T.GAT_LAYERS, steps=3)]
+# the graph transformer: every configuration on 15d_fusion1, the two with edge features on every algorithm
+P1 += [T.gt_case("gt", alg, 1, name) for name in ("table", "odd") for alg in ALGS]
+P1 += [T.gt_case("gt", "15d_fusion1", 1, name) for name in ("wide_heads", "ln_backward_generic", "ln_generic")]
 RECT = [dict(c, m=M, n=N) for k, (M, N) in enumerate(RECTANGULAR)
         for c in (T._case("base", ALGS[k], 1, 128, script=T.ALL_OPS), T._case("softmax", ALGS[k + 2], 1, 8, mask=1),
                   _attn(ALGS[k + 3], 2, 64, "bias", 0.4), _attn(ALGS[k], 1, 128, "edge"))]
@@ -52,6 +57,14 @@ RECT = [dict(c, m=M, n=N) for k, (M, N) in enumerate(RECTANGULAR)
 @pytest.mark.parametrize("case", P1 + RECT, ids=lambda c: c["name"] + (f"_{c['m']}x{c['n']}" if "m" in c else ""))
 def test_p1_ops_on_the_skewed_graph(world, case):
     CHECKS[case["kind"]]([W.run_case(D, case, 0, 1)], case, 1)
+
+
+@pytest.mark.parametrize("M,N", RECTANGULAR)
+def test_graph_transformer_refuses_rectangular_sizes(world, M, N):
+    """A and B layouts of other row counts: the constructor raises, before any launch."""
+    out = W.run_case(D, dict(T.gt_case("gt", "15d_fusion1", 1, "odd"), m=M, n=N, rejected=1), 0, 1)
+    msg = str(out.get("error"))
+    assert "code -1" in msg and "GraphTransformer" in msg, msg
 
 
 def _block(M, N, seed=5):

@@ -3,8 +3,9 @@ every rank's column block, a hub column, a rank whose row block is empty, a colu
 self-loops, 4200 nodes so that 4 ranks hold 1050 rows each) at the kernels' table widths, on 1, 2 and 4 ranks
 (tests/mp_skewed_worker.py): the base ops at R = 64, 128, 256 and 100 on every layout, the edge softmax with and without
 -inf scores, fused sparse attention (plain, dropout, a masking per-head bias, edge features) at heads x d = 2 x 64,
-1 x 128 and 4 x 7, GAT forward and backward with the four attention kinds and GAT train steps, each against the fp64
-models written per stored entry, rank by rank.  Beyond parity: rows without entries give Z = 0, L = -inf and zero dQ,
+1 x 128 and 4 x 7, GAT forward and backward with the four attention kinds and GAT train steps, and the graph
+transformer (the configurations of mp_skewed_worker.GT_CONFIGS: forward and backward, node and link train steps,
+link_evaluate), each against the fp64 models written per stored entry, rank by rank.  Beyond parity: rows without entries give Z = 0, L = -inf and zero dQ,
 untouched columns zero dK and dV; a repeat gives the same bits; the results at p = 2 and 4 equal those at p = 1 to
 1e-12; per-entry gradients (dbias, dE) of the two copies of a duplicate agree, with dropout too (one keep bit per
 (row, column), whatever the layout); trained parameters are bit-identical across ranks.
@@ -26,6 +27,8 @@ from tests import gat_additive_oracle as gao
 from tests import gat_backward_oracle as gbk
 from tests import gat_softmax_oracle as gso
 from tests import gatv2_oracle as gv2
+from tests import graph_transformer_sparse_oracle as gts
+from tests import link_prediction_oracle as lpo
 from tests import mp_skewed_worker as W
 from tests import sparse_attention_bias_oracle as sb
 from tests import sparse_attention_dropout_oracle as sd
@@ -33,10 +36,13 @@ from tests import sparse_attention_edge_oracle as se
 from tests import sparse_attention_oracle as sa
 from tests import training_oracle as tro
 from tests.mp_edge_softmax_worker import score, upstream
+from tests.mp_graph_transformer_worker import attr_of
 from tests.mp_sparse_attention_edge_worker import edge_of
 from tests.mp_util import ROOT, free_port
 from tests.mp_worker import gather_local, sval
 from tests.skewed_graph import landmarks, skewed_tuples
+from tests.test_graph_transformer_gpu import grad_err
+from tests.test_graph_transformer_sparse_oracle import kernel_tables, paths as gt_paths
 from tests.test_sparse_attention_multirank_gpu import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -53,8 +59,16 @@ ALL_OPS = ["sddmmA", "spmmA", "spmmB", "fusedA", "sddmmB", "fusedB"]
 
 
 def _case(kind, alg, c, R, **kw):
-    tag = "_".join(f"{k}{v}" for k, v in sorted(kw.items()) if k not in ("layers", "script", "mask_seed", "steps"))
+    tag = "_".join(f"{k}{v}" for k, v in sorted(kw.items()) if k not in ("layers", "script", "mask_seed", "steps", "lrs"))
     return dict(name=f"{kind}_{alg}_c{c}_R{R}" + ("_" + tag if tag else ""), kind=kind, alg=alg, c=c, R=R, seed=SEED, **kw)
+
+
+GT_CLIP = 1.0  # below the first step's gradient norm of the "table" train case (3.6), above the later ones (about 0.5)
+
+
+def gt_case(kind, alg, c, config, **kw):
+    """A graph transformer case of configuration `config` (mp_skewed_worker.GT_CONFIGS)."""
+    return _case(kind, alg, c, W.GT_CONFIGS[config]["layers"][0][0], gt=config, mask_seed=31, **kw)
 
 
 def cases_for(p):
@@ -84,9 +98,17 @@ def cases_for(p):
         out.append(_case("gat", alg, c, 64, attention=kind, layers=GAT_LAYERS))
     out += [_case("train", "15d_fusion1", 1, 64, attention="additive", layers=GAT_LAYERS, steps=3),
             _case("train", "15d_fusion2", 1, 64, attention="softmax", layers=GAT_LAYERS, steps=3)]
-    if p > 1:  # the layouts that split R have no row softmax, attention or GAT backward
+    out += [gt_case("gt", alg, c, name) for name in ("table", "odd") for alg, c in (("15d_fusion1", 1), ("15d_fusion1", c2),
+                                                                                     ("15d_fusion2", 1))]
+    if p == 4:  # rank 2's row block holds no entries (see check_gt_reach)
+        out.append(gt_case("gt", "15d_fusion1", 1, "ln_backward_generic"))
+    out += [gt_case("gt_train", "15d_fusion1", 1, "table", lrs=[1e-2, 3e-2, 2e-2], clip=GT_CLIP),
+            gt_case("gt_train", "15d_fusion1", 1, "wide_heads", lrs=[1e-2] * 3),
+            gt_case("gt_link", "15d_fusion1", 1, "table", lrs=[1e-2, 2e-2, 1e-2])]
+    if p > 1:  # the layouts that split R have no row softmax, attention, GAT backward or graph transformer
         out += [dict(attn("15d_sparse", 1, 2, 64, "plain"), rejected=1),
-                dict(_case("gat", "15d_sparse", 1, 64, attention="softmax", layers=GAT_LAYERS), rejected=1)]
+                dict(_case("gat", "15d_sparse", 1, 64, attention="softmax", layers=GAT_LAYERS), rejected=1),
+                dict(gt_case("gt", "15d_sparse", 1, "table"), rejected=1), dict(gt_case("gt", "15d_fusion2", 2, "odd"), rejected=1)]
     return list({c["name"]: c for c in out}.values())  # at p = 1 the c = 2 cases fall onto their c = 1 twins
 
 
@@ -428,6 +450,146 @@ def check_training(ranks, case, nproc):
                 assert err <= 1e-9 * max(np.abs(w).max(), 1.0), (name, key, err)
 
 
+# ---- the graph transformer -----------------------------------------------------------------------------------------
+REACH = ("topA", "nrA", "topB", "nrB", "local_rows", "nA", "nB", "longest")
+_GT_REF = {}
+
+
+def gt_problem(case):
+    """(rows, cols, N, cfg, params, X, G, model keywords) of a graph transformer case."""
+    M, N, rows, cols = graph(case)
+    cfg = W.gt_config(case)
+    params, X, G = W.gt_inputs(N, cfg, case["seed"])
+    kw = dict(attr=attr_of(rows, cols, cfg["edge_dim"]) if cfg["edge_dim"] else None, beta=cfg["beta"], ffn=cfg["ffn"])
+    return rows, cols, N, cfg, params, X, G, kw
+
+
+def gt_reference(case):
+    """The per-entry model's output, dX and parameter gradients, and its output on the rows without entries computed
+    from the skip alone (the model on a pattern without entries: M = 0 on every row)."""
+    key = (case["gt"], case["mask_seed"])
+    if key not in _GT_REF:
+        rows, cols, N, cfg, params, X, G, kw = gt_problem(case)
+        out, dX, dP = gts.backward_np(rows, cols, N, cfg["layers"], params, X, G, p=cfg["dropout"], seed=case["mask_seed"], **kw)
+        none = np.zeros(0, np.int64)
+        skip = gts.forward_np(none, none, N, cfg["layers"], params, X, **dict(kw, attr=np.zeros((0, cfg["edge_dim"])) if cfg["edge_dim"] else None))
+        _GT_REF[key] = dict(Y=out, dX=dX, dP=dP, skip=skip)
+    return _GT_REF[key]
+
+
+def check_gt_reach(ranks, case, nproc):
+    """The case reached what it is for: the configuration's kernel paths (by the tables in the sources), more rows per
+    rank than one dw_chunks chunk, at p = 1 a hub row of more than 2000 entries through attention at d >= 64, and at
+    p = 4 with c = 1 a rank with entries in one value order only: rank 2 owns the empty third row block, which is its
+    A order under local kernel fusion (15d_fusion2: S's own blocks; with edge features, GraphTransformer's branch
+    for a rank without A-order attributes) and its B order under replication reuse (15d_fusion1 keeps A-order values
+    in the transpose's blocks, which rank 2 holds by S-column)."""
+    cfg, tables = W.gt_config(case), kernel_tables()
+    att, ln = gt_paths(cfg, tables)
+    assert att == tuple(cfg["attention"]) and ln == (tuple(tuple(x) for x in cfg["ln"]) if cfg["ln"] else None), case["name"]
+    assert all(int(d["local_rows"]) > tables["min_chunk_rows"] for d in ranks), case["name"]
+    if nproc == 1 and max(d for _, d, _ in cfg["layers"]) >= 64:
+        assert int(ranks[0]["longest"]) > 2000, case["name"]
+    if nproc == 4 and case["c"] == 1:
+        empty, full = ("nA", "nB") if case["alg"] == "15d_fusion2" else ("nB", "nA")
+        assert int(ranks[2][empty]) == 0 < int(ranks[2][full]), (case["name"], empty)
+
+
+def check_gt(ranks, case, nproc):
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    check_gt_reach(ranks, case, nproc)
+    want = gt_reference(case)
+    M, N = W.sizes(case)
+    for r, d in enumerate(ranks):
+        assert bool(d["repeat"]), (name, r)
+    Y = check_rows(ranks, name, "Y", want["Y"], "topA", "nrA")
+    check_rows(ranks, name, "dX", want["dX"], "topB", "nrB")
+    # the rows without entries take the skip alone: Y = R (beta R with the gate), then the ReLU or the block
+    e0, e1 = landmarks(M, N)["empty_rows"]
+    assert np.abs(Y[e0:e1] - want["skip"][e0:e1]).max() <= 1e-10 * np.abs(want["Y"]).max(), name
+    assert np.abs(want["Y"][e0:e1] - want["skip"][e0:e1]).max() <= 1e-13 * np.abs(want["Y"]).max()
+    for l, grads in enumerate(want["dP"]):
+        scale = max(np.abs(g).max() for g in grads.values())
+        for k, g in grads.items():
+            key = f"g{l}_{k}"
+            for r, d in enumerate(ranks):
+                assert np.array_equal(d[key], ranks[0][key]), (name, r, key, "differs across ranks")
+            assert grad_err(ranks[0][key], g, scale) < 1e-10, (name, key, grad_err(ranks[0][key], g, scale))
+            assert k == "key_bias" or np.abs(g).max() > 0, (name, key)
+
+
+def check_gt_steps(ranks, case, want, tparams):
+    """Per-step results as tests/test_link_prediction_gpu.check_steps; trained parameters to 1e-9, key_bias within the
+    sum of the learning rates (its gradient is rounding noise on both sides, which Adam turns into steps of up to lr);
+    everything bit-identical across ranks."""
+    name = case["name"]
+    for r, d in enumerate(ranks):
+        for k in d:
+            if k not in REACH and k not in ("scores", "tA_rows", "tA_cols", "H"):
+                assert np.array_equal(d[k], ranks[0][k]), (name, r, k, "differs across ranks")
+    steps = ranks[0]["steps"]
+    assert len(steps) == len(want) == len(case["lrs"])
+    for t, w in enumerate(want):
+        # From the third step on the gradient norm is as sensitive to rounding as the trained parameters are: the fp64
+        # model itself, its entries merely stored in another order, moves the third norm of the "table" case by
+        # 1.4e-10 to 2.2e-10 (Adam's first steps have amplified the last bits of the earlier gradients).
+        tol = 1e-10 if t < 2 else 1e-9
+        assert abs(steps[t][0] - w[0]) <= 1e-10 * abs(w[0]) and abs(steps[t][3] - w[3]) <= tol * abs(w[3]), (name, t, steps[t], w)
+        assert (int(steps[t][1]), int(steps[t][2])) == (w[1], w[2]), (name, t, steps[t], w)
+    for l, P in enumerate(tparams):
+        for k, w in P.items():
+            got = ranks[0][f"p{l}_{k}"]
+            if k == "key_bias":
+                assert np.abs(got - w).max() <= sum(case["lrs"]) * 1.01, (name, l, k)
+            else:
+                assert np.abs(got - w).max() <= 1e-9 * max(np.abs(w).max(), 1.0), (name, l, k, np.abs(got - w).max())
+
+
+def check_gt_training(ranks, case, nproc):
+    ranks = ranks_ok(ranks, case["name"])
+    check_gt_reach(ranks, case, nproc)
+    rows, cols, N, cfg, params, X, _, kw = gt_problem(case)
+    layers = cfg["layers"]
+    labels = W.labels_of(N, layers[-1][1] * layers[-1][2], case["seed"])
+    lrs = case["lrs"]
+    want, tparams = gts.train_gt(rows, cols, N, layers, params, X, labels, len(lrs), dropout=cfg["dropout"],
+                                 seeds=[case["mask_seed"] + 7 * t for t in range(len(lrs))], lr=lrs[0], lrs=lrs,
+                                 weight_decay=0.01, max_grad_norm=case.get("clip"), **kw)
+    if case.get("clip"):
+        assert sum(w[3] > case["clip"] for w in want) == 1, [w[3] for w in want]  # clipping active on one step
+    check_gt_steps(ranks, case, want, tparams)
+
+
+def check_gt_link(ranks, case, nproc):
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    check_gt_reach(ranks, case, nproc)
+    rows, cols, N, cfg, params, X, _, kw = gt_problem(case)
+    tr, tc, y = W.link_pairs(N, case["seed"])
+    lm = landmarks(N, N)
+    empty = np.bincount(rows, minlength=N) == 0
+    assert np.isin(tr, lm["wide_hubs"]).sum() >= 60 and (empty[tr] & empty[tc]).sum() >= 20 and (tc == lm["hub_col"]).sum() >= 50
+    assert (y == 0.25).any() and len(np.unique(tr * N + tc)) < len(tr)
+    lrs = case["lrs"]
+    want, tparams = gts.link_train_gt(rows, cols, N, cfg["layers"], params, X, (tr, tc, y), len(lrs), dropout=cfg["dropout"],
+                                      seeds=[case["mask_seed"] + 7 * t for t in range(len(lrs))], lr=lrs[0], lrs=lrs,
+                                      weight_decay=0.01, **kw)
+    check_gt_steps(ranks, case, want, tparams)
+    # link_evaluate: a forward without dropout; the scores are <H_u, H_v> of the returned buffer in T's A order
+    H = assemble(ranks, "H", "topA", "nrA", N)
+    wl, wc, wn, _, _, _ = lpo.link_loss(H, H, tr, tc, y, same=True)
+    loss, correct, count = ranks[0]["evaluate"]
+    assert abs(loss - wl) <= 1e-12 * abs(wl) and int(count) == wn == len(tr) and abs(int(correct) - wc) <= 1, name
+    seen = []
+    for r, d in enumerate(ranks):
+        u, v = d["tA_rows"], d["tA_cols"]
+        s = (H[u] * H[v]).sum(1)
+        assert np.abs(d["scores"] - s).max(initial=0.0) <= 1e-12 * max(np.abs(s).max(initial=0.0), 1.0), (name, r)
+        seen.append(u * N + v)
+    assert np.array_equal(np.sort(np.concatenate(seen)), np.sort(tr * N + tc)), name
+
+
 # ---- across rank counts --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("nproc", [2, 4])
 def test_results_do_not_depend_on_the_rank_count(nproc):
@@ -437,10 +599,29 @@ def test_results_do_not_depend_on_the_rank_count(nproc):
     checked = 0
     for case in CASES[nproc]:
         name = case["name"]
-        if name not in one or case["kind"] not in ("attn", "gat", "train") or case.get("rejected"):
+        if name not in one or case["kind"] not in ("attn", "gat", "train", "gt", "gt_train", "gt_link") or case.get("rejected"):
             continue
         a, b = ranks_ok(one[name], name), ranks_ok(many[name], name)
         M, N = W.sizes(case)
+        if case["kind"] == "gt":
+            for key in ("Y", "dX"):
+                top, nr, total = ("topA", "nrA", M) if key == "Y" else ("topB", "nrB", N)
+                assert rel_err(assemble(b, key, top, nr, total), assemble(a, key, top, nr, total)) < 1e-12, (name, nproc, key)
+            for l in range(len(W.gt_config(case)["layers"])):
+                grads = {k: v for k, v in a[0].items() if k.startswith(f"g{l}_")}
+                scale = max(np.abs(g).max() for g in grads.values())  # key_bias: 0 up to rounding
+                for k, g in grads.items():
+                    assert grad_err(b[0][k], g, scale) < 1e-12, (name, nproc, k)
+            checked += 1
+            continue
+        if case["kind"] in ("gt_train", "gt_link"):
+            for k in a[0]:
+                if k.endswith("key_bias"):  # Adam's steps of up to lr on a rounding-noise gradient
+                    assert np.abs(b[0][k] - a[0][k]).max() <= sum(case["lrs"]) * 1.01, (name, nproc, k)
+                elif k == "steps" or k.startswith("p"):
+                    assert rel_err(b[0][k], a[0][k]) < 1e-9, (name, nproc, k)
+            checked += 1
+            continue
         if case["kind"] == "train":
             pairs = [(a[0][k], b[0][k]) for k in a[0] if k != "local_rows"]
         else:
@@ -488,3 +669,18 @@ def test_gat_on_the_skewed_graph(nproc, case):
 @pytest.mark.parametrize("nproc,case", params("train"))
 def test_gat_training_on_the_skewed_graph(nproc, case):
     check_training(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gt"))
+def test_graph_transformer_on_the_skewed_graph(nproc, case):
+    check_gt(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gt_train"))
+def test_graph_transformer_training_on_the_skewed_graph(nproc, case):
+    check_gt_training(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gt_link"))
+def test_graph_transformer_link_training_on_the_skewed_graph(nproc, case):
+    check_gt_link(results(nproc)[case["name"]], case, nproc)
