@@ -265,13 +265,7 @@ ABI.update({
     "hnhd_gat_set_weight": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "hnhd_gat_get_weight": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "hnhd_gat_get_attention_vectors": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
-    "hnhd_gat_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_gat_set_input": (C.c_int, [_P, _P]),
-    "hnhd_gat_get_buffer": (C.c_int, [_P, C.c_int, _P]),
-    "hnhd_gat_forward": (C.c_int, [_P]),
-    "hnhd_gat_backward": (C.c_int, [_P, _P]),
     "hnhd_gat_get_weight_grad": (C.c_int, [_P, C.c_int, C.c_int, _P]),
-    "hnhd_gat_get_input_grad": (C.c_int, [_P, _P]),
     "hnhd_gat_set_attention": (C.c_int, [_P, C.c_char_p]),
     "hnhd_gat_set_attention_vectors": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
     "hnhd_gat_get_attention_grads": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
@@ -294,72 +288,40 @@ ABI.update({
     "hnhd_alg_sparse_attention_backward_edge": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double,
                                                           C.c_double, C.c_uint64, _P, _P, _P, _P, _P, _P, _P]),
     "hnhd_alg_entry_coordinates": (C.c_int, [_P, C.c_int, _P, _P]),
-    "hnhd_gat_destroy": (None, [_P]),
     "hnhd_gt_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, _PP]),
     "hnhd_gt_create_block": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.c_double, _PP]),
-    "hnhd_gt_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_gt_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_gt_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_gt_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_gt_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_gt_set_input": (C.c_int, [_P, _P]),
-    "hnhd_gt_get_buffer": (C.c_int, [_P, C.c_int, _P]),
     "hnhd_gt_set_edge_attributes": (C.c_int, [_P, _P, _I64, _P, _I64]),
-    "hnhd_gt_forward": (C.c_int, [_P, C.c_double, C.c_uint64]),
-    "hnhd_gt_backward": (C.c_int, [_P, _P]),
-    "hnhd_gt_get_input_grad": (C.c_int, [_P, _P]),
-    "hnhd_gt_destroy": (None, [_P]),
     "hnhd_labels_create": (C.c_int, [_P, _P, _I64, C.c_int, _PP]),
     "hnhd_labels_destroy": (None, [_P]),
     "hnhd_adamw_create": (C.c_int, [C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _PP]),
     "hnhd_adamw_set_lr": (C.c_int, [_P, C.c_double]),
     "hnhd_adamw_destroy": (None, [_P]),
-    "hnhd_gt_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
-    "hnhd_gat_train_step": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_alg_link_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     "hnhd_link_targets_create": (C.c_int, [_P, _P, _PP]),
     "hnhd_link_targets_destroy": (None, [_P]),
-    "hnhd_gt_link_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
-    "hnhd_gat_link_train_step": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_gt_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_gat_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_alg_max_aggregate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_alg_max_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int]),
     "hnhd_sage_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, _PP]),
-    "hnhd_sage_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_sage_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_sage_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_sage_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_sage_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_sage_set_input": (C.c_int, [_P, _P]),
-    "hnhd_sage_get_buffer": (C.c_int, [_P, C.c_int, _P]),
-    "hnhd_sage_forward": (C.c_int, [_P]),
-    "hnhd_sage_backward": (C.c_int, [_P, _P]),
-    "hnhd_sage_get_input_grad": (C.c_int, [_P, _P]),
-    "hnhd_sage_train_step": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_sage_link_train_step": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_sage_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_sage_destroy": (None, [_P]),
     "hnhd_alg_relational_aggregate": (C.c_int, [_P, _P, _P, C.c_int]),
     "hnhd_alg_relational_aggregate_backward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int]),
     "hnhd_rgcn_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_char_p, _PP]),
     "hnhd_rgcn_create_bases": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_char_p, _PP]),
     "hnhd_alg_basis_aggregate": (C.c_int, [_P, _P, _P, _P, C.c_int, _P]),
     "hnhd_alg_basis_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P, C.c_int]),
-    "hnhd_rgcn_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_rgcn_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_rgcn_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_rgcn_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
-    "hnhd_rgcn_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "hnhd_rgcn_set_input": (C.c_int, [_P, _P]),
-    "hnhd_rgcn_get_buffer": (C.c_int, [_P, C.c_int, _P]),
-    "hnhd_rgcn_forward": (C.c_int, [_P]),
-    "hnhd_rgcn_backward": (C.c_int, [_P, _P]),
-    "hnhd_rgcn_get_input_grad": (C.c_int, [_P, _P]),
-    "hnhd_rgcn_train_step": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_rgcn_link_train_step": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_rgcn_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
-    "hnhd_rgcn_destroy": (None, [_P]),
+    "hnhd_model_buffer_shape": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_model_set_input": (C.c_int, [_P, _P]),
+    "hnhd_model_get_buffer": (C.c_int, [_P, C.c_int, _P]),
+    "hnhd_model_forward": (C.c_int, [_P, C.c_double, C.c_uint64]),
+    "hnhd_model_backward": (C.c_int, [_P, _P]),
+    "hnhd_model_get_input_grad": (C.c_int, [_P, _P]),
+    "hnhd_model_param_shape": (C.c_int, [_P, C.c_int, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_model_set_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_model_get_param": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_model_get_param_grad": (C.c_int, [_P, C.c_int, C.c_char_p, _P]),
+    "hnhd_model_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
+    "hnhd_model_link_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
+    "hnhd_model_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_model_destroy": (None, [_P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

@@ -20,6 +20,8 @@
 #include "hnh/graph_transformer.hpp"
 #include "hnh_b200.h"
 
+GAT::~GAT() = default;  // the key function (hnh/gat.hpp)
+
 Distributed_Sparse *hnh_make_algorithm(const string &name, SpmatLocal *spmat, int R, int c, KernelImplementation *k) {
     if (name == "15d_fusion1") return new Sparse15D_Dense_Shift(spmat, R, c, 1, k);
     if (name == "15d_fusion2") return new Sparse15D_Dense_Shift(spmat, R, c, 2, k);

@@ -35,17 +35,8 @@ struct hnhd_dense {
 struct hnhd_vec {
     VectorXd v;
 };
-struct hnhd_gat {
-    std::unique_ptr<GAT> g;
-};
-struct hnhd_gt {
-    std::unique_ptr<GraphTransformer> g;
-};
-struct hnhd_sage {
-    std::unique_ptr<GraphSAGE> g;
-};
-struct hnhd_rgcn {
-    std::unique_ptr<RGCN> g;
+struct hnhd_model {
+    std::unique_ptr<GraphModel> m;
 };
 struct hnhd_labels {
     std::unique_ptr<hnh::NodeLabels> l;
@@ -83,6 +74,35 @@ int copy_json(const json &j, char *out, size_t capacity) {
 }
 
 cudaEvent_t g_t0 = nullptr, g_t1 = nullptr;
+
+// ---- graph model handles: the model behind one, its buffers and its parameters by name
+GraphModel &model(hnhd_model_t *m) {
+    if (!m) throw hnh::Error(HNH_E_INVALID, "null model");
+    return *m->m;
+}
+// the model behind a handle as a T (`kind` names it), refused for a model of another kind
+template <class T>
+T &model_as(hnhd_model_t *m, const char *kind) {
+    T *t = dynamic_cast<T *>(&model(m));
+    if (!t) throw hnh::Error(HNH_E_INVALID, string("this call takes a ") + kind + " model, not a " + m->m->model_name + " one");
+    return *t;
+}
+DenseMatrix &model_buffer(hnhd_model_t *m, int buffer) {
+    GraphModel &g = model(m);
+    if (buffer < 0 || buffer >= (int)g.buffers.size()) throw hnh::Error(HNH_E_INVALID, g.model_name + ": no such buffer");
+    return g.buffers[(size_t)buffer];
+}
+ParamRef model_param(hnhd_model_t *m, int layer, const char *name) {
+    GraphModel &g = model(m);
+    if (!name) throw hnh::Error(HNH_E_INVALID, g.model_name + ": null argument");
+    return g.param(layer, name);
+}
+// copy n doubles between host and device on the compute stream and wait for the copy
+void sync_copy(double *dst, const double *src, int64_t n, cudaMemcpyKind kind) {
+    cudaStream_t s = hnh::Runtime::get().compute_stream();
+    if (n > 0) hnh::cuda_check(cudaMemcpyAsync(dst, src, sizeof(double) * (size_t)n, kind, s), "model parameter copy");
+    hnh::cuda_check(cudaStreamSynchronize(s), "model parameter copy");
+}
 
 }  // namespace
 
@@ -564,296 +584,6 @@ int hnhd_als_run(hnhd_alg_t *a, const double *hostAgt, const double *hostBgt, co
     });
 }
 
-// ---- GAT ------------------------------------------------------------------------------------------
-int hnhd_gat_create(hnhd_alg_t *a, int n_layers, const int *layers3, double alpha, hnhd_gat_t **out) {
-    return guarded([&] {
-        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_create: bad argument");
-        vector<GATLayer> layers;
-        for (int i = 0; i < n_layers; i++) {
-            if (layers3[3 * i] <= 0 || layers3[3 * i + 1] <= 0 || layers3[3 * i + 2] <= 0)
-                throw hnh::Error(HNH_E_INVALID, "hnhd_gat_create: layer sizes must be positive");
-            layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
-        }
-        std::unique_ptr<hnhd_gat> g(new hnhd_gat);
-        g->g.reset(new GAT(layers, a->alg.get()));
-        g->g->leaky_relu_alpha = alpha;
-        *out = g.release();
-    });
-}
-static DenseMatrix &gat_weight(hnhd_gat_t *g, int layer, int head) {
-    if (!g || layer < 0 || layer >= (int)g->g->layers.size()) throw hnh::Error(HNH_E_INVALID, "gat: no such layer");
-    GATLayer &l = g->g->layers[(size_t)layer];
-    if (head < 0 || head >= l.num_heads) throw hnh::Error(HNH_E_INVALID, "gat: no such head");
-    return l.wMats[(size_t)head];
-}
-static DenseMatrix &gat_buffer(hnhd_gat_t *g, int buffer) {
-    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "gat: no such buffer");
-    return g->g->buffers[(size_t)buffer];
-}
-int hnhd_gat_weight_shape(hnhd_gat_t *g, int layer, int head, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        DenseMatrix &w = gat_weight(g, layer, head);
-        if (rows) *rows = w.rows();
-        if (cols) *cols = w.cols();
-    });
-}
-int hnhd_gat_set_weight(hnhd_gat_t *g, int layer, int head, const double *host) {
-    return guarded([&] {
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_weight(g, layer, head).copy_from_host(host);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_gat_get_weight(hnhd_gat_t *g, int layer, int head, double *host) {
-    return guarded([&] {
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_weight(g, layer, head).copy_to_host(host);
-    });
-}
-int hnhd_gat_buffer_shape(hnhd_gat_t *g, int buffer, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        DenseMatrix &b = gat_buffer(g, buffer);
-        if (rows) *rows = b.rows();
-        if (cols) *cols = b.cols();
-    });
-}
-int hnhd_gat_set_input(hnhd_gat_t *g, const double *host) {
-    return guarded([&] {
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_buffer(g, 0).copy_from_host(host);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_gat_get_buffer(hnhd_gat_t *g, int buffer, double *host) {
-    return guarded([&] {
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_buffer(g, buffer).copy_to_host(host);
-    });
-}
-int hnhd_gat_forward(hnhd_gat_t *g) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null gat");
-        g->g->forwardPass();
-    });
-}
-int hnhd_gat_backward(hnhd_gat_t *g, const double *host_output_grad) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null gat");
-        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const DenseMatrix &out = g->g->buffers.back();
-        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
-        g->g->backwardPass(grad);
-    });
-}
-int hnhd_gat_get_weight_grad(hnhd_gat_t *g, int layer, int head, double *host) {
-    return guarded([&] {
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_weight(g, layer, head);  // validates layer and head
-        const GATLayer &l = g->g->layers[(size_t)layer];
-        if (l.wGrads.size() != l.wMats.size()) throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
-        l.wGrads[(size_t)head].copy_to_host(host);
-    });
-}
-int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null gat");
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
-        g->g->input_grad.copy_to_host(host);
-    });
-}
-int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind) {
-    return guarded([&] {
-        if (!g || !kind) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_set_attention: null argument");
-        g->g->set_attention(kind);
-    });
-}
-// copy n doubles between host and device on the compute stream and wait for the copy
-static void gat_copy(double *dst, const double *src, int64_t n, cudaMemcpyKind kind) {
-    cudaStream_t s = hnh::Runtime::get().compute_stream();
-    hnh::cuda_check(cudaMemcpyAsync(dst, src, sizeof(double) * (size_t)n, kind, s), "gat attention vector copy");
-    hnh::cuda_check(cudaStreamSynchronize(s), "gat attention vector copy");
-}
-int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const double *a1, const double *a2) {
-    return guarded([&] {
-        if (!a1 || !a2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_weight(g, layer, head);  // validates layer and head
-        GATLayer &l = g->g->layers[(size_t)layer];
-        const int64_t off = (int64_t)head * l.features_per_head;
-        gat_copy(l.a1.data() + off, a1, l.features_per_head, cudaMemcpyHostToDevice);
-        gat_copy(l.a2.data() + off, a2, l.features_per_head, cudaMemcpyHostToDevice);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_gat_get_attention_vectors(hnhd_gat_t *g, int layer, int head, double *a1, double *a2) {
-    return guarded([&] {
-        if (!a1 || !a2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_weight(g, layer, head);  // validates layer and head
-        GATLayer &l = g->g->layers[(size_t)layer];
-        const int64_t off = (int64_t)head * l.features_per_head;
-        gat_copy(a1, l.a1.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
-        gat_copy(a2, l.a2.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2) {
-    return guarded([&] {
-        if (!da1 || !da2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gat_weight(g, layer, head);  // validates layer and head
-        const GATLayer &l = g->g->layers[(size_t)layer];
-        if (l.a1Grads.size() != l.a1.size() || l.a2Grads.size() != l.a2.size())
-            throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
-        const int64_t off = (int64_t)head * l.features_per_head;
-        gat_copy(da1, l.a1Grads.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
-        gat_copy(da2, l.a2Grads.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
-    });
-}
-void hnhd_gat_destroy(hnhd_gat_t *g) { delete g; }
-
-// ---- graph transformer -----------------------------------------------------------------------------
-int hnhd_gt_create(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_gt_t **out) {
-    return guarded([&] {
-        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_create: bad argument");
-        vector<GraphTransformerLayer> layers;
-        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
-        std::unique_ptr<hnhd_gt> g(new hnhd_gt);
-        g->g.reset(new GraphTransformer(layers, a->alg.get(), edge_dim, beta != 0));
-        *out = g.release();
-    });
-}
-int hnhd_gt_create_block(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, int beta, int ffn_ratio, double norm_eps,
-                         hnhd_gt_t **out) {
-    return guarded([&] {
-        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_create_block: bad argument");
-        vector<GraphTransformerLayer> layers;
-        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
-        std::unique_ptr<hnhd_gt> g(new hnhd_gt);
-        g->g.reset(new GraphTransformer(layers, a->alg.get(), edge_dim, beta != 0, ffn_ratio, norm_eps));
-        *out = g.release();
-    });
-}
-// The parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
-struct GtParam {
-    int64_t offset, rows, cols;
-};
-static GtParam gt_param(hnhd_gt_t *g, int layer, const char *name) {
-    if (!g || !name) throw hnh::Error(HNH_E_INVALID, "graph transformer: null argument");
-    GraphTransformer &m = *g->g;
-    if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no such layer");
-    const GraphTransformerLayer &l = m.layers[(size_t)layer];
-    const int64_t f = l.input_features, r = l.output_features();
-    static const char *const projections[4] = {"query", "key", "value", "skip"};
-    const string s = name;
-    for (int j = 0; j < 4; j++) {
-        if (s == projections[j]) return {l.projection_offset(j), f, r};
-        if (s == string(projections[j]) + "_bias") return {l.projection_offset(j) + f * r, r, 1};
-    }
-    if (s == "edge" && m.edge_dim > 0) return {l.edge_offset(), m.edge_dim, r};
-    if (s == "beta" && m.beta) return {l.beta_offset(m.edge_dim), 3 * r, 1};
-    if (m.ffn_ratio > 0) {
-        const int64_t h = l.hidden_features(m.ffn_ratio);
-        static const char *const block[6] = {"norm1", "norm1_bias", "ffn1", "ffn2", "norm2", "norm2_bias"};
-        const int64_t rows[6] = {r, r, r + 1, h + 1, r, r}, cols[6] = {1, 1, h, r, 1, 1};
-        for (int j = 0; j < 6; j++)
-            if (s == block[j]) return {l.block_part_offset(m.edge_dim, m.beta, m.ffn_ratio, j), rows[j], cols[j]};
-    }
-    throw hnh::Error(HNH_E_INVALID, "graph transformer: no parameter \"" + s + "\" in this model");
-}
-// copy n doubles between host and device on the compute stream and wait for the copy
-static void gt_copy(double *dst, const double *src, int64_t n, cudaMemcpyKind kind) {
-    cudaStream_t s = hnh::Runtime::get().compute_stream();
-    if (n > 0) hnh::cuda_check(cudaMemcpyAsync(dst, src, sizeof(double) * (size_t)n, kind, s), "graph transformer copy");
-    hnh::cuda_check(cudaStreamSynchronize(s), "graph transformer copy");
-}
-static DenseMatrix &gt_buffer(hnhd_gt_t *g, int buffer) {
-    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no such buffer");
-    return g->g->buffers[(size_t)buffer];
-}
-int hnhd_gt_param_shape(hnhd_gt_t *g, int layer, const char *name, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        const GtParam p = gt_param(g, layer, name);
-        if (rows) *rows = p.rows;
-        if (cols) *cols = p.cols;
-    });
-}
-int hnhd_gt_set_param(hnhd_gt_t *g, int layer, const char *name, const double *host) {
-    return guarded([&] {
-        const GtParam p = gt_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gt_copy(g->g->layers[(size_t)layer].params.data() + p.offset, host, p.rows * p.cols, cudaMemcpyHostToDevice);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_gt_get_param(hnhd_gt_t *g, int layer, const char *name, double *host) {
-    return guarded([&] {
-        const GtParam p = gt_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gt_copy(host, g->g->layers[(size_t)layer].params.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_gt_get_param_grad(hnhd_gt_t *g, int layer, const char *name, double *host) {
-    return guarded([&] {
-        const GtParam p = gt_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const GraphTransformerLayer &l = g->g->layers[(size_t)layer];
-        if (l.grads.size() != l.params.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no backward pass has run");
-        gt_copy(host, l.grads.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_gt_buffer_shape(hnhd_gt_t *g, int buffer, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        DenseMatrix &b = gt_buffer(g, buffer);
-        if (rows) *rows = b.rows();
-        if (cols) *cols = b.cols();
-    });
-}
-int hnhd_gt_set_input(hnhd_gt_t *g, const double *host) {
-    return guarded([&] {
-        DenseMatrix &b = gt_buffer(g, 0);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        b.copy_from_host(host);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_gt_set_edge_attributes(hnhd_gt_t *g, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
-        if ((n_A > 0 && !attr_A) || (n_B > 0 && !attr_B)) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        g->g->setEdgeAttributes(attr_A, n_A, attr_B, n_B);
-    });
-}
-int hnhd_gt_get_buffer(hnhd_gt_t *g, int buffer, double *host) {
-    return guarded([&] {
-        DenseMatrix &b = gt_buffer(g, buffer);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        b.copy_to_host(host);
-    });
-}
-int hnhd_gt_forward(hnhd_gt_t *g, double dropout, uint64_t seed) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
-        g->g->forwardPass(dropout, seed);
-    });
-}
-int hnhd_gt_backward(hnhd_gt_t *g, const double *host_output_grad) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
-        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const DenseMatrix &out = g->g->buffers.back();
-        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
-        g->g->backwardPass(grad);
-    });
-}
-int hnhd_gt_get_input_grad(hnhd_gt_t *g, double *host) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null graph transformer");
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        if (g->g->input_grad.size() != g->g->buffers[0].size())
-            throw hnh::Error(HNH_E_INVALID, "graph transformer: no backward pass has run");
-        g->g->input_grad.copy_to_host(host);
-    });
-}
-void hnhd_gt_destroy(hnhd_gt_t *g) { delete g; }
-
 // ---- training ------------------------------------------------------------------------------------------
 int hnhd_labels_create(hnhd_alg_t *a, const int32_t *host, int64_t n, int num_classes, hnhd_labels_t **out) {
     return guarded([&] {
@@ -882,25 +612,6 @@ int hnhd_adamw_set_lr(hnhd_adamw_t *opt, double lr) {
 }
 void hnhd_adamw_destroy(hnhd_adamw_t *opt) { delete opt; }
 
-static void train_out(const hnh::TrainResult &r, double out[4]) {
-    out[0] = r.loss;
-    out[1] = (double)r.correct;
-    out[2] = (double)r.labelled;
-    out[3] = r.grad_norm;
-}
-int hnhd_gt_train_step(hnhd_gt_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double dropout, uint64_t seed, double out[4]) {
-    return guarded([&] {
-        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_train_step: null argument");
-        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o, dropout, seed), out);
-    });
-}
-int hnhd_gat_train_step(hnhd_gat_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]) {
-    return guarded([&] {
-        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_train_step: null argument");
-        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
-    });
-}
-
 // ---- link prediction -----------------------------------------------------------------------------------------
 int hnhd_alg_link_loss(hnhd_alg_t *T, hnhd_dense_t *H_A, hnhd_dense_t *H_B, hnhd_dense_t *dH_A, hnhd_dense_t *dH_B,
                        hnhd_vec_t *scores, double out[3]) {
@@ -928,36 +639,6 @@ int hnhd_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T, hnhd_link_targets
     });
 }
 void hnhd_link_targets_destroy(hnhd_link_targets_t *t) { delete t; }
-int hnhd_gt_link_train_step(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double dropout, uint64_t seed,
-                            double out[4]) {
-    return guarded([&] {
-        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_link_train_step: null argument");
-        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o, dropout, seed), out);
-    });
-}
-int hnhd_gat_link_train_step(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]) {
-    return guarded([&] {
-        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_link_train_step: null argument");
-        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o), out);
-    });
-}
-static void link_out(const hnh::LinkResult &r, double out[3]) {
-    out[0] = r.loss;
-    out[1] = (double)r.correct;
-    out[2] = (double)r.count;
-}
-int hnhd_gt_link_evaluate(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
-    return guarded([&] {
-        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_link_evaluate: null argument");
-        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
-    });
-}
-int hnhd_gat_link_evaluate(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
-    return guarded([&] {
-        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_link_evaluate: null argument");
-        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
-    });
-}
 
 // ---- max aggregation -------------------------------------------------------------------------------------------------
 int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C) {
@@ -973,130 +654,6 @@ int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t
         a->alg->maxAggregateBackward(X->m, Z->m, C->m, dZ->m, dX->m, accumulate != 0);
     });
 }
-
-// ---- GraphSAGE -------------------------------------------------------------------------------------------------------
-int hnhd_sage_create(hnhd_alg_t *a, int n_layers, const int *layers2, const char *aggr, hnhd_sage_t **out) {
-    return guarded([&] {
-        if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_create: bad argument");
-        vector<GraphSAGELayer> layers;
-        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
-        std::unique_ptr<hnhd_sage> g(new hnhd_sage);
-        g->g.reset(new GraphSAGE(layers, a->alg.get(), aggr));
-        *out = g.release();
-    });
-}
-// the parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
-static GtParam sage_param(hnhd_sage_t *g, int layer, const char *name) {
-    if (!g || !name) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: null argument");
-    GraphSAGE &m = *g->g;
-    if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no such layer");
-    const GraphSAGELayer &l = m.layers[(size_t)layer];
-    const int64_t f = l.input_features, r = l.output_features;
-    const string s = name;
-    if (s == "neigh") return {0, f, r};
-    if (s == "neigh_bias") return {f * r, r, 1};
-    if (s == "root") return {l.root_offset(), f, r};
-    throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no parameter \"" + s + "\" (neigh, neigh_bias or root)");
-}
-static DenseMatrix &sage_buffer(hnhd_sage_t *g, int buffer) {
-    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no such buffer");
-    return g->g->buffers[(size_t)buffer];
-}
-int hnhd_sage_param_shape(hnhd_sage_t *g, int layer, const char *name, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        const GtParam p = sage_param(g, layer, name);
-        if (rows) *rows = p.rows;
-        if (cols) *cols = p.cols;
-    });
-}
-int hnhd_sage_set_param(hnhd_sage_t *g, int layer, const char *name, const double *host) {
-    return guarded([&] {
-        const GtParam p = sage_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gt_copy(g->g->layers[(size_t)layer].params.data() + p.offset, host, p.rows * p.cols, cudaMemcpyHostToDevice);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_sage_get_param(hnhd_sage_t *g, int layer, const char *name, double *host) {
-    return guarded([&] {
-        const GtParam p = sage_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gt_copy(host, g->g->layers[(size_t)layer].params.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_sage_get_param_grad(hnhd_sage_t *g, int layer, const char *name, double *host) {
-    return guarded([&] {
-        const GtParam p = sage_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const GraphSAGELayer &l = g->g->layers[(size_t)layer];
-        if (l.grads.size() != l.params.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no backward pass has run");
-        gt_copy(host, l.grads.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_sage_buffer_shape(hnhd_sage_t *g, int buffer, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        DenseMatrix &b = sage_buffer(g, buffer);
-        if (rows) *rows = b.rows();
-        if (cols) *cols = b.cols();
-    });
-}
-int hnhd_sage_set_input(hnhd_sage_t *g, const double *host) {
-    return guarded([&] {
-        DenseMatrix &b = sage_buffer(g, 0);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        b.copy_from_host(host);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_sage_get_buffer(hnhd_sage_t *g, int buffer, double *host) {
-    return guarded([&] {
-        DenseMatrix &b = sage_buffer(g, buffer);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        b.copy_to_host(host);
-    });
-}
-int hnhd_sage_forward(hnhd_sage_t *g) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null GraphSAGE");
-        g->g->forwardPass();
-    });
-}
-int hnhd_sage_backward(hnhd_sage_t *g, const double *host_output_grad) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null GraphSAGE");
-        if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const DenseMatrix &out = g->g->buffers.back();
-        DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
-        g->g->backwardPass(grad);
-    });
-}
-int hnhd_sage_get_input_grad(hnhd_sage_t *g, double *host) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null GraphSAGE");
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no backward pass has run");
-        g->g->input_grad.copy_to_host(host);
-    });
-}
-int hnhd_sage_train_step(hnhd_sage_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]) {
-    return guarded([&] {
-        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_train_step: null argument");
-        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
-    });
-}
-int hnhd_sage_link_train_step(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]) {
-    return guarded([&] {
-        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_link_train_step: null argument");
-        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o), out);
-    });
-}
-int hnhd_sage_link_evaluate(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
-    return guarded([&] {
-        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_link_evaluate: null argument");
-        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
-    });
-}
-void hnhd_sage_destroy(hnhd_sage_t *g) { delete g; }
 
 // ---- relational aggregation ------------------------------------------------------------------------------------------
 int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations) {
@@ -1128,9 +685,49 @@ int hnhd_alg_basis_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dH, hnhd_dens
     });
 }
 
-// ---- R-GCN -----------------------------------------------------------------------------------------------------------
+// ---- graph models: one handle for GAT, the graph transformer, GraphSAGE and R-GCN -------------------------------------
+int hnhd_gat_create(hnhd_alg_t *a, int n_layers, const int *layers3, double alpha, hnhd_model_t **out) {
+    return guarded([&] {
+        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_create: bad argument");
+        vector<GATLayer> layers;
+        for (int i = 0; i < n_layers; i++) {
+            if (layers3[3 * i] <= 0 || layers3[3 * i + 1] <= 0 || layers3[3 * i + 2] <= 0)
+                throw hnh::Error(HNH_E_INVALID, "hnhd_gat_create: layer sizes must be positive");
+            layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
+        }
+        std::unique_ptr<GAT> g(new GAT(layers, a->alg.get()));
+        g->leaky_relu_alpha = alpha;
+        *out = new hnhd_model{std::move(g)};
+    });
+}
+int hnhd_gt_create(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_model_t **out) {
+    return guarded([&] {
+        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_create: bad argument");
+        vector<GraphTransformerLayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
+        *out = new hnhd_model{std::unique_ptr<GraphModel>(new GraphTransformer(layers, a->alg.get(), edge_dim, beta != 0))};
+    });
+}
+int hnhd_gt_create_block(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, int beta, int ffn_ratio, double norm_eps,
+                         hnhd_model_t **out) {
+    return guarded([&] {
+        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gt_create_block: bad argument");
+        vector<GraphTransformerLayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
+        *out = new hnhd_model{
+            std::unique_ptr<GraphModel>(new GraphTransformer(layers, a->alg.get(), edge_dim, beta != 0, ffn_ratio, norm_eps))};
+    });
+}
+int hnhd_sage_create(hnhd_alg_t *a, int n_layers, const int *layers2, const char *aggr, hnhd_model_t **out) {
+    return guarded([&] {
+        if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_sage_create: bad argument");
+        vector<GraphSAGELayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
+        *out = new hnhd_model{std::unique_ptr<GraphModel>(new GraphSAGE(layers, a->alg.get(), aggr))};
+    });
+}
 static int rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, int num_bases,
-                       hnhd_rgcn_t **out, const char *who) {
+                       hnhd_model_t **out, const char *who) {
     return guarded([&] {
         if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, string(who) + ": bad argument");
         // refused before the device is touched
@@ -1140,144 +737,203 @@ static int rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_
         RGCN::check_layers(widths, num_relations, num_bases);
         vector<RGCNLayer> layers;
         for (auto [f, r] : widths) layers.emplace_back(f, r);
-        std::unique_ptr<hnhd_rgcn> g(new hnhd_rgcn);
-        g->g.reset(new RGCN(layers, a->alg.get(), num_relations, aggr, num_bases));
-        *out = g.release();
+        *out = new hnhd_model{std::unique_ptr<GraphModel>(new RGCN(layers, a->alg.get(), num_relations, aggr, num_bases))};
     });
 }
+int hnhd_rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, hnhd_model_t **out) {
+    return rgcn_create(a, n_layers, layers2, num_relations, aggr, 0, out, "hnhd_rgcn_create");
+}
 int hnhd_rgcn_create_bases(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, int num_bases, const char *aggr,
-                           hnhd_rgcn_t **out) {
+                           hnhd_model_t **out) {
     if (num_bases < 1) return hnh::set_error(HNH_E_INVALID, "hnhd_rgcn_create_bases: the basis count must be positive (got %d)", num_bases);
     return rgcn_create(a, n_layers, layers2, num_relations, aggr, num_bases, out, "hnhd_rgcn_create_bases");
 }
-int hnhd_rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, hnhd_rgcn_t **out) {
+
+// ---- every model
+int hnhd_model_buffer_shape(hnhd_model_t *m, int buffer, int64_t *rows, int64_t *cols) {
     return guarded([&] {
-        if (!a || !layers2 || !aggr || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_create: bad argument");
-        // refused before the device is touched
-        vector<std::pair<int, int>> widths;
-        for (int i = 0; i < n_layers; i++) widths.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
-        RGCN::parse(aggr);
-        RGCN::check_layers(widths, num_relations);
-        vector<RGCNLayer> layers;
-        for (auto [f, r] : widths) layers.emplace_back(f, r);
-        std::unique_ptr<hnhd_rgcn> g(new hnhd_rgcn);
-        g->g.reset(new RGCN(layers, a->alg.get(), num_relations, aggr));
-        *out = g.release();
-    });
-}
-// the parameter `name` of `layer`: its place in the layer's parameter (and gradient) vector and its shape
-static GtParam rgcn_param(hnhd_rgcn_t *g, int layer, const char *name) {
-    if (!g || !name) throw hnh::Error(HNH_E_INVALID, "RGCN: null argument");
-    RGCN &m = *g->g;
-    if (layer < 0 || layer >= (int)m.layers.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no such layer");
-    const RGCNLayer &l = m.layers[(size_t)layer];
-    const int64_t f = l.input_features, r = l.output_features, K = m.windows();
-    const string s = name;
-    if (s == "weight") return {0, K * f, r};
-    if (s == "bias") return {l.bias_offset(m.windows()), r, 1};
-    if (s == "root") return {l.root_offset(m.windows()), f, r};
-    if (s == "comp" && m.num_bases > 0) return {m.comp_offset(l), m.num_relations, m.num_bases};
-    if (m.num_bases > 0) throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + s + "\" (weight, comp, bias or root)");
-    throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + s + "\" (weight, bias or root)");
-}
-static DenseMatrix &rgcn_buffer(hnhd_rgcn_t *g, int buffer) {
-    if (!g || buffer < 0 || buffer >= (int)g->g->buffers.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no such buffer");
-    return g->g->buffers[(size_t)buffer];
-}
-int hnhd_rgcn_param_shape(hnhd_rgcn_t *g, int layer, const char *name, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        const GtParam p = rgcn_param(g, layer, name);
-        if (rows) *rows = p.rows;
-        if (cols) *cols = p.cols;
-    });
-}
-int hnhd_rgcn_set_param(hnhd_rgcn_t *g, int layer, const char *name, const double *host) {
-    return guarded([&] {
-        const GtParam p = rgcn_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gt_copy(g->g->layers[(size_t)layer].params.data() + p.offset, host, p.rows * p.cols, cudaMemcpyHostToDevice);
-        g->g->activations_current = false;
-    });
-}
-int hnhd_rgcn_get_param(hnhd_rgcn_t *g, int layer, const char *name, double *host) {
-    return guarded([&] {
-        const GtParam p = rgcn_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        gt_copy(host, g->g->layers[(size_t)layer].params.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_rgcn_get_param_grad(hnhd_rgcn_t *g, int layer, const char *name, double *host) {
-    return guarded([&] {
-        const GtParam p = rgcn_param(g, layer, name);
-        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const RGCNLayer &l = g->g->layers[(size_t)layer];
-        if (l.grads.size() != l.params.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no backward pass has run");
-        gt_copy(host, l.grads.data() + p.offset, p.rows * p.cols, cudaMemcpyDeviceToHost);
-    });
-}
-int hnhd_rgcn_buffer_shape(hnhd_rgcn_t *g, int buffer, int64_t *rows, int64_t *cols) {
-    return guarded([&] {
-        DenseMatrix &b = rgcn_buffer(g, buffer);
+        DenseMatrix &b = model_buffer(m, buffer);
         if (rows) *rows = b.rows();
         if (cols) *cols = b.cols();
     });
 }
-int hnhd_rgcn_set_input(hnhd_rgcn_t *g, const double *host) {
+int hnhd_model_set_input(hnhd_model_t *m, const double *host) {
     return guarded([&] {
-        DenseMatrix &b = rgcn_buffer(g, 0);
+        DenseMatrix &b = model_buffer(m, 0);
         if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
         b.copy_from_host(host);
-        g->g->activations_current = false;
+        m->m->activations_current = false;
     });
 }
-int hnhd_rgcn_get_buffer(hnhd_rgcn_t *g, int buffer, double *host) {
+int hnhd_model_get_buffer(hnhd_model_t *m, int buffer, double *host) {
     return guarded([&] {
-        DenseMatrix &b = rgcn_buffer(g, buffer);
+        DenseMatrix &b = model_buffer(m, buffer);
         if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
         b.copy_to_host(host);
     });
 }
-int hnhd_rgcn_forward(hnhd_rgcn_t *g) {
-    return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null RGCN");
-        g->g->forwardPass();
-    });
+int hnhd_model_forward(hnhd_model_t *m, double dropout, uint64_t seed) {
+    return guarded([&] { model(m).forward(dropout, seed); });
 }
-int hnhd_rgcn_backward(hnhd_rgcn_t *g, const double *host_output_grad) {
+int hnhd_model_backward(hnhd_model_t *m, const double *host_output_grad) {
     return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null RGCN");
+        GraphModel &g = model(m);
         if (!host_output_grad) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        const DenseMatrix &out = g->g->buffers.back();
+        const DenseMatrix &out = g.buffers.back();
         DenseMatrix grad = DenseMatrix::from_host(host_output_grad, out.rows(), out.cols());
-        g->g->backwardPass(grad);
+        g.backwardPass(grad);
     });
 }
-int hnhd_rgcn_get_input_grad(hnhd_rgcn_t *g, double *host) {
+int hnhd_model_get_input_grad(hnhd_model_t *m, double *host) {
     return guarded([&] {
-        if (!g) throw hnh::Error(HNH_E_INVALID, "null RGCN");
+        GraphModel &g = model(m);
         if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
-        if (g->g->input_grad.size() != g->g->buffers[0].size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no backward pass has run");
-        g->g->input_grad.copy_to_host(host);
+        if (g.input_grad.size() != g.buffers[0].size()) throw hnh::Error(HNH_E_INVALID, g.model_name + ": no backward pass has run");
+        g.input_grad.copy_to_host(host);
     });
 }
-int hnhd_rgcn_train_step(hnhd_rgcn_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]) {
+int hnhd_model_param_shape(hnhd_model_t *m, int layer, const char *name, int64_t *rows, int64_t *cols) {
     return guarded([&] {
-        if (!g || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_train_step: null argument");
-        train_out(hnh::trainStep(*g->g, *labels->l, *opt->o), out);
+        const ParamRef p = model_param(m, layer, name);
+        if (rows) *rows = p.rows;
+        if (cols) *cols = p.cols;
     });
 }
-int hnhd_rgcn_link_train_step(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]) {
+int hnhd_model_set_param(hnhd_model_t *m, int layer, const char *name, const double *host) {
     return guarded([&] {
-        if (!g || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_link_train_step: null argument");
-        train_out(hnh::linkTrainStep(*g->g, *t->t, *opt->o), out);
+        const ParamRef p = model_param(m, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        sync_copy(p.value, host, p.rows * p.cols, cudaMemcpyHostToDevice);
+        m->m->activations_current = false;
     });
 }
-int hnhd_rgcn_link_evaluate(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
+int hnhd_model_get_param(hnhd_model_t *m, int layer, const char *name, double *host) {
     return guarded([&] {
-        if (!g || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_rgcn_link_evaluate: null argument");
-        link_out(hnh::linkEvaluate(*g->g, *t->t, scores ? &scores->v : nullptr), out);
+        const ParamRef p = model_param(m, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        sync_copy(host, p.value, p.rows * p.cols, cudaMemcpyDeviceToHost);
     });
 }
-void hnhd_rgcn_destroy(hnhd_rgcn_t *g) { delete g; }
+int hnhd_model_get_param_grad(hnhd_model_t *m, int layer, const char *name, double *host) {
+    return guarded([&] {
+        const ParamRef p = model_param(m, layer, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (!p.grad) throw hnh::Error(HNH_E_INVALID, m->m->model_name + ": no backward pass has run");
+        sync_copy(host, p.grad, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+static void train_out(const hnh::TrainResult &r, double out[4]) {
+    out[0] = r.loss;
+    out[1] = (double)r.correct;
+    out[2] = (double)r.labelled;
+    out[3] = r.grad_norm;
+}
+int hnhd_model_train_step(hnhd_model_t *m, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double dropout, uint64_t seed,
+                          double out[4]) {
+    return guarded([&] {
+        if (!m || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_train_step: null argument");
+        train_out(hnh::trainStep(*m->m, *labels->l, *opt->o, dropout, seed), out);
+    });
+}
+int hnhd_model_link_train_step(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double dropout, uint64_t seed,
+                               double out[4]) {
+    return guarded([&] {
+        if (!m || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_link_train_step: null argument");
+        train_out(hnh::linkTrainStep(*m->m, *t->t, *opt->o, dropout, seed), out);
+    });
+}
+int hnhd_model_link_evaluate(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]) {
+    return guarded([&] {
+        if (!m || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_link_evaluate: null argument");
+        const hnh::LinkResult r = hnh::linkEvaluate(*m->m, *t->t, scores ? &scores->v : nullptr);
+        out[0] = r.loss;
+        out[1] = (double)r.correct;
+        out[2] = (double)r.count;
+    });
+}
+void hnhd_model_destroy(hnhd_model_t *m) { delete m; }
+
+// ---- GAT only: weights and attention vectors by (layer, head)
+// the layer of a (layer, head) pair, refused for another model, layer or head
+static GATLayer &gat_layer(hnhd_model_t *m, int layer, int head) {
+    GAT &g = model_as<GAT>(m, "GAT");
+    if (layer < 0 || layer >= (int)g.layers.size()) throw hnh::Error(HNH_E_INVALID, "gat: no such layer");
+    GATLayer &l = g.layers[(size_t)layer];
+    if (head < 0 || head >= l.num_heads) throw hnh::Error(HNH_E_INVALID, "gat: no such head");
+    return l;
+}
+int hnhd_gat_weight_shape(hnhd_model_t *m, int layer, int head, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        DenseMatrix &w = gat_layer(m, layer, head).wMats[(size_t)head];
+        if (rows) *rows = w.rows();
+        if (cols) *cols = w.cols();
+    });
+}
+int hnhd_gat_set_weight(hnhd_model_t *m, int layer, int head, const double *host) {
+    return guarded([&] {
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_layer(m, layer, head).wMats[(size_t)head].copy_from_host(host);
+        m->m->activations_current = false;
+    });
+}
+int hnhd_gat_get_weight(hnhd_model_t *m, int layer, int head, double *host) {
+    return guarded([&] {
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        gat_layer(m, layer, head).wMats[(size_t)head].copy_to_host(host);
+    });
+}
+int hnhd_gat_get_weight_grad(hnhd_model_t *m, int layer, int head, double *host) {
+    return guarded([&] {
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const GATLayer &l = gat_layer(m, layer, head);
+        if (l.wGrads.size() != l.wMats.size()) throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
+        l.wGrads[(size_t)head].copy_to_host(host);
+    });
+}
+int hnhd_gat_set_attention(hnhd_model_t *m, const char *kind) {
+    return guarded([&] {
+        if (!m || !kind) throw hnh::Error(HNH_E_INVALID, "hnhd_gat_set_attention: null argument");
+        model_as<GAT>(m, "GAT").set_attention(kind);
+    });
+}
+int hnhd_gat_set_attention_vectors(hnhd_model_t *m, int layer, int head, const double *a1, const double *a2) {
+    return guarded([&] {
+        if (!a1 || !a2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        GATLayer &l = gat_layer(m, layer, head);
+        const int64_t off = (int64_t)head * l.features_per_head;
+        sync_copy(l.a1.data() + off, a1, l.features_per_head, cudaMemcpyHostToDevice);
+        sync_copy(l.a2.data() + off, a2, l.features_per_head, cudaMemcpyHostToDevice);
+        m->m->activations_current = false;
+    });
+}
+int hnhd_gat_get_attention_vectors(hnhd_model_t *m, int layer, int head, double *a1, double *a2) {
+    return guarded([&] {
+        if (!a1 || !a2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        GATLayer &l = gat_layer(m, layer, head);
+        const int64_t off = (int64_t)head * l.features_per_head;
+        sync_copy(a1, l.a1.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
+        sync_copy(a2, l.a2.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_gat_get_attention_grads(hnhd_model_t *m, int layer, int head, double *da1, double *da2) {
+    return guarded([&] {
+        if (!da1 || !da2) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        const GATLayer &l = gat_layer(m, layer, head);
+        if (l.a1Grads.size() != l.a1.size() || l.a2Grads.size() != l.a2.size())
+            throw hnh::Error(HNH_E_INVALID, "gat: no backward pass has run");
+        const int64_t off = (int64_t)head * l.features_per_head;
+        sync_copy(da1, l.a1Grads.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
+        sync_copy(da2, l.a2Grads.data() + off, l.features_per_head, cudaMemcpyDeviceToHost);
+    });
+}
+
+// ---- graph transformer only
+int hnhd_gt_set_edge_attributes(hnhd_model_t *m, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B) {
+    return guarded([&] {
+        GraphTransformer &g = model_as<GraphTransformer>(m, "graph transformer");
+        if ((n_A > 0 && !attr_A) || (n_B > 0 && !attr_B)) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        g.setEdgeAttributes(attr_A, n_A, attr_B, n_B);
+    });
+}
 
 }  // extern "C"

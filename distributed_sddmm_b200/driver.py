@@ -618,15 +618,141 @@ def benchmark_algorithm(S: SpmatLocal, name: str, R: int, c: int, fused=True, ap
     return json.loads(buf.value.decode())
 
 
-class GAT:
+class _Model:
+    """What the four models share: one driver handle (hnhd_model_t) with its buffers, forward and backward passes,
+    input gradient and train steps.  _PREFIX names the model in RuntimeError texts ("sage_forward failed ...")."""
+
+    _PREFIX = ""
+
+    def _check(self, rc: int, op: str):
+        check(rc, f"{self._PREFIX}_{op}")
+
+    def buffer_shape(self, i: int):
+        r, c = C.c_int64(), C.c_int64()
+        self._check(lib().hnhd_model_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "buffer_shape")
+        return r.value, c.value
+
+    def set_input(self, x):
+        """Make the activations stale: the next backward pass needs a forward pass first."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.shape != self.buffer_shape(0):
+            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
+        self._check(lib().hnhd_model_set_input(self.h, x.ctypes.data), "set_input")
+
+    def buffer(self, i: int):
+        out = np.empty(self.buffer_shape(i), dtype=np.float64)
+        self._check(lib().hnhd_model_get_buffer(self.h, int(i), out.ctypes.data), "get_buffer")
+        return out
+
+    def forward(self):
+        """Collective."""
+        self._forward(0.0, 0)
+
+    def _forward(self, dropout, seed):
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        self._check(lib().hnhd_model_forward(self.h, p, sd), "forward")
+
+    def backward(self, grad_out):
+        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the parameters or
+        the input last changed; the gradients are then read with the model's gradient accessors and input_grad."""
+        g = np.ascontiguousarray(grad_out, dtype=np.float64)
+        last = len(self.layers)
+        if g.shape != self.buffer_shape(last):
+            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
+        self._check(lib().hnhd_model_backward(self.h, g.ctypes.data), "backward")
+
+    def input_grad(self):
+        """dL/d(network input), this rank's rows."""
+        out = np.empty(self.buffer_shape(0), dtype=np.float64)
+        self._check(lib().hnhd_model_get_input_grad(self.h, out.ctypes.data), "get_input_grad")
+        return out
+
+    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
+        """One collective training step on the device: forward, the mean cross-entropy of the output buffer against
+        labels over all ranks, backward, clipping and AdamW (see AdamW).  The forward's activations are stale
+        afterwards.  Returns TrainStep(loss, correct, labelled, grad_norm)."""
+        return self._train_step(labels, opt, 0.0, 0)
+
+    def _train_step(self, labels, opt, dropout, seed):
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        out = (C.c_double * 4)()
+        self._check(lib().hnhd_model_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), p, sd, out), "train_step")
+        return TrainStep._of(out)
+
+    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
+        """One collective link-prediction step on the device: forward, the mean binary cross-entropy of the dot-product
+        scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping and AdamW.
+        Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
+        return self._link_train_step(targets, opt, 0.0, 0)
+
+    def _link_train_step(self, targets, opt, dropout, seed):
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        out = (C.c_double * 4)()
+        self._check(lib().hnhd_model_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), p, sd, out),
+                    "link_train_step")
+        return TrainStep._of(out)
+
+    def link_evaluate(self, targets: "LinkTargets"):
+        """A forward pass without dropout and the link loss without gradients (collective): (loss, correct, count,
+        scores), the scores a numpy array in the order of targets.alg_T.entry_coordinates("A") -- for AUC or Hits@K."""
+        t = _link_targets_arg(targets)
+        out = (C.c_double * 3)()
+        scores = Vec.create(0)
+        self._check(lib().hnhd_model_link_evaluate(self.h, t, scores.h, out), "link_evaluate")
+        return float(out[0]), int(out[1]), int(out[2]), scores.to_host()
+
+    def __del__(self):
+        try:
+            lib().hnhd_model_destroy(self.h)
+        except Exception:
+            pass
+
+
+class _ModelByName(_Model):
+    """A model whose parameters are addressed by layer and name; VECTORS are the names of shape (r,)."""
+
+    VECTORS = ()
+
+    def param_names(self):
+        return list(self.PARAMS)
+
+    def param_shape(self, layer: int, name: str):
+        r, c = C.c_int64(), C.c_int64()
+        self._check(lib().hnhd_model_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "param_shape")
+        return (r.value,) if name in self.VECTORS else (r.value, c.value)
+
+    def set_param(self, layer: int, name: str, value):
+        """Make the activations stale: the next backward pass needs a forward pass first."""
+        shape = self.param_shape(layer, name)
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        if v.shape != shape:
+            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
+        self._check(lib().hnhd_model_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "set_param")
+
+    def param(self, layer: int, name: str):
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        self._check(lib().hnhd_model_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "get_param")
+        return out
+
+    def param_grad(self, layer: int, name: str):
+        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
+        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
+        self._check(lib().hnhd_model_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "get_param_grad")
+        return out
+
+
+class GAT(_Model):
     """Multi-head graph attention: forward pass and weight / input gradients (include/hnh/gat.hpp).  layers: [(input_features,
     features_per_head, num_heads), ...].  attention: "leaky" (LeakyReLU of the scores, the reference's formula),
     "softmax" (their softmax over each node's neighbours) or "additive" (the softmax of LeakyReLU(a1 . h_u + a2 . h_v),
     Velickovic et al. 2018; a1 and a2 per head through set_attention_vectors, zero by default).  The algorithm object
     must outlive this one.  "gatv2" is GATv2 attention (Brody, Alon and Yahav 2022, shared weights): the softmax of
-    a1 . LeakyReLU(h_u + h_v), with a1 set through set_attention_vectors (a2 is not read)."""
+    a1 . LeakyReLU(h_u + h_v), with a1 set through set_attention_vectors (a2 is not read).  The last layer keeps its
+    ReLU (the reference's formula), so GAT's link scores are >= 0 and it cannot score a pair below 0.5: the graph
+    transformer is the model for link prediction."""
 
     ATTENTIONS = ("leaky", "softmax", "additive", "gatv2")
+    _PREFIX = "gat"
 
     def __init__(self, alg: Algorithm, layers, leaky_relu_alpha: float = 0.2, attention: str = "leaky"):
         if attention not in self.ATTENTIONS:
@@ -650,7 +776,9 @@ class GAT:
 
     def set_weight(self, layer: int, head: int, w):
         w = np.ascontiguousarray(w, dtype=np.float64)
-        assert w.shape == self.weight_shape(layer, head), (w.shape, self.weight_shape(layer, head))
+        shape = self.weight_shape(layer, head)
+        if w.shape != shape:
+            raise ValueError(f"the weight of layer {layer}, head {head} is {shape}, got {w.shape}")
         check(lib().hnhd_gat_set_weight(self.h, layer, head, w.ctypes.data), "gat_set_weight")
 
     def weight(self, layer: int, head: int):
@@ -659,38 +787,13 @@ class GAT:
         check(lib().hnhd_gat_get_weight(self.h, layer, head, out.ctypes.data), "gat_get_weight")
         return out
 
-    def buffer_shape(self, i: int):
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_gat_buffer_shape(self.h, i, C.byref(r), C.byref(c)), "gat_buffer_shape")
-        return r.value, c.value
-
-    def set_input(self, x):
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        assert x.shape == self.buffer_shape(0), (x.shape, self.buffer_shape(0))
-        check(lib().hnhd_gat_set_input(self.h, x.ctypes.data), "gat_set_input")
-
-    def buffer(self, i: int):
-        out = np.empty(self.buffer_shape(i), dtype=np.float64)
-        check(lib().hnhd_gat_get_buffer(self.h, i, out.ctypes.data), "gat_get_buffer")
-        return out
-
-    def forward(self):
-        check(lib().hnhd_gat_forward(self.h), "gat_forward")
-
-    def backward(self, grad_out):
-        """Backward pass (collective): grad_out = dL/d(network output), this rank's rows.  Needs a forward pass
-        since the last set_weight / set_input; the gradients are then read with weight_grad / input_grad."""
-        g = np.ascontiguousarray(grad_out, dtype=np.float64)
-        last = len(self.layers)
-        assert g.shape == self.buffer_shape(last), (g.shape, self.buffer_shape(last))
-        check(lib().hnhd_gat_backward(self.h, g.ctypes.data), "gat_backward")
-
     def set_attention_vectors(self, layer: int, head: int, a1, a2):
         """The attention vectors of (layer, head), features_per_head long each (additive attention reads both, GATv2
         attention a1 only); the next backward pass needs a forward pass first."""
         fph = self.layers[layer][1]
         a1, a2 = (np.ascontiguousarray(a, dtype=np.float64) for a in (a1, a2))
-        assert a1.shape == (fph,) and a2.shape == (fph,), (a1.shape, a2.shape, fph)
+        if a1.shape != (fph,) or a2.shape != (fph,):
+            raise ValueError(f"the attention vectors of layer {layer} are ({fph},), got {a1.shape} and {a2.shape}")
         check(lib().hnhd_gat_set_attention_vectors(self.h, layer, head, a1.ctypes.data, a2.ctypes.data),
               "gat_set_attention_vectors")
 
@@ -711,49 +814,14 @@ class GAT:
               "gat_get_attention_grads")
         return da1, da2
 
-    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
-        """One collective training step on the device: forward, the mean cross-entropy of the output buffer against
-        labels over all ranks, backward, clipping and AdamW (see AdamW).  The forward's activations are stale
-        afterwards.  Returns TrainStep(loss, correct, labelled, grad_norm)."""
-        out = (C.c_double * 4)()
-        check(lib().hnhd_gat_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "gat_train_step")
-        return TrainStep._of(out)
-
-    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
-        """One collective link-prediction step on the device: forward, the mean binary cross-entropy of the dot-product
-        scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping and AdamW.
-        Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm).  The last layer keeps its ReLU (the
-        reference's formula), so GAT's scores are >= 0 and it cannot score a pair below 0.5: the graph transformer is
-        the model for link prediction."""
-        out = (C.c_double * 4)()
-        check(lib().hnhd_gat_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), out), "gat_link_train_step")
-        return TrainStep._of(out)
-
-    def link_evaluate(self, targets: "LinkTargets"):
-        """A forward pass and the link loss without gradients (collective): (loss, correct, count, scores), the scores a
-        numpy array in the order of targets.alg_T.entry_coordinates("A")."""
-        return _link_evaluate(lib().hnhd_gat_link_evaluate, self.h, targets, "gat_link_evaluate")
-
     def weight_grad(self, layer: int, head: int):
         """dL/d weight (layer, head), summed over all ranks."""
         out = np.empty(self.weight_shape(layer, head), dtype=np.float64)
         check(lib().hnhd_gat_get_weight_grad(self.h, layer, head, out.ctypes.data), "gat_get_weight_grad")
         return out
 
-    def input_grad(self):
-        """dL/d(network input), this rank's rows."""
-        out = np.empty(self.buffer_shape(0), dtype=np.float64)
-        check(lib().hnhd_gat_get_input_grad(self.h, out.ctypes.data), "gat_get_input_grad")
-        return out
 
-    def __del__(self):
-        try:
-            lib().hnhd_gat_destroy(self.h)
-        except Exception:
-            pass
-
-
-class GraphTransformer:
+class GraphTransformer(_ModelByName):
     """A graph transformer on fused sparse attention: layers of PyG's TransformerConv(concat=True, root_weight=True)
     with the heads concatenated, forward and backward (include/hnh/graph_transformer.hpp).  layers: [(input_features,
     features_per_head, num_heads), ...]; every layer but the last ends in a ReLU.  edge_dim > 0 adds edge features
@@ -772,6 +840,7 @@ class GraphTransformer:
     PROJECTIONS = ("query", "key", "value", "skip")
     VECTORS = ("query_bias", "key_bias", "value_bias", "skip_bias", "beta", "norm1", "norm1_bias", "norm2", "norm2_bias")
     BLOCK = ("norm1", "norm1_bias", "ffn1", "ffn2", "norm2", "norm2_bias")
+    _PREFIX = "gt"
 
     def __init__(self, alg: Algorithm, layers, edge_dim: int = 0, beta: bool = False, ffn_ratio: int = 0,
                  norm_eps: float = 1e-5):
@@ -801,41 +870,6 @@ class GraphTransformer:
         names += (["edge"] if self.edge_dim else []) + (["beta"] if self.beta else [])
         return names + (list(self.BLOCK) if getattr(self, "ffn_ratio", 0) else [])
 
-    def param_shape(self, layer: int, name: str):
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_gt_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "gt_param_shape")
-        return (r.value,) if name in self.VECTORS else (r.value, c.value)
-
-    def set_param(self, layer: int, name: str, value):
-        """Make the activations stale: the next backward pass needs a forward pass first."""
-        shape = self.param_shape(layer, name)
-        v = np.ascontiguousarray(value, dtype=np.float64)
-        if v.shape != shape:
-            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
-        check(lib().hnhd_gt_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "gt_set_param")
-
-    def param(self, layer: int, name: str):
-        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
-        check(lib().hnhd_gt_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "gt_get_param")
-        return out
-
-    def param_grad(self, layer: int, name: str):
-        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
-        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
-        check(lib().hnhd_gt_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "gt_get_param_grad")
-        return out
-
-    def buffer_shape(self, i: int):
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_gt_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "gt_buffer_shape")
-        return r.value, c.value
-
-    def set_input(self, x):
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.shape != self.buffer_shape(0):
-            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
-        check(lib().hnhd_gt_set_input(self.h, x.ctypes.data), "gt_set_input")
-
     def set_edge_attributes(self, attr_A, attr_B):
         """The edge attributes of this rank's entries: attr_A (len(like_S_values()) x edge_dim) in the order of
         alg.entry_coordinates("A"), attr_B (len(like_ST_values()) x edge_dim) in that of entry_coordinates("B"), both
@@ -849,66 +883,26 @@ class GraphTransformer:
         check(lib().hnhd_gt_set_edge_attributes(self.h, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0]),
               "gt_set_edge_attributes")
 
-    def buffer(self, i: int):
-        out = np.empty(self.buffer_shape(i), dtype=np.float64)
-        check(lib().hnhd_gt_get_buffer(self.h, int(i), out.ctypes.data), "gt_get_buffer")
-        return out
-
     def forward(self, dropout: float = 0.0, seed: int = 0):
         """Collective.  dropout in [0, 1) is the attention dropout of every layer; layer l draws its masks at seed +
         the heads of the layers before it, so no two (layer, head) pairs share one.  Every rank passes the same
-        values."""
-        p, sd = Algorithm._dropout_args(dropout, seed)
-        check(lib().hnhd_gt_forward(self.h, p, sd), "gt_forward")
-
-    def backward(self, grad_out):
-        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the last
-        set_param / set_input / set_edge_attributes and regenerates its dropout masks; the gradients are then read
-        with param_grad / input_grad."""
-        g = np.ascontiguousarray(grad_out, dtype=np.float64)
-        last = len(self.layers)
-        if g.shape != self.buffer_shape(last):
-            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
-        check(lib().hnhd_gt_backward(self.h, g.ctypes.data), "gt_backward")
+        values.  The backward pass regenerates the masks."""
+        self._forward(dropout, seed)
 
     def train_step(self, labels: "NodeLabels", opt: "AdamW", dropout: float = 0.0, seed: int = 0) -> "TrainStep":
         """One collective training step on the device: forward(dropout, seed), the mean cross-entropy of the output
         buffer against labels over all ranks, backward, clipping and AdamW (see AdamW).  The forward's activations are
         stale afterwards.  Returns TrainStep(loss, correct, labelled, grad_norm)."""
-        p, sd = Algorithm._dropout_args(dropout, seed)
-        out = (C.c_double * 4)()
-        check(lib().hnhd_gt_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), p, sd, out), "gt_train_step")
-        return TrainStep._of(out)
+        return self._train_step(labels, opt, dropout, seed)
 
     def link_train_step(self, targets: "LinkTargets", opt: "AdamW", dropout: float = 0.0, seed: int = 0) -> "TrainStep":
         """One collective link-prediction step on the device: forward(dropout, seed), the mean binary cross-entropy of
         the dot-product scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping
         and AdamW.  Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
-        p, sd = Algorithm._dropout_args(dropout, seed)
-        out = (C.c_double * 4)()
-        check(lib().hnhd_gt_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), p, sd, out),
-              "gt_link_train_step")
-        return TrainStep._of(out)
-
-    def link_evaluate(self, targets: "LinkTargets"):
-        """A forward pass without dropout and the link loss without gradients (collective): (loss, correct, count,
-        scores), the scores a numpy array in the order of targets.alg_T.entry_coordinates("A") -- for AUC or Hits@K."""
-        return _link_evaluate(lib().hnhd_gt_link_evaluate, self.h, targets, "gt_link_evaluate")
-
-    def input_grad(self):
-        """dL/d(network input), this rank's rows."""
-        out = np.empty(self.buffer_shape(0), dtype=np.float64)
-        check(lib().hnhd_gt_get_input_grad(self.h, out.ctypes.data), "gt_get_input_grad")
-        return out
-
-    def __del__(self):
-        try:
-            lib().hnhd_gt_destroy(self.h)
-        except Exception:
-            pass
+        return self._link_train_step(targets, opt, dropout, seed)
 
 
-class GraphSAGE:
+class GraphSAGE(_ModelByName):
     """GraphSAGE: layers of PyG's SAGEConv(aggr, root_weight=True, project=False, normalize=False), forward and backward
     (include/hnh/graph_sage.hpp).  layers: [(input_features, output_features), ...]; aggr: "mean", "sum" or "max" over
     the stored entries of each S-row on all ranks (duplicates count; a row without entries aggregates to 0).  Every
@@ -921,6 +915,8 @@ class GraphSAGE:
 
     AGGREGATIONS = ("mean", "sum", "max")
     PARAMS = ("neigh", "neigh_bias", "root")
+    VECTORS = ("neigh_bias",)
+    _PREFIX = "sage"
 
     def __init__(self, alg: Algorithm, layers, aggr: str = "mean"):
         self.alg = alg
@@ -934,98 +930,8 @@ class GraphSAGE:
         self.h = C.c_void_p()
         check(lib().hnhd_sage_create(alg.h, len(self.layers), flat, aggr.encode(), C.byref(self.h)), "sage_create")
 
-    def param_names(self):
-        return list(self.PARAMS)
 
-    def param_shape(self, layer: int, name: str):
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_sage_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "sage_param_shape")
-        return (r.value,) if name == "neigh_bias" else (r.value, c.value)
-
-    def set_param(self, layer: int, name: str, value):
-        """Make the activations stale: the next backward pass needs a forward pass first."""
-        shape = self.param_shape(layer, name)
-        v = np.ascontiguousarray(value, dtype=np.float64)
-        if v.shape != shape:
-            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
-        check(lib().hnhd_sage_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "sage_set_param")
-
-    def param(self, layer: int, name: str):
-        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
-        check(lib().hnhd_sage_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "sage_get_param")
-        return out
-
-    def param_grad(self, layer: int, name: str):
-        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
-        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
-        check(lib().hnhd_sage_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "sage_get_param_grad")
-        return out
-
-    def buffer_shape(self, i: int):
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_sage_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "sage_buffer_shape")
-        return r.value, c.value
-
-    def set_input(self, x):
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.shape != self.buffer_shape(0):
-            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
-        check(lib().hnhd_sage_set_input(self.h, x.ctypes.data), "sage_set_input")
-
-    def buffer(self, i: int):
-        out = np.empty(self.buffer_shape(i), dtype=np.float64)
-        check(lib().hnhd_sage_get_buffer(self.h, int(i), out.ctypes.data), "sage_get_buffer")
-        return out
-
-    def forward(self):
-        """Collective."""
-        check(lib().hnhd_sage_forward(self.h), "sage_forward")
-
-    def backward(self, grad_out):
-        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the last set_param
-        / set_input; the gradients are then read with param_grad / input_grad."""
-        g = np.ascontiguousarray(grad_out, dtype=np.float64)
-        last = len(self.layers)
-        if g.shape != self.buffer_shape(last):
-            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
-        check(lib().hnhd_sage_backward(self.h, g.ctypes.data), "sage_backward")
-
-    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
-        """One collective training step on the device: forward, the mean cross-entropy of the output buffer against
-        labels over all ranks, backward, clipping and AdamW (see AdamW).  Returns TrainStep(loss, correct, labelled,
-        grad_norm)."""
-        out = (C.c_double * 4)()
-        check(lib().hnhd_sage_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "sage_train_step")
-        return TrainStep._of(out)
-
-    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
-        """One collective link-prediction step on the device: forward, the mean binary cross-entropy of the dot-product
-        scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping and AdamW.
-        Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
-        out = (C.c_double * 4)()
-        check(lib().hnhd_sage_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), out),
-              "sage_link_train_step")
-        return TrainStep._of(out)
-
-    def link_evaluate(self, targets: "LinkTargets"):
-        """A forward pass and the link loss without gradients (collective): (loss, correct, count, scores), the scores
-        a numpy array in the order of targets.alg_T.entry_coordinates("A")."""
-        return _link_evaluate(lib().hnhd_sage_link_evaluate, self.h, targets, "sage_link_evaluate")
-
-    def input_grad(self):
-        """dL/d(network input), this rank's rows."""
-        out = np.empty(self.buffer_shape(0), dtype=np.float64)
-        check(lib().hnhd_sage_get_input_grad(self.h, out.ctypes.data), "sage_get_input_grad")
-        return out
-
-    def __del__(self):
-        try:
-            lib().hnhd_sage_destroy(self.h)
-        except Exception:
-            pass
-
-
-class RGCN:
+class RGCN(_ModelByName):
     """R-GCN: layers of PyG's RGCNConv(in, out, num_relations, num_bases, aggr, root_weight=True, bias=True) without
     block decomposition, forward and backward (include/hnh/rgcn.hpp).  The relation of each stored entry of the
     algorithm's S is its stored value, an integer in [0, num_relations); construction refuses any other value on any
@@ -1043,6 +949,8 @@ class RGCN:
     AGGREGATIONS = ("mean", "sum")
     PARAMS = ("weight", "bias", "root")
     BASIS_PARAMS = ("weight", "comp", "bias", "root")
+    VECTORS = ("bias",)
+    _PREFIX = "rgcn"
 
     def __init__(self, alg: Algorithm, layers, num_relations: int, aggr: str = "mean", num_bases: int | None = None):
         self.alg = alg
@@ -1077,88 +985,7 @@ class RGCN:
     def param_shape(self, layer: int, name: str):
         if name not in self._params():
             raise ValueError(f"no parameter {name!r}: one of {self._params()}")
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_rgcn_param_shape(self.h, int(layer), name.encode(), C.byref(r), C.byref(c)), "rgcn_param_shape")
-        return (r.value,) if name == "bias" else (r.value, c.value)
-
-    def set_param(self, layer: int, name: str, value):
-        """Make the activations stale: the next backward pass needs a forward pass first."""
-        shape = self.param_shape(layer, name)
-        v = np.ascontiguousarray(value, dtype=np.float64)
-        if v.shape != shape:
-            raise ValueError(f"{name} of layer {layer} is {shape}, got {v.shape}")
-        check(lib().hnhd_rgcn_set_param(self.h, int(layer), name.encode(), v.ctypes.data), "rgcn_set_param")
-
-    def param(self, layer: int, name: str):
-        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
-        check(lib().hnhd_rgcn_get_param(self.h, int(layer), name.encode(), out.ctypes.data), "rgcn_get_param")
-        return out
-
-    def param_grad(self, layer: int, name: str):
-        """dL/d param after a backward pass, summed over all ranks (identical on every rank)."""
-        out = np.empty(self.param_shape(layer, name), dtype=np.float64)
-        check(lib().hnhd_rgcn_get_param_grad(self.h, int(layer), name.encode(), out.ctypes.data), "rgcn_get_param_grad")
-        return out
-
-    def buffer_shape(self, i: int):
-        r, c = C.c_int64(), C.c_int64()
-        check(lib().hnhd_rgcn_buffer_shape(self.h, int(i), C.byref(r), C.byref(c)), "rgcn_buffer_shape")
-        return r.value, c.value
-
-    def set_input(self, x):
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.shape != self.buffer_shape(0):
-            raise ValueError(f"the input is {self.buffer_shape(0)}, got {x.shape}")
-        check(lib().hnhd_rgcn_set_input(self.h, x.ctypes.data), "rgcn_set_input")
-
-    def buffer(self, i: int):
-        out = np.empty(self.buffer_shape(i), dtype=np.float64)
-        check(lib().hnhd_rgcn_get_buffer(self.h, int(i), out.ctypes.data), "rgcn_get_buffer")
-        return out
-
-    def forward(self):
-        """Collective."""
-        check(lib().hnhd_rgcn_forward(self.h), "rgcn_forward")
-
-    def backward(self, grad_out):
-        """Collective: grad_out = dL/d(network output), this rank's rows.  Needs a forward pass since the last set_param
-        / set_input; the gradients are then read with param_grad / input_grad."""
-        g = np.ascontiguousarray(grad_out, dtype=np.float64)
-        last = len(self.layers)
-        if g.shape != self.buffer_shape(last):
-            raise ValueError(f"the output gradient is {self.buffer_shape(last)}, got {g.shape}")
-        check(lib().hnhd_rgcn_backward(self.h, g.ctypes.data), "rgcn_backward")
-
-    def train_step(self, labels: "NodeLabels", opt: "AdamW") -> "TrainStep":
-        """One collective node-classification step on the device, as GraphSAGE.train_step."""
-        out = (C.c_double * 4)()
-        check(lib().hnhd_rgcn_train_step(self.h, _labels_arg(labels), _adamw_arg(opt), out), "rgcn_train_step")
-        return TrainStep._of(out)
-
-    def link_train_step(self, targets: "LinkTargets", opt: "AdamW") -> "TrainStep":
-        """One collective link-prediction step on the device (the dot-product decoder on the output buffer), as
-        GraphSAGE.link_train_step."""
-        out = (C.c_double * 4)()
-        check(lib().hnhd_rgcn_link_train_step(self.h, _link_targets_arg(targets), _adamw_arg(opt), out),
-              "rgcn_link_train_step")
-        return TrainStep._of(out)
-
-    def link_evaluate(self, targets: "LinkTargets"):
-        """A forward pass and the link loss without gradients (collective): (loss, correct, count, scores), the scores
-        a numpy array in the order of targets.alg_T.entry_coordinates("A")."""
-        return _link_evaluate(lib().hnhd_rgcn_link_evaluate, self.h, targets, "rgcn_link_evaluate")
-
-    def input_grad(self):
-        """dL/d(network input), this rank's rows."""
-        out = np.empty(self.buffer_shape(0), dtype=np.float64)
-        check(lib().hnhd_rgcn_get_input_grad(self.h, out.ctypes.data), "rgcn_get_input_grad")
-        return out
-
-    def __del__(self):
-        try:
-            lib().hnhd_rgcn_destroy(self.h)
-        except Exception:
-            pass
+        return super().param_shape(layer, name)
 
 
 class TrainStep(NamedTuple):
@@ -1262,14 +1089,6 @@ def _link_targets_arg(targets):
     if not isinstance(targets, LinkTargets):
         raise TypeError(f"targets must be a LinkTargets, not {type(targets).__name__}")
     return targets.h
-
-
-def _link_evaluate(fn, h, targets, what):
-    t = _link_targets_arg(targets)
-    out = (C.c_double * 3)()
-    scores = Vec.create(0)
-    check(fn(h, t, scores.h, out), what)
-    return float(out[0]), int(out[1]), int(out[2]), scores.to_host()
 
 
 def _labels_arg(labels):

@@ -72,10 +72,9 @@
 
 #include "hnh/15D_dense_shift.hpp"
 #include "hnh/distributed_sparse.h"
+#include "hnh/model.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
-
-struct ParamSpan;  // hnh/training.hpp
 
 class GATLayer {
 public:
@@ -98,14 +97,12 @@ public:
     int output_features() const { return features_per_head * num_heads; }
 };
 
-class GAT {
+class GAT : public GraphModel {
 public:
-    Distributed_Sparse *d_ops;
     vector<GATLayer> layers;
-    vector<DenseMatrix> buffers;  // [0] network input (B-shaped), [i + 1] output of layer i (A-shaped)
     double leaky_relu_alpha = 0.2;
 
-    GAT(vector<GATLayer> &l_input, Distributed_Sparse *ops) : d_ops(ops), layers(l_input) {
+    GAT(vector<GATLayer> &l_input, Distributed_Sparse *ops) : GraphModel(ops, "gat"), layers(l_input) {
         if (layers.empty()) throw hnh::Error(-1, "GAT: no layers");
         for (size_t i = 1; i < layers.size(); i++)
             if (layers[i].input_features != layers[i - 1].output_features())
@@ -128,6 +125,11 @@ public:
             layer.a2 = VectorXd::Constant((int64_t)layer.num_heads * layer.features_per_head, 0.0);
         }
     }
+
+    // GAT's key function, defined in the library (csrc/benchmark_dist.cpp): the vtable, and the backward pass it names
+    // (which calls the CUDA runtime), are emitted there, so a program that only constructs GAT and runs forwardPass
+    // links without the CUDA runtime, as the reference's drivers do
+    ~GAT() override;
 
     // head j of layer i: reads buffers[i], writes its column window of buffers[i + 1]
     void computeSelfAttentionHead(int i, int j) {
@@ -170,20 +172,30 @@ public:
             for (int j = 0; j < layers[i].num_heads; j++) computeSelfAttentionHead((int)i, j);
         activations_current = true;
     }
+    void forward(double dropout, uint64_t) override {
+        refuse_dropout(dropout);
+        forwardPass();
+    }
 
     // ---- backward pass -------------------------------------------------------------------------------
-    DenseMatrix input_grad;  // dL/d buffers[0] after backwardPass (B-shaped, like buffers[0])
-    // The activations in `buffers` belong to the current wMats and input.  forwardPass sets it; whoever changes
-    // wMats or buffers[0] clears it (the driver ABI does), and backwardPass refuses to run on stale activations.
-    bool activations_current = false;
-
     // Throws HNH_E_INVALID unless the backward pass is defined on this algorithm object (see the top of this
     // file).  Decided from global quantities only, so every rank throws together and no collective is left waiting.
     void check_backward_supported() const { d_ops->check_full_rows("GAT::backwardPass"); }
+    void check_trainable() const override { check_backward_supported(); }
 
     // Every (layer, head) weight with its gradient, then a1 and a2 of every layer with theirs; grad is null before the
-    // first backward pass.  Defined in hnh/training.hpp.  Read afresh for every use: set_weight may replace storage.
-    std::vector<ParamSpan> parameters();
+    // first backward pass.
+    std::vector<ParamSpan> parameters() override {
+        std::vector<ParamSpan> s;
+        for (GATLayer &l : layers)
+            for (size_t h = 0; h < l.wMats.size(); h++)
+                s.push_back({l.wMats[h].data(), l.wGrads.size() == l.wMats.size() ? l.wGrads[h].data() : nullptr, l.wMats[h].size()});
+        for (GATLayer &l : layers) {
+            s.push_back({l.a1.data(), l.a1Grads.size() == l.a1.size() ? l.a1Grads.data() : nullptr, l.a1.size()});
+            s.push_back({l.a2.data(), l.a2Grads.size() == l.a2.size() ? l.a2Grads.data() : nullptr, l.a2.size()});
+        }
+        return s;
+    }
 
     // "leaky" (the reference's attention, the default), "softmax", "additive" or "gatv2" (see the top of this file).
     // Changing it makes the activations stale.
@@ -203,7 +215,7 @@ public:
     // in layers[i].a1Grads / a2Grads (summed over all ranks: identical everywhere), and dL/d buffers[0] in
     // input_grad.  Collective.  Reads buffers, wMats, a1, a2 and leaky_relu_alpha and changes none of them; gradient
     // storage is allocated on the first call.
-    void backwardPass(const DenseMatrix &output_grad) {
+    void backwardPass(const DenseMatrix &output_grad) override {
         check_backward_supported();
         if (!activations_current)
             throw hnh::Error(HNH_E_INVALID, "GAT::backwardPass: no forward pass since the weights or the input changed");

@@ -34,10 +34,9 @@
 #include <vector>
 
 #include "hnh/distributed_sparse.h"
+#include "hnh/model.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
-
-struct ParamSpan;  // hnh/training.hpp
 
 class GraphSAGELayer {
 public:
@@ -52,23 +51,17 @@ public:
     int64_t param_count() const { return (2 * (int64_t)input_features + 1) * output_features; }
 };
 
-class GraphSAGE {
+class GraphSAGE : public GraphModel {
 public:
     enum Aggregation { kMean, kSum, kMax };
 
-    Distributed_Sparse *d_ops;
     vector<GraphSAGELayer> layers;
-    vector<DenseMatrix> buffers;  // [0] network input (B-shaped), [i + 1] output of layer i (A-shaped)
     const Aggregation aggr;
     vector<DenseMatrix> aggregated, counts;  // A (and C for max) of every layer from the last forward pass
-    DenseMatrix input_grad;                  // dL/d buffers[0] after backwardPass
-    // The activations belong to the current parameters and input: forwardPass sets it, whoever changes one of them
-    // clears it, and backwardPass refuses to run on stale activations.
-    bool activations_current = false;
 
     // aggr: "mean", "sum" or "max"
     GraphSAGE(vector<GraphSAGELayer> &l_input, Distributed_Sparse *ops, const string &aggregation)
-        : d_ops(ops), layers(l_input), aggr(parse(aggregation)) {
+        : GraphModel(ops, "GraphSAGE"), layers(l_input), aggr(parse(aggregation)) {
         d_ops->check_full_rows("GraphSAGE");
         if (layers.empty()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no layers");
         for (size_t i = 0; i < layers.size(); i++) {
@@ -121,9 +114,23 @@ public:
         return DenseMatrix::view(v.data() + l.root_offset(), l.input_features, l.output_features);
     }
 
-    // Each layer's params with its grads, one span per layer; grad is null before the first backward pass.  Defined in
-    // hnh/training.hpp.
-    std::vector<ParamSpan> parameters();
+    // Each layer's params with its grads, one span per layer
+    std::vector<ParamSpan> parameters() override {
+        std::vector<ParamSpan> s;
+        for (GraphSAGELayer &l : layers) s.push_back(span(l.params, l.grads));
+        return s;
+    }
+
+    // By name (the layout above): "neigh" (W_l, f x r), "neigh_bias" (b_l, r x 1), "root" (W_r, f x r)
+    ParamRef param(int layer, const string &name) override {
+        if (layer < 0 || layer >= (int)layers.size()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no such layer");
+        GraphSAGELayer &l = layers[(size_t)layer];
+        const int64_t f = l.input_features, r = l.output_features;
+        if (name == "neigh") return slice(l.params, l.grads, 0, f, r);
+        if (name == "neigh_bias") return slice(l.params, l.grads, f * r, r, 1);
+        if (name == "root") return slice(l.params, l.grads, l.root_offset(), f, r);
+        throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no parameter \"" + name + "\" (neigh, neigh_bias or root)");
+    }
 
     // Collective.
     void forwardPass() {
@@ -144,10 +151,14 @@ public:
         }
         activations_current = true;
     }
+    void forward(double dropout, uint64_t) override {
+        refuse_dropout(dropout);
+        forwardPass();
+    }
 
     // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d params in layers[i].grads (summed over all
     // ranks) and dL/d buffers[0] in input_grad.  Collective.
-    void backwardPass(const DenseMatrix &output_grad) {
+    void backwardPass(const DenseMatrix &output_grad) override {
         d_ops->check_full_rows("GraphSAGE::backwardPass");
         if (!activations_current)
             throw hnh::Error(HNH_E_INVALID, "GraphSAGE::backwardPass: no forward pass since the parameters or the input changed");

@@ -50,10 +50,9 @@
 #include <vector>
 
 #include "hnh/distributed_sparse.h"
+#include "hnh/model.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
-
-struct ParamSpan;  // hnh/training.hpp
 
 class GraphTransformerLayer {
 public:
@@ -87,11 +86,9 @@ public:
     }
 };
 
-class GraphTransformer {
+class GraphTransformer : public GraphModel {
 public:
-    Distributed_Sparse *d_ops;
     vector<GraphTransformerLayer> layers;
-    vector<DenseMatrix> buffers;  // [0] network input (B-shaped), [i + 1] output of layer i (A-shaped)
     const int edge_dim;
     const bool beta;
     const int ffn_ratio;    // > 0: transformer blocks with hidden width ffn_ratio * r
@@ -100,14 +97,11 @@ public:
     bool has_edge_attributes = false;
     vector<DenseMatrix> attention, lse;   // M and L of every layer from the last forward pass
     vector<DenseMatrix> norm_stats;       // with blocks: (mean, rstd) per row of LN1 and LN2 of layer i at [2i], [2i + 1]
-    DenseMatrix input_grad;               // dL/d buffers[0] after backwardPass
-    // The activations belong to the current parameters, input and edge attributes: forwardPass sets it, whoever
-    // changes one of them clears it, and backwardPass refuses to run on stale activations.
-    bool activations_current = false;
+    // activations_current also covers the edge attributes
 
     GraphTransformer(vector<GraphTransformerLayer> &l_input, Distributed_Sparse *ops, int edge_features, bool gate,
                      int ffn = 0, double eps = 1e-5)
-        : d_ops(ops), layers(l_input), edge_dim(edge_features), beta(gate), ffn_ratio(ffn), norm_eps(eps) {
+        : GraphModel(ops, "graph transformer"), layers(l_input), edge_dim(edge_features), beta(gate), ffn_ratio(ffn), norm_eps(eps) {
         d_ops->check_full_rows("GraphTransformer");
         if (layers.empty()) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: no layers");
         if (edge_dim < 0) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: edge_dim must not be negative");
@@ -174,9 +168,37 @@ public:
         activations_current = false;
     }
 
-    // Each layer's params with its grads, one span per layer; grad is null before the first backward pass.  Defined in
-    // hnh/training.hpp.
-    std::vector<ParamSpan> parameters();
+    // Each layer's params with its grads, one span per layer
+    std::vector<ParamSpan> parameters() override {
+        std::vector<ParamSpan> s;
+        for (GraphTransformerLayer &l : layers) s.push_back(span(l.params, l.grads));
+        return s;
+    }
+
+    // By name (the layout above): "query", "key", "value", "skip" (f x r) and their "_bias" (r x 1), "edge" (edge_dim x
+    // r) with edge features, "beta" (3r x 1) with the gate; with blocks "norm1", "norm1_bias" (r x 1), "ffn1" ((r + 1) x
+    // h), "ffn2" ((h + 1) x r), "norm2", "norm2_bias"
+    ParamRef param(int layer, const string &name) override {
+        if (layer < 0 || layer >= (int)layers.size()) throw hnh::Error(HNH_E_INVALID, "graph transformer: no such layer");
+        GraphTransformerLayer &l = layers[(size_t)layer];
+        const int64_t f = l.input_features, r = l.output_features();
+        auto at = [&](int64_t offset, int64_t rows, int64_t cols) { return slice(l.params, l.grads, offset, rows, cols); };
+        static const char *const projections[4] = {"query", "key", "value", "skip"};
+        for (int j = 0; j < 4; j++) {
+            if (name == projections[j]) return at(l.projection_offset(j), f, r);
+            if (name == string(projections[j]) + "_bias") return at(l.projection_offset(j) + f * r, r, 1);
+        }
+        if (name == "edge" && edge_dim > 0) return at(l.edge_offset(), edge_dim, r);
+        if (name == "beta" && beta) return at(l.beta_offset(edge_dim), 3 * r, 1);
+        if (ffn_ratio > 0) {
+            const int64_t h = l.hidden_features(ffn_ratio);
+            static const char *const block[6] = {"norm1", "norm1_bias", "ffn1", "ffn2", "norm2", "norm2_bias"};
+            const int64_t rows[6] = {r, r, r + 1, h + 1, r, r}, cols[6] = {1, 1, h, r, 1, 1};
+            for (int j = 0; j < 6; j++)
+                if (name == block[j]) return at(l.block_part_offset(edge_dim, beta, ffn_ratio, j), rows[j], cols[j]);
+        }
+        throw hnh::Error(HNH_E_INVALID, "graph transformer: no parameter \"" + name + "\" in this model");
+    }
 
     // Collective.  dropout in [0, 1) and seed go to every layer's attention (seed_l as above); the backward pass
     // regenerates the same masks.
@@ -218,10 +240,11 @@ public:
         seed_ = seed;
         activations_current = true;
     }
+    void forward(double dropout, uint64_t seed) override { forwardPass(dropout, seed); }
 
     // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d params in layers[i].grads (summed over all
     // ranks) and dL/d buffers[0] in input_grad.  Collective.  Uses the forward pass's dropout and seed.
-    void backwardPass(const DenseMatrix &output_grad) {
+    void backwardPass(const DenseMatrix &output_grad) override {
         check_supported("GraphTransformer::backwardPass", dropout_);
         if (!activations_current)
             throw hnh::Error(HNH_E_INVALID,

@@ -44,10 +44,9 @@
 #include <vector>
 
 #include "hnh/distributed_sparse.h"
+#include "hnh/model.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
-
-struct ParamSpan;  // hnh/training.hpp
 
 class RGCNLayer {
 public:
@@ -63,20 +62,14 @@ public:
     int64_t param_count(int R) const { return (((int64_t)R + 1) * input_features + 1) * output_features; }
 };
 
-class RGCN {
+class RGCN : public GraphModel {
 public:
     enum Aggregation { kMean, kSum };
 
-    Distributed_Sparse *d_ops;
     vector<RGCNLayer> layers;
     const int num_relations;
-    vector<DenseMatrix> buffers;  // [0] network input (B-shaped), [i + 1] output of layer i (A-shaped)
     const Aggregation aggr;
     vector<DenseMatrix> aggregated;  // Ab (localArows x R f), or H with bases (localArows x B f), of every layer
-    DenseMatrix input_grad;          // dL/d buffers[0] after backwardPass
-    // The activations belong to the current parameters and input: forwardPass sets it, whoever changes one of them
-    // clears it, and backwardPass refuses to run on stale activations.
-    bool activations_current = false;
     const int num_bases;  // B >= 1: basis decomposition; 0: none
 
     // aggr: "mean" or "sum".  Collective: checks every stored value of S (Distributed_Sparse::relationCheck).
@@ -85,7 +78,7 @@ public:
 
     // The same with `bases` bases (0: without decomposition, as above).
     RGCN(vector<RGCNLayer> &l_input, Distributed_Sparse *ops, int relations, const string &aggregation, int bases)
-        : d_ops(ops), layers(l_input), num_relations(relations), aggr(parse(aggregation)), num_bases(bases) {
+        : GraphModel(ops, "RGCN"), layers(l_input), num_relations(relations), aggr(parse(aggregation)), num_bases(bases) {
         vector<std::pair<int, int>> widths;
         for (const RGCNLayer &l : layers) widths.emplace_back(l.input_features, l.output_features);
         check_layers(widths, num_relations, num_bases);
@@ -162,9 +155,26 @@ public:
         return DenseMatrix::view(v.data() + comp_offset(l), num_relations, num_bases);
     }
 
-    // Each layer's params with its grads, one span per layer; grad is null before the first backward pass.  Defined in
-    // hnh/training.hpp.
-    std::vector<ParamSpan> parameters();
+    // Each layer's params with its grads, one span per layer
+    std::vector<ParamSpan> parameters() override {
+        std::vector<ParamSpan> s;
+        for (RGCNLayer &l : layers) s.push_back(span(l.params, l.grads));
+        return s;
+    }
+
+    // By name (the layout above): "weight" (R f x r, or B f x r with bases), "bias" (r x 1), "root" (f x r), and with
+    // bases "comp" (R x B)
+    ParamRef param(int layer, const string &name) override {
+        if (layer < 0 || layer >= (int)layers.size()) throw hnh::Error(HNH_E_INVALID, "RGCN: no such layer");
+        RGCNLayer &l = layers[(size_t)layer];
+        const int64_t f = l.input_features, r = l.output_features, K = windows();
+        if (name == "weight") return slice(l.params, l.grads, 0, K * f, r);
+        if (name == "bias") return slice(l.params, l.grads, l.bias_offset(windows()), r, 1);
+        if (name == "root") return slice(l.params, l.grads, l.root_offset(windows()), f, r);
+        if (name == "comp" && num_bases > 0) return slice(l.params, l.grads, comp_offset(l), num_relations, num_bases);
+        if (num_bases > 0) throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + name + "\" (weight, comp, bias or root)");
+        throw hnh::Error(HNH_E_INVALID, "RGCN: no parameter \"" + name + "\" (weight, bias or root)");
+    }
 
     // Collective.
     void forwardPass() {
@@ -191,10 +201,14 @@ public:
         }
         activations_current = true;
     }
+    void forward(double dropout, uint64_t) override {
+        refuse_dropout(dropout);
+        forwardPass();
+    }
 
     // output_grad = dL/d buffers.back() (this rank's rows).  Leaves dL/d params in layers[i].grads (summed over all
     // ranks) and dL/d buffers[0] in input_grad.  Collective.
-    void backwardPass(const DenseMatrix &output_grad) {
+    void backwardPass(const DenseMatrix &output_grad) override {
         d_ops->check_full_rows("RGCN::backwardPass");
         if (!activations_current)
             throw hnh::Error(HNH_E_INVALID, "RGCN::backwardPass: no forward pass since the parameters or the input changed");

@@ -1,4 +1,4 @@
-// hnh/training.hpp -- training GAT and the graph transformer on the device: a masked cross-entropy loss for node
+// hnh/training.hpp -- training the graph models on the device: a masked cross-entropy loss for node
 // classification, gradient-norm clipping and AdamW, and one collective train step.  torch is the definition:
 //     loss = F.cross_entropy(logits, labels, ignore_index = <any negative>, reduction = "mean") over the labelled rows of
 //            all ranks (0 and a zero gradient when no row is labelled anywhere; torch gives NaN there)
@@ -12,7 +12,8 @@
 // Link prediction (LinkTargets, linkTrainStep, linkEvaluate, at the end) shares the step: its loss is the binary
 // cross-entropy of dot-product scores over the entries of a target matrix (Distributed_Sparse::linkLoss).
 //
-// Parameters are device spans read afresh at every step (set_weight may replace a matrix's storage), in a fixed order:
+// One step serves every GraphModel (hnh/model.hpp): GAT, GraphTransformer, GraphSAGE and RGCN.  Parameters are device
+// spans read afresh at every step (set_weight may replace a matrix's storage), in a fixed order:
 //     GraphTransformer, GraphSAGE, RGCN: each layer's params vector with its grads, one span per layer;
 //     GAT: every (layer, head) weight with its gradient, then a1 and a2 of every layer with theirs.  Where an attention
 //     kind does not read a1 or a2 their gradient is 0, and AdamW's decoupled decay alone moves them.
@@ -24,51 +25,9 @@
 
 #include "hnh/15D_dense_shift.hpp"
 #include "hnh/comm.h"
-#include "hnh/gat.hpp"
-#include "hnh/graph_sage.hpp"
-#include "hnh/graph_transformer.hpp"
-#include "hnh/rgcn.hpp"
+#include "hnh/model.hpp"
 #include "hnh/world_allreduce.hpp"
 #include "hnh_b200.h"
-
-struct ParamSpan {
-    double *param;
-    const double *grad;  // null before the model's first backward pass
-    int64_t n;
-};
-
-inline std::vector<ParamSpan> GAT::parameters() {
-    std::vector<ParamSpan> s;
-    for (GATLayer &l : layers)
-        for (size_t h = 0; h < l.wMats.size(); h++)
-            s.push_back({l.wMats[h].data(), l.wGrads.size() == l.wMats.size() ? l.wGrads[h].data() : nullptr, l.wMats[h].size()});
-    for (GATLayer &l : layers) {
-        s.push_back({l.a1.data(), l.a1Grads.size() == l.a1.size() ? l.a1Grads.data() : nullptr, l.a1.size()});
-        s.push_back({l.a2.data(), l.a2Grads.size() == l.a2.size() ? l.a2Grads.data() : nullptr, l.a2.size()});
-    }
-    return s;
-}
-
-inline std::vector<ParamSpan> GraphTransformer::parameters() {
-    std::vector<ParamSpan> s;
-    for (GraphTransformerLayer &l : layers)
-        s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
-    return s;
-}
-
-inline std::vector<ParamSpan> GraphSAGE::parameters() {
-    std::vector<ParamSpan> s;
-    for (GraphSAGELayer &l : layers)
-        s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
-    return s;
-}
-
-inline std::vector<ParamSpan> RGCN::parameters() {
-    std::vector<ParamSpan> s;
-    for (RGCNLayer &l : layers)
-        s.push_back({l.params.data(), l.grads.size() == l.params.size() ? l.grads.data() : nullptr, l.params.size()});
-    return s;
-}
 
 namespace hnh {
 
@@ -227,40 +186,13 @@ TrainResult finishStep(Model &net, int64_t count, AdamW &opt, Loss loss, Backwar
 }
 }  // namespace detail
 
-// One training step of the graph transformer (see the top of this file).  Collective.  Refuses, on every rank before
-// any launch, labels of another row count or class count, an optimizer of other parameters and a layout the model
-// refuses.  Leaves the activations stale.
-inline TrainResult trainStep(GraphTransformer &net, const NodeLabels &labels, AdamW &opt, double dropout, uint64_t seed) {
+// One training step (see the top of this file): forward(dropout, seed) -- models without dropout refuse dropout != 0 --,
+// cross-entropy, backward, clip and AdamW.  Collective.  Refuses, on every rank before any launch, labels of another row
+// count or class count, an optimizer of other parameters and a layout the model refuses.  Leaves the activations stale.
+inline TrainResult trainStep(GraphModel &net, const NodeLabels &labels, AdamW &opt, double dropout, uint64_t seed) {
     detail::check_train(net.buffers.back(), labels, opt, net.parameters());
-    net.forwardPass(dropout, seed);
-    return detail::finishStep(
-        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
-}
-
-// The same for GAT (no dropout).
-inline TrainResult trainStep(GAT &net, const NodeLabels &labels, AdamW &opt) {
-    detail::check_train(net.buffers.back(), labels, opt, net.parameters());
-    net.check_backward_supported();
-    net.forwardPass();
-    return detail::finishStep(
-        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
-}
-
-// The same for GraphSAGE (no dropout).
-inline TrainResult trainStep(GraphSAGE &net, const NodeLabels &labels, AdamW &opt) {
-    detail::check_train(net.buffers.back(), labels, opt, net.parameters());
-    net.forwardPass();
-    return detail::finishStep(
-        net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
-}
-
-// The same for RGCN (no dropout).
-inline TrainResult trainStep(RGCN &net, const NodeLabels &labels, AdamW &opt) {
-    detail::check_train(net.buffers.back(), labels, opt, net.parameters());
-    net.forwardPass();
+    net.check_trainable();
+    net.forward(dropout, seed);
     return detail::finishStep(
         net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
         [&](const DenseMatrix &g) { net.backwardPass(g); });
@@ -341,42 +273,15 @@ inline LinkResult linkResult(DenseMatrix &H, const LinkTargets &targets, VectorX
 }
 }  // namespace detail
 
-// One link-prediction training step of the graph transformer: forward(dropout, seed), the mean binary cross-entropy of
-// the scores of T's entries (LinkTargets) with its gradient dH from Distributed_Sparse::linkLoss, backwardPass(dH),
-// clip and AdamW, as trainStep.  TrainResult's `labelled` is the entry count of T.  Collective.  Refuses, on every rank
-// before any launch, targets made for another model's algorithm object, an optimizer of other parameters and a layout
-// the model refuses.  Leaves the activations stale.
-inline TrainResult linkTrainStep(GraphTransformer &net, const LinkTargets &targets, AdamW &opt, double dropout, uint64_t seed) {
+// One link-prediction training step: forward(dropout, seed), the mean binary cross-entropy of the scores of T's entries
+// (LinkTargets) with its gradient dH from Distributed_Sparse::linkLoss, backwardPass(dH), clip and AdamW, as trainStep.
+// TrainResult's `labelled` is the entry count of T.  Collective.  Refuses, on every rank before any launch, targets made
+// for another model's algorithm object, an optimizer of other parameters and a layout the model refuses.  Leaves the
+// activations stale.  GAT's last layer keeps its ReLU, so its scores are >= 0; the other models' last layers have none.
+inline TrainResult linkTrainStep(GraphModel &net, const LinkTargets &targets, AdamW &opt, double dropout, uint64_t seed) {
     detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
-    net.forwardPass(dropout, seed);
-    return detail::finishStep(
-        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
-}
-
-// The same for GAT (no dropout).  Its last layer keeps its ReLU, so its scores are >= 0.
-inline TrainResult linkTrainStep(GAT &net, const LinkTargets &targets, AdamW &opt) {
-    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
-    net.check_backward_supported();
-    net.forwardPass();
-    return detail::finishStep(
-        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
-}
-
-// The same for GraphSAGE (no dropout).  Its last layer has no ReLU, so its scores take either sign.
-inline TrainResult linkTrainStep(GraphSAGE &net, const LinkTargets &targets, AdamW &opt) {
-    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
-    net.forwardPass();
-    return detail::finishStep(
-        net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
-}
-
-// The same for RGCN (no dropout): the dot-product decoder on its embeddings.  Its last layer has no ReLU.
-inline TrainResult linkTrainStep(RGCN &net, const LinkTargets &targets, AdamW &opt) {
-    detail::check_link(net.d_ops, targets, &opt, net.parameters(), "linkTrainStep");
-    net.forwardPass();
+    net.check_trainable();
+    net.forward(dropout, seed);
     return detail::finishStep(
         net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
         [&](const DenseMatrix &g) { net.backwardPass(g); });
@@ -385,25 +290,9 @@ inline TrainResult linkTrainStep(RGCN &net, const LinkTargets &targets, AdamW &o
 // A forward pass without dropout and the link loss without gradients: (mean loss, correct, count) over all ranks, and
 // scores (nullable, resized) = s in the order of T's like_S_values (Distributed_Sparse::entryCoordinates(k_sddmmA) of
 // T gives their node pairs).  Collective.
-inline LinkResult linkEvaluate(GraphTransformer &net, const LinkTargets &targets, VectorXd *scores) {
+inline LinkResult linkEvaluate(GraphModel &net, const LinkTargets &targets, VectorXd *scores) {
     detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
-    net.forwardPass(0.0, 0);
-    return detail::linkResult(net.buffers.back(), targets, scores);
-}
-inline LinkResult linkEvaluate(GAT &net, const LinkTargets &targets, VectorXd *scores) {
-    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
-    net.forwardPass();
-    return detail::linkResult(net.buffers.back(), targets, scores);
-}
-inline LinkResult linkEvaluate(GraphSAGE &net, const LinkTargets &targets, VectorXd *scores) {
-    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
-    net.forwardPass();
-    return detail::linkResult(net.buffers.back(), targets, scores);
-}
-
-inline LinkResult linkEvaluate(RGCN &net, const LinkTargets &targets, VectorXd *scores) {
-    detail::check_link(net.d_ops, targets, nullptr, {}, "linkEvaluate");
-    net.forwardPass();
+    net.forward(0.0, 0);
     return detail::linkResult(net.buffers.back(), targets, scores);
 }
 

@@ -257,94 +257,6 @@ int hnhd_als_run(hnhd_alg_t *alg, const double *hostAgt, const double *hostBgt, 
                  const double *hostB0, int steps, int cg_iters, double *out2, double *hostA_out,
                  double *hostB_out);
 
-/* ---- GAT forward pass (include/hnh/gat.hpp; reference gat.hpp:26-113) -----------------------
- * layers3: n_layers triples (input_features, features_per_head, num_heads).  The object keeps a
- * pointer to `alg`, which must outlive it.  buffer 0 is the network input, buffer i + 1 the output
- * of layer i; weights are input_width x head_width, row-major, as hnhd_gat_weight_shape reports. */
-typedef struct hnhd_gat hnhd_gat_t;
-int hnhd_gat_create(hnhd_alg_t *alg, int n_layers, const int *layers3, double leaky_relu_alpha,
-                    hnhd_gat_t **out);
-int hnhd_gat_weight_shape(hnhd_gat_t *g, int layer, int head, int64_t *rows, int64_t *cols);
-int hnhd_gat_set_weight(hnhd_gat_t *g, int layer, int head, const double *host);
-int hnhd_gat_get_weight(hnhd_gat_t *g, int layer, int head, double *host); /* synchronises (e.g. after train steps) */
-int hnhd_gat_buffer_shape(hnhd_gat_t *g, int buffer, int64_t *rows, int64_t *cols);
-int hnhd_gat_set_input(hnhd_gat_t *g, const double *host);          /* buffer 0 */
-int hnhd_gat_get_buffer(hnhd_gat_t *g, int buffer, double *host);   /* synchronises */
-int hnhd_gat_forward(hnhd_gat_t *g);                                /* forwardPass(); stream-ordered */
-/* GAT backward pass (GAT::backwardPass): host_output_grad = dL/d(last buffer), this rank's rows, in the
- * shape hnhd_gat_buffer_shape reports for the last buffer.  Collective.  HNH_E_INVALID on every rank where the
- * layout has no backward pass (R-split layouts at p > 1; 1.5D dense shift with local kernel fusion at c > 1),
- * and when no forward pass has run since the last set_weight / set_input.  The gradients are then read with: */
-int hnhd_gat_backward(hnhd_gat_t *g, const double *host_output_grad);
-/* dL/d weight (layer, head), summed over all ranks (identical on every rank); hnhd_gat_weight_shape's shape */
-int hnhd_gat_get_weight_grad(hnhd_gat_t *g, int layer, int head, double *host);
-/* dL/d buffer 0 (this rank's rows); hnhd_gat_buffer_shape(0)'s shape */
-int hnhd_gat_get_input_grad(hnhd_gat_t *g, double *host);
-/* attention of every head (GAT::set_attention): "leaky" (the default: LeakyReLU of the scores, the
- * reference's formula), "softmax" (their edge softmax over each row of S) or "additive" (below).  Makes the
- * activations stale.
- * With "softmax" the forward pass raises HNH_E_INVALID on every rank, before any launch, where the layout has
- * no edge softmax (as hnhd_alg_edge_softmax). */
-int hnhd_gat_set_attention(hnhd_gat_t *g, const char *kind);
-/* "gatv2": x_uv = a1 . LeakyReLU(h_u + h_v) (GATv2 with shared weights, Brody, Alon and Yahav 2022), then the edge
- * softmax; a1 is set with hnhd_gat_set_attention_vectors (a2 is not read, its gradient stays zero).  Defined on
- * the layouts where "softmax" is. */
-/* additive attention ("additive": x_uv = LeakyReLU(a1 . h_u + a2 . h_v) with h = X W the head's projection,
- * then the edge softmax; Velickovic et al. 2018): the attention vectors of (layer, head), features_per_head
- * doubles each (host pointers; zero after hnhd_gat_create: uniform attention).  Makes the activations stale.
- * "additive" is defined on the layouts where "softmax" is. */
-int hnhd_gat_set_attention_vectors(hnhd_gat_t *g, int layer, int head, const double *a1, const double *a2);
-int hnhd_gat_get_attention_vectors(hnhd_gat_t *g, int layer, int head, double *a1, double *a2); /* synchronises */
-/* dL/d a1 and dL/d a2 of (layer, head) after hnhd_gat_backward (features_per_head doubles each, summed over all
- * ranks; zero unless the attention is additive).  HNH_E_INVALID before the first backward pass. */
-int hnhd_gat_get_attention_grads(hnhd_gat_t *g, int layer, int head, double *da1, double *da2);
-void hnhd_gat_destroy(hnhd_gat_t *g);
-
-/* ---- graph transformer (include/hnh/graph_transformer.hpp): TransformerConv layers on fused sparse attention ---
- * layers3: n_layers triples (input_features, features_per_head, num_heads); every layer concatenates its heads, so
- * layer i + 1 takes features_per_head * num_heads of layer i.  edge_dim > 0 adds edge features (attributes of S's
- * entries projected by each layer's "edge" weight onto the keys and values), beta != 0 the gated skip connection.
- * The object keeps a pointer to `alg`, which must outlive it.  HNH_E_INVALID on every rank, before any launch,
- * where the layout has no fused sparse attention (as hnhd_alg_edge_softmax), and for bad layer sizes. */
-typedef struct hnhd_gt hnhd_gt_t;
-int hnhd_gt_create(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_gt_t **out);
-/* The same with transformer blocks: ffn_ratio = k >= 1 makes every layer a post-norm block, LN2(H1 + FFN(H1)) with
- * H1 = LN1(the layer's output without ReLU) and a ReLU FFN of hidden width k r; LayerNorm epsilon norm_eps.  ffn_ratio
- * = 0 is hnhd_gt_create.  HNH_E_INVALID for ffn_ratio < 0 or a norm_eps that is not finite and > 0. */
-int hnhd_gt_create_block(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, int ffn_ratio,
-                         double norm_eps, hnhd_gt_t **out);
-/* Parameters by layer and name: "query", "key", "value", "skip" (input_features x r, row-major: the transpose of
- * PyG's lin_*.weight), "query_bias", "key_bias", "value_bias", "skip_bias" (r x 1), "edge" (edge_dim x r; models
- * with edge features only), "beta" (3r x 1, the weight of PyG's lin_beta; gated models only).  Models with blocks
- * (ffn_ratio > 0, hidden width h) add "norm1", "norm1_bias" (r x 1; LN1's weight and bias), "ffn1" ((r + 1) x h:
- * lin1.weight^T with lin1.bias as the last row), "ffn2" ((h + 1) x r), "norm2", "norm2_bias".  All zero after
- * hnhd_gt_create, except the LayerNorm weights, which are 1.  set_param makes the activations stale; get_param_grad reads dL/d param after hnhd_gt_backward,
- * summed over all ranks (identical on every rank). */
-int hnhd_gt_param_shape(hnhd_gt_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
-int hnhd_gt_set_param(hnhd_gt_t *g, int layer, const char *name, const double *host);
-int hnhd_gt_get_param(hnhd_gt_t *g, int layer, const char *name, double *host);
-int hnhd_gt_get_param_grad(hnhd_gt_t *g, int layer, const char *name, double *host);
-/* buffer 0 is the network input, buffer i + 1 the output of layer i (this rank's rows) */
-int hnhd_gt_buffer_shape(hnhd_gt_t *g, int buffer, int64_t *rows, int64_t *cols);
-int hnhd_gt_set_input(hnhd_gt_t *g, const double *host);
-int hnhd_gt_get_buffer(hnhd_gt_t *g, int buffer, double *host); /* synchronises */
-/* Edge attributes of this rank's entries in both value orders: attr_A is n_A x edge_dim in the order of
- * hnhd_vec_like(.., 0, ..) (hnhd_alg_entry_coordinates mode 0), attr_B n_B x edge_dim in the B order; n_A and n_B
- * must be this rank's entry counts.  Both hold the same attribute for every stored (u, v).  Makes the activations
- * stale.  HNH_E_INVALID for a model without edge features or wrong counts. */
-int hnhd_gt_set_edge_attributes(hnhd_gt_t *g, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B);
-/* Forward pass with attention dropout `dropout` in [0, 1): layer l uses the dropout seed seed + the heads of the
- * layers before it.  Collective, stream-ordered.  HNH_E_INVALID before any launch for a bad dropout or a model with
- * edge features whose attributes were not set. */
-int hnhd_gt_forward(hnhd_gt_t *g, double dropout, uint64_t seed);
-/* Backward pass: host_output_grad = dL/d(last buffer), this rank's rows; regenerates the forward's dropout masks.
- * Collective.  HNH_E_INVALID when no forward pass has run since the last set_param / set_input /
- * set_edge_attributes. */
-int hnhd_gt_backward(hnhd_gt_t *g, const double *host_output_grad);
-/* dL/d buffer 0 (this rank's rows) after hnhd_gt_backward */
-int hnhd_gt_get_input_grad(hnhd_gt_t *g, double *host);
-void hnhd_gt_destroy(hnhd_gt_t *g);
-
 /* ---- training (include/hnh/training.hpp): cross-entropy, clipping and AdamW on the device -------------------------
  * Labels of this rank's rows of the model's output buffer (alg's localArows of them), one int32 per row: a class in
  * [0, num_classes) or negative for "ignored" (padding rows and unlabelled nodes must be negative).  Collective: a bad
@@ -362,15 +274,6 @@ int hnhd_adamw_create(double lr, double beta1, double beta2, double eps, double 
                       hnhd_adamw_t **out);
 int hnhd_adamw_set_lr(hnhd_adamw_t *opt, double lr);
 void hnhd_adamw_destroy(hnhd_adamw_t *opt);
-/* One training step: forward (the graph transformer with attention dropout `dropout` and `seed`), the mean
- * cross-entropy of the output buffer against the labels over all ranks, the backward pass, clipping and AdamW.
- * out = {loss, correct, labelled, grad_norm}: the loss, the labelled rows whose argmax is their label and the labelled
- * rows (all ranks), and the gradient norm before clipping.  With no labelled row the loss and the gradient are 0.
- * Collective; afterwards the activations are stale.  HNH_E_INVALID on every rank before any launch for labels of
- * another row or class count, an optimizer of other parameter sizes, and layouts without a backward pass. */
-int hnhd_gt_train_step(hnhd_gt_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double dropout, uint64_t seed,
-                       double out[4]);
-int hnhd_gat_train_step(hnhd_gat_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
 
 /* ---- link prediction: a dot-product edge decoder with binary cross-entropy (Distributed_Sparse::linkLoss) ---------
  * On the algorithm object of a target matrix T (its stored values are the targets y_uv in [0, 1]; an SDDMM, SpMM or
@@ -389,47 +292,6 @@ int hnhd_alg_link_loss(hnhd_alg_t *T, hnhd_dense_t *H_A, hnhd_dense_t *H_B, hnhd
 typedef struct hnhd_link_targets hnhd_link_targets_t;
 int hnhd_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T, hnhd_link_targets_t **out);
 void hnhd_link_targets_destroy(hnhd_link_targets_t *t);
-/* One link-prediction training step: forward, the mean binary cross-entropy of the output buffer's dot-product scores
- * over T's entries, the backward pass, clipping and AdamW.  out = {loss, correct, count, grad_norm}.  GAT's last layer
- * keeps its ReLU, so its scores are >= 0: the graph transformer is the model for link prediction.  Collective;
- * HNH_E_INVALID on every rank before any launch for targets of another model's algorithm object, an optimizer of
- * other parameter sizes, and layouts without a backward pass. */
-int hnhd_gt_link_train_step(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double dropout, uint64_t seed,
-                            double out[4]);
-int hnhd_gat_link_train_step(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]);
-/* A forward pass without dropout and the link loss without gradients: out = {loss, correct, count}; scores (nullable)
- * is resized and receives s in the A order of T (hnhd_alg_entry_coordinates(T, 0, ..) gives the pairs).  Collective. */
-int hnhd_gt_link_evaluate(hnhd_gt_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
-int hnhd_gat_link_evaluate(hnhd_gat_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
-
-/* ---- GraphSAGE (include/hnh/graph_sage.hpp) ----------------------------------------------------------------------
- * Layers of PyG's SAGEConv(aggr, root_weight = True): layers2 = {input_features, output_features} per layer; aggr is
- * "mean", "sum" or "max".  Every layer but the last ends in a ReLU.  Parameters (zero after construction), by layer
- * and name: "neigh" (input_features x r: lin_l.weight.T), "neigh_bias" (r x 1: lin_l.bias), "root" (input_features x
- * r: lin_r.weight.T).  Buffers: 0 is the input (B-shaped), i + 1 the output of layer i (A-shaped).  set_param and
- * set_input make the activations stale; get_param_grad reads dL/d param after hnhd_sage_backward, summed over all
- * ranks.  Collective where the model's algorithm is; HNH_E_INVALID on every rank before any launch where
- * hnhd_alg_edge_softmax is, for unknown aggregations, non-positive sizes, widths that do not chain, and a backward
- * on stale activations.  The algorithm object must outlive the model. */
-typedef struct hnhd_sage hnhd_sage_t;
-int hnhd_sage_create(hnhd_alg_t *alg, int n_layers, const int *layers2, const char *aggr, hnhd_sage_t **out);
-int hnhd_sage_param_shape(hnhd_sage_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
-int hnhd_sage_set_param(hnhd_sage_t *g, int layer, const char *name, const double *host);
-int hnhd_sage_get_param(hnhd_sage_t *g, int layer, const char *name, double *host);
-int hnhd_sage_get_param_grad(hnhd_sage_t *g, int layer, const char *name, double *host);
-int hnhd_sage_buffer_shape(hnhd_sage_t *g, int buffer, int64_t *rows, int64_t *cols);
-int hnhd_sage_set_input(hnhd_sage_t *g, const double *host);
-int hnhd_sage_get_buffer(hnhd_sage_t *g, int buffer, double *host); /* synchronises */
-int hnhd_sage_forward(hnhd_sage_t *g);
-/* host_output_grad: dL/d(the last buffer), this rank's rows */
-int hnhd_sage_backward(hnhd_sage_t *g, const double *host_output_grad);
-/* dL/d buffer 0 (this rank's rows) after hnhd_sage_backward */
-int hnhd_sage_get_input_grad(hnhd_sage_t *g, double *host);
-/* hnhd_gt_train_step, hnhd_gt_link_train_step and hnhd_gt_link_evaluate for GraphSAGE (no dropout) */
-int hnhd_sage_train_step(hnhd_sage_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
-int hnhd_sage_link_train_step(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]);
-int hnhd_sage_link_evaluate(hnhd_sage_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
-void hnhd_sage_destroy(hnhd_sage_t *g);
 
 /* ---- max aggregation (Distributed_Sparse::maxAggregate) -------------------------------------------------------------
  * Z, C (A-shaped, f wide) = the per-column maximum of X (B-shaped) over the stored entries of each S-row and the number
@@ -440,33 +302,6 @@ int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd
 int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C, hnhd_dense_t *dZ,
                                     hnhd_dense_t *dX, int accumulate);
 
-/* ---- R-GCN (include/hnh/rgcn.hpp) ----------------------------------------------------------------------------------
- * Layers of PyG's RGCNConv(in, out, num_relations, aggr, root_weight = True, bias = True) without basis or block
- * decomposition: layers2 = {input_features, output_features} per layer; aggr is "mean" or "sum".  The relation of each
- * stored entry of S is its stored value, an integer in [0, num_relations); create refuses any other value on any rank.
- * Every layer but the last ends in a ReLU.  Parameters (zero after construction), by layer and name: "weight"
- * (num_relations * input_features x r: RGCNConv.weight reshaped, no transpose), "bias" (r x 1), "root"
- * (input_features x r).  Buffers, staleness and gradients as hnhd_sage_*.  Collective where the model's algorithm is;
- * HNH_E_INVALID on every rank before any launch where hnhd_alg_edge_softmax is, for unknown aggregations,
- * num_relations < 1, non-positive sizes, widths that do not chain, R f >= 2^31, and a backward on stale activations.
- * The algorithm object must outlive the model. */
-typedef struct hnhd_rgcn hnhd_rgcn_t;
-int hnhd_rgcn_create(hnhd_alg_t *alg, int n_layers, const int *layers2, int num_relations, const char *aggr, hnhd_rgcn_t **out);
-int hnhd_rgcn_param_shape(hnhd_rgcn_t *g, int layer, const char *name, int64_t *rows, int64_t *cols);
-int hnhd_rgcn_set_param(hnhd_rgcn_t *g, int layer, const char *name, const double *host);
-int hnhd_rgcn_get_param(hnhd_rgcn_t *g, int layer, const char *name, double *host);
-int hnhd_rgcn_get_param_grad(hnhd_rgcn_t *g, int layer, const char *name, double *host);
-int hnhd_rgcn_buffer_shape(hnhd_rgcn_t *g, int buffer, int64_t *rows, int64_t *cols);
-int hnhd_rgcn_set_input(hnhd_rgcn_t *g, const double *host);
-int hnhd_rgcn_get_buffer(hnhd_rgcn_t *g, int buffer, double *host); /* synchronises */
-int hnhd_rgcn_forward(hnhd_rgcn_t *g);
-int hnhd_rgcn_backward(hnhd_rgcn_t *g, const double *host_output_grad);
-int hnhd_rgcn_get_input_grad(hnhd_rgcn_t *g, double *host);
-int hnhd_rgcn_train_step(hnhd_rgcn_t *g, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double out[4]);
-int hnhd_rgcn_link_train_step(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double out[4]);
-int hnhd_rgcn_link_evaluate(hnhd_rgcn_t *g, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
-void hnhd_rgcn_destroy(hnhd_rgcn_t *g);
-
 /* ---- relational aggregation (Distributed_Sparse::relationalAggregate) -----------------------------------------------
  * A (A-shaped, num_relations * f wide) = for each S-row u and relation rho, the sum of X_v (B-shaped, f wide) over the
  * stored entries (u, v) whose value is rho (0 where there are none; entries whose value is not an integer in
@@ -476,11 +311,7 @@ void hnhd_rgcn_destroy(hnhd_rgcn_t *g);
 int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations);
 int hnhd_alg_relational_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dA, hnhd_dense_t *dX, int num_relations, int accumulate);
 
-/* ---- R-GCN with basis decomposition (include/hnh/rgcn.hpp, Distributed_Sparse::basisAggregate) ---------------------
- * hnhd_rgcn_create_bases: the model of hnhd_rgcn_create with PyG's num_bases = B >= 1: W_rho = sum_b comp[rho, b] V_b.
- * Parameters by layer and name: "weight" (B f x r: RGCNConv.weight.reshape(-1, r)), "comp" (R x B), "bias" and "root"
- * as without bases.  Refuses num_bases < 1 and B f or R B >= 2^31 besides what hnhd_rgcn_create refuses; every other
- * hnhd_rgcn_* call works on the model unchanged.
+/* ---- basis aggregation (Distributed_Sparse::basisAggregate) ----------------------------------------------------------
  * hnhd_alg_basis_aggregate: H (A-shaped, B f wide, B = comp's columns) = for each S-row u and basis b, the sum over the
  * stored entries (u, v) of scale[u, rho] comp[rho, b] X_v (X B-shaped, f wide; comp R x B; scale A-shaped and R wide,
  * or null for ones).  hnhd_alg_basis_aggregate_backward: dX (overwritten, or added to with accumulate != 0) =
@@ -488,12 +319,136 @@ int hnhd_alg_relational_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dA, hnhd
  * the same on every rank) = sum over the stored entries of relation rho on all ranks of scale[u, rho]
  * <dH[u, b f .. b f + f), X_v>.  Collective; HNH_E_INVALID on every rank where hnhd_alg_edge_softmax is, for
  * num_relations < 1, B < 1, wrong shapes, and for an output that is another operand. */
-int hnhd_rgcn_create_bases(hnhd_alg_t *alg, int n_layers, const int *layers2, int num_relations, int num_bases, const char *aggr,
-                           hnhd_rgcn_t **out);
 int hnhd_alg_basis_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *H, hnhd_dense_t *comp, int num_relations,
                              hnhd_dense_t *scale);
 int hnhd_alg_basis_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *dH, hnhd_dense_t *X, hnhd_dense_t *dX, hnhd_dense_t *comp,
                                       hnhd_dense_t *dcomp, int num_relations, hnhd_dense_t *scale, int accumulate);
+
+/* ---- graph models: GAT, the graph transformer, GraphSAGE and R-GCN behind one handle ---------------------------------
+ * The constructors below return an hnhd_model_t; every hnhd_model_* call takes any of them, the GAT and graph transformer
+ * calls below only a model of their kind (another kind is refused with HNH_E_INVALID).  A model keeps a pointer to its `alg`,
+ * which must outlive it.  Buffers: 0 is the network input (B-shaped), i + 1 the output of layer i (A-shaped), this
+ * rank's rows.  Parameters are zero after construction unless stated otherwise.  Changing a parameter, the input (or a
+ * model's own state: GAT's attention, the graph transformer's edge attributes) makes the activations stale; a backward
+ * pass on stale activations, and a gradient read before the first backward pass, are refused with HNH_E_INVALID.
+ * Gradients of parameters are summed over all ranks (identical on every rank).  Forward, backward and the steps are
+ * collective and refuse, on every rank before any launch, a layout the model does not support. */
+typedef struct hnhd_model hnhd_model_t;
+int hnhd_model_buffer_shape(hnhd_model_t *m, int buffer, int64_t *rows, int64_t *cols);
+int hnhd_model_set_input(hnhd_model_t *m, const double *host);         /* buffer 0 */
+int hnhd_model_get_buffer(hnhd_model_t *m, int buffer, double *host);  /* synchronises */
+/* Forward pass with attention dropout `dropout` in [0, 1) and `seed` (the graph transformer; every rank passes the same
+ * values).  The other models have no dropout and refuse dropout != 0.  Stream-ordered. */
+int hnhd_model_forward(hnhd_model_t *m, double dropout, uint64_t seed);
+/* host_output_grad = dL/d(the last buffer), this rank's rows, in the shape hnhd_model_buffer_shape reports for it */
+int hnhd_model_backward(hnhd_model_t *m, const double *host_output_grad);
+/* dL/d buffer 0 (this rank's rows) after hnhd_model_backward */
+int hnhd_model_get_input_grad(hnhd_model_t *m, double *host);
+/* A parameter by layer and name (see the models below): rows x cols doubles, row-major.  get_param synchronises;
+ * get_param_grad reads dL/d param after hnhd_model_backward.  GAT has no parameters by name and refuses: its weights and
+ * attention vectors are read and written by (layer, head) with the GAT calls below. */
+int hnhd_model_param_shape(hnhd_model_t *m, int layer, const char *name, int64_t *rows, int64_t *cols);
+int hnhd_model_set_param(hnhd_model_t *m, int layer, const char *name, const double *host);
+int hnhd_model_get_param(hnhd_model_t *m, int layer, const char *name, double *host);
+int hnhd_model_get_param_grad(hnhd_model_t *m, int layer, const char *name, double *host);
+/* One training step: forward(dropout, seed), the mean cross-entropy of the output buffer against the labels over all
+ * ranks, the backward pass, clipping and AdamW.  out = {loss, correct, labelled, grad_norm}: the loss, the labelled rows
+ * whose argmax is their label and the labelled rows (all ranks), and the gradient norm before clipping.  With no
+ * labelled row the loss and the gradient are 0.  Collective; afterwards the activations are stale.  HNH_E_INVALID on
+ * every rank before any launch for labels of another row or class count, an optimizer of other parameter sizes,
+ * dropout on a model without it, and layouts without a backward pass. */
+int hnhd_model_train_step(hnhd_model_t *m, const hnhd_labels_t *labels, hnhd_adamw_t *opt, double dropout, uint64_t seed,
+                          double out[4]);
+/* One link-prediction training step: forward(dropout, seed), the mean binary cross-entropy of the output buffer's
+ * dot-product scores over T's entries, the backward pass, clipping and AdamW.  out = {loss, correct, count, grad_norm}.
+ * GAT's last layer keeps its ReLU, so its scores are >= 0; the other models' last layers have none.  Collective;
+ * HNH_E_INVALID on every rank before any launch for targets of another model's algorithm object, an optimizer of other
+ * parameter sizes, dropout on a model without it, and layouts without a backward pass. */
+int hnhd_model_link_train_step(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd_adamw_t *opt, double dropout,
+                               uint64_t seed, double out[4]);
+/* A forward pass without dropout and the link loss without gradients: out = {loss, correct, count}; scores (nullable)
+ * is resized and receives s in the A order of T (hnhd_alg_entry_coordinates(T, 0, ..) gives the pairs).  Collective. */
+int hnhd_model_link_evaluate(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
+void hnhd_model_destroy(hnhd_model_t *m);
+
+/* ---- GAT (include/hnh/gat.hpp; reference gat.hpp:26-113) --------------------------------------------------------------
+ * layers3: n_layers triples (input_features, features_per_head, num_heads).  Weights are input_width x head_width,
+ * row-major, as hnhd_gat_weight_shape reports.  The backward pass is refused on every rank where the layout has none
+ * (R-split layouts at p > 1; 1.5D dense shift with local kernel fusion at c > 1). */
+int hnhd_gat_create(hnhd_alg_t *alg, int n_layers, const int *layers3, double leaky_relu_alpha, hnhd_model_t **out);
+int hnhd_gat_weight_shape(hnhd_model_t *g, int layer, int head, int64_t *rows, int64_t *cols);
+int hnhd_gat_set_weight(hnhd_model_t *g, int layer, int head, const double *host);
+int hnhd_gat_get_weight(hnhd_model_t *g, int layer, int head, double *host); /* synchronises (e.g. after train steps) */
+/* dL/d weight (layer, head) after hnhd_model_backward; hnhd_gat_weight_shape's shape */
+int hnhd_gat_get_weight_grad(hnhd_model_t *g, int layer, int head, double *host);
+/* attention of every head (GAT::set_attention): "leaky" (the default: LeakyReLU of the scores, the
+ * reference's formula), "softmax" (their edge softmax over each row of S) or "additive" (below).  Makes the
+ * activations stale.
+ * With "softmax" the forward pass raises HNH_E_INVALID on every rank, before any launch, where the layout has
+ * no edge softmax (as hnhd_alg_edge_softmax). */
+int hnhd_gat_set_attention(hnhd_model_t *g, const char *kind);
+/* "gatv2": x_uv = a1 . LeakyReLU(h_u + h_v) (GATv2 with shared weights, Brody, Alon and Yahav 2022), then the edge
+ * softmax; a1 is set with hnhd_gat_set_attention_vectors (a2 is not read, its gradient stays zero).  Defined on
+ * the layouts where "softmax" is. */
+/* additive attention ("additive": x_uv = LeakyReLU(a1 . h_u + a2 . h_v) with h = X W the head's projection,
+ * then the edge softmax; Velickovic et al. 2018): the attention vectors of (layer, head), features_per_head
+ * doubles each (host pointers; zero after hnhd_gat_create: uniform attention).  Makes the activations stale.
+ * "additive" is defined on the layouts where "softmax" is. */
+int hnhd_gat_set_attention_vectors(hnhd_model_t *g, int layer, int head, const double *a1, const double *a2);
+int hnhd_gat_get_attention_vectors(hnhd_model_t *g, int layer, int head, double *a1, double *a2); /* synchronises */
+/* dL/d a1 and dL/d a2 of (layer, head) after hnhd_model_backward (features_per_head doubles each, summed over all
+ * ranks; zero unless the attention reads them).  HNH_E_INVALID before the first backward pass. */
+int hnhd_gat_get_attention_grads(hnhd_model_t *g, int layer, int head, double *da1, double *da2);
+
+/* ---- graph transformer (include/hnh/graph_transformer.hpp): TransformerConv layers on fused sparse attention ---
+ * layers3: n_layers triples (input_features, features_per_head, num_heads); every layer concatenates its heads, so
+ * layer i + 1 takes features_per_head * num_heads of layer i.  edge_dim > 0 adds edge features (attributes of S's
+ * entries projected by each layer's "edge" weight onto the keys and values), beta != 0 the gated skip connection.
+ * HNH_E_INVALID on every rank, before any launch, where the layout has no fused sparse attention (as
+ * hnhd_alg_edge_softmax), and for bad layer sizes. */
+int hnhd_gt_create(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, hnhd_model_t **out);
+/* The same with transformer blocks: ffn_ratio = k >= 1 makes every layer a post-norm block, LN2(H1 + FFN(H1)) with
+ * H1 = LN1(the layer's output without ReLU) and a ReLU FFN of hidden width k r; LayerNorm epsilon norm_eps.  ffn_ratio
+ * = 0 is hnhd_gt_create.  HNH_E_INVALID for ffn_ratio < 0 or a norm_eps that is not finite and > 0. */
+int hnhd_gt_create_block(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, int beta, int ffn_ratio,
+                         double norm_eps, hnhd_model_t **out);
+/* Parameters by layer and name: "query", "key", "value", "skip" (input_features x r, row-major: the transpose of
+ * PyG's lin_*.weight), "query_bias", "key_bias", "value_bias", "skip_bias" (r x 1), "edge" (edge_dim x r; models
+ * with edge features only), "beta" (3r x 1, the weight of PyG's lin_beta; gated models only).  Models with blocks
+ * (ffn_ratio > 0, hidden width h) add "norm1", "norm1_bias" (r x 1; LN1's weight and bias), "ffn1" ((r + 1) x h:
+ * lin1.weight^T with lin1.bias as the last row), "ffn2" ((h + 1) x r), "norm2", "norm2_bias".  The LayerNorm weights
+ * start at 1.  Layer l of the forward pass uses the dropout seed seed + the heads of the layers before it; the backward
+ * pass regenerates the forward's masks.  The forward refuses a bad dropout and a model with edge features whose
+ * attributes were not set. */
+/* Edge attributes of this rank's entries in both value orders: attr_A is n_A x edge_dim in the order of
+ * hnhd_vec_like(.., 0, ..) (hnhd_alg_entry_coordinates mode 0), attr_B n_B x edge_dim in the B order; n_A and n_B
+ * must be this rank's entry counts.  Both hold the same attribute for every stored (u, v).  Makes the activations
+ * stale.  HNH_E_INVALID for a model without edge features or wrong counts. */
+int hnhd_gt_set_edge_attributes(hnhd_model_t *g, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B);
+
+/* ---- GraphSAGE (include/hnh/graph_sage.hpp) ----------------------------------------------------------------------
+ * Layers of PyG's SAGEConv(aggr, root_weight = True): layers2 = {input_features, output_features} per layer; aggr is
+ * "mean", "sum" or "max".  Every layer but the last ends in a ReLU.  Parameters by layer and name: "neigh"
+ * (input_features x r: lin_l.weight.T), "neigh_bias" (r x 1: lin_l.bias), "root" (input_features x r: lin_r.weight.T).
+ * HNH_E_INVALID on every rank before any launch where hnhd_alg_edge_softmax is, for unknown aggregations, non-positive
+ * sizes and widths that do not chain. */
+int hnhd_sage_create(hnhd_alg_t *alg, int n_layers, const int *layers2, const char *aggr, hnhd_model_t **out);
+
+/* ---- R-GCN (include/hnh/rgcn.hpp) ----------------------------------------------------------------------------------
+ * Layers of PyG's RGCNConv(in, out, num_relations, aggr, root_weight = True, bias = True) without basis or block
+ * decomposition: layers2 = {input_features, output_features} per layer; aggr is "mean" or "sum".  The relation of each
+ * stored entry of S is its stored value, an integer in [0, num_relations); create refuses any other value on any rank.
+ * Every layer but the last ends in a ReLU.  Parameters by layer and name: "weight" (num_relations * input_features x r:
+ * RGCNConv.weight reshaped, no transpose), "bias" (r x 1), "root" (input_features x r).  HNH_E_INVALID on every rank
+ * before any launch where hnhd_alg_edge_softmax is, for unknown aggregations, num_relations < 1, non-positive sizes,
+ * widths that do not chain and R f >= 2^31.
+ * hnhd_rgcn_create_bases: the same with PyG's num_bases = B >= 1: W_rho = sum_b comp[rho, b] V_b.  Parameters by layer
+ * and name: "weight" (B f x r: RGCNConv.weight.reshape(-1, r)), "comp" (R x B), "bias" and "root" as without bases.
+ * Refuses num_bases < 1 and B f or R B >= 2^31 besides what hnhd_rgcn_create refuses. */
+int hnhd_rgcn_create(hnhd_alg_t *alg, int n_layers, const int *layers2, int num_relations, const char *aggr,
+                     hnhd_model_t **out);
+int hnhd_rgcn_create_bases(hnhd_alg_t *alg, int n_layers, const int *layers2, int num_relations, int num_bases,
+                           const char *aggr, hnhd_model_t **out);
 
 #ifdef __cplusplus
 }

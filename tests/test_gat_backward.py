@@ -53,7 +53,7 @@ def test_backward_model_returns_every_gradient():
     assert np.allclose(dX0b, 2 * dX0, rtol=1e-13, atol=0) and np.allclose(dWb[1][1], 2 * dW[1][1], rtol=1e-13, atol=0)
 
 
-def test_backward_entry_points_validate_without_a_gpu(hnh):
+def test_backward_entry_points_on_the_model_handle_validate_without_a_gpu(hnh):
     """Bad shapes and null pointers are rejected before the device is touched; empty sizes are successful no-ops."""
     buf = (C.c_double * 8)()
     p = C.addressof(buf)
@@ -91,6 +91,6 @@ def test_backward_entry_points_validate_without_a_gpu(hnh):
     assert hnh.hnh_relu_cols_backward_f64(None, None, None, 6, 2, 0, 3, None) == 0
     assert hnh.hnh_relu_cols_backward_f64(p, None, p, 6, 2, 2, 3, None) == -1
     # driver entries: null handles / pointers
-    assert hnh.hnhd_gat_backward(None, p) == -1
+    assert hnh.hnhd_model_backward(None, p) == -1
     assert hnh.hnhd_gat_get_weight_grad(None, 0, 0, p) == -1
-    assert hnh.hnhd_gat_get_input_grad(None, p) == -1
+    assert hnh.hnhd_model_get_input_grad(None, p) == -1

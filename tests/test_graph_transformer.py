@@ -134,8 +134,9 @@ def test_kernel_entry_points_validate_without_a_gpu(hnh):
         assert bw(w=None, dw=None, dR=None, Y=None, relu=0) == -2
 
 
-def test_driver_entry_points_validate_without_a_gpu(hnh):
-    """Null handles and arguments are refused by every hnhd_gt_* entry point."""
+def test_gt_create_and_edge_attributes_validate_without_a_gpu(hnh):
+    """Null handles and arguments are refused by the graph transformer's own entry points (the shared hnhd_model_* ones:
+    test_model.py)."""
     buf = (C.c_double * 8)()
     p = C.addressof(buf)
     i64 = C.c_int64()
@@ -146,20 +147,8 @@ def test_driver_entry_points_validate_without_a_gpu(hnh):
     assert hnh.hnhd_gt_create(p, 1, None, 0, 0, C.byref(out)) == -1
     assert hnh.hnhd_gt_create(p, 1, layers, 0, 0, None) == -1
     assert b"bad argument" in hnh.hnh_last_error_string()
-    for name in (b"query", b"beta", b"nope"):
-        assert hnh.hnhd_gt_param_shape(None, 0, name, C.byref(i64), C.byref(i64)) == -1
-        assert hnh.hnhd_gt_set_param(None, 0, name, p) == -1
-        assert hnh.hnhd_gt_get_param(None, 0, name, p) == -1
-        assert hnh.hnhd_gt_get_param_grad(None, 0, name, p) == -1
-    assert hnh.hnhd_gt_buffer_shape(None, 0, C.byref(i64), C.byref(i64)) == -1
-    assert hnh.hnhd_gt_set_input(None, p) == -1
-    assert hnh.hnhd_gt_get_buffer(None, 0, p) == -1
     assert hnh.hnhd_gt_set_edge_attributes(None, p, 1, p, 1) == -1
-    assert hnh.hnhd_gt_forward(None, 0.0, 0) == -1
-    assert hnh.hnhd_gt_backward(None, p) == -1
-    assert hnh.hnhd_gt_get_input_grad(None, p) == -1
     assert b"null" in hnh.hnh_last_error_string()
-    hnh.hnhd_gt_destroy(None)  # a no-op
 
 
 def test_python_front_end_validates_arguments():

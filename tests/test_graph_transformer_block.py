@@ -146,7 +146,7 @@ def test_block_kernel_entry_points_validate_without_a_gpu(hnh):
         assert bw(n=0) == -2  # the zero fill of dgamma and dbeta needs the device
 
 
-def test_block_driver_entry_point_validates_without_a_gpu(hnh):
+def test_block_create_and_block_parameters_validate_without_a_gpu(hnh):
     buf = (C.c_double * 8)()
     p = C.addressof(buf)
     layers = (C.c_int * 3)(4, 2, 2)
@@ -158,9 +158,9 @@ def test_block_driver_entry_point_validates_without_a_gpu(hnh):
     assert b"bad argument" in hnh.hnh_last_error_string()
     i64 = C.c_int64()
     for name in (b"norm1", b"norm1_bias", b"ffn1", b"ffn2", b"norm2", b"norm2_bias"):
-        assert hnh.hnhd_gt_param_shape(None, 0, name, C.byref(i64), C.byref(i64)) == -1
-        assert hnh.hnhd_gt_set_param(None, 0, name, p) == -1
-        assert hnh.hnhd_gt_get_param_grad(None, 0, name, p) == -1
+        assert hnh.hnhd_model_param_shape(None, 0, name, C.byref(i64), C.byref(i64)) == -1
+        assert hnh.hnhd_model_set_param(None, 0, name, p) == -1
+        assert hnh.hnhd_model_get_param_grad(None, 0, name, p) == -1
 
 
 def test_python_front_end_validates_block_arguments():

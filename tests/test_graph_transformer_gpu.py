@@ -157,7 +157,7 @@ def test_backward_needs_a_current_forward_pass(world):
         net.backward(P["G"][:, :-1])
 
 
-def test_model_arguments_are_refused(world):
+def test_model_arguments_are_refused_on_the_model_handle(world):
     """Bad layer chains, unknown parameters, wrong attribute counts and a missing edge attribute are refused with
     HNH_E_INVALID before any launch."""
     N = 64
@@ -181,7 +181,7 @@ def test_model_arguments_are_refused(world):
     assert net.param_shape(0, "query") == (6, 8) and net.param_shape(0, "key_bias") == (8,)
     with pytest.raises(ValueError):
         net.set_param(0, "query", np.zeros((8, 6)))
-    assert lib().hnhd_gt_forward(net.h, 1.0, 0) == -1 and b"dropout" in lib().hnh_last_error_string()
+    assert lib().hnhd_model_forward(net.h, 1.0, 0) == -1 and b"dropout" in lib().hnh_last_error_string()
     edged = D.GraphTransformer(alg, [(6, 4, 2)], edge_dim=2, beta=True)
     assert edged.param_shape(0, "edge") == (2, 8) and edged.param_shape(0, "beta") == (24,)
     with pytest.raises(RuntimeError, match="code -1.*no edge attributes"):

@@ -125,7 +125,7 @@ def test_link_kernels_validate_without_a_gpu(hnh):
         assert hnh.hnh_link_target_check_f64(st, t, 4, None) == -2
 
 
-def test_link_driver_entry_points_validate_without_a_gpu(hnh):
+def test_link_entry_points_on_the_model_handle_validate_without_a_gpu(hnh):
     out = C.c_void_p()
     res = (C.c_double * 4)()
     p = C.addressof(res)
@@ -136,11 +136,10 @@ def test_link_driver_entry_points_validate_without_a_gpu(hnh):
     assert hnh.hnhd_link_targets_create(p, None, C.byref(out)) == -1
     assert hnh.hnhd_link_targets_create(p, p, None) == -1
     for args in ((None, p, p), (p, None, p), (p, p, None)):
-        assert hnh.hnhd_gt_link_train_step(*args, 0.0, 0, res) == -1 and b"null" in hnh.hnh_last_error_string()
-        assert hnh.hnhd_gat_link_train_step(*args, res) == -1 and b"null" in hnh.hnh_last_error_string()
-    assert hnh.hnhd_gt_link_train_step(p, p, p, 0.0, 0, None) == -1
-    assert hnh.hnhd_gt_link_evaluate(None, p, None, res) == -1 and hnh.hnhd_gat_link_evaluate(p, None, None, res) == -1
-    assert hnh.hnhd_gt_link_evaluate(p, p, None, None) == -1
+        assert hnh.hnhd_model_link_train_step(*args, 0.0, 0, res) == -1 and b"null" in hnh.hnh_last_error_string()
+    assert hnh.hnhd_model_link_train_step(p, p, p, 0.0, 0, None) == -1
+    assert hnh.hnhd_model_link_evaluate(None, p, None, res) == -1 and hnh.hnhd_model_link_evaluate(p, None, None, res) == -1
+    assert hnh.hnhd_model_link_evaluate(p, p, None, None) == -1
     hnh.hnhd_link_targets_destroy(None)
 
 

@@ -385,7 +385,7 @@ def test_backward_repeats_bit_identical_and_needs_a_forward(world):
         net.backward(P["G"])
 
 
-def test_model_refusals(world):
+def test_basis_model_refusals(world):
     P = build(LAYER_SETS[1], "sum", 3, 2)
     alg, net = P["alg"], P["net"]
     out = C.c_void_p()
@@ -395,7 +395,7 @@ def test_model_refusals(world):
     assert lib().hnhd_rgcn_create_bases(alg.h, 1, flat, 3, 2, b"max", C.byref(out)) == -1
     for name in (b"query", b"neigh", b"basis"):
         r, c = C.c_int64(), C.c_int64()
-        assert lib().hnhd_rgcn_param_shape(net.h, 0, name, C.byref(r), C.byref(c)) == -1
+        assert lib().hnhd_model_param_shape(net.h, 0, name, C.byref(r), C.byref(c)) == -1
         assert b"no parameter" in lib().hnh_last_error_string()
     assert net.param_names() == ["weight", "comp", "bias", "root"]
     assert net.param_shape(0, "weight") == (12, 4) and net.param_shape(0, "comp") == (3, 2)
@@ -412,7 +412,7 @@ def test_model_refusals(world):
     with pytest.raises(ValueError, match="no parameter"):
         plain.param_shape(0, "comp")
     r, c = C.c_int64(), C.c_int64()
-    assert lib().hnhd_rgcn_param_shape(plain.h, 0, b"comp", C.byref(r), C.byref(c)) == -1
+    assert lib().hnhd_model_param_shape(plain.h, 0, b"comp", C.byref(r), C.byref(c)) == -1
 
 
 # ---- training -----------------------------------------------------------------------------------------------------------

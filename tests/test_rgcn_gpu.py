@@ -373,7 +373,7 @@ def test_backward_repeats_bit_identical_and_needs_a_forward(world):
         net.backward(P["G"])
 
 
-def test_model_refusals(world):
+def test_rgcn_model_refusals(world):
     P = build(LAYER_SETS[1], "sum", 3)
     alg, net = P["alg"], P["net"]
     out = C.c_void_p()
@@ -385,7 +385,7 @@ def test_model_refusals(world):
     assert b"does not take the width" in lib().hnh_last_error_string()
     for name in (b"query", b"neigh"):
         r, c = C.c_int64(), C.c_int64()
-        assert lib().hnhd_rgcn_param_shape(net.h, 0, name, C.byref(r), C.byref(c)) == -1
+        assert lib().hnhd_model_param_shape(net.h, 0, name, C.byref(r), C.byref(c)) == -1
         assert b"no parameter" in lib().hnh_last_error_string()
     with pytest.raises(RuntimeError, match="no such layer"):
         net.param(1, "root")

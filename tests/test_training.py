@@ -141,7 +141,7 @@ def test_training_kernels_validate_without_a_gpu(hnh):
         assert hnh.hnh_clip_coef_f64(a, b, 2, 1.0, None) == -2
 
 
-def test_training_driver_entry_points_validate_without_a_gpu(hnh):
+def test_training_entry_points_on_the_model_handle_validate_without_a_gpu(hnh):
     out = C.c_void_p()
     lab = (C.c_int32 * 4)(0, 1, -1, 2)
     res = (C.c_double * 4)()
@@ -167,10 +167,8 @@ def test_training_driver_entry_points_validate_without_a_gpu(hnh):
     assert hnh.hnhd_adamw_set_lr(None, 0.5) == -1
     p = C.addressof(res)
     for args in ((None, p, opt), (p, None, opt), (p, p, None)):
-        assert hnh.hnhd_gt_train_step(*args, 0.0, 0, res) == -1 and b"null" in hnh.hnh_last_error_string()
-        assert hnh.hnhd_gat_train_step(*args, res) == -1 and b"null" in hnh.hnh_last_error_string()
-    assert hnh.hnhd_gt_train_step(p, p, opt, 0.0, 0, None) == -1
-    assert hnh.hnhd_gat_train_step(p, p, opt, None) == -1
+        assert hnh.hnhd_model_train_step(*args, 0.0, 0, res) == -1 and b"null" in hnh.hnh_last_error_string()
+    assert hnh.hnhd_model_train_step(p, p, opt, 0.0, 0, None) == -1
     assert hnh.hnhd_gat_get_weight(None, 0, 0, p) == -1
     assert hnh.hnhd_gat_get_attention_vectors(None, 0, 0, p, p) == -1
     hnh.hnhd_adamw_destroy(opt)
