@@ -118,6 +118,10 @@ ABI = {
     "hnh_max_aggregate_finish_f64": (C.c_int, [_P, _P, _I64, _P]),
     "hnh_max_aggregate_grad_scale_f64": (C.c_int, [_P, _P, _P, _I64, _P]),
     "hnh_max_aggregate_grad_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
+    "hnh_segment_pool_workspace_bytes": (C.c_int64, [_I64, C.c_int, C.c_int]),
+    "hnh_segment_pool_f64": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _P, _I64, C.c_int, _P, _I64, _P, _I64, _P, C.c_size_t, _P]),
+    "hnh_segment_max_count_merge_f64": (C.c_int, [_P, _P, _P, _I64, _P]),
+    "hnh_segment_pool_grad_f64": (C.c_int, [_P, _I64, _I64, _P, _I64, _P, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
     "hnh_relational_aggregate_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_relational_aggregate_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_window_scale_f64": (C.c_int, [_P, _I64, _P, _I64, _I64, C.c_int, C.c_int, _P]),
@@ -322,6 +326,18 @@ ABI.update({
     "hnhd_model_link_train_step": (C.c_int, [_P, _P, _P, C.c_double, C.c_uint64, _P]),
     "hnhd_model_link_evaluate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_model_destroy": (None, [_P]),
+    "hnhd_readout_create": (C.c_int, [_P, _P, _I64, _I64, C.c_char_p, C.c_int, _PP]),
+    "hnhd_readout_destroy": (None, [_P]),
+    "hnhd_readout_pool": (C.c_int, [_P, _P, _P]),
+    "hnhd_readout_pool_backward": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_readout_param_shape": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_readout_set_param": (C.c_int, [_P, C.c_char_p, _P]),
+    "hnhd_readout_get_param": (C.c_int, [_P, C.c_char_p, _P]),
+    "hnhd_readout_get_param_grad": (C.c_int, [_P, C.c_char_p, _P]),
+    "hnhd_graph_labels_create": (C.c_int, [_P, _P, _I64, C.c_int, _PP]),
+    "hnhd_graph_labels_destroy": (None, [_P]),
+    "hnhd_model_graph_train_step": (C.c_int, [_P, _P, _P, _P, C.c_double, C.c_uint64, _P]),
+    "hnhd_model_graph_evaluate": (C.c_int, [_P, _P, _P, _P, _P]),
     "hnhd_timer_start": (C.c_int, []),
     "hnhd_timer_stop": (C.c_int, [C.POINTER(C.c_double)]),
     "hnhd_als_residuals": (C.c_int, [_P, C.c_int, _P]),

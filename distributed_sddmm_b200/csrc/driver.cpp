@@ -13,6 +13,7 @@
 #include "hnh/benchmark_dist.hpp"
 #include "hnh/distributed_sparse.h"
 #include "hnh/gat.hpp"
+#include "hnh/graph_readout.hpp"
 #include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
 #include "hnh/rgcn.hpp"
@@ -46,6 +47,12 @@ struct hnhd_adamw {
 };
 struct hnhd_link_targets {
     std::unique_ptr<hnh::LinkTargets> t;
+};
+struct hnhd_readout {
+    std::unique_ptr<hnh::GraphReadout> r;
+};
+struct hnhd_graph_labels {
+    std::unique_ptr<hnh::GraphLabels> l;
 };
 
 namespace {
@@ -852,6 +859,90 @@ int hnhd_model_link_evaluate(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd
     });
 }
 void hnhd_model_destroy(hnhd_model_t *m) { delete m; }
+
+// ---- graph-level prediction
+static hnh::GraphReadout &readout(hnhd_readout_t *r) {
+    if (!r) throw hnh::Error(HNH_E_INVALID, "null readout");
+    return *r->r;
+}
+static ParamRef readout_param(hnhd_readout_t *r, const char *name) {
+    if (!name) throw hnh::Error(HNH_E_INVALID, "GraphReadout: null argument");
+    return readout(r).param(name);
+}
+int hnhd_readout_create(hnhd_model_t *m, const int64_t *batch, int64_t n, int64_t num_graphs, const char *pool, int num_classes,
+                        hnhd_readout_t **out) {
+    return guarded([&] {
+        if (!m || !pool || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_readout_create: null argument");
+        *out = new hnhd_readout{std::make_unique<hnh::GraphReadout>(model(m), batch, n, num_graphs, pool, num_classes)};
+    });
+}
+void hnhd_readout_destroy(hnhd_readout_t *r) { delete r; }
+int hnhd_readout_pool(hnhd_readout_t *r, hnhd_dense_t *H, hnhd_dense_t *P) {
+    return guarded([&] {
+        if (!r || !H || !P) throw hnh::Error(HNH_E_INVALID, "hnhd_readout_pool: null argument");
+        P->m = readout(r).pool(H->m);
+    });
+}
+int hnhd_readout_pool_backward(hnhd_readout_t *r, hnhd_dense_t *H, hnhd_dense_t *dP, hnhd_dense_t *dH) {
+    return guarded([&] {
+        if (!r || !H || !dP || !dH) throw hnh::Error(HNH_E_INVALID, "hnhd_readout_pool_backward: null argument");
+        if (dH == H || dH == dP) throw hnh::Error(HNH_E_INVALID, "hnhd_readout_pool_backward: dH may not be H or dP");
+        readout(r).poolBackward(H->m, dP->m, dH->m);
+    });
+}
+int hnhd_readout_param_shape(hnhd_readout_t *r, const char *name, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        const ParamRef p = readout_param(r, name);
+        if (rows) *rows = p.rows;
+        if (cols) *cols = p.cols;
+    });
+}
+int hnhd_readout_set_param(hnhd_readout_t *r, const char *name, const double *host) {
+    return guarded([&] {
+        const ParamRef p = readout_param(r, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        sync_copy(p.value, host, p.rows * p.cols, cudaMemcpyHostToDevice);
+    });
+}
+int hnhd_readout_get_param(hnhd_readout_t *r, const char *name, double *host) {
+    return guarded([&] {
+        const ParamRef p = readout_param(r, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        sync_copy(host, p.value, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_readout_get_param_grad(hnhd_readout_t *r, const char *name, double *host) {
+    return guarded([&] {
+        const ParamRef p = readout_param(r, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (!p.grad) throw hnh::Error(HNH_E_INVALID, "GraphReadout: no graph train step has run");
+        sync_copy(host, p.grad, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_graph_labels_create(hnhd_readout_t *r, const int32_t *host_labels, int64_t n, int num_classes, hnhd_graph_labels_t **out) {
+    return guarded([&] {
+        if (!r || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_graph_labels_create: null argument");
+        *out = new hnhd_graph_labels{std::make_unique<hnh::GraphLabels>(readout(r), host_labels, n, num_classes)};
+    });
+}
+void hnhd_graph_labels_destroy(hnhd_graph_labels_t *l) { delete l; }
+int hnhd_model_graph_train_step(hnhd_model_t *m, hnhd_readout_t *r, const hnhd_graph_labels_t *labels, hnhd_adamw_t *opt,
+                                double dropout, uint64_t seed, double out[4]) {
+    return guarded([&] {
+        if (!m || !r || !labels || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_graph_train_step: null argument");
+        train_out(hnh::graphTrainStep(*m->m, *r->r, *labels->l, *opt->o, dropout, seed), out);
+    });
+}
+int hnhd_model_graph_evaluate(hnhd_model_t *m, hnhd_readout_t *r, const hnhd_graph_labels_t *labels, double *host_logits,
+                              double out[3]) {
+    return guarded([&] {
+        if (!m || !r || !labels || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_graph_evaluate: null argument");
+        const hnh::LinkResult res = hnh::graphEvaluate(*m->m, *r->r, *labels->l, host_logits);
+        out[0] = res.loss;
+        out[1] = (double)res.correct;
+        out[2] = (double)res.count;
+    });
+}
 
 // ---- GAT only: weights and attention vectors by (layer, head)
 // the layer of a (layer, head) pair, refused for another model, layer or head

@@ -24,25 +24,6 @@ using hnh::set_error;
 
 constexpr int kWindow = 256;  // the widest column window of one launch
 
-// (m, c) absorbs one candidate x
-__device__ __forceinline__ void max_take(double &m, double &c, double x) {
-    if (x > m) {
-        m = x;
-        c = 1.0;
-    } else if (x == m) {
-        c += 1.0;
-    }
-}
-// the stored (z, n) absorbs a row's (m, c)
-__device__ __forceinline__ void max_merge(double &z, double &n, double m, double c) {
-    if (m > z) {
-        z = m;
-        n = c;
-    } else if (m == z) {
-        n += c;
-    }
-}
-
 // ---- fast row kernels ------------------------------------------------------------------------------------------------
 template <int R, int G, int VW, int UN>
 __global__ void __launch_bounds__(kBlock, 1)

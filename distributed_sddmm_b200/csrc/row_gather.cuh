@@ -71,6 +71,25 @@ __device__ __forceinline__ double warp_sum(double v) {
     return v;
 }
 
+// the (max, count) pairs of max aggregation (graph_sage.cu) and max readout (graph_readout.cu): (m, c) absorbs one
+// candidate x; the stored (z, n) absorbs another (m, c).  The larger maximum wins, equal maxima add their counts.
+__device__ __forceinline__ void max_take(double &m, double &c, double x) {
+    if (x > m) {
+        m = x;
+        c = 1.0;
+    } else if (x == m) {
+        c += 1.0;
+    }
+}
+__device__ __forceinline__ void max_merge(double &z, double &n, double m, double c) {
+    if (m > z) {
+        z = m;
+        n = c;
+    } else if (m == z) {
+        n += c;
+    }
+}
+
 bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 // The width table of the fast kernels: R -> (G lanes per row, VW doubles per vector load, UN rows in flight).

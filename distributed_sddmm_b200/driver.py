@@ -701,6 +701,28 @@ class _Model:
         self._check(lib().hnhd_model_link_evaluate(self.h, t, scores.h, out), "link_evaluate")
         return float(out[0]), int(out[1]), int(out[2]), scores.to_host()
 
+    def graph_train_step(self, readout: "GraphReadout", labels: "GraphLabels", opt: "AdamW") -> "TrainStep":
+        """One collective graph-classification step on the device: forward, the readout's pool and head, the mean
+        cross-entropy over the labelled graphs, backward, clipping and AdamW over the model's parameters and then the
+        head's.  Returns TrainStep(loss, correct, labelled = the labelled graphs, grad_norm)."""
+        return self._graph_train_step(readout, labels, opt, 0.0, 0)
+
+    def _graph_train_step(self, readout, labels, opt, dropout, seed):
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        out = (C.c_double * 4)()
+        self._check(lib().hnhd_model_graph_train_step(self.h, _readout_arg(readout), _graph_labels_arg(labels), _adamw_arg(opt),
+                                                      p, sd, out), "graph_train_step")
+        return TrainStep._of(out)
+
+    def graph_evaluate(self, readout: "GraphReadout", labels: "GraphLabels"):
+        """A forward pass without dropout, the readout and the loss without gradients (collective): (loss, correct,
+        labelled, logits), the logits a num_graphs x C numpy array, the same on every rank -- for accuracy or ROC-AUC."""
+        r, lab = _readout_arg(readout), _graph_labels_arg(labels)
+        out = (C.c_double * 3)()
+        logits = np.empty((readout.num_graphs, readout.num_classes), np.float64)
+        self._check(lib().hnhd_model_graph_evaluate(self.h, r, lab, logits.ctypes.data, out), "graph_evaluate")
+        return float(out[0]), int(out[1]), int(out[2]), logits
+
     def __del__(self):
         try:
             lib().hnhd_model_destroy(self.h)
@@ -901,6 +923,13 @@ class GraphTransformer(_ModelByName):
         and AdamW.  Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
         return self._link_train_step(targets, opt, dropout, seed)
 
+    def graph_train_step(self, readout: "GraphReadout", labels: "GraphLabels", opt: "AdamW", dropout: float = 0.0,
+                         seed: int = 0) -> "TrainStep":
+        """One collective graph-classification step on the device: forward(dropout, seed), the readout's pool and
+        head, the mean cross-entropy over the labelled graphs, backward, clipping and AdamW over the model's parameters
+        and then the head's.  Returns TrainStep(loss, correct, labelled = the labelled graphs, grad_norm)."""
+        return self._graph_train_step(readout, labels, opt, dropout, seed)
+
 
 class GraphSAGE(_ModelByName):
     """GraphSAGE: layers of PyG's SAGEConv(aggr, root_weight=True, project=False, normalize=False), forward and backward
@@ -1083,6 +1112,134 @@ class LinkTargets:
             lib().hnhd_link_targets_destroy(self.h)
         except Exception:
             pass
+
+
+class GraphReadout:
+    """The readout of graph-level prediction on the device (include/hnh/graph_readout.hpp): pools the rows of net's
+    output into one row per graph and, with num_classes, applies a torch.nn.Linear(r, num_classes) head.  batch: this
+    rank's graph id of every output row (net.buffer_shape(last)[0] entries, e.g. a slice of PyG's Batch.batch), in [0,
+    num_graphs) or negative for a row in no graph (padding rows must be negative); the ids need not be sorted.  pool:
+    "sum" (global_add_pool), "mean" (global_mean_pool; an empty graph pools to 0) or "max" (global_max_pool; 0 for an
+    empty graph; ties share the gradient equally, -0.0 and +0.0 tying).  num_classes None: no head, and the output
+    width is the class count.  Collective: a bad batch on one rank is refused on every rank.  net must outlive this.
+
+    Parameters of the head (zero after construction), by name: "weight" (r x C, Linear.weight.T) and "bias" (C)."""
+
+    POOLS = ("sum", "mean", "max")
+    PARAMS = ("weight", "bias")
+    VECTORS = ("bias",)
+
+    def __init__(self, net, batch, num_graphs: int, pool: str = "mean", num_classes: int | None = None):
+        b = np.asarray(batch)
+        if b.dtype.kind not in "iu" or b.ndim != 1:
+            raise ValueError(f"batch must be a 1-D integer array, got {b.dtype} of shape {b.shape}")
+        if pool not in self.POOLS:
+            raise ValueError(f"pool = {pool!r} must be one of {self.POOLS}")
+        for name, v in (("num_graphs", num_graphs), ("num_classes", num_classes)):
+            if v is not None and (isinstance(v, bool) or not isinstance(v, numbers.Integral)):
+                raise ValueError(f"{name} = {v!r} must be an integer")
+        if num_classes is not None and num_classes < 1:
+            raise ValueError(f"num_classes = {num_classes} must be positive (None: no head)")
+        self.net, self.pool_kind, self.num_graphs = net, pool, int(num_graphs)
+        self.head = num_classes is not None
+        self.num_classes = int(num_classes) if self.head else net.buffer_shape(len(net.layers))[1]
+        self._batch = np.ascontiguousarray(b, np.int64)
+        self._H = None
+        self.h = C.c_void_p()
+        check(lib().hnhd_readout_create(net.h, self._batch.ctypes.data, len(self._batch), self.num_graphs, pool.encode(),
+                                        int(num_classes or 0), C.byref(self.h)), "readout_create")
+
+    def pool(self, H: Dense) -> Dense:
+        """P = the pool of H (a Dense of the model's output shape) over all ranks: a num_graphs x r Dense.  Collective."""
+        if not isinstance(H, Dense):
+            raise TypeError(f"H must be a Dense, not {type(H).__name__}")
+        P = Dense.create(1, 1)
+        check(lib().hnhd_readout_pool(self.h, H.h, P.h), "readout_pool")
+        self._H = H
+        return P
+
+    def pool_backward(self, dP: Dense) -> Dense:
+        """dL/dH for the H of the last pool, given dP = dL/dP (num_graphs x r, the same on every rank)."""
+        if not isinstance(dP, Dense):
+            raise TypeError(f"dP must be a Dense, not {type(dP).__name__}")
+        if self._H is None:
+            raise ValueError("pool_backward needs a pool first")
+        dH = Dense.create(1, 1)
+        check(lib().hnhd_readout_pool_backward(self.h, self._H.h, dP.h, dH.h), "readout_pool_backward")
+        return dH
+
+    def param_names(self):
+        return list(self.PARAMS) if self.head else []
+
+    def param_shape(self, name: str):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_readout_param_shape(self.h, name.encode(), C.byref(r), C.byref(c)), "readout_param_shape")
+        return (r.value,) if name in self.VECTORS else (r.value, c.value)
+
+    def set_param(self, name: str, value):
+        shape = self.param_shape(name)
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        if v.shape != shape:
+            raise ValueError(f"{name} is {shape}, got {v.shape}")
+        check(lib().hnhd_readout_set_param(self.h, name.encode(), v.ctypes.data), "readout_set_param")
+
+    def param(self, name: str):
+        out = np.empty(self.param_shape(name), dtype=np.float64)
+        check(lib().hnhd_readout_get_param(self.h, name.encode(), out.ctypes.data), "readout_get_param")
+        return out
+
+    def param_grad(self, name: str):
+        """dL/d param after a graph train step (identical on every rank)."""
+        out = np.empty(self.param_shape(name), dtype=np.float64)
+        check(lib().hnhd_readout_get_param_grad(self.h, name.encode(), out.ctypes.data), "readout_get_param_grad")
+        return out
+
+    def __del__(self):
+        try:
+            lib().hnhd_readout_destroy(self.h)
+        except Exception:
+            pass
+
+
+class GraphLabels:
+    """The labels of a readout's num_graphs graphs on the device: each a class in [0, num_classes) or negative for
+    "ignored" (train / validation / test splits), the same array on every rank.  num_classes is the logits' width.
+    Collective: labels of another length, a label >= num_classes, or labels differing between ranks are refused on every
+    rank.  The readout must outlive this one."""
+
+    def __init__(self, readout: GraphReadout, labels, num_classes: int):
+        if not isinstance(readout, GraphReadout):
+            raise TypeError(f"readout must be a GraphReadout, not {type(readout).__name__}")
+        lab = np.asarray(labels)
+        if lab.dtype.kind not in "iu" or lab.ndim != 1:
+            raise ValueError(f"labels must be a 1-D integer array, got {lab.dtype} of shape {lab.shape}")
+        if len(lab) and (lab.max() > np.iinfo(np.int32).max or lab.min() < np.iinfo(np.int32).min):
+            raise ValueError("labels must fit in int32")
+        if isinstance(num_classes, bool) or not isinstance(num_classes, numbers.Integral):
+            raise ValueError(f"num_classes = {num_classes!r} must be an integer")
+        self.readout, self.num_classes = readout, int(num_classes)
+        self._host = np.ascontiguousarray(lab, np.int32)
+        self.h = C.c_void_p()
+        check(lib().hnhd_graph_labels_create(readout.h, self._host.ctypes.data, len(self._host), self.num_classes,
+                                             C.byref(self.h)), "graph_labels_create")
+
+    def __del__(self):
+        try:
+            lib().hnhd_graph_labels_destroy(self.h)
+        except Exception:
+            pass
+
+
+def _readout_arg(readout):
+    if not isinstance(readout, GraphReadout):
+        raise TypeError(f"readout must be a GraphReadout, not {type(readout).__name__}")
+    return readout.h
+
+
+def _graph_labels_arg(labels):
+    if not isinstance(labels, GraphLabels):
+        raise TypeError(f"labels must be a GraphLabels, not {type(labels).__name__}")
+    return labels.h
 
 
 def _link_targets_arg(targets):

@@ -167,16 +167,17 @@ inline void check_train(const DenseMatrix &out, const NodeLabels &labels, const 
     opt.check_spans(spans);
 }
 // the loss (by the caller's `loss`: the output buffer's gradient and the device sums (loss sum, correct) over all
-// ranks), backward (by the caller's `backward`), clip and AdamW; then the 4 scalars to the host.  count: the
-// denominator of the mean loss (labelled rows, or link targets).
-template <class Model, class Loss, class Backward>
-TrainResult finishStep(Model &net, int64_t count, AdamW &opt, Loss loss, Backward backward) {
+// ranks), backward (by the caller's `backward`), clip and AdamW on the span list `spans()` returns after the backward
+// (a first backward pass allocates the gradients); then the 4 scalars to the host.  count: the denominator of the
+// mean loss (labelled rows, link targets or labelled graphs).
+template <class Model, class Loss, class Backward, class Spans>
+TrainResult finishStep(Model &net, int64_t count, AdamW &opt, Loss loss, Backward backward, Spans spans) {
     VectorXd stats(4);  // loss sum, correct, total norm, clip coefficient
     DenseMatrix dlogits;
     loss(dlogits, stats.data());
     backward(dlogits);
     dlogits = DenseMatrix();
-    opt.step(net.parameters(), stats.data() + 2);
+    opt.step(spans(), stats.data() + 2);
     net.activations_current = false;
     double h[4];
     cudaStream_t s = Runtime::get().compute_stream();
@@ -195,7 +196,7 @@ inline TrainResult trainStep(GraphModel &net, const NodeLabels &labels, AdamW &o
     net.forward(dropout, seed);
     return detail::finishStep(
         net, labels.labelled, opt, [&](DenseMatrix &g, double *sums) { crossEntropy(net.buffers.back(), labels, g, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
+        [&](const DenseMatrix &g) { net.backwardPass(g); }, [&] { return net.parameters(); });
 }
 
 // ---- link prediction ----------------------------------------------------------------------------------------------
@@ -284,7 +285,7 @@ inline TrainResult linkTrainStep(GraphModel &net, const LinkTargets &targets, Ad
     net.forward(dropout, seed);
     return detail::finishStep(
         net, targets.count, opt, [&](DenseMatrix &g, double *sums) { targets.loss(net.buffers.back(), &g, nullptr, sums); },
-        [&](const DenseMatrix &g) { net.backwardPass(g); });
+        [&](const DenseMatrix &g) { net.backwardPass(g); }, [&] { return net.parameters(); });
 }
 
 // A forward pass without dropout and the link loss without gradients: (mean loss, correct, count) over all ranks, and

@@ -510,6 +510,39 @@ int hnh_max_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, 
                                int64_t ldx, const double *Z, int64_t ldz, const double *G, int64_t ldg, int f, double *dX,
                                int64_t lddx, void *stream);
 
+/* ---- graph readout (include/hnh/graph_readout.hpp; csrc/graph_readout.cu) -------------------------------------------
+ * Pools the rows of H (rows x r, leading dimension ldh) into one row per segment.  The segment CSR lists, for segment
+ * g < segments, the rows seg_rows[seg_start[g] .. seg_start[g + 1]) of H (any order; the sums run in the listed order).
+ * The chunk plan cuts every segment into chunks of HNH_SEGMENT_CHUNK rows, an empty segment into one empty chunk:
+ * chunk_first[g] (segments + 1 entries) is the first chunk of segment g, chunk_first[segments] = chunks, and
+ * chunk_seg[k] (chunks entries) the segment of chunk k.  Row indices are not bounds-checked; seg_rows may be null when
+ * no segment has a row.
+ * hnh_segment_pool_f64 overwrites row g of P (leading dimension ldp) for every segment; C null gives the sum
+ *     P_g = sum_{u in g} H_u                                           (0 for an empty segment)
+ * and C non-null (leading dimension ldc) the maximum with its tie count, as hnh_max_aggregate_step_f64:
+ *     (P_g,k, C_g,k) = (max_u H_u,k, #{u : H_u,k == max})              ((-inf, 0) for an empty segment)
+ * Every chunk's rows are read once, by its own lane group; the segments of more than one chunk then combine their
+ * chunk results from `workspace` (hnh_segment_pool_workspace_bytes(chunks, r, C != 0) bytes; none needed, and null
+ * allowed, when chunks == segments) in an order fixed by the segment lengths.  r >= 1, every leading dimension >= r;
+ * P and C may not be H or each other.
+ * hnh_segment_max_count_merge_f64: C[i] = 0 where local_max[i] != global_max[i] (n contiguous doubles): the counts of a
+ * rank whose maximum is not the maximum over all ranks drop out before the counts are summed over the ranks.
+ * hnh_segment_pool_grad_f64 overwrites every row u < rows of dH (leading dimension lddh): with g = row_graph[u],
+ *     dH_u = scale[g] dP_g                          (H, P, C null; scale nullable: 1) -- sum and mean
+ *     dH_u,k = [H_u,k == P_g,k] dP_g,k / C_g,k      (H, P, C all non-null, scale null; 0 where C = 0) -- max
+ * and dH_u = 0 where g lies outside [0, graphs).  dH may not be an input.
+ * Widths 4..256 (powers of two) with 16-byte aligned operands and even leading dimensions take 128-bit chunk and row
+ * kernels; others one-warp-per-chunk and one-warp-per-row kernels.  No atomics: repeated calls are bit-identical. */
+#define HNH_SEGMENT_CHUNK 256
+int64_t hnh_segment_pool_workspace_bytes(int64_t chunks, int r, int with_counts);
+int hnh_segment_pool_f64(const int64_t *seg_start, const int64_t *seg_rows, const int64_t *chunk_first, const int32_t *chunk_seg,
+                         int64_t segments, int64_t chunks, const double *H, int64_t ldh, int r, double *P, int64_t ldp, double *C,
+                         int64_t ldc, void *workspace, size_t workspace_bytes, void *stream);
+int hnh_segment_max_count_merge_f64(double *C, const double *local_max, const double *global_max, int64_t n, void *stream);
+int hnh_segment_pool_grad_f64(const int32_t *row_graph, int64_t rows, int64_t graphs, const double *dP, int64_t lddp,
+                              const double *scale, const double *H, int64_t ldh, const double *P, int64_t ldp, const double *C,
+                              int64_t ldc, int r, double *dH, int64_t lddh, void *stream);
+
 /* ---- relational aggregation (Distributed_Sparse::relationalAggregate; csrc/rgcn.cu) ---------------------------------
  * R-GCN's neighbour aggregation on one CSR block: the stored value of an entry is its relation rho, an integer in
  * [0, R).  An entry whose value is anything else (negative, >= R, fractional, infinite, NaN) contributes nothing and

@@ -371,6 +371,48 @@ int hnhd_model_link_train_step(hnhd_model_t *m, const hnhd_link_targets_t *t, hn
 int hnhd_model_link_evaluate(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
 void hnhd_model_destroy(hnhd_model_t *m);
 
+/* ---- graph-level prediction (include/hnh/graph_readout.hpp) ---------------------------------------------------------
+ * A readout of a model: batch (n = the model's localArows entries) gives the graph of each of this rank's output rows,
+ * in [0, num_graphs) or negative for none (padding rows must be negative); pool is "sum", "mean" or "max";
+ * num_classes = 0 pools without a head (the logits are the pooled rows, so the class count is the output width r),
+ * > 0 adds a Linear(r, num_classes) head with the parameters "weight" (r x C) and "bias" (C x 1), zero after
+ * construction.  Collective; HNH_E_INVALID on every rank before any launch for a layout where check_full_rows fails,
+ * a batch of another length, num_graphs < 1, num_graphs or num_graphs r >= 2^31, an id >= num_graphs or on a padding
+ * row on any rank, a graph count differing between ranks, an unknown pool and num_classes < 0.  The model must
+ * outlive the readout. */
+typedef struct hnhd_readout hnhd_readout_t;
+int hnhd_readout_create(hnhd_model_t *m, const int64_t *batch, int64_t n, int64_t num_graphs, const char *pool, int num_classes,
+                        hnhd_readout_t **out);
+void hnhd_readout_destroy(hnhd_readout_t *r);
+/* P (resized to num_graphs x r) = the pool of H (the model's output shape) over all ranks.  Collective. */
+int hnhd_readout_pool(hnhd_readout_t *r, hnhd_dense_t *H, hnhd_dense_t *P);
+/* dH (resized to H's shape) = dL/dH given dP = dL/dP (num_graphs x r, the same on every rank), for the H of the last
+ * pool (max reads that pool's maxima and counts).  No communication. */
+int hnhd_readout_pool_backward(hnhd_readout_t *r, hnhd_dense_t *H, hnhd_dense_t *dP, hnhd_dense_t *dH);
+/* the head's parameters by name; HNH_E_INVALID without a head or for another name, and for a gradient before a graph
+ * train step */
+int hnhd_readout_param_shape(hnhd_readout_t *r, const char *name, int64_t *rows, int64_t *cols);
+int hnhd_readout_set_param(hnhd_readout_t *r, const char *name, const double *host);
+int hnhd_readout_get_param(hnhd_readout_t *r, const char *name, double *host);
+int hnhd_readout_get_param_grad(hnhd_readout_t *r, const char *name, double *host);
+/* The labels of a readout's num_graphs graphs, in [0, num_classes) or negative for "ignored", the same on every rank.
+ * Collective; HNH_E_INVALID on every rank for n != num_graphs, num_classes other than the logits' width, a label >=
+ * num_classes, or labels differing between ranks. */
+typedef struct hnhd_graph_labels hnhd_graph_labels_t;
+int hnhd_graph_labels_create(hnhd_readout_t *r, const int32_t *host_labels, int64_t n, int num_classes, hnhd_graph_labels_t **out);
+void hnhd_graph_labels_destroy(hnhd_graph_labels_t *l);
+/* One graph-classification step: forward(dropout, seed), pool, head, the mean cross-entropy over the labelled graphs,
+ * the backward pass, clipping and AdamW over the model's parameters and then the head's.  out = {loss, correct,
+ * labelled graphs, grad_norm}.  Collective; HNH_E_INVALID on every rank before any launch for a readout of another
+ * model, labels of another readout, an optimizer of other parameter sizes, dropout on a model without it, and layouts
+ * without a backward pass. */
+int hnhd_model_graph_train_step(hnhd_model_t *m, hnhd_readout_t *r, const hnhd_graph_labels_t *labels, hnhd_adamw_t *opt,
+                                double dropout, uint64_t seed, double out[4]);
+/* A forward pass without dropout, the readout and the loss without gradients: out = {loss, correct, labelled graphs};
+ * host_logits (nullable) receives the num_graphs x C logits, row-major.  Collective. */
+int hnhd_model_graph_evaluate(hnhd_model_t *m, hnhd_readout_t *r, const hnhd_graph_labels_t *labels, double *host_logits,
+                              double out[3]);
+
 /* ---- GAT (include/hnh/gat.hpp; reference gat.hpp:26-113) --------------------------------------------------------------
  * layers3: n_layers triples (input_features, features_per_head, num_heads).  Weights are input_width x head_width,
  * row-major, as hnhd_gat_weight_shape reports.  The backward pass is refused on every rank where the layout has none
