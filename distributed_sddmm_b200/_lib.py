@@ -122,6 +122,14 @@ ABI = {
     "hnh_segment_pool_f64": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _P, _I64, C.c_int, _P, _I64, _P, _I64, _P, C.c_size_t, _P]),
     "hnh_segment_max_count_merge_f64": (C.c_int, [_P, _P, _P, _I64, _P]),
     "hnh_segment_pool_grad_f64": (C.c_int, [_P, _I64, _I64, _P, _I64, _P, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
+    "hnh_multi_aggregate_step_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
+    "hnh_multi_aggregate_finish_f64": (C.c_int, [_P, _I64, _I64, C.c_int, C.c_int, _P]),
+    "hnh_multi_aggregate_grad_prep_f64": (C.c_int, [_P, _I64, _P, _I64, _I64, C.c_int, C.c_int, _P, _I64, _P]),
+    "hnh_multi_aggregate_grad_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
+    "hnh_pna_combine_f64": (C.c_int, [_P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _I64, C.c_int, C.c_uint, C.c_int, C.c_uint,
+                                      C.c_int, C.c_double, C.c_double, _P, _I64, _P]),
+    "hnh_pna_combine_grad_f64": (C.c_int, [_P, _I64, _P, _I64, C.c_int, _P, _I64, _I64, C.c_int, C.c_uint, C.c_int, C.c_uint,
+                                           C.c_int, C.c_double, C.c_double, _P, _I64, _P, _I64, _P]),
     "hnh_relational_aggregate_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_relational_aggregate_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_window_scale_f64": (C.c_int, [_P, _I64, _P, _I64, _I64, C.c_int, C.c_int, _P]),
@@ -308,6 +316,9 @@ ABI.update({
     "hnhd_sage_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, _PP]),
     "hnhd_alg_relational_aggregate": (C.c_int, [_P, _P, _P, C.c_int]),
     "hnhd_alg_relational_aggregate_backward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int]),
+    "hnhd_alg_multi_aggregate": (C.c_int, [_P, _P, _P, C.c_int]),
+    "hnhd_alg_multi_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int]),
+    "hnhd_pna_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, C.c_char_p, C.c_double, C.c_double, _PP]),
     "hnhd_rgcn_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_char_p, _PP]),
     "hnhd_rgcn_create_bases": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_char_p, _PP]),
     "hnhd_alg_basis_aggregate": (C.c_int, [_P, _P, _P, _P, C.c_int, _P]),

@@ -1155,6 +1155,88 @@ void Distributed_Sparse::maxAggregateBackward(DenseMatrix &X, DenseMatrix &Z, De
                 });
 }
 
+// ---- multi-statistic aggregation -------------------------------------------------------------------------------------
+namespace {
+// the checks of multiAggregate / multiAggregateBackward (every rank decides alike: a layout gives every rank the same
+// widths and the caller passes the same matrices); returns f
+int64_t check_multi_aggregate(const Distributed_Sparse &d, const string &who, const DenseMatrix &X, int which,
+                              std::initializer_list<const DenseMatrix *> A_like, std::initializer_list<const DenseMatrix *> outs,
+                              const DenseMatrix *dX) {
+    if (which < 1 || which > HNH_MULTI_ALL)
+        throw hnh::Error(HNH_E_INVALID, who + ": which = " + to_string(which) + " selects no statistic or an unknown one");
+    const int64_t f = X.cols();
+    const int64_t W = 2 * (((which & HNH_MULTI_MOMENTS) != 0) + ((which & HNH_MULTI_MAX) != 0) + ((which & HNH_MULTI_MIN) != 0));
+    if (X.rows() != d.localBrows || f < 1 || f > INT32_MAX / W)
+        throw hnh::Error(HNH_E_INVALID, who + ": X is " + to_string(X.rows()) + " x " + to_string(f) + "; like_B_matrix has " +
+                                            to_string(d.localBrows) + " rows and the width f must be positive with " + to_string(W) +
+                                            " f below 2^31");
+    for (const DenseMatrix *m : A_like)
+        if (m->rows() != d.localArows || m->cols() != W * f)
+            throw hnh::Error(HNH_E_INVALID, who + ": an A-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                ", not localArows x " + to_string(W) + " f = " + to_string(d.localArows) + " x " +
+                                                to_string(W * f));
+    if (dX && (dX->rows() != X.rows() || dX->cols() != f))
+        throw hnh::Error(HNH_E_INVALID, who + ": dX is " + to_string(dX->rows()) + " x " + to_string(dX->cols()) + ", X " +
+                                            to_string(X.rows()) + " x " + to_string(f));
+    vector<const DenseMatrix *> all{&X};
+    all.insert(all.end(), A_like.begin(), A_like.end());
+    if (dX) all.push_back(dX);
+    for (const DenseMatrix *o : outs) {
+        int same = 0;
+        for (const DenseMatrix *m : all) same += m == o || (o->size() > 0 && m->data() == o->data());
+        if (same != 1) throw hnh::Error(HNH_E_INVALID, who + ": an output may not be another operand of the call");
+    }
+    return f;
+}
+}  // namespace
+
+void Distributed_Sparse::multiAggregate(DenseMatrix &X, DenseMatrix &A, int which) {
+    const string who = "multiAggregate";
+    check_full_rows(who);
+    const int64_t f = check_multi_aggregate(*this, who, X, which, {&A}, {&A}, nullptr);
+    const int64_t w = A.cols();
+    // the initial state: sums 0, maxima -inf, minima +inf, counts 0
+    A.setZero();
+    int64_t col = (which & HNH_MULTI_MOMENTS) ? 2 * f : 0;
+    for (int flag : {HNH_MULTI_MAX, HNH_MULTI_MIN})
+        if (which & flag) {
+            DenseMatrix init = DenseMatrix::Constant(A.rows(), f, flag == HNH_MULTI_MAX ? -INFINITY : INFINITY);
+            copy_cols(A, col, init, 0, f);
+            col += 2 * f;
+        }
+    gather_pass(k_sddmmA, {{&A, 0, w, true}}, {{&X, 0, f, false}},
+                [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, true, "multiAggregate");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_multi_aggregate_step_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords,
+                                                                Y[0].p, Y[0].ld, (int)f, which, R[0].p, R[0].ld, compute()),
+                                   "multi_aggregate_step");
+                });
+    hnh::abi_check(hnh_multi_aggregate_finish_f64(A.data(), w, A.rows(), (int)f, which, compute()), "multi_aggregate_finish");
+}
+
+void Distributed_Sparse::multiAggregateBackward(DenseMatrix &X, DenseMatrix &A, DenseMatrix &dA, DenseMatrix &dX, int which,
+                                                bool accumulate) {
+    const string who = "multiAggregateBackward";
+    check_full_rows(who);
+    const int64_t f = check_multi_aggregate(*this, who, X, which, {&A, &dA}, {&dX}, &dX);
+    const int64_t w = A.cols();
+    // D = [dS1 | dS2 | max | dA_max / C_max | min | dA_min / C_min]: what every entry of a row gathers
+    DenseMatrix D(localArows, w);
+    hnh::abi_check(hnh_multi_aggregate_grad_prep_f64(A.data(), w, dA.data(), w, A.rows(), (int)f, which, D.data(), w, compute()),
+                   "multi_aggregate_grad_prep");
+    if (!accumulate) dX.setZero();
+    gather_pass(k_sddmmB, {{&D, 0, w, false}}, {{&X, 0, f, false}, {&dX, 0, f, true}},
+                [&](int, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, false, "multiAggregateBackward");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_multi_aggregate_grad_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords,
+                                                                R[0].p, R[0].ld, Y[0].p, Y[0].ld, (int)f, which, R[1].p, R[1].ld,
+                                                                compute()),
+                                   "multi_aggregate_grad");
+                });
+}
+
 // ---- relational aggregation --------------------------------------------------------------------------------------------
 namespace {
 // the shape and aliasing checks of relationalAggregate / relationalAggregateBackward: X-shaped (localBrows x f) and

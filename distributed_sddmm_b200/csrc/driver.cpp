@@ -16,6 +16,7 @@
 #include "hnh/graph_readout.hpp"
 #include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
+#include "hnh/pna.hpp"
 #include "hnh/rgcn.hpp"
 #include "hnh/training.hpp"
 #include "hnh_b200.h"
@@ -662,6 +663,21 @@ int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t
     });
 }
 
+// ---- multi-statistic aggregation -------------------------------------------------------------------------------------
+int hnhd_alg_multi_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int which) {
+    return guarded([&] {
+        if (!a || !X || !A) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_multi_aggregate: null argument");
+        a->alg->multiAggregate(X->m, A->m, which);
+    });
+}
+int hnhd_alg_multi_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, hnhd_dense_t *dA, hnhd_dense_t *dX, int which,
+                                      int accumulate) {
+    return guarded([&] {
+        if (!a || !X || !A || !dA || !dX) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_multi_aggregate_backward: null argument");
+        a->alg->multiAggregateBackward(X->m, A->m, dA->m, dX->m, which, accumulate != 0);
+    });
+}
+
 // ---- relational aggregation ------------------------------------------------------------------------------------------
 int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations) {
     return guarded([&] {
@@ -731,6 +747,15 @@ int hnhd_sage_create(hnhd_alg_t *a, int n_layers, const int *layers2, const char
         vector<GraphSAGELayer> layers;
         for (int i = 0; i < n_layers; i++) layers.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
         *out = new hnhd_model{std::unique_ptr<GraphModel>(new GraphSAGE(layers, a->alg.get(), aggr))};
+    });
+}
+int hnhd_pna_create(hnhd_alg_t *a, int n_layers, const int *layers2, const char *aggregators, const char *scalers, double avg_deg_lin,
+                    double avg_deg_log, hnhd_model_t **out) {
+    return guarded([&] {
+        if (!a || !layers2 || !aggregators || !scalers || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_pna_create: bad argument");
+        vector<PNALayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
+        *out = new hnhd_model{std::unique_ptr<GraphModel>(new PNA(layers, a->alg.get(), aggregators, scalers, avg_deg_lin, avg_deg_log))};
     });
 }
 static int rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, int num_bases,

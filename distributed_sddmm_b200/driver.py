@@ -474,6 +474,41 @@ class Algorithm:
                                                     self._dense_arg(dX, "dX"), int(bool(accumulate))),
               "max_aggregate_backward")
 
+    MULTI_STATISTICS = {"moments": 1, "max": 2, "min": 4}
+
+    @classmethod
+    def _which(cls, which) -> int:
+        """The flags of a collection of statistic names (see multi_aggregate)."""
+        names = [which] if isinstance(which, str) else list(which)
+        if not names or any(n not in cls.MULTI_STATISTICS for n in names) or len(set(names)) != len(names):
+            raise ValueError(f"which = {which!r} must be a non-empty set of {tuple(cls.MULTI_STATISTICS)} without repeats")
+        return sum(cls.MULTI_STATISTICS[n] for n in names)
+
+    @classmethod
+    def multi_aggregate_width(cls, which, f: int) -> int:
+        """The width of multi_aggregate's output for the statistics `which` at input width f."""
+        return 2 * len(set([which] if isinstance(which, str) else which)) * int(f)
+
+    def multi_aggregate(self, X: Dense, A: Dense, which=("moments", "max", "min")):
+        """Collective: several statistics of each S-row's neighbours in one gather pass (Distributed_Sparse::multiAggregate,
+        PNA's aggregation).  which: a non-empty collection of "moments", "max" and "min".  X is B-shaped, f wide; A
+        (A-shaped, multi_aggregate_width(which, f) wide) is overwritten with the selected f-wide windows in the fixed order
+        [sum_v X_v | sum_v X_v^2 | max_v X_v | #ties of the max | min_v X_v | #ties of the min] over the stored entries
+        (u, v) of S on all ranks (duplicates count; S's values are not read), every window 0 on a row without entries."""
+        w = self._which(which)
+        check(lib().hnhd_alg_multi_aggregate(self.h, self._dense_arg(X, "X"), self._dense_arg(A, "A"), w), "multi_aggregate")
+
+    def multi_aggregate_backward(self, X: Dense, A: Dense, dA: Dense, dX: Dense, which=("moments", "max", "min"),
+                                 accumulate: bool = False):
+        """Collective: given the forward's A and dA = dLoss/dA (A's layout; its count windows are not read), dX (X's shape)
+        is overwritten -- or, with accumulate, added to -- with dX_v = sum_u dA_sum[u] + 2 X_v dA_sq[u] + [X_v == max_u]
+        dA_max[u] / C_max[u] + [X_v == min_u] dA_min[u] / C_min[u]: tied entries share the gradient of an extreme
+        equally (Distributed_Sparse::multiAggregateBackward)."""
+        w = self._which(which)
+        check(lib().hnhd_alg_multi_aggregate_backward(self.h, self._dense_arg(X, "X"), self._dense_arg(A, "A"),
+                                                      self._dense_arg(dA, "dA"), self._dense_arg(dX, "dX"), w,
+                                                      int(bool(accumulate))), "multi_aggregate_backward")
+
     def relational_aggregate(self, X: Dense, A: Dense, num_relations: int):
         """Collective: R-GCN's aggregation (Distributed_Sparse::relationalAggregate).  The relation of each stored entry
         (u, v) of S is its stored value (SpmatLocal.from_tuples' vals; an SDDMM, SpMM or FusedMM on this object
@@ -1015,6 +1050,78 @@ class RGCN(_ModelByName):
         if name not in self._params():
             raise ValueError(f"no parameter {name!r}: one of {self._params()}")
         return super().param_shape(layer, name)
+
+
+def pna_degree_averages(deg):
+    """PyG's PNAConv averages of a degree histogram deg (deg[k] = the number of nodes of in-degree k), in fp64:
+    (delta_lin, delta_log) = (sum_k k deg[k], sum_k log(k + 1) deg[k]) / sum_k deg[k].  Raises ValueError for a histogram
+    that is not a 1-D array of non-negative integers with a positive sum."""
+    h = np.asarray(deg)
+    if h.ndim != 1 or h.size == 0:
+        raise ValueError(f"deg must be a 1-D degree histogram, got shape {h.shape}")
+    h = h.astype(np.float64)
+    if not np.all(np.isfinite(h)) or np.any(h < 0) or np.any(h != np.round(h)):
+        raise ValueError("deg must hold non-negative integer counts")
+    total = h.sum()
+    if total <= 0:
+        raise ValueError("deg counts no node")
+    k = np.arange(h.size, dtype=np.float64)
+    return float((k * h).sum() / total), float((np.log(k + 1.0) * h).sum() / total)
+
+
+class PNA(_ModelByName):
+    """PNA: layers of PyG's PNAConv(in, out, aggregators, scalers, deg, towers=1, pre_layers=1, post_layers=1,
+    divide_input=False, edge_dim=None, train_norm=False), forward and backward (include/hnh/pna.hpp).  layers:
+    [(input_features, output_features), ...]; aggregators: an ordered collection of "mean", "sum", "min", "max", "var"
+    and "std" over the stored entries of each S-row on all ranks (duplicates count; a row without entries aggregates
+    to 0); scalers: of "identity", "amplification", "attenuation", "linear" and "inverse_linear"; deg: the integer
+    in-degree histogram PNAConv takes (needed when a scaler reads the degree averages, which are taken in fp64;
+    a histogram that is given is always checked).  Min and max
+    split their gradient equally over tied entries.  Every layer but the last ends in a ReLU.  The algorithm object must
+    outlive this one.  Construction is collective: a bad argument on any rank is refused on every rank.
+
+    Parameters (zero after construction), by layer and name: "pre" (2 input_features x input_features), "pre_bias",
+    "post" ((A S + 1) input_features x r), "post_bias", "lin" (r x r) and "lin_bias".  A PNAConv state dict maps onto
+    them as pre_nns.0.0.weight.T -> "pre", pre_nns.0.0.bias -> "pre_bias", post_nns.0.0.weight.T -> "post",
+    post_nns.0.0.bias -> "post_bias", lin.weight.T -> "lin" and lin.bias -> "lin_bias"."""
+
+    AGGREGATORS = ("mean", "sum", "min", "max", "var", "std")
+    SCALERS = ("identity", "amplification", "attenuation", "linear", "inverse_linear")
+    DEGREE_SCALERS = ("amplification", "attenuation", "linear", "inverse_linear")  # the scalers that read deg
+    PARAMS = ("pre", "pre_bias", "post", "post_bias", "lin", "lin_bias")
+    VECTORS = ("pre_bias", "post_bias", "lin_bias")
+    _PREFIX = "pna"
+
+    def __init__(self, alg: Algorithm, layers, aggregators=("mean", "min", "max", "std"),
+                 scalers=("identity", "amplification", "attenuation"), deg=None):
+        self.alg = alg
+        self.layers = [tuple(int(x) for x in l) for l in layers]
+        if not self.layers or any(len(l) != 2 for l in self.layers):
+            raise ValueError("layers are a non-empty list of (input_features, output_features) pairs")
+        self.aggregators = [aggregators] if isinstance(aggregators, str) else [str(a) for a in aggregators]
+        self.scalers = [scalers] if isinstance(scalers, str) else [str(s) for s in scalers]
+        # A refused histogram reaches the collective constructor as NaN averages, which it refuses on every rank, so
+        # that no rank is left waiting in the constructor's collectives.  Without a histogram the averages are 0, which
+        # the constructor refuses where a scaler reads them.
+        problem = None
+        if deg is None:
+            lin = log = 0.0
+            if any(s in self.DEGREE_SCALERS for s in self.scalers):
+                problem = f"deg, the degree histogram, is needed by the scalers {self.scalers}"
+        else:
+            try:
+                lin, log = pna_degree_averages(deg)
+            except ValueError as e:
+                lin = log = math.nan
+                problem = str(e)
+        self.avg_deg_lin, self.avg_deg_log = lin, log
+        flat = (C.c_int * (2 * len(self.layers)))(*[x for l in self.layers for x in l])
+        self.h = C.c_void_p()
+        rc = lib().hnhd_pna_create(alg.h, len(self.layers), flat, ",".join(self.aggregators).encode(),
+                                   ",".join(self.scalers).encode(), lin, log, C.byref(self.h))
+        if rc != 0 and problem is not None:
+            raise ValueError(problem)
+        check(rc, "pna_create")
 
 
 class TrainStep(NamedTuple):

@@ -326,6 +326,23 @@ public:
     void maxAggregate(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C);
     void maxAggregateBackward(DenseMatrix &X, DenseMatrix &Z, DenseMatrix &C, DenseMatrix &dZ, DenseMatrix &dX, bool accumulate);
 
+    // ---- multi-statistic aggregation (PNA): several statistics of each row's neighbours in one gather ----------------
+    // `which` is a non-empty union of HNH_MULTI_MOMENTS, HNH_MULTI_MAX and HNH_MULTI_MIN (hnh_b200.h).  multiAggregate
+    // overwrites A (localArows x W f, W = 2, 4 or 6) with the selected f-wide windows, in the fixed order
+    //     [sum_v X_v | sum_v X_v^2 | max_v X_v | #ties of the max | min_v X_v | #ties of the min]
+    // over the stored entries (u, v) of S on all ranks (duplicates count; S's values are not read), every window 0 on a
+    // row without entries.  The maxima and minima follow maxAggregate.  multiAggregateBackward, given the forward's A
+    // and dA (A's layout; its count windows are not read), writes
+    //     dX_v = sum_u dA_sum[u] + 2 X_v dA_sq[u] + [X_v == max_u] dA_max[u] / C_max[u] + [X_v == min_u] dA_min[u] / C_min[u]
+    // overwriting dX or, with `accumulate`, adding to it.  One gather_pass each, as maxAggregate: the forward in A order
+    // with A riding with the stored rows, the backward in B order with X and dX on the stored-row side.  Sums run in
+    // stored order without atomics: repeated calls are bit-identical.  Collective; defined where check_full_rows passes.
+    // HNH_E_INVALID on every rank before any launch for an empty or unknown `which`, an X that is not localBrows rows of
+    // width f >= 1, a total width W f of 2^31 or more, an A or dA that is not localArows x W f, a dX that is not X's
+    // shape, or an output that is another operand of the call.
+    void multiAggregate(DenseMatrix &X, DenseMatrix &A, int which);
+    void multiAggregateBackward(DenseMatrix &X, DenseMatrix &A, DenseMatrix &dA, DenseMatrix &dX, int which, bool accumulate);
+
     // ---- relational aggregation (R-GCN): each stored entry's value picks the window its neighbour is summed into ------
     // The relation of a stored entry (u, v) of S is its stored value (SpmatLocal::from_tuples' vals; an SDDMM or
     // FusedMM on this object overwrites it), an integer in [0, num_relations).  An entry with any other value

@@ -510,6 +510,63 @@ int hnh_max_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, 
                                int64_t ldx, const double *Z, int64_t ldz, const double *G, int64_t ldg, int f, double *dX,
                                int64_t lddx, void *stream);
 
+/* ---- multi-statistic aggregation (Distributed_Sparse::multiAggregate, PNA; csrc/pna.cu) -----------------------------
+ * Several statistics of the gathered rows of every CSR row in one pass.  `which` selects them (any non-empty union of
+ * the flags); the state A of a row holds the selected f-wide windows side by side in the fixed order
+ *     [S1 | S2 | MAX | CMAX | MIN | CMIN]          (HNH_MULTI_MOMENTS: S1, S2; HNH_MULTI_MAX: MAX, CMAX; HNH_MULTI_MIN: MIN, CMIN)
+ * so it is 2 f, 4 f or 6 f wide.  S's values are not read; duplicates count.
+ * hnh_multi_aggregate_step_f64: for every stored row u, over its entries v (X: gathered, leading dimension ldx),
+ *     S1_u += sum_v X_v,   S2_u += sum_v X_v^2,   (MAX_u, CMAX_u) = merge(.., (max_v X_v, #{v : X_v == max})),
+ *     (MIN_u, CMIN_u) likewise with the minimum
+ * merging as hnh_max_aggregate_step_f64 does.  A is read and written once per row (it may carry earlier blocks); before
+ * the first block it holds (0, 0, -inf, 0, +inf, 0).  Rows without entries are not touched.
+ * hnh_multi_aggregate_finish_f64 then sets MAX and MIN to 0 where their count is 0 (rows x f per window).
+ * hnh_multi_aggregate_grad_prep_f64: D (A's layout) = [dA_S1 | dA_S2 | MAX | dA_MAX / CMAX | MIN | dA_MIN / CMIN], the
+ * quotients 0 where the count is 0; dA has A's layout (its count windows are not read).
+ * hnh_multi_aggregate_grad_f64, on a block whose stored rows are X's (the B order): for every stored row v, over its
+ * entries u (D gathered),
+ *     dX_v += sum_u D_S1,u + 2 X_v sum_u D_S2,u + sum_u [X_v == MAX_u] D_CMAX,u + sum_u [X_v == MIN_u] D_CMIN,u
+ * (each sum in stored order in registers, then one read-modify-write of dX).
+ * f >= 1, the state's width below 2^31, every leading dimension >= its operand's width; outputs may not alias inputs.
+ * Column windows of 256 run separately; a window of width 4..256 (a power of two) with 16-byte aligned windows and
+ * even leading dimensions takes a row kernel with 128-bit gathers, others a one-warp-per-row kernel.  No atomics:
+ * repeated calls are bit-identical.
+ * hnh_pna_combine_f64 / _grad_f64: PNA's aggregators and degree scalers (include/hnh/pna.hpp) for rows x f elements.
+ * aggs and scalers hold n_aggs (1..6) and n_scalers (1..5) of the codes below, 4 bits each, the first in the lowest
+ * bits; deg (stride ldg) holds each row's entry count.  With h_uv = C_u + z_v and A the state of z:
+ *     P_u = [X_u | scale_s0(u) [agg_0(u) .. agg_n-1(u)] | scale_s1(u) [..] | ..]          ((n_aggs n_scalers + 1) f wide)
+ * and the gradient writes dC (rows x f) and dA (A's layout, count windows 0) from dP.  An aggregator whose statistic
+ * `which` does not hold (min without HNH_MULTI_MIN, max without HNH_MULTI_MAX, the others without HNH_MULTI_MOMENTS)
+ * is refused. */
+#define HNH_MULTI_MOMENTS 1
+#define HNH_MULTI_MAX 2
+#define HNH_MULTI_MIN 4
+#define HNH_MULTI_ALL 7
+#define HNH_PNA_MEAN 0
+#define HNH_PNA_SUM 1
+#define HNH_PNA_MIN 2
+#define HNH_PNA_MAX 3
+#define HNH_PNA_VAR 4
+#define HNH_PNA_STD 5
+#define HNH_PNA_IDENTITY 0
+#define HNH_PNA_AMPLIFICATION 1
+#define HNH_PNA_ATTENUATION 2
+#define HNH_PNA_LINEAR 3
+#define HNH_PNA_INVERSE_LINEAR 4
+int hnh_multi_aggregate_step_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, const double *X,
+                                 int64_t ldx, int f, int which, double *A, int64_t lda, void *stream);
+int hnh_multi_aggregate_finish_f64(double *A, int64_t lda, int64_t rows, int f, int which, void *stream);
+int hnh_multi_aggregate_grad_prep_f64(const double *A, int64_t lda, const double *dA, int64_t ldda, int64_t rows, int f, int which,
+                                      double *D, int64_t ldd, void *stream);
+int hnh_multi_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, const double *X,
+                                 int64_t ldx, const double *D, int64_t ldd, int f, int which, double *dX, int64_t lddx, void *stream);
+int hnh_pna_combine_f64(const double *X, int64_t ldx, const double *C, int64_t ldc, const double *A, int64_t lda, int which,
+                        const double *deg, int64_t ldg, int64_t rows, int f, unsigned aggs, int n_aggs, unsigned scalers, int n_scalers,
+                        double avg_deg_lin, double avg_deg_log, double *P, int64_t ldp, void *stream);
+int hnh_pna_combine_grad_f64(const double *dP, int64_t lddp, const double *A, int64_t lda, int which, const double *deg, int64_t ldg,
+                             int64_t rows, int f, unsigned aggs, int n_aggs, unsigned scalers, int n_scalers, double avg_deg_lin,
+                             double avg_deg_log, double *dC, int64_t lddc, double *dA, int64_t ldda, void *stream);
+
 /* ---- graph readout (include/hnh/graph_readout.hpp; csrc/graph_readout.cu) -------------------------------------------
  * Pools the rows of H (rows x r, leading dimension ldh) into one row per segment.  The segment CSR lists, for segment
  * g < segments, the rows seg_rows[seg_start[g] .. seg_start[g + 1]) of H (any order; the sums run in the listed order).

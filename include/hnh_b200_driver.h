@@ -302,6 +302,18 @@ int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd
 int hnhd_alg_max_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C, hnhd_dense_t *dZ,
                                     hnhd_dense_t *dX, int accumulate);
 
+/* ---- multi-statistic aggregation (Distributed_Sparse::multiAggregate) ----------------------------------------------
+ * which: a non-empty union of HNH_MULTI_MOMENTS (1), HNH_MULTI_MAX (2) and HNH_MULTI_MIN (4).  A (A-shaped, W f wide with
+ * W = 2 per selected flag) = the selected windows of [sum_v X_v | sum_v X_v^2 | max_v X_v | #ties | min_v X_v | #ties]
+ * over the stored entries (u, v) of each S-row (X B-shaped, f wide), 0 on a row without entries.  The backward overwrites
+ * dX (or adds to it with accumulate != 0) with sum_u dA_sum[u] + 2 X_v dA_sq[u] + [X_v == max_u] dA_max[u] / C_max[u] +
+ * [X_v == min_u] dA_min[u] / C_min[u], dA in A's layout (its count windows are not read).  Collective; HNH_E_INVALID on
+ * every rank where hnhd_alg_edge_softmax is, for an empty or unknown `which`, W f >= 2^31, wrong shapes, and for an
+ * output that is another operand. */
+int hnhd_alg_multi_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int which);
+int hnhd_alg_multi_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, hnhd_dense_t *dA, hnhd_dense_t *dX, int which,
+                                      int accumulate);
+
 /* ---- relational aggregation (Distributed_Sparse::relationalAggregate) -----------------------------------------------
  * A (A-shaped, num_relations * f wide) = for each S-row u and relation rho, the sum of X_v (B-shaped, f wide) over the
  * stored entries (u, v) whose value is rho (0 where there are none; entries whose value is not an integer in
@@ -475,6 +487,20 @@ int hnhd_gt_set_edge_attributes(hnhd_model_t *g, const double *attr_A, int64_t n
  * HNH_E_INVALID on every rank before any launch where hnhd_alg_edge_softmax is, for unknown aggregations, non-positive
  * sizes and widths that do not chain. */
 int hnhd_sage_create(hnhd_alg_t *alg, int n_layers, const int *layers2, const char *aggr, hnhd_model_t **out);
+
+/* ---- PNA (include/hnh/pna.hpp) --------------------------------------------------------------------------------------
+ * Layers of PyG's PNAConv(towers = 1, pre_layers = 1, post_layers = 1, divide_input = False, edge_dim = None):
+ * layers2 = {input_features, output_features} per layer; aggregators is a comma-separated, order-preserving list of
+ * mean, sum, min, max, var, std and scalers one of identity, amplification, attenuation, linear, inverse_linear;
+ * avg_deg_lin and avg_deg_log are PyG's averages of d and log(d + 1) over the degree histogram (read only when a scaler
+ * uses them; NaN is refused always, and marks a histogram the caller refused).  Every layer but the last ends in a ReLU.  Parameters by layer and name: "pre" (2f x f:
+ * pre_nns.0.0.weight.T), "pre_bias" (f x 1), "post" ((A S + 1) f x r: post_nns.0.0.weight.T), "post_bias" (r x 1),
+ * "lin" (r x r: lin.weight.T), "lin_bias" (r x 1).  Collective; HNH_E_INVALID on every rank before any launch where
+ * hnhd_alg_edge_softmax is, for an empty, unknown or repeated aggregator or scaler, a NaN average, an average a scaler
+ * uses that is not finite and > 0, non-positive sizes, widths that do not chain, (A S + 1) f >= 2^31, and arguments that differ between
+ * ranks. */
+int hnhd_pna_create(hnhd_alg_t *alg, int n_layers, const int *layers2, const char *aggregators, const char *scalers,
+                    double avg_deg_lin, double avg_deg_log, hnhd_model_t **out);
 
 /* ---- R-GCN (include/hnh/rgcn.hpp) ----------------------------------------------------------------------------------
  * Layers of PyG's RGCNConv(in, out, num_relations, aggr, root_weight = True, bias = True) without basis or block
