@@ -130,6 +130,11 @@ ABI = {
                                       C.c_int, C.c_double, C.c_double, _P, _I64, _P]),
     "hnh_pna_combine_grad_f64": (C.c_int, [_P, _I64, _P, _I64, C.c_int, _P, _I64, _I64, C.c_int, C.c_uint, C.c_int, C.c_uint,
                                            C.c_int, C.c_double, C.c_double, _P, _I64, _P, _I64, _P]),
+    "hnh_edge_relu_aggregate_step_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
+    "hnh_edge_relu_aggregate_grad_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
+    "hnh_edge_relu_aggregate_edge_grad_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P, _I64, _P, _I64, C.c_int, _P, _I64, _P]),
+    "hnh_gin_combine_f64": (C.c_int, [_P, _P, _P, _P, _I64, _P]),
+    "hnh_gin_combine_grad_f64": (C.c_int, [_P, _P, _P, _P, _P, _I64, _P]),
     "hnh_relational_aggregate_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_relational_aggregate_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),
     "hnh_window_scale_f64": (C.c_int, [_P, _I64, _P, _I64, _I64, C.c_int, C.c_int, _P]),
@@ -318,6 +323,10 @@ ABI.update({
     "hnhd_alg_relational_aggregate_backward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int]),
     "hnhd_alg_multi_aggregate": (C.c_int, [_P, _P, _P, C.c_int]),
     "hnhd_alg_multi_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int]),
+    "hnhd_alg_edge_relu_aggregate": (C.c_int, [_P, _P, _P, _P]),
+    "hnhd_alg_edge_relu_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int]),
+    "hnhd_gin_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_double, C.c_int, _PP]),
+    "hnhd_gin_set_edge_attributes": (C.c_int, [_P, _P, _I64, _P, _I64]),
     "hnhd_pna_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, C.c_char_p, C.c_double, C.c_double, _PP]),
     "hnhd_rgcn_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_char_p, _PP]),
     "hnhd_rgcn_create_bases": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_char_p, _PP]),

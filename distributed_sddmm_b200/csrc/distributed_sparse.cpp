@@ -1237,6 +1237,86 @@ void Distributed_Sparse::multiAggregateBackward(DenseMatrix &X, DenseMatrix &A, 
                 });
 }
 
+// ---- edge-ReLU aggregation -------------------------------------------------------------------------------------------
+namespace {
+// the checks of edgeReluAggregate / edgeReluAggregateBackward (every rank decides alike: a layout gives every rank the
+// same widths and the caller passes the same matrices); returns f
+int64_t check_edge_relu(const Distributed_Sparse &d, const string &who, const DenseMatrix &X,
+                        std::initializer_list<const DenseMatrix *> A_like, std::initializer_list<const DenseMatrix *> outs,
+                        std::initializer_list<const DenseMatrix *> others) {
+    const int64_t f = X.cols();
+    if (X.rows() != d.localBrows || f < 1 || f > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": X is " + to_string(X.rows()) + " x " + to_string(f) + "; like_B_matrix has " +
+                                            to_string(d.localBrows) + " rows and the width must lie in [1, 2^31)");
+    for (const DenseMatrix *m : A_like)
+        if (m->rows() != d.localArows || m->cols() != f)
+            throw hnh::Error(HNH_E_INVALID, who + ": an A-shaped operand is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                ", not localArows x f = " + to_string(d.localArows) + " x " + to_string(f));
+    vector<const DenseMatrix *> all{&X};
+    all.insert(all.end(), A_like.begin(), A_like.end());
+    all.insert(all.end(), others.begin(), others.end());
+    for (const DenseMatrix *o : outs) {
+        if (!o) continue;
+        int same = 0;
+        for (const DenseMatrix *m : all) same += m && (m == o || (o->size() > 0 && m->data() == o->data()));
+        if (same != 1) throw hnh::Error(HNH_E_INVALID, who + ": an output may not be another operand of the call");
+    }
+    return f;
+}
+}  // namespace
+
+void Distributed_Sparse::edgeReluAggregate(DenseMatrix &X, const DenseMatrix &E_A, DenseMatrix &A) {
+    const string who = "edgeReluAggregate";
+    check_full_rows(who);
+    const int64_t f = check_edge_relu(*this, who, X, {&A}, {&A}, {&E_A});
+    const EdgeView ev = edge_view(*this, who, "E_A", &E_A, nullptr, k_sddmmA, f, f);
+    A.setZero();
+    gather_pass(k_sddmmA, {{&A, 0, f, true}}, {{&X, 0, f, false}},
+                [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, true, "edgeReluAggregate");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_edge_relu_aggregate_step_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords,
+                                                                    Y[0].p, Y[0].ld, ev.at(0, b), ev.ld(), (int)f, R[0].p, R[0].ld,
+                                                                    compute()),
+                                   "edge_relu_aggregate_step");
+                });
+}
+
+void Distributed_Sparse::edgeReluAggregateBackward(DenseMatrix &X, const DenseMatrix *E_A, const DenseMatrix *E_B, DenseMatrix &dA,
+                                                   DenseMatrix &dX, DenseMatrix *dE_A, bool accumulate) {
+    const string who = "edgeReluAggregateBackward";
+    check_full_rows(who);
+    if (E_A == nullptr || E_B == nullptr) throw hnh::Error(HNH_E_INVALID, who + ": the edge rows need both orders, E_A and E_B");
+    const int64_t f = check_edge_relu(*this, who, X, {&dA}, {&dX, dE_A}, {E_A, E_B, &dX, dE_A});
+    if (dX.rows() != X.rows() || dX.cols() != f)
+        throw hnh::Error(HNH_E_INVALID, who + ": dX is " + to_string(dX.rows()) + " x " + to_string(dX.cols()) + ", X " +
+                                            to_string(X.rows()) + " x " + to_string(f));
+    const EdgeView evA = edge_view(*this, who, "E_A", E_A, dE_A, k_sddmmA, f, f),
+                   evB = edge_view(*this, who, "E_B", E_B, nullptr, k_sddmmB, f, f);
+    if (!accumulate) dX.setZero();
+    gather_pass(k_sddmmB, {{&dA, 0, f, false}}, {{&X, 0, f, false}, {&dX, 0, f, true}},
+                [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, false, "edgeReluAggregateBackward");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_edge_relu_aggregate_grad_f64(h->rowStart.data(), h->col_idx.data(), blk.rows, blk.num_coords,
+                                                                    R[0].p, R[0].ld, evB.at(0, b), evB.ld(), Y[0].p, Y[0].ld, (int)f,
+                                                                    R[1].p, R[1].ld, compute()),
+                                   "edge_relu_aggregate_grad");
+                });
+    if (!dE_A) return;
+    dE_A->resize(E_A->rows(), f);
+    gather_pass(k_sddmmA, {{&dA, 0, f, false}}, {{&X, 0, f, false}},
+                [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                    need_rows(rows_are_A, true, "edgeReluAggregateBackward");
+                    CSRHandle *h = blk.getActive();
+                    hnh::abi_check(hnh_edge_relu_aggregate_edge_grad_f64(h->rowStart.data(), h->col_idx.data(), blk.rows,
+                                                                         blk.num_coords, R[0].p, R[0].ld, Y[0].p, Y[0].ld,
+                                                                         evA.at(0, b), evA.ld(), (int)f, evA.grad_at(0, b), evA.ld(),
+                                                                         compute()),
+                                   "edge_relu_aggregate_edge_grad");
+                });
+}
+
 // ---- relational aggregation --------------------------------------------------------------------------------------------
 namespace {
 // the shape and aliasing checks of relationalAggregate / relationalAggregateBackward: X-shaped (localBrows x f) and

@@ -13,6 +13,7 @@
 #include "hnh/benchmark_dist.hpp"
 #include "hnh/distributed_sparse.h"
 #include "hnh/gat.hpp"
+#include "hnh/gin.hpp"
 #include "hnh/graph_readout.hpp"
 #include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
@@ -678,6 +679,22 @@ int hnhd_alg_multi_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense
     });
 }
 
+// ---- edge-ReLU aggregation -------------------------------------------------------------------------------------------
+int hnhd_alg_edge_relu_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *E_A, hnhd_dense_t *A) {
+    return guarded([&] {
+        if (!a || !X || !E_A || !A) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_edge_relu_aggregate: null argument");
+        a->alg->edgeReluAggregate(X->m, E_A->m, A->m);
+    });
+}
+int hnhd_alg_edge_relu_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *E_A, hnhd_dense_t *E_B, hnhd_dense_t *dA,
+                                          hnhd_dense_t *dX, hnhd_dense_t *dE_A, int accumulate) {
+    return guarded([&] {
+        if (!a || !X || !dA || !dX) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_edge_relu_aggregate_backward: null argument");
+        a->alg->edgeReluAggregateBackward(X->m, E_A ? &E_A->m : nullptr, E_B ? &E_B->m : nullptr, dA->m, dX->m,
+                                          dE_A ? &dE_A->m : nullptr, accumulate != 0);
+    });
+}
+
 // ---- relational aggregation ------------------------------------------------------------------------------------------
 int hnhd_alg_relational_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, int num_relations) {
     return guarded([&] {
@@ -756,6 +773,14 @@ int hnhd_pna_create(hnhd_alg_t *a, int n_layers, const int *layers2, const char 
         vector<PNALayer> layers;
         for (int i = 0; i < n_layers; i++) layers.emplace_back(layers2[2 * i], layers2[2 * i + 1]);
         *out = new hnhd_model{std::unique_ptr<GraphModel>(new PNA(layers, a->alg.get(), aggregators, scalers, avg_deg_lin, avg_deg_log))};
+    });
+}
+int hnhd_gin_create(hnhd_alg_t *a, int n_layers, const int *layers3, int edge_dim, double eps, int train_eps, hnhd_model_t **out) {
+    return guarded([&] {
+        if (!a || !layers3 || !out || n_layers <= 0) throw hnh::Error(HNH_E_INVALID, "hnhd_gin_create: bad argument");
+        vector<GINLayer> layers;
+        for (int i = 0; i < n_layers; i++) layers.emplace_back(layers3[3 * i], layers3[3 * i + 1], layers3[3 * i + 2]);
+        *out = new hnhd_model{std::unique_ptr<GraphModel>(new GIN(layers, a->alg.get(), edge_dim, eps, train_eps != 0))};
     });
 }
 static int rgcn_create(hnhd_alg_t *a, int n_layers, const int *layers2, int num_relations, const char *aggr, int num_bases,
@@ -1047,6 +1072,16 @@ int hnhd_gat_get_attention_grads(hnhd_model_t *m, int layer, int head, double *d
 int hnhd_gt_set_edge_attributes(hnhd_model_t *m, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B) {
     return guarded([&] {
         GraphTransformer &g = model_as<GraphTransformer>(m, "graph transformer");
+        if ((n_A > 0 && !attr_A) || (n_B > 0 && !attr_B)) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        g.setEdgeAttributes(attr_A, n_A, attr_B, n_B);
+    });
+}
+
+
+// ---- GIN only
+int hnhd_gin_set_edge_attributes(hnhd_model_t *m, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B) {
+    return guarded([&] {
+        GIN &g = model_as<GIN>(m, "GIN");
         if ((n_A > 0 && !attr_A) || (n_B > 0 && !attr_B)) throw hnh::Error(HNH_E_INVALID, "null host pointer");
         g.setEdgeAttributes(attr_A, n_A, attr_B, n_B);
     });

@@ -509,6 +509,26 @@ class Algorithm:
                                                       self._dense_arg(dA, "dA"), self._dense_arg(dX, "dX"), w,
                                                       int(bool(accumulate))), "multi_aggregate_backward")
 
+    def edge_relu_aggregate(self, X: Dense, E: Dense, A: Dense):
+        """Collective: GINE's aggregation (Distributed_Sparse::edgeReluAggregate).  X is B-shaped, f wide; E holds one
+        f-wide row per entry of this rank's A value order (len(like_S_values()) x f, in the order of
+        entry_coordinates("A")); A (A-shaped, f wide) is overwritten with A_u = sum_i ReLU(X_v + E_i) over the stored
+        entries i = (u, v) of S on all ranks (duplicates count; S's values are not read), 0 on a row without entries."""
+        check(lib().hnhd_alg_edge_relu_aggregate(self.h, self._dense_arg(X, "X"), self._dense_arg(E, "E"),
+                                                 self._dense_arg(A, "A")), "edge_relu_aggregate")
+
+    def edge_relu_aggregate_backward(self, X: Dense, E_A: Dense, E_B: Dense, dA: Dense, dX: Dense, dE: Dense | None = None,
+                                     accumulate: bool = False):
+        """Collective: given dA = dLoss/dA (A-shaped), dX (X's shape) is overwritten -- or, with accumulate, added to --
+        with dX_v = sum_i [X_v + E_i > 0] dA_u, and dE (optional; resized to E_A's shape) with dE_i = [X_v + E_i > 0]
+        dA_u for every entry of the A order (Distributed_Sparse::edgeReluAggregateBackward).  E_A and E_B are the edge
+        rows of the A and B value orders (entry_coordinates("A") / ("B")), the same e(u, v) in both.  The mask is strict,
+        as torch's relu backward."""
+        check(lib().hnhd_alg_edge_relu_aggregate_backward(self.h, self._dense_arg(X, "X"), self._dense_arg(E_A, "E_A"),
+                                                          self._dense_arg(E_B, "E_B"), self._dense_arg(dA, "dA"),
+                                                          self._dense_arg(dX, "dX"), self._dense_arg(dE, "dE"),
+                                                          int(bool(accumulate))), "edge_relu_aggregate_backward")
+
     def relational_aggregate(self, X: Dense, A: Dense, num_relations: int):
         """Collective: R-GCN's aggregation (Distributed_Sparse::relationalAggregate).  The relation of each stored entry
         (u, v) of S is its stored value (SpmatLocal.from_tuples' vals; an SDDMM, SpMM or FusedMM on this object
@@ -878,6 +898,17 @@ class GAT(_Model):
         return out
 
 
+def _set_edge_attributes(net, set_fn, attr_A, attr_B):
+    """Checks the attributes against net.edge_dim and uploads them through the model's set_fn."""
+    if not net.edge_dim:
+        raise ValueError("the model has no edge features (edge_dim = 0)")
+    a, b = (np.ascontiguousarray(x, dtype=np.float64) for x in (attr_A, attr_B))
+    for name, x in (("attr_A", a), ("attr_B", b)):
+        if x.ndim != 2 or x.shape[1] != net.edge_dim:
+            raise ValueError(f"{name} must be n x {net.edge_dim}, got {x.shape}")
+    net._check(set_fn(net.h, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0]), "set_edge_attributes")
+
+
 class GraphTransformer(_ModelByName):
     """A graph transformer on fused sparse attention: layers of PyG's TransformerConv(concat=True, root_weight=True)
     with the heads concatenated, forward and backward (include/hnh/graph_transformer.hpp).  layers: [(input_features,
@@ -931,14 +962,7 @@ class GraphTransformer(_ModelByName):
         """The edge attributes of this rank's entries: attr_A (len(like_S_values()) x edge_dim) in the order of
         alg.entry_coordinates("A"), attr_B (len(like_ST_values()) x edge_dim) in that of entry_coordinates("B"), both
         holding the same attribute for every stored (u, v)."""
-        if not self.edge_dim:
-            raise ValueError("the model has no edge features (edge_dim = 0)")
-        a, b = (np.ascontiguousarray(x, dtype=np.float64) for x in (attr_A, attr_B))
-        for name, x in (("attr_A", a), ("attr_B", b)):
-            if x.ndim != 2 or x.shape[1] != self.edge_dim:
-                raise ValueError(f"{name} must be n x {self.edge_dim}, got {x.shape}")
-        check(lib().hnhd_gt_set_edge_attributes(self.h, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0]),
-              "gt_set_edge_attributes")
+        _set_edge_attributes(self, lib().hnhd_gt_set_edge_attributes, attr_A, attr_B)
 
     def forward(self, dropout: float = 0.0, seed: int = 0):
         """Collective.  dropout in [0, 1) is the attention dropout of every layer; layer l draws its masks at seed +
@@ -1050,6 +1074,52 @@ class RGCN(_ModelByName):
         if name not in self._params():
             raise ValueError(f"no parameter {name!r}: one of {self._params()}")
         return super().param_shape(layer, name)
+
+
+class GIN(_ModelByName):
+    """GIN and GINE: layers of PyG's GINConv(nn, eps, train_eps) or, with edge_dim > 0, GINEConv(nn, eps, train_eps,
+    edge_dim), with nn = Sequential(Linear(f, h), ReLU(), Linear(h, r)), forward and backward (include/hnh/gin.hpp).
+    layers: [(f, h, r), ...].  GIN sums the neighbours X_v of each S-row over its stored entries on all ranks
+    (duplicates count; a row without entries aggregates to 0); GINE sums ReLU(X_v + e_uv) with e = attr lin.weight.T +
+    lin.bias on the per-entry attributes set with set_edge_attributes.  Then H = M + (1 + eps) X and the MLP.  Every
+    layer but the last ends in a ReLU.  eps starts at `eps` and is trained only with train_eps; otherwise it is a
+    constant that no optimizer step, weight decay included, moves (its gradient reads 0).  The algorithm object must
+    outlive this one.
+
+    Parameters, by layer and name: "lin1" (f x h), "lin1_bias" (h), "lin2" (h x r), "lin2_bias" (r), with edge features
+    "edge" (edge_dim x f) and "edge_bias" (f), and "eps" (1); all zero after construction except eps.  A GINConv /
+    GINEConv state dict maps onto them as nn.0.weight.T -> "lin1", nn.0.bias -> "lin1_bias", nn.2.weight.T -> "lin2",
+    nn.2.bias -> "lin2_bias", lin.weight.T -> "edge", lin.bias -> "edge_bias" and eps -> "eps"."""
+
+    VECTORS = ("lin1_bias", "lin2_bias", "edge_bias", "eps")
+    _PREFIX = "gin"
+
+    def __init__(self, alg: Algorithm, layers, edge_dim: int = 0, eps: float = 0.0, train_eps: bool = False):
+        self.alg = alg
+        self.layers = [tuple(int(x) for x in l) for l in layers]
+        if not self.layers or any(len(l) != 3 for l in self.layers):
+            raise ValueError("layers are a non-empty list of (input_features, hidden_features, output_features) triples")
+        if any(a[2] != b[0] for a, b in zip(self.layers, self.layers[1:])):
+            raise ValueError(f"the layer widths {self.layers} do not chain")
+        if isinstance(edge_dim, bool) or not isinstance(edge_dim, numbers.Integral) or edge_dim < 0:
+            raise ValueError(f"edge_dim = {edge_dim!r} must be a non-negative integer")
+        if isinstance(eps, bool) or not isinstance(eps, numbers.Real) or not math.isfinite(eps):
+            raise ValueError(f"eps = {eps!r} must be a finite number")
+        self.edge_dim, self.eps, self.train_eps = int(edge_dim), float(eps), bool(train_eps)
+        flat = (C.c_int * (3 * len(self.layers)))(*[x for l in self.layers for x in l])
+        self.h = C.c_void_p()
+        check(lib().hnhd_gin_create(alg.h, len(self.layers), flat, self.edge_dim, self.eps, int(self.train_eps),
+                                    C.byref(self.h)), "gin_create")
+
+    def param_names(self):
+        names = ["lin1", "lin1_bias", "lin2", "lin2_bias"]
+        return names + (["edge", "edge_bias"] if self.edge_dim else []) + ["eps"]
+
+    def set_edge_attributes(self, attr_A, attr_B):
+        """The edge attributes of this rank's entries: attr_A (len(like_S_values()) x edge_dim) in the order of
+        alg.entry_coordinates("A"), attr_B (len(like_ST_values()) x edge_dim) in that of entry_coordinates("B"), both
+        holding the same attribute for every stored (u, v)."""
+        _set_edge_attributes(self, lib().hnhd_gin_set_edge_attributes, attr_A, attr_B)
 
 
 def pna_degree_averages(deg):

@@ -343,6 +343,24 @@ public:
     void multiAggregate(DenseMatrix &X, DenseMatrix &A, int which);
     void multiAggregateBackward(DenseMatrix &X, DenseMatrix &A, DenseMatrix &dA, DenseMatrix &dX, int which, bool accumulate);
 
+    // ---- edge-ReLU aggregation (GINE): a per-entry vector added to each gathered row before a ReLU ---------------------
+    // E_A (num_S_values x f) and E_B (num_ST_values x f) are per-entry rows in the A and B value orders, laid out as
+    // sparseAttention's edge features (entry i of block b at row blockStarts[b] + i; they stay on the rank that owns the
+    // entry) and holding the same e(u, v) for every stored (u, v), so stored duplicates share one row.  Over the stored
+    // entries i = (u, v) of S on all ranks (duplicates count; S's values are not read):
+    //     edgeReluAggregate:          A_u  = sum_i ReLU(X_v + E_i)                  (0 on a row without entries)
+    //     edgeReluAggregateBackward:  dX_v (+)= sum_i [X_v + E_i > 0] dA_u,   dE_A,i = [X_v + E_i > 0] dA_u
+    // with the strict mask of torch's relu backward.  One gather_pass each: the forward in A order with A riding with
+    // the stored rows, dX in B order (X and dX stored, dA gathered, E_B read), dE_A in A order (dA stored, X gathered,
+    // E_A read; every row written once) and skipped for a null dE_A.  dX is overwritten or, with `accumulate`, added
+    // to.  Sums run in stored order without atomics: repeated calls are bit-identical.  Collective; defined where
+    // check_full_rows passes.  HNH_E_INVALID on every rank before any launch for an X that is not localBrows rows of
+    // width 1 <= f < 2^31, an A or dA that is not localArows x f, a dX that is not X's shape, an E_A or E_B that is not
+    // its order's entry count x f, only one of E_A / E_B, or an output that is another operand of the call.
+    void edgeReluAggregate(DenseMatrix &X, const DenseMatrix &E_A, DenseMatrix &A);
+    void edgeReluAggregateBackward(DenseMatrix &X, const DenseMatrix *E_A, const DenseMatrix *E_B, DenseMatrix &dA, DenseMatrix &dX,
+                                   DenseMatrix *dE_A, bool accumulate);
+
     // ---- relational aggregation (R-GCN): each stored entry's value picks the window its neighbour is summed into ------
     // The relation of a stored entry (u, v) of S is its stored value (SpmatLocal::from_tuples' vals; an SDDMM or
     // FusedMM on this object overwrites it), an integer in [0, num_relations).  An entry with any other value

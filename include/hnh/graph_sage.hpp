@@ -194,17 +194,6 @@ private:
         }
     }
 
-    // [A 1]: the bias gradients are the products with its ones column
-    static DenseMatrix with_ones(const DenseMatrix &A) {
-        const int64_t n = A.rows(), f = A.cols();
-        DenseMatrix Aa = DenseMatrix::Constant(n, f + 1, 1.0);
-        const size_t dsz = sizeof(double);
-        hnh::cuda_check(cudaMemcpy2DAsync(Aa.data(), (f + 1) * dsz, A.data(), f * dsz, f * dsz, (size_t)n, cudaMemcpyDeviceToDevice,
-                                          stream()),
-                        "[A 1]");
-        return Aa;
-    }
-
     // layer i: G = dL/d buffers[i + 1]; writes layers[i].grads and dX = dL/d buffers[i]
     void backwardLayer(int i, const DenseMatrix &G, DenseMatrix &dX) {
         GraphSAGELayer &layer = layers[(size_t)i];

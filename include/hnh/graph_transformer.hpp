@@ -156,16 +156,8 @@ public:
     // Edge attributes of S's entries in both value orders (row i belongs to entry i of like_S_values /
     // like_ST_values); every rank passes its part of the same attributes.  Makes the activations stale.
     void setEdgeAttributes(const double *host_A, int64_t n_A, const double *host_B, int64_t n_B) {
-        if (edge_dim == 0) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: the model has no edge features (edge_dim = 0)");
-        if (n_A != d_ops->num_S_values() || n_B != d_ops->num_ST_values())
-            throw hnh::Error(HNH_E_INVALID, "GraphTransformer: edge attributes for " + std::to_string(n_A) + " and " +
-                                                std::to_string(n_B) + " entries; this rank holds " +
-                                                std::to_string(d_ops->num_S_values()) + " (A order) and " +
-                                                std::to_string(d_ops->num_ST_values()) + " (B order)");
-        edge_attr_A = DenseMatrix::from_host(host_A, n_A, edge_dim);
-        edge_attr_B = DenseMatrix::from_host(host_B, n_B, edge_dim);
+        uploadEdgeAttributes("GraphTransformer", edge_dim, host_A, n_A, host_B, n_B, edge_attr_A, edge_attr_B);
         has_edge_attributes = true;
-        activations_current = false;
     }
 
     // Each layer's params with its grads, one span per layer
@@ -330,17 +322,6 @@ private:
                                             n, r, stream()),
                        "row_bias_add");
         if (keep_Z) *keep_Z = std::move(Z);
-    }
-
-    // [A 1]: the bias gradients are the products with its ones column
-    static DenseMatrix with_ones(const DenseMatrix &A) {
-        const int64_t n = A.rows(), f = A.cols();
-        DenseMatrix Aa = DenseMatrix::Constant(n, f + 1, 1.0);
-        const size_t dsz = sizeof(double);
-        hnh::cuda_check(cudaMemcpy2DAsync(Aa.data(), (f + 1) * dsz, A.data(), f * dsz, f * dsz, (size_t)n, cudaMemcpyDeviceToDevice,
-                                          stream()),
-                        "[A 1]");
-        return Aa;
     }
 
     // LN backward of G for block part j (0: LN1 on X, 4: LN2 on X + Res) into dX, its gain and bias gradients into grads

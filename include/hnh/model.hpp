@@ -1,13 +1,14 @@
-// hnh/model.hpp -- what GAT, GraphTransformer, GraphSAGE and RGCN share, so that one train step (hnh/training.hpp) and
-// one driver handle (hnhd_model_t) serve them all: the algorithm object, the activation buffers, the input gradient,
-// the staleness flag, and virtual forward, backward, parameter list and parameter lookup.  Host-side dispatch only; the
-// device work of each model is its own.
+// hnh/model.hpp -- what GAT, GraphTransformer, GraphSAGE, RGCN, PNA and GIN share, so that one train step
+// (hnh/training.hpp) and one driver handle (hnhd_model_t) serve them all: the algorithm object, the activation buffers,
+// the input gradient, the staleness flag, and virtual forward, backward, parameter list and parameter lookup; and the
+// host helpers several models use.  Host-side dispatch only; the device work of each model is its own.
 #pragma once
 #include <cstdint>
 #include <string>
 #include <vector>
 
 #include "hnh/distributed_sparse.h"
+#include "hnh/runtime.h"
 #include "hnh_b200.h"
 
 // One parameter tensor of a model as the optimizer sees it: n doubles on the device with their gradient
@@ -59,6 +60,31 @@ protected:
     void refuse_dropout(double dropout) const {
         if (dropout != 0.0)
             throw hnh::Error(HNH_E_INVALID, model_name + ": the model has no dropout, got dropout = " + std::to_string(dropout));
+    }
+    // Edge attributes of S's entries in both value orders, edge_dim wide (row i of host_A / host_B belongs to entry i of
+    // like_S_values / like_ST_values; every rank passes its part of the same attributes), uploaded into attr_A / attr_B.
+    // Makes the activations stale.  HNH_E_INVALID, `who` first, for a model without edge features (edge_dim = 0) or
+    // entry counts that are not this rank's.
+    void uploadEdgeAttributes(const string &who, int edge_dim, const double *host_A, int64_t n_A, const double *host_B, int64_t n_B,
+                              DenseMatrix &attr_A, DenseMatrix &attr_B) {
+        if (edge_dim == 0) throw hnh::Error(HNH_E_INVALID, who + ": the model has no edge features (edge_dim = 0)");
+        if (n_A != d_ops->num_S_values() || n_B != d_ops->num_ST_values())
+            throw hnh::Error(HNH_E_INVALID, who + ": edge attributes for " + std::to_string(n_A) + " and " + std::to_string(n_B) +
+                                                " entries; this rank holds " + std::to_string(d_ops->num_S_values()) + " (A order) and " +
+                                                std::to_string(d_ops->num_ST_values()) + " (B order)");
+        attr_A = DenseMatrix::from_host(host_A, n_A, edge_dim);
+        attr_B = DenseMatrix::from_host(host_B, n_B, edge_dim);
+        activations_current = false;
+    }
+    // [A 1]: the bias gradients are the products with its ones column
+    static DenseMatrix with_ones(const DenseMatrix &A) {
+        const int64_t n = A.rows(), f = A.cols();
+        DenseMatrix Aa = DenseMatrix::Constant(n, f + 1, 1.0);
+        const size_t dsz = sizeof(double);
+        hnh::cuda_check(cudaMemcpy2DAsync(Aa.data(), (f + 1) * dsz, A.data(), f * dsz, f * dsz, (size_t)n, cudaMemcpyDeviceToDevice,
+                                          hnh::Runtime::get().compute_stream()),
+                        "[A 1]");
+        return Aa;
     }
     // the span of one layer's parameter vector, and a named slice of it
     static ParamSpan span(VectorXd &params, VectorXd &grads) {

@@ -567,6 +567,33 @@ int hnh_pna_combine_grad_f64(const double *dP, int64_t lddp, const double *A, in
                              int64_t rows, int f, unsigned aggs, int n_aggs, unsigned scalers, int n_scalers, double avg_deg_lin,
                              double avg_deg_log, double *dC, int64_t lddc, double *dA, int64_t ldda, void *stream);
 
+/* ---- edge-ReLU aggregation (Distributed_Sparse::edgeReluAggregate, GINE; csrc/gine.cu) ------------------------------
+ * Entry i of the block (u its stored row, v = col_idx[i]) reads the f-wide edge row E_i at E + i lde.
+ * hnh_edge_relu_aggregate_step_f64:      A_u  += sum_i ReLU(X_v + E_i)           (X gathered; A read and written once per
+ *                                                                                 row, so it may carry earlier blocks)
+ * hnh_edge_relu_aggregate_grad_f64:      dX_v += sum_i [X_v + E_i > 0] dA_u       (stored rows are X's: the B order; dA
+ *                                                                                 gathered; one read-modify-write of dX)
+ * hnh_edge_relu_aggregate_edge_grad_f64: dE_i  = [X_v + E_i > 0] dA_u             (stored rows are dA's: the A order; X
+ *                                                                                 gathered; every row of dE written once)
+ * The mask is strict (torch's relu backward).  Rows without entries are not touched.  S's values are not read.  f >= 1,
+ * every leading dimension >= f; outputs may not alias inputs.  Column windows of 256 run separately; a window of width
+ * 4..256 (a power of two) with 16-byte aligned operands and even leading dimensions takes a row kernel with 128-bit
+ * loads, others a one-warp-per-row kernel.  E is streamed with an L2 evict-first policy.  No atomics: repeated calls
+ * are bit-identical.
+ * hnh_gin_combine_f64:      H = M + (1 + *eps) X over n contiguous elements (eps a device scalar; H may be M).
+ * hnh_gin_combine_grad_f64: dX = (1 + *eps) dH over n elements and, unless deps is null, *deps (device) = sum dH X in
+ *                           an order fixed by the device and n (repeated calls are bit-identical). */
+int hnh_edge_relu_aggregate_step_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, const double *X,
+                                     int64_t ldx, const double *E, int64_t lde, int f, double *A, int64_t lda, void *stream);
+int hnh_edge_relu_aggregate_grad_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz, const double *X,
+                                     int64_t ldx, const double *E, int64_t lde, const double *dA, int64_t ldda, int f, double *dX,
+                                     int64_t lddx, void *stream);
+int hnh_edge_relu_aggregate_edge_grad_f64(const int64_t *rowStart, const int64_t *col_idx, int64_t rows, int64_t nnz,
+                                          const double *dA, int64_t ldda, const double *X, int64_t ldx, const double *E, int64_t lde,
+                                          int f, double *dE, int64_t ldde, void *stream);
+int hnh_gin_combine_f64(double *H, const double *M, const double *X, const double *eps, int64_t n, void *stream);
+int hnh_gin_combine_grad_f64(double *dX, double *deps, const double *dH, const double *X, const double *eps, int64_t n, void *stream);
+
 /* ---- graph readout (include/hnh/graph_readout.hpp; csrc/graph_readout.cu) -------------------------------------------
  * Pools the rows of H (rows x r, leading dimension ldh) into one row per segment.  The segment CSR lists, for segment
  * g < segments, the rows seg_rows[seg_start[g] .. seg_start[g + 1]) of H (any order; the sums run in the listed order).

@@ -314,6 +314,18 @@ int hnhd_alg_multi_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, in
 int hnhd_alg_multi_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *A, hnhd_dense_t *dA, hnhd_dense_t *dX, int which,
                                       int accumulate);
 
+/* ---- edge-ReLU aggregation (Distributed_Sparse::edgeReluAggregate, GINE) ----------------------------------------------
+ * A (A-shaped, f wide) = sum_i ReLU(X_v + E_A,i) over the stored entries i = (u, v) of each S-row (X B-shaped, f wide;
+ * 0 on a row without entries).  E_A / E_B are per-entry rows of the A / B value orders (len(like_S_values) /
+ * len(like_ST_values) x f, rows in the order of hnhd_alg_entry_coordinates) holding the same e(u, v) in both.  The
+ * backward overwrites dX (or adds to it with accumulate != 0) with sum_i [X_v + E_i > 0] dA_u and, unless dE_A is null,
+ * sets dE_A (resized to E_A's shape) to [X_v + E_i > 0] dA_u per entry of the A order.  Collective; HNH_E_INVALID on
+ * every rank where hnhd_alg_edge_softmax is, for wrong shapes, only one of E_A / E_B, and an output that is another
+ * operand. */
+int hnhd_alg_edge_relu_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *E_A, hnhd_dense_t *A);
+int hnhd_alg_edge_relu_aggregate_backward(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *E_A, hnhd_dense_t *E_B, hnhd_dense_t *dA,
+                                          hnhd_dense_t *dX, hnhd_dense_t *dE_A, int accumulate);
+
 /* ---- relational aggregation (Distributed_Sparse::relationalAggregate) -----------------------------------------------
  * A (A-shaped, num_relations * f wide) = for each S-row u and relation rho, the sum of X_v (B-shaped, f wide) over the
  * stored entries (u, v) whose value is rho (0 where there are none; entries whose value is not an integer in
@@ -487,6 +499,17 @@ int hnhd_gt_set_edge_attributes(hnhd_model_t *g, const double *attr_A, int64_t n
  * HNH_E_INVALID on every rank before any launch where hnhd_alg_edge_softmax is, for unknown aggregations, non-positive
  * sizes and widths that do not chain. */
 int hnhd_sage_create(hnhd_alg_t *alg, int n_layers, const int *layers2, const char *aggr, hnhd_model_t **out);
+
+/* ---- GIN and GINE (include/hnh/gin.hpp) ------------------------------------------------------------------------------
+ * Layers of PyG's GINConv(nn, eps, train_eps), or GINEConv(nn, eps, train_eps, edge_dim) with edge_dim > 0, where nn =
+ * Sequential(Linear(f, h), ReLU(), Linear(h, r)): layers3 = {f, h, r} per layer.  Every layer but the last ends in a
+ * ReLU.  Parameters by layer and name: "lin1" (f x h: nn.0.weight.T), "lin1_bias" (h x 1), "lin2" (h x r: nn.2.weight.T),
+ * "lin2_bias" (r x 1), with edge features "edge" (edge_dim x f: lin.weight.T) and "edge_bias" (f x 1), and "eps" (1 x 1;
+ * trained only with train_eps != 0).  hnhd_gin_set_edge_attributes is hnhd_gt_set_edge_attributes for a GIN handle
+ * and refuses any other.  Collective; HNH_E_INVALID on every rank before any launch where hnhd_alg_edge_softmax is,
+ * for non-positive sizes, widths that do not chain, a negative edge_dim and a non-finite eps. */
+int hnhd_gin_create(hnhd_alg_t *alg, int n_layers, const int *layers3, int edge_dim, double eps, int train_eps, hnhd_model_t **out);
+int hnhd_gin_set_edge_attributes(hnhd_model_t *g, const double *attr_A, int64_t n_A, const double *attr_B, int64_t n_B);
 
 /* ---- PNA (include/hnh/pna.hpp) --------------------------------------------------------------------------------------
  * Layers of PyG's PNAConv(towers = 1, pre_layers = 1, post_layers = 1, divide_input = False, edge_dim = None):
