@@ -12,6 +12,9 @@ algorithm and runs the case's kind:
   gt       graph transformer forward and backward (a configuration of GT_CONFIGS)
   gt_train graph transformer node train steps
   gt_link  graph transformer link train steps against the targets of link_pairs, then link_evaluate
+  gnn      PNA, GIN or GINE forward and backward (a configuration of GNN_CONFIGS)
+  gnn_train  PNA, GIN or GINE node, link (the targets of link_pairs) or graph (readout_batch) train steps
+  gine_int edge_relu_aggregate and its backward on integer inputs (exact results)
 
 Every op runs twice and the worker records whether the repeat gave the same bits.  It writes its rows of the results
 -- or the error the layout must raise -- to <outdir>/<case>_rank<r>.npz.
@@ -27,7 +30,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tests import gat_additive_oracle as gao  # noqa: E402
+from tests import gin_oracle as go  # noqa: E402
 from tests import graph_transformer_block_oracle as gbo  # noqa: E402
+from tests import pna_oracle as po  # noqa: E402
 from tests.mp_edge_softmax_worker import score, upstream  # noqa: E402
 from tests.mp_graph_transformer_worker import attr_of  # noqa: E402
 from tests.mp_sparse_attention_edge_worker import edge_of  # noqa: E402
@@ -427,8 +432,211 @@ def run_gt_link(D, alg, case, M, N, out):
     del t, algT
 
 
+# ---- PNA, GIN and GINE ---------------------------------------------------------------------------------------------
+# Configurations and, per layer, the width and the path of the layer's sparse aggregation (tests/test_skewed_gnn_fixture.py
+# checks these against the kernels' tables): PNA gathers the statistics of z (input-wide) with multiAggregate, GIN sums
+# X with spmmA, GINE sums ReLU(X_v + E_i) with edgeReluAggregate.  "table": one window of a width of HNH_DISPATCH_R
+# (the 128-bit row kernels); "windows": wider than kWindow, so several column windows; "generic": an odd width, the
+# one-warp-per-row kernels.
+PNA_DEFAULT = (("mean", "min", "max", "std"), ("identity", "amplification", "attenuation"))
+GNN_CONFIGS = {
+    "pna_table": dict(model="pna", layers=[[64, 128], [128, 256], [256, 4]], aggregators=PNA_DEFAULT[0], scalers=PNA_DEFAULT[1],
+                      reach=("table", "table", "table")),
+    "pna_all": dict(model="pna", layers=[[128, 16], [16, 4]], aggregators=po.AGGREGATORS, scalers=po.SCALERS,
+                    reach=("table", "table")),
+    "pna_wide": dict(model="pna", layers=[[300, 4]], aggregators=("sum", "var"), scalers=("linear",), reach=("windows",)),
+    "pna_odd": dict(model="pna", layers=[[7, 13], [13, 4]], aggregators=PNA_DEFAULT[0], scalers=PNA_DEFAULT[1],
+                    reach=("generic", "generic")),
+    "gin_table": dict(model="gin", layers=[[64, 32, 128], [128, 32, 256], [256, 32, 4]], edge_dim=0,
+                      reach=("table", "table", "table")),
+    "gine_table": dict(model="gin", layers=[[64, 32, 128], [128, 32, 256], [256, 32, 4]], edge_dim=3,
+                       reach=("table", "table", "table")),
+    "gine_odd": dict(model="gin", layers=[[7, 9, 13], [13, 9, 4]], edge_dim=2, reach=("generic", "generic")),
+}
+GINE_INT_WIDTH = 64  # the gine_int case: edge_relu_aggregate at a table width
+TIE_ROWS = (4, 3154)  # rows without entries (row % 9 == 4) in the first and the last of 4 row blocks, given equal inputs
+READOUT_GRAPHS, READOUT_CLASSES = 24, 3
+GNN_LR = 1e-3  # the train cases: at 1e-2 the hub rows' sums make the losses grow tenfold per step
+
+
+def gnn_config(case):
+    cfg = dict(GNN_CONFIGS[case["gnn"]])
+    cfg["layers"] = [tuple(l) for l in cfg["layers"]]
+    return cfg
+
+
+_HIST = {}
+
+
+def degree_histogram(N, seed):
+    """The skewed graph's in-degree histogram (PNAConv's deg): the entries of each S-row, duplicates counted."""
+    if (N, seed) not in _HIST:
+        rows, _ = skewed_tuples(N, N, seed)
+        _HIST[N, seed] = np.bincount(np.bincount(rows.astype(np.int64), minlength=N))
+    return _HIST[N, seed]
+
+
+def gnn_inputs(N, cfg, seed):
+    """(params, X, G) of a PNA / GIN case, the same on every rank.  Rows TIE_ROWS of X are equal: they have no entries, so
+    their outputs are equal too, which gives max readout a maximum attained on two ranks."""
+    layers = cfg["layers"]
+    rng = np.random.default_rng(seed + 37)
+    if cfg["model"] == "pna":
+        params = po.random_params(layers, len(cfg["aggregators"]), len(cfg["scalers"]), rng)
+    else:
+        params = go.random_params(layers, cfg["edge_dim"], rng)
+    X = rng.uniform(-1, 1, (N, layers[0][0]))
+    X[TIE_ROWS[1]] = X[TIE_ROWS[0]]
+    G = rng.uniform(-1, 1, (N, layers[-1][-1]))
+    return params, X, G
+
+
+def gine_int_inputs(N, f, seed):
+    """(X, dA) of the gine_int case: integers, so that X_v + E_i == 0 happens and every sum is exact."""
+    rng = np.random.default_rng(seed + 43)
+    return rng.integers(-3, 4, (N, f)).astype(np.float64), rng.integers(-3, 4, (N, f)).astype(np.float64)
+
+
+def readout_batch(N, seed):
+    """(batch, G, labels) of the graph train cases: graph 0 holds 150 random rows and hub row 3, so it spans every row
+    block; graph 1 is TIE_ROWS alone (one maximum on two ranks); graph 2 is empty; the others take random rows; 10 % of
+    the rows are in no graph; two graphs are unlabelled."""
+    rng = np.random.default_rng(seed + 41)
+    G = READOUT_GRAPHS
+    batch = rng.integers(3, G, N)
+    batch[rng.random(N) < 0.1] = -1
+    batch[rng.choice(N, 150, replace=False)] = 0
+    batch[landmarks(N, N)["wide_hubs"][0]] = 0
+    batch[list(TIE_ROWS)] = 1
+    labels = rng.integers(0, READOUT_CLASSES, G)
+    labels[[5, 9]] = -1
+    return batch, G, labels
+
+
+def readout_head(width, seed):
+    rng = np.random.default_rng(seed + 47)
+    return rng.uniform(-1, 1, (width, READOUT_CLASSES)), rng.uniform(-0.5, 0.5, READOUT_CLASSES)
+
+
+def _gnn(D, alg, case, N):
+    cfg = gnn_config(case)
+    layers = cfg["layers"]
+    if cfg["model"] == "pna":
+        net = D.PNA(alg, layers, aggregators=cfg["aggregators"], scalers=cfg["scalers"], deg=degree_histogram(N, case["seed"]))
+    else:
+        net = D.GIN(alg, layers, edge_dim=cfg["edge_dim"], eps=0.0, train_eps=case.get("train_eps", True))
+    params, X, G = gnn_inputs(N, cfg, case["seed"])
+    for l, P in enumerate(params):
+        for k, v in P.items():
+            net.set_param(l, k, v)
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    rA, cA = alg.entry_coordinates("A")
+    rB, cB = alg.entry_coordinates("B")
+    # what the case reached on this rank: local rows, entries in each value order, the longest A-order row
+    reach = dict(topA=topA, nrA=nrA, topB=topB, nrB=nrB, local_rows=net.buffer_shape(0)[0], nA=len(rA), nB=len(rB),
+                 longest=np.bincount(np.asarray(rA, np.int64)).max(initial=0) if len(rA) else 0)
+    net.set_input(gather_local(X, [(topB, 0, nrB, layers[0][0])], net.buffer_shape(0)))
+    if cfg["model"] == "gin" and cfg["edge_dim"]:
+        net.set_edge_attributes(go.attr_of(rA, cA, cfg["edge_dim"]), go.attr_of(rB, cB, cfg["edge_dim"]))
+    return cfg, net, G, reach
+
+
+def _gnn_params(net, layers, out):
+    for l in range(len(layers)):
+        for k in net.param_names():
+            out[f"p{l}_{k}"] = net.param(l, k)
+
+
+def run_gnn(D, alg, case, M, N, out):
+    cfg, net, G, reach = _gnn(D, alg, case, N)
+    out.update(reach)
+    layers = cfg["layers"]
+    Gl = gather_local(G, [(reach["topA"], 0, reach["nrA"], G.shape[1])], net.buffer_shape(len(layers)))
+    got = []
+    for _ in range(2):
+        net.forward()
+        o = dict(Y=net.buffer(len(layers)))
+        net.backward(Gl)
+        o["dX"] = net.input_grad()
+        for l in range(len(layers)):
+            for k in net.param_names():
+                o[f"g{l}_{k}"] = net.param_grad(l, k)
+        got.append(o)
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k], equal_nan=True) for k in got[0])
+    out.update(got[0])
+
+
+def run_gnn_train(D, alg, case, M, N, out):
+    """Three node, link or graph train steps (case["task"])."""
+    cfg, net, _, reach = _gnn(D, alg, case, N)
+    out.update(reach)
+    layers = cfg["layers"]
+    rows = net.buffer_shape(len(layers))[0]
+    topA = reach["topA"]
+    hi = min(topA + rows, N)
+    opt = D.AdamW(lr=GNN_LR)
+    if case["task"] == "node":
+        lab = -np.ones(rows, np.int64)
+        lab[:hi - topA] = labels_of(N, layers[-1][-1], case["seed"])[topA:hi]
+        nl = D.NodeLabels(net, lab, layers[-1][-1])
+        out["steps"] = np.array([list(net.train_step(nl, opt)) for _ in range(case["steps"])])
+    elif case["task"] == "link":
+        from distributed_sddmm_b200 import lib
+        rank, world = lib().hnhd_world_rank(), lib().hnhd_world_size()
+        tr, tc, y = link_pairs(N, case["seed"])
+        sr, sc = rank_slice(tr, tc, rank, world)
+        algT = D.Algorithm(case["alg"], D.SpmatLocal.from_tuples(N, N, sr.astype(np.uint64), sc.astype(np.uint64), y[rank::world]),
+                           layers[0][0], case["c"])
+        t = D.LinkTargets(net, algT)
+        out["steps"] = np.array([list(net.link_train_step(t, opt)) for _ in range(case["steps"])])
+        del t, algT
+    else:
+        batch, G, labels = readout_batch(N, case["seed"])
+        local = np.full(rows, -1, np.int64)
+        local[:hi - topA] = batch[topA:hi]
+        ro = D.GraphReadout(net, local, G, pool=case["pool"], num_classes=READOUT_CLASSES)
+        W_head, b_head = readout_head(layers[-1][-1], case["seed"])
+        ro.set_param("weight", W_head)
+        ro.set_param("bias", b_head)
+        gl = D.GraphLabels(ro, labels, READOUT_CLASSES)
+        out["steps"] = np.array([list(net.graph_train_step(ro, gl, opt)) for _ in range(case["steps"])])
+        for k in ro.param_names():
+            out[f"head_{k}"] = ro.param(k)
+        del gl, ro
+    _gnn_params(net, layers, out)
+
+
+def run_gine_int(D, alg, case, M, N, out):
+    """edge_relu_aggregate and its backward on integer X, dA and E = gin_oracle.edge_rows: every partial sum is an
+    integer far below 2^53, so the results are exact."""
+    f = case["R"]
+    X, dA = gine_int_inputs(N, f, case["seed"])
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    nA, nB = alg.like_A_matrix().shape[0], alg.like_B_matrix().shape[0]
+    Xd, A, dAd, dX, dE = D.Dense.create(nB, f), D.Dense.create(nA, f), D.Dense.create(nA, f), D.Dense.create(nB, f), D.Dense.create(0, 0)
+    rA, cA = alg.entry_coordinates("A")
+    rB, cB = alg.entry_coordinates("B")
+    EA, EB = D.Dense.create(len(rA), f), D.Dense.create(len(rB), f)
+    if len(rA):
+        EA.from_host(go.edge_rows(rA, cA, f))
+    if len(rB):
+        EB.from_host(go.edge_rows(rB, cB, f))
+    Xd.from_host(gather_local(X, [(topB, 0, nrB, f)], (nB, f)))
+    dAd.from_host(gather_local(dA, [(topA, 0, nrA, f)], (nA, f)))
+    out.update(topA=topA, nrA=nrA, topB=topB, nrB=nrB, rA=rA, cA=cA, nA=len(rA))
+    got = []
+    for _ in range(2):
+        alg.edge_relu_aggregate(Xd, EA, A)
+        alg.edge_relu_aggregate_backward(Xd, EA, EB, dAd, dX, dE)
+        got.append(dict(A=A.to_host(), dX=dX.to_host(), dE=dE.to_host()))
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k]) for k in got[0])
+    out.update(got[0])
+
+
 KINDS = dict(base=run_base, softmax=run_softmax, attn=run_attn, gat=run_gat, train=run_train, gt=run_gt, gt_train=run_gt_train,
-             gt_link=run_gt_link)
+             gt_link=run_gt_link, gnn=run_gnn, gnn_train=run_gnn_train, gine_int=run_gine_int)
 
 
 def run_case(D, case, rank, world):

@@ -5,10 +5,14 @@ self-loops, 4200 nodes so that 4 ranks hold 1050 rows each) at the kernels' tabl
 -inf scores, fused sparse attention (plain, dropout, a masking per-head bias, edge features) at heads x d = 2 x 64,
 1 x 128 and 4 x 7, GAT forward and backward with the four attention kinds and GAT train steps, and the graph
 transformer (the configurations of mp_skewed_worker.GT_CONFIGS: forward and backward, node and link train steps,
-link_evaluate), each against the fp64 models written per stored entry, rank by rank.  Beyond parity: rows without entries give Z = 0, L = -inf and zero dQ,
-untouched columns zero dK and dV; a repeat gives the same bits; the results at p = 2 and 4 equal those at p = 1 to
-1e-12; per-entry gradients (dbias, dE) of the two copies of a duplicate agree, with dropout too (one keep bit per
-(row, column), whatever the layout); trained parameters are bit-identical across ranks.
+link_evaluate), and PNA, GIN and GINE (the configurations of mp_skewed_worker.GNN_CONFIGS, aggregating at 64, 128
+and 256, past one 256-wide column window and at odd widths: forward and backward, node, link and graph train steps with
+all three pools, and GINE's edge-ReLU aggregation on integers, exact), each against the fp64 models written per stored
+entry, rank by rank.  Beyond parity: rows without entries give Z = 0, L = -inf and zero dQ, and PNA's and GIN's
+output from the row's own input alone; untouched columns zero dK, dV and GINE's dX; a repeat gives the same bits; the
+results at p = 2 and 4 equal those at p = 1 to 1e-12; per-entry gradients (dbias, dE) of the two copies of a duplicate
+agree, with dropout too (one keep bit per (row, column), whatever the layout); parameter gradients and trained
+parameters are bit-identical across ranks; GINE on 15d_fusion2 at p = 4 has a rank without A-order entries.
 
 One worker launch per rank count serves every test of that count.  Ranks share cuda:0 over the gloo-backed transport
 unless there is one GPU per rank (then NCCL)."""
@@ -27,9 +31,12 @@ from tests import gat_additive_oracle as gao
 from tests import gat_backward_oracle as gbk
 from tests import gat_softmax_oracle as gso
 from tests import gatv2_oracle as gv2
+from tests import gin_oracle as go
+from tests import graph_readout_oracle as gro
 from tests import graph_transformer_sparse_oracle as gts
 from tests import link_prediction_oracle as lpo
 from tests import mp_skewed_worker as W
+from tests import pna_oracle as po
 from tests import sparse_attention_bias_oracle as sb
 from tests import sparse_attention_dropout_oracle as sd
 from tests import sparse_attention_edge_oracle as se
@@ -71,6 +78,11 @@ def gt_case(kind, alg, c, config, **kw):
     return _case(kind, alg, c, W.GT_CONFIGS[config]["layers"][0][0], gt=config, mask_seed=31, **kw)
 
 
+def gnn_case(kind, alg, c, config, **kw):
+    """A PNA, GIN or GINE case of configuration `config` (mp_skewed_worker.GNN_CONFIGS)."""
+    return _case(kind, alg, c, W.GNN_CONFIGS[config]["layers"][0][0], gnn=config, **kw)
+
+
 def cases_for(p):
     out = []
     for alg, cs in REPLICATION[p].items():
@@ -105,10 +117,22 @@ def cases_for(p):
     out += [gt_case("gt_train", "15d_fusion1", 1, "table", lrs=[1e-2, 3e-2, 2e-2], clip=GT_CLIP),
             gt_case("gt_train", "15d_fusion1", 1, "wide_heads", lrs=[1e-2] * 3),
             gt_case("gt_link", "15d_fusion1", 1, "table", lrs=[1e-2, 2e-2, 1e-2])]
-    if p > 1:  # the layouts that split R have no row softmax, attention, GAT backward or graph transformer
+    # PNA, GIN and GINE: every configuration on the three layouts with full rows, the op on integers, and train steps
+    gnn_layouts = (("15d_fusion1", 1), ("15d_fusion1", c2), ("15d_fusion2", 1))
+    out += [gnn_case("gnn", alg, c, name) for name in W.GNN_CONFIGS for alg, c in gnn_layouts]
+    out += [gnn_case("gnn", "15d_fusion1", 1, "gin_table", train_eps=False)]
+    out += [_case("gine_int", alg, c, W.GINE_INT_WIDTH) for alg, c in gnn_layouts]
+    out += [gnn_case("gnn_train", "15d_fusion1", 1, name, task="node", steps=3, **kw)
+            for name, kw in (("pna_table", {}), ("gin_table", {}), ("gin_table", dict(train_eps=False)), ("gine_table", {}))]
+    out += [gnn_case("gnn_train", "15d_fusion1", 1, name, task="link", steps=3) for name in ("pna_table", "gine_table")]
+    out += [gnn_case("gnn_train", "15d_fusion1", 1, name, task="graph", pool=pool, steps=3)
+            for name in ("pna_table", "gin_table") for pool in gro.POOLS]
+    if p > 1:  # the layouts that split R have no row softmax, attention, GAT backward, graph transformer, PNA or GIN
         out += [dict(attn("15d_sparse", 1, 2, 64, "plain"), rejected=1),
                 dict(_case("gat", "15d_sparse", 1, 64, attention="softmax", layers=GAT_LAYERS), rejected=1),
                 dict(gt_case("gt", "15d_sparse", 1, "table"), rejected=1), dict(gt_case("gt", "15d_fusion2", 2, "odd"), rejected=1)]
+        out += [dict(gnn_case("gnn", alg, c, name), rejected=1) for name in ("pna_table", "gine_table")
+                for alg, c in (("15d_sparse", 1), ("15d_fusion2", 2))]
     return list({c["name"]: c for c in out}.values())  # at p = 1 the c = 2 cases fall onto their c = 1 twins
 
 
@@ -590,28 +614,229 @@ def check_gt_link(ranks, case, nproc):
     assert np.array_equal(np.sort(np.concatenate(seen)), np.sort(tr * N + tc)), name
 
 
+# ---- PNA, GIN and GINE ---------------------------------------------------------------------------------------------
+_GNN_REF = {}
+
+
+def gnn_problem(case):
+    """(rows, cols, N, cfg, params, X, G, oracle) of a PNA / GIN case; oracle: PNA's (aggregators, scalers, avg_lin,
+    avg_log) from the graph's own degree histogram, or GINE's per-entry attributes (None for GIN)."""
+    M, N, rows, cols = graph(case)
+    cfg = W.gnn_config(case)
+    params, X, G = W.gnn_inputs(N, cfg, case["seed"])
+    if cfg["model"] == "pna":
+        hist = np.bincount(np.bincount(rows, minlength=N))
+        oracle = (cfg["aggregators"], cfg["scalers"], *po.degree_averages(hist))
+    else:
+        oracle = go.attr_of(rows, cols, cfg["edge_dim"]) if cfg["edge_dim"] else None
+    return rows, cols, N, cfg, params, X, G, oracle
+
+
+def gnn_reference(case):
+    """The per-entry model's output, dX and parameter gradients, and its output on a pattern without entries (what the
+    rows without entries must give: PNA's post([x, 0..]) with d clamped to 1, GIN's MLP of (1 + eps) x)."""
+    if case["gnn"] not in _GNN_REF:
+        rows, cols, N, cfg, params, X, G, oracle = gnn_problem(case)
+        layers = cfg["layers"]
+        none = np.zeros(0, np.int64)
+        tp = [{k: po._t(v) for k, v in P.items()} for P in params]
+        if cfg["model"] == "pna":
+            Y, dX, dP = po.forward_backward(rows, cols, N, layers, params, X, G, *oracle)
+            alone = po.model_torch(none, none, N, layers, tp, po._t(X), *oracle)
+        else:
+            Y, dX, dP = go.forward_backward(rows, cols, N, layers, params, X, G, oracle)
+            attr = None if oracle is None else torch.zeros(0, cfg["edge_dim"], dtype=torch.float64)
+            alone = go.model_torch(none, none, N, layers, tp, go._t(X), attr)
+        _GNN_REF[case["gnn"]] = dict(Y=Y, dX=dX, dP=dP, alone=alone.numpy())
+    return _GNN_REF[case["gnn"]]
+
+
+def check_gnn_reach(ranks, case, nproc):
+    """More rows per rank than one reduction chunk, at p = 1 a hub row of more than 2000 entries, and at p = 4 with
+    c = 1 a rank without entries in one value order (rank 2's row block is the empty third one; see check_gt_reach):
+    under 15d_fusion2 that is the A order, so GINE's edge projection and its dW_e run on 0 rows there."""
+    tables = kernel_tables()
+    assert all(int(d["local_rows"]) > tables["min_chunk_rows"] for d in ranks), case["name"]
+    if nproc == 1:
+        assert int(ranks[0]["longest"]) > 2000, case["name"]
+    if nproc == 4 and case["c"] == 1:
+        empty, full = ("nA", "nB") if case["alg"] == "15d_fusion2" else ("nB", "nA")
+        assert int(ranks[2][empty]) == 0 < int(ranks[2][full]), (case["name"], [int(d["nA"]) for d in ranks])
+
+
+def check_gnn(ranks, case, nproc):
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    check_gnn_reach(ranks, case, nproc)
+    want = gnn_reference(case)
+    M, N, rows, _ = graph(case)
+    cfg = W.gnn_config(case)
+    for r, d in enumerate(ranks):
+        assert bool(d["repeat"]), (name, r)
+    Y = check_rows(ranks, name, "Y", want["Y"], "topA", "nrA")
+    check_rows(ranks, name, "dX", want["dX"], "topB", "nrB")
+    # the rows without entries (the empty third row block, every row % 9 == 4) take their own input alone
+    empty = np.bincount(rows, minlength=M) == 0
+    e0, e1 = landmarks(M, N)["empty_rows"]
+    assert empty[e0:e1].all() and empty[list(W.TIE_ROWS)].all()
+    scale = np.abs(want["Y"]).max()
+    assert np.abs(Y[empty] - want["alone"][empty]).max() <= 1e-10 * scale, name
+    assert np.abs(want["Y"][empty] - want["alone"][empty]).max() <= 1e-13 * scale
+    train_eps = case.get("train_eps", True)
+    for l, grads in enumerate(want["dP"]):
+        gscale = max(np.abs(g).max() for g in grads.values())
+        for k, g in grads.items():
+            key = f"g{l}_{k}"
+            for r, d in enumerate(ranks):
+                assert np.array_equal(d[key], ranks[0][key]), (name, r, key, "differs across ranks")
+            if k == "eps" and not train_eps:  # a constant: its gradient reads 0
+                assert not ranks[0][key].any(), (name, key)
+                continue
+            assert np.abs(g).max() > 0, (name, key)
+            assert grad_err(ranks[0][key], g, gscale) < 1e-10, (name, key, grad_err(ranks[0][key], g, gscale))
+    if cfg["model"] == "gin" and cfg["edge_dim"] and nproc == 4 and case["alg"] == "15d_fusion2" and case["c"] == 1:
+        # a rank without A-order entries adds nothing to dW_e; the all-reduced dW_e above matched the model
+        assert [int(d["nA"]) for d in ranks].count(0) >= 1, name
+
+
+def check_gine_int(ranks, case, nproc):
+    """edge_relu_aggregate on integers: A, dX and dE equal numpy exactly, on every rank; the copies of a duplicate get
+    bit-equal dE; X_v + E_i == 0 happens on the hub row (the strict mask decides those entries); rows without entries
+    give A = 0 and the untouched columns dX = 0."""
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    M, N, rows, cols = graph(case)
+    f = case["R"]
+    X, dA = W.gine_int_inputs(N, f, case["seed"])
+    E = go.edge_rows(rows, cols, f)
+    lm = landmarks(M, N)
+    hub = rows == lm["wide_hubs"][0]
+    assert ((X[cols] + E == 0) & hub[:, None]).sum() > 100
+    A = go.edge_relu_aggregate(rows, cols, M, X, E)
+    dX, dE = go.edge_relu_aggregate_backward(rows, cols, X, E, dA, N)
+    assert np.abs(A).max() < 2 ** 20 and np.abs(dX).max() < 2 ** 20  # integers: every partial sum is exact
+    for r, d in enumerate(ranks):
+        assert bool(d["repeat"]), (name, r)
+        for key, want, top, nr in (("A", A, "topA", "nrA"), ("dX", dX, "topB", "nrB")):
+            t, n = int(d[top]), min(int(d[nr]), len(want) - int(d[top]))
+            assert np.array_equal(d[key][:n], want[t:t + n]), (name, r, key)
+        assert np.array_equal(d["dE"], lookup(N, rows, cols, dE, d["rA"], d["cA"])), (name, r, "dE")
+    Ag, dXg = assemble(ranks, "A", "topA", "nrA", M), assemble(ranks, "dX", "topB", "nrB", N)
+    assert not Ag[np.bincount(rows, minlength=M) == 0].any() and not dXg[lm["empty_cols"][0]:lm["empty_cols"][1]].any()
+    keys = np.concatenate([d["rA"] * N + d["cA"] for d in ranks])
+    vals = np.concatenate([d["dE"] for d in ranks])
+    order = np.argsort(keys, kind="stable")
+    keys, vals = keys[order], vals[order]
+    same = np.flatnonzero(np.diff(keys) == 0)
+    assert len(same) >= 50 and np.array_equal(vals[same], vals[same + 1]), (name, "copies of a duplicate differ")
+
+
+_GNN_TRAIN_REF = {}
+
+
+def gnn_train_reference(case):
+    """(per-step results, trained parameters, trained head or None) of the per-entry model."""
+    key = (case["gnn"], case["task"], case.get("pool"), case.get("train_eps", True))
+    if key in _GNN_TRAIN_REF:
+        return _GNN_TRAIN_REF[key]
+    rows, cols, N, cfg, params, X, _, oracle = gnn_problem(case)
+    layers, steps = cfg["layers"], case["steps"]
+    pna, train_eps = cfg["model"] == "pna", case.get("train_eps", True)
+    head = None
+    if case["task"] == "node":
+        labels = W.labels_of(N, layers[-1][-1], case["seed"])
+        if pna:
+            res, trained = po.train(rows, cols, N, layers, params, X, oracle, labels, steps, lr=W.GNN_LR)
+        else:
+            res, trained = go.train(rows, cols, N, layers, params, X, labels, steps, attr=oracle, train_eps=train_eps, lr=W.GNN_LR)
+    elif case["task"] == "link":
+        pairs = W.link_pairs(N, case["seed"])
+        if pna:
+            res, trained = po.train_link(rows, cols, N, layers, params, X, oracle, pairs, steps, lr=W.GNN_LR)
+        else:
+            res, trained = go.train_link(rows, cols, N, layers, params, X, pairs, steps, attr=oracle, train_eps=train_eps, lr=W.GNN_LR)
+    else:
+        batch, G, labels = W.readout_batch(N, case["seed"])
+        tp = po._leaves(params) if pna else go._leaves(params, train_eps)
+        x = po._t(X)
+        if pna:
+            fwd = lambda _: po.model_torch(rows, cols, N, layers, tp, x, *oracle)  # noqa: E731
+            leaves = [v for P in tp for v in P.values()]
+        else:
+            attr = None if oracle is None else go._t(oracle)
+            fwd = lambda _: go.model_torch(rows, cols, N, layers, tp, x, attr)  # noqa: E731
+            leaves = go._trained(tp)
+        res, head = gro.train(fwd, leaves, batch, G, case["pool"], W.readout_head(layers[-1][-1], case["seed"]), labels, steps, lr=W.GNN_LR)
+        trained = [{k: v.detach().numpy().copy() for k, v in P.items()} for P in tp]
+    _GNN_TRAIN_REF[key] = (res, trained, head)
+    return _GNN_TRAIN_REF[key]
+
+
+def check_gnn_training(ranks, case, nproc):
+    """Three steps against the per-entry model with torch's AdamW: losses to 1e-10; gradient norms and trained
+    parameters to 1e-9, since Adam's g / (sqrt(v) + eps) amplifies the last bits of the earlier gradients (the graph
+    transformer's cases measured the fp64 model itself, its entries merely reordered, moving the third norm by 2.2e-10);
+    correct and labelled exactly; everything bit-identical across ranks."""
+    name = case["name"]
+    ranks = ranks_ok(ranks, name)
+    check_gnn_reach(ranks, case, nproc)
+    for r, d in enumerate(ranks):
+        for k in d:
+            if k not in REACH:
+                assert np.array_equal(d[k], ranks[0][k]), (name, r, k, "differs across ranks")
+    # the graph cases' batch (a graph over every row block with a hub row, a maximum on two ranks, an empty graph) is
+    # checked by tests/test_skewed_gnn_fixture.py
+    want, trained, head = gnn_train_reference(case)
+    steps = ranks[0]["steps"]
+    assert len(steps) == len(want) == case["steps"]
+    for t, w in enumerate(want):
+        assert abs(steps[t][0] - w[0]) <= 1e-10 * abs(w[0]) and abs(steps[t][3] - w[3]) <= 1e-9 * abs(w[3]), (name, t, steps[t], w)
+        assert (int(steps[t][1]), int(steps[t][2])) == (w[1], w[2]), (name, t, steps[t], w)
+    for l, P in enumerate(trained):
+        for k, w in P.items():
+            got = ranks[0][f"p{l}_{k}"]
+            assert np.abs(got - w).max() <= 1e-9 * max(np.abs(w).max(), 1.0), (name, l, k, np.abs(got - w).max())
+    if head is not None:
+        for k, w in zip(("weight", "bias"), head):
+            assert np.abs(ranks[0][f"head_{k}"] - w).max() <= 1e-9 * max(np.abs(w).max(), 1.0), (name, k)
+
+
 # ---- across rank counts --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("nproc", [2, 4])
 def test_results_do_not_depend_on_the_rank_count(nproc):
-    """Every attention, GAT and training case that also runs at p = 1: the assembled global result equals p = 1's to
-    1e-12 of its largest entry (the sums run in another order), +-inf exactly."""
+    """Every attention, GAT, graph transformer, PNA / GIN and training case that also runs at p = 1: the assembled global
+    result equals p = 1's to 1e-12 of its largest entry (the sums run in another order), +-inf exactly; trained
+    parameters to 1e-9; the integer GINE aggregation bit for bit."""
     one, many = results(1), results(nproc)
     checked = 0
     for case in CASES[nproc]:
         name = case["name"]
-        if name not in one or case["kind"] not in ("attn", "gat", "train", "gt", "gt_train", "gt_link") or case.get("rejected"):
+        if name not in one or case["kind"] not in ("attn", "gat", "train", "gt", "gt_train", "gt_link", "gnn", "gnn_train",
+                                                   "gine_int") or case.get("rejected"):
             continue
         a, b = ranks_ok(one[name], name), ranks_ok(many[name], name)
         M, N = W.sizes(case)
-        if case["kind"] == "gt":
+        if case["kind"] == "gine_int":  # integers: the same on any layout, bit for bit
+            for key, top, nr, total in (("A", "topA", "nrA", M), ("dX", "topB", "nrB", N)):
+                assert np.array_equal(assemble(b, key, top, nr, total), assemble(a, key, top, nr, total)), (name, nproc, key)
+            checked += 1
+            continue
+        if case["kind"] in ("gt", "gnn"):
             for key in ("Y", "dX"):
                 top, nr, total = ("topA", "nrA", M) if key == "Y" else ("topB", "nrB", N)
                 assert rel_err(assemble(b, key, top, nr, total), assemble(a, key, top, nr, total)) < 1e-12, (name, nproc, key)
-            for l in range(len(W.gt_config(case)["layers"])):
+            cfg = W.gt_config(case) if case["kind"] == "gt" else W.gnn_config(case)
+            for l in range(len(cfg["layers"])):
                 grads = {k: v for k, v in a[0].items() if k.startswith(f"g{l}_")}
-                scale = max(np.abs(g).max() for g in grads.values())  # key_bias: 0 up to rounding
+                scale = max(np.abs(g).max() for g in grads.values())  # key_bias, a constant eps: 0 (up to rounding)
                 for k, g in grads.items():
                     assert grad_err(b[0][k], g, scale) < 1e-12, (name, nproc, k)
+            checked += 1
+            continue
+        if case["kind"] == "gnn_train":
+            for k in a[0]:
+                if k == "steps" or k.startswith("p") or k.startswith("head_"):
+                    assert rel_err(b[0][k], a[0][k]) < 1e-9, (name, nproc, k)
             checked += 1
             continue
         if case["kind"] in ("gt_train", "gt_link"):
@@ -684,3 +909,18 @@ def test_graph_transformer_training_on_the_skewed_graph(nproc, case):
 @pytest.mark.parametrize("nproc,case", params("gt_link"))
 def test_graph_transformer_link_training_on_the_skewed_graph(nproc, case):
     check_gt_link(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gnn"))
+def test_pna_and_gin_on_the_skewed_graph(nproc, case):
+    check_gnn(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gine_int"))
+def test_gine_aggregation_on_integers_on_the_skewed_graph(nproc, case):
+    check_gine_int(results(nproc)[case["name"]], case, nproc)
+
+
+@pytest.mark.parametrize("nproc,case", params("gnn_train"))
+def test_pna_and_gin_training_on_the_skewed_graph(nproc, case):
+    check_gnn_training(results(nproc)[case["name"]], case, nproc)
