@@ -113,6 +113,12 @@ ABI = {
     "hnh_pair_sums_f64": (C.c_int, [_P, _P, _I64, _P, C.c_size_t, _P]),
     "hnh_link_bce_f64": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _I64, _P, _I64, C.c_int, C.c_double, _P, _I64, _P, _I64, _P, _P]),
     "hnh_link_target_check_f64": (C.c_int, [_P, _P, _I64, _P]),
+    "hnh_distmult_bce_f64": (C.c_int, [_P, _P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, C.c_int, C.c_double,
+                                       C.c_double, _P, _I64, _P, _I64, _P, _P, _P]),
+    "hnh_distmult_bce_grad_f64": (C.c_int, [_P, _P, _P, _I64, _I64, C.c_int, _P, _I64, _P, _I64, _P, _I64, C.c_int, C.c_double,
+                                            C.c_double, _P, _I64, _P]),
+    "hnh_distmult_relation_grad_f64": (C.c_int, [_P, _P, _P, _P, _I64, C.c_int, _P, _P, _P, _P, _I64, _P, _I64, C.c_int, _P, _P,
+                                                 _I64, _P]),
     "hnh_entry_coords_from_index_f64":(C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_max_aggregate_step_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, C.c_int, _P, _I64, _P, _I64, _P]),
     "hnh_max_aggregate_finish_f64": (C.c_int, [_P, _P, _I64, _P]),
@@ -316,6 +322,17 @@ ABI.update({
     "hnhd_alg_link_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     "hnhd_link_targets_create": (C.c_int, [_P, _P, _PP]),
     "hnhd_link_targets_destroy": (None, [_P]),
+    "hnhd_alg_distmult_loss": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_double, C.c_double, _P, _P, _P, _P, C.c_int, _P]),
+    "hnhd_distmult_create": (C.c_int, [_P, C.c_int, C.c_int, _PP]),
+    "hnhd_distmult_destroy": (None, [_P]),
+    "hnhd_distmult_param_shape": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hnhd_distmult_set_param": (C.c_int, [_P, C.c_char_p, _P]),
+    "hnhd_distmult_get_param": (C.c_int, [_P, C.c_char_p, _P]),
+    "hnhd_distmult_get_param_grad": (C.c_int, [_P, C.c_char_p, _P]),
+    "hnhd_relational_link_targets_create": (C.c_int, [_P, _P, _P, C.c_int, _PP]),
+    "hnhd_relational_link_targets_destroy": (None, [_P]),
+    "hnhd_model_relational_link_train_step": (C.c_int, [_P, _P, _P, _P, C.c_double, C.c_uint64, _P]),
+    "hnhd_model_relational_link_evaluate": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "hnhd_alg_max_aggregate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_alg_max_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int]),
     "hnhd_sage_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, _PP]),

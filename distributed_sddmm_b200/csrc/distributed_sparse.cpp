@@ -1088,6 +1088,152 @@ int64_t Distributed_Sparse::linkTargetCount() {
     return (int64_t)x[1];
 }
 
+// ---- relation-aware link prediction ------------------------------------------------------------------------------
+std::unique_ptr<RelationPlan> Distributed_Sparse::relationPlan(int num_relations) {
+    const string who = "relationPlan";
+    check_full_rows(who);
+    if (num_relations < 1) throw hnh::Error(HNH_E_INVALID, who + ": the relation count must be positive, got " + to_string(num_relations));
+    std::unique_ptr<RelationPlan> plan(new RelationPlan);
+    plan->owner = this;
+    plan->num_relations = num_relations;
+    SpmatLocal &m = *values_matrix(*this, k_sddmmA);
+    const int64_t keys_n = (int64_t)num_relations + 1;
+    for (size_t b = 0; b + 1 < m.blockStarts.size(); b++) {
+        const int64_t nb = (int64_t)m.blockStarts[b + 1] - (int64_t)m.blockStarts[b];
+        plan->blocks.emplace_back();
+        if (nb == 0) continue;
+        CSRLocal *blk = m.csr_blocks[b];
+        if (blk == nullptr || blk->num_coords != nb)
+            throw hnh::Error(HNH_E_INVALID, who + ": block " + to_string(b) + " does not match its value range");
+        if (nb >= INT32_MAX) throw hnh::Error(HNH_E_INVALID, who + ": " + to_string(nb) + " entries in one block; at most 2^31 - 2");
+        std::unique_ptr<RelationPlan::Block> p(new RelationPlan::Block);
+        hnh::DeviceBuffer<int32_t> keys((size_t)nb);
+        hnh::abi_check(hnh_relation_keys(keys.data(), blk->getActive()->values.data(), nb, num_relations, compute()), "relation_keys");
+        p->perm.resize((size_t)nb);
+        p->key_start.resize((size_t)keys_n + 1);
+        p->piece_first.resize((size_t)keys_n + 1);
+        const int64_t bound = hnh_edge_softmax_piece_bound(nb, keys_n);
+        if (bound < 0) hnh::abi_check((int)bound, "edge_softmax_piece_bound");
+        p->piece_key.resize((size_t)std::max<int64_t>(bound, 1));
+        hnh::abi_check(hnh_edge_softmax_plan(keys.data(), nb, keys_n, p->perm.data(), p->key_start.data(), p->piece_first.data(),
+                                             p->piece_key.data(), (int64_t)p->piece_key.size(), &p->pieces, compute()),
+                       "edge_softmax_plan");
+        blk->row_idx_device();  // the dD pass reads every entry's stored row
+        plan->blocks.back() = std::move(p);
+    }
+    return plan;
+}
+
+void Distributed_Sparse::distmultLoss(DenseMatrix &H_A, DenseMatrix &H_B, const DenseMatrix &D, int num_relations, double target,
+                                      double inv_count, DenseMatrix *dH_A, DenseMatrix *dH_B, DenseMatrix *dD, VectorXd *scores,
+                                      double *sums, bool accumulate, const RelationPlan *plan) {
+    const string who = "distmultLoss";
+    check_full_rows(who);
+    const int64_t r = H_A.cols();
+    if (H_A.rows() != localArows || H_B.rows() != localBrows || H_B.cols() != r || r < 1 || r > INT32_MAX)
+        throw hnh::Error(HNH_E_INVALID, who + ": H_A is " + to_string(H_A.rows()) + " x " + to_string(r) + " and H_B " +
+                                            to_string(H_B.rows()) + " x " + to_string(H_B.cols()) + "; like_A_matrix has " +
+                                            to_string(localArows) + " rows and like_B_matrix " + to_string(localBrows) +
+                                            ", both of one width");
+    if (num_relations < 1) throw hnh::Error(HNH_E_INVALID, who + ": the relation count must be positive, got " + to_string(num_relations));
+    for (auto [m, name] : {std::make_pair(&D, "D"), std::make_pair((const DenseMatrix *)dD, "dD")})
+        if (m && (m->rows() != num_relations || m->cols() != r))
+            throw hnh::Error(HNH_E_INVALID, who + ": " + name + " is " + to_string(m->rows()) + " x " + to_string(m->cols()) +
+                                                ", not num_relations x r = " + to_string(num_relations) + " x " + to_string(r));
+    using Grad = std::tuple<const DenseMatrix *, const DenseMatrix *, const char *>;
+    for (auto [g, h, name] : {Grad(dH_A, &H_A, "dH_A"), Grad(dH_B, &H_B, "dH_B"), Grad(dD, &D, "dD")}) {
+        if (g && (g == &H_A || g == &H_B || g == &D)) throw hnh::Error(HNH_E_INVALID, who + ": " + name + " may not be H_A, H_B or D");
+        if (g && (g->rows() != h->rows() || g->cols() != r))
+            throw hnh::Error(HNH_E_INVALID, who + ": " + name + " is " + to_string(g->rows()) + " x " + to_string(g->cols()) +
+                                                ", its input " + to_string(h->rows()) + " x " + to_string(r));
+    }
+    if (dD && (dD == dH_A || dD == dH_B)) throw hnh::Error(HNH_E_INVALID, who + ": dD may not be dH_A or dH_B");
+    if (scores && scores->size() != num_S_values())
+        throw hnh::Error(HNH_E_INVALID, who + ": the scores have " + to_string(scores->size()) + " entries, the A order " +
+                                            to_string(num_S_values()));
+    if (!(target >= 0.0 && target <= 1.0)) throw hnh::Error(HNH_E_INVALID, who + ": the target must lie in [0, 1]");
+    if (!(inv_count >= 0.0) || !std::isfinite(inv_count)) throw hnh::Error(HNH_E_INVALID, who + ": inv_count must be finite and >= 0");
+    if (sums == nullptr) throw hnh::Error(HNH_E_INVALID, who + ": null sums");
+    if (plan && (plan->owner != this || plan->num_relations != num_relations))
+        throw hnh::Error(HNH_E_INVALID, who + ": the relation plan was made for another object or relation count");
+    std::unique_ptr<RelationPlan> own;
+    if (dD && !plan) {
+        own = relationPlan(num_relations);
+        plan = own.get();
+    }
+    DenseMatrix stats(localArows, 2);
+    stats.setZero();
+    if (!accumulate) {
+        if (dH_A) dH_A->setZero();
+        if (dH_B && dH_B != dH_A) dH_B->setZero();
+    }
+    SpmatLocal &mA = *values_matrix(*this, k_sddmmA);
+    VectorXd g(dD ? std::max<int64_t>(num_S_values(), 1) : 0);
+    // one pass: the stored-row side is [H, its gradient (when wanted), the row statistics (A order only)]
+    auto pass = [&](KernelMode order, DenseMatrix &H, DenseMatrix *dH, DenseMatrix &G, DenseMatrix *st) {
+        const bool a_rows = order == k_sddmmA;
+        vector<PassOperand> rows{{&H, 0, r, false}}, gathered{{&G, 0, r, false}};
+        const int i_grad = dH ? (int)rows.size() : -1;
+        if (dH) rows.push_back({dH, 0, r, true});
+        const int i_stats = st ? (int)rows.size() : -1;
+        if (st) rows.push_back({st, 0, 2, true});
+        gather_pass(order, a_rows ? rows : gathered, a_rows ? gathered : rows,
+                    [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                        if (rows_are_A != a_rows)
+                            throw hnh::Error(HNH_E_INVALID, who + ": a block of this order does not hold the expected side as its rows");
+                        CSRHandle *h = blk.getActive();
+                        double *dR = i_grad >= 0 ? R[i_grad].p : nullptr;
+                        const int64_t lddr = i_grad >= 0 ? R[i_grad].ld : r;
+                        if (!a_rows) {
+                            hnh::abi_check(hnh_distmult_bce_grad_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(), blk.rows,
+                                                                     blk.num_coords, num_relations, R[0].p, R[0].ld, Y[0].p, Y[0].ld,
+                                                                     D.data(), r, (int)r, target, inv_count, dR, lddr, compute()),
+                                           "distmult_bce_grad");
+                            return;
+                        }
+                        const int64_t off = (int64_t)mA.blockStarts[(size_t)b];
+                        hnh::abi_check(hnh_distmult_bce_f64(h->rowStart.data(), h->col_idx.data(), h->values.data(), blk.rows,
+                                                            blk.num_coords, num_relations, R[0].p, R[0].ld, Y[0].p, Y[0].ld, D.data(), r,
+                                                            (int)r, target, inv_count, dR, lddr, i_stats >= 0 ? R[i_stats].p : nullptr,
+                                                            i_stats >= 0 ? R[i_stats].ld : 2, scores ? scores->data() + off : nullptr,
+                                                            dD ? g.data() + off : nullptr, compute()),
+                                       "distmult_bce");
+                    });
+    };
+    pass(k_sddmmA, H_A, dH_A, H_B, &stats);
+    if (dH_B) pass(k_sddmmB, H_B, dH_B, H_A, nullptr);
+    if (dD) {
+        // the relation-table gradient of this rank's entries, block by block in a fixed order, then over the world
+        DenseMatrix local(num_relations, r);
+        local.setZero();
+        VectorXd partial;
+        gather_pass(k_sddmmA, {{&H_A, 0, r, false}}, {{&H_B, 0, r, false}},
+                    [&](int b, CSRLocal &blk, bool rows_are_A, const PassView *R, const PassView *Y) {
+                        if (!rows_are_A) throw hnh::Error(HNH_E_INVALID, who + ": an A-order block does not hold H_A's rows");
+                        const RelationPlan::Block *p = (size_t)b < plan->blocks.size() ? plan->blocks[(size_t)b].get() : nullptr;
+                        if (p == nullptr) throw hnh::Error(HNH_E_INVALID, who + ": the relation plan has no block " + to_string(b));
+                        if (partial.size() < p->pieces * r) partial.resize(p->pieces * r);
+                        hnh::abi_check(hnh_distmult_relation_grad_f64(p->perm.data(), p->key_start.data(), p->piece_first.data(),
+                                                                      p->piece_key.data(), p->pieces, num_relations, blk.row_idx_device(),
+                                                                      blk.getActive()->col_idx.data(),
+                                                                      g.data() + (int64_t)mA.blockStarts[(size_t)b], R[0].p, R[0].ld,
+                                                                      Y[0].p, Y[0].ld, (int)r, partial.data(), local.data(), r,
+                                                                      compute()),
+                                       "distmult_relation_grad");
+                    });
+        allreduce_rows(local.data(), local.size(), false);
+        hnh::abi_check(hnh_row_axpy_f64(dD->data(), accumulate ? dD->data() : nullptr, 1.0, nullptr, local.data(), num_relations, (int)r,
+                                        compute()),
+                       "row_axpy");
+    }
+    const int64_t ws_bytes = hnh_pair_sums_workspace_bytes(localArows);
+    if (ws_bytes < 0) hnh::abi_check((int)ws_bytes, "pair_sums_workspace_bytes");
+    VectorXd ws(std::max<int64_t>(ws_bytes / 8, 1)), call(2);
+    hnh::abi_check(hnh_pair_sums_f64(call.data(), stats.data(), localArows, ws.data(), (size_t)ws_bytes, compute()), "pair_sums");
+    allreduce_rows(call.data(), 2, false);
+    hnh::abi_check(hnh_row_axpy_f64(sums, sums, 1.0, nullptr, call.data(), 1, 2, compute()), "row_axpy");
+}
+
 // ---- max aggregation -------------------------------------------------------------------------------------------------
 namespace {
 // the shape and aliasing checks of maxAggregate / maxAggregateBackward (every rank decides alike: shapes are local, but

@@ -11,6 +11,7 @@
 #include "hnh/25D_cannon_sparse.hpp"
 #include "hnh/als_conjugate_gradients.h"
 #include "hnh/benchmark_dist.hpp"
+#include "hnh/distmult.hpp"
 #include "hnh/distributed_sparse.h"
 #include "hnh/gat.hpp"
 #include "hnh/gin.hpp"
@@ -49,6 +50,12 @@ struct hnhd_adamw {
 };
 struct hnhd_link_targets {
     std::unique_ptr<hnh::LinkTargets> t;
+};
+struct hnhd_distmult {
+    std::unique_ptr<hnh::DistMultDecoder> d;
+};
+struct hnhd_relational_link_targets {
+    std::unique_ptr<hnh::RelationalLinkTargets> t;
 };
 struct hnhd_readout {
     std::unique_ptr<hnh::GraphReadout> r;
@@ -649,6 +656,72 @@ int hnhd_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T, hnhd_link_targets
 }
 void hnhd_link_targets_destroy(hnhd_link_targets_t *t) { delete t; }
 
+// ---- relation-aware link prediction ------------------------------------------------------------------------------
+int hnhd_alg_distmult_loss(hnhd_alg_t *T, hnhd_dense_t *H_A, hnhd_dense_t *H_B, hnhd_dense_t *D, int num_relations, double target,
+                           double inv_count, hnhd_dense_t *dH_A, hnhd_dense_t *dH_B, hnhd_dense_t *dD, hnhd_vec_t *scores,
+                           int accumulate, double out[2]) {
+    return guarded([&] {
+        if (!T || !H_A || !H_B || !D || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_alg_distmult_loss: null argument");
+        VectorXd sums(2);
+        sums.setZero();
+        T->alg->distmultLoss(H_A->m, H_B->m, D->m, num_relations, target, inv_count, dH_A ? &dH_A->m : nullptr,
+                             dH_B ? &dH_B->m : nullptr, dD ? &dD->m : nullptr, scores ? &scores->v : nullptr, sums.data(),
+                             accumulate != 0);
+        cudaStream_t s = hnh::Runtime::get().compute_stream();
+        hnh::cuda_check(cudaMemcpyAsync(out, sums.data(), 2 * sizeof(double), cudaMemcpyDeviceToHost, s), "distmult loss results");
+        hnh::cuda_check(cudaStreamSynchronize(s), "distmult loss results");
+    });
+}
+static ParamRef distmult_param(hnhd_distmult_t *d, const char *name) {
+    if (!d || !name) throw hnh::Error(HNH_E_INVALID, "DistMultDecoder: null argument");
+    return d->d->param(name);
+}
+int hnhd_distmult_create(hnhd_alg_t *model, int num_relations, int width, hnhd_distmult_t **out) {
+    return guarded([&] {
+        if (!model || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_distmult_create: null argument");
+        *out = new hnhd_distmult{std::make_unique<hnh::DistMultDecoder>(*model->alg, num_relations, width)};
+    });
+}
+void hnhd_distmult_destroy(hnhd_distmult_t *d) { delete d; }
+int hnhd_distmult_param_shape(hnhd_distmult_t *d, const char *name, int64_t *rows, int64_t *cols) {
+    return guarded([&] {
+        const ParamRef p = distmult_param(d, name);
+        if (rows) *rows = p.rows;
+        if (cols) *cols = p.cols;
+    });
+}
+int hnhd_distmult_set_param(hnhd_distmult_t *d, const char *name, const double *host) {
+    return guarded([&] {
+        const ParamRef p = distmult_param(d, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        sync_copy(p.value, host, p.rows * p.cols, cudaMemcpyHostToDevice);
+    });
+}
+int hnhd_distmult_get_param(hnhd_distmult_t *d, const char *name, double *host) {
+    return guarded([&] {
+        const ParamRef p = distmult_param(d, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        sync_copy(host, p.value, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_distmult_get_param_grad(hnhd_distmult_t *d, const char *name, double *host) {
+    return guarded([&] {
+        const ParamRef p = distmult_param(d, name);
+        if (!host) throw hnh::Error(HNH_E_INVALID, "null host pointer");
+        if (!p.grad) throw hnh::Error(HNH_E_INVALID, "DistMultDecoder: no relational train step has run");
+        sync_copy(host, p.grad, p.rows * p.cols, cudaMemcpyDeviceToHost);
+    });
+}
+int hnhd_relational_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T_pos, hnhd_alg_t *T_neg, int num_relations,
+                                        hnhd_relational_link_targets_t **out) {
+    return guarded([&] {
+        if (!model || !T_pos || !T_neg || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_relational_link_targets_create: null argument");
+        *out = new hnhd_relational_link_targets{
+            std::make_unique<hnh::RelationalLinkTargets>(*model->alg, *T_pos->alg, *T_neg->alg, num_relations)};
+    });
+}
+void hnhd_relational_link_targets_destroy(hnhd_relational_link_targets_t *t) { delete t; }
+
 // ---- max aggregation -------------------------------------------------------------------------------------------------
 int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C) {
     return guarded([&] {
@@ -903,6 +976,24 @@ int hnhd_model_link_evaluate(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd
     return guarded([&] {
         if (!m || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_link_evaluate: null argument");
         const hnh::LinkResult r = hnh::linkEvaluate(*m->m, *t->t, scores ? &scores->v : nullptr);
+        out[0] = r.loss;
+        out[1] = (double)r.correct;
+        out[2] = (double)r.count;
+    });
+}
+int hnhd_model_relational_link_train_step(hnhd_model_t *m, hnhd_distmult_t *d, const hnhd_relational_link_targets_t *t,
+                                          hnhd_adamw_t *opt, double dropout, uint64_t seed, double out[4]) {
+    return guarded([&] {
+        if (!m || !d || !t || !opt || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_relational_link_train_step: null argument");
+        train_out(hnh::relationalLinkTrainStep(*m->m, *t->t, *d->d, *opt->o, dropout, seed), out);
+    });
+}
+int hnhd_model_relational_link_evaluate(hnhd_model_t *m, hnhd_distmult_t *d, const hnhd_relational_link_targets_t *t,
+                                        hnhd_vec_t *scores_pos, hnhd_vec_t *scores_neg, double out[3]) {
+    return guarded([&] {
+        if (!m || !d || !t || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_model_relational_link_evaluate: null argument");
+        const hnh::LinkResult r = hnh::relationalLinkEvaluate(*m->m, *t->t, *d->d, scores_pos ? &scores_pos->v : nullptr,
+                                                              scores_neg ? &scores_neg->v : nullptr);
         out[0] = r.loss;
         out[1] = (double)r.correct;
         out[2] = (double)r.count;

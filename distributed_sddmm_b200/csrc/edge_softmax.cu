@@ -27,6 +27,7 @@ using hnh::set_error;
 
 constexpr int kCtasPerSm = 16;  // grid cap of every kernel here
 constexpr int kPiece = 1024;    // entries of a row that one warp reduces
+static_assert(kPiece == HNH_EDGE_PIECE, "the plan's piece size is public (distmult.cu walks plans)");
 
 // (m, s) <- the (max, sum of exp(x - max)) of the union of two sets; (-inf, 0) is the empty set
 __device__ __forceinline__ void ms_merge(double &m, double &s, double m2, double s2) {

@@ -456,6 +456,31 @@ class Algorithm:
                                        self._vec_arg(scores, "scores"), out), "link_loss")
         return float(out[0]), int(out[1]), int(out[2])
 
+    def distmult_loss(self, H_A: Dense, H_B: Dense, D: Dense, num_relations: int, target: float, inv_count: float,
+                      dH_A: Dense | None = None, dH_B: Dense | None = None, dD: Dense | None = None, scores: Vec | None = None,
+                      accumulate: bool = False):
+        """Relation-aware link prediction on this algorithm object's S, a target matrix T whose stored values are
+        relations in [0, num_relations) (collective; Distributed_Sparse::distmultLoss): s_uv = sum_k H_A[u, k] D[rho, k]
+        H_B[v, k] for every stored (u, v) of relation rho -- PyG's DistMult, (z[src] * rel_emb[edge_type] *
+        z[dst]).sum(-1) -- with H_A A-shaped, H_B B-shaped (one Dense may be both) and D the num_relations x r relation
+        table; an entry whose value is no relation contributes nothing.  Every entry's binary cross-entropy against
+        `target` (in [0, 1]) is weighted by inv_count.  Returns (loss sum, correct) of this call over all ranks.  dH_A,
+        dH_B, dD (optional) receive the gradients, overwritten or, with accumulate, added to (so a positive and a
+        negative call sum into one gradient); scores (optional, len(like_S_values())) receives s in the A order."""
+        for name, v in (("num_relations", num_relations),):
+            if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+                raise ValueError(f"{name} = {v!r} must be an integer")
+        for name, v in (("target", target), ("inv_count", inv_count)):
+            if isinstance(v, bool) or not isinstance(v, numbers.Real):
+                raise ValueError(f"{name} = {v!r} must be a number")
+        out = (C.c_double * 2)()
+        check(lib().hnhd_alg_distmult_loss(self.h, self._dense_arg(H_A, "H_A"), self._dense_arg(H_B, "H_B"),
+                                           self._dense_arg(D, "D"), int(num_relations), float(target), float(inv_count),
+                                           self._dense_arg(dH_A, "dH_A"), self._dense_arg(dH_B, "dH_B"),
+                                           self._dense_arg(dD, "dD"), self._vec_arg(scores, "scores"), int(bool(accumulate)),
+                                           out), "distmult_loss")
+        return float(out[0]), int(out[1])
+
     def max_aggregate(self, X: Dense, Z: Dense, C: Dense):
         """Collective: the SpMM over the (max, .) semiring (Distributed_Sparse::maxAggregate).  X is B-shaped, f wide;
         Z and C (A-shaped, f wide: Dense.create(localArows, f)) are overwritten with Z_u,k = max_v X_v,k over the stored
@@ -756,6 +781,31 @@ class _Model:
         self._check(lib().hnhd_model_link_evaluate(self.h, t, scores.h, out), "link_evaluate")
         return float(out[0]), int(out[1]), int(out[2]), scores.to_host()
 
+    def relational_link_train_step(self, decoder: "DistMultDecoder", targets: "RelationalLinkTargets",
+                                   opt: "AdamW") -> "TrainStep":
+        """One collective relational link-prediction step on the device: forward, the mean binary cross-entropy of the
+        DistMult scores of the output buffer over the pairs of the targets' T_pos (target 1) and T_neg (target 0),
+        backward, clipping and AdamW over the model's parameters and then the decoder's relation table.  Returns
+        TrainStep(loss, correct, labelled = the pair count, grad_norm)."""
+        return self._relational_link_train_step(decoder, targets, opt, 0.0, 0)
+
+    def _relational_link_train_step(self, decoder, targets, opt, dropout, seed):
+        p, sd = Algorithm._dropout_args(dropout, seed)
+        out = (C.c_double * 4)()
+        self._check(lib().hnhd_model_relational_link_train_step(self.h, _distmult_arg(decoder), _relational_targets_arg(targets),
+                                                                _adamw_arg(opt), p, sd, out), "relational_link_train_step")
+        return TrainStep._of(out)
+
+    def relational_link_evaluate(self, decoder: "DistMultDecoder", targets: "RelationalLinkTargets"):
+        """A forward pass without dropout and the relational link loss without gradients (collective): (loss, correct,
+        count, scores_pos, scores_neg), the scores numpy arrays in the orders of targets.alg_pos.entry_coordinates("A")
+        and targets.alg_neg.entry_coordinates("A") -- for MRR or Hits@K."""
+        d, t = _distmult_arg(decoder), _relational_targets_arg(targets)
+        out = (C.c_double * 3)()
+        sp, sn = Vec.create(0), Vec.create(0)
+        self._check(lib().hnhd_model_relational_link_evaluate(self.h, d, t, sp.h, sn.h, out), "relational_link_evaluate")
+        return float(out[0]), int(out[1]), int(out[2]), sp.to_host(), sn.to_host()
+
     def graph_train_step(self, readout: "GraphReadout", labels: "GraphLabels", opt: "AdamW") -> "TrainStep":
         """One collective graph-classification step on the device: forward, the readout's pool and head, the mean
         cross-entropy over the labelled graphs, backward, clipping and AdamW over the model's parameters and then the
@@ -981,6 +1031,13 @@ class GraphTransformer(_ModelByName):
         the dot-product scores <H_u, H_v> of the output buffer H over the entries of the targets' T, backward, clipping
         and AdamW.  Returns TrainStep(loss, correct, labelled = T's entry count, grad_norm)."""
         return self._link_train_step(targets, opt, dropout, seed)
+
+    def relational_link_train_step(self, decoder: "DistMultDecoder", targets: "RelationalLinkTargets", opt: "AdamW",
+                                   dropout: float = 0.0, seed: int = 0) -> "TrainStep":
+        """One collective relational link-prediction step on the device: forward(dropout, seed), the mean binary
+        cross-entropy of the DistMult scores over the targets' pairs, backward, clipping and AdamW over the model's
+        parameters and then the decoder's.  Returns TrainStep(loss, correct, labelled = the pair count, grad_norm)."""
+        return self._relational_link_train_step(decoder, targets, opt, dropout, seed)
 
     def graph_train_step(self, readout: "GraphReadout", labels: "GraphLabels", opt: "AdamW", dropout: float = 0.0,
                          seed: int = 0) -> "TrainStep":
@@ -1291,6 +1348,82 @@ class LinkTargets:
             pass
 
 
+class DistMultDecoder:
+    """The DistMult decoder of relational link prediction on the device (include/hnh/distmult.hpp): one relation table
+    "rel", num_relations x r with r the width of net's output, zero after construction -- the rel_emb of PyG's
+    examples/rgcn_link_pred.py, which maps onto it with no transpose.  net's algorithm object must outlive this one."""
+
+    PARAMS = ("rel",)
+
+    def __init__(self, net, num_relations: int):
+        if isinstance(num_relations, bool) or not isinstance(num_relations, numbers.Integral):
+            raise ValueError(f"num_relations = {num_relations!r} must be an integer")
+        if num_relations < 1:
+            raise ValueError(f"num_relations = {num_relations} must be positive")
+        self.net, self.num_relations = net, int(num_relations)
+        self.width = net.buffer_shape(len(net.layers))[1]
+        self.h = C.c_void_p()
+        check(lib().hnhd_distmult_create(net.alg.h, self.num_relations, self.width, C.byref(self.h)), "distmult_create")
+
+    def param_names(self):
+        return list(self.PARAMS)
+
+    def param_shape(self, name: str):
+        r, c = C.c_int64(), C.c_int64()
+        check(lib().hnhd_distmult_param_shape(self.h, name.encode(), C.byref(r), C.byref(c)), "distmult_param_shape")
+        return r.value, c.value
+
+    def set_param(self, name: str, value):
+        shape = self.param_shape(name)
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        if v.shape != shape:
+            raise ValueError(f"{name} is {shape}, got {v.shape}")
+        check(lib().hnhd_distmult_set_param(self.h, name.encode(), v.ctypes.data), "distmult_set_param")
+
+    def param(self, name: str):
+        out = np.empty(self.param_shape(name), dtype=np.float64)
+        check(lib().hnhd_distmult_get_param(self.h, name.encode(), out.ctypes.data), "distmult_get_param")
+        return out
+
+    def param_grad(self, name: str):
+        """dL/d param after a relational link train step (identical on every rank)."""
+        out = np.empty(self.param_shape(name), dtype=np.float64)
+        check(lib().hnhd_distmult_get_param_grad(self.h, name.encode(), out.ctypes.data), "distmult_get_param_grad")
+        return out
+
+    def __del__(self):
+        try:
+            lib().hnhd_distmult_destroy(self.h)
+        except Exception:
+            pass
+
+
+class RelationalLinkTargets:
+    """The relational link-prediction targets of a model, on the device: alg_pos and alg_neg are Algorithms over the
+    target matrices T_pos (target 1) and T_neg (target 0; it may have no entry), each built as LinkTargets' T, whose
+    stored values are the pairs' relations, integers in [0, num_relations) -- the edge_type of the example.  Duplicates
+    count, each under its own relation.  Fresh negatives every epoch are a new alg_neg and a new RelationalLinkTargets.
+    Collective: a T of another layout, a T that is not square, or a value that is no relation on any rank is refused
+    on every rank.  The three algorithm objects must outlive this one."""
+
+    def __init__(self, net, alg_pos: Algorithm, alg_neg: Algorithm, num_relations: int):
+        for name, a in (("alg_pos", alg_pos), ("alg_neg", alg_neg)):
+            if not isinstance(a, Algorithm):
+                raise TypeError(f"{name} must be an Algorithm, not {type(a).__name__}")
+        if isinstance(num_relations, bool) or not isinstance(num_relations, numbers.Integral):
+            raise ValueError(f"num_relations = {num_relations!r} must be an integer")
+        self.net, self.alg_pos, self.alg_neg, self.num_relations = net, alg_pos, alg_neg, int(num_relations)
+        self.h = C.c_void_p()
+        check(lib().hnhd_relational_link_targets_create(net.alg.h, alg_pos.h, alg_neg.h, self.num_relations, C.byref(self.h)),
+              "relational_link_targets_create")
+
+    def __del__(self):
+        try:
+            lib().hnhd_relational_link_targets_destroy(self.h)
+        except Exception:
+            pass
+
+
 class GraphReadout:
     """The readout of graph-level prediction on the device (include/hnh/graph_readout.hpp): pools the rows of net's
     output into one row per graph and, with num_classes, applies a torch.nn.Linear(r, num_classes) head.  batch: this
@@ -1422,6 +1555,18 @@ def _graph_labels_arg(labels):
 def _link_targets_arg(targets):
     if not isinstance(targets, LinkTargets):
         raise TypeError(f"targets must be a LinkTargets, not {type(targets).__name__}")
+    return targets.h
+
+
+def _distmult_arg(decoder):
+    if not isinstance(decoder, DistMultDecoder):
+        raise TypeError(f"decoder must be a DistMultDecoder, not {type(decoder).__name__}")
+    return decoder.h
+
+
+def _relational_targets_arg(targets):
+    if not isinstance(targets, RelationalLinkTargets):
+        raise TypeError(f"targets must be a RelationalLinkTargets, not {type(targets).__name__}")
     return targets.h
 
 

@@ -35,6 +35,22 @@ public:
     DenseSubmatrix(int tR, int lC, int rC, int cC) : topRow(tR), leftCol(lC), rowCount(rC), colCount(cC) {}
 };
 
+class Distributed_Sparse;
+
+// The entries of a value order grouped by relation, block by block: for block b with entries, an edge-softmax plan
+// (hnh_edge_softmax_plan) of its entries over R + 1 keys, key R holding the entries that are no relation.  Built by
+// Distributed_Sparse::relationPlan from the stored values as they are then; distmultLoss's relation-table gradient
+// walks it.
+struct RelationPlan {
+    struct Block {
+        hnh::DeviceBuffer<int32_t> perm, key_start, piece_first, piece_key;
+        int64_t pieces = 0;
+    };
+    const Distributed_Sparse *owner = nullptr;
+    int num_relations = 0;
+    vector<std::unique_ptr<Block>> blocks;  // null for a block without entries
+};
+
 class Distributed_Sparse {
 public:
     int proc_rank;  // global rank
@@ -303,6 +319,34 @@ public:
     // [0, 1] (link targets).  Collective: one world all-reduce of 2 doubles; a value elsewhere (NaN and infinities
     // included) on any rank is refused with HNH_E_INVALID on every rank.  Defined where check_full_rows passes.
     int64_t linkTargetCount();
+
+    // ---- relation-aware link prediction: the DistMult edge decoder with binary cross-entropy ---------------------------
+    // Called on the object of a target matrix T whose stored values are relations: the relation rho of a stored (u, v)
+    // is its value, an integer in [0, num_relations) as for relationalAggregate (an entry with any other value
+    // contributes nothing: no loss, no count, no gradient, score 0).  H_A (localArows x r) and H_B (localBrows x r) are
+    // the embeddings as for linkLoss, D (num_relations x r, the same on every rank) the relation table and `target` in
+    // [0, 1] the target of every entry of the call.  For every stored (u, v) of T (duplicates count, each under its own
+    // relation):
+    //     s_uv = sum_k H_A[u, k] D[rho, k] H_B[v, k],   l and g = (sigmoid(s) - target) inv_count as linkLoss,
+    // torch's (z[src] * rel_emb[edge_type] * z[dst]).sum(-1) and F.binary_cross_entropy_with_logits.  sums (device, 2
+    // doubles) += (sum l, the entries with (s > 0) == (target > 0.5)) over all ranks; dH_A (nullable) = sum_v g D[rho] o
+    // H_B[v], dH_B (nullable) = sum_u g D[rho] o H_A[u] (the sum of both when they are one matrix), dD (nullable,
+    // num_relations x r, the same on every rank) = sum over the entries of relation rho on all ranks of g H_A[u] o H_B[v];
+    // the gradients are overwritten or, with `accumulate`, added to, so calls for the positive and the negative
+    // targets sum into one gradient.  scores (nullable, an A-order vector: like_S_values) = s.  Passes: one gather_pass
+    // in the A order (scores, dH_A, the rows' loss and count, and every entry's g when dD is wanted), one in the B order
+    // only with dH_B, and for dD one more in the A order that walks `plan` (relationPlan(num_relations) of this object;
+    // null: built for the call), writes one r-wide partial per piece and sums each relation's pieces in plan order, then
+    // one world all-reduce of R r doubles.  The row statistics are summed in a fixed order and all-reduced (2 doubles).
+    // No atomics: repeated calls are bit-identical.  Collective; defined where check_full_rows passes.  HNH_E_INVALID on
+    // every rank before any launch for linkLoss's refusals, num_relations < 1, a D or dD that is not num_relations x r,
+    // a target outside [0, 1], a gradient that is H_A, H_B or D, or a plan of another object or relation count.
+    void distmultLoss(DenseMatrix &H_A, DenseMatrix &H_B, const DenseMatrix &D, int num_relations, double target, double inv_count,
+                      DenseMatrix *dH_A, DenseMatrix *dH_B, DenseMatrix *dD, VectorXd *scores, double *sums, bool accumulate,
+                      const RelationPlan *plan = nullptr);
+    // The A order's entries grouped by relation for distmultLoss (the relations as the stored values are now).
+    // No communication.  Defined where check_full_rows passes; HNH_E_INVALID for num_relations < 1.
+    std::unique_ptr<RelationPlan> relationPlan(int num_relations);
 
     // ---- max aggregation: the SpMM over the (max, .) semiring (GraphSAGE's max aggregator) ---------------------------
     // X (localBrows x f, the B-shaped operand: rows are S-columns v) is gathered over the stored entries (u, v) of S on

@@ -200,6 +200,28 @@ inline TrainResult trainStep(GraphModel &net, const NodeLabels &labels, AdamW &o
 }
 
 // ---- link prediction ----------------------------------------------------------------------------------------------
+namespace detail {
+inline int fusion(const Distributed_Sparse &d) {
+    const Sparse15D_Dense_Shift *ds = dynamic_cast<const Sparse15D_Dense_Shift *>(&d);
+    return ds ? ds->fusionApproach : 0;
+}
+// why a target matrix T's layout is not the model's ("" when it is): link targets (LinkTargets, and
+// RelationalLinkTargets in hnh/distmult.hpp) live in an algorithm object of the model's layout.  Global quantities
+// only, so every rank decides alike.
+inline string link_layout_mismatch(const Distributed_Sparse &m, const Distributed_Sparse &t) {
+    auto dims = [](const Distributed_Sparse &d) {
+        return std::to_string(d.p) + ", c = " + std::to_string(d.c) + ", " + std::to_string(d.M) + " x " + std::to_string(d.N) +
+               ", local rows " + std::to_string(d.localArows) + " / " + std::to_string(d.localBrows);
+    };
+    if (t.algorithm_name != m.algorithm_name || fusion(t) != fusion(m) || t.p != m.p || t.c != m.c || t.M != m.M || t.N != m.N ||
+        t.localArows != m.localArows || t.localBrows != m.localBrows)
+        return "T's layout (" + t.algorithm_name + ", fusion " + std::to_string(fusion(t)) + ", p = " + dims(t) +
+               ") is not the model's (" + m.algorithm_name + ", fusion " + std::to_string(fusion(m)) + ", p = " + dims(m) + ")";
+    if (t.M != t.N) return "T is " + std::to_string(t.M) + " x " + std::to_string(t.N) + "; link targets are square";
+    return "";
+}
+}  // namespace detail
+
 // The link targets of a model: T, a square sparse matrix over the model's nodes in its own algorithm object of the
 // model's layout (algorithm, fusion, p, c, M = N = the model's S dimensions, localArows, localBrows), so the dense row
 // partition is the model's.  T's stored values are the targets y_uv in [0, 1] (1 a positive pair, 0 a negative one,
@@ -218,7 +240,7 @@ public:
     double inv_count;  // 1 / count, 0 when T has no entry anywhere
 
     LinkTargets(const Distributed_Sparse &model_ops, Distributed_Sparse &T_ops) : model(&model_ops), T(&T_ops) {
-        const string why = mismatch(model_ops, T_ops);
+        const string why = detail::link_layout_mismatch(model_ops, T_ops);
         if (!why.empty()) throw Error(HNH_E_INVALID, "LinkTargets: " + why);
         count = T_ops.linkTargetCount();
         inv_count = count > 0 ? 1.0 / (double)count : 0.0;
@@ -229,25 +251,6 @@ public:
         if (dH) dH->resize(H.rows(), H.cols());
         if (scores) scores->resize(T->num_S_values());
         T->linkLoss(H, H, inv_count, dH, dH, scores, sums);
-    }
-
-private:
-    static int fusion(const Distributed_Sparse &d) {
-        const Sparse15D_Dense_Shift *ds = dynamic_cast<const Sparse15D_Dense_Shift *>(&d);
-        return ds ? ds->fusionApproach : 0;
-    }
-    // why T's layout is not the model's ("" when it is); global quantities only, so every rank decides alike
-    static string mismatch(const Distributed_Sparse &m, const Distributed_Sparse &t) {
-        auto dims = [](const Distributed_Sparse &d) {
-            return std::to_string(d.p) + ", c = " + std::to_string(d.c) + ", " + std::to_string(d.M) + " x " + std::to_string(d.N) +
-                   ", local rows " + std::to_string(d.localArows) + " / " + std::to_string(d.localBrows);
-        };
-        if (t.algorithm_name != m.algorithm_name || fusion(t) != fusion(m) || t.p != m.p || t.c != m.c || t.M != m.M ||
-            t.N != m.N || t.localArows != m.localArows || t.localBrows != m.localBrows)
-            return "T's layout (" + t.algorithm_name + ", fusion " + std::to_string(fusion(t)) + ", p = " + dims(t) +
-                   ") is not the model's (" + m.algorithm_name + ", fusion " + std::to_string(fusion(m)) + ", p = " + dims(m) + ")";
-        if (t.M != t.N) return "T is " + std::to_string(t.M) + " x " + std::to_string(t.N) + "; link targets are square";
-        return "";
     }
 };
 

@@ -187,6 +187,7 @@ int hnh_dgemm_nt_f64(double *C, const double *A, const double *B, int64_t m, int
  *
  * keys[i] = (int32) (idx[i] + offset): the global row of the entries of one CSR block from its stored row or
  * column index */
+#define HNH_EDGE_PIECE 1024 /* the most entries of one piece */
 int hnh_edge_keys_from_index(int32_t *keys, const int64_t *idx, int64_t n, int64_t offset, void *stream);
 /* out[i] = (double) (idx[i] + offset): the same as doubles, exact below 2^53 (Distributed_Sparse::entryCoordinates) */
 int hnh_entry_coords_from_index_f64(double *out, const int64_t *idx, int64_t n, int64_t offset, void *stream);
@@ -486,6 +487,38 @@ int hnh_link_bce_f64(const int64_t *rowStart, const int64_t *col_idx, const doub
                      int64_t lddx, double *stats, int64_t lds, double *scores, void *stream);
 /* bad[0] (device) += the number of target[0 .. n) that are not in [0, 1] (NaN and infinities count) */
 int hnh_link_target_check_f64(double *bad, const double *target, int64_t n, void *stream);
+
+/* ---- relation-aware link prediction (Distributed_Sparse::distmultLoss; csrc/distmult.cu) ----------------------------
+ * The DistMult edge decoder with binary cross-entropy on one CSR block.  values[i] is entry i's relation rho, an integer
+ * in [0, R) (any other value: the entry contributes nothing, and its score and g are 0); D (R x r, leading dimension
+ * ldd) is the relation table and `target` (in [0, 1]) the target of every entry of the call.  X is indexed by the stored
+ * row u, Y gathered by col_idx v.  Per entry:
+ *     s = sum_k X_u,k D_rho,k Y_v,k,  loss, correct and g = (sigmoid(s) - target) inv_count as hnh_link_bce_f64,
+ * hnh_distmult_bce_f64 (the A order) with the nullable outputs dX_u += sum_v g (D_rho o Y_v), stats[u * lds] += sum
+ * loss, stats[u * lds + 1] += sum correct (lds >= 2), scores[i] = s and g[i] = g; hnh_distmult_bce_grad_f64 (the B
+ * order: X is the B side) only dX_v += sum_u g (D_rho o Y_u).  Rows without entries are not touched.  r, R >= 1, every
+ * leading dimension >= r (the stats' >= 2), inv_count finite and >= 0; an output may not be an input or another output.
+ * Widths 4..256 (powers of two) with 16-byte aligned X, Y, D, dX and even leading dimensions take a row kernel with X_u
+ * in registers and 128-bit gathers, D with an L2 evict-last policy and the block's index and value streams with
+ * evict-first; others a one-warp-per-row kernel.  No atomics: repeated calls are bit-identical.
+ * hnh_distmult_relation_grad_f64: the relation-table gradient of one block from a plan of its entries keyed by relation
+ * (hnh_relation_keys over R + 1 keys, then hnh_edge_softmax_plan): num_pieces pieces, the key of piece q piece_key[q]
+ * (the plan's piece_row), and
+ *     dD[rho, :] += sum over the entries i of relation rho of g[i] (X[row_idx[i], :] o Y[col_idx[i], :])   (rho < R)
+ * with row_idx / col_idx the entries' stored rows and gathered rows.  Each piece's sum goes to row q of `partial`
+ * (num_pieces x r, contiguous), then the pieces of each relation are added in plan order: repeated calls are
+ * bit-identical. */
+int hnh_distmult_bce_f64(const int64_t *rowStart, const int64_t *col_idx, const double *values, int64_t rows, int64_t nnz, int R,
+                         const double *X, int64_t ldx, const double *Y, int64_t ldy, const double *D, int64_t ldd, int r,
+                         double target, double inv_count, double *dX, int64_t lddx, double *stats, int64_t lds, double *scores,
+                         double *g, void *stream);
+int hnh_distmult_bce_grad_f64(const int64_t *rowStart, const int64_t *col_idx, const double *values, int64_t rows, int64_t nnz,
+                              int R, const double *X, int64_t ldx, const double *Y, int64_t ldy, const double *D, int64_t ldd, int r,
+                              double target, double inv_count, double *dX, int64_t lddx, void *stream);
+int hnh_distmult_relation_grad_f64(const int32_t *perm, const int32_t *key_start, const int32_t *piece_first, const int32_t *piece_key,
+                                   int64_t num_pieces, int R, const int64_t *row_idx, const int64_t *col_idx, const double *g,
+                                   const double *X, int64_t ldx, const double *Y, int64_t ldy, int r, double *partial, double *dD,
+                                   int64_t ldd, void *stream);
 
 /* ---- max aggregation (Distributed_Sparse::maxAggregate; csrc/graph_sage.cu) ----------------------------------------
  * The SpMM over the (max, .) semiring on one CSR block, and its gradient.  S's values are not read; duplicates count.

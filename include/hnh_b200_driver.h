@@ -293,6 +293,37 @@ typedef struct hnhd_link_targets hnhd_link_targets_t;
 int hnhd_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T, hnhd_link_targets_t **out);
 void hnhd_link_targets_destroy(hnhd_link_targets_t *t);
 
+/* ---- relation-aware link prediction: a DistMult edge decoder (Distributed_Sparse::distmultLoss) --------------------
+ * On the algorithm object of a target matrix T whose stored values are relations in [0, num_relations) (any other value
+ * contributes nothing): s_uv = sum_k H_A[u, k] D[rho, k] H_B[v, k] for every stored (u, v) of relation rho, D the
+ * num_relations x r relation table (the same on every rank), and the binary cross-entropy of s against `target` in
+ * [0, 1], each entry weighted by inv_count.  out = {loss sum, correct} of this call over all ranks.  dH_A, dH_B, dD
+ * (nullable) receive the gradients of the weighted loss, overwritten or, with accumulate != 0, added to; scores (nullable,
+ * of hnhd_vec_like(T, 0) length) = s in the A order.  Collective; HNH_E_INVALID on every rank where hnhd_alg_link_loss
+ * is, for num_relations < 1, a D or dD that is not num_relations x r, a target outside [0, 1], and a gradient that is an
+ * input. */
+int hnhd_alg_distmult_loss(hnhd_alg_t *T, hnhd_dense_t *H_A, hnhd_dense_t *H_B, hnhd_dense_t *D, int num_relations, double target,
+                           double inv_count, hnhd_dense_t *dH_A, hnhd_dense_t *dH_B, hnhd_dense_t *dD, hnhd_vec_t *scores,
+                           int accumulate, double out[2]);
+/* The DistMult decoder of a model (hnh::DistMultDecoder, include/hnh/distmult.hpp): its relation table "rel"
+ * (num_relations x width, zero after creation; PyG's rel_emb with no transpose) and, after a relational train step, its
+ * gradient.  model: the model's algorithm object; width: the model's output width. */
+typedef struct hnhd_distmult hnhd_distmult_t;
+int hnhd_distmult_create(hnhd_alg_t *model, int num_relations, int width, hnhd_distmult_t **out);
+void hnhd_distmult_destroy(hnhd_distmult_t *d);
+int hnhd_distmult_param_shape(hnhd_distmult_t *d, const char *name, int64_t *rows, int64_t *cols);
+int hnhd_distmult_set_param(hnhd_distmult_t *d, const char *name, const double *host);
+int hnhd_distmult_get_param(hnhd_distmult_t *d, const char *name, double *host);
+int hnhd_distmult_get_param_grad(hnhd_distmult_t *d, const char *name, double *host);
+/* The relational link targets of a model (hnh::RelationalLinkTargets): T_pos (target 1) and T_neg (target 0; it may
+ * have no entry), each an algorithm object of the model's layout whose stored values are relations in [0,
+ * num_relations).  Collective; HNH_E_INVALID on every rank for another layout, a T that is not square, num_relations <
+ * 1 or a stored value that is no relation on any rank.  The three algorithm objects must outlive it. */
+typedef struct hnhd_relational_link_targets hnhd_relational_link_targets_t;
+int hnhd_relational_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T_pos, hnhd_alg_t *T_neg, int num_relations,
+                                        hnhd_relational_link_targets_t **out);
+void hnhd_relational_link_targets_destroy(hnhd_relational_link_targets_t *t);
+
 /* ---- max aggregation (Distributed_Sparse::maxAggregate) -------------------------------------------------------------
  * Z, C (A-shaped, f wide) = the per-column maximum of X (B-shaped) over the stored entries of each S-row and the number
  * of entries that attain it; Z = C = 0 on a row without entries.  The backward overwrites dX (or adds to it with
@@ -393,6 +424,18 @@ int hnhd_model_link_train_step(hnhd_model_t *m, const hnhd_link_targets_t *t, hn
 /* A forward pass without dropout and the link loss without gradients: out = {loss, correct, count}; scores (nullable)
  * is resized and receives s in the A order of T (hnhd_alg_entry_coordinates(T, 0, ..) gives the pairs).  Collective. */
 int hnhd_model_link_evaluate(hnhd_model_t *m, const hnhd_link_targets_t *t, hnhd_vec_t *scores, double out[3]);
+/* One relational link-prediction step (hnh::relationalLinkTrainStep): forward(dropout, seed), the mean binary
+ * cross-entropy of the DistMult scores over the pairs of T_pos and T_neg, the backward pass, clipping and AdamW over the
+ * model's parameters and then the decoder's.  out = {loss, correct, pair count, grad_norm}.  Collective; HNH_E_INVALID on
+ * every rank before any launch for targets or a decoder of another model's algorithm object, a decoder of another
+ * relation count or width, an optimizer of other parameter sizes, dropout on a model without it, and layouts without a
+ * backward pass. */
+int hnhd_model_relational_link_train_step(hnhd_model_t *m, hnhd_distmult_t *d, const hnhd_relational_link_targets_t *t,
+                                          hnhd_adamw_t *opt, double dropout, uint64_t seed, double out[4]);
+/* A forward pass without dropout and the relational link loss without gradients: out = {loss, correct, pair count};
+ * scores_pos / scores_neg (nullable) are resized and receive s in the A order of T_pos / T_neg.  Collective. */
+int hnhd_model_relational_link_evaluate(hnhd_model_t *m, hnhd_distmult_t *d, const hnhd_relational_link_targets_t *t,
+                                        hnhd_vec_t *scores_pos, hnhd_vec_t *scores_neg, double out[3]);
 void hnhd_model_destroy(hnhd_model_t *m);
 
 /* ---- graph-level prediction (include/hnh/graph_readout.hpp) ---------------------------------------------------------
