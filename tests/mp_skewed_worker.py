@@ -15,6 +15,12 @@ algorithm and runs the case's kind:
   gnn      PNA, GIN or GINE forward and backward (a configuration of GNN_CONFIGS)
   gnn_train  PNA, GIN or GINE node, link (the targets of link_pairs) or graph (readout_batch) train steps
   gine_int edge_relu_aggregate and its backward on integer inputs (exact results)
+  max_agg  max_aggregate and its backward on inputs with exact ties
+  distmult distmult_loss over T_pos = S (relations of distmult_relations) and T_neg (link_pairs), H_A = H_B
+  rel_link GraphSAGE or R-GCN relational link train steps with the DistMult decoder, then relational_link_evaluate
+
+GraphSAGE and R-GCN (SAGE_RGCN_CONFIGS) run as the gnn and gnn_train kinds.  S holds sval for base, the relations of
+s_relations for R-GCN, those of distmult_relations for distmult, and ones otherwise.
 
 Every op runs twice and the worker records whether the repeat gave the same bits.  It writes its rows of the results
 -- or the error the layout must raise -- to <outdir>/<case>_rank<r>.npz.
@@ -31,8 +37,11 @@ sys.path.insert(0, ROOT)
 
 from tests import gat_additive_oracle as gao  # noqa: E402
 from tests import gin_oracle as go  # noqa: E402
+from tests import graph_sage_oracle as gsa  # noqa: E402
 from tests import graph_transformer_block_oracle as gbo  # noqa: E402
 from tests import pna_oracle as po  # noqa: E402
+from tests import rgcn_basis_oracle as bo  # noqa: E402
+from tests import rgcn_oracle as ro  # noqa: E402
 from tests.mp_edge_softmax_worker import score, upstream  # noqa: E402
 from tests.mp_graph_transformer_worker import attr_of  # noqa: E402
 from tests.mp_sparse_attention_edge_worker import edge_of  # noqa: E402
@@ -460,7 +469,10 @@ GNN_LR = 1e-3  # the train cases: at 1e-2 the hub rows' sums make the losses gro
 
 
 def gnn_config(case):
-    cfg = dict(GNN_CONFIGS[case["gnn"]])
+    cfg = dict(GNN_CONFIGS[case["gnn"]] if case["gnn"] in GNN_CONFIGS else SAGE_RGCN_CONFIGS[case["gnn"]])
+    for k in ("aggr", "bases"):  # a case's own aggregation or basis count
+        if k in case:
+            cfg[k] = case[k]
     cfg["layers"] = [tuple(l) for l in cfg["layers"]]
     return cfg
 
@@ -483,6 +495,11 @@ def gnn_inputs(N, cfg, seed):
     rng = np.random.default_rng(seed + 37)
     if cfg["model"] == "pna":
         params = po.random_params(layers, len(cfg["aggregators"]), len(cfg["scalers"]), rng)
+    elif cfg["model"] == "sage":
+        params = gsa.random_params(layers, rng)
+    elif cfg["model"] == "rgcn":
+        params = bo.random_params(layers, NUM_RELATIONS, cfg["bases"], rng) if cfg.get("bases") else \
+            ro.random_params(layers, NUM_RELATIONS, rng)
     else:
         params = go.random_params(layers, cfg["edge_dim"], rng)
     X = rng.uniform(-1, 1, (N, layers[0][0]))
@@ -523,6 +540,10 @@ def _gnn(D, alg, case, N):
     layers = cfg["layers"]
     if cfg["model"] == "pna":
         net = D.PNA(alg, layers, aggregators=cfg["aggregators"], scalers=cfg["scalers"], deg=degree_histogram(N, case["seed"]))
+    elif cfg["model"] == "sage":
+        net = D.GraphSAGE(alg, layers, aggr=cfg["aggr"])
+    elif cfg["model"] == "rgcn":
+        net = D.RGCN(alg, layers, num_relations=NUM_RELATIONS, aggr=cfg["aggr"], num_bases=cfg.get("bases"))
     else:
         net = D.GIN(alg, layers, edge_dim=cfg["edge_dim"], eps=0.0, train_eps=case.get("train_eps", True))
     params, X, G = gnn_inputs(N, cfg, case["seed"])
@@ -607,6 +628,159 @@ def run_gnn_train(D, alg, case, M, N, out):
     _gnn_params(net, layers, out)
 
 
+# ---- GraphSAGE, R-GCN and DistMult ---------------------------------------------------------------------------------
+# Configurations as GNN_CONFIGS': GraphSAGE aggregates X (mean and sum with spmmA, max with maxAggregate), R-GCN X per
+# relation (relationalAggregate) or per basis (basisAggregate), each at its layer's input width.  "aggr" is the default
+# a case may override; the *_link configurations feed the DistMult decoder at their output width.
+SAGE_RGCN_CONFIGS = {
+    "sage_table": dict(model="sage", aggr="max", layers=[[64, 128], [128, 256], [256, 4]], reach=("table", "table", "table")),
+    "sage_wide": dict(model="sage", aggr="max", layers=[[300, 4]], reach=("windows",)),
+    "sage_odd": dict(model="sage", aggr="max", layers=[[7, 13], [13, 4]], reach=("generic", "generic")),
+    "rgcn_table": dict(model="rgcn", aggr="mean", layers=[[64, 128], [128, 256], [256, 4]], reach=("table", "table", "table")),
+    "rgcn_wide": dict(model="rgcn", aggr="mean", layers=[[300, 4]], reach=("windows",)),
+    "rgcn_odd": dict(model="rgcn", aggr="mean", layers=[[7, 13], [13, 4]], reach=("generic", "generic")),
+    "basis_table": dict(model="rgcn", aggr="mean", bases=3, layers=[[64, 128], [128, 256], [256, 4]],
+                        reach=("table", "table", "table")),
+    "basis_many": dict(model="rgcn", aggr="mean", bases=30, layers=[[64, 4]], reach=("table",)),  # more bases than registers
+    "rgcn_link": dict(model="rgcn", aggr="mean", layers=[[64, 128], [128, 64]], reach=("table", "table")),
+    "sage_link": dict(model="sage", aggr="max", layers=[[64, 128], [128, 256]], reach=("table", "table")),
+}
+# R-GCN's S and DistMult's targets declare one relation more than their relations use: relation 5 is carried by no entry
+NUM_RELATIONS, USED_RELATIONS = 6, 5
+MAX_AGG_WIDTHS = (64, 128, 256, 300, 7)
+DISTMULT_WIDTHS = (64, 128, 256, 7, 300)
+
+
+def copies(rows, cols, N):
+    """Per tuple, how many earlier copies of its pair the list holds."""
+    keys = np.asarray(rows, np.int64) * N + np.asarray(cols, np.int64)
+    o = np.argsort(keys, kind="stable")
+    ks = keys[o]
+    start = np.r_[0, np.flatnonzero(ks[1:] != ks[:-1]) + 1]
+    out = np.empty(len(ks), np.int64)
+    out[o] = np.arange(len(ks)) - np.repeat(start, np.diff(np.r_[start, len(ks)]))
+    return out
+
+
+def s_relations(rows, cols, N):
+    """R-GCN's relation of every tuple of S's global list (rgcn_oracle.hashed_relations: the copies of a duplicate
+    differ).  A rank takes its slice of these: hashed on the rank's own slice, a copy would lose its earlier copies."""
+    return ro.hashed_relations(rows, cols, N, USED_RELATIONS)
+
+
+def distmult_relations(rows, cols, N):
+    """DistMult's relation of every tuple of a target list: relation 0 for the wide hub rows and a third of the rest, so
+    that it spans more than 8 pieces of HNH_EDGE_PIECE at p = 1 and more than one on every rank at p = 4; the others
+    hashed over 1 .. 4; the k-th copy of a pair moves k relations on, so copies differ."""
+    rows, cols = np.asarray(rows, np.int64), np.asarray(cols, np.int64)
+    base = np.where(np.isin(rows, landmarks(N, N)["wide_hubs"]) | ((rows * 31 + cols * 17) % 3 == 0), 0,
+                    1 + (rows * 7 + cols * 3) % 4)
+    return ((base + copies(rows, cols, N)) % USED_RELATIONS).astype(np.float64)
+
+
+def distmult_targets(N, seed):
+    """(T_pos, T_neg) as (rows, cols, relations): the skewed graph's own tuples, and link_pairs' pairs."""
+    pr, pc = (x.astype(np.int64) for x in skewed_tuples(N, N, seed))
+    nr, nc, _ = link_pairs(N, seed)
+    return (pr, pc, distmult_relations(pr, pc, N)), (nr, nc, distmult_relations(nr, nc, N))
+
+
+def distmult_inputs(N, r, seed):
+    """(H, relation table) of the distmult case."""
+    rng = np.random.default_rng(seed + 53)
+    return rng.uniform(-1, 1, (N, r)), rng.uniform(-1, 1, (NUM_RELATIONS, r))
+
+
+def max_agg_inputs(N, f, seed):
+    """(X, dZ) of the max_agg case: X >= 0 with about half its entries exactly 0 (ties), rows TIE_ROWS equal."""
+    rng = np.random.default_rng(seed + 59)
+    X = np.maximum(rng.standard_normal((N, f)), 0.0)
+    X[TIE_ROWS[1]] = X[TIE_ROWS[0]]
+    return X, rng.standard_normal((N, f))
+
+
+def run_max_agg(D, alg, case, M, N, out):
+    """max_aggregate and its backward at width case["R"]."""
+    f = case["R"]
+    X, dZh = max_agg_inputs(N, f, case["seed"])
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    topB, _, nrB, _ = alg.submatrices("B")[0]
+    nA, nB = alg.like_A_matrix().shape[0], alg.like_B_matrix().shape[0]
+    Xd, Z, Cn, dZ, dX = (D.Dense.create(n, f) for n in (nB, nA, nA, nA, nB))
+    Xd.from_host(gather_local(X, [(topB, 0, nrB, f)], (nB, f)))
+    dZ.from_host(gather_local(dZh, [(topA, 0, nrA, f)], (nA, f)))
+    rA, _ = alg.entry_coordinates("A")
+    out.update(topA=topA, nrA=nrA, topB=topB, nrB=nrB, nA=len(rA),
+               longest=np.bincount(np.asarray(rA, np.int64)).max(initial=0) if len(rA) else 0)
+    got = []
+    for _ in range(2):
+        alg.max_aggregate(Xd, Z, Cn)
+        alg.max_aggregate_backward(Xd, Z, Cn, dZ, dX)
+        got.append(dict(Z=Z.to_host(), C=Cn.to_host(), dX=dX.to_host()))
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k]) for k in got[0])
+    out.update(got[0])
+
+
+def _rank_targets(D, case, N, trip, width):
+    """An Algorithm over this rank's round-robin share of the triples trip = (rows, cols, relations)."""
+    from distributed_sddmm_b200 import lib
+    rank, world = lib().hnhd_world_rank(), lib().hnhd_world_size()
+    sr, sc = rank_slice(trip[0].astype(np.uint64), trip[1].astype(np.uint64), rank, world)
+    return D.Algorithm(case["alg"], D.SpmatLocal.from_tuples(N, N, sr, sc, trip[2][rank::world].copy()), width, case["c"])
+
+
+def run_distmult(D, alg, case, M, N, out):
+    """distmult_loss at r = case["R"] with H_A = H_B: S is T_pos; a positive call and an accumulated negative call over
+    T_neg, twice."""
+    r = case["R"]
+    pos, neg = distmult_targets(N, case["seed"])
+    algN = _rank_targets(D, case, N, neg, r)
+    H, rel = distmult_inputs(N, r, case["seed"])
+    topA, _, nrA, _ = alg.submatrices("A")[0]
+    Hl = D.Dense.create(alg.like_A_matrix().shape[0], r)
+    Hl.from_host(gather_local(H, [(topA, 0, nrA, r)], Hl.shape))
+    Dd = D.Dense.create(NUM_RELATIONS, r)
+    Dd.from_host(rel)
+    dH, dD = D.Dense.create(*Hl.shape), D.Dense.create(NUM_RELATIONS, r)
+    sp, sn = alg.like_S_values(), algN.like_S_values()
+    inv = 1.0 / (len(pos[0]) + len(neg[0]))
+    erp, ecp = alg.entry_coordinates("A")
+    ern, ecn = algN.entry_coordinates("A")
+    out.update(topA=topA, nrA=nrA, nA=len(erp), erp=erp, ecp=ecp, ern=ern, ecn=ecn)
+    got = []
+    for _ in range(2):
+        res = [alg.distmult_loss(Hl, Hl, Dd, NUM_RELATIONS, 1.0, inv, dH, dH, dD, sp),
+               algN.distmult_loss(Hl, Hl, Dd, NUM_RELATIONS, 0.0, inv, dH, dH, dD, sn, accumulate=True)]
+        got.append(dict(res=np.array(res, np.float64), dH=dH.to_host(), dD=dD.to_host(), sp=sp.to_host(), sn=sn.to_host()))
+    out["repeat"] = all(np.array_equal(got[0][k], got[1][k]) for k in got[0])
+    out.update(got[0])
+    del algN
+
+
+def run_rel_link(D, alg, case, M, N, out):
+    """Relational link train steps of a GraphSAGE or R-GCN configuration with the DistMult decoder over
+    distmult_targets, then relational_link_evaluate."""
+    cfg, net, _, reach = _gnn(D, alg, case, N)
+    out.update(reach)
+    layers = cfg["layers"]
+    pos, neg = distmult_targets(N, case["seed"])
+    algP, algN = _rank_targets(D, case, N, pos, layers[0][0]), _rank_targets(D, case, N, neg, layers[0][0])
+    dec = D.DistMultDecoder(net, NUM_RELATIONS)
+    dec.set_param("rel", distmult_inputs(N, layers[-1][-1], case["seed"])[1])
+    t = D.RelationalLinkTargets(net, algP, algN, NUM_RELATIONS)
+    opt = D.AdamW(lr=GNN_LR)
+    out["steps"] = np.array([list(net.relational_link_train_step(dec, t, opt)) for _ in range(case["steps"])])
+    out["rel"], out["drel"] = dec.param("rel"), dec.param_grad("rel")
+    _gnn_params(net, layers, out)
+    loss, correct, count, sp, sn = net.relational_link_evaluate(dec, t)
+    out["evaluate"] = np.array([loss, correct, count])
+    out["sp"], out["sn"] = sp, sn
+    out["erp"], out["ecp"] = algP.entry_coordinates("A")
+    out["ern"], out["ecn"] = algN.entry_coordinates("A")
+    out["H"] = net.buffer(len(layers))
+    del t, dec, algP, algN
+
+
 def run_gine_int(D, alg, case, M, N, out):
     """edge_relu_aggregate and its backward on integer X, dA and E = gin_oracle.edge_rows: every partial sum is an
     integer far below 2^53, so the results are exact."""
@@ -636,7 +810,20 @@ def run_gine_int(D, alg, case, M, N, out):
 
 
 KINDS = dict(base=run_base, softmax=run_softmax, attn=run_attn, gat=run_gat, train=run_train, gt=run_gt, gt_train=run_gt_train,
-             gt_link=run_gt_link, gnn=run_gnn, gnn_train=run_gnn_train, gine_int=run_gine_int)
+             gt_link=run_gt_link, gnn=run_gnn, gnn_train=run_gnn_train, gine_int=run_gine_int, max_agg=run_max_agg,
+             distmult=run_distmult, rel_link=run_rel_link)
+
+
+def s_values(case, rows, cols, tr, tc, rank, world):
+    """The values of this rank's tuples tr, tc: slices of what the global list rows, cols defines."""
+    N = sizes(case)[1]
+    if case["kind"] == "base":
+        return sval(tr, tc)
+    if case["kind"] == "distmult":
+        return distmult_relations(rows, cols, N)[rank::world].copy()
+    if case.get("gnn") and gnn_config(case)["model"] == "rgcn":
+        return s_relations(rows, cols, N)[rank::world].copy()
+    return np.ones(len(tr))
 
 
 def run_case(D, case, rank, world):
@@ -644,7 +831,7 @@ def run_case(D, case, rank, world):
     M, N = sizes(case)
     rows, cols = skewed_tuples(M, N, case["seed"])
     tr, tc = rank_slice(rows, cols, rank, world)
-    S = D.SpmatLocal.from_tuples(M, N, tr, tc, sval(tr, tc) if case["kind"] == "base" else np.ones(len(tr)))
+    S = D.SpmatLocal.from_tuples(M, N, tr, tc, s_values(case, rows, cols, tr, tc, rank, world))
     alg = D.Algorithm(case["alg"], S, case["R"], case["c"])
     out = {}
     try:

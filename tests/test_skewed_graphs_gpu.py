@@ -1,7 +1,8 @@
 """The skewed graph of tests/skewed_graph.py on one rank, in-process: the op table of
 tests/test_skewed_graphs_multirank_gpu.py (its cases, worker code and checks) on all five algorithms and on the
 rectangular variants, every graph transformer configuration (and its refusal of the rectangular sizes), every PNA / GIN
-configuration and GINE's integer edge-ReLU aggregation on all five algorithms, and the
+configuration and GINE's integer edge-ReLU aggregation on all five algorithms, every GraphSAGE and R-GCN configuration
+and max_aggregate and distmult_loss at every width of the multi-rank cases on all five algorithms, and the
 kernel-level entry points fed one skewed block directly -- the sparse-attention step, finish, grad_q and grad_kv kernels
 on the block and on its transpose (where the hub column is one very long row), and the edge-softmax plan, statistics,
 apply and backward kernels keyed by row and by column -- so that a failure on several ranks can be told apart from a
@@ -44,7 +45,7 @@ def _cases(alg, i):
 
 
 CHECKS = dict(base=T.check_base, softmax=T.check_softmax, attn=T.check_attention, gat=T.check_gat, train=T.check_training,
-              gt=T.check_gt, gnn=T.check_gnn, gine_int=T.check_gine_int)
+              gt=T.check_gt, gnn=T.check_gnn, gine_int=T.check_gine_int, max_agg=T.check_max_agg, distmult=T.check_distmult)
 P1 = [c for i, alg in enumerate(ALGS) for c in _cases(alg, i)]
 P1 += [T._case("train", "25d_dense_replicate", 1, 64, attention="additive", layers=T.GAT_LAYERS, steps=3)]
 # the graph transformer: every configuration on 15d_fusion1, the two with edge features on every algorithm
@@ -53,6 +54,10 @@ P1 += [T.gt_case("gt", "15d_fusion1", 1, name) for name in ("wide_heads", "ln_ba
 # PNA, GIN and GINE: every configuration and the integer op on every algorithm
 P1 += [T.gnn_case("gnn", alg, 1, name) for name in W.GNN_CONFIGS for alg in ALGS]
 P1 += [T._case("gine_int", alg, 1, W.GINE_INT_WIDTH) for alg in ALGS]
+# GraphSAGE and R-GCN: every configuration and aggregation; max_aggregate and distmult_loss at every width; on every algorithm
+P1 += [T.gnn_case("gnn", alg, 1, name, **kw) for name, kw in T.SAGE_RGCN_TABLE + T.SAGE_RGCN_OTHER for alg in ALGS]
+P1 += [T._case(kind, alg, 1, f) for kind, widths in (("max_agg", W.MAX_AGG_WIDTHS), ("distmult", W.DISTMULT_WIDTHS))
+       for f in widths for alg in ALGS]
 RECT = [dict(c, m=M, n=N) for k, (M, N) in enumerate(RECTANGULAR)
         for c in (T._case("base", ALGS[k], 1, 128, script=T.ALL_OPS), T._case("softmax", ALGS[k + 2], 1, 8, mask=1),
                   _attn(ALGS[k + 3], 2, 64, "bias", 0.4), _attn(ALGS[k], 1, 128, "edge"))]
