@@ -119,6 +119,9 @@ ABI = {
                                             C.c_double, _P, _I64, _P]),
     "hnh_distmult_relation_grad_f64": (C.c_int, [_P, _P, _P, _P, _I64, C.c_int, _P, _P, _P, _P, _I64, _P, _I64, C.c_int, _P, _P,
                                                  _I64, _P]),
+    "hnh_rank_count_f64": (C.c_int, [_P, _I64, _I64, _P, _I64, _I64, C.c_int, _P, _P, _P, _P]),
+    "hnh_rank_queries_f64": (C.c_int, [_P, _I64, _I64, _P, _I64, _I64, _I64, _P, _P, _P, _I64, C.c_int, C.c_int, _P]),
+    "hnh_rank_pairs_f64": (C.c_int, [_P, _I64, _I64, _P, _I64, _I64, C.c_int, _P, _P, _I64, _P, _P, _P, _P, _P]),
     "hnh_entry_coords_from_index_f64":(C.c_int, [_P, _P, _I64, _I64, _P]),
     "hnh_max_aggregate_step_f64": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, C.c_int, _P, _I64, _P, _I64, _P]),
     "hnh_max_aggregate_finish_f64": (C.c_int, [_P, _P, _I64, _P]),
@@ -333,6 +336,9 @@ ABI.update({
     "hnhd_relational_link_targets_destroy": (None, [_P]),
     "hnhd_model_relational_link_train_step": (C.c_int, [_P, _P, _P, _P, C.c_double, C.c_uint64, _P]),
     "hnhd_model_relational_link_evaluate": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "hnhd_link_ranking_create": (C.c_int, [_P, _P, _P, _P, _I64, C.c_int, _PP]),
+    "hnhd_link_ranking_destroy": (None, [_P]),
+    "hnhd_model_link_rank": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _P, _P, C.POINTER(C.c_double)]),
     "hnhd_alg_max_aggregate": (C.c_int, [_P, _P, _P, _P]),
     "hnhd_alg_max_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int]),
     "hnhd_sage_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.c_char_p, _PP]),

@@ -18,6 +18,7 @@
 #include "hnh/graph_readout.hpp"
 #include "hnh/graph_sage.hpp"
 #include "hnh/graph_transformer.hpp"
+#include "hnh/link_ranking.hpp"
 #include "hnh/pna.hpp"
 #include "hnh/rgcn.hpp"
 #include "hnh/training.hpp"
@@ -56,6 +57,9 @@ struct hnhd_distmult {
 };
 struct hnhd_relational_link_targets {
     std::unique_ptr<hnh::RelationalLinkTargets> t;
+};
+struct hnhd_link_ranking {
+    std::unique_ptr<hnh::LinkRanking> r;
 };
 struct hnhd_readout {
     std::unique_ptr<hnh::GraphReadout> r;
@@ -721,6 +725,14 @@ int hnhd_relational_link_targets_create(hnhd_alg_t *model, hnhd_alg_t *T_pos, hn
     });
 }
 void hnhd_relational_link_targets_destroy(hnhd_relational_link_targets_t *t) { delete t; }
+int hnhd_link_ranking_create(hnhd_alg_t *model, const int64_t *heads, const int64_t *rels, const int64_t *tails, int64_t n,
+                             int num_relations, hnhd_link_ranking_t **out) {
+    return guarded([&] {
+        if (!model || !out) throw hnh::Error(HNH_E_INVALID, "hnhd_link_ranking_create: null argument");
+        *out = new hnhd_link_ranking{std::make_unique<hnh::LinkRanking>(*model->alg, heads, rels, tails, n, num_relations)};
+    });
+}
+void hnhd_link_ranking_destroy(hnhd_link_ranking_t *r) { delete r; }
 
 // ---- max aggregation -------------------------------------------------------------------------------------------------
 int hnhd_alg_max_aggregate(hnhd_alg_t *a, hnhd_dense_t *X, hnhd_dense_t *Z, hnhd_dense_t *C) {
@@ -997,6 +1009,13 @@ int hnhd_model_relational_link_evaluate(hnhd_model_t *m, hnhd_distmult_t *d, con
         out[0] = r.loss;
         out[1] = (double)r.correct;
         out[2] = (double)r.count;
+    });
+}
+int hnhd_model_link_rank(hnhd_model_t *m, const hnhd_link_ranking_t *ranking, hnhd_distmult_t *d, const int64_t *heads,
+                         const int64_t *rels, const int64_t *tails, int64_t n_q, double *tail_ranks, double *head_ranks, double *mrr) {
+    return guarded([&] {
+        if (!m || !ranking || !mrr) throw hnh::Error(HNH_E_INVALID, "hnhd_model_link_rank: null argument");
+        *mrr = hnh::linkRank(*m->m, *ranking->r, d ? d->d.get() : nullptr, heads, rels, tails, n_q, tail_ranks, head_ranks);
     });
 }
 void hnhd_model_destroy(hnhd_model_t *m) { delete m; }

@@ -9,6 +9,7 @@
 // The backward pass (GAT::backwardPass) adds the two other products of a projection on the same DMMA tiling --
 // dW = X^T dP (dgemm_tn_kernel, split over the long k and reduced in a fixed order) and dX += dP W^T
 // (dgemm_nt_kernel) -- and the derivatives of the two activations.
+#include "dmma.cuh"
 #include "launch.h"
 
 namespace {
@@ -48,12 +49,6 @@ __global__ void relu_cols_kernel(double *__restrict__ dst, int64_t ld_dst, int64
 // the 16 lanes of a half-warp on 16 different bank pairs for both fragment loads.  Edges are zero-filled on load and
 // masked on store, so any m, n, k >= 1 works.
 constexpr int GM = 64, GN = 64, GK = 16, GA_LD = GK + 4, GB_LD = GN + 4;
-
-__device__ __forceinline__ void dmma_8x8x4(double &c0, double &c1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                 : "+d"(c0), "+d"(c1)
-                 : "d"(a), "d"(b));
-}
 
 __global__ void __launch_bounds__(128)
 dgemm_dmma_kernel(double *__restrict__ C, const double *__restrict__ A, const double *__restrict__ B, int64_t m, int n, int k) {

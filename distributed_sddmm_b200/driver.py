@@ -806,6 +806,23 @@ class _Model:
         self._check(lib().hnhd_model_relational_link_evaluate(self.h, d, t, sp.h, sn.h, out), "relational_link_evaluate")
         return float(out[0]), int(out[1]), int(out[2]), sp.to_host(), sn.to_host()
 
+    def link_rank(self, ranking: "LinkRanking", queries, decoder: "DistMultDecoder" = None) -> "LinkRanks":
+        """Filtered link ranking (collective; include/hnh/link_ranking.hpp): a forward pass without dropout, then the
+        rank of each query triple's true tail among every corrupted tail and of its true head among every corrupted
+        head, the ranking's known triples filtered out, by the DistMult scores of decoder -- or by dot products with
+        decoder=None, which needs a ranking of one relation.  queries = (heads, rels, tails), the same on every rank.
+        A rank is ((gt + 1) + (ge + 1)) / 2 over the candidates scoring above / at least the true one.  Returns
+        LinkRanks(mrr, tail_ranks, head_ranks), the same on every rank; .hits_at(k) gives Hits@K."""
+        if not isinstance(ranking, LinkRanking):
+            raise TypeError(f"ranking must be a LinkRanking, not {type(ranking).__name__}")
+        h, r, t = _triples(queries, "queries")
+        tr, hr = np.empty(len(h), np.float64), np.empty(len(h), np.float64)
+        mrr = C.c_double()
+        self._check(lib().hnhd_model_link_rank(self.h, ranking.h, _distmult_arg(decoder) if decoder is not None else None,
+                                               h.ctypes.data, r.ctypes.data, t.ctypes.data, len(h), tr.ctypes.data,
+                                               hr.ctypes.data, C.byref(mrr)), "link_rank")
+        return LinkRanks(mrr.value, tr, hr)
+
     def graph_train_step(self, readout: "GraphReadout", labels: "GraphLabels", opt: "AdamW") -> "TrainStep":
         """One collective graph-classification step on the device: forward, the readout's pool and head, the mean
         cross-entropy over the labelled graphs, backward, clipping and AdamW over the model's parameters and then the
@@ -1422,6 +1439,53 @@ class RelationalLinkTargets:
             lib().hnhd_relational_link_targets_destroy(self.h)
         except Exception:
             pass
+
+
+def _triples(triples, what):
+    """(heads, rels, tails) as three equally long contiguous int64 arrays."""
+    try:
+        h, r, t = (np.ascontiguousarray(np.asarray(x).reshape(-1), dtype=np.int64) for x in triples)
+    except (TypeError, ValueError) as e:
+        raise ValueError(f"{what} must be (heads, rels, tails): {e}") from None
+    if not len(h) == len(r) == len(t):
+        raise ValueError(f"{what}: heads, rels and tails have {len(h)}, {len(r)} and {len(t)} entries")
+    return h, r, t
+
+
+class LinkRanking:
+    """The filter of filtered link ranking on the device's host side (include/hnh/link_ranking.hpp): the known triples
+    filter_triples = (heads, rels, tails) of net's nodes, the example's train + valid + test, indexed once by (head,
+    relation) and (tail, relation).  Relations lie in [0, num_relations); dot-product ranking (no decoder) uses one
+    relation, 0.  Collective: a node outside [0, M), a relation out of range, a layout without full rows, or triples
+    that differ between ranks is refused on every rank.  net's algorithm object must outlive this one."""
+
+    def __init__(self, net, filter_triples, num_relations: int = 1):
+        if isinstance(num_relations, bool) or not isinstance(num_relations, numbers.Integral):
+            raise ValueError(f"num_relations = {num_relations!r} must be an integer")
+        self.net, self.num_relations = net, int(num_relations)
+        h, r, t = _triples(filter_triples, "filter_triples")
+        self.count = len(h)
+        self.h = C.c_void_p()
+        check(lib().hnhd_link_ranking_create(net.alg.h, h.ctypes.data, r.ctypes.data, t.ctypes.data, len(h), self.num_relations,
+                                             C.byref(self.h)), "link_ranking_create")
+
+    def __del__(self):
+        try:
+            lib().hnhd_link_ranking_destroy(self.h)
+        except Exception:
+            pass
+
+
+class LinkRanks(NamedTuple):
+    """What link_rank reports: the MRR over all 2 n_q ranks and the tail and head rank of each query."""
+    mrr: float
+    tail_ranks: np.ndarray
+    head_ranks: np.ndarray
+
+    def hits_at(self, k) -> float:
+        """The share of the 2 n_q ranks that are <= k (0 for no query)."""
+        n = len(self.tail_ranks) + len(self.head_ranks)
+        return float(((self.tail_ranks <= k).sum() + (self.head_ranks <= k).sum()) / n) if n else 0.0
 
 
 class GraphReadout:

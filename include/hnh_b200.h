@@ -520,6 +520,28 @@ int hnh_distmult_relation_grad_f64(const int32_t *perm, const int32_t *key_start
                                    const double *X, int64_t ldx, const double *Y, int64_t ldy, int r, double *partial, double *dD,
                                    int64_t ldd, void *stream);
 
+/* ---- filtered link ranking (include/hnh/link_ranking.hpp; csrc/link_ranking.cu) ----------------------------------
+ * Z is `rows` x r (leading dimension ldz): the rows that are ranking candidates; Q is n_q x r (ldq): one query vector
+ * per row; scores are s(u, q) = sum_k Z_u,k Q_q,k.  r >= 1 and every leading dimension >= r; ids are 0-based.
+ * hnh_rank_count_f64: gt[q] += #{u < rows : s(u, q) > s_true[q]} and ge[q] += #{u < rows : s(u, q) >= s_true[q]}, for
+ *     every q < n_q, in 64-bit integers (gt and ge separate arrays).  The n_q x rows scores are compared where they are
+ *     computed and never stored.  fp64 DMMA (mma.sync m8n8k4) in 64 x 64 tiles with K in steps of 16; integer atomics,
+ *     so repeated calls are bit-identical.
+ * hnh_rank_queries_f64: Q[q, :] = Z[anchors[q] - row0, :] o D[rels[q], :] for the anchors in [row0, row0 + rows) (Z's
+ *     row alone when D is null), and 0 for every other anchor and for a relation outside [0, R) (D: R x r, ldd).
+ * hnh_rank_pairs_f64: for the pairs p < n_pairs, s = s(pair_row[p], pair_q[p]) with hnh_rank_count_f64's arithmetic,
+ *     bit for bit: the same instruction, k steps and zero padding, at the count kernel's fragment position.  Nullable
+ *     outputs: scores[p] = s; with gt, ge and s_true, gt[q] -= (s > s_true[q]) and ge[q] -= (s >= s_true[q]), which
+ *     takes a pair the count kernel counted back out exactly.  Pairs with q outside [0, n_q) or a row outside
+ *     [0, rows) are skipped. */
+int hnh_rank_count_f64(const double *Z, int64_t ldz, int64_t rows, const double *Q, int64_t ldq, int64_t n_q, int r,
+                       const double *s_true, int64_t *gt, int64_t *ge, void *stream);
+int hnh_rank_queries_f64(double *Q, int64_t ldq, int64_t n_q, const double *Z, int64_t ldz, int64_t row0, int64_t rows,
+                         const int64_t *anchors, const int64_t *rels, const double *D, int64_t ldd, int R, int r, void *stream);
+int hnh_rank_pairs_f64(const double *Z, int64_t ldz, int64_t rows, const double *Q, int64_t ldq, int64_t n_q, int r,
+                       const int64_t *pair_q, const int64_t *pair_row, int64_t n_pairs, double *scores, const double *s_true,
+                       int64_t *gt, int64_t *ge, void *stream);
+
 /* ---- max aggregation (Distributed_Sparse::maxAggregate; csrc/graph_sage.cu) ----------------------------------------
  * The SpMM over the (max, .) semiring on one CSR block, and its gradient.  S's values are not read; duplicates count.
  * hnh_max_aggregate_step_f64: for every stored row u, over its entries v (X: gathered, leading dimension ldx),

@@ -436,6 +436,21 @@ int hnhd_model_relational_link_train_step(hnhd_model_t *m, hnhd_distmult_t *d, c
  * scores_pos / scores_neg (nullable) are resized and receive s in the A order of T_pos / T_neg.  Collective. */
 int hnhd_model_relational_link_evaluate(hnhd_model_t *m, hnhd_distmult_t *d, const hnhd_relational_link_targets_t *t,
                                         hnhd_vec_t *scores_pos, hnhd_vec_t *scores_neg, double out[3]);
+/* Filtered link ranking (include/hnh/link_ranking.hpp).  A ranking holds the filter F, the known triples (heads[i],
+ * rels[i], tails[i]), i < n, of a model's nodes (model: the model's algorithm object).  Collective; HNH_E_INVALID on
+ * every rank for a layout without full rows, num_relations < 1, a node outside [0, M), a relation outside
+ * [0, num_relations) or triples that differ between ranks.  hnhd_model_link_rank: forward without dropout, then the
+ * filtered tail and head ranks of the n_q query triples (host arrays of n_q doubles, the same on every rank) by the
+ * DistMult scores of decoder d, or by dot products when d is null (the ranking then has 1 relation); *mrr = the mean
+ * of 1 / rank over the 2 n_q ranks.  Collective; HNH_E_INVALID on every rank before any launch for a ranking or
+ * decoder of another model's algorithm object, a decoder of another relation count or width, a null decoder with
+ * num_relations != 1, and queries that are out of range on any rank or differ between ranks. */
+typedef struct hnhd_link_ranking hnhd_link_ranking_t;
+int hnhd_link_ranking_create(hnhd_alg_t *model, const int64_t *heads, const int64_t *rels, const int64_t *tails, int64_t n,
+                             int num_relations, hnhd_link_ranking_t **out);
+void hnhd_link_ranking_destroy(hnhd_link_ranking_t *r);
+int hnhd_model_link_rank(hnhd_model_t *m, const hnhd_link_ranking_t *ranking, hnhd_distmult_t *d, const int64_t *heads,
+                         const int64_t *rels, const int64_t *tails, int64_t n_q, double *tail_ranks, double *head_ranks, double *mrr);
 void hnhd_model_destroy(hnhd_model_t *m);
 
 /* ---- graph-level prediction (include/hnh/graph_readout.hpp) ---------------------------------------------------------
