@@ -104,10 +104,9 @@ public:
 
     GAT(vector<GATLayer> &l_input, Distributed_Sparse *ops) : GraphModel(ops, "gat"), layers(l_input) {
         if (layers.empty()) throw hnh::Error(-1, "GAT: no layers");
-        for (size_t i = 1; i < layers.size(); i++)
-            if (layers[i].input_features != layers[i - 1].output_features())
-                throw hnh::Error(-1, "GAT: layer " + std::to_string(i) + " does not take the width layer " +
-                                         std::to_string(i - 1) + " produces");
+        vector<LayerWidths> widths;
+        for (const GATLayer &l : layers) widths.push_back({l.input_features, l.output_features(), true});
+        if (const string problem = layer_chain_problem(widths); !problem.empty()) throw hnh::Error(-1, "GAT: " + problem);
         // Shapes come from the algorithm object at the R in force, as in the reference (gat.hpp:60-79):
         // the input is B-shaped at R = input width, layer outputs are A-shaped at R = heads * head width,
         // a head's projection maps the previous buffer's local columns onto localAcols at R = head width.
@@ -217,13 +216,7 @@ public:
     // storage is allocated on the first call.
     void backwardPass(const DenseMatrix &output_grad) override {
         check_backward_supported();
-        if (!activations_current)
-            throw hnh::Error(HNH_E_INVALID, "GAT::backwardPass: no forward pass since the weights or the input changed");
-        if (output_grad.rows() != buffers.back().rows() || output_grad.cols() != buffers.back().cols())
-            throw hnh::Error(HNH_E_INVALID, "GAT::backwardPass: the output gradient is " + std::to_string(output_grad.rows()) +
-                                                " x " + std::to_string(output_grad.cols()) + ", the network output " +
-                                                std::to_string(buffers.back().rows()) + " x " +
-                                                std::to_string(buffers.back().cols()));
+        check_backward("GAT::backwardPass", "the weights or the input", output_grad);
         for (GATLayer &layer : layers)
             if (layer.wGrads.size() != layer.wMats.size()) {
                 layer.wGrads.clear();
@@ -236,16 +229,10 @@ public:
                 layer.a1Grads = VectorXd::Constant(layer.a1.size(), 0.0);
                 layer.a2Grads = VectorXd::Constant(layer.a2.size(), 0.0);
             }
-        // two layer gradients are live at a time: that of the layer's output (upstream) and that of its input
-        DenseMatrix upstream;
-        for (int i = (int)layers.size() - 1; i >= 0; i--) {
-            const DenseMatrix &G = i + 1 == (int)layers.size() ? output_grad : upstream;
-            DenseMatrix downstream;
-            DenseMatrix &dX = i == 0 ? input_grad : downstream;
+        backward_layers(output_grad, [&](int i, const DenseMatrix &G, DenseMatrix &dX) {
             dX.resize(buffers[(size_t)i].rows(), buffers[(size_t)i].cols());
             for (int j = 0; j < layers[(size_t)i].num_heads; j++) backwardHead(i, j, G, dX, j > 0);
-            if (i > 0) upstream = std::move(downstream);
-        }
+        });
     }
 
     // head j of layer i: G = dL/d buffers[i + 1]; writes layers[i].wGrads[j] and adds (or, accumulate == false,

@@ -76,20 +76,13 @@ public:
         if (layers.empty()) throw hnh::Error(HNH_E_INVALID, "GIN: no layers");
         if (edge_dim < 0) throw hnh::Error(HNH_E_INVALID, "GIN: edge_dim must not be negative");
         if (!std::isfinite(eps)) throw hnh::Error(HNH_E_INVALID, "GIN: eps must be finite");
-        for (size_t i = 0; i < layers.size(); i++) {
-            const GINLayer &l = layers[i];
-            if (l.input_features <= 0 || l.hidden_features <= 0 || l.output_features <= 0)
-                throw hnh::Error(HNH_E_INVALID, "GIN: layer " + std::to_string(i) + ": sizes must be positive");
-            if (i > 0 && l.input_features != layers[i - 1].output_features)
-                throw hnh::Error(HNH_E_INVALID, "GIN: layer " + std::to_string(i) + " does not take the width layer " +
-                                                    std::to_string(i - 1) + " produces");
-        }
-        if (d_ops->localArows != d_ops->localBrows) throw hnh::Error(HNH_E_INVALID, "GIN: the A and B layouts hold different rows");
-        d_ops->setRValue(layers.front().input_features);
-        buffers.push_back(d_ops->like_B_matrix(0.0));
+        vector<LayerWidths> widths;
+        for (const GINLayer &l : layers)
+            widths.push_back({l.input_features, l.output_features, l.input_features > 0 && l.hidden_features > 0 && l.output_features > 0});
+        refuse("GIN", layer_chain_problem(widths));
+        refuse("GIN", rows_problem());
+        allocate_buffers(widths);
         for (GINLayer &layer : layers) {
-            d_ops->setRValue(layer.output_features);
-            buffers.push_back(d_ops->like_A_matrix(0.0));
             layer.params = VectorXd::Constant(layer.param_count(edge_dim), 0.0);
             hnh::abi_check(hnh_fill_f64(layer.params.data() + layer.eps_offset(edge_dim), 1, eps, stream()), "fill");
         }
@@ -108,12 +101,9 @@ public:
 
     // Each layer's params with its grads, one span per layer; eps (the last entry) only with train_eps
     std::vector<ParamSpan> parameters() override {
-        std::vector<ParamSpan> s;
-        for (GINLayer &l : layers) {
-            ParamSpan p = span(l.params, l.grads);
-            if (!train_eps) p.n -= 1;
-            s.push_back(p);
-        }
+        std::vector<ParamSpan> s = layer_spans(layers);
+        if (!train_eps)
+            for (ParamSpan &p : s) p.n -= 1;
         return s;
     }
 
@@ -152,10 +142,7 @@ public:
             }
             DenseMatrix Y = hidden[i] * block(l.params, l, 1, false);
             hnh::abi_check(hnh_row_bias_add_f64(Y.data(), bias(l.params, l, 1), n, r, stream()), "row_bias_add");
-            if (i + 1 < layers.size())
-                buffers[i + 1].setMiddleColsRelu(0, Y);
-            else
-                buffers[i + 1].take(Y);
+            set_layer_output(i, Y);
         }
         activations_current = true;
     }
@@ -168,26 +155,12 @@ public:
     // ranks) and dL/d buffers[0] in input_grad.  Collective.
     void backwardPass(const DenseMatrix &output_grad) override {
         check_supported("GIN::backwardPass");
-        if (!activations_current)
-            throw hnh::Error(HNH_E_INVALID,
-                             "GIN::backwardPass: no forward pass since the parameters, the input or the edge attributes changed");
-        if (output_grad.rows() != buffers.back().rows() || output_grad.cols() != buffers.back().cols())
-            throw hnh::Error(HNH_E_INVALID, "GIN::backwardPass: the output gradient is " + std::to_string(output_grad.rows()) + " x " +
-                                                std::to_string(output_grad.cols()) + ", the network output " +
-                                                std::to_string(buffers.back().rows()) + " x " + std::to_string(buffers.back().cols()));
-        DenseMatrix upstream;
-        for (int i = (int)layers.size() - 1; i >= 0; i--) {
-            const DenseMatrix &G = i + 1 == (int)layers.size() ? output_grad : upstream;
-            DenseMatrix downstream;
-            backwardLayer(i, G, i == 0 ? input_grad : downstream);
-            if (i > 0) upstream = std::move(downstream);
-        }
+        check_backward("GIN::backwardPass", "the parameters, the input or the edge attributes", output_grad);
+        backward_layers(output_grad, [&](int i, const DenseMatrix &G, DenseMatrix &dX) { backwardLayer(i, G, dX); });
     }
 
 private:
     VectorXd ones_A, ones_B;  // GIN: the aggregation weight 1 of every entry in the A and B orders
-
-    static cudaStream_t stream() { return hnh::Runtime::get().compute_stream(); }
 
     void check_supported(const string &who) const {
         d_ops->check_full_rows(who);
@@ -238,14 +211,10 @@ private:
     void backwardLayer(int i, const DenseMatrix &G, DenseMatrix &dX) {
         GINLayer &l = layers[(size_t)i];
         DenseMatrix &X = buffers[(size_t)i], &Z = hidden[(size_t)i];
-        const int64_t n = X.rows(), f = l.input_features, h = l.hidden_features, r = l.output_features;
+        const int64_t n = X.rows(), f = l.input_features, h = l.hidden_features;
         if (l.grads.size() != l.params.size()) l.grads = VectorXd(l.params.size());
         DenseMatrix dY_relu;
-        if (i + 1 < (int)layers.size()) {
-            dY_relu.resize(n, r);
-            dY_relu.setMiddleColsReluGrad(G, buffers[(size_t)i + 1], 0);
-        }
-        const DenseMatrix &dY = i + 1 < (int)layers.size() ? dY_relu : G;
+        const DenseMatrix &dY = relu_grad_unless_last(i, G, dY_relu);
         {
             DenseMatrix Za = with_ones(Z);
             block(l.grads, l, 1, true).setTransposeTimes(Za, dY);

@@ -64,22 +64,13 @@ public:
         : GraphModel(ops, "GraphSAGE"), layers(l_input), aggr(parse(aggregation)) {
         d_ops->check_full_rows("GraphSAGE");
         if (layers.empty()) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: no layers");
-        for (size_t i = 0; i < layers.size(); i++) {
-            const GraphSAGELayer &l = layers[i];
-            if (l.input_features <= 0 || l.output_features <= 0)
-                throw hnh::Error(HNH_E_INVALID, "GraphSAGE: layer " + std::to_string(i) + ": sizes must be positive");
-            if (i > 0 && l.input_features != layers[i - 1].output_features)
-                throw hnh::Error(HNH_E_INVALID, "GraphSAGE: layer " + std::to_string(i) + " does not take the width layer " +
-                                                    std::to_string(i - 1) + " produces");
-        }
-        if (d_ops->localArows != d_ops->localBrows) throw hnh::Error(HNH_E_INVALID, "GraphSAGE: the A and B layouts hold different rows");
-        d_ops->setRValue(layers.front().input_features);
-        buffers.push_back(d_ops->like_B_matrix(0.0));
-        for (GraphSAGELayer &layer : layers) {
-            d_ops->setRValue(layer.output_features);
-            buffers.push_back(d_ops->like_A_matrix(0.0));
-            layer.params = VectorXd::Constant(layer.param_count(), 0.0);
-        }
+        vector<LayerWidths> widths;
+        for (const GraphSAGELayer &l : layers)
+            widths.push_back({l.input_features, l.output_features, l.input_features > 0 && l.output_features > 0});
+        refuse("GraphSAGE", layer_chain_problem(widths));
+        refuse("GraphSAGE", rows_problem());
+        allocate_buffers(widths);
+        for (GraphSAGELayer &layer : layers) layer.params = VectorXd::Constant(layer.param_count(), 0.0);
         if (aggr == kSum) {
             weights_A = d_ops->like_S_values(1.0);
             weights_B = d_ops->like_ST_values(1.0);
@@ -115,11 +106,7 @@ public:
     }
 
     // Each layer's params with its grads, one span per layer
-    std::vector<ParamSpan> parameters() override {
-        std::vector<ParamSpan> s;
-        for (GraphSAGELayer &l : layers) s.push_back(span(l.params, l.grads));
-        return s;
-    }
+    std::vector<ParamSpan> parameters() override { return layer_spans(layers); }
 
     // By name (the layout above): "neigh" (W_l, f x r), "neigh_bias" (b_l, r x 1), "root" (W_r, f x r)
     ParamRef param(int layer, const string &name) override {
@@ -144,10 +131,7 @@ public:
             DenseMatrix Y = aggregated[i] * neigh(layer.params, layer, false);
             hnh::abi_check(hnh_row_bias_add_f64(Y.data(), neigh_bias(layer.params, layer), Y.rows(), Y.cols(), stream()), "row_bias_add");
             Y += X * root(layer.params, layer);
-            if (i + 1 < layers.size())
-                buffers[i + 1].setMiddleColsRelu(0, Y);
-            else
-                buffers[i + 1].take(Y);
+            set_layer_output(i, Y);
         }
         activations_current = true;
     }
@@ -160,25 +144,12 @@ public:
     // ranks) and dL/d buffers[0] in input_grad.  Collective.
     void backwardPass(const DenseMatrix &output_grad) override {
         d_ops->check_full_rows("GraphSAGE::backwardPass");
-        if (!activations_current)
-            throw hnh::Error(HNH_E_INVALID, "GraphSAGE::backwardPass: no forward pass since the parameters or the input changed");
-        if (output_grad.rows() != buffers.back().rows() || output_grad.cols() != buffers.back().cols())
-            throw hnh::Error(HNH_E_INVALID, "GraphSAGE::backwardPass: the output gradient is " + std::to_string(output_grad.rows()) +
-                                                " x " + std::to_string(output_grad.cols()) + ", the network output " +
-                                                std::to_string(buffers.back().rows()) + " x " + std::to_string(buffers.back().cols()));
-        DenseMatrix upstream;
-        for (int i = (int)layers.size() - 1; i >= 0; i--) {
-            const DenseMatrix &G = i + 1 == (int)layers.size() ? output_grad : upstream;
-            DenseMatrix downstream;
-            backwardLayer(i, G, i == 0 ? input_grad : downstream);
-            if (i > 0) upstream = std::move(downstream);
-        }
+        check_backward("GraphSAGE::backwardPass", "the parameters or the input", output_grad);
+        backward_layers(output_grad, [&](int i, const DenseMatrix &G, DenseMatrix &dX) { backwardLayer(i, G, dX); });
     }
 
 private:
     VectorXd weights_A, weights_B;  // sum / mean: the aggregation weight of every entry in the A and B orders
-
-    static cudaStream_t stream() { return hnh::Runtime::get().compute_stream(); }
 
     // aggregated[i] (and counts[i]) = aggr(X)
     void aggregate(size_t i, DenseMatrix &X) {
@@ -198,14 +169,10 @@ private:
     void backwardLayer(int i, const DenseMatrix &G, DenseMatrix &dX) {
         GraphSAGELayer &layer = layers[(size_t)i];
         DenseMatrix &X = buffers[(size_t)i], &A = aggregated[(size_t)i];
-        const int64_t n = G.rows(), f = X.cols(), r = layer.output_features;
+        const int64_t f = X.cols();
         if (layer.grads.size() != layer.params.size()) layer.grads = VectorXd(layer.params.size());
         DenseMatrix dY_relu;
-        if (i + 1 < (int)layers.size()) {
-            dY_relu.resize(n, r);
-            dY_relu.setMiddleColsReluGrad(G, buffers[(size_t)i + 1], 0);
-        }
-        const DenseMatrix &dY = i + 1 < (int)layers.size() ? dY_relu : G;
+        const DenseMatrix &dY = relu_grad_unless_last(i, G, dY_relu);
         {
             DenseMatrix Aa = with_ones(A);
             neigh(layer.grads, layer, true).setTransposeTimes(Aa, dY);

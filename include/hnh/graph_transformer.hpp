@@ -108,24 +108,17 @@ public:
         if (ffn_ratio < 0) throw hnh::Error(HNH_E_INVALID, "GraphTransformer: ffn_ratio must not be negative");
         if (!(norm_eps > 0.0) || !std::isfinite(norm_eps))
             throw hnh::Error(HNH_E_INVALID, "GraphTransformer: norm_eps must be finite and > 0");
-        for (size_t i = 0; i < layers.size(); i++) {
-            const GraphTransformerLayer &l = layers[i];
-            if (l.input_features <= 0 || l.features_per_head <= 0 || l.num_heads <= 0)
-                throw hnh::Error(HNH_E_INVALID, "GraphTransformer: layer " + std::to_string(i) + ": sizes must be positive");
-            if ((int64_t)l.features_per_head * l.num_heads > INT32_MAX ||
-                (int64_t)l.features_per_head * l.num_heads * std::max(ffn_ratio, 1) > INT32_MAX)
-                throw hnh::Error(HNH_E_INVALID, "GraphTransformer: layer " + std::to_string(i) + " is too wide");
-            if (i > 0 && l.input_features != layers[i - 1].output_features())
-                throw hnh::Error(HNH_E_INVALID, "GraphTransformer: layer " + std::to_string(i) + " does not take the width layer " +
-                                                    std::to_string(i - 1) + " produces");
-        }
-        if (d_ops->localArows != d_ops->localBrows)
-            throw hnh::Error(HNH_E_INVALID, "GraphTransformer: the A and B layouts hold different rows");
-        d_ops->setRValue(layers.front().input_features);
-        buffers.push_back(d_ops->like_B_matrix(0.0));
+        vector<LayerWidths> widths;
+        for (const GraphTransformerLayer &l : layers)
+            widths.push_back({l.input_features, (int64_t)l.features_per_head * l.num_heads,
+                              l.input_features > 0 && l.features_per_head > 0 && l.num_heads > 0});
+        refuse("GraphTransformer", layer_chain_problem(widths, [&](size_t i) -> string {
+                   const int64_t r = widths[i].out;
+                   return r > INT32_MAX || r * std::max(ffn_ratio, 1) > INT32_MAX ? "layer " + std::to_string(i) + " is too wide" : "";
+               }));
+        refuse("GraphTransformer", rows_problem());
+        allocate_buffers(widths);
         for (GraphTransformerLayer &layer : layers) {
-            d_ops->setRValue(layer.output_features());
-            buffers.push_back(d_ops->like_A_matrix(0.0));
             layer.params = VectorXd::Constant(layer.param_count(edge_dim, beta, ffn_ratio), 0.0);
             if (ffn_ratio > 0)
                 for (int j : {0, 4}) block_vector(layer.params, layer, j).setConstant(1.0);  // the LayerNorm gains
@@ -161,11 +154,7 @@ public:
     }
 
     // Each layer's params with its grads, one span per layer
-    std::vector<ParamSpan> parameters() override {
-        std::vector<ParamSpan> s;
-        for (GraphTransformerLayer &l : layers) s.push_back(span(l.params, l.grads));
-        return s;
-    }
+    std::vector<ParamSpan> parameters() override { return layer_spans(layers); }
 
     // By name (the layout above): "query", "key", "value", "skip" (f x r) and their "_bias" (r x 1), "edge" (edge_dim x
     // r) with edge features, "beta" (3r x 1) with the gate; with blocks "norm1", "norm1_bias" (r x 1), "ffn1" ((r + 1) x
@@ -238,33 +227,20 @@ public:
     // ranks) and dL/d buffers[0] in input_grad.  Collective.  Uses the forward pass's dropout and seed.
     void backwardPass(const DenseMatrix &output_grad) override {
         check_supported("GraphTransformer::backwardPass", dropout_);
-        if (!activations_current)
-            throw hnh::Error(HNH_E_INVALID,
-                             "GraphTransformer::backwardPass: no forward pass since the parameters, the input or the edge attributes changed");
-        if (output_grad.rows() != buffers.back().rows() || output_grad.cols() != buffers.back().cols())
-            throw hnh::Error(HNH_E_INVALID, "GraphTransformer::backwardPass: the output gradient is " + std::to_string(output_grad.rows()) +
-                                                " x " + std::to_string(output_grad.cols()) + ", the network output " +
-                                                std::to_string(buffers.back().rows()) + " x " + std::to_string(buffers.back().cols()));
+        check_backward("GraphTransformer::backwardPass", "the parameters, the input or the edge attributes", output_grad);
         uint64_t seed_l = seed_;
         vector<uint64_t> seeds;
         for (const GraphTransformerLayer &layer : layers) {
             seeds.push_back(seed_l);
             seed_l += (uint64_t)layer.num_heads;
         }
-        DenseMatrix upstream;
-        for (int i = (int)layers.size() - 1; i >= 0; i--) {
-            const DenseMatrix &G = i + 1 == (int)layers.size() ? output_grad : upstream;
-            DenseMatrix downstream;
-            backwardLayer(i, G, i == 0 ? input_grad : downstream, seeds[(size_t)i]);
-            if (i > 0) upstream = std::move(downstream);
-        }
+        backward_layers(output_grad, [&](int i, const DenseMatrix &G, DenseMatrix &dX) { backwardLayer(i, G, dX, seeds[(size_t)i]); });
     }
 
 private:
     double dropout_ = 0.0;
     uint64_t seed_ = 0;
 
-    static cudaStream_t stream() { return hnh::Runtime::get().compute_stream(); }
     static double scale(const GraphTransformerLayer &l) { return 1.0 / std::sqrt((double)l.features_per_head); }
 
     // Everything a pass needs that every rank decides alike, checked before any launch

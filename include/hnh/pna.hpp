@@ -74,11 +74,14 @@ public:
         double delta_log)
         : GraphModel(ops, "PNA"), layers(l_input), avg_deg_lin(delta_lin), avg_deg_log(delta_log) {
         d_ops->check_full_rows("PNA");
+        vector<LayerWidths> widths;
+        for (const PNALayer &l : layers)
+            widths.push_back({l.input_features, l.output_features, l.input_features > 0 && l.output_features > 0});
         string problem;
         try {
             aggregators = parse_codes(aggregator_list, kAggregators, 6);
             scalers = parse_codes(scaler_list, kScalers, 5);
-            problem = check_arguments();
+            problem = check_arguments(widths);
         } catch (const hnh::Error &e) {
             problem = e.what();
         }
@@ -92,13 +95,8 @@ public:
         if (x[0] != 0.0) throw hnh::Error(HNH_E_INVALID, "PNA: another rank's arguments are bad");
         if (!hnh::detail::agree(x))
             throw hnh::Error(HNH_E_INVALID, "PNA: the aggregators, scalers or degree averages differ between ranks");
-        d_ops->setRValue(layers.front().input_features);
-        buffers.push_back(d_ops->like_B_matrix(0.0));
-        for (PNALayer &layer : layers) {
-            d_ops->setRValue(layer.output_features);
-            buffers.push_back(d_ops->like_A_matrix(0.0));
-            layer.params = VectorXd::Constant(param_count(layer), 0.0);
-        }
+        allocate_buffers(widths);
+        for (PNALayer &layer : layers) layer.params = VectorXd::Constant(param_count(layer), 0.0);
         // deg_u over all ranks: the sum window of a ones column
         DenseMatrix ones = DenseMatrix::Constant(d_ops->localBrows, 1, 1.0);
         degree.resize(d_ops->localArows, 2);
@@ -143,11 +141,7 @@ public:
     int64_t off_lin_bias(const PNALayer &l) const { return off_lin(l) + (int64_t)l.output_features * l.output_features; }
 
     // Each layer's params with its grads, one span per layer
-    std::vector<ParamSpan> parameters() override {
-        std::vector<ParamSpan> s;
-        for (PNALayer &l : layers) s.push_back(span(l.params, l.grads));
-        return s;
-    }
+    std::vector<ParamSpan> parameters() override { return layer_spans(layers); }
 
     // By name (the layout above): "pre" (2f x f), "pre_bias" (f x 1), "post" ((A S + 1) f x r), "post_bias" (r x 1),
     // "lin" (r x r), "lin_bias" (r x 1)
@@ -192,10 +186,7 @@ public:
             DenseMatrix Y = Qs[i] * view(l.params, off_lin(l), l.output_features, l.output_features);
             hnh::abi_check(hnh_row_bias_add_f64(Y.data(), l.params.data() + off_lin_bias(l), n, l.output_features, stream()),
                            "row_bias_add");
-            if (i + 1 < layers.size())
-                buffers[i + 1].setMiddleColsRelu(0, Y);
-            else
-                buffers[i + 1].take(Y);
+            set_layer_output(i, Y);
         }
         activations_current = true;
     }
@@ -208,26 +199,14 @@ public:
     // ranks) and dL/d buffers[0] in input_grad.  Collective.
     void backwardPass(const DenseMatrix &output_grad) override {
         d_ops->check_full_rows("PNA::backwardPass");
-        if (!activations_current)
-            throw hnh::Error(HNH_E_INVALID, "PNA::backwardPass: no forward pass since the parameters or the input changed");
-        if (output_grad.rows() != buffers.back().rows() || output_grad.cols() != buffers.back().cols())
-            throw hnh::Error(HNH_E_INVALID, "PNA::backwardPass: the output gradient is " + std::to_string(output_grad.rows()) + " x " +
-                                                std::to_string(output_grad.cols()) + ", the network output " +
-                                                std::to_string(buffers.back().rows()) + " x " + std::to_string(buffers.back().cols()));
-        DenseMatrix upstream;
-        for (int i = (int)layers.size() - 1; i >= 0; i--) {
-            const DenseMatrix &G = i + 1 == (int)layers.size() ? output_grad : upstream;
-            DenseMatrix downstream;
-            backwardLayer(i, G, i == 0 ? input_grad : downstream);
-            if (i > 0) upstream = std::move(downstream);
-        }
+        check_backward("PNA::backwardPass", "the parameters or the input", output_grad);
+        backward_layers(output_grad, [&](int i, const DenseMatrix &G, DenseMatrix &dX) { backwardLayer(i, G, dX); });
     }
 
 private:
     DenseMatrix degree;    // localArows x 2: deg_u over all ranks in column 0 (the moments of a ones column)
     DenseMatrix row_ones;  // localArows x 1 ones: the bias gradients are products with it
 
-    static cudaStream_t stream() { return hnh::Runtime::get().compute_stream(); }
     static DenseMatrix view(VectorXd &v, int64_t offset, int64_t rows, int64_t cols) {
         return DenseMatrix::view(v.data() + offset, rows, cols);
     }
@@ -260,18 +239,16 @@ private:
         return 2 * f * (((w & HNH_MULTI_MOMENTS) != 0) + ((w & HNH_MULTI_MAX) != 0) + ((w & HNH_MULTI_MIN) != 0));
     }
 
-    // "" or what is wrong with this rank's arguments
-    string check_arguments() const {
+    // "" or what is wrong with this rank's arguments; widths are the layers'
+    string check_arguments(const vector<LayerWidths> &widths) const {
         if (layers.empty()) return "no layers";
-        for (size_t i = 0; i < layers.size(); i++) {
-            const PNALayer &l = layers[i];
-            if (l.input_features <= 0 || l.output_features <= 0) return "layer " + std::to_string(i) + ": sizes must be positive";
-            if (i > 0 && l.input_features != layers[i - 1].output_features)
-                return "layer " + std::to_string(i) + " does not take the width layer " + std::to_string(i - 1) + " produces";
-            if (post_rows(l) >= INT32_MAX || state_width(l.input_features) >= INT32_MAX)
+        const string chain = layer_chain_problem(widths, nullptr, [&](size_t i) -> string {
+            if (post_rows(layers[i]) >= INT32_MAX || state_width(layers[i].input_features) >= INT32_MAX)
                 return "layer " + std::to_string(i) + ": (A S + 1) f must be below 2^31";
-        }
-        if (d_ops->localArows != d_ops->localBrows) return "the A and B layouts hold different rows";
+            return "";
+        });
+        if (!chain.empty()) return chain;
+        if (const string rows = rows_problem(); !rows.empty()) return rows;
         if (std::isnan(avg_deg_lin) || std::isnan(avg_deg_log)) return "a degree average is NaN: the degree histogram was refused";
         if (uses_lin() && !(std::isfinite(avg_deg_lin) && avg_deg_lin > 0.0))
             return "the average degree delta_lin = " + std::to_string(avg_deg_lin) + " must be finite and > 0";
@@ -288,11 +265,7 @@ private:
         const int which = statistics();
         if (l.grads.size() != l.params.size()) l.grads = VectorXd(l.params.size());
         DenseMatrix dY_relu;
-        if (i + 1 < (int)layers.size()) {
-            dY_relu.resize(n, r);
-            dY_relu.setMiddleColsReluGrad(G, buffers[(size_t)i + 1], 0);
-        }
-        const DenseMatrix &dY = i + 1 < (int)layers.size() ? dY_relu : G;
+        const DenseMatrix &dY = relu_grad_unless_last(i, G, dY_relu);
         view(l.grads, off_lin(l), r, r).setTransposeTimes(Qs[(size_t)i], dY);
         view(l.grads, off_lin_bias(l), 1, r).setTransposeTimes(row_ones, dY);
         DenseMatrix dQ;

@@ -81,17 +81,12 @@ public:
         : GraphModel(ops, "RGCN"), layers(l_input), num_relations(relations), aggr(parse(aggregation)), num_bases(bases) {
         vector<std::pair<int, int>> widths;
         for (const RGCNLayer &l : layers) widths.emplace_back(l.input_features, l.output_features);
-        check_layers(widths, num_relations, num_bases);
+        const vector<LayerWidths> chain = check_layers(widths, num_relations, num_bases);
         d_ops->check_full_rows("RGCN");
-        if (d_ops->localArows != d_ops->localBrows) throw hnh::Error(HNH_E_INVALID, "RGCN: the A and B layouts hold different rows");
+        refuse("RGCN", rows_problem());
         d_ops->relationCheck(num_relations);
-        d_ops->setRValue(layers.front().input_features);
-        buffers.push_back(d_ops->like_B_matrix(0.0));
-        for (RGCNLayer &layer : layers) {
-            d_ops->setRValue(layer.output_features);
-            buffers.push_back(d_ops->like_A_matrix(0.0));
-            layer.params = VectorXd::Constant(param_count(layer), 0.0);
-        }
+        allocate_buffers(chain);
+        for (RGCNLayer &layer : layers) layer.params = VectorXd::Constant(param_count(layer), 0.0);
         ones = DenseMatrix::Constant(d_ops->localArows, 1, 1.0);
         if (aggr == kMean) {
             // |N_rho(u)| over all ranks: the relational sum of a ones column
@@ -109,23 +104,22 @@ public:
     }
 
     // the checks that need no device, on the (input, output) widths of the layers: a relation count >= 1, a basis count
-    // >= 0, positive widths that chain, R f < 2^31, and with bases B f and R B < 2^31
-    static void check_layers(const vector<std::pair<int, int>> &widths, int num_relations, int num_bases = 0) {
+    // >= 0, positive widths that chain, R f < 2^31, and with bases B f and R B < 2^31.  Returns the widths as
+    // allocate_buffers takes them.
+    static vector<LayerWidths> check_layers(const vector<std::pair<int, int>> &widths, int num_relations, int num_bases = 0) {
         if (widths.empty()) throw hnh::Error(HNH_E_INVALID, "RGCN: no layers");
         if (num_relations < 1) throw hnh::Error(HNH_E_INVALID, "RGCN: the relation count must be positive");
         if (num_bases < 0) throw hnh::Error(HNH_E_INVALID, "RGCN: the basis count must not be negative");
         if ((int64_t)num_relations * num_bases > INT32_MAX) throw hnh::Error(HNH_E_INVALID, "RGCN: R B must be below 2^31");
-        for (size_t i = 0; i < widths.size(); i++) {
-            const auto [f, r] = widths[i];
-            if (f <= 0 || r <= 0) throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + ": sizes must be positive");
-            if (num_bases == 0 && (int64_t)num_relations * f > INT32_MAX)
-                throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + ": R f must be below 2^31");
-            if ((int64_t)num_bases * f > INT32_MAX)
-                throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + ": B f must be below 2^31");
-            if (i > 0 && f != widths[i - 1].second)
-                throw hnh::Error(HNH_E_INVALID, "RGCN: layer " + std::to_string(i) + " does not take the width layer " +
-                                                    std::to_string(i - 1) + " produces");
-        }
+        vector<LayerWidths> chain;
+        for (const auto &[f, r] : widths) chain.push_back({f, r, f > 0 && r > 0});
+        refuse("RGCN", layer_chain_problem(chain, [&](size_t i) -> string {
+                   const int64_t f = chain[i].in;
+                   if (num_bases == 0 && num_relations * f > INT32_MAX) return "layer " + std::to_string(i) + ": R f must be below 2^31";
+                   if (num_bases * f > INT32_MAX) return "layer " + std::to_string(i) + ": B f must be below 2^31";
+                   return "";
+               }));
+        return chain;
     }
 
     static Aggregation parse(const string &a) {
@@ -156,11 +150,7 @@ public:
     }
 
     // Each layer's params with its grads, one span per layer
-    std::vector<ParamSpan> parameters() override {
-        std::vector<ParamSpan> s;
-        for (RGCNLayer &l : layers) s.push_back(span(l.params, l.grads));
-        return s;
-    }
+    std::vector<ParamSpan> parameters() override { return layer_spans(layers); }
 
     // By name (the layout above): "weight" (R f x r, or B f x r with bases), "bias" (r x 1), "root" (f x r), and with
     // bases "comp" (R x B)
@@ -194,10 +184,7 @@ public:
             DenseMatrix Y = A * weight(layer.params, layer);
             hnh::abi_check(hnh_row_bias_add_f64(Y.data(), bias(layer.params, layer).data(), Y.rows(), Y.cols(), stream()), "row_bias_add");
             Y += X * root(layer.params, layer);
-            if (i + 1 < layers.size())
-                buffers[i + 1].setMiddleColsRelu(0, Y);
-            else
-                buffers[i + 1].take(Y);
+            set_layer_output(i, Y);
         }
         activations_current = true;
     }
@@ -210,26 +197,13 @@ public:
     // ranks) and dL/d buffers[0] in input_grad.  Collective.
     void backwardPass(const DenseMatrix &output_grad) override {
         d_ops->check_full_rows("RGCN::backwardPass");
-        if (!activations_current)
-            throw hnh::Error(HNH_E_INVALID, "RGCN::backwardPass: no forward pass since the parameters or the input changed");
-        if (output_grad.rows() != buffers.back().rows() || output_grad.cols() != buffers.back().cols())
-            throw hnh::Error(HNH_E_INVALID, "RGCN::backwardPass: the output gradient is " + std::to_string(output_grad.rows()) +
-                                                " x " + std::to_string(output_grad.cols()) + ", the network output " +
-                                                std::to_string(buffers.back().rows()) + " x " + std::to_string(buffers.back().cols()));
-        DenseMatrix upstream;
-        for (int i = (int)layers.size() - 1; i >= 0; i--) {
-            const DenseMatrix &G = i + 1 == (int)layers.size() ? output_grad : upstream;
-            DenseMatrix downstream;
-            backwardLayer(i, G, i == 0 ? input_grad : downstream);
-            if (i > 0) upstream = std::move(downstream);
-        }
+        check_backward("RGCN::backwardPass", "the parameters or the input", output_grad);
+        backward_layers(output_grad, [&](int i, const DenseMatrix &G, DenseMatrix &dX) { backwardLayer(i, G, dX); });
     }
 
 private:
     DenseMatrix ones;    // localArows x 1 of 1.0: the bias gradient is its product with dY
     DenseMatrix counts;  // mean: |N_rho(u)| (localArows x R); with bases 1 / |N_rho(u)|, 0 where the count is 0
-
-    static cudaStream_t stream() { return hnh::Runtime::get().compute_stream(); }
 
     // M[u, rho f + k] /= |N_rho(u)| (0 where the count is 0)
     void window_scale(DenseMatrix &M, int f) {
@@ -241,14 +215,10 @@ private:
     void backwardLayer(int i, const DenseMatrix &G, DenseMatrix &dX) {
         RGCNLayer &layer = layers[(size_t)i];
         DenseMatrix &X = buffers[(size_t)i], &A = aggregated[(size_t)i];
-        const int64_t n = G.rows(), f = X.cols(), r = layer.output_features;
+        const int64_t f = X.cols();
         if (layer.grads.size() != layer.params.size()) layer.grads = VectorXd(layer.params.size());
         DenseMatrix dY_relu;
-        if (i + 1 < (int)layers.size()) {
-            dY_relu.resize(n, r);
-            dY_relu.setMiddleColsReluGrad(G, buffers[(size_t)i + 1], 0);
-        }
-        const DenseMatrix &dY = i + 1 < (int)layers.size() ? dY_relu : G;
+        const DenseMatrix &dY = relu_grad_unless_last(i, G, dY_relu);
         weight(layer.grads, layer).setTransposeTimes(A, dY);
         bias(layer.grads, layer).setTransposeTimes(ones, dY);
         root(layer.grads, layer).setTransposeTimes(X, dY);
