@@ -5,8 +5,9 @@ that builds the filter masks from the known triple sets and decodes [true, candi
 tests/distmult_oracle.py, in fp64 instead of the example's fp32.  `filtered_ranks` is the vectorised definition the
 library implements: candidates exclude the true entity and F, rank = ((gt + 1) + (ge + 1)) / 2.  The two agree wherever
 every query is in F; with the true triple missing from F the loop counts the true entity twice, so its rank is 0.5
-higher.  Both associate the score as (z_u * rel) * z_v, summed by torch.  Nothing under distributed_sddmm_b200/ imports
-this module.
+higher.  Both associate the score as (z_u * rel) * z_v, summed by torch.  `matmul_ranks` is `filtered_ranks` by one
+matrix product per query chunk with a vectorised filter mask: it scales to wide outputs and many queries, and on
+integer-valued operands it is exact.  Nothing under distributed_sddmm_b200/ imports this module.
 """
 from __future__ import annotations
 
@@ -108,3 +109,63 @@ def filtered_ranks(z, rel, queries, known, num_nodes, chunk=256):
     allr = np.concatenate(out_ranks)
     mrr = float((1.0 / allr).mean()) if len(allr) else 0.0
     return mrr, out_ranks[0], out_ranks[1], out_scores[0], out_scores[1]
+
+
+def separated(scores_t, scores_h, q):
+    """True when every score either equals the true one or differs from it far beyond rounding (so that the
+    oracle's association and the library's decide alike).  scores_t / scores_h are the n_q x num_nodes tail and head
+    scores of filtered_ranks or matmul_ranks, q = (heads, rels, tails)."""
+    for s, col in ((scores_t, q[2]), (scores_h, q[0])):
+        true = s[np.arange(len(col)), col][:, None]
+        d = np.abs(s - true)
+        if not ((d == 0) | (d > 1e-9 * max(np.abs(s).max(), 1e-300))).all():
+            return False
+    return True
+
+
+def filter_keys(known, R, num_nodes):
+    """The sorted distinct int64 keys (h R + rho) num_nodes + t of the known triples."""
+    if not known:
+        return np.zeros(0, np.int64)
+    F = np.concatenate([np.stack([np.asarray(a, np.int64) for a in k], 1) for k in known])
+    return np.unique((F[:, 0] * R + F[:, 1]) * num_nodes + F[:, 2])
+
+
+def matmul_ranks(z, rel, queries, known, num_nodes, chunk=None):
+    """filtered_ranks by one matrix product per chunk of queries, (z[anchor] o rel[rho]) @ z.T, with the filter mask
+    built by np.isin on int64 triple keys: the same tuple, at any width and any number of queries.  On integer-valued z
+    and rel whose products and partial sums stay integers below 2^53 every score is exact whatever the summation order,
+    so the ranks are the library's bit for bit with no separation guard."""
+    z = np.ascontiguousarray(np.asarray(z, np.float64)[:num_nodes])
+    rel = np.asarray(rel, np.float64)
+    h, rho, t = (np.asarray(a, np.int64) for a in queries)
+    R, n_q = rel.shape[0], len(h)
+    chunk = chunk or max(1, (1 << 22) // max(z.shape[1], 1))  # a query block of at most 32 MB
+    keys = filter_keys(known, R, num_nodes)
+    v = np.arange(num_nodes, dtype=np.int64)
+    out_ranks, out_scores = [], []
+    for tail in (True, False):
+        anchor, target = (h, t) if tail else (t, h)
+        ranks, scores = np.zeros(n_q), np.zeros((n_q, num_nodes))
+        for c0 in range(0, n_q, chunk):
+            a, rr, tg = anchor[c0:c0 + chunk], rho[c0:c0 + chunk], target[c0:c0 + chunk]
+            s = (z[a] * rel[rr]) @ z.T  # n x num_nodes
+            true = s[np.arange(len(a)), tg]
+            k = ((a * R + rr)[:, None] * num_nodes + v[None, :]) if tail else ((v[None, :] * R + rr[:, None]) * num_nodes + a[:, None])
+            cand = ~np.isin(k, keys)
+            cand[np.arange(len(a)), tg] = False
+            gt = ((s > true[:, None]) & cand).sum(1)
+            ge = ((s >= true[:, None]) & cand).sum(1)
+            ranks[c0:c0 + chunk] = ((gt + 1) + (ge + 1)) / 2.0
+            scores[c0:c0 + chunk] = s
+        out_ranks.append(ranks)
+        out_scores.append(scores)
+    allr = np.concatenate(out_ranks)
+    mrr = float((1.0 / allr).mean()) if len(allr) else 0.0
+    return mrr, out_ranks[0], out_ranks[1], out_scores[0], out_scores[1]
+
+
+def integer_bound(z, rel):
+    """A bound on |any partial sum| of a score z_u . (z_v o rel_rho): r max|z|^2 max|rel|."""
+    z, rel = np.asarray(z, np.float64), np.asarray(rel, np.float64)
+    return float(z.shape[1]) * float(np.abs(z).max(initial=0.0)) ** 2 * float(np.abs(rel).max(initial=0.0))

@@ -3,7 +3,10 @@ kernels against numpy -- exactly on integer-valued operands, and on float operan
 cancel the count path exactly -- at the table and odd widths, off the 64-tile, past one resident wave, with odd leading
 dimensions and misaligned operands, and with exact ties; then net.link_rank on R-GCN (plain and with bases) with a
 trained DistMult decoder and on GraphSAGE without one, against tests/link_ranking_oracle.py exactly; duplicate
-queries, hub filters, every refusal, and a learning check."""
+queries, hub filters, every refusal, and a learning check.  Then integer-valued models r = 40001 to 262145 wide
+(tests/link_ranking_cases.py), ranked in one to three query chunks and on all five layouts, exactly against
+tests/link_ranking_oracle.matmul_ranks; every model on the float path, by dot product and two with DistMult; and
+link_rank after a train step (stale activations) and after a dropout step."""
 import math
 
 import numpy as np
@@ -12,7 +15,9 @@ import torch
 
 from distributed_sddmm_b200 import driver as D
 from distributed_sddmm_b200 import lib
+from tests import gin_oracle as go
 from tests import graph_sage_oracle as so
+from tests import link_ranking_cases as lrc
 from tests import link_ranking_oracle as lro
 from tests import rgcn_basis_oracle as bo
 from tests import rgcn_oracle as ro
@@ -203,17 +208,6 @@ def _kg(rng, N, R, n):
     return h.astype(np.int64), rr.astype(np.int64), t.astype(np.int64)
 
 
-def _separated(scores_t, scores_h, tr, hr, q, N):
-    """True when every score either equals the true one or differs from it far beyond rounding (so that the
-    oracle's association and the library's decide alike)."""
-    for s, col in ((scores_t, q[2]), (scores_h, q[0])):
-        true = s[np.arange(len(col)), col][:, None]
-        d = np.abs(s - true)
-        if not ((d == 0) | (d > 1e-9 * max(np.abs(s).max(), 1e-300))).all():
-            return False
-    return True
-
-
 def rgcn_kg(B, seed, N=160, R=3, f=6, r=8):
     rng = np.random.default_rng(seed)
     train, valid, test = _kg(rng, N, R, 900), _kg(rng, N, R, 60), _kg(rng, N, R, 60)
@@ -251,7 +245,7 @@ def test_rgcn_distmult_ranks_match_the_oracle(world, B):
     res = net.link_rank(ranking, q, decoder=dec)
     z, rel = net.buffer(len(net.layers))[:N], dec.param("rel")
     mrr, t, h, st, sh = lro.filtered_ranks(z, rel, q, known, N)
-    assert _separated(st, sh, t, h, q, N)
+    assert lro.separated(st, sh, q)
     assert np.array_equal(res.tail_ranks, t) and np.array_equal(res.head_ranks, h)
     assert res.mrr == pytest.approx(mrr, rel=1e-14)
     n = len(K["test"][0])
@@ -298,7 +292,7 @@ def test_graph_sage_dot_product_ranks_match_the_oracle(world):
     z = net.buffer(len(net.layers))[:N]
     assert np.array_equal(z[20], z[21]) and np.array_equal(z[20], z[140])
     mrr, t, h, st, sh = lro.filtered_ranks(z, np.ones((1, z.shape[1])), q, known, N)
-    assert _separated(st, sh, t, h, q, N)
+    assert lro.separated(st, sh, q)
     assert np.array_equal(res.tail_ranks, t) and np.array_equal(res.head_ranks, h)
     assert (t != np.round(t)).any() or (h != np.round(h)).any()  # the copies tie: half ranks
 
@@ -376,3 +370,229 @@ def test_filtered_mrr_rises_with_training(world):
     after = net.link_rank(ranking, held, decoder=dec)
     print(f"filtered MRR before {before.mrr:.4f} after {after.mrr:.4f}, Hits@10 {before.hits_at(10):.3f} -> {after.hits_at(10):.3f}")
     assert after.mrr >= 1.3 * before.mrr and after.hits_at(10) >= before.hits_at(10) + 0.04, (before, after)
+
+
+# ---- wide integer-valued models: several query chunks, exactly --------------------------------------------------------
+def integer_net(model, r, M, seed, alg_name="15d_fusion1", R=None, nonneg=False):
+    """An integer-valued model of tests/link_ranking_cases.py (GraphSAGE sum, GIN eps = 0, R-GCN sum with and without
+    bases) r wide on M nodes, its input set, and a DistMult decoder of R relations (None: no decoder)."""
+    rows, cols, rels = lrc.graph(M, seed)
+    vals = rels if model.startswith("rgcn") else np.ones(len(rows))
+    alg = D.Algorithm(alg_name, D.SpmatLocal.from_tuples(M, M, rows, cols, vals), lrc.F_IN, 1)
+    L = lrc.layers(model, r)
+    net = {"sage": lambda: D.GraphSAGE(alg, L, aggr="sum"), "gin": lambda: D.GIN(alg, L, eps=0.0),
+           "rgcn": lambda: D.RGCN(alg, L, lrc.RELS, aggr="sum"),
+           "rgcn_bases": lambda: D.RGCN(alg, L, lrc.RELS, aggr="sum", num_bases=lrc.BASES)}[model]()
+    rng = np.random.default_rng(seed + 1)
+    for l in range(len(L)):
+        for name in net.param_names():
+            if name != "eps":
+                net.set_param(l, name, lrc.integer_param(net.param_shape(l, name), rng, nonneg))
+    X = lrc.integer_input(M, seed + 2, nonneg)
+    net.set_input(np.vstack([X, np.zeros((net.buffer_shape(0)[0] - M, X.shape[1]))]))
+    dec = rel = None
+    if R:
+        dec = D.DistMultDecoder(net, R)
+        rel = lrc.relation_table(R, r, seed + 3, nonneg)
+        dec.set_param("rel", rel)
+    return net, alg, dec, (rel if R else np.ones((1, r)))
+
+
+def candidates(F, R, M, q, tail):
+    """|C| per query: the nodes other than the true entity and outside the filter."""
+    keys = lro.filter_keys([F], R, M)
+    v = np.arange(M)
+    h, rr, t = q
+    k = ((h * R + rr)[:, None] * M + v[None, :]) if tail else ((v[None, :] * R + rr[:, None]) * M + t[:, None])
+    c = ~np.isin(k, keys)
+    c[np.arange(len(h)), t if tail else h] = False
+    return c.sum(1)
+
+
+def check_exact(res, z, rel, q, known, M):
+    """link_rank's result against the exact oracle on the integer-valued output z."""
+    assert np.array_equal(z, np.round(z)), "the output is not integer-valued"
+    assert lro.integer_bound(z, rel) < 2.0 ** 43  # a 2^10 margin below 2^53
+    mrr, t, h, st, sh = lro.matmul_ranks(z, rel, q, known, M)
+    assert np.array_equal(res.tail_ranks, t) and np.array_equal(res.head_ranks, h)
+    assert res.mrr == pytest.approx(mrr, rel=1e-14)
+    for k in (1, 3, 10):
+        assert res.hits_at(k) == ((t <= k).sum() + (h <= k).sum()) / (2 * len(t))
+    return t, h, st, sh
+
+
+@pytest.mark.parametrize("name", sorted(lrc.WIDE))
+def test_wide_integer_ranks_are_exact_across_chunks(world, name):
+    cfg = lrc.WIDE[name]
+    M, r, R, n_q = cfg["M"], cfg["r"], cfg["R"], cfg["n_q"]
+    seed = lrc.case_seed(name)
+    net, alg, dec, rel = integer_net(cfg["model"], r, M, seed, R=R)
+    chunk = lrc.chunk_of(r, n_q)
+    F, q, lonely, hub, edges = lrc.queries(M, R or 1, n_q, chunk, seed + 4)
+    ranking = D.LinkRanking(net, F, R or 1)
+    res = net.link_rank(ranking, q, decoder=dec)
+    z = net.buffer(len(net.layers))[:M]
+    iso = lrc.isolated(M)
+    assert all(np.array_equal(z[iso[0]], z[i]) for i in iso[1:])  # copies: their scores tie exactly
+    t, h, st, sh = check_exact(res, z, rel, q, [F], M)
+    assert (st[:, iso] == st[:, iso[:1]]).all()
+    again = net.link_rank(ranking, q, decoder=dec)
+    assert np.array_equal(again.tail_ranks, res.tail_ranks) and np.array_equal(again.head_ranks, res.head_ranks)
+    assert again.mrr == res.mrr
+    for e in edges:  # one query on both sides of a chunk edge
+        assert (q[0][e - 1], q[1][e - 1], q[2][e - 1]) == (q[0][e], q[1][e], q[2][e])
+        assert t[e - 1] == t[e] and h[e - 1] == h[e]
+    assert (t[(q[0] == hub) & (q[1] == 0)] == 1.0).all()  # every node is a known tail of (hub, 0)
+    if R:
+        zero = q[1] == lrc.ZERO_REL  # every score is 0: every candidate ties with the true entity
+        assert zero.any() and not (q[1] == lrc.UNUSED_REL).any()
+        assert np.array_equal(t[zero], (1 + (candidates(F, R, M, q, True)[zero] + 1)) / 2)
+        assert np.array_equal(h[zero], (1 + (candidates(F, R, M, q, False)[zero] + 1)) / 2)
+    assert ((st == st[np.arange(n_q), q[2]][:, None]).sum(1) > 1).any()  # candidates tie with the true tail
+    # an empty filter: the raw ranks
+    raw = net.link_rank(D.LinkRanking(net, ([], [], []), R or 1), q, decoder=dec)
+    check_exact(raw, z, rel, q, [], M)
+
+
+ALL_LAYOUTS = ["15d_fusion1", "15d_fusion2", "15d_sparse", "25d_dense_replicate", "25d_sparse_replicate"]
+
+
+def test_integer_ranks_on_every_layout_at_p1(world):
+    """The five layouts hold full rows at p = 1: the same output, the same ranks."""
+    cfg = lrc.WIDE["rgcn_r40001_distmult"]
+    M, r, R, n_q = cfg["M"], cfg["r"], cfg["R"], cfg["n_q"]
+    seed = SEED + 70
+    F, q, _, _, _ = lrc.queries(M, R, n_q, lrc.chunk_of(r, n_q), seed + 4)
+    z0 = want = None
+    for name in ALL_LAYOUTS:
+        net, alg, dec, rel = integer_net(cfg["model"], r, M, seed, alg_name=name, R=R)
+        res = net.link_rank(D.LinkRanking(net, F, R), q, decoder=dec)
+        z = net.buffer(len(net.layers))[:M]
+        if z0 is None:
+            z0, want = z, check_exact(res, z, rel, q, [F], M)
+        assert np.array_equal(z, z0), name
+        assert np.array_equal(res.tail_ranks, want[0]) and np.array_equal(res.head_ranks, want[1]), name
+
+
+# ---- every model, on the float path ----------------------------------------------------------------------------------
+FLOAT_MODELS = ["gat_leaky", "gat_softmax", "gat_additive", "gat_gatv2", "gt_plain", "gt_edge_beta_ffn", "sage_mean",
+                "sage_sum", "sage_max", "pna", "gin", "gine"]
+N_FLOAT, F_FLOAT = 150, 6
+
+
+def float_net(kind, seed):
+    """A model of kind with every parameter random, its input (and edge attributes) set; output 6 wide."""
+    rng = np.random.default_rng(seed)
+    N, f = N_FLOAT, F_FLOAT
+    rows, cols = rng.integers(0, N, 800), rng.integers(0, N, 800)
+    alg = D.Algorithm("15d_fusion1", D.SpmatLocal.from_tuples(N, N, rows, cols, np.ones(len(rows))), f, 1)
+    if kind.startswith("gat"):
+        L = [(f, 4, 2), (8, 6, 1)]
+        net = D.GAT(alg, L, attention=kind[4:])
+        for l, (fi, d, H) in enumerate(L):
+            for hd in range(H):
+                net.set_weight(l, hd, rng.uniform(-1, 1, (fi, d)) / np.sqrt(fi))
+                net.set_attention_vectors(l, hd, rng.uniform(-1, 1, d), rng.uniform(-1, 1, d))
+    else:
+        if kind.startswith("gt"):
+            full = kind == "gt_edge_beta_ffn"
+            L = [(f, 4, 2), (8, 3, 2)]
+            net = D.GraphTransformer(alg, L, edge_dim=3 if full else 0, beta=full, ffn_ratio=2 if full else 0)
+        elif kind.startswith("sage"):
+            L = [(f, 10), (10, 6)]
+            net = D.GraphSAGE(alg, L, aggr=kind[5:])
+        elif kind == "pna":
+            L = [(f, 10), (10, 6)]
+            net = D.PNA(alg, L, deg=np.bincount(np.bincount(rows, minlength=N)))
+        else:
+            L = [(f, 10, 8), (8, 10, 6)]
+            net = D.GIN(alg, L, edge_dim=3 if kind == "gine" else 0, eps=0.25)
+        for l in range(len(L)):
+            for name in net.param_names():
+                shape = net.param_shape(l, name)
+                net.set_param(l, name, rng.uniform(-1, 1, shape) / (np.sqrt(shape[0]) if len(shape) == 2 else 2.0))
+        if getattr(net, "edge_dim", 0):
+            net.set_edge_attributes(go.attr_of(*alg.entry_coordinates("A"), 3), go.attr_of(*alg.entry_coordinates("B"), 3))
+    X = rng.uniform(-1, 1, (N, f))
+    net.set_input(np.vstack([X, np.zeros((net.buffer_shape(0)[0] - N, f))]))
+    return net, alg, rows, cols
+
+
+def float_queries(rng, N, R, n=120):
+    known = [_kg(rng, N, R, 600)]
+    q = _kg(rng, N, R, n)
+    known.append(tuple(a[: n // 2] for a in q))
+    return known, q
+
+
+def check_float(res, z, rel, q, known, N):
+    mrr, t, h, st, sh = lro.matmul_ranks(z, rel, q, known, N)
+    assert lro.separated(st, sh, q)
+    assert np.array_equal(res.tail_ranks, t) and np.array_equal(res.head_ranks, h)
+    assert res.mrr == pytest.approx(mrr, rel=1e-14)
+
+
+@pytest.mark.parametrize("kind", FLOAT_MODELS)
+def test_every_model_dot_product_ranks_match_the_oracle(world, kind):
+    net, alg, _, _ = float_net(kind, SEED + 80 + len(kind))
+    rng = np.random.default_rng(SEED + 81)
+    known, q = float_queries(rng, N_FLOAT, 1)
+    ranking = D.LinkRanking(net, tuple(np.concatenate(x) for x in zip(*known)))
+    res = net.link_rank(ranking, q)
+    z = net.buffer(len(net.layers))[:N_FLOAT]
+    assert np.abs(z).max() > 0
+    check_float(res, z, np.ones((1, z.shape[1])), q, known, N_FLOAT)
+
+
+@pytest.mark.parametrize("kind", ["gt_plain", "gine"])
+def test_distmult_ranks_of_other_models_match_the_oracle(world, kind):
+    net, alg, _, _ = float_net(kind, SEED + 90 + len(kind))
+    rng = np.random.default_rng(SEED + 91)
+    R = 2
+    dec = D.DistMultDecoder(net, R)
+    dec.set_param("rel", rng.uniform(-1, 1, (R, 6)))
+    known, q = float_queries(rng, N_FLOAT, R)
+    res = net.link_rank(D.LinkRanking(net, tuple(np.concatenate(x) for x in zip(*known)), R), q, decoder=dec)
+    check_float(res, net.buffer(len(net.layers))[:N_FLOAT], dec.param("rel"), q, known, N_FLOAT)
+
+
+def _link_targets(net, rng, N):
+    tr, tc = rng.integers(0, N, 400), rng.integers(0, N, 400)
+    algT = D.Algorithm("15d_fusion1", D.SpmatLocal.from_tuples(N, N, tr, tc, rng.choice([0.0, 1.0], 400)), F_FLOAT, 1)
+    return algT, D.LinkTargets(net, algT)
+
+
+@pytest.mark.parametrize("kind", ["sage_mean", "gin", "gat_softmax"])
+def test_link_rank_after_a_train_step_ranks_the_updated_model(world, kind):
+    """A train step leaves the activations of the parameters before its update: link_rank must run the forward."""
+    net, alg, _, _ = float_net(kind, SEED + 100 + len(kind))
+    rng = np.random.default_rng(SEED + 101)
+    known, q = float_queries(rng, N_FLOAT, 1)
+    ranking = D.LinkRanking(net, tuple(np.concatenate(x) for x in zip(*known)))
+    net.forward()
+    before = net.buffer(len(net.layers))
+    algT, t = _link_targets(net, rng, N_FLOAT)
+    net.link_train_step(t, D.AdamW(lr=5e-2))
+    assert np.array_equal(net.buffer(len(net.layers)), before)  # the buffer still holds the old activations
+    res = net.link_rank(ranking, q)
+    z = net.buffer(len(net.layers))
+    assert not np.array_equal(z, before)
+    net.forward()
+    assert np.array_equal(net.buffer(len(net.layers)), z)  # bit for bit an explicit forward's
+    check_float(res, z[:N_FLOAT], np.ones((1, z.shape[1])), q, known, N_FLOAT)
+
+
+def test_link_rank_after_a_dropout_step_ranks_without_dropout(world):
+    net, alg, _, _ = float_net("gt_plain", SEED + 110)
+    rng = np.random.default_rng(SEED + 111)
+    known, q = float_queries(rng, N_FLOAT, 1)
+    ranking = D.LinkRanking(net, tuple(np.concatenate(x) for x in zip(*known)))
+    algT, t = _link_targets(net, rng, N_FLOAT)
+    net.link_train_step(t, D.AdamW(lr=1e-2), dropout=0.4, seed=9)
+    res = net.link_rank(ranking, q)
+    z = net.buffer(len(net.layers))
+    net.forward(dropout=0.4, seed=9)
+    assert not np.array_equal(net.buffer(len(net.layers)), z)  # dropout changes the output
+    net.forward()
+    assert np.array_equal(net.buffer(len(net.layers)), z)
+    check_float(res, z[:N_FLOAT], np.ones((1, z.shape[1])), q, known, N_FLOAT)
